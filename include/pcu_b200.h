@@ -94,8 +94,11 @@ typedef struct pcu_b200_options {
     int disable_tie_replay;  /* diagnostic only.  1: keep the (distance, lowest index) order for tied queries;        */
                              /* 2: replay on full reference trees only (no pruned build); 3: pruned build with    */
                              /* zero slack (every walk hits a stub, which exercises the full-rebuild path)        */
-    int binning;             /* 0: automatic; 1: always the multi-launch grid build; 2: the one-CTA-per-cloud     */
-                             /* build whenever a cloud's cell counters fit in shared memory (diagnostic only)    */
+    int binning;             /* 0: automatic (one CTA per cloud up to 8192 points, the cell-wise passes for a    */
+                             /* single pair up to 65536, else the slab build); 1: always the cell-wise          */
+                             /* passes; 2: the one-CTA-per-cloud build whenever a cloud's cell counters fit in   */
+                             /* shared memory; 3: the slab build above 8192 points, batches included             */
+                             /* (1 .. 3 are diagnostic only)                                                      */
     int host_staging;        /* host entry points, inputs of >= 4 MB: 0 pageable memory goes through the          */
                              /* workspace's pinned ring filled by copy threads, pinned memory is DMA'd as it is;  */
                              /* 1 always the ring; 2 never (plain cudaMemcpyAsync: the driver stages)             */
@@ -141,7 +144,9 @@ int pcu_b200_workspace_grid_refinement(const pcu_b200_workspace* ws, float out_m
 /* Per-stage device timing (diagnostic; bench.py's roofline pass).  When enabled, every device entry
  * point records CUDA events on the launching stream between its stages; after that stream has been
  * synchronised, last_profile() returns the milliseconds of the LAST call's 8 stages (descriptors,
- * bbox+grid, histogram, scan, scatter, search, search_far, finalize) and their count (0 if none); after a
+ * bbox+grid, slab_count, partition, cell_sort, search, search_far, finalize) and their count (0 if none);
+ * the three grid-build slots after bbox+grid hold the slab build's kernels, or cell_count, scan_lookback
+ * and scatter where the cell-wise passes run, or nothing where one CTA bins a whole cloud; after a
  * host entry point and with capacity >= 10, two more: the host-to-device copies in front of the first stage
  * and the device-to-host copies behind the last ("h2d", "d2h"). */
 int pcu_b200_workspace_set_profiling(pcu_b200_workspace* ws, int enabled);

@@ -1067,7 +1067,7 @@ PYBIND11_MODULE(_pcu_internal, mod) {
         if (host_staging < 0 || host_staging > 2) throw py::value_error("host_staging must be 0 (auto), 1 (always) or 2 (never)");
         defaults().host_staging = host_staging;
         if (disable_tie_replay < 0 || disable_tie_replay > 3) throw py::value_error("disable_tie_replay must be 0 .. 3");
-        if (binning < 0 || binning > 2) throw py::value_error("binning must be 0 (auto), 1 (multi-launch) or 2 (one CTA per cloud)");
+        if (binning < 0 || binning > 3) throw py::value_error("binning must be 0 (auto), 1 (cell-wise passes), 2 (one CTA per cloud) or 3 (slab build)");
         defaults().occupancy = cell_occupancy;
         defaults().disable_replay = disable_tie_replay;
         defaults().binning = binning;

@@ -156,14 +156,19 @@ struct Cloud {
     const T* raw;           // (n, 3) caller's points
     long long n;
     Pt<T>* sorted;          // n points in cell order
-    unsigned* rank;         // n: arrival rank of each point inside its cell
+    unsigned* rank;         // n: arrival rank of each point inside its cell (cell-wise passes; null in the slab build)
+    Pt<T>* part;            // n: the points partitioned by slab (slab build; null in the cell-wise passes)
+    unsigned* slab_count;   // slabs: points per slab, then the partition cursors; zeroed per call (slab build)
+    unsigned* slab_base;    // slabs + 1: first point of every slab in part / sorted (slab build)
+    unsigned* slab_hist;    // slab_chunks * slabs: points per slab of every chunk (slab build)
     unsigned* cell_start;   // cell_cap + 1: counts, then exclusive prefix sums
     GridHeader<T>* grid;
     T* wall_lo;             // 3 * stride
     T* wall_hi;             // 3 * stride
     T* bbox_partial;        // bbox_blocks * 6
     unsigned long long* scan_state;  // per scan tile: status | value (decoupled look-back), zeroed per call
-    unsigned* scan_ticket;           // [0] scan tile ticket, [1] finished bbox CTAs; zeroed per call
+    unsigned* scan_ticket;           // [0] scan tiles / finished slab-histogram CTAs, [1] finished bbox CTAs,
+                                     // [2] finished slab-sort CTAs; zeroed per call
     unsigned* occupied;     // number of non-empty cells (counted by the scan), zeroed per call
     unsigned* hint_out;     // host-mapped 8 words of feedback for the next call's grid sizing (grid.cuh), or null
     unsigned* pyramid;      // cell_cap + 64: point counts of the coarser levels (built only when needed)
@@ -171,7 +176,9 @@ struct Cloud {
     int cell_cap;           // upper bound on ncells (host-known)
     int stride;             // wall table stride (host-known)
     int bbox_blocks;        // partial bounding boxes of this cloud (host-known, <= kMaxBBoxBlocks)
-    float min_cell;         // lower limit of the cell size (0: none) -- radius searches ask for cells no finer than their reach
+    int slabs;              // slab build: slabs of consecutive cells (host-known, <= kMaxSlabs)
+    int slab_chunks;        // slab build: CTAs that partition the cloud, one contiguous chunk of points each
+    float min_cell;        // lower limit of the cell size (0: none) -- radius searches ask for cells no finer than their reach
 };
 
 // How kernels receive the cloud descriptors: a device array (batches) or, for a single pair, by value
@@ -196,5 +203,13 @@ constexpr int kScanTile = kScanItems * kScanThreads;
 constexpr int kSmallThreads = 1024;
 constexpr int kSmallMaxCells = 50 * 1024;      // counters: 200 KB of the 227 KB a CTA may own
 constexpr long long kSmallMaxPoints = 128 * 1024;
+// slab build of larger clouds (grid.cuh)
+constexpr int kSlabThreads = 512;               // = kScanThreads: the slab kernels scan with block_exclusive_scan
+constexpr int kSlabTile = 2048;                 // points per staged tile of the chunk walk (4 per thread)
+constexpr long long kSlabChunkPoints = 16384;   // points per chunk CTA, until kMaxSlabChunks CTAs are reached
+constexpr int kMaxSlabChunks = 128;             // chunk CTAs per cloud
+constexpr int kSlabStageBytes = 64 * 1024;      // shared-memory staging of one slab's records (twice the mean slab)
+constexpr int kSlabMaxCells = 16 * 1024;        // cells per slab, upper bound (shared-memory counters)
+constexpr int kMaxSlabs = 8192;                 // = 2^27 cells (the largest cell_cap) / kSlabMaxCells
 
 }  // namespace pcu

@@ -2,8 +2,10 @@
 //
 // Replaces what the reference does before it can answer a query: nanoflann's serial kd-tree build
 // (external/nanoflann/nanoflann.hpp:1363-1375, divideTree :1001-1059), which the reference runs three
-// times per call (SURVEY.md 3a).  Here: bounding box -> grid shape -> per-cell histogram (atomics
-// that also hand out each point's rank in its cell) -> exclusive scan -> scatter into cell order.
+// times per call (SURVEY.md 3a).  Here: bounding box -> grid shape -> cell order, by one of three builds:
+// the slab build (slab histogram -> partition by slab -> per-slab cell sort in shared memory), the
+// cell-wise passes (per-cell histogram whose atomics hand out each point's rank in its cell ->
+// exclusive scan -> scatter), or one CTA per small cloud.
 // Every kernel takes an array of cloud descriptors and uses blockIdx.y as the cloud index, so the
 // two clouds of a Chamfer call -- or the 2*B clouds of a batch -- are binned by the same launches.
 // Nothing here synchronises with the host: the grid shape is chosen on the device.
@@ -461,6 +463,225 @@ __global__ void __launch_bounds__(kThreads) scatter_kernel(const __grid_constant
     if (!load_tile_point<T>(c, g, tile, bar, i, x, y, z)) return;
     const unsigned pos = c.cell_start[linear_cell<T>(g, x, y, z)] + c.rank[i];
     store_pt<T>(c.sorted + pos, x, y, z, i);
+}
+
+// ---------------------------------------------------------------------------------------------
+// 3-5 as a slab build (single pairs above 8192 points).  The linear cell indices 0 .. ncells - 1 are cut
+// into c.slabs slabs of W = ceil(ncells / slabs) consecutive cells.  The host picks `slabs` so that a
+// slab holds half a staging buffer (kSlabStageBytes) of points on average and its cells fit
+// shared-memory counters; W follows from the actual ncells on the device.  Every point is read twice
+// from the caller's array and its record is written twice, each time as contiguous runs, instead of
+// one returning L2 atomic, one dependent gather and one 16-byte store at a random address per point.
+//   slab_hist_kernel       chunk CTAs histogram the slabs of their points; the last one scans the totals
+//   slab_partition_kernel  the same chunks: one run per (chunk, slab), reserved with one atomic
+//   slab_sort_kernel       one CTA per slab sorts its records by cell in shared memory
+// The result is the layout of the cell-wise passes: same cell_start, same set of points per cell.
+// Only the order inside a cell differs, and that order was arrival order there too.
+//
+// The chunk CTAs (grid (max slab_chunks, nclouds)) walk their chunk kSlabTile points at a time: the
+// 3 * kSlabTile scalars of a tile are read flat (coalesced, any alignment) into registers, put in shared
+// memory, and thread t takes points t, t + kSlabThreads, ... of the tile.  The next tile's loads are
+// issued before the current tile is processed.  Dynamic shared memory: the per-slab counters, then the
+// tile (slab_chunk_smem on the host).
+template <typename T>
+__device__ __forceinline__ int slab_width(const GridHeader<T>& g, int slabs) { return (g.ncells + slabs - 1) / slabs; }
+
+template <typename T, typename F>
+__device__ __forceinline__ void for_chunk_points(const Cloud<T>& c, T* tile, F&& f) {
+    constexpr int kPer = 3 * kSlabTile / kSlabThreads;
+    const long long len = (((c.n + c.slab_chunks - 1) / c.slab_chunks) + 3) & ~3ll;
+    const long long first = (long long)blockIdx.x * len;
+    const long long end = first + len < c.n ? first + len : c.n;
+    T v[kPer];
+    auto fetch = [&](long long t0) {
+        const long long left = 3 * (end - t0);
+        const T* src = c.raw + 3 * t0;
+#pragma unroll
+        for (int k = 0; k < kPer; ++k) {
+            const int e = (int)threadIdx.x + k * kSlabThreads;
+            v[k] = e < left ? __ldg(src + e) : (T)0;
+        }
+    };
+    if (first < end) fetch(first);
+    for (long long t0 = first; t0 < end; t0 += kSlabTile) {
+        __syncthreads();   // the previous tile has been consumed
+#pragma unroll
+        for (int k = 0; k < kPer; ++k) tile[threadIdx.x + k * kSlabThreads] = v[k];
+        __syncthreads();
+        if (t0 + kSlabTile < end) fetch(t0 + kSlabTile);
+        const int count = end - t0 < kSlabTile ? (int)(end - t0) : kSlabTile;
+#pragma unroll
+        for (int j = 0; j < kSlabTile / kSlabThreads; ++j) {
+            const int p = (int)threadIdx.x + j * kSlabThreads;
+            if (p < count) f(t0 + p, tile[3 * p], tile[3 * p + 1], tile[3 * p + 2]);
+        }
+    }
+}
+
+__host__ __device__ __forceinline__ size_t slab_counter_bytes(int slabs) { return ((size_t)slabs * sizeof(unsigned) + 15) & ~(size_t)15; }
+
+// 3. slab histogram + scan of the slab totals: grid (max slab_chunks, nclouds), kSlabThreads threads.
+//    Row blockIdx.x of slab_hist gets this chunk's count of every slab; the CTA that finishes last (ticket
+//    in scan_ticket[0]) scans the totals into slab_base and resets slab_count to those bases.
+template <typename T, typename CS>
+__global__ void __launch_bounds__(kSlabThreads) slab_hist_kernel(const __grid_constant__ CS clouds) {
+    grid_dependency_wait();
+    const Cloud<T> c = clouds[blockIdx.y];
+    if ((int)blockIdx.x >= c.slab_chunks) return;
+    extern __shared__ __align__(16) unsigned char slab_smem[];
+    const int S = c.slabs;
+    unsigned* cnt = reinterpret_cast<unsigned*>(slab_smem);
+    T* tile = reinterpret_cast<T*>(slab_smem + slab_counter_bytes(S));
+    __shared__ GridHeader<T> g;
+    __shared__ bool s_last;
+    if (threadIdx.x == 0) g = *c.grid;
+    for (int i = threadIdx.x; i < S; i += kSlabThreads) cnt[i] = 0u;
+    __syncthreads();
+    const int W = slab_width<T>(g, S);
+    for_chunk_points<T>(c, tile, [&](long long, T x, T y, T z) { atomicAdd(&cnt[linear_cell<T>(g, x, y, z) / W], 1u); });
+    __syncthreads();
+    unsigned* row = c.slab_hist + (size_t)blockIdx.x * S;
+    for (int i = threadIdx.x; i < S; i += kSlabThreads) {
+        const unsigned v = cnt[i];
+        row[i] = v;
+        if (v != 0u) atomicAdd(c.slab_count + i, v);
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(c.scan_ticket, 1u) == (unsigned)c.slab_chunks - 1u;
+    __syncthreads();
+    if (!s_last) return;
+    __threadfence();
+    unsigned carry = 0;
+    for (int b = 0; b < S; b += kSlabThreads) {
+        const int i = b + threadIdx.x;
+        const unsigned v = i < S ? __ldcg(c.slab_count + i) : 0u;
+        unsigned total;
+        const unsigned ex = carry + block_exclusive_scan(v, &total);
+        if (i < S) { c.slab_base[i] = ex; c.slab_count[i] = ex; }
+        carry += total;
+    }
+    if (threadIdx.x == 0) c.slab_base[S] = carry;
+}
+
+// 4. slab partition: grid and shared memory as slab_hist_kernel.  The chunk's run in slab s is
+//    reserved with one atomic on slab_count[s]; the points are placed in their runs with shared cursors.
+template <typename T, typename CS>
+__global__ void __launch_bounds__(kSlabThreads) slab_partition_kernel(const __grid_constant__ CS clouds) {
+    grid_dependency_wait();
+    const Cloud<T> c = clouds[blockIdx.y];
+    if ((int)blockIdx.x >= c.slab_chunks) return;
+    extern __shared__ __align__(16) unsigned char slab_smem[];
+    const int S = c.slabs;
+    unsigned* cur = reinterpret_cast<unsigned*>(slab_smem);
+    T* tile = reinterpret_cast<T*>(slab_smem + slab_counter_bytes(S));
+    __shared__ GridHeader<T> g;
+    if (threadIdx.x == 0) g = *c.grid;
+    const unsigned* row = c.slab_hist + (size_t)blockIdx.x * S;
+    for (int i = threadIdx.x; i < S; i += kSlabThreads) {
+        const unsigned v = row[i];
+        cur[i] = v != 0u ? atomicAdd(c.slab_count + i, v) : 0u;
+    }
+    __syncthreads();
+    const int W = slab_width<T>(g, S);
+    for_chunk_points<T>(c, tile, [&](long long i, T x, T y, T z) {
+        const unsigned pos = atomicAdd(&cur[linear_cell<T>(g, x, y, z) / W], 1u);
+        store_pt<T>(c.part + pos, x, y, z, i);
+    });
+}
+
+// 5. per-slab cell sort: grid (max slabs, nclouds), kSlabThreads threads, dynamic shared memory
+//    kSlabStageBytes + 4 * (most cells a slab can have).  A slab that fits the staging buffer ranks its
+//    records with shared counters (cell and rank stay in one register per record), reads them again (from
+//    L2: the slab was just read), places them in shared memory and writes them out coalesced.  A larger slab (clusters, duplicates, surfaces) counts from global memory, then
+//    scatters with shared cursors into its own range of `sorted`: slower, bounded by the slab's size.
+//    Writes cell_start for the slab's cells (slab_base + local prefix), and the last slab also the entries
+//    ncells .. cell_cap (= n).  The last CTA to finish publishes the count of non-empty cells.
+template <typename T, typename CS>
+__global__ void __launch_bounds__(kSlabThreads) slab_sort_kernel(const __grid_constant__ CS clouds) {
+    grid_dependency_wait();
+    constexpr int kCap = kSlabStageBytes / (int)sizeof(Pt<T>);
+    constexpr int kPer = kCap / kSlabThreads;
+    const Cloud<T> c = clouds[blockIdx.y];
+    const int S = c.slabs, s = blockIdx.x;
+    if (s >= S) return;
+    extern __shared__ __align__(16) unsigned char slab_smem[];
+    Pt<T>* stage = reinterpret_cast<Pt<T>*>(slab_smem);
+    unsigned* cnt = reinterpret_cast<unsigned*>(slab_smem + kSlabStageBytes);
+    __shared__ GridHeader<T> g;
+    if (threadIdx.x == 0) g = *c.grid;
+    __syncthreads();
+    const int W = slab_width<T>(g, S);
+    const int cell0 = s * W;
+    const int ncell = max(0, min(W, g.ncells - cell0));
+    const unsigned base = c.slab_base[s];
+    const int count = (int)(c.slab_base[s + 1] - base);
+    const Pt<T>* src = c.part + base;
+    for (int i = threadIdx.x; i < ncell; i += kSlabThreads) cnt[i] = 0u;
+    __syncthreads();
+    const bool staged = count <= kCap;
+    static_assert(kSlabMaxCells <= (1 << 18) && kCap <= (1 << 14), "cell and rank share one word");
+    unsigned slot[kPer];   // cell inside the slab << 14 | rank inside the cell
+    if (staged) {
+        Pt<T> r[kPer];
+#pragma unroll
+        for (int j = 0; j < kPer; ++j) {
+            const int p = (int)threadIdx.x + j * kSlabThreads;
+            if (p < count) r[j] = load_pt<T>(src + p);
+        }
+#pragma unroll
+        for (int j = 0; j < kPer; ++j) {
+            const int p = (int)threadIdx.x + j * kSlabThreads;
+            if (p < count) {
+                const unsigned lc = (unsigned)(linear_cell<T>(g, r[j].x, r[j].y, r[j].z) - cell0);
+                slot[j] = lc << 14 | atomicAdd(&cnt[lc], 1u);
+            }
+        }
+    } else {
+        for (int p = threadIdx.x; p < count; p += kSlabThreads) {
+            const Pt<T> q = load_pt<T>(src + p);
+            atomicAdd(&cnt[linear_cell<T>(g, q.x, q.y, q.z) - cell0], 1u);
+        }
+    }
+    __syncthreads();
+    unsigned carry = 0, nonempty = 0;
+    for (int b = 0; b < ncell; b += kSlabThreads) {
+        const int i = b + threadIdx.x;
+        const unsigned v = i < ncell ? cnt[i] : 0u;
+        unsigned total;
+        const unsigned ex = carry + block_exclusive_scan(v, &total);
+        if (i < ncell) { cnt[i] = ex; c.cell_start[cell0 + i] = base + ex; }
+        nonempty += v != 0u;
+        carry += total;
+    }
+    if (s == S - 1)
+        for (int i = g.ncells + threadIdx.x; i <= c.cell_cap; i += kSlabThreads) c.cell_start[i] = (unsigned)c.n;
+    __syncthreads();
+    if (staged) {
+#pragma unroll
+        for (int j = 0; j < kPer; ++j) {
+            const int p = (int)threadIdx.x + j * kSlabThreads;
+            if (p < count) stage[cnt[slot[j] >> 14] + (slot[j] & 0x3fffu)] = load_pt<T>(src + p);
+        }
+        __syncthreads();
+        for (int p = threadIdx.x; p < count; p += kSlabThreads) c.sorted[base + p] = stage[p];
+    } else {
+        for (int p = threadIdx.x; p < count; p += kSlabThreads) {
+            const Pt<T> q = load_pt<T>(src + p);
+            const unsigned pos = atomicAdd(&cnt[linear_cell<T>(g, q.x, q.y, q.z) - cell0], 1u);
+            store_pt<T>(c.sorted + base + pos, q.x, q.y, q.z, q.i);
+        }
+    }
+    if (c.hint_out != nullptr) {
+        __shared__ bool s_last;
+        nonempty = __reduce_add_sync(0xffffffffu, nonempty);
+        if ((threadIdx.x & 31) == 0 && nonempty != 0u) atomicAdd(c.occupied, nonempty);
+        __threadfence();
+        __syncthreads();
+        if (threadIdx.x == 0) s_last = atomicAdd(c.scan_ticket + 2, 1u) == (unsigned)S - 1u;
+        __syncthreads();
+        if (s_last && threadIdx.x == 0) publish_grid_hint<T>(c, atomicAdd(c.occupied, 0u));
+    }
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -131,7 +131,7 @@ bool runs_this_build(int device) {
 
 // Per-field byte strides between consecutive pairs of a batch (side 0 = first cloud of each pair,
 // side 1 = second cloud; direction 0 = first -> second, direction 1 = second -> first).
-struct CloudStrides { size_t raw, sorted, rank, cell_start, grid, wall_lo, wall_hi, bbox_partial, scan_state, scan_ticket, occupied, pyramid, shape; };
+struct CloudStrides { size_t raw, sorted, rank, part, slab_count, slab_base, slab_hist, cell_start, grid, wall_lo, wall_hi, bbox_partial, scan_state, scan_ticket, occupied, pyramid, shape; };
 struct SweepStrides { size_t out_dist, out_idx, partial, far_list, vfar_list, counters, tie_list; };
 
 template <typename U>
@@ -164,6 +164,10 @@ __global__ void descriptors_kernel(const __grid_constant__ DescriptorArgs<T> a, 
         c.raw = advance(c.raw, p * st.raw);
         c.sorted = advance(c.sorted, p * st.sorted);
         c.rank = advance(c.rank, p * st.rank);
+        c.part = advance(c.part, p * st.part);
+        c.slab_count = advance(c.slab_count, p * st.slab_count);
+        c.slab_base = advance(c.slab_base, p * st.slab_base);
+        c.slab_hist = advance(c.slab_hist, p * st.slab_hist);
         c.cell_start = advance(c.cell_start, p * st.cell_start);
         c.grid = advance(c.grid, p * st.grid);
         c.wall_lo = advance(c.wall_lo, p * st.wall_lo);
@@ -212,6 +216,7 @@ struct pcu_b200_workspace {
     int sm_count = 132;                  // set from the device in pcu_b200_workspace_create
     // optional per-stage timing (bench.py's roofline pass): events recorded on the launching stream
     unsigned small_attr = 0;             // bin_small_kernel instantiations whose shared-memory limit has been raised
+    unsigned slab_attr = 0;              // the same for the slab-build kernels
     // grid-sizing feedback: the kernels leave {cell_cap, non-empty cells, n, valid, unsettled queries, queries, valid, -}
     // per cloud in this
     // host-mapped buffer; the next call with the same shapes reads it (no synchronisation: a hint only)
@@ -254,7 +259,7 @@ template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
 template <> KdReplayBuffers<double>& cloud_tree<double>(pcu_b200_cloud* c) { return c->kd64; }
 
-#define PCU_STAGE_NAMES "descriptors", "bbox+grid", "histogram", "scan", "scatter", "search", "search_far", "finalize", "h2d", "d2h"
+#define PCU_STAGE_NAMES "descriptors", "bbox+grid", "slab_count", "partition", "cell_sort", "search", "search_far", "finalize", "h2d", "d2h"
 
 namespace {
 
@@ -396,6 +401,9 @@ struct Plan {
     size_t zero_bytes = 0;
     size_t zero_cells_bytes = 0;           // leading part that only the multi-launch grid build needs zeroed
     bool one_cta_binning = false;          // bin_small_kernel instead of the five grid-wide passes
+    bool slab_build = false;               // slab_hist / slab_partition / slab_sort instead of the cell-wise passes
+    int max_slabs = 1, max_slab_chunks = 1;
+    size_t slab_chunk_smem = 0, slab_sort_smem = 0;   // dynamic shared memory of the slab kernels
     long long max_n = 0;
     int max_cap = 0;
     int max_bbox_blocks = 1;
@@ -447,19 +455,37 @@ struct Plan {
             max_cap = std::max(max_cap, cl.cell_cap);
         }
         zero_cells_bytes = cv.off - zero_from;
-        for (int s = 0; s < 2; ++s) {
-            Cloud<T>& cl = args.cloud[s];
-            cl.scan_state = take_strided<unsigned long long>(cv, ((size_t)cl.cell_cap + 1 + kScanTile - 1) / kScanTile + 1, B,
-                                                             args.cs[s].scan_state);
-            cl.scan_ticket = take_strided<unsigned>(cv, 2, B, args.cs[s].scan_ticket);   // [0] scan tiles, [1] bbox CTAs
-            cl.occupied = take_strided<unsigned>(cv, 1, B, args.cs[s].occupied);
-        }
         // One CTA per cloud when the counters fit in shared memory and the clouds are small: five dependent
         // launches then cost more than one CTA's serial passes (tools/binning_time.py compares the two; at 65536
         // points one SM takes longer than the grid-wide passes, so larger clouds keep the grid-wide passes
         // whatever the batch size).
         const bool fits = max_cap + 1 <= kSmallMaxCells && max_n <= kSmallMaxPoints;
         one_cta_binning = !sp.prepared_second && fits && (sp.binning == 2 || (sp.binning == 0 && max_n <= 8192));
+        // The slab build for batches and for single pairs above 65536 points: below that, one pair's cell-wise
+        // passes are a few microseconds faster (tools/binning_time.py; DESIGN.md §4).
+        slab_build = !one_cta_binning && (sp.binning == 3 || (sp.binning == 0 && (B > 1 || max_n > 65536)));
+        max_slabs = max_slab_chunks = 1;
+        int max_slab_cells = 1;
+        for (int s = 0; s < 2; ++s) {
+            Cloud<T>& cl = args.cloud[s];
+            cl.scan_state = take_strided<unsigned long long>(cv, ((size_t)cl.cell_cap + 1 + kScanTile - 1) / kScanTile + 1, B,
+                                                             args.cs[s].scan_state);
+            cl.scan_ticket = take_strided<unsigned>(cv, 3, B, args.cs[s].scan_ticket);
+            cl.occupied = take_strided<unsigned>(cv, 1, B, args.cs[s].occupied);
+            if (slab_build) {
+                // a slab holds half the staging buffer on average, and at most kSlabMaxCells cells
+                const long long per_slab = kSlabStageBytes / (2 * (long long)sizeof(Pt<T>));
+                const long long want = std::max((sizes[s] + per_slab - 1) / per_slab, ((long long)cl.cell_cap + kSlabMaxCells - 1) / kSlabMaxCells);
+                cl.slabs = (int)std::min<long long>(kMaxSlabs, std::max(1LL, want));
+                cl.slab_chunks = (int)std::min<long long>(kMaxSlabChunks, (sizes[s] + kSlabChunkPoints - 1) / kSlabChunkPoints);
+                cl.slab_count = take_strided<unsigned>(cv, (size_t)cl.slabs, B, args.cs[s].slab_count);
+                max_slabs = std::max(max_slabs, cl.slabs);
+                max_slab_chunks = std::max(max_slab_chunks, cl.slab_chunks);
+                max_slab_cells = std::max(max_slab_cells, (cl.cell_cap + cl.slabs - 1) / cl.slabs);
+            }
+        }
+        slab_chunk_smem = slab_counter_bytes(max_slabs) + (size_t)3 * kSlabTile * sizeof(T);
+        slab_sort_smem = (size_t)kSlabStageBytes + (size_t)max_slab_cells * sizeof(unsigned);
         for (int d = 0; d < sp.nsweeps; ++d)
             args.sweep[d].counters = take_strided<unsigned>(cv, 8, B, args.ss[d].counters);
         zero_begin = base ? base + zero_from : nullptr;
@@ -468,7 +494,13 @@ struct Plan {
             Cloud<T>& cl = args.cloud[s];
             CloudStrides& st = args.cs[s];
             cl.sorted = take_strided<Pt<T>>(cv, (size_t)cl.n, B, st.sorted);
-            cl.rank = take_strided<unsigned>(cv, (size_t)cl.n, B, st.rank);
+            if (slab_build) {
+                cl.part = take_strided<Pt<T>>(cv, (size_t)cl.n, B, st.part);
+                cl.slab_base = take_strided<unsigned>(cv, (size_t)cl.slabs + 1, B, st.slab_base);
+                cl.slab_hist = take_strided<unsigned>(cv, (size_t)cl.slab_chunks * cl.slabs, B, st.slab_hist);
+            } else {
+                cl.rank = take_strided<unsigned>(cv, (size_t)cl.n, B, st.rank);
+            }
             cl.grid = take_strided<GridHeader<T>>(cv, 1, B, st.grid);
             cl.wall_lo = take_strided<T>(cv, (size_t)3 * cl.stride, B, st.wall_lo);
             cl.wall_hi = take_strided<T>(cv, (size_t)3 * cl.stride, B, st.wall_hi);
@@ -582,7 +614,29 @@ int prepare_plan(pcu_b200_workspace* ws, Plan<T>& plan, PlanSpec<T>& spec, cudaS
     return PCU_B200_OK;
 }
 
-// bbox -> grid -> histogram -> scan -> scatter for every cloud of the plan
+// The slab build's three launches for `clouds` (gridDim.y = ny), each followed by its stage mark.
+template <typename T, typename CS>
+int launch_slab_build(pcu_b200_workspace* ws, const Plan<T>& plan, const CS& clouds, unsigned ny, cudaStream_t stream) {
+    const unsigned bit = 1u << ((sizeof(T) == 8 ? 1 : 0) + (std::is_same<CS, CloudsVal<T>>::value ? 2 : 0));
+    if (!(ws->slab_attr & bit)) {
+        const int chunk_most = (int)(slab_counter_bytes(kMaxSlabs) + (size_t)3 * kSlabTile * sizeof(T));
+        const int sort_most = kSlabStageBytes + kSlabMaxCells * (int)sizeof(unsigned);
+        PCU_CUDA(cudaFuncSetAttribute(slab_hist_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, chunk_most));
+        PCU_CUDA(cudaFuncSetAttribute(slab_partition_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, chunk_most));
+        PCU_CUDA(cudaFuncSetAttribute(slab_sort_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, sort_most));
+        ws->slab_attr |= bit;
+    }
+    const dim3 chunks((unsigned)plan.max_slab_chunks, ny), slabs((unsigned)plan.max_slabs, ny);
+    PCU_LAUNCH_PDL_SMEM((slab_hist_kernel<T, CS>), chunks, kSlabThreads, plan.slab_chunk_smem, stream, clouds);
+    mark(ws, 3, stream);
+    PCU_LAUNCH_PDL_SMEM((slab_partition_kernel<T, CS>), chunks, kSlabThreads, plan.slab_chunk_smem, stream, clouds);
+    mark(ws, 4, stream);
+    PCU_LAUNCH_PDL_SMEM((slab_sort_kernel<T, CS>), slabs, kSlabThreads, plan.slab_sort_smem, stream, clouds);
+    mark(ws, 5, stream);
+    return PCU_B200_OK;
+}
+
+// bbox -> grid -> cell order (slab build, cell-wise passes or one CTA per cloud) for every cloud of the plan
 // `ready` (host entry points, single pairs): two events, recorded on the copy stream when the first / the second
 // cloud has arrived on the device.  The first cloud is then binned -- all five passes -- while the second is
 // still crossing PCIe, and only the second cloud's passes follow its copy.
@@ -593,8 +647,10 @@ template <typename T>
 int enqueue_binning(pcu_b200_workspace* ws, const Plan<T>& plan, cudaStream_t stream, const cudaEvent_t* ready = nullptr,
                     bool first_only = false, const std::function<int()>* between = nullptr) {
     const int nclouds = plan.nclouds;
+    // the slab build writes every cell_start entry: only the counters after the cell counters need zeroing
+    const size_t zero_skip = plan.slab_build ? plan.zero_cells_bytes : 0;
     if ((ready != nullptr || first_only) && plan.by_value && !plan.one_cta_binning) {
-        PCU_CUDA(cudaMemsetAsync(plan.zero_begin, 0, plan.zero_bytes, stream));
+        PCU_CUDA(cudaMemsetAsync(plan.zero_begin + zero_skip, 0, plan.zero_bytes - zero_skip, stream));
         const unsigned scan_blocks = (unsigned)(((long long)plan.max_cap + 1 + kScanTile - 1) / kScanTile);
         const unsigned bin_blocks = (unsigned)((plan.max_n + kThreads - 1) / kThreads);
         for (int s = 0; s < (first_only ? 1 : 2); ++s) {   // first_only: the second cloud is a prepared one
@@ -605,6 +661,10 @@ int enqueue_binning(pcu_b200_workspace* ws, const Plan<T>& plan, cudaStream_t st
             one.v[1] = plan.cv.v[s];
             PCU_LAUNCH_PDL((bbox_partial_kernel<T, CloudsVal<T>, true>), dim3(plan.max_bbox_blocks, 1), kThreads, stream, one);
             mark(ws, 2, stream);
+            if (plan.slab_build) {
+                PCU_TRY(launch_slab_build<T>(ws, plan, one, 1, stream));
+                continue;
+            }
             PCU_LAUNCH_PDL((cell_count_kernel<T, CloudsVal<T>>), dim3(bin_blocks, 1), kThreads, stream, one);
             mark(ws, 3, stream);
             PCU_LAUNCH_PDL((scan_lookback_kernel<T, CloudsVal<T>>), dim3(scan_blocks, 1), kScanThreads, stream, one);
@@ -637,7 +697,7 @@ int enqueue_binning(pcu_b200_workspace* ws, const Plan<T>& plan, cudaStream_t st
         for (int stage = 2; stage <= 5; ++stage) mark(ws, stage, stream);   // the whole build shows up as "bbox+grid"
         return PCU_B200_OK;
     }
-    PCU_CUDA(cudaMemsetAsync(plan.zero_begin, 0, plan.zero_bytes, stream));
+    PCU_CUDA(cudaMemsetAsync(plan.zero_begin + zero_skip, 0, plan.zero_bytes - zero_skip, stream));
     const unsigned scan_blocks = (unsigned)(((long long)plan.max_cap + 1 + kScanTile - 1) / kScanTile);
     if (plan.by_value) {
         PCU_LAUNCH_PDL((bbox_partial_kernel<T, CloudsVal<T>, true>), dim3(plan.max_bbox_blocks, nclouds), kThreads, stream, plan.cv);
@@ -646,6 +706,10 @@ int enqueue_binning(pcu_b200_workspace* ws, const Plan<T>& plan, cudaStream_t st
         PCU_LAUNCH_PDL((grid_setup_kernel<T, CloudsPtr<T>>), dim3(1, nclouds), kThreads, stream, plan.cp);
     }
     mark(ws, 2, stream);
+    if (plan.slab_build) {
+        if (plan.by_value) return launch_slab_build<T>(ws, plan, plan.cv, (unsigned)nclouds, stream);
+        return launch_slab_build<T>(ws, plan, plan.cp, (unsigned)nclouds, stream);
+    }
     const unsigned bin_blocks = (unsigned)((plan.max_n + kThreads - 1) / kThreads);
     PCU_LAUNCH_C(cell_count_kernel, dim3(bin_blocks, nclouds), kThreads);
     mark(ws, 3, stream);
@@ -878,7 +942,6 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
     spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
     spec.nsweeps = 1; spec.k = 1;
     spec.occupancy = 0.125f;          // the cell budget; the cell size itself is held up by min_cell below
-    spec.binning = 1;
     spec.prepared_second = true;      // the one-point second cloud is a dummy: only the first is binned
     Plan<T> plan;
     plan.layout(nullptr, spec);
@@ -1066,7 +1129,6 @@ int cloud_prepare_device(pcu_b200_workspace* ws, const T* points, long long n, p
     spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
     spec.nsweeps = 1; spec.k = 1;
     spec.occupancy = occupancy_for(ws, knn_k);   // the cell size the searches with this k want
-    spec.binning = 1;                 // the grid-wide passes: the handle's buffers are global memory either way
     spec.prepared_second = true;      // (also keeps the dummy out of the one-CTA build)
     Plan<T> plan;
     plan.layout(nullptr, spec);
@@ -1449,7 +1511,7 @@ int pcu_b200_workspace_set_options(pcu_b200_workspace* ws, const pcu_b200_option
     if (opts->cell_occupancy < 0.f) return fail(PCU_B200_INVALID_ARGUMENT, "cell_occupancy must be >= 0");
     if (opts->disable_tie_replay < 0 || opts->disable_tie_replay > 3)
         return fail(PCU_B200_INVALID_ARGUMENT, "disable_tie_replay must be 0 .. 3");
-    if (opts->binning < 0 || opts->binning > 2) return fail(PCU_B200_INVALID_ARGUMENT, "binning must be 0, 1 or 2");
+    if (opts->binning < 0 || opts->binning > 3) return fail(PCU_B200_INVALID_ARGUMENT, "binning must be 0, 1, 2 or 3");
     if (opts->host_staging < 0 || opts->host_staging > 2) return fail(PCU_B200_INVALID_ARGUMENT, "host_staging must be 0, 1 or 2");
     ws->opts = *opts;
     return PCU_B200_OK;

@@ -1,5 +1,5 @@
-"""Scratch timing: the two grid builds (options.binning 1 = five grid-wide passes, 2 = one CTA per cloud)
-for single pairs of several sizes and for batches, with the per-stage device times."""
+"""Scratch timing: the three grid builds (options.binning 1 = cell-wise grid-wide passes, 2 = one CTA per
+cloud, 3 = slab build) for single pairs of several sizes and for batches."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch, numpy as np
@@ -17,19 +17,19 @@ def timeit(fn, warm=3, it=15):
     return float(np.median(ts))
 
 g = torch.Generator(device="cuda").manual_seed(0)
-for n in (1024, 4096, 16384, 32768, 65536, 100000):
+for n in (1024, 4096, 16384, 32768, 65536, 100000, 1000000):
     x = torch.rand((n, 3), generator=g, device="cuda"); y = torch.rand((n, 3), generator=g, device="cuda")
     row = []
-    for mode in (1, 2):
+    for mode in (1, 2, 3):
         I._set_defaults(binning=mode)
         row.append(timeit(lambda: pcu.chamfer_distance(x, y)))
-    print("pair n=%6d: passes %.4f ms  one-CTA %.4f ms" % (n, row[0], row[1]), flush=True)
+    print("pair n=%7d: passes %.4f ms  one-CTA %.4f ms  slabs %.4f ms" % (n, row[0], row[1], row[2]), flush=True)
 for B, n in ((8, 16384), (32, 4096), (64, 65536), (1024, 65536)):
     xb = torch.rand((B, n, 3), generator=g, device="cuda"); yb = torch.rand((B, n, 3), generator=g, device="cuda")
     row = []
-    for mode in (1, 2):
+    for mode in (1, 2, 3):
         I._set_defaults(binning=mode)
         row.append(timeit(lambda: pcu.batched_chamfer_distance(xb, yb), warm=2, it=5))
-    print("batch %4d x %6d: passes %.4f ms  one-CTA %.4f ms -> %.3e qpts/s" % (B, n, row[0], row[1], 2 * B * n / row[1] * 1e3), flush=True)
+    print("batch %4d x %6d: passes %.4f ms  one-CTA %.4f ms  slabs %.4f ms" % (B, n, row[0], row[1], row[2]), flush=True)
     del xb, yb
 I._set_defaults()

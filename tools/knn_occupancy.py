@@ -28,7 +28,7 @@ for k, occs in ((16, (0, 4, 5, 6, 7, 8, 10, 12)), (8, (0, 2, 3, 4, 5, 6)), (4, (
                 for key, val in I._last_profile(dev, stream).items():
                     acc[key] = acc.get(key, 0.0) + val / reps
         I._set_profiling(dev, stream, False)
-        build = sum(acc.get(s, 0) for s in ("bbox+grid", "histogram", "scan", "scatter"))
+        build = sum(acc.get(s, 0) for s in ("bbox+grid", "slab_count", "partition", "cell_sort"))
         print("k=%2d occupancy %5s: build %.3f  search %.3f  far %.3f ms   (per 10^6 queries: %.3f ms)" %
               (k, occ if occ else "dflt", build, acc.get("search", 0), acc.get("search_far", 0),
                (acc.get("search", 0) + acc.get("search_far", 0)) * 1e6 / n), flush=True)
