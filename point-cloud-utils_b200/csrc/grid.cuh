@@ -482,12 +482,24 @@ __global__ void __launch_bounds__(kThreads) scatter_kernel(const __grid_constant
 // 3 * kSlabTile scalars of a tile are read flat (coalesced, any alignment) into registers, put in shared
 // memory, and thread t takes points t, t + kSlabThreads, ... of the tile.  The next tile's loads are
 // issued before the current tile is processed.  Dynamic shared memory: the per-slab counters, then the
-// tile (slab_chunk_smem on the host).
+// tile (slab_hist_smem / slab_part_smem below).
 template <typename T>
 __device__ __forceinline__ int slab_width(const GridHeader<T>& g, int slabs) { return (g.ncells + slabs - 1) / slabs; }
 
+// n / w for any 32-bit n without a divide instruction: m = floor((2^32 - 1) / w) makes umulhi(n, m) either
+// the quotient or one less, and the remainder tells which.
+struct SlabOf {
+    unsigned w, m;
+    __device__ explicit SlabOf(unsigned width) : w(width), m(0xffffffffu / width) {}
+    __device__ __forceinline__ unsigned operator()(unsigned n) const {
+        const unsigned q = __umulhi(n, m);
+        return q + (n - q * w >= w ? 1u : 0u);
+    }
+};
+
+// f(t0, count) runs once per tile, with points t0 .. t0 + count - 1 of the cloud in `tile` (x, y, z each).
 template <typename T, typename F>
-__device__ __forceinline__ void for_chunk_points(const Cloud<T>& c, T* tile, F&& f) {
+__device__ __forceinline__ void for_chunk_tiles(const Cloud<T>& c, T* tile, F&& f) {
     constexpr int kPer = 3 * kSlabTile / kSlabThreads;
     const long long len = (((c.n + c.slab_chunks - 1) / c.slab_chunks) + 3) & ~3ll;
     const long long first = (long long)blockIdx.x * len;
@@ -509,16 +521,27 @@ __device__ __forceinline__ void for_chunk_points(const Cloud<T>& c, T* tile, F&&
         for (int k = 0; k < kPer; ++k) tile[threadIdx.x + k * kSlabThreads] = v[k];
         __syncthreads();
         if (t0 + kSlabTile < end) fetch(t0 + kSlabTile);
-        const int count = end - t0 < kSlabTile ? (int)(end - t0) : kSlabTile;
-#pragma unroll
-        for (int j = 0; j < kSlabTile / kSlabThreads; ++j) {
-            const int p = (int)threadIdx.x + j * kSlabThreads;
-            if (p < count) f(t0 + p, tile[3 * p], tile[3 * p + 1], tile[3 * p + 2]);
-        }
+        f(t0, end - t0 < kSlabTile ? (int)(end - t0) : kSlabTile);
     }
 }
 
 __host__ __device__ __forceinline__ size_t slab_counter_bytes(int slabs) { return ((size_t)slabs * sizeof(unsigned) + 15) & ~(size_t)15; }
+
+// The partition stages a tile in slab order when the tile holds at least one point per slab on average;
+// with fewer, the scan over the slab counters costs more than the coalesced stores win back, and every
+// point goes straight to its run.
+__host__ __device__ __forceinline__ bool slab_staged(int slabs) { return slabs <= kSlabTile; }
+
+template <typename T>
+__host__ __device__ __forceinline__ size_t slab_hist_smem(int slabs) { return slab_counter_bytes(slabs) + (size_t)3 * kSlabTile * sizeof(T); }
+
+// Staged partition: cursors, tile counts and tile offsets (one counter array each), the tile, then the
+// tile's order by slab (one word per point).
+template <typename T>
+__host__ __device__ __forceinline__ size_t slab_part_smem(int slabs) {
+    return slab_staged(slabs) ? 2 * slab_counter_bytes(slabs) + slab_hist_smem<T>(slabs) + (size_t)kSlabTile * sizeof(unsigned)
+                              : slab_hist_smem<T>(slabs);
+}
 
 // 3. slab histogram + scan of the slab totals: grid (max slab_chunks, nclouds), kSlabThreads threads.
 //    Row blockIdx.x of slab_hist gets this chunk's count of every slab; the CTA that finishes last (ticket
@@ -537,8 +560,14 @@ __global__ void __launch_bounds__(kSlabThreads) slab_hist_kernel(const __grid_co
     if (threadIdx.x == 0) g = *c.grid;
     for (int i = threadIdx.x; i < S; i += kSlabThreads) cnt[i] = 0u;
     __syncthreads();
-    const int W = slab_width<T>(g, S);
-    for_chunk_points<T>(c, tile, [&](long long, T x, T y, T z) { atomicAdd(&cnt[linear_cell<T>(g, x, y, z) / W], 1u); });
+    const SlabOf slab_of((unsigned)slab_width<T>(g, S));
+    for_chunk_tiles<T>(c, tile, [&](long long, int count) {
+#pragma unroll
+        for (int j = 0; j < kSlabTile / kSlabThreads; ++j) {
+            const int p = (int)threadIdx.x + j * kSlabThreads;
+            if (p < count) atomicAdd(&cnt[slab_of((unsigned)linear_cell<T>(g, tile[3 * p], tile[3 * p + 1], tile[3 * p + 2]))], 1u);
+        }
+    });
     __syncthreads();
     unsigned* row = c.slab_hist + (size_t)blockIdx.x * S;
     for (int i = threadIdx.x; i < S; i += kSlabThreads) {
@@ -564,29 +593,92 @@ __global__ void __launch_bounds__(kSlabThreads) slab_hist_kernel(const __grid_co
     if (threadIdx.x == 0) c.slab_base[S] = carry;
 }
 
-// 4. slab partition: grid and shared memory as slab_hist_kernel.  The chunk's run in slab s is
-//    reserved with one atomic on slab_count[s]; the points are placed in their runs with shared cursors.
+// 4. slab partition: grid as slab_hist_kernel, dynamic shared memory slab_part_smem.  The chunk's run in
+//    slab s is reserved with one atomic on slab_count[s]; cur[s] is the next free position of that run.
+//    When slab_staged(S), each tile is counting-sorted by slab in shared memory first: its slab counts are
+//    scanned into the tile's order by slab, and thread q stores the q-th point of that order, so consecutive
+//    lanes store consecutive addresses of a run.  Otherwise each point is stored at its run's cursor.
 template <typename T, typename CS>
 __global__ void __launch_bounds__(kSlabThreads) slab_partition_kernel(const __grid_constant__ CS clouds) {
     grid_dependency_wait();
+    constexpr int kPer = kSlabTile / kSlabThreads;
+    static_assert(kSlabTile <= (1 << 16), "slab and tile position share one word");
     const Cloud<T> c = clouds[blockIdx.y];
     if ((int)blockIdx.x >= c.slab_chunks) return;
     extern __shared__ __align__(16) unsigned char slab_smem[];
     const int S = c.slabs;
+    const bool staged = slab_staged(S);
+    const size_t counters = slab_counter_bytes(S);
     unsigned* cur = reinterpret_cast<unsigned*>(slab_smem);
-    T* tile = reinterpret_cast<T*>(slab_smem + slab_counter_bytes(S));
+    unsigned* tcnt = reinterpret_cast<unsigned*>(slab_smem + counters);       // tile counts, then their prefix
+    unsigned* off = reinterpret_cast<unsigned*>(slab_smem + 2 * counters);    // run position - position in the order
+    T* tile = reinterpret_cast<T*>(slab_smem + (staged ? 3 : 1) * counters);
+    unsigned* order = reinterpret_cast<unsigned*>(tile + 3 * kSlabTile);      // slab << 16 | tile position
     __shared__ GridHeader<T> g;
     if (threadIdx.x == 0) g = *c.grid;
     const unsigned* row = c.slab_hist + (size_t)blockIdx.x * S;
     for (int i = threadIdx.x; i < S; i += kSlabThreads) {
         const unsigned v = row[i];
         cur[i] = v != 0u ? atomicAdd(c.slab_count + i, v) : 0u;
+        if (staged) tcnt[i] = 0u;
     }
     __syncthreads();
-    const int W = slab_width<T>(g, S);
-    for_chunk_points<T>(c, tile, [&](long long i, T x, T y, T z) {
-        const unsigned pos = atomicAdd(&cur[linear_cell<T>(g, x, y, z) / W], 1u);
-        store_pt<T>(c.part + pos, x, y, z, i);
+    const SlabOf slab_of((unsigned)slab_width<T>(g, S));
+    if (!staged) {
+        for_chunk_tiles<T>(c, tile, [&](long long t0, int count) {
+#pragma unroll
+            for (int j = 0; j < kPer; ++j) {
+                const int p = (int)threadIdx.x + j * kSlabThreads;
+                if (p < count) {
+                    const T x = tile[3 * p], y = tile[3 * p + 1], z = tile[3 * p + 2];
+                    const unsigned pos = atomicAdd(&cur[slab_of((unsigned)linear_cell<T>(g, x, y, z))], 1u);
+                    store_pt<T>(c.part + pos, x, y, z, t0 + p);
+                }
+            }
+        });
+        return;
+    }
+    for_chunk_tiles<T>(c, tile, [&](long long t0, int count) {
+        unsigned key[kPer];   // slab << 16 | rank inside the tile's share of the slab
+#pragma unroll
+        for (int j = 0; j < kPer; ++j) {
+            const int p = (int)threadIdx.x + j * kSlabThreads;
+            if (p < count) {
+                const unsigned s = slab_of((unsigned)linear_cell<T>(g, tile[3 * p], tile[3 * p + 1], tile[3 * p + 2]));
+                key[j] = s << 16 | atomicAdd(&tcnt[s], 1u);
+            }
+        }
+        __syncthreads();
+        unsigned carry = 0;
+        for (int b = 0; b < S; b += kSlabThreads) {
+            const int i = b + threadIdx.x;
+            const unsigned v = i < S ? tcnt[i] : 0u;
+            unsigned total;
+            const unsigned ex = carry + block_exclusive_scan(v, &total);
+            if (i < S) {
+                const unsigned run = cur[i];
+                tcnt[i] = ex;
+                off[i] = run - ex;
+                cur[i] = run + v;
+            }
+            carry += total;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < kPer; ++j) {
+            const int p = (int)threadIdx.x + j * kSlabThreads;
+            if (p < count) order[tcnt[key[j] >> 16] + (key[j] & 0xffffu)] = (key[j] & 0xffff0000u) | (unsigned)p;
+        }
+        __syncthreads();
+#pragma unroll
+        for (int j = 0; j < kPer; ++j) {
+            const int q = (int)threadIdx.x + j * kSlabThreads;
+            if (q < count) {
+                const unsigned w = order[q], p = w & 0xffffu;
+                store_pt<T>(c.part + off[w >> 16] + q, tile[3 * p], tile[3 * p + 1], tile[3 * p + 2], t0 + p);
+            }
+        }
+        for (int i = threadIdx.x; i < S; i += kSlabThreads) tcnt[i] = 0u;
     });
 }
 

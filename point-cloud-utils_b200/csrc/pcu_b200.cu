@@ -403,7 +403,7 @@ struct Plan {
     bool one_cta_binning = false;          // bin_small_kernel instead of the five grid-wide passes
     bool slab_build = false;               // slab_hist / slab_partition / slab_sort instead of the cell-wise passes
     int max_slabs = 1, max_slab_chunks = 1;
-    size_t slab_chunk_smem = 0, slab_sort_smem = 0;   // dynamic shared memory of the slab kernels
+    size_t slab_hist_smem = 0, slab_part_smem = 0, slab_sort_smem = 0;   // dynamic shared memory of the slab kernels
     long long max_n = 0;
     int max_cap = 0;
     int max_bbox_blocks = 1;
@@ -465,6 +465,7 @@ struct Plan {
         // passes are a few microseconds faster (tools/binning_time.py; DESIGN.md §4).
         slab_build = !one_cta_binning && (sp.binning == 3 || (sp.binning == 0 && (B > 1 || max_n > 65536)));
         max_slabs = max_slab_chunks = 1;
+        slab_part_smem = 0;
         int max_slab_cells = 1;
         for (int s = 0; s < 2; ++s) {
             Cloud<T>& cl = args.cloud[s];
@@ -482,9 +483,10 @@ struct Plan {
                 max_slabs = std::max(max_slabs, cl.slabs);
                 max_slab_chunks = std::max(max_slab_chunks, cl.slab_chunks);
                 max_slab_cells = std::max(max_slab_cells, (cl.cell_cap + cl.slabs - 1) / cl.slabs);
+                slab_part_smem = std::max(slab_part_smem, pcu::slab_part_smem<T>(cl.slabs));
             }
         }
-        slab_chunk_smem = slab_counter_bytes(max_slabs) + (size_t)3 * kSlabTile * sizeof(T);
+        slab_hist_smem = pcu::slab_hist_smem<T>(max_slabs);
         slab_sort_smem = (size_t)kSlabStageBytes + (size_t)max_slab_cells * sizeof(unsigned);
         for (int d = 0; d < sp.nsweeps; ++d)
             args.sweep[d].counters = take_strided<unsigned>(cv, 8, B, args.ss[d].counters);
@@ -619,17 +621,18 @@ template <typename T, typename CS>
 int launch_slab_build(pcu_b200_workspace* ws, const Plan<T>& plan, const CS& clouds, unsigned ny, cudaStream_t stream) {
     const unsigned bit = 1u << ((sizeof(T) == 8 ? 1 : 0) + (std::is_same<CS, CloudsVal<T>>::value ? 2 : 0));
     if (!(ws->slab_attr & bit)) {
-        const int chunk_most = (int)(slab_counter_bytes(kMaxSlabs) + (size_t)3 * kSlabTile * sizeof(T));
+        const int hist_most = (int)slab_hist_smem<T>(kMaxSlabs);
+        const int part_most = (int)std::max(slab_part_smem<T>(kMaxSlabs), slab_part_smem<T>(kSlabTile));
         const int sort_most = kSlabStageBytes + kSlabMaxCells * (int)sizeof(unsigned);
-        PCU_CUDA(cudaFuncSetAttribute(slab_hist_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, chunk_most));
-        PCU_CUDA(cudaFuncSetAttribute(slab_partition_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, chunk_most));
+        PCU_CUDA(cudaFuncSetAttribute(slab_hist_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, hist_most));
+        PCU_CUDA(cudaFuncSetAttribute(slab_partition_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, part_most));
         PCU_CUDA(cudaFuncSetAttribute(slab_sort_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, sort_most));
         ws->slab_attr |= bit;
     }
     const dim3 chunks((unsigned)plan.max_slab_chunks, ny), slabs((unsigned)plan.max_slabs, ny);
-    PCU_LAUNCH_PDL_SMEM((slab_hist_kernel<T, CS>), chunks, kSlabThreads, plan.slab_chunk_smem, stream, clouds);
+    PCU_LAUNCH_PDL_SMEM((slab_hist_kernel<T, CS>), chunks, kSlabThreads, plan.slab_hist_smem, stream, clouds);
     mark(ws, 3, stream);
-    PCU_LAUNCH_PDL_SMEM((slab_partition_kernel<T, CS>), chunks, kSlabThreads, plan.slab_chunk_smem, stream, clouds);
+    PCU_LAUNCH_PDL_SMEM((slab_partition_kernel<T, CS>), chunks, kSlabThreads, plan.slab_part_smem, stream, clouds);
     mark(ws, 4, stream);
     PCU_LAUNCH_PDL_SMEM((slab_sort_kernel<T, CS>), slabs, kSlabThreads, plan.slab_sort_smem, stream, clouds);
     mark(ws, 5, stream);
