@@ -316,6 +316,23 @@ int pcu_b200_normals_ball_f32(pcu_b200_workspace* ws, const float* points, int64
 int pcu_b200_normals_ball_f64(pcu_b200_workspace* ws, const double* points, int64_t n, const double* view_dirs,
                               const pcu_b200_ball_options* options, int64_t* out_idx, double* out_normals, int64_t* out_count, void* stream);
 
+/* ---- Poisson-disk down-sampling ---------------------------------------------------------------
+ * Replaces blue_noise_downsample as called by downsample_point_cloud_poisson_disk (src/sample_point_cloud.cpp:14-109,
+ * :328) for one radius; the target-count search around it (:278-326) stays with the caller, one call per radius.
+ * The reference's subset (libigl blue_noise + std::mt19937 over an unordered_map) cannot be reproduced; the sample
+ * here is a pure function of (points, radius, seed):
+ *   r = (scalar)radius, rr = r * r rounded in the scalar type (:16, :72);  rows p, q conflict iff d2(p, q) < rr, d2
+ *   rounded like the library's metric (the boundary d2 == rr is unpinned against the reference);  every row has the
+ *   key (mix32(seed ^ mix32(row * 0x9e3779b9 + 0x85ebca6b)), row), 32-bit wrap-around, compared lexicographically;
+ *   the sample is the greedy maximal independent set in key order (visit rows by ascending key, keep a row that
+ *   conflicts with no kept row): no two samples conflict, every row is a sample or conflicts with one.
+ *   radius > 0; n <= 2^31 - 1.  out_idx (capacity n, int32): the sampled rows, ascending;  out_count: device int64;
+ *   out_rounds (may be NULL): device int32, selection rounds run (one grid barrier each).  DEVICE pointers. */
+int pcu_b200_poisson_disk_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double radius, uint32_t seed,
+                              int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream);
+int pcu_b200_poisson_disk_f64(pcu_b200_workspace* ws, const double* points, int64_t n, double radius, uint32_t seed,
+                              int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

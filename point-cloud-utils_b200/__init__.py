@@ -39,7 +39,8 @@ except ImportError as _e:  # pragma: no cover - exercised only on a broken insta
 __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_distance", "chamfer_distance",
            "batched_chamfer_distance", "estimate_point_cloud_normals_knn", "estimate_point_cloud_normals_ball",
            "morton_encode", "morton_decode", "morton_add", "morton_subtract", "morton_knn", "pairwise_distances", "sinkhorn",
-           "earth_movers_distance", "downsample_point_cloud_on_voxel_grid", "deduplicate_point_cloud",
+           "earth_movers_distance", "downsample_point_cloud_on_voxel_grid", "downsample_point_cloud_poisson_disk",
+           "deduplicate_point_cloud",
            "deduplicate_mesh_vertices", "prepare_cloud", "pinned_empty", "PreparedCloud", "device_count",
            "current_device", "launch_count"]
 
@@ -767,6 +768,7 @@ def morton_knn(codes, qcodes, k, sort_dist=True, *, device=None):
 
 from ._sinkhorn import pairwise_distances, sinkhorn, earth_movers_distance  # noqa: E402  (N4: dense metrics)
 from ._dedup import deduplicate_point_cloud, deduplicate_mesh_vertices  # noqa: E402  (N2: duplicate removal)
+from ._poisson import downsample_point_cloud_poisson_disk  # noqa: E402  (Poisson-disk downsampling)
 
 
 def _voxel_internal(points, attrib, voxel_size, min_bound, max_bound, min_points_per_voxel, device, return_counts=False):

@@ -530,6 +530,22 @@ void normals_ball_device(bool is_f64, uintptr_t points, int64_t n, uintptr_t vie
     check(status);
 }
 
+// One Poisson-disk sample of a device cloud at one radius (the search over radii is in _poisson.py).
+void poisson_disk_device(bool is_f64, uintptr_t points, int64_t n, double radius, uint32_t seed, uintptr_t out_idx,
+                         uintptr_t out_count, uintptr_t out_rounds, int device, uintptr_t stream) {
+    Slot& slot = pool().get(device, stream);
+    pcu_b200_workspace* ws = slot.ws;
+    int status;
+    {
+        CallScope scope(slot);
+        status = is_f64 ? pcu_b200_poisson_disk_f64(ws, (const double*)points, n, radius, seed, (int32_t*)out_idx,
+                                                    (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream)
+                        : pcu_b200_poisson_disk_f32(ws, (const float*)points, n, radius, seed, (int32_t*)out_idx,
+                                                    (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream);
+    }
+    check(status);
+}
+
 // ---- Morton codes (src/morton.cpp) ----------------------------------------------------------------
 // dtype rules of the bindings: pts int32 / int64; codes uint32 / uint64 (uint32 codes are widened, as the
 // reference's MortonCode64(uint64_t) constructor does implicitly); results are uint64 / int32 / int64 like the reference's.
@@ -990,6 +1006,7 @@ PYBIND11_MODULE(_pcu_internal, mod) {
             py::arg("weight_function") = "constant", py::arg("random_seed") = -1, py::arg("device") = -1,
             "Indices of the kept points and their unit normals (plane fit to the points in a ball around each point).");
     mod.def("_normals_ball_device", &normals_ball_device);
+    mod.def("_poisson_disk_device", &poisson_disk_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),

@@ -117,6 +117,13 @@ __device__ __forceinline__ T sq_gap(T q, T wall) {  // lower bound for one axis,
     return R::mul(d, d);
 }
 
+// 32-bit integer finaliser (a bijection): the counter-based hash behind the random choices of the ball normals'
+// neighbour subsets and of the Poisson-disk sample's priorities.
+__device__ __forceinline__ unsigned mix32(unsigned h) {
+    h ^= h >> 16; h *= 0x7feb352du; h ^= h >> 15; h *= 0x846ca68bu; h ^= h >> 16;
+    return h;
+}
+
 // Uniform grid over one cloud's bounding box.  Lives in device memory; written by grid_setup.
 //   cell(p) = clamp(int(fl(fl(p - origin) * inv_h)), 0, dim-1)   -- monotone in p, so the walls
 //   below are exact statements about where points of a given cell can lie:

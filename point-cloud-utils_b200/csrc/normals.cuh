@@ -128,11 +128,6 @@ struct BallParams {
     unsigned seed;
 };
 
-__device__ __forceinline__ unsigned mix32(unsigned h) {
-    h ^= h >> 16; h *= 0x7feb352du; h ^= h >> 15; h *= 0x846ca68bu; h ^= h >> 16;
-    return h;
-}
-
 template <typename T> __device__ __forceinline__ T sub_down(T a, T b);
 template <> __device__ __forceinline__ float sub_down<float>(float a, float b) { return __fsub_rd(a, b); }
 template <> __device__ __forceinline__ double sub_down<double>(double a, double b) { return __dsub_rd(a, b); }
@@ -140,12 +135,13 @@ template <typename T> __device__ __forceinline__ T add_up(T a, T b);
 template <> __device__ __forceinline__ float add_up<float>(float a, float b) { return __fadd_ru(a, b); }
 template <> __device__ __forceinline__ double add_up<double>(double a, double b) { return __dadd_ru(a, b); }
 
-// Calls visit(point, d2) for every point of the binned cloud with d2(q, point) < r2, in cell order.
+// Calls visit(pos, point, d2) for every point of the binned cloud with d2(q, point) < r2, in cell order, until visit
+// returns true (the walk then ends and returns true); pos is the point's position in cl.sorted.
 // Coverage: d2 >= fl(fl(q-p)^2) per axis and every rounding is monotone, so |q_a - p_a| <= sqrt(r2) (1 + 2 ulp) for
 // every qualifying point; the box below is that interval, widened and rounded outwards, mapped through the monotone
 // cell_of.  Rows (fixed y, z) whose wall gap already reaches r2 are skipped with the bound of search.cuh.
 template <typename T, typename Visit>
-__device__ __forceinline__ void walk_ball(const Cloud<T>& cl, const GridHeader<T>& g, const Pt<T>& q, T r2, Visit&& visit) {
+__device__ __forceinline__ bool walk_ball_until(const Cloud<T>& cl, const GridHeader<T>& g, const Pt<T>& q, T r2, Visit&& visit) {
     using R = Real<T>;
     const T eps = sizeof(T) == 4 ? (T)1.1920929e-7 : (T)2.220446049250313e-16;
     const T reach = R::root(r2) * ((T)1 + (T)8 * eps) + (sizeof(T) == 4 ? (T)1.1754944e-38 : (T)2.2250738585072014e-308);
@@ -171,10 +167,17 @@ __device__ __forceinline__ void walk_ball(const Cloud<T>& cl, const GridHeader<T
             for (unsigned j = a; j < b; ++j) {
                 const Pt<T> p = load_pt<T>(cl.sorted + j);
                 const T d2 = dist2<T>(q.x, q.y, q.z, p.x, p.y, p.z);
-                if (d2 < r2) visit(p, d2);
+                if (d2 < r2 && visit(j, p, d2)) return true;
             }
         }
     }
+    return false;
+}
+
+// Calls visit(point, d2) for every point of the binned cloud with d2(q, point) < r2, in cell order.
+template <typename T, typename Visit>
+__device__ __forceinline__ void walk_ball(const Cloud<T>& cl, const GridHeader<T>& g, const Pt<T>& q, T r2, Visit&& visit) {
+    walk_ball_until<T>(cl, g, q, r2, [&](unsigned, const Pt<T>& p, T d2) { visit(p, d2); return false; });
 }
 
 // The binning kernels place the points of a cell in arrival order (an atomic counter), which changes from run to run.

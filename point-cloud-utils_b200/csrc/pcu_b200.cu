@@ -31,6 +31,7 @@
 #include "sinkhorn.cuh"
 #include "voxel.cuh"
 #include "dedup.cuh"
+#include "poisson.cuh"
 
 using namespace pcu;
 
@@ -984,6 +985,89 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
     return PCU_B200_OK;
 }
 
+// ---- Poisson-disk downsampling (downsample_point_cloud_poisson_disk) --------------------------------------------
+// The cloud is binned once (cells no finer than half the radius, as for the ball normals), then ONE cooperative launch
+// runs every selection round of poisson.cuh with grid barriers between them -- the number of rounds depends on the
+// data, and a barrier keeps that decision on the device without a launch per possible round -- and the kept rows are
+// compacted in ascending order like the normals' kept points.
+template <typename T>
+int poisson_grid_blocks(int device, int sm_count, long long n, unsigned* out_blocks) {
+    constexpr int kMaxDevices = 64;   // co-residency limit of the cooperative launch, cached per device
+    static std::atomic<int> cached[kMaxDevices];
+    const int slot = device >= 0 && device < kMaxDevices ? device : 0;
+    int per_sm = cached[slot].load(std::memory_order_acquire);
+    if (per_sm == 0 || slot != device) {
+        int fit = 0;
+        PCU_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, poisson_rounds_kernel<T>, kThreads, 0));
+        if (fit < 1) return fail(PCU_B200_CUDA_ERROR, "poisson_rounds_kernel cannot be resident on this device");
+        per_sm = std::min(8, fit);
+        cached[slot].store(per_sm, std::memory_order_release);
+    }
+    const long long want = (n + kThreads - 1) / kThreads;
+    *out_blocks = (unsigned)std::max<long long>(1, std::min<long long>(want, (long long)per_sm * sm_count));
+    return PCU_B200_OK;
+}
+
+template <typename T>
+int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, double radius, unsigned seed, int* out_idx,
+                        long long* out_count, int* out_rounds, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!(radius > 0.0)) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid radius (%f) must be greater than 0.", radius);
+    if (!points || n <= 0)
+        return fail(PCU_B200_INVALID_ARGUMENT, "Invalid point set with zero elements: points must have shape (n, 3) (got %lld rows)", n);
+    if (n > 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "poisson_disk: at most 2^31 - 1 points (the indices are int32), got %lld", n);
+    PCU_TRY(check_cloud_args<T>(points, n, points, 1));
+    if (!out_idx || !out_count) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    const T r = (T)radius;        // blue_noise_downsample takes the radius as the cloud's scalar (:299, :328)
+    const T rr = r * r;           // `const double rr = r*r;` with r of that type: the product is rounded in T (:72)
+    PlanSpec<T> spec;
+    spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
+    spec.nsweeps = 1; spec.k = 1;
+    spec.occupancy = 0.125f;          // the cell budget; the cell size itself is held up by min_cell below
+    spec.prepared_second = true;      // the one-point second cloud is a dummy: only the first is binned
+    Plan<T> plan;
+    plan.layout(nullptr, spec);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(ensure_arena(ws, plan.total, stream));
+    plan.layout(ws->arena, spec);
+    plan.cv.v[0].min_cell = (float)std::min(1e30, 0.5 * (double)r);
+    plan.cv.v[0].hint_out = nullptr;
+    unsigned blocks = 1;
+    PCU_TRY(poisson_grid_blocks<T>(ws->device, ws->sm_count, n, &blocks));
+    const long long nblocks = (n + kThreads - 1) / kThreads;
+    Carver measure(nullptr);
+    auto carve = [&](Carver& cv, PoissonScratch& s, unsigned*& counts) {
+        s.ring = cv.take<unsigned>(4);
+        s.state = cv.take<unsigned char>((size_t)n);
+        s.keep = cv.take<unsigned char>((size_t)n);
+        s.list[0] = cv.take<unsigned>((size_t)n);
+        s.list[1] = cv.take<unsigned>((size_t)n);
+        counts = cv.take<unsigned>((size_t)nblocks);
+    };
+    PoissonScratch s; unsigned* counts;
+    carve(measure, s, counts);
+    PCU_TRY(grow_block(ws->aux, ws->aux_bytes, measure.off, stream, "Poisson-disk scratch"));
+    Carver cv(ws->aux);
+    carve(cv, s, counts);
+    PCU_CUDA(cudaMemsetAsync(s.ring, 0, (size_t)((unsigned char*)s.list[0] - (unsigned char*)s.ring), stream));   // ring, state, keep
+    mark(ws, 0, stream);
+    mark(ws, 1, stream);
+    PCU_TRY(enqueue_binning(ws, plan, stream, nullptr, true));
+    Cloud<T> cl = plan.cv.v[0];
+    T rr_arg = rr;
+    void* args[] = {(void*)&cl, (void*)&rr_arg, (void*)&seed, (void*)&s, (void*)&out_rounds};
+    PCU_CUDA(cudaLaunchCooperativeKernel((void*)poisson_rounds_kernel<T>, dim3(blocks), dim3(kThreads), args, 0, stream));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    mark(ws, 6, stream);
+    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, s.keep, n, counts);
+    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, counts, nblocks, out_count);
+    PCU_LAUNCH(keep_scatter_rows_kernel, (unsigned)nblocks, kThreads, stream, s.keep, n, counts, out_idx);
+    mark(ws, 7, stream);
+    mark(ws, 8, stream);
+    return PCU_B200_OK;
+}
+
 // ---- duplicate removal (SURVEY.md 8f N2, src/remove_duplicates.cpp) ----------------------------------------
 // Stable LSD radix sort of `n` records between two buffers; returns the buffer holding the sorted records.
 template <typename Rec>
@@ -1683,6 +1767,15 @@ int pcu_b200_normals_ball_f32(pcu_b200_workspace* ws, const float* points, int64
 int pcu_b200_normals_ball_f64(pcu_b200_workspace* ws, const double* points, int64_t n, const double* view_dirs,
                               const pcu_b200_ball_options* options, int64_t* out_idx, double* out_normals, int64_t* out_count, void* stream) {
     return normals_ball_device<double>(ws, points, n, view_dirs, options, (long long*)out_idx, out_normals, (long long*)out_count, (cudaStream_t)stream);
+}
+
+int pcu_b200_poisson_disk_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double radius, uint32_t seed,
+                              int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream) {
+    return poisson_disk_device<float>(ws, points, n, radius, seed, out_idx, (long long*)out_count, out_rounds, (cudaStream_t)stream);
+}
+int pcu_b200_poisson_disk_f64(pcu_b200_workspace* ws, const double* points, int64_t n, double radius, uint32_t seed,
+                              int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream) {
+    return poisson_disk_device<double>(ws, points, n, radius, seed, out_idx, (long long*)out_count, out_rounds, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,
