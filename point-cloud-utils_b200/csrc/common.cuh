@@ -124,6 +124,59 @@ __device__ __forceinline__ unsigned mix32(unsigned h) {
     return h;
 }
 
+// Block-wide exclusive scan, kBlock threads: returns the exclusive prefix of v and sets *total to the block sum in
+// every thread.  Ends with a barrier, so it may be called again right away (in a loop, on the same warp_sum).
+template <int kBlock>
+__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned* total) {
+    static_assert(kBlock % 32 == 0 && kBlock <= 1024, "whole warps, at most 32 of them");
+    constexpr int kWarps = kBlock / 32;
+    __shared__ unsigned warp_sum[kWarps];
+    const int l = threadIdx.x & 31, w = threadIdx.x >> 5;
+    unsigned inc = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
+        if (l >= o) inc += u;
+    }
+    if (l == 31) warp_sum[w] = inc;
+    __syncthreads();
+    if (w == 0) {
+        unsigned s = l < kWarps ? warp_sum[l] : 0u;
+#pragma unroll
+        for (int o = 1; o < kWarps; o <<= 1) {
+            const unsigned u = __shfl_up_sync(0xffffffffu, s, o);
+            if (l >= o) s += u;
+        }
+        if (l < kWarps) warp_sum[l] = s;   // inclusive over warps
+    }
+    __syncthreads();
+    const unsigned before = w ? warp_sum[w - 1] : 0u;
+    *total = warp_sum[kWarps - 1];
+    __syncthreads();
+    return before + inc - v;
+}
+
+// Exclusive scan of `count` values, kBlock of them per round, with the running total carried between rounds:
+// thread t handles i = t, t + kBlock, ...; load(i) gives value i and store(i, prefix, value) receives its exclusive
+// prefix.  Returns the sum of all values to every thread.  Block-wide; ends with a barrier, so the stores are visible
+// to the whole block on return.  The rounds are counted in the index type `I` of `count`: nvcc unrolls the loop over a
+// signed count (the slab build's per-tile scan needs that) and keeps the one over an unsigned count rolled (fewer
+// registers where the scan is the whole kernel).
+template <int kBlock, class I, class Load, class Store>
+__device__ __forceinline__ unsigned block_scan_rounds(I count, Load load, Store store) {
+    unsigned carry = 0;
+    for (I b = 0; b < count; b += kBlock) {
+        const I i = b + (I)threadIdx.x;
+        const unsigned v = i < count ? load(i) : 0u;
+        unsigned total;
+        const unsigned ex = carry + block_exclusive_scan<kBlock>(v, &total);
+        if (i < count) store(i, ex, v);
+        carry += total;
+    }
+    __syncthreads();
+    return carry;
+}
+
 // Uniform grid over one cloud's bounding box.  Lives in device memory; written by grid_setup.
 //   cell(p) = clamp(int(fl(fl(p - origin) * inv_h)), 0, dim-1)   -- monotone in p, so the walls
 //   below are exact statements about where points of a given cell can lie:
@@ -211,7 +264,7 @@ constexpr int kSmallThreads = 1024;
 constexpr int kSmallMaxCells = 50 * 1024;      // counters: 200 KB of the 227 KB a CTA may own
 constexpr long long kSmallMaxPoints = 128 * 1024;
 // slab build of larger clouds (grid.cuh)
-constexpr int kSlabThreads = 512;               // = kScanThreads: the slab kernels scan with block_exclusive_scan
+constexpr int kSlabThreads = 512;               // threads of every slab kernel
 constexpr int kSlabTile = 2048;                 // points per staged tile of the chunk walk (4 per thread)
 constexpr long long kSlabChunkPoints = 16384;   // points per chunk CTA, until kMaxSlabChunks CTAs are reached
 constexpr int kMaxSlabChunks = 128;             // chunk CTAs per cloud

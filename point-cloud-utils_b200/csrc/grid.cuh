@@ -360,40 +360,11 @@ __global__ void __launch_bounds__(kThreads) cell_count_kernel(const __grid_const
 }
 
 // ---------------------------------------------------------------------------------------------
-// 4. exclusive scan of cell_start[0 .. cell_cap], in place
-__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned* total) {
-    // kScanThreads threads; returns the exclusive prefix of v, *total = block sum
-    __shared__ unsigned warp_sum[kScanThreads / 32];
-    const int l = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (l >= o) inc += u;
-    }
-    if (l == 31) warp_sum[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-        unsigned s = l < kScanThreads / 32 ? warp_sum[l] : 0u;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned u = __shfl_up_sync(0xffffffffu, s, o);
-            if (l >= o) s += u;
-        }
-        if (l < kScanThreads / 32) warp_sum[l] = s;   // inclusive over warps
-    }
-    __syncthreads();
-    const unsigned before = w ? warp_sum[w - 1] : 0u;
-    *total = warp_sum[kScanThreads / 32 - 1];
-    __syncthreads();
-    return before + inc - v;
-}
-
-// Single-pass scan with decoupled look-back: every CTA draws a tile ticket, scans its tile, publishes
-// the tile total, and resolves its carry by walking back over the published states of the tiles
-// before it.  state word = status (bits 63:62; 1 = tile total, 2 = inclusive prefix) | value (low 32).
-// Ticket and states must be zero on entry (they live in the call's zeroed region).
-// grid (tiles, nclouds)
+// 4. exclusive scan of cell_start[0 .. cell_cap], in place: a single-pass scan with decoupled look-back.
+//    Every CTA draws a tile ticket, scans its tile, publishes the tile total, and resolves its carry by walking
+//    back over the published states of the tiles before it.
+//    state word = status (bits 63:62; 1 = tile total, 2 = inclusive prefix) | value (low 32).
+//    Ticket and states must be zero on entry (they live in the call's zeroed region).  grid (tiles, nclouds)
 template <typename T, typename CS>
 __global__ void __launch_bounds__(kScanThreads) scan_lookback_kernel(const __grid_constant__ CS clouds) {
     grid_dependency_wait();
@@ -417,7 +388,7 @@ __global__ void __launch_bounds__(kScanThreads) scan_lookback_kernel(const __gri
     nonempty = __reduce_add_sync(0xffffffffu, nonempty);
     if ((threadIdx.x & 31) == 0 && nonempty != 0u) atomicAdd(c.occupied, nonempty);
     unsigned total;
-    const unsigned ex = block_exclusive_scan(s, &total);
+    const unsigned ex = block_exclusive_scan<kScanThreads>(s, &total);
     if (threadIdx.x < 32) {
         // warp-wide look-back: lane l inspects tile (tile - 1 - l), 32 predecessors per step
         volatile unsigned long long* state = c.scan_state;
@@ -581,16 +552,10 @@ __global__ void __launch_bounds__(kSlabThreads) slab_hist_kernel(const __grid_co
     __syncthreads();
     if (!s_last) return;
     __threadfence();
-    unsigned carry = 0;
-    for (int b = 0; b < S; b += kSlabThreads) {
-        const int i = b + threadIdx.x;
-        const unsigned v = i < S ? __ldcg(c.slab_count + i) : 0u;
-        unsigned total;
-        const unsigned ex = carry + block_exclusive_scan(v, &total);
-        if (i < S) { c.slab_base[i] = ex; c.slab_count[i] = ex; }
-        carry += total;
-    }
-    if (threadIdx.x == 0) c.slab_base[S] = carry;
+    const unsigned all = block_scan_rounds<kSlabThreads>(
+        S, [&](int i) { return __ldcg(c.slab_count + i); },
+        [&](int i, unsigned ex, unsigned) { c.slab_base[i] = ex; c.slab_count[i] = ex; });
+    if (threadIdx.x == 0) c.slab_base[S] = all;
 }
 
 // 4. slab partition: grid as slab_hist_kernel, dynamic shared memory slab_part_smem.  The chunk's run in
@@ -649,21 +614,12 @@ __global__ void __launch_bounds__(kSlabThreads) slab_partition_kernel(const __gr
             }
         }
         __syncthreads();
-        unsigned carry = 0;
-        for (int b = 0; b < S; b += kSlabThreads) {
-            const int i = b + threadIdx.x;
-            const unsigned v = i < S ? tcnt[i] : 0u;
-            unsigned total;
-            const unsigned ex = carry + block_exclusive_scan(v, &total);
-            if (i < S) {
-                const unsigned run = cur[i];
-                tcnt[i] = ex;
-                off[i] = run - ex;
-                cur[i] = run + v;
-            }
-            carry += total;
-        }
-        __syncthreads();
+        block_scan_rounds<kSlabThreads>(S, [&](int i) { return tcnt[i]; }, [&](int i, unsigned ex, unsigned v) {
+            const unsigned run = cur[i];
+            tcnt[i] = ex;
+            off[i] = run - ex;
+            cur[i] = run + v;
+        });
 #pragma unroll
         for (int j = 0; j < kPer; ++j) {
             const int p = (int)threadIdx.x + j * kSlabThreads;
@@ -736,19 +692,14 @@ __global__ void __launch_bounds__(kSlabThreads) slab_sort_kernel(const __grid_co
         }
     }
     __syncthreads();
-    unsigned carry = 0, nonempty = 0;
-    for (int b = 0; b < ncell; b += kSlabThreads) {
-        const int i = b + threadIdx.x;
-        const unsigned v = i < ncell ? cnt[i] : 0u;
-        unsigned total;
-        const unsigned ex = carry + block_exclusive_scan(v, &total);
-        if (i < ncell) { cnt[i] = ex; c.cell_start[cell0 + i] = base + ex; }
+    unsigned nonempty = 0;
+    block_scan_rounds<kSlabThreads>(ncell, [&](int i) { return cnt[i]; }, [&](int i, unsigned ex, unsigned v) {
+        cnt[i] = ex;
+        c.cell_start[cell0 + i] = base + ex;
         nonempty += v != 0u;
-        carry += total;
-    }
+    });
     if (s == S - 1)
         for (int i = g.ncells + threadIdx.x; i <= c.cell_cap; i += kSlabThreads) c.cell_start[i] = (unsigned)c.n;
-    __syncthreads();
     if (staged) {
 #pragma unroll
         for (int j = 0; j < kPer; ++j) {
@@ -786,15 +737,14 @@ __global__ void __launch_bounds__(kSlabThreads) slab_sort_kernel(const __grid_co
 template <typename T, typename CS>
 __global__ void __launch_bounds__(kSmallThreads, 1) bin_small_kernel(const __grid_constant__ CS clouds) {
     grid_dependency_wait();
-    static_assert(kSmallThreads % 3 == 1 && kSmallThreads == 1024, "block_bbox / the scan below assume 32 warps");
+    static_assert(kSmallThreads % 3 == 1, "block_bbox relies on blockDim = 1 (mod 3)");
     extern __shared__ __align__(16) unsigned char small_smem[];
     unsigned* cnt = reinterpret_cast<unsigned*>(small_smem);
     const Cloud<T> c = clouds[blockIdx.x];
     __shared__ T box[6];
     __shared__ GridHeader<T> hdr;
-    __shared__ unsigned warp_tot[32];
     __shared__ unsigned s_nonempty;
-    const int t = threadIdx.x, lane = t & 31, w = t >> 5;
+    const int t = threadIdx.x, lane = t & 31;
     const int ncount = c.cell_cap + 1;
     if (t == 0) s_nonempty = 0u;
     for (int i = t; i < ncount; i += kSmallThreads) cnt[i] = 0u;
@@ -817,36 +767,13 @@ __global__ void __launch_bounds__(kSmallThreads, 1) bin_small_kernel(const __gri
             if (first + b * kSmallThreads < n) atomicAdd(&cnt[linear_cell<T>(g, p[b][0], p[b][1], p[b][2])], 1u);
     }
     __syncthreads();
-    // exclusive scan of the counters, kSmallThreads entries per round; the prefix goes to cell_start
-    // and stays in shared memory as the scatter cursors
-    unsigned carry = 0, nonempty = 0;
-    for (int base = 0; base < ncount; base += kSmallThreads) {
-        const int i = base + t;
-        const unsigned v = i < ncount ? cnt[i] : 0u;
-        unsigned inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += u;
-        }
-        if (lane == 31) warp_tot[w] = inc;
-        __syncthreads();
-        if (w == 0) {
-            unsigned s = warp_tot[lane];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned u = __shfl_up_sync(0xffffffffu, s, o);
-                if (lane >= o) s += u;
-            }
-            warp_tot[lane] = s;
-        }
-        __syncthreads();
-        const unsigned ex = carry + (w ? warp_tot[w - 1] : 0u) + inc - v;
-        if (i < ncount) { cnt[i] = ex; c.cell_start[i] = ex; }
-        carry += warp_tot[31];
+    // exclusive scan of the counters; the prefix goes to cell_start and stays in shared memory as the scatter cursors
+    unsigned nonempty = 0;
+    block_scan_rounds<kSmallThreads>(ncount, [&](int i) { return cnt[i]; }, [&](int i, unsigned ex, unsigned v) {
+        cnt[i] = ex;
+        c.cell_start[i] = ex;
         nonempty += v != 0u;
-        __syncthreads();
-    }
+    });
     if (c.hint_out != nullptr) {
         nonempty = __reduce_add_sync(0xffffffffu, nonempty);
         if (lane == 0 && nonempty != 0u) atomicAdd(&s_nonempty, nonempty);

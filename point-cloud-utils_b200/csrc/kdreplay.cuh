@@ -119,34 +119,6 @@ struct KdReplayBuffers {
 __global__ void widen_counter_kernel(const unsigned* src, long long* dst) { *dst = (long long)*src; }
 
 // ---- build -----------------------------------------------------------------------------------------
-__device__ __forceinline__ unsigned kd_block_exclusive_scan(unsigned v, unsigned* total) {
-    // kThreads threads; returns the exclusive prefix of v, *total = block sum
-    __shared__ unsigned warp_sum[kThreads / 32];
-    const int l = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned inc = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
-        if (l >= o) inc += u;
-    }
-    if (l == 31) warp_sum[w] = inc;
-    __syncthreads();
-    if (w == 0) {
-        unsigned s = l < kThreads / 32 ? warp_sum[l] : 0u;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned u = __shfl_up_sync(0xffffffffu, s, o);
-            if (l >= o) s += u;
-        }
-        if (l < kThreads / 32) warp_sum[l] = s;
-    }
-    __syncthreads();
-    const unsigned before = w ? warp_sum[w - 1] : 0u;
-    *total = warp_sum[kThreads / 32 - 1];
-    __syncthreads();
-    return before + inc - v;
-}
-
 // tight bounding box contribution of slot s to its node (atomics on the ordered integer image; a warp
 // whose lanes all sit in the same node reduces first).  Called by whole warps.
 template <typename T>
@@ -458,7 +430,7 @@ __device__ __forceinline__ void kd_scan_phase(cooperative_groups::grid_group& gr
         }
         if (kSweep == 1 && __syncthreads_or((int)eq) && threadIdx.x == 0) atomicOr(&b.counters->any_eq, 1);
         unsigned total;
-        unsigned run = kd_block_exclusive_scan(sum, &total);
+        unsigned run = block_exclusive_scan<kThreads>(sum, &total);
 #pragma unroll
         for (int k = 0; k < kKdItems; ++k) {
             if ((first + k) < count) b.prefix[first + k] = run;
@@ -479,7 +451,7 @@ __device__ __forceinline__ void kd_scan_phase(cooperative_groups::grid_group& gr
             sum += v[k];
         }
         unsigned total;
-        unsigned run = kd_block_exclusive_scan(sum, &total);
+        unsigned run = block_exclusive_scan<kThreads>(sum, &total);
 #pragma unroll
         for (int k = 0; k < kPer; ++k) {
             const int i = threadIdx.x * kPer + k;
@@ -495,7 +467,7 @@ __device__ __forceinline__ void kd_scan_phase(cooperative_groups::grid_group& gr
             const int i = base + threadIdx.x;
             const unsigned v = i < ntiles ? b.scan_partial[i] : 0u;
             unsigned total;
-            const unsigned ex = kd_block_exclusive_scan(v, &total);
+            const unsigned ex = block_exclusive_scan<kThreads>(v, &total);
             if (i < ntiles) b.scan_partial[i] = carry + ex;
             carry += total;
         }
@@ -520,7 +492,7 @@ __device__ __forceinline__ void kd_scan_subtree(const KdReplayBuffers<T>& b, con
         }
         if (kSweep == 1 && eq) *s_any_eq = 1;   // benign race: every writer stores 1
         unsigned total;
-        unsigned run = carry + kd_block_exclusive_scan(sum, &total);
+        unsigned run = carry + block_exclusive_scan<kThreads>(sum, &total);
 #pragma unroll
         for (int k = 0; k < kKdItems; ++k) {
             if ((at + k) < last) b.prefix[at + k] = run;

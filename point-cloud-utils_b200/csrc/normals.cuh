@@ -284,39 +284,10 @@ __global__ void __launch_bounds__(kThreads) keep_count_kernel(const unsigned cha
 }
 
 __global__ void __launch_bounds__(1024) keep_offsets_kernel(unsigned* __restrict__ block_count, long long nblocks, long long* __restrict__ out_count) {
-    __shared__ unsigned warp_sum[32];
-    __shared__ unsigned carry_s;
-    if (threadIdx.x == 0) carry_s = 0u;
-    __syncthreads();
-    for (long long base = 0; base < nblocks; base += 1024) {
-        const long long b = base + threadIdx.x;
-        const unsigned v = b < nblocks ? block_count[b] : 0u;
-        unsigned inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
-            if ((threadIdx.x & 31) >= o) inc += u;
-        }
-        if ((threadIdx.x & 31) == 31) warp_sum[threadIdx.x >> 5] = inc;
-        __syncthreads();
-        if (threadIdx.x < 32) {
-            unsigned s = warp_sum[threadIdx.x];
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const unsigned u = __shfl_up_sync(0xffffffffu, s, o);
-                if (threadIdx.x >= o) s += u;
-            }
-            warp_sum[threadIdx.x] = s;
-        }
-        __syncthreads();
-        const unsigned before = (threadIdx.x >> 5) ? warp_sum[(threadIdx.x >> 5) - 1] : 0u;
-        const unsigned carry = carry_s;
-        if (b < nblocks) block_count[b] = carry + before + inc - v;
-        __syncthreads();
-        if (threadIdx.x == 0) carry_s = carry + warp_sum[31];
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) *out_count = (long long)carry_s;
+    // nblocks = ceil(n / kThreads) with n < 2^31 rows: fits 32 bits
+    const unsigned kept = block_scan_rounds<1024>(
+        (unsigned)nblocks, [&](unsigned b) { return block_count[b]; }, [&](unsigned b, unsigned ex, unsigned) { block_count[b] = ex; });
+    if (threadIdx.x == 0) *out_count = (long long)kept;
 }
 
 template <typename T>

@@ -84,51 +84,29 @@ bool runs_this_build(int device) {
 
 // Launch with programmatic stream serialisation: the kernel (which starts with grid_dependency_wait())
 // may have its CTAs scheduled while its predecessor in the stream is still draining.
-#define PCU_LAUNCH_PDL(kernel, grid, block, stream, ...)                                       \
-    do {                                                                                       \
-        cudaLaunchConfig_t cfg__ = {};                                                         \
-        cfg__.gridDim = dim3(grid);                                                            \
-        cfg__.blockDim = dim3(block);                                                          \
-        cfg__.stream = stream;                                                                 \
-        cudaLaunchAttribute attr__[1];                                                         \
-        attr__[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                     \
-        attr__[0].val.programmaticStreamSerializationAllowed = 1;                              \
-        cfg__.attrs = attr__;                                                                  \
-        cfg__.numAttrs = 1;                                                                    \
-        PCU_CUDA(cudaLaunchKernelEx(&cfg__, kernel, __VA_ARGS__));                             \
-        g_launches.fetch_add(1, std::memory_order_relaxed);                                    \
-    } while (0)
-
-#define PCU_LAUNCH_PDL_SMEM(kernel, grid, block, smem, stream, ...)                            \
-    do {                                                                                       \
-        cudaLaunchConfig_t cfg__ = {};                                                         \
-        cfg__.gridDim = dim3(grid);                                                            \
-        cfg__.blockDim = dim3(block);                                                          \
-        cfg__.dynamicSmemBytes = (smem);                                                       \
-        cfg__.stream = stream;                                                                 \
-        cudaLaunchAttribute attr__[1];                                                         \
-        attr__[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;                     \
-        attr__[0].val.programmaticStreamSerializationAllowed = 1;                              \
-        cfg__.attrs = attr__;                                                                  \
-        cfg__.numAttrs = 1;                                                                    \
-        PCU_CUDA(cudaLaunchKernelEx(&cfg__, kernel, __VA_ARGS__));                             \
-        g_launches.fetch_add(1, std::memory_order_relaxed);                                    \
-    } while (0)
+template <typename... Params, typename... Args>
+int launch_pdl(void (*kernel)(Params...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, const Args&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    PCU_CUDA(cudaLaunchKernelEx(&cfg, kernel, args...));
+    g_launches.fetch_add(1, std::memory_order_relaxed);
+    return PCU_B200_OK;
+}
 
 // Descriptor-taking kernels exist in two flavours: descriptors by value in parameter space (single
-// pair: `plan.by_value`) or in a device array (batches).  K<T, CloudsX<T>[, SweepsX<T>][, extra...]>.
-#define PCU_LAUNCH_C(K, grid, block)                                                                      \
-    do {                                                                                                  \
-        if (plan.by_value) PCU_LAUNCH_PDL((K<T, CloudsVal<T>>), grid, block, stream, plan.cv);            \
-        else PCU_LAUNCH_PDL((K<T, CloudsPtr<T>>), grid, block, stream, plan.cp);                          \
-    } while (0)
-#define PCU_LAUNCH_CS(K, grid, block, ...)                                                                \
-    do {                                                                                                  \
-        if (plan.by_value)                                                                                \
-            PCU_LAUNCH_PDL((K<T, CloudsVal<T>, SweepsVal<T>, ##__VA_ARGS__>), grid, block, stream, plan.cv, plan.sv); \
-        else                                                                                              \
-            PCU_LAUNCH_PDL((K<T, CloudsPtr<T>, SweepsPtr<T>, ##__VA_ARGS__>), grid, block, stream, plan.cp, plan.sp); \
-    } while (0)
+// pair: `plan.by_value`) or in a device array (batches).  K<T, CloudsX<T>, SweepsX<T>[, extra...]>.
+#define PCU_LAUNCH_CS(K, grid, block, ...)                                                                                   \
+    PCU_TRY(plan.by_value                                                                                                    \
+                ? launch_pdl(K<T, CloudsVal<T>, SweepsVal<T>, ##__VA_ARGS__>, grid, block, 0, stream, plan.cv, plan.sv) \
+                : launch_pdl(K<T, CloudsPtr<T>, SweepsPtr<T>, ##__VA_ARGS__>, grid, block, 0, stream, plan.cp, plan.sp))
 
 // Per-field byte strides between consecutive pairs of a batch (side 0 = first cloud of each pair,
 // side 1 = second cloud; direction 0 = first -> second, direction 1 = second -> first).
@@ -216,8 +194,7 @@ struct pcu_b200_workspace {
     pcu_b200_options opts{};
     int sm_count = 132;                  // set from the device in pcu_b200_workspace_create
     // optional per-stage timing (bench.py's roofline pass): events recorded on the launching stream
-    unsigned small_attr = 0;             // bin_small_kernel instantiations whose shared-memory limit has been raised
-    unsigned slab_attr = 0;              // the same for the slab-build kernels
+    unsigned smem_raised = 0;            // kernel instantiations whose dynamic shared-memory limit has been raised (raise_smem_limit)
     // grid-sizing feedback: the kernels leave {cell_cap, non-empty cells, n, valid, unsettled queries, queries, valid, -}
     // per cloud in this
     // host-mapped buffer; the next call with the same shapes reads it (no synchronisation: a hint only)
@@ -617,25 +594,52 @@ int prepare_plan(pcu_b200_workspace* ws, Plan<T>& plan, PlanSpec<T>& spec, cudaS
     return PCU_B200_OK;
 }
 
-// The slab build's three launches for `clouds` (gridDim.y = ny), each followed by its stage mark.
-template <typename T, typename CS>
-int launch_slab_build(pcu_b200_workspace* ws, const Plan<T>& plan, const CS& clouds, unsigned ny, cudaStream_t stream) {
-    const unsigned bit = 1u << ((sizeof(T) == 8 ? 1 : 0) + (std::is_same<CS, CloudsVal<T>>::value ? 2 : 0));
-    if (!(ws->slab_attr & bit)) {
-        const int hist_most = (int)slab_hist_smem<T>(kMaxSlabs);
-        const int part_most = (int)std::max(slab_part_smem<T>(kMaxSlabs), slab_part_smem<T>(kSlabTile));
-        const int sort_most = kSlabStageBytes + kSlabMaxCells * (int)sizeof(unsigned);
-        PCU_CUDA(cudaFuncSetAttribute(slab_hist_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, hist_most));
-        PCU_CUDA(cudaFuncSetAttribute(slab_partition_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, part_most));
-        PCU_CUDA(cudaFuncSetAttribute(slab_sort_kernel<T, CS>, cudaFuncAttributeMaxDynamicSharedMemorySize, sort_most));
-        ws->slab_attr |= bit;
+// Kernels whose dynamic shared-memory limit is raised above the default, one group of four bits each in
+// pcu_b200_workspace::smem_raised.
+enum SmemKernel { kSmemBinSmall, kSmemSlabHist, kSmemSlabPartition, kSmemSlabSort };
+
+// Raises the dynamic shared-memory limit of `kernel` (kernel `which`, instantiated for Clouds<T>) to `bytes`, once per
+// workspace: bit 4 * which + 2 * (T is double) + (Clouds is CloudsVal) of ws->smem_raised records that it is done.
+template <template <typename> class Clouds, typename T>
+int raise_smem_limit(pcu_b200_workspace* ws, SmemKernel which, void (*kernel)(Clouds<T>), size_t bytes) {
+    const unsigned bit = 1u << (4 * which + (sizeof(T) == 8 ? 2 : 0) + (std::is_same<Clouds<T>, CloudsVal<T>>::value ? 1 : 0));
+    if (!(ws->smem_raised & bit)) {
+        PCU_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+        ws->smem_raised |= bit;
     }
-    const dim3 chunks((unsigned)plan.max_slab_chunks, ny), slabs((unsigned)plan.max_slabs, ny);
-    PCU_LAUNCH_PDL_SMEM((slab_hist_kernel<T, CS>), chunks, kSlabThreads, plan.slab_hist_smem, stream, clouds);
+    return PCU_B200_OK;
+}
+
+// bbox -> grid -> cell order of `clouds` (gridDim.y = ny) by the slab build or the cell-wise passes, each stage
+// followed by its mark.  Descriptors by value take the bounding box and the grid set-up in one launch
+// (bbox_partial_kernel's kSetup); descriptors in a device array (batches) set up their grids in a launch of its own.
+template <typename T, typename CS>
+int launch_grid_build(pcu_b200_workspace* ws, const Plan<T>& plan, const CS& clouds, unsigned ny, cudaStream_t stream) {
+    constexpr bool by_value = std::is_same<CS, CloudsVal<T>>::value;
+    PCU_TRY(launch_pdl(bbox_partial_kernel<T, CS, by_value>, dim3(plan.max_bbox_blocks, ny), kThreads, 0, stream, clouds));
+    if constexpr (!by_value) PCU_TRY(launch_pdl(grid_setup_kernel<T, CS>, dim3(1, ny), kThreads, 0, stream, clouds));
+    mark(ws, 2, stream);
+    if (plan.slab_build) {
+        const size_t part_most = std::max(slab_part_smem<T>(kMaxSlabs), slab_part_smem<T>(kSlabTile));
+        PCU_TRY(raise_smem_limit(ws, kSmemSlabHist, slab_hist_kernel<T, CS>, slab_hist_smem<T>(kMaxSlabs)));
+        PCU_TRY(raise_smem_limit(ws, kSmemSlabPartition, slab_partition_kernel<T, CS>, part_most));
+        PCU_TRY(raise_smem_limit(ws, kSmemSlabSort, slab_sort_kernel<T, CS>, (size_t)kSlabStageBytes + kSlabMaxCells * sizeof(unsigned)));
+        const dim3 chunks((unsigned)plan.max_slab_chunks, ny), slabs((unsigned)plan.max_slabs, ny);
+        PCU_TRY(launch_pdl(slab_hist_kernel<T, CS>, chunks, kSlabThreads, plan.slab_hist_smem, stream, clouds));
+        mark(ws, 3, stream);
+        PCU_TRY(launch_pdl(slab_partition_kernel<T, CS>, chunks, kSlabThreads, plan.slab_part_smem, stream, clouds));
+        mark(ws, 4, stream);
+        PCU_TRY(launch_pdl(slab_sort_kernel<T, CS>, slabs, kSlabThreads, plan.slab_sort_smem, stream, clouds));
+        mark(ws, 5, stream);
+        return PCU_B200_OK;
+    }
+    const unsigned bin_blocks = (unsigned)((plan.max_n + kThreads - 1) / kThreads);
+    const unsigned scan_blocks = (unsigned)(((long long)plan.max_cap + 1 + kScanTile - 1) / kScanTile);
+    PCU_TRY(launch_pdl(cell_count_kernel<T, CS>, dim3(bin_blocks, ny), kThreads, 0, stream, clouds));
     mark(ws, 3, stream);
-    PCU_LAUNCH_PDL_SMEM((slab_partition_kernel<T, CS>), chunks, kSlabThreads, plan.slab_part_smem, stream, clouds);
+    PCU_TRY(launch_pdl(scan_lookback_kernel<T, CS>, dim3(scan_blocks, ny), kScanThreads, 0, stream, clouds));
     mark(ws, 4, stream);
-    PCU_LAUNCH_PDL_SMEM((slab_sort_kernel<T, CS>), slabs, kSlabThreads, plan.slab_sort_smem, stream, clouds);
+    PCU_TRY(launch_pdl(scatter_kernel<T, CS>, dim3(bin_blocks, ny), kThreads, 0, stream, clouds));
     mark(ws, 5, stream);
     return PCU_B200_OK;
 }
@@ -650,77 +654,44 @@ int launch_slab_build(pcu_b200_workspace* ws, const Plan<T>& plan, const CS& clo
 template <typename T>
 int enqueue_binning(pcu_b200_workspace* ws, const Plan<T>& plan, cudaStream_t stream, const cudaEvent_t* ready = nullptr,
                     bool first_only = false, const std::function<int()>* between = nullptr) {
-    const int nclouds = plan.nclouds;
-    // the slab build writes every cell_start entry: only the counters after the cell counters need zeroing
-    const size_t zero_skip = plan.slab_build ? plan.zero_cells_bytes : 0;
-    if ((ready != nullptr || first_only) && plan.by_value && !plan.one_cta_binning) {
-        PCU_CUDA(cudaMemsetAsync(plan.zero_begin + zero_skip, 0, plan.zero_bytes - zero_skip, stream));
-        const unsigned scan_blocks = (unsigned)(((long long)plan.max_cap + 1 + kScanTile - 1) / kScanTile);
-        const unsigned bin_blocks = (unsigned)((plan.max_n + kThreads - 1) / kThreads);
-        for (int s = 0; s < (first_only ? 1 : 2); ++s) {   // first_only: the second cloud is a prepared one
-            if (s == 1 && between != nullptr) PCU_TRY((*between)());
-            if (ready != nullptr) PCU_CUDA(cudaStreamWaitEvent(stream, ready[s], 0));
-            CloudsVal<T> one;
-            one.v[0] = plan.cv.v[s];
-            one.v[1] = plan.cv.v[s];
-            PCU_LAUNCH_PDL((bbox_partial_kernel<T, CloudsVal<T>, true>), dim3(plan.max_bbox_blocks, 1), kThreads, stream, one);
-            mark(ws, 2, stream);
-            if (plan.slab_build) {
-                PCU_TRY(launch_slab_build<T>(ws, plan, one, 1, stream));
-                continue;
-            }
-            PCU_LAUNCH_PDL((cell_count_kernel<T, CloudsVal<T>>), dim3(bin_blocks, 1), kThreads, stream, one);
-            mark(ws, 3, stream);
-            PCU_LAUNCH_PDL((scan_lookback_kernel<T, CloudsVal<T>>), dim3(scan_blocks, 1), kScanThreads, stream, one);
-            mark(ws, 4, stream);
-            PCU_LAUNCH_PDL((scatter_kernel<T, CloudsVal<T>>), dim3(bin_blocks, 1), kThreads, stream, one);
-            mark(ws, 5, stream);
+    // one cloud after the other (single pairs whose clouds arrive one by one, or whose second cloud is prepared)
+    const bool per_cloud = (ready != nullptr || first_only) && plan.by_value && !plan.one_cta_binning;
+    if (!per_cloud) {
+        if (between != nullptr) PCU_TRY((*between)());   // the other build paths take both clouds at once
+        if (ready != nullptr) {
+            PCU_CUDA(cudaStreamWaitEvent(stream, ready[0], 0));
+            if (!first_only) PCU_CUDA(cudaStreamWaitEvent(stream, ready[1], 0));
         }
-        if (first_only && between != nullptr) PCU_TRY((*between)());
-        return PCU_B200_OK;
     }
-    if (between != nullptr) PCU_TRY((*between)());   // the other build paths take both clouds at once
-    if (ready != nullptr) {
-        PCU_CUDA(cudaStreamWaitEvent(stream, ready[0], 0));
-        if (!first_only) PCU_CUDA(cudaStreamWaitEvent(stream, ready[1], 0));
-    }
+    // the cell-wise passes count into cell_start; the other builds write every entry of it and need only the
+    // counters after it zeroed
+    const size_t zero_skip = plan.slab_build || plan.one_cta_binning ? plan.zero_cells_bytes : 0;
+    PCU_CUDA(cudaMemsetAsync(plan.zero_begin + zero_skip, 0, plan.zero_bytes - zero_skip, stream));
     if (plan.one_cta_binning) {
-        PCU_CUDA(cudaMemsetAsync(plan.zero_begin + plan.zero_cells_bytes, 0, plan.zero_bytes - plan.zero_cells_bytes, stream));
-        const size_t smem = ((size_t)plan.max_cap + 1) * sizeof(unsigned);
-        const unsigned bit = 1u << ((sizeof(T) == 8 ? 2 : 0) + (plan.by_value ? 1 : 0));
-        if (!(ws->small_attr & bit)) {
-            const size_t most = (size_t)kSmallMaxCells * sizeof(unsigned);
-            if (plan.by_value)
-                PCU_CUDA(cudaFuncSetAttribute(bin_small_kernel<T, CloudsVal<T>>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)most));
-            else
-                PCU_CUDA(cudaFuncSetAttribute(bin_small_kernel<T, CloudsPtr<T>>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)most));
-            ws->small_attr |= bit;
+        const size_t smem = ((size_t)plan.max_cap + 1) * sizeof(unsigned), most = (size_t)kSmallMaxCells * sizeof(unsigned);
+        if (plan.by_value) {
+            PCU_TRY(raise_smem_limit(ws, kSmemBinSmall, bin_small_kernel<T, CloudsVal<T>>, most));
+            PCU_TRY(launch_pdl(bin_small_kernel<T, CloudsVal<T>>, dim3(plan.nclouds), kSmallThreads, smem, stream, plan.cv));
+        } else {
+            PCU_TRY(raise_smem_limit(ws, kSmemBinSmall, bin_small_kernel<T, CloudsPtr<T>>, most));
+            PCU_TRY(launch_pdl(bin_small_kernel<T, CloudsPtr<T>>, dim3(plan.nclouds), kSmallThreads, smem, stream, plan.cp));
         }
-        if (plan.by_value) PCU_LAUNCH_PDL_SMEM((bin_small_kernel<T, CloudsVal<T>>), dim3(nclouds), kSmallThreads, smem, stream, plan.cv);
-        else PCU_LAUNCH_PDL_SMEM((bin_small_kernel<T, CloudsPtr<T>>), dim3(nclouds), kSmallThreads, smem, stream, plan.cp);
         for (int stage = 2; stage <= 5; ++stage) mark(ws, stage, stream);   // the whole build shows up as "bbox+grid"
         return PCU_B200_OK;
     }
-    PCU_CUDA(cudaMemsetAsync(plan.zero_begin + zero_skip, 0, plan.zero_bytes - zero_skip, stream));
-    const unsigned scan_blocks = (unsigned)(((long long)plan.max_cap + 1 + kScanTile - 1) / kScanTile);
-    if (plan.by_value) {
-        PCU_LAUNCH_PDL((bbox_partial_kernel<T, CloudsVal<T>, true>), dim3(plan.max_bbox_blocks, nclouds), kThreads, stream, plan.cv);
-    } else {
-        PCU_LAUNCH_PDL((bbox_partial_kernel<T, CloudsPtr<T>, false>), dim3(plan.max_bbox_blocks, nclouds), kThreads, stream, plan.cp);
-        PCU_LAUNCH_PDL((grid_setup_kernel<T, CloudsPtr<T>>), dim3(1, nclouds), kThreads, stream, plan.cp);
+    if (!per_cloud) {
+        const unsigned ny = (unsigned)plan.nclouds;
+        return plan.by_value ? launch_grid_build(ws, plan, plan.cv, ny, stream) : launch_grid_build(ws, plan, plan.cp, ny, stream);
     }
-    mark(ws, 2, stream);
-    if (plan.slab_build) {
-        if (plan.by_value) return launch_slab_build<T>(ws, plan, plan.cv, (unsigned)nclouds, stream);
-        return launch_slab_build<T>(ws, plan, plan.cp, (unsigned)nclouds, stream);
+    for (int s = 0; s < (first_only ? 1 : 2); ++s) {   // first_only: the second cloud is a prepared one
+        if (s == 1 && between != nullptr) PCU_TRY((*between)());
+        if (ready != nullptr) PCU_CUDA(cudaStreamWaitEvent(stream, ready[s], 0));
+        CloudsVal<T> one;
+        one.v[0] = plan.cv.v[s];
+        one.v[1] = plan.cv.v[s];
+        PCU_TRY(launch_grid_build(ws, plan, one, 1, stream));
     }
-    const unsigned bin_blocks = (unsigned)((plan.max_n + kThreads - 1) / kThreads);
-    PCU_LAUNCH_C(cell_count_kernel, dim3(bin_blocks, nclouds), kThreads);
-    mark(ws, 3, stream);
-    PCU_LAUNCH_C(scan_lookback_kernel, dim3(scan_blocks, nclouds), kScanThreads);
-    mark(ws, 4, stream);
-    PCU_LAUNCH_C(scatter_kernel, dim3(bin_blocks, nclouds), kThreads);
-    mark(ws, 5, stream);
+    if (first_only && between != nullptr) PCU_TRY((*between)());
     return PCU_B200_OK;
 }
 
@@ -922,6 +893,22 @@ int normals_knn_device(pcu_b200_workspace* ws, const T* points, long long n, con
     return PCU_B200_OK;
 }
 
+// The plan, carved from the arena, of a call that bins one cloud into cells no finer than `min_cell`.
+template <typename T>
+int single_cloud_plan(pcu_b200_workspace* ws, const T* points, long long n, double min_cell, Plan<T>& plan, cudaStream_t stream) {
+    PlanSpec<T> spec;
+    spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
+    spec.nsweeps = 1; spec.k = 1;
+    spec.occupancy = 0.125f;          // the cell budget; the cell size itself is held up by min_cell below
+    spec.prepared_second = true;      // the one-point second cloud is a dummy: only the first is binned
+    plan.layout(nullptr, spec);
+    PCU_TRY(ensure_arena(ws, plan.total, stream));
+    plan.layout(ws->arena, spec);
+    plan.cv.v[0].min_cell = (float)std::min(1e30, min_cell);
+    plan.cv.v[0].hint_out = nullptr;
+    return PCU_B200_OK;
+}
+
 // ---- normals from all points in a ball (SURVEY.md 8f N1, the radius variant) ---------------------------
 // The cloud is binned once (cells no finer than half the reach of the search, at most 8 per point), one thread per
 // point walks the cells its ball touches; the compaction is the k-NN variant's.
@@ -942,19 +929,9 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
     PCU_TRY(check_cloud_args<T>(points, n, points, 1));
     if (!out_idx || !out_normals || !out_count) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    PlanSpec<T> spec;
-    spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
-    spec.nsweeps = 1; spec.k = 1;
-    spec.occupancy = 0.125f;          // the cell budget; the cell size itself is held up by min_cell below
-    spec.prepared_second = true;      // the one-point second cloud is a dummy: only the first is binned
-    Plan<T> plan;
-    plan.layout(nullptr, spec);
-    PCU_TRY(adopt_stream(ws, stream));
-    PCU_TRY(ensure_arena(ws, plan.total, stream));
-    plan.layout(ws->arena, spec);
     const double reach = std::sqrt((double)(T)o->radius);     // the search radius is a squared distance (normals.cuh)
-    plan.cv.v[0].min_cell = (float)std::min(1e30, 0.5 * reach);
-    plan.cv.v[0].hint_out = nullptr;
+    Plan<T> plan;
+    PCU_TRY(single_cloud_plan<T>(ws, points, n, 0.5 * reach, plan, stream));
     const long long nblocks = (n + kThreads - 1) / kThreads;
     Carver measure(nullptr);
     auto carve = [&](Carver& cv, T*& dense, unsigned char*& keep, unsigned*& counts) {
@@ -1021,18 +998,8 @@ int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, do
     PCU_ON_DEVICE(ws);
     const T r = (T)radius;        // blue_noise_downsample takes the radius as the cloud's scalar (:299, :328)
     const T rr = r * r;           // `const double rr = r*r;` with r of that type: the product is rounded in T (:72)
-    PlanSpec<T> spec;
-    spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
-    spec.nsweeps = 1; spec.k = 1;
-    spec.occupancy = 0.125f;          // the cell budget; the cell size itself is held up by min_cell below
-    spec.prepared_second = true;      // the one-point second cloud is a dummy: only the first is binned
     Plan<T> plan;
-    plan.layout(nullptr, spec);
-    PCU_TRY(adopt_stream(ws, stream));
-    PCU_TRY(ensure_arena(ws, plan.total, stream));
-    plan.layout(ws->arena, spec);
-    plan.cv.v[0].min_cell = (float)std::min(1e30, 0.5 * (double)r);
-    plan.cv.v[0].hint_out = nullptr;
+    PCU_TRY(single_cloud_plan<T>(ws, points, n, 0.5 * (double)r, plan, stream));
     unsigned blocks = 1;
     PCU_TRY(poisson_grid_blocks<T>(ws->device, ws->sm_count, n, &blocks));
     const long long nblocks = (n + kThreads - 1) / kThreads;

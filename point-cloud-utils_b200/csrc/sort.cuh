@@ -75,35 +75,13 @@ __global__ void __launch_bounds__(kSortThreads) sort_hist_kernel(const Rec* __re
     hist[(size_t)threadIdx.x * ntiles + blockIdx.x] = h[threadIdx.x];
 }
 
-// grid 256: CTA b turns hist[b][0 .. ntiles) into its exclusive prefix sums and writes the row total
+// grid 256: CTA b turns hist[b][0 .. ntiles) into its exclusive prefix sums and writes the row total.  A row counts
+// records, at most n < 2^31, so prefixes and total fit 32 bits.
 __global__ void __launch_bounds__(kSortThreads) sort_scan_rows(unsigned* __restrict__ hist, unsigned ntiles, unsigned long long* __restrict__ total) {
-    __shared__ unsigned warp_sum[kSortWarps];
-    __shared__ unsigned long long carry_s;
     unsigned* row = hist + (size_t)blockIdx.x * ntiles;
-    if (threadIdx.x == 0) carry_s = 0ull;
-    __syncthreads();
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    for (unsigned base = 0; base < ntiles; base += kSortThreads) {
-        const unsigned i = base + threadIdx.x;
-        const unsigned v = i < ntiles ? row[i] : 0u;
-        unsigned inc = v;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
-            if (lane >= o) inc += u;
-        }
-        if (lane == 31) warp_sum[w] = inc;
-        __syncthreads();
-        unsigned before = 0u, all = 0u;
-#pragma unroll
-        for (int j = 0; j < kSortWarps; ++j) { const unsigned s = warp_sum[j]; if (j < w) before += s; all += s; }
-        const unsigned long long carry = carry_s;
-        if (i < ntiles) row[i] = (unsigned)(carry + before + inc - v);   // positions fit 32 bits (n < 2^31)
-        __syncthreads();
-        if (threadIdx.x == 0) carry_s = carry + all;
-        __syncthreads();
-    }
-    if (threadIdx.x == 0) total[blockIdx.x] = carry_s;
+    const unsigned all = block_scan_rounds<kSortThreads>(
+        ntiles, [&](unsigned i) { return row[i]; }, [&](unsigned i, unsigned ex, unsigned) { row[i] = ex; });
+    if (threadIdx.x == 0) total[blockIdx.x] = all;
 }
 
 // one CTA of 256 threads: base[bin] = records with a smaller digit; *constant = 1 when one bin holds everything

@@ -83,6 +83,9 @@ def test_sort_sizes_and_patterns(pcu, oracle):
     big = (rng.random((300000, 3)) * 1e6).astype(np.float64)                 # wide exponent range: every digit pass is live
     for g, r in zip(pcu.deduplicate_point_cloud(big, 0.0), oracle.deduplicate_point_cloud(big, 0.0)):
         assert np.array_equal(g, r)
+    many = np.round(rng.random((1100000, 3)) * 200).astype(np.float32)      # 269 tiles: the scan over a digit's tile counts takes two rounds
+    for g, r in zip(pcu.deduplicate_point_cloud(many, 0.0), oracle.deduplicate_point_cloud(many, 0.0)):
+        assert np.array_equal(g, r)
     x, i, j = pcu.deduplicate_point_cloud(np.zeros((0, 3), dtype=np.float32), 0.1)
     assert x.shape == (0, 3) and i.shape == (0,) and j.shape == (0,)
 
