@@ -333,6 +333,57 @@ int pcu_b200_poisson_disk_f32(pcu_b200_workspace* ws, const float* points, int64
 int pcu_b200_poisson_disk_f64(pcu_b200_workspace* ws, const double* points, int64_t n, double radius, uint32_t seed,
                               int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream);
 
+/* ---- mesh sampling and barycentric interpolation ----------------------------------------------
+ * Replaces sample_mesh_random / sample_mesh_poisson_disk (src/sample_mesh.cpp) and interpolate_barycentric_coords
+ * (point_cloud_utils/__init__.py:203-217).  The reference draws with std::rand and libigl; the samples here are pure
+ * functions of (v, f, seed), defined in DESIGN.md §3 and csrc/meshsample.cuh:
+ *   face weights  A_f = |(b - a) x (c - a)| in fp64, every operation rounded on its own; 0 when not finite or when a
+ *                 corner is outside [0, nv) (such faces are counted in bad_faces);  scale S = 2^(62 - ceil(log2 nf)) / max A
+ *                 (0 when max A = 0);  w_f = floor(A_f * S) (uint64);  C = inclusive prefix sum of w;  W = C[nf - 1].
+ *   sample s      h(j) = mix64(mix64(3 s + j) ^ seed), mix64 = splitmix64 with its +0x9E3779B97F4A7C15 step;
+ *                 face = first f with C_f > mulhi64(h(0), W);  u1, u2 = (h(1) >> 11) 2^-53, (h(2) >> 11) 2^-53;
+ *                 a = sqrt(u1);  bc = (1 - a, a (1 - u2), a u2) in fp64, rounded once to the vertices' type.
+ * Faces are (nf, 3) integers of the kind f_kind; every pointer is a DEVICE pointer and every call is stream-ordered. */
+enum pcu_b200_index_kind { PCU_B200_INDEX_I32 = 0, PCU_B200_INDEX_I64 = 1, PCU_B200_INDEX_U32 = 2, PCU_B200_INDEX_U64 = 3 };
+typedef struct pcu_b200_mesh_area {
+    uint64_t total_weight;   /* W; 0: the mesh has zero area.  The total area is total_weight / scale / 2. */
+    double scale;            /* S */
+    uint64_t bad_faces;      /* faces with a corner outside [0, nv): weight 0 (the reference reads out of bounds) */
+} pcu_b200_mesh_area;
+/* Writes {W, S, bad_faces} to *out_area (device, 24 bytes). */
+int pcu_b200_mesh_area_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                           pcu_b200_mesh_area* out_area, void* stream);
+int pcu_b200_mesh_area_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                           pcu_b200_mesh_area* out_area, void* stream);
+/* Samples 0 .. num_samples - 1: out_fidx (num_samples, f's width: 4 bytes for I32 / U32, 8 for I64 / U64), out_bc
+ * (num_samples, 3).  out_area (may be NULL) receives {W, S, bad_faces}; when W == 0 the outputs are not written. */
+int pcu_b200_sample_mesh_random_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                    int64_t num_samples, uint32_t seed, void* out_fidx, float* out_bc, pcu_b200_mesh_area* out_area,
+                                    void* stream);
+int pcu_b200_sample_mesh_random_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                    int64_t num_samples, uint32_t seed, void* out_fidx, double* out_bc, pcu_b200_mesh_area* out_area,
+                                    void* stream);
+/* Draws the samples 0 .. n_dense - 1, positions p_s = fl((bc0 a + bc1 b) + bc2 c) per axis in fp64 from the unrounded
+ * coordinates, selects among them with pcu_b200_poisson_disk_* at (radius, seed), and writes the kept samples' faces
+ * and coordinates in ascending sample order: out_fidx / out_bc (capacity n_dense), out_count (device int64).
+ * radius > 0, 1 <= n_dense <= 2^31 - 1; the caller derives both from {W, S} (pcu_b200_mesh_area_*). */
+int pcu_b200_sample_mesh_poisson_disk_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                          double radius, int64_t n_dense, uint32_t seed, void* out_fidx, float* out_bc,
+                                          int64_t* out_count, void* stream);
+int pcu_b200_sample_mesh_poisson_disk_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                          double radius, int64_t n_dense, uint32_t seed, void* out_fidx, double* out_bc,
+                                          int64_t* out_count, void* stream);
+/* out[i, d] = ((x0 b0 + x1 b1) + x2 b2), x_k = attribute[f[fi[i], k], d], products and sums in the output type with
+ * no FMA (numpy's (attribute[f[fi]] * bc[:, :, None]).sum(1) bit for bit).  Negative indices of signed kinds wrap as
+ * in numpy; a row with an index out of range is never loaded: it is NaN and counted in *out_bad (device uint64).
+ * _f32: bc and attribute float32; _f64: each float32 or float64. */
+int pcu_b200_interpolate_barycentric_f32(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, const void* fi, int64_t n,
+                                         int fi_kind, const float* bc, const float* attribute, int64_t nv, int64_t dim, float* out,
+                                         uint64_t* out_bad, void* stream);
+int pcu_b200_interpolate_barycentric_f64(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, const void* fi, int64_t n,
+                                         int fi_kind, const void* bc, int bc_is_f64, const void* attribute, int attribute_is_f64,
+                                         int64_t nv, int64_t dim, double* out, uint64_t* out_bad, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

@@ -546,6 +546,72 @@ void poisson_disk_device(bool is_f64, uintptr_t points, int64_t n, double radius
     check(status);
 }
 
+// Mesh sampling (sample_mesh_random / sample_mesh_poisson_disk, _mesh_sampling.py).  f_kind: 0 int32, 1 int64,
+// 2 uint32, 3 uint64; out_area: 3 device words {W, S, faces with a corner out of range}.
+void mesh_area_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out_area, int device,
+                      uintptr_t stream) {
+    Slot& slot = pool().get(device, stream);
+    int status;
+    {
+        CallScope scope(slot);
+        status = is_f64 ? pcu_b200_mesh_area_f64(slot.ws, (const double*)v, nv, (const void*)f, nf, f_kind,
+                                                 (pcu_b200_mesh_area*)out_area, (void*)stream)
+                        : pcu_b200_mesh_area_f32(slot.ws, (const float*)v, nv, (const void*)f, nf, f_kind,
+                                                 (pcu_b200_mesh_area*)out_area, (void*)stream);
+    }
+    check(status);
+}
+
+void sample_mesh_random_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int64_t num_samples,
+                               uint32_t seed, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_area, int device, uintptr_t stream) {
+    Slot& slot = pool().get(device, stream);
+    int status;
+    {
+        CallScope scope(slot);
+        status = is_f64 ? pcu_b200_sample_mesh_random_f64(slot.ws, (const double*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
+                                                          (void*)out_fidx, (double*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream)
+                        : pcu_b200_sample_mesh_random_f32(slot.ws, (const float*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
+                                                          (void*)out_fidx, (float*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream);
+    }
+    check(status);
+}
+
+void sample_mesh_poisson_disk_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, double radius,
+                                     int64_t n_dense, uint32_t seed, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_count,
+                                     int device, uintptr_t stream) {
+    Slot& slot = pool().get(device, stream);
+    int status;
+    {
+        CallScope scope(slot);
+        status = is_f64 ? pcu_b200_sample_mesh_poisson_disk_f64(slot.ws, (const double*)v, nv, (const void*)f, nf, f_kind, radius,
+                                                                n_dense, seed, (void*)out_fidx, (double*)out_bc, (int64_t*)out_count,
+                                                                (void*)stream)
+                        : pcu_b200_sample_mesh_poisson_disk_f32(slot.ws, (const float*)v, nv, (const void*)f, nf, f_kind, radius,
+                                                                n_dense, seed, (void*)out_fidx, (float*)out_bc, (int64_t*)out_count,
+                                                                (void*)stream);
+    }
+    check(status);
+}
+
+// out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
+void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
+                                    bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
+                                    uintptr_t out_bad, int device, uintptr_t stream) {
+    Slot& slot = pool().get(device, stream);
+    int status;
+    {
+        CallScope scope(slot);
+        status = (bc_f64 || attr_f64)
+                     ? pcu_b200_interpolate_barycentric_f64(slot.ws, (const void*)f, nf, f_kind, (const void*)fi, n, fi_kind,
+                                                            (const void*)bc, bc_f64, (const void*)attr, attr_f64, nv, dim,
+                                                            (double*)out, (uint64_t*)out_bad, (void*)stream)
+                     : pcu_b200_interpolate_barycentric_f32(slot.ws, (const void*)f, nf, f_kind, (const void*)fi, n, fi_kind,
+                                                            (const float*)bc, (const float*)attr, nv, dim, (float*)out,
+                                                            (uint64_t*)out_bad, (void*)stream);
+    }
+    check(status);
+}
+
 // ---- Morton codes (src/morton.cpp) ----------------------------------------------------------------
 // dtype rules of the bindings: pts int32 / int64; codes uint32 / uint64 (uint32 codes are widened, as the
 // reference's MortonCode64(uint64_t) constructor does implicitly); results are uint64 / int32 / int64 like the reference's.
@@ -1007,6 +1073,10 @@ PYBIND11_MODULE(_pcu_internal, mod) {
             "Indices of the kept points and their unit normals (plane fit to the points in a ball around each point).");
     mod.def("_normals_ball_device", &normals_ball_device);
     mod.def("_poisson_disk_device", &poisson_disk_device);
+    mod.def("_mesh_area_device", &mesh_area_device);
+    mod.def("_sample_mesh_random_device", &sample_mesh_random_device);
+    mod.def("_sample_mesh_poisson_disk_device", &sample_mesh_poisson_disk_device);
+    mod.def("_interpolate_barycentric_device", &interpolate_barycentric_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),

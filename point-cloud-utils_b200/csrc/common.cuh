@@ -124,33 +124,43 @@ __device__ __forceinline__ unsigned mix32(unsigned h) {
     return h;
 }
 
+// splitmix64 (its +0x9E3779B97F4A7C15 step, then its finaliser; a bijection, mix64(0) = 0xE220A8397B1DCDAF): the
+// counter-based hash behind the mesh samples' faces and barycentric coordinates.
+__device__ __forceinline__ unsigned long long mix64(unsigned long long x) {
+    x += 0x9e3779b97f4a7c15ull;
+    x = (x ^ (x >> 30)) * 0xbf58476d1ce4e5b9ull;
+    x = (x ^ (x >> 27)) * 0x94d049bb133111ebull;
+    return x ^ (x >> 31);
+}
+
 // Block-wide exclusive scan, kBlock threads: returns the exclusive prefix of v and sets *total to the block sum in
-// every thread.  Ends with a barrier, so it may be called again right away (in a loop, on the same warp_sum).
-template <int kBlock>
-__device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned* total) {
+// every thread.  Ends with a barrier, so it may be called again right away (in a loop, on the same warp_sum).  V is
+// the value type: 32-bit counts almost everywhere, 64-bit for the mesh samplers' face weights.
+template <int kBlock, class V = unsigned>
+__device__ __forceinline__ V block_exclusive_scan(V v, V* total) {
     static_assert(kBlock % 32 == 0 && kBlock <= 1024, "whole warps, at most 32 of them");
     constexpr int kWarps = kBlock / 32;
-    __shared__ unsigned warp_sum[kWarps];
+    __shared__ V warp_sum[kWarps];
     const int l = threadIdx.x & 31, w = threadIdx.x >> 5;
-    unsigned inc = v;
+    V inc = v;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
-        const unsigned u = __shfl_up_sync(0xffffffffu, inc, o);
+        const V u = __shfl_up_sync(0xffffffffu, inc, o);
         if (l >= o) inc += u;
     }
     if (l == 31) warp_sum[w] = inc;
     __syncthreads();
     if (w == 0) {
-        unsigned s = l < kWarps ? warp_sum[l] : 0u;
+        V s = l < kWarps ? warp_sum[l] : (V)0;
 #pragma unroll
         for (int o = 1; o < kWarps; o <<= 1) {
-            const unsigned u = __shfl_up_sync(0xffffffffu, s, o);
+            const V u = __shfl_up_sync(0xffffffffu, s, o);
             if (l >= o) s += u;
         }
         if (l < kWarps) warp_sum[l] = s;   // inclusive over warps
     }
     __syncthreads();
-    const unsigned before = w ? warp_sum[w - 1] : 0u;
+    const V before = w ? warp_sum[w - 1] : (V)0;
     *total = warp_sum[kWarps - 1];
     __syncthreads();
     return before + inc - v;
@@ -161,15 +171,15 @@ __device__ __forceinline__ unsigned block_exclusive_scan(unsigned v, unsigned* t
 // prefix.  Returns the sum of all values to every thread.  Block-wide; ends with a barrier, so the stores are visible
 // to the whole block on return.  The rounds are counted in the index type `I` of `count`: nvcc unrolls the loop over a
 // signed count (the slab build's per-tile scan needs that) and keeps the one over an unsigned count rolled (fewer
-// registers where the scan is the whole kernel).
-template <int kBlock, class I, class Load, class Store>
-__device__ __forceinline__ unsigned block_scan_rounds(I count, Load load, Store store) {
-    unsigned carry = 0;
+// registers where the scan is the whole kernel).  V is the value type, as for block_exclusive_scan.
+template <int kBlock, class V = unsigned, class I, class Load, class Store>
+__device__ __forceinline__ V block_scan_rounds(I count, Load load, Store store) {
+    V carry = 0;
     for (I b = 0; b < count; b += kBlock) {
         const I i = b + (I)threadIdx.x;
-        const unsigned v = i < count ? load(i) : 0u;
-        unsigned total;
-        const unsigned ex = carry + block_exclusive_scan<kBlock>(v, &total);
+        const V v = i < count ? (V)load(i) : (V)0;
+        V total;
+        const V ex = carry + block_exclusive_scan<kBlock, V>(v, &total);
         if (i < count) store(i, ex, v);
         carry += total;
     }

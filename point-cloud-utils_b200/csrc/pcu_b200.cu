@@ -32,6 +32,7 @@
 #include "voxel.cuh"
 #include "dedup.cuh"
 #include "poisson.cuh"
+#include "meshsample.cuh"
 
 using namespace pcu;
 
@@ -191,6 +192,8 @@ struct pcu_b200_workspace {
     size_t io_bytes = 0;
     unsigned char* aux = nullptr;        // intermediate results that outlive a nested call's re-carving of the arena (normals)
     size_t aux_bytes = 0;
+    unsigned char* mesh = nullptr;       // the face CDF and dense samples of mesh Poisson-disk sampling, which outlive the
+    size_t mesh_bytes = 0;               // point-cloud Poisson-disk call it makes (that one re-carves the arena and aux)
     pcu_b200_options opts{};
     int sm_count = 132;                  // set from the device in pcu_b200_workspace_create
     // optional per-stage timing (bench.py's roofline pass): events recorded on the launching stream
@@ -1035,6 +1038,161 @@ int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, do
     return PCU_B200_OK;
 }
 
+// ---- mesh sampling and barycentric interpolation (sample_mesh_random / sample_mesh_poisson_disk) -----------------
+int mesh_check(const void* v, long long nv, const void* f, long long m, int fkind) {
+    if (!v || !f || nv <= 0 || m <= 0)
+        return fail(PCU_B200_INVALID_ARGUMENT, "Invalid input mesh with zero elements: v and f must have shape (n, 3) and (m, 3) (n, m > 0)");
+    if (m > 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "mesh sampling: at most 2^31 - 1 faces, got %lld", m);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    return PCU_B200_OK;
+}
+
+inline long long mesh_tiles(long long m) { return (m + kMeshScanTile - 1) / kMeshScanTile; }
+
+// The face CDF of meshsample.cuh: areas, then the three-launch scan.  `cdf` (m words), `tiles` (one word per scan
+// tile) and `sc` are carved by the caller; {W, S, bad} land in *out.
+template <typename T>
+int enqueue_mesh_cdf(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, int fkind, long long m,
+                     unsigned long long* cdf, unsigned long long* tiles, MeshScratch* sc, MeshArea* out, cudaStream_t stream) {
+    PCU_CUDA(cudaMemsetAsync(sc, 0, sizeof(MeshScratch), stream));
+    const unsigned blocks = (unsigned)std::min<long long>((m + kThreads - 1) / kThreads, (long long)ws->sm_count * 8);
+    PCU_LAUNCH((mesh_area_kernel<T>), blocks, kThreads, stream, v, nv, f, fkind, m, cdf, sc);
+    PCU_LAUNCH(mesh_cdf_reduce_kernel, (unsigned)mesh_tiles(m), kMeshScanThreads, stream, (const unsigned long long*)cdf, m,
+               (const MeshScratch*)sc, tiles);
+    PCU_LAUNCH(mesh_cdf_tiles_kernel, 1, 1024, stream, tiles, mesh_tiles(m), m, (const MeshScratch*)sc, out);
+    PCU_LAUNCH(mesh_cdf_scan_kernel, (unsigned)mesh_tiles(m), kMeshScanThreads, stream, cdf, m, (const MeshScratch*)sc,
+               (const unsigned long long*)tiles);
+    return PCU_B200_OK;
+}
+
+struct MeshCdfScratch {
+    unsigned long long* cdf;
+    unsigned long long* tiles;
+    MeshScratch* sc;
+    MeshArea* area;       // the caller's, or this one when the caller passes none
+    void carve(Carver& cv, long long m) {
+        cdf = cv.take<unsigned long long>((size_t)m);
+        tiles = cv.take<unsigned long long>((size_t)mesh_tiles(m));
+        sc = cv.take<MeshScratch>(1);
+        area = cv.take<MeshArea>(1);
+    }
+};
+
+template <typename T>
+int mesh_area_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, MeshArea* out,
+                     cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (!out) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    Carver measure(nullptr);
+    MeshCdfScratch ms;
+    ms.carve(measure, m);
+    PCU_TRY(ensure_arena(ws, measure.off, stream));
+    Carver cv(ws->arena);
+    ms.carve(cv, m);
+    return enqueue_mesh_cdf<T>(ws, v, nv, f, fkind, m, ms.cdf, ms.tiles, ms.sc, out, stream);
+}
+
+template <typename T>
+int sample_mesh_random_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, long long n,
+                              unsigned seed, void* out_fidx, T* out_bc, MeshArea* out_area, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "num_samples must be positive");
+    if (!out_fidx || !out_bc) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    Carver measure(nullptr);
+    MeshCdfScratch ms;
+    ms.carve(measure, m);
+    PCU_TRY(ensure_arena(ws, measure.off, stream));
+    Carver cv(ws->arena);
+    ms.carve(cv, m);
+    MeshArea* area = out_area ? out_area : ms.area;
+    PCU_TRY(enqueue_mesh_cdf<T>(ws, v, nv, f, fkind, m, ms.cdf, ms.tiles, ms.sc, area, stream));
+    const unsigned blocks = (unsigned)std::min<long long>((n + kThreads - 1) / kThreads, (long long)ws->sm_count * 16);
+    PCU_LAUNCH((mesh_sample_kernel<T>), blocks, kThreads, stream, (const unsigned long long*)ms.cdf, m, (const MeshArea*)area,
+               (unsigned long long)seed, n, (const int*)nullptr, (const long long*)nullptr, v, nv, f, fkind, out_fidx,
+               (fkind & 1), out_bc, (T*)nullptr);
+    return PCU_B200_OK;
+}
+
+// Dense samples (positions only) -> the point-cloud Poisson-disk selection of poisson.cuh at the same seed -> the
+// kept rows' faces and coordinates, re-evaluated from their sample indices.  The CDF, the dense positions and the kept
+// rows live in ws->mesh: poisson_disk_device carves the arena and aux for itself.
+template <typename T>
+int sample_mesh_poisson_disk_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind,
+                                    double radius, long long n_dense, unsigned seed, void* out_fidx, T* out_bc, long long* out_count,
+                                    cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (!(radius > 0.0)) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid radius (%f) must be greater than 0.", radius);
+    if (n_dense <= 0 || n_dense > 0x7fffffffLL)
+        return fail(PCU_B200_INVALID_ARGUMENT, "the dense sample must have 1 .. 2^31 - 1 rows, got %lld", n_dense);
+    if (!out_fidx || !out_bc || !out_count) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    Carver measure(nullptr);
+    MeshCdfScratch ms;
+    T* pos;
+    int* kept;
+    auto carve = [&](Carver& cv) {
+        ms.carve(cv, m);
+        pos = cv.take<T>((size_t)3 * n_dense);
+        kept = cv.take<int>((size_t)n_dense);
+    };
+    carve(measure);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(grow_block(ws->mesh, ws->mesh_bytes, measure.off, stream, "mesh-sampling scratch"));
+    Carver cv(ws->mesh);
+    carve(cv);
+    PCU_TRY(enqueue_mesh_cdf<T>(ws, v, nv, f, fkind, m, ms.cdf, ms.tiles, ms.sc, ms.area, stream));
+    const unsigned blocks = (unsigned)std::min<long long>((n_dense + kThreads - 1) / kThreads, (long long)ws->sm_count * 16);
+    PCU_LAUNCH((mesh_sample_kernel<T>), blocks, kThreads, stream, (const unsigned long long*)ms.cdf, m, (const MeshArea*)ms.area,
+               (unsigned long long)seed, n_dense, (const int*)nullptr, (const long long*)nullptr, v, nv, f, fkind, (void*)nullptr, 0,
+               (T*)nullptr, pos);
+    PCU_TRY(poisson_disk_device<T>(ws, pos, n_dense, radius, seed, kept, out_count, nullptr, stream));
+    PCU_LAUNCH((mesh_sample_kernel<T>), blocks, kThreads, stream, (const unsigned long long*)ms.cdf, m, (const MeshArea*)ms.area,
+               (unsigned long long)seed, n_dense, (const int*)kept, (const long long*)out_count, v, nv, f, fkind, out_fidx,
+               (fkind & 1), out_bc, (T*)nullptr);
+    return PCU_B200_OK;
+}
+
+template <typename A, typename B, typename P>
+int interpolate_launch(pcu_b200_workspace* ws, const void* f, long long m, int fkind, const void* fi, long long n, int fikind,
+                       const void* bc, const void* attr, long long nv, long long dim, P* out, unsigned long long* out_bad,
+                       cudaStream_t stream) {
+    const long long work = n * dim;
+    const unsigned blocks = (unsigned)std::min<long long>((work + kThreads - 1) / kThreads, (long long)ws->sm_count * 16);
+    PCU_LAUNCH((interpolate_bary_kernel<A, B, P>), blocks, kThreads, stream, f, m, fkind, fi, n, fikind, (const B*)bc,
+               (const A*)attr, nv, dim, out, out_bad);
+    return PCU_B200_OK;
+}
+
+template <typename P>
+int interpolate_device(pcu_b200_workspace* ws, const void* f, long long m, int fkind, const void* fi, long long n, int fikind,
+                       const void* bc, int bc_is_f64, const void* attr, int attr_is_f64, long long nv, long long dim, P* out,
+                       unsigned long long* out_bad, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!f || !fi || !bc || !attr || !out || !out_bad) return fail(PCU_B200_INVALID_ARGUMENT, "null pointer");
+    if (m <= 0 || nv <= 0 || n <= 0 || dim <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "interpolate_barycentric: empty input");
+    if (fkind < kIdxI32 || fkind > kIdxU64 || fikind < kIdxI32 || fikind > kIdxU64)
+        return fail(PCU_B200_INVALID_ARGUMENT, "unknown index kind");
+    if (sizeof(P) == 4 && (bc_is_f64 || attr_is_f64))
+        return fail(PCU_B200_INVALID_ARGUMENT, "a float64 input promotes the result to float64: use the _f64 entry point");
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_CUDA(cudaMemsetAsync(out_bad, 0, sizeof(unsigned long long), stream));
+    if constexpr (sizeof(P) == 4) {
+        return interpolate_launch<float, float, float>(ws, f, m, fkind, fi, n, fikind, bc, attr, nv, dim, out, out_bad, stream);
+    } else {
+        if (attr_is_f64)
+            return bc_is_f64 ? interpolate_launch<double, double, P>(ws, f, m, fkind, fi, n, fikind, bc, attr, nv, dim, out, out_bad, stream)
+                             : interpolate_launch<double, float, P>(ws, f, m, fkind, fi, n, fikind, bc, attr, nv, dim, out, out_bad, stream);
+        return bc_is_f64 ? interpolate_launch<float, double, P>(ws, f, m, fkind, fi, n, fikind, bc, attr, nv, dim, out, out_bad, stream)
+                         : interpolate_launch<float, float, P>(ws, f, m, fkind, fi, n, fikind, bc, attr, nv, dim, out, out_bad, stream);
+    }
+}
+
 // ---- duplicate removal (SURVEY.md 8f N2, src/remove_duplicates.cpp) ----------------------------------------
 // Stable LSD radix sort of `n` records between two buffers; returns the buffer holding the sorted records.
 template <typename Rec>
@@ -1500,6 +1658,7 @@ int pcu_b200_workspace_destroy(pcu_b200_workspace* ws) {
     if (ws->arena) cudaFree(ws->arena);
     if (ws->io) cudaFree(ws->io);
     if (ws->aux) cudaFree(ws->aux);
+    if (ws->mesh) cudaFree(ws->mesh);
     if (ws->handover) cudaEventDestroy(ws->handover);
     if (ws->hint_host) cudaFreeHost((void*)ws->hint_host);
     if (ws->own_stream) cudaStreamDestroy(ws->own_stream);
@@ -1513,7 +1672,7 @@ int pcu_b200_workspace_destroy(pcu_b200_workspace* ws) {
 }
 
 int64_t pcu_b200_workspace_bytes(const pcu_b200_workspace* ws) {
-    return ws ? (int64_t)(ws->arena_bytes + ws->io_bytes + ws->aux_bytes) : 0;
+    return ws ? (int64_t)(ws->arena_bytes + ws->io_bytes + ws->aux_bytes + ws->mesh_bytes) : 0;
 }
 
 int pcu_b200_workspace_set_profiling(pcu_b200_workspace* ws, int enabled) {
@@ -1743,6 +1902,51 @@ int pcu_b200_poisson_disk_f32(pcu_b200_workspace* ws, const float* points, int64
 int pcu_b200_poisson_disk_f64(pcu_b200_workspace* ws, const double* points, int64_t n, double radius, uint32_t seed,
                               int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream) {
     return poisson_disk_device<double>(ws, points, n, radius, seed, out_idx, (long long*)out_count, out_rounds, (cudaStream_t)stream);
+}
+
+int pcu_b200_mesh_area_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                           pcu_b200_mesh_area* out_area, void* stream) {
+    return mesh_area_device<float>(ws, v, nv, f, nf, f_kind, (MeshArea*)out_area, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_area_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                           pcu_b200_mesh_area* out_area, void* stream) {
+    return mesh_area_device<double>(ws, v, nv, f, nf, f_kind, (MeshArea*)out_area, (cudaStream_t)stream);
+}
+int pcu_b200_sample_mesh_random_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                    int64_t num_samples, uint32_t seed, void* out_fidx, float* out_bc, pcu_b200_mesh_area* out_area,
+                                    void* stream) {
+    return sample_mesh_random_device<float>(ws, v, nv, f, nf, f_kind, num_samples, seed, out_fidx, out_bc, (MeshArea*)out_area,
+                                            (cudaStream_t)stream);
+}
+int pcu_b200_sample_mesh_random_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                    int64_t num_samples, uint32_t seed, void* out_fidx, double* out_bc, pcu_b200_mesh_area* out_area,
+                                    void* stream) {
+    return sample_mesh_random_device<double>(ws, v, nv, f, nf, f_kind, num_samples, seed, out_fidx, out_bc, (MeshArea*)out_area,
+                                             (cudaStream_t)stream);
+}
+int pcu_b200_sample_mesh_poisson_disk_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                          double radius, int64_t n_dense, uint32_t seed, void* out_fidx, float* out_bc,
+                                          int64_t* out_count, void* stream) {
+    return sample_mesh_poisson_disk_device<float>(ws, v, nv, f, nf, f_kind, radius, n_dense, seed, out_fidx, out_bc,
+                                                  (long long*)out_count, (cudaStream_t)stream);
+}
+int pcu_b200_sample_mesh_poisson_disk_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                          double radius, int64_t n_dense, uint32_t seed, void* out_fidx, double* out_bc,
+                                          int64_t* out_count, void* stream) {
+    return sample_mesh_poisson_disk_device<double>(ws, v, nv, f, nf, f_kind, radius, n_dense, seed, out_fidx, out_bc,
+                                                   (long long*)out_count, (cudaStream_t)stream);
+}
+int pcu_b200_interpolate_barycentric_f32(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, const void* fi, int64_t n,
+                                         int fi_kind, const float* bc, const float* attribute, int64_t nv, int64_t dim, float* out,
+                                         uint64_t* out_bad, void* stream) {
+    return interpolate_device<float>(ws, f, nf, f_kind, fi, n, fi_kind, bc, 0, attribute, 0, nv, dim, out,
+                                     (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_interpolate_barycentric_f64(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, const void* fi, int64_t n,
+                                         int fi_kind, const void* bc, int bc_is_f64, const void* attribute, int attribute_is_f64,
+                                         int64_t nv, int64_t dim, double* out, uint64_t* out_bad, void* stream) {
+    return interpolate_device<double>(ws, f, nf, f_kind, fi, n, fi_kind, bc, bc_is_f64, attribute, attribute_is_f64, nv, dim, out,
+                                      (unsigned long long*)out_bad, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,
