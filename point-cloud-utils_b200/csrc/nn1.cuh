@@ -6,6 +6,7 @@
 // (src/point_cloud_distance.cpp:221-225, point_cloud_utils/__init__.py:112-113), so no per-point
 // distance buffer is ever written for the scalar metrics.
 #pragma once
+#include <type_traits>
 #include "search.cuh"
 
 namespace pcu {
@@ -123,46 +124,47 @@ __global__ void __launch_bounds__(kThreads, sizeof(T) == 4 ? 6 : 4) nn1_kernel(c
     if (active) {
         const Pt<T> q = load_pt<T>(qc.sorted + t);
         row = (long long)q.i;
-        const int st = g.stride;
-        const int cx = cell_of<T>(q.x, g.origin[0], g.inv_h, g.dim[0]);
-        const int cy = cell_of<T>(q.y, g.origin[1], g.inv_h, g.dim[1]);
-        const int cz = cell_of<T>(q.z, g.origin[2], g.inv_h, g.dim[2]);
-        const int xa = max(cx - 1, 0), xb = min(cx + 1, g.dim[0] - 1);
-        // gaps to the walls of the query's own cell along y and z
-        // wall tables indexed with unsigned 32-bit offsets off the two base pointers (axis a starts at a * st)
+        // wall tables indexed with unsigned 32-bit offsets off the two base pointers (axis a starts at a * stride)
         const T* __restrict__ wl = dc.wall_lo;
         const T* __restrict__ wh = dc.wall_hi;
-        const unsigned ust = (unsigned)st;
-        const T gy[3] = {(T)0, sq_gap<T>(q.y, __ldg(wl + (ust + (unsigned)cy))), sq_gap<T>(q.y, __ldg(wh + (ust + (unsigned)cy + 1u)))};
-        const T gz[3] = {(T)0, sq_gap<T>(q.z, __ldg(wl + (2u * ust + (unsigned)cz))), sq_gap<T>(q.z, __ldg(wh + (2u * ust + (unsigned)cz + 1u)))};
-        // (dy, dz) as indices into {0: same, 1: minus one, 2: plus one}; nearest rows first.  All index
-        // arithmetic in unsigned 32 bits off one centre-row index (one IMAD.WIDE per load instead of a
-        // 64-bit add chain), the in-range tests once per direction instead of once per row.
-        const int order_y[9] = {0, 1, 2, 0, 0, 1, 2, 1, 2};
-        const int order_z[9] = {0, 0, 0, 1, 2, 1, 1, 2, 2};
-        const unsigned d0 = (unsigned)g.dim[0], slab = d0 * (unsigned)g.dim[1];
-        const unsigned centre = ((unsigned)cz * (unsigned)g.dim[1] + (unsigned)cy) * d0;
-        const bool ok_y[3] = {true, cy > 0, cy + 1 < g.dim[1]};
-        const bool ok_z[3] = {true, cz > 0, cz + 1 < g.dim[2]};
-        const unsigned off_y[3] = {0u, 0u - d0, d0};
-        const unsigned off_z[3] = {0u, 0u - slab, slab};
-        const unsigned* __restrict__ cs = dc.cell_start;
-        const unsigned first_x = (unsigned)xa, past_x = (unsigned)xb + 1u;
+        int cx = cell_of<T>(q.x, g.origin[0], g.inv_h, g.dim[0]);
+        int cy = cell_of<T>(q.y, g.origin[1], g.inv_h, g.dim[1]);
+        int cz = cell_of<T>(q.z, g.origin[2], g.inv_h, g.dim[2]);
         unsigned j = 0, e = 0;
+        {   // phase A: the query's own row's run and the row table
+            const int xa = max(cx - 1, 0), xb = min(cx + 1, g.dim[0] - 1);
+            // gaps to the walls of the query's own cell along y and z
+            const unsigned ust = (unsigned)g.stride;
+            const T gy[3] = {(T)0, sq_gap<T>(q.y, __ldg(wl + (ust + (unsigned)cy))), sq_gap<T>(q.y, __ldg(wh + (ust + (unsigned)cy + 1u)))};
+            const T gz[3] = {(T)0, sq_gap<T>(q.z, __ldg(wl + (2u * ust + (unsigned)cz))), sq_gap<T>(q.z, __ldg(wh + (2u * ust + (unsigned)cz + 1u)))};
+            // (dy, dz) as indices into {0: same, 1: minus one, 2: plus one}; nearest rows first.  All index
+            // arithmetic in unsigned 32 bits off one centre-row index (one IMAD.WIDE per load instead of a
+            // 64-bit add chain), the in-range tests once per direction instead of once per row.
+            const int order_y[9] = {0, 1, 2, 0, 0, 1, 2, 1, 2};
+            const int order_z[9] = {0, 0, 0, 1, 2, 1, 1, 2, 2};
+            const unsigned d0 = (unsigned)g.dim[0], slab = d0 * (unsigned)g.dim[1];
+            const unsigned centre = ((unsigned)cz * (unsigned)g.dim[1] + (unsigned)cy) * d0;
+            const bool ok_y[3] = {true, cy > 0, cy + 1 < g.dim[1]};
+            const bool ok_z[3] = {true, cz > 0, cz + 1 < g.dim[2]};
+            const unsigned off_y[3] = {0u, 0u - d0, d0};
+            const unsigned off_z[3] = {0u, 0u - slab, slab};
+            const unsigned* __restrict__ cs = dc.cell_start;
+            const unsigned first_x = (unsigned)xa, past_x = (unsigned)xb + 1u;
 #pragma unroll
-        for (int s = 0; s < 9; ++s) {
-            const int oy = order_y[s], oz = order_z[s];
-            const unsigned base = centre + off_y[oy] + off_z[oz];
-            unsigned a = 0, b = 0;
-            if (ok_y[oy] && ok_z[oz]) {
-                a = __ldg(cs + (base + first_x));
-                b = __ldg(cs + (base + past_x));
-            }
-            if (s == 0) { j = a; e = b; }
-            else {
-                rows.begin[s - 1][tid] = a;
-                rows.end[s - 1][tid] = b;
-                rows.bound[s - 1][tid] = R::add(gy[oy], gz[oz]);
+            for (int s = 0; s < 9; ++s) {
+                const int oy = order_y[s], oz = order_z[s];
+                const unsigned base = centre + off_y[oy] + off_z[oz];
+                unsigned a = 0, b = 0;
+                if (ok_y[oy] && ok_z[oz]) {
+                    a = __ldg(cs + (base + first_x));
+                    b = __ldg(cs + (base + past_x));
+                }
+                if (s == 0) { j = a; e = b; }
+                else {
+                    rows.begin[s - 1][tid] = a;
+                    rows.end[s - 1][tid] = b;
+                    rows.bound[s - 1][tid] = R::add(gy[oy], gz[oz]);
+                }
             }
         }
         int r = 0;
@@ -198,8 +200,20 @@ __global__ void __launch_bounds__(kThreads, sizeof(T) == 4 ? 6 : 4) nn1_kernel(c
                 }
             }
         }
+        if constexpr (std::is_same<CS, CloudsVal<T>>::value) {
+            // The query's cell, recomputed from q and the shared header rather than kept live through the loop.
+            // At the 40-register cap of six CTAs per SM, keeping it made the allocator load both candidates of a
+            // trip of the by-value fp32 sweep (C3) into the same four registers, so each trip waited for two L1/L2
+            // round trips in series (tools/sweep_sass.py shows the loads in flight).  The pointer-descriptor
+            // sweeps had both loads in flight already and measured slower with the recomputation.
+            cx = cell_of<T>(q.x, g.origin[0], g.inv_h, g.dim[0]);
+            cy = cell_of<T>(q.y, g.origin[1], g.inv_h, g.dim[1]);
+            cz = cell_of<T>(q.z, g.origin[2], g.inv_h, g.dim[2]);
+        }
+        const int xa = max(cx - 1, 0), xb = min(cx + 1, g.dim[0] - 1);
         const int ya = max(cy - 1, 0), yb = min(cy + 1, g.dim[1] - 1);
         const int za = max(cz - 1, 0), zb = min(cz + 1, g.dim[2] - 1);
+        const unsigned ust = (unsigned)g.stride;
         T lb = sq_gap<T>(q.x, __ldg(wl + (unsigned)xa));
         lb = R::vmin(lb, sq_gap<T>(q.x, __ldg(wh + ((unsigned)xb + 1u))));
         lb = R::vmin(lb, sq_gap<T>(q.y, __ldg(wl + (ust + (unsigned)ya))));
