@@ -278,7 +278,11 @@ constexpr int kSlabThreads = 512;               // threads of every slab kernel
 constexpr int kSlabTile = 2048;                 // points per staged tile of the chunk walk (4 per thread)
 constexpr long long kSlabChunkPoints = 16384;   // points per chunk CTA, until kMaxSlabChunks CTAs are reached
 constexpr int kMaxSlabChunks = 128;             // chunk CTAs per cloud
-constexpr int kSlabStageBytes = 64 * 1024;      // shared-memory staging of one slab's records (twice the mean slab)
+constexpr int kSlabStageBytes = 64 * 1024;      // shared-memory staging of one slab's records
+// Mean slab as a share of the staging buffer.  Fuller slabs mean fewer slabs: a cheaper tile scan and longer runs
+// per (tile, slab) in the partition, fewer sort CTAs.  At 3/4 a uniform slab (3072 fp32 records, sd ~55) stays far
+// below the buffer; a slab that does not fit takes the slower global-memory path (DESIGN.md §4).
+constexpr double kSlabMeanFill = 0.75;
 constexpr int kSlabMaxCells = 16 * 1024;        // cells per slab, upper bound (shared-memory counters)
 constexpr int kMaxSlabs = 8192;                 // = 2^27 cells (the largest cell_cap) / kSlabMaxCells
 

@@ -439,7 +439,7 @@ __global__ void __launch_bounds__(kThreads) scatter_kernel(const __grid_constant
 // ---------------------------------------------------------------------------------------------
 // 3-5 as a slab build (single pairs above 8192 points).  The linear cell indices 0 .. ncells - 1 are cut
 // into c.slabs slabs of W = ceil(ncells / slabs) consecutive cells.  The host picks `slabs` so that a
-// slab holds half a staging buffer (kSlabStageBytes) of points on average and its cells fit
+// slab holds kSlabMeanFill of a staging buffer (kSlabStageBytes) of points on average and its cells fit
 // shared-memory counters; W follows from the actual ncells on the device.  Every point is read twice
 // from the caller's array and its record is written twice, each time as contiguous runs, instead of
 // one returning L2 atomic, one dependent gather and one 16-byte store at a random address per point.

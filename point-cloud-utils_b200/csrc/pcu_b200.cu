@@ -455,8 +455,8 @@ struct Plan {
             cl.scan_ticket = take_strided<unsigned>(cv, 3, B, args.cs[s].scan_ticket);
             cl.occupied = take_strided<unsigned>(cv, 1, B, args.cs[s].occupied);
             if (slab_build) {
-                // a slab holds half the staging buffer on average, and at most kSlabMaxCells cells
-                const long long per_slab = kSlabStageBytes / (2 * (long long)sizeof(Pt<T>));
+                // a slab holds kSlabMeanFill of the staging buffer on average, and at most kSlabMaxCells cells
+                const long long per_slab = (long long)(kSlabMeanFill * kSlabStageBytes) / (long long)sizeof(Pt<T>);
                 const long long want = std::max((sizes[s] + per_slab - 1) / per_slab, ((long long)cl.cell_cap + kSlabMaxCells - 1) / kSlabMaxCells);
                 cl.slabs = (int)std::min<long long>(kMaxSlabs, std::max(1LL, want));
                 cl.slab_chunks = (int)std::min<long long>(kMaxSlabChunks, (sizes[s] + kSlabChunkPoints - 1) / kSlabChunkPoints);
