@@ -177,8 +177,9 @@ py::array pinned_cloud(py::ssize_t rows, py::ssize_t cols) {
     return py::array_t<T>({rows, cols}, {(py::ssize_t)(cols * sizeof(T)), (py::ssize_t)sizeof(T)}, static_cast<T*>(p), owner);
 }
 
-struct Options { int leaf = 10; float occupancy = 0.f; int disable_replay = 0; int binning = 0; int host_staging = 0; };
+struct Options { float occupancy = 0.f; int disable_replay = 0; int binning = 0; int host_staging = 0; };
 Options& defaults() { static Options o; return o; }
+constexpr int kDefaultLeaf = 10;   // the leaf size of calls that take none
 
 // Validates the per-call options (with the GIL held); they are applied to the workspace inside the
 // call's exclusive section so that concurrent callers cannot mix them up.
@@ -191,6 +192,22 @@ pcu_b200_options make_options(int max_points_per_leaf) {
     o.binning = defaults().binning;
     o.host_staging = defaults().host_staging;
     return o;
+}
+
+// Every binding enters a workspace here: the workspace of (device, key), the process defaults plus this call's leaf
+// size, then `call(ws)` with the GIL released and the workspace held exclusively, under exactly those options (never
+// what an earlier call left behind).  A failed status becomes a Python exception.
+template <class F>
+void on_workspace(int device, uintptr_t key, int leaf, F&& call) {
+    Slot& slot = pool().get(device, key);
+    const pcu_b200_options opts = make_options(leaf);
+    int status;
+    {
+        CallScope scope(slot);
+        status = pcu_b200_workspace_set_options(slot.ws, &opts);
+        if (status == PCU_B200_OK) status = call(slot.ws);
+    }
+    check(status);
 }
 
 enum class Dt { f32, f64 };
@@ -259,22 +276,14 @@ py::tuple knn_numpy(const py::array& q_in, const py::array& d_in, int k, bool sq
     const int64_t n = q.shape(0), m = d.shape(0);
     py::array_t<T> dists = result_array<T>((py::ssize_t)n, (py::ssize_t)k);
     py::array_t<int64_t> corrs = result_array<int64_t>((py::ssize_t)n, (py::ssize_t)k);
-    Slot& slot = pool().get(device, kHostKey);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(leaf);
-    int status;
     int64_t tied = 0;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
         if (sizeof(T) == 4)
-            status = pcu_b200_knn_host_f32(ws, (const float*)q.data(), n, (const float*)d.data(), m, k, squared,
-                                           (float*)dists.mutable_data(), corrs.mutable_data(), &tied);
-        else
-            status = pcu_b200_knn_host_f64(ws, (const double*)q.data(), n, (const double*)d.data(), m, k, squared,
-                                           (double*)dists.mutable_data(), corrs.mutable_data(), &tied);
-    }
-    check(status);
+            return pcu_b200_knn_host_f32(ws, (const float*)q.data(), n, (const float*)d.data(), m, k, squared,
+                                         (float*)dists.mutable_data(), corrs.mutable_data(), &tied);
+        return pcu_b200_knn_host_f64(ws, (const double*)q.data(), n, (const double*)d.data(), m, k, squared,
+                                     (double*)dists.mutable_data(), corrs.mutable_data(), &tied);
+    });
     // npe::move hands the matrix to numpy and squeezes every size-1 dimension
     // (pinned for (n, 1) -> (n,) by tests/test_examples.py:363-368)
     return py::make_tuple(dists.attr("squeeze")(), corrs.attr("squeeze")());
@@ -310,20 +319,12 @@ template <typename T>
 pcu_b200_nn_stats one_sided_numpy(const py::array& s_in, const py::array& t_in, int leaf, int device) {
     auto s = dense<T>(s_in);
     auto t = dense<T>(t_in);
-    Slot& slot = pool().get(device, kHostKey);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(leaf);
     pcu_b200_nn_stats st{};
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
         if (sizeof(T) == 4)
-            status = pcu_b200_nn_stats_host_f32(ws, (const float*)s.data(), s.shape(0), (const float*)t.data(), t.shape(0), &st);
-        else
-            status = pcu_b200_nn_stats_host_f64(ws, (const double*)s.data(), s.shape(0), (const double*)t.data(), t.shape(0), &st);
-    }
-    check(status);
+            return pcu_b200_nn_stats_host_f32(ws, (const float*)s.data(), s.shape(0), (const float*)t.data(), t.shape(0), &st);
+        return pcu_b200_nn_stats_host_f64(ws, (const double*)s.data(), s.shape(0), (const double*)t.data(), t.shape(0), &st);
+    });
     return st;
 }
 
@@ -351,27 +352,23 @@ py::tuple chamfer_stats(const py::array& x_in, const py::array& y_in, int max_po
     const Dt dt = common_dtype(x_in, y_in, "x", "y");
     check_shapes(x_in, y_in, "x", "y");
     const int dev = current_device_or_default(device);
-    Slot& slot = pool().get(dev, kHostKey);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
     pcu_b200_nn_stats st[2] = {};
-    int status;
     py::object value;
     if (dt == Dt::f32) {
         auto x = dense<float>(x_in);
         auto y = dense<float>(y_in);
         float v = 0.f;
-        { CallScope scope(slot); pcu_b200_workspace_set_options(ws, &opts);
-          status = pcu_b200_chamfer_host_f32(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v); }
-        check(status);
+        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+            return pcu_b200_chamfer_host_f32(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v);
+        });
         value = py::module_::import("numpy").attr("float32")(v);
     } else {
         auto x = dense<double>(x_in);
         auto y = dense<double>(y_in);
         double v = 0.0;
-        { CallScope scope(slot); pcu_b200_workspace_set_options(ws, &opts);
-          status = pcu_b200_chamfer_host_f64(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v); }
-        check(status);
+        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+            return pcu_b200_chamfer_host_f64(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v);
+        });
         value = py::module_::import("numpy").attr("float64")(v);
     }
     return py::make_tuple(value, stats_to_dict(st[0]), stats_to_dict(st[1]));
@@ -408,21 +405,13 @@ py::tuple normals_knn_numpy(const py::array& p_in, const py::array& v_in, int k,
     py::array_t<int64_t> idx({(py::ssize_t)n});
     py::array_t<T> normals({(py::ssize_t)n, (py::ssize_t)3});
     int64_t kept = 0;
-    Slot& slot = pool().get(device, kHostKey);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
         if (sizeof(T) == 4)
-            status = pcu_b200_normals_knn_host_f32(ws, (const float*)pts.data(), n, has_dirs ? (const float*)dirs.data() : nullptr, k,
-                                                   drop_angle, idx.mutable_data(), (float*)normals.mutable_data(), &kept);
-        else
-            status = pcu_b200_normals_knn_host_f64(ws, (const double*)pts.data(), n, has_dirs ? (const double*)dirs.data() : nullptr, k,
-                                                   drop_angle, idx.mutable_data(), (double*)normals.mutable_data(), &kept);
-    }
-    check(status);
+            return pcu_b200_normals_knn_host_f32(ws, (const float*)pts.data(), n, has_dirs ? (const float*)dirs.data() : nullptr, k,
+                                                 drop_angle, idx.mutable_data(), (float*)normals.mutable_data(), &kept);
+        return pcu_b200_normals_knn_host_f64(ws, (const double*)pts.data(), n, has_dirs ? (const double*)dirs.data() : nullptr, k,
+                                             drop_angle, idx.mutable_data(), (double*)normals.mutable_data(), &kept);
+    });
     idx.resize({(py::ssize_t)kept});
     normals.resize({(py::ssize_t)kept, (py::ssize_t)3});
     return py::make_tuple(idx, normals);
@@ -444,19 +433,12 @@ void normals_knn_device(bool is_f64, uintptr_t points, int64_t n, uintptr_t view
                         uintptr_t out_idx, uintptr_t out_normals, uintptr_t out_count, int max_points_per_leaf, int device,
                         uintptr_t stream) {
     if (k <= 0) throw py::value_error("Invalid number of neighbors (" + std::to_string(k) + ") must be greater than 0.");
-    Slot& slot = pool().get(device, stream);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
-        status = is_f64 ? pcu_b200_normals_knn_f64(ws, (const double*)points, n, (const double*)view_dirs, k, drop_angle,
-                                                   (int64_t*)out_idx, (double*)out_normals, (int64_t*)out_count, (void*)stream)
-                        : pcu_b200_normals_knn_f32(ws, (const float*)points, n, (const float*)view_dirs, k, drop_angle,
-                                                   (int64_t*)out_idx, (float*)out_normals, (int64_t*)out_count, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_normals_knn_f64(ws, (const double*)points, n, (const double*)view_dirs, k, drop_angle,
+                                                 (int64_t*)out_idx, (double*)out_normals, (int64_t*)out_count, (void*)stream)
+                      : pcu_b200_normals_knn_f32(ws, (const float*)points, n, (const float*)view_dirs, k, drop_angle,
+                                                 (int64_t*)out_idx, (float*)out_normals, (int64_t*)out_count, (void*)stream);
+    });
 }
 
 // estimate_point_cloud_normals_ball_internal (src/point_cloud_normals.cpp:303-370), argument order of the reference
@@ -484,19 +466,13 @@ py::tuple normals_ball_numpy(const py::array& p_in, const py::array& v_in, const
     py::array_t<int64_t> idx({(py::ssize_t)n});
     py::array_t<T> normals({(py::ssize_t)n, (py::ssize_t)3});
     int64_t kept = 0;
-    Slot& slot = pool().get(device, kHostKey);
-    pcu_b200_workspace* ws = slot.ws;
-    int status;
-    {
-        CallScope scope(slot);
+    on_workspace(device, kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
         if (sizeof(T) == 4)
-            status = pcu_b200_normals_ball_host_f32(ws, (const float*)pts.data(), n, has_dirs ? (const float*)dirs.data() : nullptr, &o,
-                                                    idx.mutable_data(), (float*)normals.mutable_data(), &kept);
-        else
-            status = pcu_b200_normals_ball_host_f64(ws, (const double*)pts.data(), n, has_dirs ? (const double*)dirs.data() : nullptr, &o,
-                                                    idx.mutable_data(), (double*)normals.mutable_data(), &kept);
-    }
-    check(status);
+            return pcu_b200_normals_ball_host_f32(ws, (const float*)pts.data(), n, has_dirs ? (const float*)dirs.data() : nullptr, &o,
+                                                  idx.mutable_data(), (float*)normals.mutable_data(), &kept);
+        return pcu_b200_normals_ball_host_f64(ws, (const double*)pts.data(), n, has_dirs ? (const double*)dirs.data() : nullptr, &o,
+                                              idx.mutable_data(), (double*)normals.mutable_data(), &kept);
+    });
     idx.resize({(py::ssize_t)kept});
     normals.resize({(py::ssize_t)kept, (py::ssize_t)3});
     return py::make_tuple(idx, normals);
@@ -517,99 +493,70 @@ void normals_ball_device(bool is_f64, uintptr_t points, int64_t n, uintptr_t vie
                          double drop_angle, const std::string& weight_function, int seed, uintptr_t out_idx, uintptr_t out_normals,
                          uintptr_t out_count, int device, uintptr_t stream) {
     const pcu_b200_ball_options o = ball_options(radius, min_pts, max_pts, drop_angle, weight_function, seed);
-    Slot& slot = pool().get(device, stream);
-    pcu_b200_workspace* ws = slot.ws;
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_normals_ball_f64(ws, (const double*)points, n, (const double*)view_dirs, &o, (int64_t*)out_idx,
-                                                    (double*)out_normals, (int64_t*)out_count, (void*)stream)
-                        : pcu_b200_normals_ball_f32(ws, (const float*)points, n, (const float*)view_dirs, &o, (int64_t*)out_idx,
-                                                    (float*)out_normals, (int64_t*)out_count, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_normals_ball_f64(ws, (const double*)points, n, (const double*)view_dirs, &o, (int64_t*)out_idx,
+                                                  (double*)out_normals, (int64_t*)out_count, (void*)stream)
+                      : pcu_b200_normals_ball_f32(ws, (const float*)points, n, (const float*)view_dirs, &o, (int64_t*)out_idx,
+                                                  (float*)out_normals, (int64_t*)out_count, (void*)stream);
+    });
 }
 
 // One Poisson-disk sample of a device cloud at one radius (the search over radii is in _poisson.py).
 void poisson_disk_device(bool is_f64, uintptr_t points, int64_t n, double radius, uint32_t seed, uintptr_t out_idx,
                          uintptr_t out_count, uintptr_t out_rounds, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    pcu_b200_workspace* ws = slot.ws;
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_poisson_disk_f64(ws, (const double*)points, n, radius, seed, (int32_t*)out_idx,
-                                                    (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream)
-                        : pcu_b200_poisson_disk_f32(ws, (const float*)points, n, radius, seed, (int32_t*)out_idx,
-                                                    (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_poisson_disk_f64(ws, (const double*)points, n, radius, seed, (int32_t*)out_idx,
+                                                  (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream)
+                      : pcu_b200_poisson_disk_f32(ws, (const float*)points, n, radius, seed, (int32_t*)out_idx,
+                                                  (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream);
+    });
 }
 
 // Mesh sampling (sample_mesh_random / sample_mesh_poisson_disk, _mesh_sampling.py).  f_kind: 0 int32, 1 int64,
 // 2 uint32, 3 uint64; out_area: 3 device words {W, S, faces with a corner out of range}.
 void mesh_area_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out_area, int device,
                       uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_mesh_area_f64(slot.ws, (const double*)v, nv, (const void*)f, nf, f_kind,
-                                                 (pcu_b200_mesh_area*)out_area, (void*)stream)
-                        : pcu_b200_mesh_area_f32(slot.ws, (const float*)v, nv, (const void*)f, nf, f_kind,
-                                                 (pcu_b200_mesh_area*)out_area, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_mesh_area_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (pcu_b200_mesh_area*)out_area,
+                                               (void*)stream)
+                      : pcu_b200_mesh_area_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (pcu_b200_mesh_area*)out_area,
+                                               (void*)stream);
+    });
 }
 
 void sample_mesh_random_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int64_t num_samples,
                                uint32_t seed, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_area, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_sample_mesh_random_f64(slot.ws, (const double*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
-                                                          (void*)out_fidx, (double*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream)
-                        : pcu_b200_sample_mesh_random_f32(slot.ws, (const float*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
-                                                          (void*)out_fidx, (float*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_sample_mesh_random_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
+                                                        (void*)out_fidx, (double*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream)
+                      : pcu_b200_sample_mesh_random_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
+                                                        (void*)out_fidx, (float*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream);
+    });
 }
 
 void sample_mesh_poisson_disk_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, double radius,
                                      int64_t n_dense, uint32_t seed, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_count,
                                      int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_sample_mesh_poisson_disk_f64(slot.ws, (const double*)v, nv, (const void*)f, nf, f_kind, radius,
-                                                                n_dense, seed, (void*)out_fidx, (double*)out_bc, (int64_t*)out_count,
-                                                                (void*)stream)
-                        : pcu_b200_sample_mesh_poisson_disk_f32(slot.ws, (const float*)v, nv, (const void*)f, nf, f_kind, radius,
-                                                                n_dense, seed, (void*)out_fidx, (float*)out_bc, (int64_t*)out_count,
-                                                                (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_sample_mesh_poisson_disk_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, radius, n_dense,
+                                                              seed, (void*)out_fidx, (double*)out_bc, (int64_t*)out_count, (void*)stream)
+                      : pcu_b200_sample_mesh_poisson_disk_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, radius, n_dense,
+                                                              seed, (void*)out_fidx, (float*)out_bc, (int64_t*)out_count, (void*)stream);
+    });
 }
 
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
                                     uintptr_t out_bad, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = (bc_f64 || attr_f64)
-                     ? pcu_b200_interpolate_barycentric_f64(slot.ws, (const void*)f, nf, f_kind, (const void*)fi, n, fi_kind,
-                                                            (const void*)bc, bc_f64, (const void*)attr, attr_f64, nv, dim,
-                                                            (double*)out, (uint64_t*)out_bad, (void*)stream)
-                     : pcu_b200_interpolate_barycentric_f32(slot.ws, (const void*)f, nf, f_kind, (const void*)fi, n, fi_kind,
-                                                            (const float*)bc, (const float*)attr, nv, dim, (float*)out,
-                                                            (uint64_t*)out_bad, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return (bc_f64 || attr_f64)
+                   ? pcu_b200_interpolate_barycentric_f64(ws, (const void*)f, nf, f_kind, (const void*)fi, n, fi_kind, (const void*)bc,
+                                                          bc_f64, (const void*)attr, attr_f64, nv, dim, (double*)out,
+                                                          (uint64_t*)out_bad, (void*)stream)
+                   : pcu_b200_interpolate_barycentric_f32(ws, (const void*)f, nf, f_kind, (const void*)fi, n, fi_kind, (const float*)bc,
+                                                          (const float*)attr, nv, dim, (float*)out, (uint64_t*)out_bad, (void*)stream);
+    });
 }
 
 // ---- Morton codes (src/morton.cpp) ----------------------------------------------------------------
@@ -634,18 +581,18 @@ py::array morton_encode(const py::array& pts, int num_threads, int device) {
     if (pts.shape(1) != 3) throw py::value_error("pts must be an array of shape [n, 3] but got an invalid number of columns");
     const int64_t n = pts.shape(0);
     py::array_t<uint64_t> codes({(py::ssize_t)n});
-    Slot& slot = pool().get(current_device_or_default(device), kHostKey);
-    int status;
+    const int dev = current_device_or_default(device);
     if (i32) {
         auto p = py::array_t<int32_t, py::array::c_style | py::array::forcecast>::ensure(pts);
-        CallScope scope(slot);
-        status = pcu_b200_morton_encode_host_i32(slot.ws, p.data(), n, codes.mutable_data());
+        on_workspace(dev, kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+            return pcu_b200_morton_encode_host_i32(ws, p.data(), n, codes.mutable_data());
+        });
     } else {
         auto p = py::array_t<int64_t, py::array::c_style | py::array::forcecast>::ensure(pts);
-        CallScope scope(slot);
-        status = pcu_b200_morton_encode_host_i64(slot.ws, p.data(), n, codes.mutable_data());
+        on_workspace(dev, kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+            return pcu_b200_morton_encode_host_i64(ws, p.data(), n, codes.mutable_data());
+        });
     }
-    check(status);
     return codes;
 }
 
@@ -654,10 +601,9 @@ py::array morton_decode(const py::array& codes_in, int num_threads, int device) 
     auto codes = as_codes(codes_in, "codes");
     const int64_t n = codes.size();
     py::array_t<int32_t> pts({(py::ssize_t)n, (py::ssize_t)3});
-    Slot& slot = pool().get(current_device_or_default(device), kHostKey);
-    int status;
-    { CallScope scope(slot); status = pcu_b200_morton_decode_host(slot.ws, codes.data(), n, pts.mutable_data()); }
-    check(status);
+    on_workspace(current_device_or_default(device), kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_morton_decode_host(ws, codes.data(), n, pts.mutable_data());
+    });
     return pts;
 }
 
@@ -668,14 +614,10 @@ py::array morton_addsub(const py::array& a_in, const py::array& b_in, int num_th
     if (a.size() != b.size()) throw py::value_error("codes_1 and codes_2 must have the same number of entries.");
     const int64_t n = a.size();
     py::array_t<uint64_t> out({(py::ssize_t)n});
-    Slot& slot = pool().get(current_device_or_default(device), kHostKey);
-    int status;
-    {
-        CallScope scope(slot);
-        status = subtract ? pcu_b200_morton_subtract_host(slot.ws, a.data(), b.data(), n, out.mutable_data())
-                          : pcu_b200_morton_add_host(slot.ws, a.data(), b.data(), n, out.mutable_data());
-    }
-    check(status);
+    on_workspace(current_device_or_default(device), kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return subtract ? pcu_b200_morton_subtract_host(ws, a.data(), b.data(), n, out.mutable_data())
+                        : pcu_b200_morton_add_host(ws, a.data(), b.data(), n, out.mutable_data());
+    });
     return out;
 }
 
@@ -688,10 +630,9 @@ py::array morton_knn(const py::array& codes_in, const py::array& qcodes_in, int 
     const int64_t n = codes.size(), m = qcodes.size();
     k = (int)std::min<int64_t>(k, n);                       // morton.cpp:351
     py::array_t<int64_t> idx({(py::ssize_t)m, (py::ssize_t)k});
-    Slot& slot = pool().get(current_device_or_default(device), kHostKey);
-    int status;
-    { CallScope scope(slot); status = pcu_b200_morton_knn_host(slot.ws, codes.data(), n, qcodes.data(), m, k, sort_dist ? 1 : 0, idx.mutable_data()); }
-    check(status);
+    on_workspace(current_device_or_default(device), kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_morton_knn_host(ws, codes.data(), n, qcodes.data(), m, k, sort_dist ? 1 : 0, idx.mutable_data());
+    });
     return idx;
 }
 
@@ -703,37 +644,32 @@ uintptr_t cloud_prepare_numpy(const py::array& pts_in, int device, int knn_k, in
     if (pts_in.ndim() != 2 || pts_in.shape(1) != 3 || pts_in.shape(0) == 0)
         throw py::value_error("Only 3D inputs are supported: points must have shape (n, 3) with n > 0.");
     const int dev = current_device_or_default(device);
-    Slot& slot = pool().get(dev, kHostKey);
+    const int call_leaf = leaf > 0 ? leaf : kDefaultLeaf;   // a leaf size of 0 asks the library for its default
     pcu_b200_cloud* cloud = nullptr;
-    int status;
     if (f32) {
         auto p = dense<float>(pts_in);
-        CallScope scope(slot);
-        status = knn_k > 0 ? pcu_b200_cloud_prepare_knn_host_f32(slot.ws, p.data(), p.shape(0), knn_k, leaf, &cloud)
-                           : pcu_b200_cloud_prepare_host_f32(slot.ws, p.data(), p.shape(0), &cloud);
+        on_workspace(dev, kHostKey, call_leaf, [&](pcu_b200_workspace* ws) {
+            return knn_k > 0 ? pcu_b200_cloud_prepare_knn_host_f32(ws, p.data(), p.shape(0), knn_k, leaf, &cloud)
+                             : pcu_b200_cloud_prepare_host_f32(ws, p.data(), p.shape(0), &cloud);
+        });
     } else {
         auto p = dense<double>(pts_in);
-        CallScope scope(slot);
-        status = knn_k > 0 ? pcu_b200_cloud_prepare_knn_host_f64(slot.ws, p.data(), p.shape(0), knn_k, leaf, &cloud)
-                           : pcu_b200_cloud_prepare_host_f64(slot.ws, p.data(), p.shape(0), &cloud);
+        on_workspace(dev, kHostKey, call_leaf, [&](pcu_b200_workspace* ws) {
+            return knn_k > 0 ? pcu_b200_cloud_prepare_knn_host_f64(ws, p.data(), p.shape(0), knn_k, leaf, &cloud)
+                             : pcu_b200_cloud_prepare_host_f64(ws, p.data(), p.shape(0), &cloud);
+        });
     }
-    check(status);
     return (uintptr_t)cloud;
 }
 uintptr_t cloud_prepare_device(bool is_f64, uintptr_t pts, int64_t n, int device, uintptr_t stream, int knn_k, int leaf) {
-    Slot& slot = pool().get(device, stream);
     pcu_b200_cloud* cloud = nullptr;
-    int status;
-    {
-        CallScope scope(slot);
+    on_workspace(device, stream, leaf > 0 ? leaf : kDefaultLeaf, [&](pcu_b200_workspace* ws) {
         if (knn_k > 0)
-            status = is_f64 ? pcu_b200_cloud_prepare_knn_f64(slot.ws, (const double*)pts, n, knn_k, leaf, &cloud, (void*)stream)
-                            : pcu_b200_cloud_prepare_knn_f32(slot.ws, (const float*)pts, n, knn_k, leaf, &cloud, (void*)stream);
-        else
-            status = is_f64 ? pcu_b200_cloud_prepare_f64(slot.ws, (const double*)pts, n, &cloud, (void*)stream)
-                            : pcu_b200_cloud_prepare_f32(slot.ws, (const float*)pts, n, &cloud, (void*)stream);
-    }
-    check(status);
+            return is_f64 ? pcu_b200_cloud_prepare_knn_f64(ws, (const double*)pts, n, knn_k, leaf, &cloud, (void*)stream)
+                          : pcu_b200_cloud_prepare_knn_f32(ws, (const float*)pts, n, knn_k, leaf, &cloud, (void*)stream);
+        return is_f64 ? pcu_b200_cloud_prepare_f64(ws, (const double*)pts, n, &cloud, (void*)stream)
+                      : pcu_b200_cloud_prepare_f32(ws, (const float*)pts, n, &cloud, (void*)stream);
+    });
     return (uintptr_t)cloud;
 }
 void cloud_destroy(uintptr_t cloud) {
@@ -747,21 +683,14 @@ py::tuple knn_prepared_numpy_t(const py::array& q_in, pcu_b200_cloud* cloud, int
     const int64_t n = q.shape(0);
     py::array_t<T> dists = result_array<T>((py::ssize_t)n, (py::ssize_t)k);
     py::array_t<int64_t> corrs = result_array<int64_t>((py::ssize_t)n, (py::ssize_t)k);
-    Slot& slot = pool().get(device, kHostKey);
-    const pcu_b200_options opts = make_options(leaf);
-    int status;
     int64_t tied = 0;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(slot.ws, &opts);
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
         if (sizeof(T) == 4)
-            status = pcu_b200_knn_prepared_host_f32(slot.ws, (const float*)q.data(), n, cloud, k, squared, (float*)dists.mutable_data(),
-                                                    corrs.mutable_data(), &tied);
-        else
-            status = pcu_b200_knn_prepared_host_f64(slot.ws, (const double*)q.data(), n, cloud, k, squared, (double*)dists.mutable_data(),
-                                                    corrs.mutable_data(), &tied);
-    }
-    check(status);
+            return pcu_b200_knn_prepared_host_f32(ws, (const float*)q.data(), n, cloud, k, squared, (float*)dists.mutable_data(),
+                                                  corrs.mutable_data(), &tied);
+        return pcu_b200_knn_prepared_host_f64(ws, (const double*)q.data(), n, cloud, k, squared, (double*)dists.mutable_data(),
+                                              corrs.mutable_data(), &tied);
+    });
     return py::make_tuple(dists.attr("squeeze")(), corrs.attr("squeeze")());
 }
 py::tuple knn_prepared_numpy(const py::array& q_in, uintptr_t cloud, bool cloud_is_f64, int k, bool squared, int max_points_per_leaf, int device) {
@@ -780,18 +709,12 @@ py::tuple knn_prepared_numpy(const py::array& q_in, uintptr_t cloud, bool cloud_
 void knn_prepared_device(bool is_f64, uintptr_t query, int64_t n, uintptr_t cloud, int k, bool squared, uintptr_t out_dist,
                          uintptr_t out_idx, uintptr_t out_n_tied, int max_points_per_leaf, int device, uintptr_t stream) {
     if (k <= 0) throw py::value_error("Invalid value for k (" + std::to_string(k) + ") must be greater than 0.");
-    Slot& slot = pool().get(device, stream);
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(slot.ws, &opts);
-        status = is_f64 ? pcu_b200_knn_prepared_f64(slot.ws, (const double*)query, n, (pcu_b200_cloud*)cloud, k, squared, (double*)out_dist,
-                                                    (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream)
-                        : pcu_b200_knn_prepared_f32(slot.ws, (const float*)query, n, (pcu_b200_cloud*)cloud, k, squared, (float*)out_dist,
-                                                    (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_knn_prepared_f64(ws, (const double*)query, n, (pcu_b200_cloud*)cloud, k, squared, (double*)out_dist,
+                                                  (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream)
+                      : pcu_b200_knn_prepared_f32(ws, (const float*)query, n, (pcu_b200_cloud*)cloud, k, squared, (float*)out_dist,
+                                                  (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream);
+    });
 }
 
 // fused sweep(s) of numpy points against a prepared cloud: (value or None, stats[, stats])
@@ -804,27 +727,24 @@ py::tuple stats_prepared_numpy(const py::array& x_in, uintptr_t cloud, bool clou
         throw py::value_error("Only 3D inputs are supported: points must have shape (n, 3).");
     if (x_in.shape(0) == 0) throw py::value_error("Invalid input set with zero elements: points must have shape (n, 3) with n > 0.");
     const int dev = current_device_or_default(device);
-    Slot& slot = pool().get(dev, kHostKey);
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
     pcu_b200_nn_stats st[2] = {};
-    int status;
     py::object value = py::none();
     auto* y = (const pcu_b200_cloud*)cloud;
     if (f32) {
         auto x = dense<float>(x_in);
         float v = 0.f;
-        { CallScope scope(slot); pcu_b200_workspace_set_options(slot.ws, &opts);
-          status = both ? pcu_b200_chamfer_prepared_host_f32(slot.ws, x.data(), x.shape(0), y, st, &v)
-                        : pcu_b200_nn_stats_prepared_host_f32(slot.ws, x.data(), x.shape(0), y, st); }
-        check(status);
+        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+            return both ? pcu_b200_chamfer_prepared_host_f32(ws, x.data(), x.shape(0), y, st, &v)
+                        : pcu_b200_nn_stats_prepared_host_f32(ws, x.data(), x.shape(0), y, st);
+        });
         if (both) value = py::module_::import("numpy").attr("float32")(v);
     } else {
         auto x = dense<double>(x_in);
         double v = 0.0;
-        { CallScope scope(slot); pcu_b200_workspace_set_options(slot.ws, &opts);
-          status = both ? pcu_b200_chamfer_prepared_host_f64(slot.ws, x.data(), x.shape(0), y, st, &v)
-                        : pcu_b200_nn_stats_prepared_host_f64(slot.ws, x.data(), x.shape(0), y, st); }
-        check(status);
+        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+            return both ? pcu_b200_chamfer_prepared_host_f64(ws, x.data(), x.shape(0), y, st, &v)
+                        : pcu_b200_nn_stats_prepared_host_f64(ws, x.data(), x.shape(0), y, st);
+        });
         if (both) value = py::module_::import("numpy").attr("float64")(v);
     }
     if (both) return py::make_tuple(value, stats_to_dict(st[0]), stats_to_dict(st[1]));
@@ -832,83 +752,60 @@ py::tuple stats_prepared_numpy(const py::array& x_in, uintptr_t cloud, bool clou
 }
 void stats_prepared_device(bool is_f64, bool both, uintptr_t a, int64_t n, uintptr_t cloud, uintptr_t out_stats, uintptr_t out_value,
                            int max_points_per_leaf, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(slot.ws, &opts);
-        auto* st = (pcu_b200_nn_stats*)out_stats;
-        auto* y = (const pcu_b200_cloud*)cloud;
+    auto* st = (pcu_b200_nn_stats*)out_stats;
+    auto* y = (const pcu_b200_cloud*)cloud;
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
         if (both)
-            status = is_f64 ? pcu_b200_chamfer_prepared_f64(slot.ws, (const double*)a, n, y, st, (double*)out_value, (void*)stream)
-                            : pcu_b200_chamfer_prepared_f32(slot.ws, (const float*)a, n, y, st, (float*)out_value, (void*)stream);
-        else
-            status = is_f64 ? pcu_b200_nn_stats_prepared_f64(slot.ws, (const double*)a, n, y, st, (void*)stream)
-                            : pcu_b200_nn_stats_prepared_f32(slot.ws, (const float*)a, n, y, st, (void*)stream);
-    }
-    check(status);
+            return is_f64 ? pcu_b200_chamfer_prepared_f64(ws, (const double*)a, n, y, st, (double*)out_value, (void*)stream)
+                          : pcu_b200_chamfer_prepared_f32(ws, (const float*)a, n, y, st, (float*)out_value, (void*)stream);
+        return is_f64 ? pcu_b200_nn_stats_prepared_f64(ws, (const double*)a, n, y, st, (void*)stream)
+                      : pcu_b200_nn_stats_prepared_f32(ws, (const float*)a, n, y, st, (void*)stream);
+    });
 }
 
 // ---- voxel-grid down-sampling on device pointers (the Python layer owns the arrays) ----
 void voxel_downsample_device(bool is_f64, uintptr_t pts, int64_t n, uintptr_t attr, int attr_cols, bool attr_is_f64,
                              std::array<double, 3> size, std::array<double, 3> lo, std::array<double, 3> hi, int min_points,
                              uintptr_t out_pts, uintptr_t out_attr, uintptr_t out_counts, uintptr_t out_rows, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_voxel_downsample_f64(slot.ws, (const double*)pts, n, (const void*)attr, attr_cols, attr_is_f64 ? 1 : 0,
-                                                        size.data(), lo.data(), hi.data(), min_points, (double*)out_pts, (void*)out_attr,
-                                                        (int32_t*)out_counts, (int64_t*)out_rows, (void*)stream)
-                        : pcu_b200_voxel_downsample_f32(slot.ws, (const float*)pts, n, (const void*)attr, attr_cols, attr_is_f64 ? 1 : 0,
-                                                        size.data(), lo.data(), hi.data(), min_points, (float*)out_pts, (void*)out_attr,
-                                                        (int32_t*)out_counts, (int64_t*)out_rows, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_voxel_downsample_f64(ws, (const double*)pts, n, (const void*)attr, attr_cols, attr_is_f64 ? 1 : 0,
+                                                      size.data(), lo.data(), hi.data(), min_points, (double*)out_pts, (void*)out_attr,
+                                                      (int32_t*)out_counts, (int64_t*)out_rows, (void*)stream)
+                      : pcu_b200_voxel_downsample_f32(ws, (const float*)pts, n, (const void*)attr, attr_cols, attr_is_f64 ? 1 : 0,
+                                                      size.data(), lo.data(), hi.data(), min_points, (float*)out_pts, (void*)out_attr,
+                                                      (int32_t*)out_counts, (int64_t*)out_rows, (void*)stream);
+    });
 }
 
 void deduplicate_device(bool is_f64, uintptr_t pts, int64_t n, double epsilon, uintptr_t faces, int64_t nf, int cols, bool faces_i64,
                         uintptr_t out_pts, uintptr_t out_svi, uintptr_t out_svj, uintptr_t out_faces, uintptr_t out_counts, int device,
                         uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_deduplicate_f64(slot.ws, (const double*)pts, n, epsilon, (const void*)faces, nf, cols, faces_i64 ? 1 : 0,
-                                                   (double*)out_pts, (int32_t*)out_svi, (int32_t*)out_svj, (void*)out_faces,
-                                                   (int64_t*)out_counts, (void*)stream)
-                        : pcu_b200_deduplicate_f32(slot.ws, (const float*)pts, n, epsilon, (const void*)faces, nf, cols, faces_i64 ? 1 : 0,
-                                                   (float*)out_pts, (int32_t*)out_svi, (int32_t*)out_svj, (void*)out_faces,
-                                                   (int64_t*)out_counts, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_deduplicate_f64(ws, (const double*)pts, n, epsilon, (const void*)faces, nf, cols, faces_i64 ? 1 : 0,
+                                                 (double*)out_pts, (int32_t*)out_svi, (int32_t*)out_svj, (void*)out_faces,
+                                                 (int64_t*)out_counts, (void*)stream)
+                      : pcu_b200_deduplicate_f32(ws, (const float*)pts, n, epsilon, (const void*)faces, nf, cols, faces_i64 ? 1 : 0,
+                                                 (float*)out_pts, (int32_t*)out_svi, (int32_t*)out_svj, (void*)out_faces,
+                                                 (int64_t*)out_counts, (void*)stream);
+    });
 }
 
 // ---- dense pairwise distances / Sinkhorn on device pointers (the Python layer owns the arrays) ----
 void pairwise_device(bool is_f64, uintptr_t a, uintptr_t b, int64_t nb, int64_t n, int64_t m, int d, int norm_kind, double p,
                      uintptr_t out, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_pairwise_distances_f64(slot.ws, (const double*)a, (const double*)b, nb, n, m, d, norm_kind, p, (double*)out, (void*)stream)
-                        : pcu_b200_pairwise_distances_f32(slot.ws, (const float*)a, (const float*)b, nb, n, m, d, norm_kind, p, (float*)out, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_pairwise_distances_f64(ws, (const double*)a, (const double*)b, nb, n, m, d, norm_kind, p, (double*)out, (void*)stream)
+                      : pcu_b200_pairwise_distances_f32(ws, (const float*)a, (const float*)b, nb, n, m, d, norm_kind, p, (float*)out, (void*)stream);
+    });
 }
 void sinkhorn_device(bool is_f64, uintptr_t a, uintptr_t b, uintptr_t M, int64_t nb, int64_t n, int64_t m, double eps, int max_iters,
                      double stop_thresh, uintptr_t out_P, uintptr_t out_cost, uintptr_t out_iters, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    int status;
-    {
-        CallScope scope(slot);
-        status = is_f64 ? pcu_b200_sinkhorn_f64(slot.ws, (const double*)a, (const double*)b, (const double*)M, nb, n, m, eps, max_iters,
-                                                stop_thresh, (double*)out_P, (double*)out_cost, (int32_t*)out_iters, (void*)stream)
-                        : pcu_b200_sinkhorn_f32(slot.ws, (const float*)a, (const float*)b, (const float*)M, nb, n, m, eps, max_iters,
-                                                stop_thresh, (float*)out_P, (double*)out_cost, (int32_t*)out_iters, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_sinkhorn_f64(ws, (const double*)a, (const double*)b, (const double*)M, nb, n, m, eps, max_iters,
+                                              stop_thresh, (double*)out_P, (double*)out_cost, (int32_t*)out_iters, (void*)stream)
+                      : pcu_b200_sinkhorn_f32(ws, (const float*)a, (const float*)b, (const float*)M, nb, n, m, eps, max_iters,
+                                              stop_thresh, (float*)out_P, (double*)out_cost, (int32_t*)out_iters, (void*)stream);
+    });
 }
 
 // ---- raw device-pointer entry points (CUDA torch tensors) --------------------------------------
@@ -916,39 +813,24 @@ void knn_device(bool is_f64, uintptr_t query, int64_t n, uintptr_t dataset, int6
                 uintptr_t out_dist, uintptr_t out_idx, uintptr_t out_n_tied, int max_points_per_leaf, int device,
                 uintptr_t stream) {
     if (k <= 0) throw py::value_error("Invalid value for k (" + std::to_string(k) + ") must be greater than 0.");
-    Slot& slot = pool().get(device, stream);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
-        status = is_f64 ? pcu_b200_knn_f64(ws, (const double*)query, n, (const double*)dataset, m, k, squared,
-                                           (double*)out_dist, (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream)
-                        : pcu_b200_knn_f32(ws, (const float*)query, n, (const float*)dataset, m, k, squared,
-                                           (float*)out_dist, (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_knn_f64(ws, (const double*)query, n, (const double*)dataset, m, k, squared,
+                                         (double*)out_dist, (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream)
+                      : pcu_b200_knn_f32(ws, (const float*)query, n, (const float*)dataset, m, k, squared,
+                                         (float*)out_dist, (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream);
+    });
 }
 
 void stats_device(bool is_f64, bool both, uintptr_t a, int64_t n, uintptr_t b, int64_t m, uintptr_t out_stats,
                   uintptr_t out_value, int max_points_per_leaf, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
-        auto* st = (pcu_b200_nn_stats*)out_stats;
+    auto* st = (pcu_b200_nn_stats*)out_stats;
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
         if (both)
-            status = is_f64 ? pcu_b200_chamfer_f64(ws, (const double*)a, n, (const double*)b, m, st, (double*)out_value, (void*)stream)
-                            : pcu_b200_chamfer_f32(ws, (const float*)a, n, (const float*)b, m, st, (float*)out_value, (void*)stream);
-        else
-            status = is_f64 ? pcu_b200_nn_stats_f64(ws, (const double*)a, n, (const double*)b, m, st, (void*)stream)
-                            : pcu_b200_nn_stats_f32(ws, (const float*)a, n, (const float*)b, m, st, (void*)stream);
-    }
-    check(status);
+            return is_f64 ? pcu_b200_chamfer_f64(ws, (const double*)a, n, (const double*)b, m, st, (double*)out_value, (void*)stream)
+                          : pcu_b200_chamfer_f32(ws, (const float*)a, n, (const float*)b, m, st, (float*)out_value, (void*)stream);
+        return is_f64 ? pcu_b200_nn_stats_f64(ws, (const double*)a, n, (const double*)b, m, st, (void*)stream)
+                      : pcu_b200_nn_stats_f32(ws, (const float*)a, n, (const float*)b, m, st, (void*)stream);
+    });
 }
 
 // Batched Chamfer on numpy inputs: x (B, n, 3), y (B, m, 3) float32 -> ((B,) float32, fp64 sum)
@@ -964,34 +846,18 @@ py::tuple batched_chamfer_numpy(const py::array& x_in, const py::array& y_in, in
     const int64_t B = x.shape(0), n = x.shape(1), m = y.shape(1);
     py::array_t<float> out({(py::ssize_t)B});
     double sum = 0.0;
-    const int dev = current_device_or_default(device);
-    Slot& slot = pool().get(dev, kHostKey);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
-        status = pcu_b200_batched_chamfer_host_f32(ws, x.data(), y.data(), B, n, m, out.mutable_data(),
-                                                   &sum);
-    }
-    check(status);
+    on_workspace(current_device_or_default(device), kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_batched_chamfer_host_f32(ws, x.data(), y.data(), B, n, m, out.mutable_data(), &sum);
+    });
     return py::make_tuple(out, sum);
 }
 
 void batched_chamfer_device(uintptr_t x, uintptr_t y, int64_t B, int64_t n, int64_t m, uintptr_t out_per_pair,
                             uintptr_t out_sum, int max_points_per_leaf, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
-        status = pcu_b200_batched_chamfer_f32(ws, (const float*)x, (const float*)y, B, n, m, (float*)out_per_pair,
-                                              (double*)out_sum, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_batched_chamfer_f32(ws, (const float*)x, (const float*)y, B, n, m, (float*)out_per_pair, (double*)out_sum,
+                                            (void*)stream);
+    });
 }
 
 template <typename T>
@@ -1002,20 +868,15 @@ py::dict debug_kd_tree_t(const py::array& pts_in, int leaf, int device) {
     py::array_t<int32_t> order(m), feat(cap), first(cap), last(cap), kid0(cap), kid1(cap);
     py::array_t<T> lo(cap), hi(cap);
     int64_t nn = 0;
-    Slot& slot = pool().get(device, kHostKey);
-    pcu_b200_workspace* ws = slot.ws;
-    int status;
-    if (sizeof(T) == 4)
-        status = pcu_b200_debug_kd_tree_f32(ws, (const float*)pts.data(), m, leaf, order.mutable_data(), cap,
-                                            feat.mutable_data(), (float*)lo.mutable_data(), (float*)hi.mutable_data(),
-                                            first.mutable_data(), last.mutable_data(), kid0.mutable_data(),
-                                            kid1.mutable_data(), &nn);
-    else
-        status = pcu_b200_debug_kd_tree_f64(ws, (const double*)pts.data(), m, leaf, order.mutable_data(), cap,
-                                            feat.mutable_data(), (double*)lo.mutable_data(), (double*)hi.mutable_data(),
-                                            first.mutable_data(), last.mutable_data(), kid0.mutable_data(),
-                                            kid1.mutable_data(), &nn);
-    check(status);
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
+        if (sizeof(T) == 4)
+            return pcu_b200_debug_kd_tree_f32(ws, (const float*)pts.data(), m, leaf, order.mutable_data(), cap, feat.mutable_data(),
+                                              (float*)lo.mutable_data(), (float*)hi.mutable_data(), first.mutable_data(),
+                                              last.mutable_data(), kid0.mutable_data(), kid1.mutable_data(), &nn);
+        return pcu_b200_debug_kd_tree_f64(ws, (const double*)pts.data(), m, leaf, order.mutable_data(), cap, feat.mutable_data(),
+                                          (double*)lo.mutable_data(), (double*)hi.mutable_data(), first.mutable_data(),
+                                          last.mutable_data(), kid0.mutable_data(), kid1.mutable_data(), &nn);
+    });
     py::dict d;
     d["order"] = order; d["feat"] = feat; d["div_lo"] = lo; d["div_hi"] = hi; d["first"] = first; d["last"] = last;
     d["kid0"] = kid0; d["kid1"] = kid1; d["n_nodes"] = nn;
@@ -1032,19 +893,10 @@ py::dict debug_kd_tree(const py::array& pts, int leaf, int device) {
 
 void resolve_witness_device(bool is_f64, uintptr_t q, int64_t n, uintptr_t d, int64_t m, uintptr_t stats,
                             int max_points_per_leaf, int device, uintptr_t stream) {
-    Slot& slot = pool().get(device, stream);
-    pcu_b200_workspace* ws = slot.ws;
-    const pcu_b200_options opts = make_options(max_points_per_leaf);
-    int status;
-    {
-        CallScope scope(slot);
-        pcu_b200_workspace_set_options(ws, &opts);
-        status = is_f64 ? pcu_b200_resolve_witness_f64(ws, (const double*)q, n, (const double*)d, m,
-                                                       (pcu_b200_nn_stats*)stats, (void*)stream)
-                        : pcu_b200_resolve_witness_f32(ws, (const float*)q, n, (const float*)d, m,
-                                                       (pcu_b200_nn_stats*)stats, (void*)stream);
-    }
-    check(status);
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_resolve_witness_f64(ws, (const double*)q, n, (const double*)d, m, (pcu_b200_nn_stats*)stats, (void*)stream)
+                      : pcu_b200_resolve_witness_f32(ws, (const float*)q, n, (const float*)d, m, (pcu_b200_nn_stats*)stats, (void*)stream);
+    });
 }
 
 }  // namespace
@@ -1112,10 +964,13 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_knn_device", &knn_device);
     mod.def("_stats_device", &stats_device);
     mod.def("_resolve_witness_device", &resolve_witness_device);
-    mod.def("_debug_kd_times", [](int device, py::object stream) {
-        Slot& slot = pool().get(current_device_or_default(device), stream.is_none() ? kHostKey : stream.cast<uintptr_t>());
+    // diagnostics address a workspace by (device, stream); stream None = the numpy path's own workspace,
+    // device < 0 = the device a call that names none would use
+    auto key_of = [](const py::object& stream) { return stream.is_none() ? kHostKey : stream.cast<uintptr_t>(); };
+    mod.def("_debug_kd_times", [key_of](int device, py::object stream) {
         std::array<uint64_t, 40> t{};
-        { CallScope scope(slot); check(pcu_b200_debug_kd_times(slot.ws, t.data())); }
+        on_workspace(current_device_or_default(device), key_of(stream), kDefaultLeaf,
+                     [&](pcu_b200_workspace* ws) { return pcu_b200_debug_kd_times(ws, t.data()); });
         return t;
     }, py::arg("device") = -1, py::arg("stream") = py::none());
     mod.def("_debug_kd_tree", &debug_kd_tree, py::arg("points"), py::arg("max_points_per_leaf") = 10,
@@ -1124,28 +979,38 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_device_count", []() { return pcu_b200_device_count(); });
     mod.def("_launch_count", []() { return (int64_t)pcu_b200_launch_count(); });
     mod.def("_abi_version", []() { return pcu_b200_abi_version(); });
-    // diagnostics address a workspace by (device, stream); stream None = the numpy path's own workspace,
-    // device < 0 = the device a call that names none would use
-    auto key_of = [](const py::object& stream) { return stream.is_none() ? kHostKey : stream.cast<uintptr_t>(); };
     mod.def("_current_device", []() { return pcu_b200_current_device(); });
     mod.def("_grid_refinement", [key_of](int device, py::object stream) {
         float m[2] = {1.f, 1.f};
-        pcu_b200_workspace_grid_refinement(pool().get(current_device_or_default(device), key_of(stream)).ws, m);
+        on_workspace(current_device_or_default(device), key_of(stream), kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+            pcu_b200_workspace_grid_refinement(ws, m);
+            return PCU_B200_OK;
+        });
         return py::make_tuple(m[0], m[1]);
     }, py::arg("device") = -1, py::arg("stream") = py::none());
     mod.def("_workspace_bytes", [key_of](int device, py::object stream) {
-        return (int64_t)pcu_b200_workspace_bytes(pool().get(current_device_or_default(device), key_of(stream)).ws);
+        int64_t bytes = 0;
+        on_workspace(current_device_or_default(device), key_of(stream), kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+            bytes = pcu_b200_workspace_bytes(ws);
+            return PCU_B200_OK;
+        });
+        return bytes;
     }, py::arg("device") = -1, py::arg("stream") = py::none());
     mod.def("_workspace_exists", [key_of](int device, py::object stream) {
         std::lock_guard<std::mutex> lock(pool().mu);
         return pool().items.count(std::make_pair(current_device_or_default(device), key_of(stream))) != 0;
     }, py::arg("device") = -1, py::arg("stream") = py::none());
     mod.def("_set_profiling", [key_of](int device, py::object stream, bool on) {
-        check(pcu_b200_workspace_set_profiling(pool().get(current_device_or_default(device), key_of(stream)).ws, on ? 1 : 0));
+        on_workspace(current_device_or_default(device), key_of(stream), kDefaultLeaf,
+                     [&](pcu_b200_workspace* ws) { return pcu_b200_workspace_set_profiling(ws, on ? 1 : 0); });
     });
     mod.def("_last_profile", [key_of](int device, py::object stream) {
         float ms[10];
-        const int n = pcu_b200_workspace_last_profile(pool().get(current_device_or_default(device), key_of(stream)).ws, ms, 10);
+        int n = 0;
+        on_workspace(current_device_or_default(device), key_of(stream), kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+            n = pcu_b200_workspace_last_profile(ws, ms, 10);   // the number of stages, or -1
+            return PCU_B200_OK;
+        });
         py::dict d;
         for (int i = 0; i < n; ++i) d[py::str(pcu_b200_profile_stage_name(i))] = ms[i];
         return d;

@@ -183,17 +183,23 @@ __global__ void descriptors_kernel(const __grid_constant__ DescriptorArgs<T> a, 
 
 }  // namespace
 
+// The workspace's device scratch blocks (carve_scratch).  Every call carves the blocks it uses afresh, so buffers that
+// must outlive a nested call live in a block that the nested call does not carve.
+enum Scratch {
+    kArena,   // the device-pointer entry points' own scratch; any nested call may re-carve it
+    kIo,      // device copies of a host entry point's inputs and outputs: outlive the device call they are passed to
+    kAux,     // intermediate results (normals, Poisson disk) that outlive a nested call's re-carving of the arena
+    kMesh,    // the face CDF and dense samples of mesh Poisson-disk sampling, which outlive the point-cloud Poisson-disk
+              // call it makes (that one re-carves the arena and aux)
+    kScratchBlocks
+};
+static const char* const kScratchName[kScratchBlocks] = {"scratch", "staging", "intermediate scratch", "mesh-sampling scratch"};
+
 struct pcu_b200_workspace {
     int device = 0;
     cudaStream_t own_stream = nullptr;
-    unsigned char* arena = nullptr;      // scratch of the device-pointer entry points
-    size_t arena_bytes = 0;
-    unsigned char* io = nullptr;         // device copies of host inputs / outputs (host entry points)
-    size_t io_bytes = 0;
-    unsigned char* aux = nullptr;        // intermediate results that outlive a nested call's re-carving of the arena (normals)
-    size_t aux_bytes = 0;
-    unsigned char* mesh = nullptr;       // the face CDF and dense samples of mesh Poisson-disk sampling, which outlive the
-    size_t mesh_bytes = 0;               // point-cloud Poisson-disk call it makes (that one re-carves the arena and aux)
+    unsigned char* block[kScratchBlocks] = {};   // indexed by Scratch
+    size_t block_bytes[kScratchBlocks] = {};
     pcu_b200_options opts{};
     int sm_count = 132;                  // set from the device in pcu_b200_workspace_create
     // optional per-stage timing (bench.py's roofline pass): events recorded on the launching stream
@@ -301,13 +307,24 @@ int grow_block(unsigned char*& block, size_t& have, size_t bytes, cudaStream_t s
     return PCU_B200_OK;
 }
 
-int ensure_arena(pcu_b200_workspace* ws, size_t bytes, cudaStream_t stream) {
-    PCU_TRY(adopt_stream(ws, stream));
-    return grow_block(ws->arena, ws->arena_bytes, bytes, stream, "scratch");
+// Runs `carve(Carver&)` from `base` (a null base only measures) and returns the bytes it took.
+template <class F>
+size_t carve_at(unsigned char* base, F&& carve) {
+    Carver cv(base);
+    carve(cv);
+    return cv.off;
 }
 
-int ensure_io(pcu_b200_workspace* ws, size_t bytes, cudaStream_t stream) {
-    return grow_block(ws->io, ws->io_bytes, bytes, stream, "staging");
+// Carves a call's buffers out of scratch block `which`: measures them, hands the workspace over to `stream` (the block
+// may still be in use by work queued on the previous stream), grows the block in the order of `stream`, then carves.
+// `carve` assigns the buffers to the caller's variables; it runs twice, first from a null base.
+template <class F>
+int carve_scratch(pcu_b200_workspace* ws, Scratch which, cudaStream_t stream, F&& carve) {
+    const size_t bytes = carve_at(nullptr, carve);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(grow_block(ws->block[which], ws->block_bytes[which], bytes, stream, kScratchName[which]));
+    carve_at(ws->block[which], carve);
+    return PCU_B200_OK;
 }
 
 void mark(pcu_b200_workspace* ws, int index, cudaStream_t stream) {
@@ -390,7 +407,6 @@ struct Plan {
     int max_bbox_blocks = 1;
     int far_blocks = 1;
     int nclouds = 0, nsweeps_total = 0;
-    size_t total = 0;
     KdReplayBuffers<T> replay{};
 
     template <typename U>
@@ -399,9 +415,8 @@ struct Plan {
         return reinterpret_cast<U*>(cv.take<unsigned char>(stride_bytes * (size_t)batch));
     }
 
-    // Carves (or, with base == nullptr, just measures) the layout.
-    void layout(unsigned char* base, const PlanSpec<T>& sp) {
-        Carver cv(base);
+    // Carves (or, with a null base, just measures) the layout.
+    void layout(Carver& cv, const PlanSpec<T>& sp) {
         const long long B = sp.batch;
         nclouds = (int)(2 * B);
         nsweeps_total = (int)(B * sp.nsweeps);
@@ -471,7 +486,7 @@ struct Plan {
         slab_sort_smem = (size_t)kSlabStageBytes + (size_t)max_slab_cells * sizeof(unsigned);
         for (int d = 0; d < sp.nsweeps; ++d)
             args.sweep[d].counters = take_strided<unsigned>(cv, 8, B, args.ss[d].counters);
-        zero_begin = base ? base + zero_from : nullptr;
+        zero_begin = cv.base ? cv.base + zero_from : nullptr;
         zero_bytes = cv.off - zero_from;
         for (int s = 0; s < 2; ++s) {
             Cloud<T>& cl = args.cloud[s];
@@ -510,7 +525,6 @@ struct Plan {
                 sw.partial = take_strided<SweepPartial<T>>(cv, (size_t)sw.main_blocks + 2 * far_blocks, B, st.partial);
         }
         if (sp.replay_points > 0) replay.carve(cv, sp.replay_points);
-        total = cv.off;
         // descriptor sources
         this->cp.p = d_clouds;
         this->sp.p = d_sweeps;
@@ -591,10 +605,7 @@ void apply_grid_feedback(pcu_b200_workspace* ws, PlanSpec<T>& spec) {
 template <typename T>
 int prepare_plan(pcu_b200_workspace* ws, Plan<T>& plan, PlanSpec<T>& spec, cudaStream_t stream) {
     apply_grid_feedback(ws, spec);
-    plan.layout(nullptr, spec);
-    PCU_TRY(ensure_arena(ws, plan.total, stream));
-    plan.layout(ws->arena, spec);
-    return PCU_B200_OK;
+    return carve_scratch(ws, kArena, stream, [&](Carver& cv) { plan.layout(cv, spec); });
 }
 
 // Kernels whose dynamic shared-memory limit is raised above the default, one group of four bits each in
@@ -849,11 +860,7 @@ int resolve_witness_device(pcu_b200_workspace* ws, const T* query, long long n, 
     PCU_ON_DEVICE(ws);
     // the arena is re-carved in stream order: the sweep that produced `stats` has been enqueued before us
     KdReplayBuffers<T> rb;
-    Carver measure(nullptr);
-    rb.carve(measure, m);
-    PCU_TRY(ensure_arena(ws, measure.off, stream));
-    Carver cv(ws->arena);
-    rb.carve(cv, m);
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { rb.carve(cv, m); }));
     const int leaf = ws->opts.max_points_per_leaf > 0 ? ws->opts.max_points_per_leaf : 10;
     const int rs = enqueue_witness_replay<T>(rb, query, n, dataset, m, leaf, stats, stream, g_launches);
     if (rs != PCU_B200_OK) return fail(rs, "witness replay failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -874,20 +881,14 @@ int normals_knn_device(pcu_b200_workspace* ws, const T* points, long long n, con
     if (!out_idx || !out_normals || !out_count) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
     const long long nblocks = (n + kThreads - 1) / kThreads;
-    Carver measure(nullptr);
-    auto carve = [&](Carver& cv, long long*& nn_idx, T*& nn_dist, T*& dense, unsigned char*& keep, unsigned*& counts) {
+    long long* nn_idx; T *nn_dist, *dense; unsigned char* keep; unsigned* counts;
+    PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
         nn_idx = cv.take<long long>((size_t)n * k);
         nn_dist = cv.take<T>((size_t)n * k);
         dense = cv.take<T>((size_t)3 * n);
         keep = cv.take<unsigned char>((size_t)n);
         counts = cv.take<unsigned>((size_t)nblocks);
-    };
-    long long* nn_idx; T *nn_dist, *dense; unsigned char* keep; unsigned* counts;
-    carve(measure, nn_idx, nn_dist, dense, keep, counts);
-    PCU_TRY(adopt_stream(ws, stream));
-    PCU_TRY(grow_block(ws->aux, ws->aux_bytes, measure.off, stream, "neighbour scratch"));
-    Carver cv(ws->aux);
-    carve(cv, nn_idx, nn_dist, dense, keep, counts);
+    }));
     PCU_TRY(knn_device<T>(ws, points, n, points, n, k, 1, nn_dist, nn_idx, nullptr, stream));
     PCU_LAUNCH((normals_knn_kernel<T>), (unsigned)nblocks, kThreads, stream, points, n, nn_idx, k, view_dirs, drop_angle_threshold, dense, keep);
     PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, keep, n, counts);
@@ -896,17 +897,23 @@ int normals_knn_device(pcu_b200_workspace* ws, const T* points, long long n, con
     return PCU_B200_OK;
 }
 
-// The plan, carved from the arena, of a call that bins one cloud into cells no finer than `min_cell`.
+// A call that bins one cloud: the plan of an ordinary pair whose second cloud is a one-point dummy that is never binned
+// (prepared_second; it also keeps the dummy out of the one-CTA build).
 template <typename T>
-int single_cloud_plan(pcu_b200_workspace* ws, const T* points, long long n, double min_cell, Plan<T>& plan, cudaStream_t stream) {
+PlanSpec<T> one_cloud_spec(const T* points, long long n, float occupancy) {
     PlanSpec<T> spec;
     spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
     spec.nsweeps = 1; spec.k = 1;
-    spec.occupancy = 0.125f;          // the cell budget; the cell size itself is held up by min_cell below
-    spec.prepared_second = true;      // the one-point second cloud is a dummy: only the first is binned
-    plan.layout(nullptr, spec);
-    PCU_TRY(ensure_arena(ws, plan.total, stream));
-    plan.layout(ws->arena, spec);
+    spec.occupancy = occupancy;
+    spec.prepared_second = true;
+    return spec;
+}
+
+// The plan, carved from the arena, of a call that bins one cloud into cells no finer than `min_cell`.
+template <typename T>
+int single_cloud_plan(pcu_b200_workspace* ws, const T* points, long long n, double min_cell, Plan<T>& plan, cudaStream_t stream) {
+    const PlanSpec<T> spec = one_cloud_spec(points, n, 0.125f);   // the cell budget; the cell size is held up by min_cell below
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { plan.layout(cv, spec); }));
     plan.cv.v[0].min_cell = (float)std::min(1e30, min_cell);
     plan.cv.v[0].hint_out = nullptr;
     return PCU_B200_OK;
@@ -936,17 +943,12 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
     Plan<T> plan;
     PCU_TRY(single_cloud_plan<T>(ws, points, n, 0.5 * reach, plan, stream));
     const long long nblocks = (n + kThreads - 1) / kThreads;
-    Carver measure(nullptr);
-    auto carve = [&](Carver& cv, T*& dense, unsigned char*& keep, unsigned*& counts) {
+    T* dense; unsigned char* keep; unsigned* counts;
+    PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
         dense = cv.take<T>((size_t)3 * n);
         keep = cv.take<unsigned char>((size_t)n);
         counts = cv.take<unsigned>((size_t)nblocks);
-    };
-    T* dense; unsigned char* keep; unsigned* counts;
-    carve(measure, dense, keep, counts);
-    PCU_TRY(grow_block(ws->aux, ws->aux_bytes, measure.off, stream, "normal scratch"));
-    Carver cv(ws->aux);
-    carve(cv, dense, keep, counts);
+    }));
     mark(ws, 0, stream);
     mark(ws, 1, stream);
     PCU_TRY(enqueue_binning(ws, plan, stream, nullptr, true));
@@ -1006,20 +1008,15 @@ int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, do
     unsigned blocks = 1;
     PCU_TRY(poisson_grid_blocks<T>(ws->device, ws->sm_count, n, &blocks));
     const long long nblocks = (n + kThreads - 1) / kThreads;
-    Carver measure(nullptr);
-    auto carve = [&](Carver& cv, PoissonScratch& s, unsigned*& counts) {
+    PoissonScratch s; unsigned* counts;
+    PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
         s.ring = cv.take<unsigned>(4);
         s.state = cv.take<unsigned char>((size_t)n);
         s.keep = cv.take<unsigned char>((size_t)n);
         s.list[0] = cv.take<unsigned>((size_t)n);
         s.list[1] = cv.take<unsigned>((size_t)n);
         counts = cv.take<unsigned>((size_t)nblocks);
-    };
-    PoissonScratch s; unsigned* counts;
-    carve(measure, s, counts);
-    PCU_TRY(grow_block(ws->aux, ws->aux_bytes, measure.off, stream, "Poisson-disk scratch"));
-    Carver cv(ws->aux);
-    carve(cv, s, counts);
+    }));
     PCU_CUDA(cudaMemsetAsync(s.ring, 0, (size_t)((unsigned char*)s.list[0] - (unsigned char*)s.ring), stream));   // ring, state, keep
     mark(ws, 0, stream);
     mark(ws, 1, stream);
@@ -1085,12 +1082,8 @@ int mesh_area_device(pcu_b200_workspace* ws, const T* v, long long nv, const voi
     PCU_TRY(mesh_check(v, nv, f, m, fkind));
     if (!out) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    Carver measure(nullptr);
     MeshCdfScratch ms;
-    ms.carve(measure, m);
-    PCU_TRY(ensure_arena(ws, measure.off, stream));
-    Carver cv(ws->arena);
-    ms.carve(cv, m);
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { ms.carve(cv, m); }));
     return enqueue_mesh_cdf<T>(ws, v, nv, f, fkind, m, ms.cdf, ms.tiles, ms.sc, out, stream);
 }
 
@@ -1102,12 +1095,8 @@ int sample_mesh_random_device(pcu_b200_workspace* ws, const T* v, long long nv, 
     if (n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "num_samples must be positive");
     if (!out_fidx || !out_bc) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    Carver measure(nullptr);
     MeshCdfScratch ms;
-    ms.carve(measure, m);
-    PCU_TRY(ensure_arena(ws, measure.off, stream));
-    Carver cv(ws->arena);
-    ms.carve(cv, m);
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { ms.carve(cv, m); }));
     MeshArea* area = out_area ? out_area : ms.area;
     PCU_TRY(enqueue_mesh_cdf<T>(ws, v, nv, f, fkind, m, ms.cdf, ms.tiles, ms.sc, area, stream));
     const unsigned blocks = (unsigned)std::min<long long>((n + kThreads - 1) / kThreads, (long long)ws->sm_count * 16);
@@ -1119,7 +1108,7 @@ int sample_mesh_random_device(pcu_b200_workspace* ws, const T* v, long long nv, 
 
 // Dense samples (positions only) -> the point-cloud Poisson-disk selection of poisson.cuh at the same seed -> the
 // kept rows' faces and coordinates, re-evaluated from their sample indices.  The CDF, the dense positions and the kept
-// rows live in ws->mesh: poisson_disk_device carves the arena and aux for itself.
+// rows live in kMesh: poisson_disk_device carves the arena and aux for itself.
 template <typename T>
 int sample_mesh_poisson_disk_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind,
                                     double radius, long long n_dense, unsigned seed, void* out_fidx, T* out_bc, long long* out_count,
@@ -1131,20 +1120,14 @@ int sample_mesh_poisson_disk_device(pcu_b200_workspace* ws, const T* v, long lon
         return fail(PCU_B200_INVALID_ARGUMENT, "the dense sample must have 1 .. 2^31 - 1 rows, got %lld", n_dense);
     if (!out_fidx || !out_bc || !out_count) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    Carver measure(nullptr);
     MeshCdfScratch ms;
     T* pos;
     int* kept;
-    auto carve = [&](Carver& cv) {
+    PCU_TRY(carve_scratch(ws, kMesh, stream, [&](Carver& cv) {
         ms.carve(cv, m);
         pos = cv.take<T>((size_t)3 * n_dense);
         kept = cv.take<int>((size_t)n_dense);
-    };
-    carve(measure);
-    PCU_TRY(adopt_stream(ws, stream));
-    PCU_TRY(grow_block(ws->mesh, ws->mesh_bytes, measure.off, stream, "mesh-sampling scratch"));
-    Carver cv(ws->mesh);
-    carve(cv);
+    }));
     PCU_TRY(enqueue_mesh_cdf<T>(ws, v, nv, f, fkind, m, ms.cdf, ms.tiles, ms.sc, ms.area, stream));
     const unsigned blocks = (unsigned)std::min<long long>((n_dense + kThreads - 1) / kThreads, (long long)ws->sm_count * 16);
     PCU_LAUNCH((mesh_sample_kernel<T>), blocks, kThreads, stream, (const unsigned long long*)ms.cdf, m, (const MeshArea*)ms.area,
@@ -1231,10 +1214,9 @@ int dedup_device(pcu_b200_workspace* ws, const T* pts, long long n, double epsil
     const long long nblocks = (n + kThreads - 1) / kThreads;
     const long long fblocks = faces ? (nf + kThreads - 1) / kThreads : 0;
     const unsigned ntiles = (unsigned)((n + kSortTile - 1) / kSortTile);
-    Carver measure(nullptr);
-    struct Scratch { Rec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; unsigned char* head;
-                     unsigned* counts; unsigned char* fkeep; unsigned* fcounts; unsigned* bad; } sc;
-    auto carve = [&](Carver& cv) {
+    struct { Rec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; unsigned char* head;
+             unsigned* counts; unsigned char* fkeep; unsigned* fcounts; unsigned* bad; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
         sc.a = cv.take<Rec>((size_t)n);
         sc.b = cv.take<Rec>((size_t)n);
         sc.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
@@ -1246,11 +1228,7 @@ int dedup_device(pcu_b200_workspace* ws, const T* pts, long long n, double epsil
         sc.fkeep = cv.take<unsigned char>((size_t)std::max<long long>(1, nf));
         sc.fcounts = cv.take<unsigned>((size_t)std::max<long long>(1, fblocks));
         sc.bad = cv.take<unsigned>(1);
-    };
-    carve(measure);
-    PCU_TRY(ensure_arena(ws, measure.off, stream));
-    Carver cv(ws->arena);
-    carve(cv);
+    }));
     PCU_CUDA(cudaMemsetAsync(out_counts, 0, 3 * sizeof(long long), stream));
     PCU_LAUNCH((dedup_keys_kernel<T>), (unsigned)nblocks, kThreads, stream, pts, n, (T)epsilon, sc.a);
     Rec* sorted = nullptr;
@@ -1326,8 +1304,8 @@ int morton_knn_device(pcu_b200_workspace* ws, const unsigned long long* codes, l
 }
 
 // ---- prepared clouds ---------------------------------------------------------------------------------------
-// Bins `points` once into a private block: the layout of an ordinary plan whose second cloud is a one-point
-// dummy, with only the first cloud binned; the handle keeps that cloud's descriptor.
+// Bins a copy of `points` once into a private block (the one-cloud plan of one_cloud_spec); the handle keeps that
+// cloud's descriptor.
 template <typename T>
 int cloud_prepare_device(pcu_b200_workspace* ws, const T* points, long long n, pcu_b200_cloud** out, cudaStream_t stream,
                          int knn_k = 1, int leaf = 0) {
@@ -1337,43 +1315,36 @@ int cloud_prepare_device(pcu_b200_workspace* ws, const T* points, long long n, p
     if (leaf < 0) return fail(PCU_B200_INVALID_ARGUMENT, "max_points_per_leaf must be >= 0");
     PCU_TRY(check_cloud_args<T>(points, n, points, 1));
     PCU_ON_DEVICE(ws);
-    PlanSpec<T> spec;
-    spec.a = points; spec.n = n; spec.b = points; spec.m = 1;
-    spec.nsweeps = 1; spec.k = 1;
-    spec.occupancy = occupancy_for(ws, knn_k);   // the cell size the searches with this k want
-    spec.prepared_second = true;      // (also keeps the dummy out of the one-CTA build)
-    Plan<T> plan;
-    plan.layout(nullptr, spec);
-    const size_t raw_bytes = align_up(sizeof(T) * 3 * (size_t)n);
-    size_t tree_bytes = 0;
-    if (leaf > 0) {
-        Carver measure(nullptr);
-        KdReplayBuffers<T> probe;
-        probe.carve(measure, n);
-        tree_bytes = measure.off;
-    }
     pcu_b200_cloud* c = new (std::nothrow) pcu_b200_cloud();
     if (!c) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
-    c->device = ws->device; c->is_f64 = sizeof(T) == 8 ? 1 : 0; c->n = n; c->bytes = plan.total + raw_bytes + tree_bytes;
-    c->knn_k = knn_k;
-    cudaError_t e = cudaMalloc((void**)&c->block, c->bytes);
+    c->device = ws->device; c->is_f64 = sizeof(T) == 8 ? 1 : 0; c->n = n; c->knn_k = knn_k;
+    // the block: the handle's own copy of the points, the plan that bins that copy (at the cell size the searches with
+    // this k want), and with a leaf size the reference tree
+    PlanSpec<T> spec = one_cloud_spec<T>(nullptr, n, occupancy_for(ws, knn_k));
+    Plan<T> plan;
+    T* raw_copy = nullptr;
+    auto carve = [&](Carver& cv) {
+        raw_copy = cv.take<T>((size_t)3 * n);
+        spec.a = spec.b = raw_copy;
+        plan.layout(cv, spec);
+        if (leaf > 0) cloud_tree<T>(c).carve(cv, n);
+    };
+    const size_t bytes = carve_at(nullptr, carve);
+    c->bytes = bytes;
+    cudaError_t e = cudaMalloc((void**)&c->block, bytes);
     if (e != cudaSuccess) {
         cudaGetLastError();
         delete c;
-        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMalloc of %zu bytes for a prepared cloud failed: %s", plan.total + raw_bytes, cudaGetErrorString(e));
+        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMalloc of %zu bytes for a prepared cloud failed: %s", bytes, cudaGetErrorString(e));
     }
-    T* raw_copy = reinterpret_cast<T*>(c->block + plan.total);
+    carve_at(c->block, carve);
     auto bail = [&](int status) { cudaFree(c->block); delete c; return status; };
     if (cudaMemcpyAsync(raw_copy, points, sizeof(T) * 3 * n, cudaMemcpyDeviceToDevice, stream) != cudaSuccess)
         return bail(fail(PCU_B200_CUDA_ERROR, "copy of the points failed: %s", cudaGetErrorString(cudaGetLastError())));
-    spec.a = raw_copy; spec.b = raw_copy;
-    plan.layout(c->block, spec);
     const int st = enqueue_binning(ws, plan, stream, nullptr, true);
     if (st != PCU_B200_OK) return bail(st);
     if (leaf > 0) {   // the full reference tree, once: k-NN calls against the handle only replay their tied rows on it
-        Carver cv(c->block + plan.total + raw_bytes);
         KdReplayBuffers<T>& tree = cloud_tree<T>(c);
-        tree.carve(cv, n);
         const int ts = build_kd_replica<T>(tree, raw_copy, n, leaf, nullptr, KdPrune<T>{}, stream, g_launches);
         if (ts != PCU_B200_OK) return bail(fail(ts, "building the reference tree failed: %s", cudaGetErrorString(cudaGetLastError())));
         c->leaf = leaf;
@@ -1407,20 +1378,15 @@ int voxel_downsample_device(pcu_b200_workspace* ws, const T* pts, long long n, c
     const long long nblocks = (n + kThreads - 1) / kThreads;
     unsigned slots = 64;
     while ((long long)slots < 2 * n) slots <<= 1;     // load factor <= 1/2
-    Carver measure(nullptr);
-    auto carve = [&](Carver& cv, int*& table, VoxelAcc*& acc, int*& slot_of, double*& attr_sum, unsigned char*& keep, unsigned*& counts) {
+    int *table, *slot_of; VoxelAcc* acc; double* attr_sum; unsigned char* keep; unsigned* counts;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
         table = cv.take<int>(slots);
         acc = cv.take<VoxelAcc>(slots);
         slot_of = cv.take<int>((size_t)n);
         attr_sum = cv.take<double>((size_t)slots * (attr_cols > 0 ? attr_cols : 0) + 1);
         keep = cv.take<unsigned char>((size_t)n);
         counts = cv.take<unsigned>((size_t)nblocks);
-    };
-    int *table, *slot_of; VoxelAcc* acc; double* attr_sum; unsigned char* keep; unsigned* counts;
-    carve(measure, table, acc, slot_of, attr_sum, keep, counts);
-    PCU_TRY(ensure_arena(ws, measure.off, stream));
-    Carver cv(ws->arena);
-    carve(cv, table, acc, slot_of, attr_sum, keep, counts);
+    }));
     PCU_LAUNCH(voxel_init_kernel, (slots + kThreads - 1) / kThreads, kThreads, stream, table, acc, slots);
     if (attr_cols > 0) PCU_CUDA(cudaMemsetAsync(attr_sum, 0, sizeof(double) * (size_t)slots * attr_cols, stream));
     PCU_LAUNCH((voxel_insert_kernel<T, A>), (unsigned)nblocks, kThreads, stream, pts, n, g, table, slots, acc, slot_of, attr, attr_cols, attr_sum);
@@ -1468,20 +1434,17 @@ int sinkhorn_device(pcu_b200_workspace* ws, const T* a, const T* b, const T* M, 
     if (nb > 65535 || n > 65535) return fail(PCU_B200_INVALID_ARGUMENT, "sinkhorn: at most 65535 batches and rows per launch");
     if (max_iters < 0) return fail(PCU_B200_INVALID_ARGUMENT, "max_iters must be >= 0");
     PCU_ON_DEVICE(ws);
-    Carver measure(nullptr);
-    auto carve = [&](Carver& cv, T*& u, T*& v, double*& eu, double*& ev, int*& flags) {
+    T *u, *v; double *eu, *ev; int* flags;
+    auto carve = [&](Carver& cv) {
         u = cv.take<T>((size_t)nb * n);
         v = cv.take<T>((size_t)nb * m);
         eu = cv.take<double>((size_t)nb);
         ev = cv.take<double>((size_t)nb);
         flags = cv.take<int>(2);   // [0] done, [1] iterations
     };
-    T *u, *v; double *eu, *ev; int* flags;
-    carve(measure, u, v, eu, ev, flags);
-    PCU_TRY(ensure_arena(ws, measure.off, stream));
-    Carver cv(ws->arena);
-    carve(cv, u, v, eu, ev, flags);
-    PCU_CUDA(cudaMemsetAsync(ws->arena, 0, measure.off, stream));   // u = v = 0 (:101-102), accumulators, flags
+    const size_t bytes = carve_at(nullptr, carve);
+    PCU_TRY(carve_scratch(ws, kArena, stream, carve));
+    PCU_CUDA(cudaMemsetAsync(u, 0, bytes, stream));   // u = v = 0 (:101-102), accumulators, flags
     if (out_cost) PCU_CUDA(cudaMemsetAsync(out_cost, 0, sizeof(double) * nb, stream));
     const T e = (T)eps;
     for (int it = 0; it < max_iters; ++it) {
@@ -1655,10 +1618,7 @@ int pcu_b200_workspace_destroy(pcu_b200_workspace* ws) {
     if (!ws) return PCU_B200_OK;
     DeviceGuard guard(ws->device);
     cudaDeviceSynchronize();
-    if (ws->arena) cudaFree(ws->arena);
-    if (ws->io) cudaFree(ws->io);
-    if (ws->aux) cudaFree(ws->aux);
-    if (ws->mesh) cudaFree(ws->mesh);
+    for (auto* b : ws->block) if (b) cudaFree(b);
     if (ws->handover) cudaEventDestroy(ws->handover);
     if (ws->hint_host) cudaFreeHost((void*)ws->hint_host);
     if (ws->own_stream) cudaStreamDestroy(ws->own_stream);
@@ -1672,7 +1632,10 @@ int pcu_b200_workspace_destroy(pcu_b200_workspace* ws) {
 }
 
 int64_t pcu_b200_workspace_bytes(const pcu_b200_workspace* ws) {
-    return ws ? (int64_t)(ws->arena_bytes + ws->io_bytes + ws->aux_bytes + ws->mesh_bytes) : 0;
+    if (!ws) return 0;
+    size_t bytes = 0;
+    for (size_t b : ws->block_bytes) bytes += b;
+    return (int64_t)bytes;
 }
 
 int pcu_b200_workspace_set_profiling(pcu_b200_workspace* ws, int enabled) {
