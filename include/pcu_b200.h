@@ -500,6 +500,11 @@ int pcu_b200_debug_kd_tree_f32(pcu_b200_workspace* ws, const float* points, int6
 int pcu_b200_debug_kd_tree_f64(pcu_b200_workspace* ws, const double* points, int64_t m, int max_points_per_leaf,
                                int32_t* order, int64_t node_cap, int32_t* feat, double* div_lo, double* div_hi,
                                int32_t* first, int32_t* last, int32_t* kid0, int32_t* kid1, int64_t* out_nodes);
+/* pcu_b200_batched_chamfer_f32 that also leaves every pair's two statistics records in out_stats (DEVICE, 2 * batch
+ * records: [2p] = x_p -> y_p, [2p + 1] = y_p -> x_p), so tests can check each pair's sweeps query by query through
+ * their sums.  out_per_pair (DEVICE, batch scalars) as for the batched call; runs the same kernels. */
+int pcu_b200_debug_batched_chamfer_stats_f32(pcu_b200_workspace* ws, const float* x, const float* y, int64_t batch, int64_t n,
+                                             int64_t m, pcu_b200_nn_stats* out_stats, float* out_per_pair, void* stream);
 
 #ifdef __cplusplus
 }

@@ -860,6 +860,14 @@ void batched_chamfer_device(uintptr_t x, uintptr_t y, int64_t B, int64_t n, int6
     });
 }
 
+void batched_chamfer_stats_device(uintptr_t x, uintptr_t y, int64_t B, int64_t n, int64_t m, uintptr_t out_stats,
+                                  uintptr_t out_per_pair, int max_points_per_leaf, int device, uintptr_t stream) {
+    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_debug_batched_chamfer_stats_f32(ws, (const float*)x, (const float*)y, B, n, m, (pcu_b200_nn_stats*)out_stats,
+                                                        (float*)out_per_pair, (void*)stream);
+    });
+}
+
 template <typename T>
 py::dict debug_kd_tree_t(const py::array& pts_in, int leaf, int device) {
     auto pts = dense<T>(pts_in);
@@ -961,6 +969,7 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_batched_chamfer", &batched_chamfer_numpy, py::arg("x"), py::arg("y"), py::arg("max_points_per_leaf") = 10,
             py::arg("device") = -1);
     mod.def("_batched_chamfer_device", &batched_chamfer_device);
+    mod.def("_batched_chamfer_stats_device", &batched_chamfer_stats_device);
     mod.def("_knn_device", &knn_device);
     mod.def("_stats_device", &stats_device);
     mod.def("_resolve_witness_device", &resolve_witness_device);

@@ -1458,9 +1458,11 @@ int sinkhorn_device(pcu_b200_workspace* ws, const T* a, const T* b, const T* M, 
 }
 
 // ---- batched Chamfer ---------------------------------------------------------------------------
+// out_stats (diagnostic, may be null): 2 * batch device records that receive every pair's two sweeps in place
+// of the ones carved from the arena.
 template <typename T>
 int batched_chamfer_device(pcu_b200_workspace* ws, const T* x, const T* y, long long batch, long long n, long long m,
-                           T* out_per_pair, double* out_sum, cudaStream_t stream) {
+                           T* out_per_pair, double* out_sum, cudaStream_t stream, pcu_b200_nn_stats* out_stats = nullptr) {
     if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
     if (batch <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "batch must be positive (got %lld)", batch);
     PCU_TRY(check_cloud_args<T>(x, n, y, m));
@@ -1474,6 +1476,7 @@ int batched_chamfer_device(pcu_b200_workspace* ws, const T* x, const T* y, long 
         spec.batch = B;
         spec.a = x + first * 3 * n; spec.n = n; spec.b = y + first * 3 * m; spec.m = m;
         spec.nsweeps = 2; spec.k = 1; spec.want_stats = true;
+        spec.stats = out_stats ? out_stats + 2 * first : nullptr;
         spec.occupancy = occupancy_for(ws, 1);
         spec.binning = ws->opts.binning;
         Plan<T> plan;
@@ -1936,6 +1939,12 @@ int pcu_b200_debug_kd_times(pcu_b200_workspace* ws, uint64_t* out40) {
 int pcu_b200_batched_chamfer_f32(pcu_b200_workspace* ws, const float* x, const float* y, int64_t batch, int64_t n,
                                  int64_t m, float* out_per_pair, double* out_sum, void* stream) {
     return batched_chamfer_device<float>(ws, x, y, batch, n, m, out_per_pair, out_sum, (cudaStream_t)stream);
+}
+
+int pcu_b200_debug_batched_chamfer_stats_f32(pcu_b200_workspace* ws, const float* x, const float* y, int64_t batch, int64_t n,
+                                             int64_t m, pcu_b200_nn_stats* out_stats, float* out_per_pair, void* stream) {
+    if (!out_stats) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    return batched_chamfer_device<float>(ws, x, y, batch, n, m, out_per_pair, nullptr, (cudaStream_t)stream, out_stats);
 }
 
 }  // extern "C"
