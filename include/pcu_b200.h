@@ -384,6 +384,20 @@ int pcu_b200_interpolate_barycentric_f64(pcu_b200_workspace* ws, const void* f, 
                                          int fi_kind, const void* bc, int bc_is_f64, const void* attribute, int attribute_is_f64,
                                          int64_t nv, int64_t dim, double* out, uint64_t* out_bad, void* stream);
 
+/* ---- closest points on a mesh ---------------------------------------------------------------------------------
+ * Replaces closest_points_on_mesh (src/closest_point_on_mesh.cpp, libigl's AABB tree).  For each query p_i (np rows,
+ * np >= 0): out_d[i] = sqrt(d^2), out_fidx[i] (f's width: 4 bytes for I32 / U32, 8 for I64 / U64) and out_bc[i, 0:3]
+ * of the face that minimises (d^2, face index) lexicographically, d^2 and bc from the Voronoi-region closest point on
+ * each face in the vertices' precision with every operation rounded on its own (DESIGN.md §3, csrc/meshquery.cuh).
+ * Faces with a corner outside [0, nv) are left out and counted in *out_bad (device uint64); when it is not zero the
+ * outputs are unspecified.  Every pointer is a DEVICE pointer and the call is stream-ordered. */
+int pcu_b200_closest_points_on_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
+                                        int64_t nf, int f_kind, float* out_d, void* out_fidx, float* out_bc, uint64_t* out_bad,
+                                        void* stream);
+int pcu_b200_closest_points_on_mesh_f64(pcu_b200_workspace* ws, const double* p, int64_t np, const double* v, int64_t nv, const void* f,
+                                        int64_t nf, int f_kind, double* out_d, void* out_fidx, double* out_bc, uint64_t* out_bad,
+                                        void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

@@ -1,0 +1,438 @@
+// meshquery.cuh -- closest points on a triangle mesh (closest_points_on_mesh of the reference,
+// src/closest_point_on_mesh.cpp, which walks libigl's AABB tree).
+//
+// The result is defined exactly (DESIGN.md §3, point-to-mesh distance) as a pure function of (p, v, f):
+//   per (query, face)  the Voronoi-region closest point of Ericson, Real-Time Collision Detection §5.1.5, in the input
+//                      precision T with every operation rounded on its own (closest_on_face below); faces whose
+//                      interior denominator D = (e1.e1)(e2.e2) - (e1.e2)^2 is not positive are the union of their edges.
+//   per query          the lexicographic minimum of (d^2, face index) over the faces with every corner in [0, #v);
+//                      d = sqrt(d^2) rounded once, bc the chosen face's coordinates.
+// So neither the tree's shape, nor the sort, nor thread scheduling can change a result.
+//
+// The tree is a linear BVH (Karras 2012) built per call over the valid faces:
+//   mq_bounds_kernel    scene box of the face boxes, count of faces with a corner out of range
+//   mq_codes_kernel     63-bit Morton code of each face's box centre over the scene box (invalid faces: ~0, last)
+//   (sort.cuh)          stable radix sort of (code, face): equal codes stay in face order
+//   mq_leaves_kernel    corners packed in leaf order (face id and degeneracy in the spare lanes), leaf boxes
+//   mq_nodes_kernel     Karras's internal nodes; equal codes are split by position (delta = 64 + clz(i ^ j))
+//   mq_refit_kernel     bottom-up boxes with per-node arrival counters: the second child to arrive writes both
+//                       children's boxes into the parent (one 64-byte record per visit)
+//   mq_query_kernel     one thread per query: nearer child first, the other pushed; pruning with the margin of §3.
+#pragma once
+#include "common.cuh"
+#include "meshsample.cuh"
+#include "morton.cuh"
+#include "sort.cuh"
+
+namespace pcu {
+
+using MqRec = SortRec<unsigned long long, 1>;
+
+// Tree depth bound: along a root-to-leaf path the nodes' common-prefix lengths strictly increase.  They lie in
+// [1, 63] for distinct codes (codes are < 2^63, so two of them share at least the top bit) and in [65, 95] for equal
+// codes (64 + clz(i ^ j) with 0 < i ^ j < 2^31), so a path has at most 63 + 31 = 94 internal nodes.  Traversal pushes
+// at most one node per internal node of the current path, so this stack cannot overflow.
+constexpr int kMqStack = 96;
+
+// Both children of an internal node: their boxes (fp32, rounded outward and widened, §3) and their ids (>= 0: internal
+// node, < 0: ~leaf position).
+struct __align__(16) MqNode {
+    float lo0[3], hi0[3], lo1[3], hi1[3];
+    int c0, c1, pad0, pad1;
+};
+struct MqBox { float lo[3], hi[3]; };
+
+struct MqScratch {
+    int scene[6];                 // ordered-int images of the scene box (min x y z, max x y z)
+    unsigned long long bad;       // faces with a corner out of range: left out of the tree, counted for the caller
+};
+
+__device__ __forceinline__ int mq_ord(float x) { const int b = __float_as_int(x); return b >= 0 ? b : b ^ 0x7fffffff; }
+__device__ __forceinline__ float mq_unord(int b) { return __int_as_float(b >= 0 ? b : b ^ 0x7fffffff); }
+
+// The face's corners when all three are in range.
+template <typename T>
+__device__ __forceinline__ bool mq_corners(const T* v, long long nv, const void* f, int fkind, long long t, double a[3],
+                                           double b[3], double c[3]) {
+    const long long i0 = load_index(f, 3 * t, fkind, nv, false), i1 = load_index(f, 3 * t + 1, fkind, nv, false),
+                    i2 = load_index(f, 3 * t + 2, fkind, nv, false);
+    if (i0 < 0 || i1 < 0 || i2 < 0) return false;
+    load_vertex<T>(v, i0, a); load_vertex<T>(v, i1, b); load_vertex<T>(v, i2, c);
+    return true;
+}
+
+// The face's box, widened by mu = 16 u M per side (u: unit roundoff of T, M: largest corner magnitude) and rounded
+// outward to fp32.  DESIGN.md §3 shows that every closest point closest_on_face computes lies inside it.
+template <typename T>
+__device__ __forceinline__ MqBox mq_face_box(const double a[3], const double b[3], const double c[3]) {
+    const double u = sizeof(T) == 4 ? 0x1p-24 : 0x1p-53;
+    double M = 0.0;
+    for (int k = 0; k < 3; ++k) M = fmax(M, fmax(fabs(a[k]), fmax(fabs(b[k]), fabs(c[k]))));
+    const double mu = M * (16.0 * u);
+    MqBox bx;
+    for (int k = 0; k < 3; ++k) {
+        bx.lo[k] = __double2float_rd(__dsub_rd(fmin(a[k], fmin(b[k], c[k])), mu));
+        bx.hi[k] = __double2float_ru(__dadd_ru(fmax(a[k], fmax(b[k], c[k])), mu));
+    }
+    return bx;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mq_bounds_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f,
+                                                             int fkind, long long m, MqScratch* __restrict__ sc) {
+    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
+    unsigned long long bad = 0;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < m; t += (long long)gridDim.x * blockDim.x) {
+        double a[3], b[3], c[3];
+        if (!mq_corners<T>(v, nv, f, fkind, t, a, b, c)) { ++bad; continue; }
+        const MqBox bx = mq_face_box<T>(a, b, c);
+        for (int k = 0; k < 3; ++k) { lo[k] = min(lo[k], mq_ord(bx.lo[k])); hi[k] = max(hi[k], mq_ord(bx.hi[k])); }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+        for (int k = 0; k < 3; ++k) {
+            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
+            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
+        }
+        bad += __shfl_xor_sync(0xffffffffu, bad, o);
+    }
+    if ((threadIdx.x & 31) == 0) {
+        for (int k = 0; k < 3; ++k) { atomicMin(&sc->scene[k], lo[k]); atomicMax(&sc->scene[3 + k], hi[k]); }
+        if (bad) atomicAdd(&sc->bad, bad);
+    }
+}
+
+// Record t = (code of face t, t).  The box centre is quantised to 21 bits per axis over the scene box.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mq_codes_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f,
+                                                            int fkind, long long m, const MqScratch* __restrict__ sc,
+                                                            MqRec* __restrict__ recs) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= m) return;
+    unsigned long long code = ~0ull;
+    double a[3], b[3], c[3];
+    if (mq_corners<T>(v, nv, f, fkind, t, a, b, c)) {
+        const MqBox bx = mq_face_box<T>(a, b, c);
+        code = 0;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const float slo = mq_unord(sc->scene[k]), shi = mq_unord(sc->scene[3 + k]);
+            const float ext = shi - slo;
+            const float centre = 0.5f * bx.lo[k] + 0.5f * bx.hi[k];
+            const float s = ext > 0.f ? __fdividef(centre - slo, ext) * 2097152.f : 0.f;   // only orders the leaves
+            code |= morton_split21((int)fminf(fmaxf(s, 0.f), 2097151.f)) << k;   // NaN -> 0
+        }
+    }
+    *reinterpret_cast<ulonglong2*>(recs + t) = make_ulonglong2(code, (unsigned long long)t);   // {key[0], idx}
+}
+
+// Leaf i (i < valid = m - bad): its face's corners as three Pt<T> (lane i: face id in the first, 1 for a degenerate
+// face in the second) and its box.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mq_leaves_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f,
+                                                             int fkind, long long m, const MqScratch* __restrict__ sc,
+                                                             const MqRec* __restrict__ sorted, Pt<T>* __restrict__ leaves,
+                                                             MqBox* __restrict__ boxes) {
+    using R = Real<T>;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m - (long long)sc->bad) return;
+    const long long t = (long long)sorted[i].idx;
+    double a[3], b[3], c[3];
+    mq_corners<T>(v, nv, f, fkind, t, a, b, c);
+    boxes[i] = mq_face_box<T>(a, b, c);
+    const T ax = (T)a[0], ay = (T)a[1], az = (T)a[2];
+    const T e1x = R::sub((T)b[0], ax), e1y = R::sub((T)b[1], ay), e1z = R::sub((T)b[2], az);
+    const T e2x = R::sub((T)c[0], ax), e2y = R::sub((T)c[1], ay), e2z = R::sub((T)c[2], az);
+    const T d00 = R::add(R::add(R::mul(e1x, e1x), R::mul(e1y, e1y)), R::mul(e1z, e1z));
+    const T d11 = R::add(R::add(R::mul(e2x, e2x), R::mul(e2y, e2y)), R::mul(e2z, e2z));
+    const T d01 = R::add(R::add(R::mul(e1x, e2x), R::mul(e1y, e2y)), R::mul(e1z, e2z));
+    const T D = R::sub(R::mul(d00, d11), R::mul(d01, d01));
+    Pt<T> pa, pb, pc;
+    pa.x = ax; pa.y = ay; pa.z = az; pa.i = (typename Real<T>::index_t)t;
+    pb.x = (T)b[0]; pb.y = (T)b[1]; pb.z = (T)b[2]; pb.i = D > (T)0 ? 0 : 1;
+    pc.x = (T)c[0]; pc.y = (T)c[1]; pc.z = (T)c[2]; pc.i = 0;
+    leaves[3 * i] = pa; leaves[3 * i + 1] = pb; leaves[3 * i + 2] = pc;
+}
+
+__device__ __forceinline__ int mq_delta(const MqRec* __restrict__ recs, long long n, long long i, unsigned long long ci, long long j) {
+    if (j < 0 || j >= n) return -1;
+    const unsigned long long cj = recs[j].key[0];
+    return ci == cj ? 64 + __clz((int)(i ^ j)) : __clzll((long long)(ci ^ cj));
+}
+
+// Karras 2012, internal node i of n - 1 (n = valid leaves); node 0 is the root.
+__global__ void __launch_bounds__(kThreads) mq_nodes_kernel(const MqRec* __restrict__ recs, long long m, const MqScratch* __restrict__ sc,
+                                                            MqNode* __restrict__ nodes, int* __restrict__ node_parent,
+                                                            int* __restrict__ leaf_parent) {
+    const long long n = m - (long long)sc->bad;   // < 2^31
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n - 1) return;
+    const unsigned long long ci = recs[i].key[0];
+    const int d = mq_delta(recs, n, i, ci, i + 1) - mq_delta(recs, n, i, ci, i - 1) >= 0 ? 1 : -1;
+    const int dmin = mq_delta(recs, n, i, ci, i - d);
+    long long lmax = 2;
+    while (mq_delta(recs, n, i, ci, i + lmax * d) > dmin) lmax <<= 1;
+    long long l = 0;
+    for (long long t = lmax >> 1; t >= 1; t >>= 1)
+        if (mq_delta(recs, n, i, ci, i + (l + t) * d) > dmin) l += t;
+    const int dnode = mq_delta(recs, n, i, ci, i + l * d);
+    long long s = 0;
+    for (int k = 1; k < 33; ++k) {                 // t = ceil(l / 2^k) down to 1
+        const long long t = (l + (1ll << k) - 1) >> k;
+        if (mq_delta(recs, n, i, ci, i + (s + t) * d) > dnode) s += t;
+        if (t <= 1) break;
+    }
+    const int gamma = (int)(i + s * d) + (d < 0 ? -1 : 0);
+    const int c0 = (d < 0 ? i - l : i) == gamma ? ~gamma : gamma;             // the range's ends are min / max(i, j)
+    const int c1 = (d < 0 ? i : i + l) == gamma + 1 ? ~(gamma + 1) : gamma + 1;
+    nodes[i].c0 = c0;
+    nodes[i].c1 = c1;
+    if (c0 < 0) leaf_parent[~c0] = (int)i; else node_parent[c0] = (int)i;
+    if (c1 < 0) leaf_parent[~c1] = (int)i; else node_parent[c1] = (int)i;
+}
+
+__device__ __forceinline__ MqBox mq_child_box(const MqNode* nodes, const MqBox* boxes, int c) {
+    if (c < 0) return boxes[~c];
+    const float4* p = reinterpret_cast<const float4*>(nodes + c);
+    const float4 q0 = __ldcg(p), q1 = __ldcg(p + 1), q2 = __ldcg(p + 2);   // written by other threads of this launch
+    MqBox b;
+    b.lo[0] = fminf(q0.x, q1.z); b.lo[1] = fminf(q0.y, q1.w); b.lo[2] = fminf(q0.z, q2.x);
+    b.hi[0] = fmaxf(q0.w, q2.y); b.hi[1] = fmaxf(q1.x, q2.z); b.hi[2] = fmaxf(q1.y, q2.w);
+    return b;
+}
+
+// One thread per leaf climbs towards the root; at each node the first arrival stops and the second, which finds both
+// children's boxes complete, writes them into the node.
+__global__ void __launch_bounds__(kThreads) mq_refit_kernel(long long m, const MqScratch* __restrict__ sc, MqNode* nodes,
+                                                            const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
+                                                            const MqBox* __restrict__ boxes, int* __restrict__ arrivals) {
+    const long long n = m - (long long)sc->bad;
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (n < 2 || i >= n) return;
+    int node = leaf_parent[i];
+    while (true) {
+        __threadfence();
+        if (atomicAdd(&arrivals[node], 1) == 0) return;
+        const int c0 = nodes[node].c0, c1 = nodes[node].c1;
+        const MqBox b0 = mq_child_box(nodes, boxes, c0), b1 = mq_child_box(nodes, boxes, c1);
+        float4* p = reinterpret_cast<float4*>(nodes + node);
+        p[0] = make_float4(b0.lo[0], b0.lo[1], b0.lo[2], b0.hi[0]);
+        p[1] = make_float4(b0.hi[1], b0.hi[2], b1.lo[0], b1.lo[1]);
+        p[2] = make_float4(b1.lo[2], b1.hi[0], b1.hi[1], b1.hi[2]);
+        if (node == 0) return;
+        node = node_parent[node];
+    }
+}
+
+// ---- the per-(query, face) definition (DESIGN.md §3) ---------------------------------------------------------------
+template <typename T>
+struct MqHit { T d2, b0, b1, b2; };
+
+template <typename T>
+__device__ __forceinline__ T mq_dot(T ux, T uy, T uz, T wx, T wy, T wz) {
+    using R = Real<T>;
+    return R::add(R::add(R::mul(ux, wx), R::mul(uy, wy)), R::mul(uz, wz));
+}
+template <typename T>
+__device__ __forceinline__ T mq_div(T a, T b);
+template <> __device__ __forceinline__ float mq_div<float>(float a, float b) { return __fdiv_rn(a, b); }
+template <> __device__ __forceinline__ double mq_div<double>(double a, double b) { return __ddiv_rn(a, b); }
+
+// d^2 = ((px - cx)^2 + (py - cy)^2) + (pz - cz)^2
+template <typename T>
+__device__ __forceinline__ T mq_d2(const T p[3], T cx, T cy, T cz) {
+    using R = Real<T>;
+    const T dx = R::sub(p[0], cx), dy = R::sub(p[1], cy), dz = R::sub(p[2], cz);
+    return R::add(R::add(R::mul(dx, dx), R::mul(dy, dy)), R::mul(dz, dz));
+}
+
+// Closest point of segment [x, y]: e = y - x, l = e.e; t = 0 when l is not positive, else (p - x).e / l clamped to
+// [0, 1]; the point is x at t = 0, y at t = 1, else x + t e.  Returns d^2 and t.
+template <typename T>
+__device__ __forceinline__ T mq_segment(const T p[3], const T x[3], const T y[3], T& t) {
+    using R = Real<T>;
+    const T ex = R::sub(y[0], x[0]), ey = R::sub(y[1], x[1]), ez = R::sub(y[2], x[2]);
+    const T l = mq_dot<T>(ex, ey, ez, ex, ey, ez);
+    t = (T)0;
+    if (l > (T)0) {
+        t = mq_div<T>(mq_dot<T>(R::sub(p[0], x[0]), R::sub(p[1], x[1]), R::sub(p[2], x[2]), ex, ey, ez), l);
+        t = t < (T)0 ? (T)0 : (t > (T)1 ? (T)1 : t);
+    }
+    if (t == (T)0) return mq_d2<T>(p, x[0], x[1], x[2]);
+    if (t == (T)1) return mq_d2<T>(p, y[0], y[1], y[2]);
+    return mq_d2<T>(p, R::add(x[0], R::mul(t, ex)), R::add(x[1], R::mul(t, ey)), R::add(x[2], R::mul(t, ez)));
+}
+
+// A degenerate face: the closest of its edges AB, BC, CA (the first on ties).
+template <typename T>
+__device__ __forceinline__ MqHit<T> mq_edges(const T p[3], const T a[3], const T b[3], const T c[3]) {
+    using R = Real<T>;
+    T t;
+    MqHit<T> h;
+    h.d2 = mq_segment<T>(p, a, b, t); h.b0 = R::sub((T)1, t); h.b1 = t; h.b2 = (T)0;
+    T d2 = mq_segment<T>(p, b, c, t);
+    if (d2 < h.d2) { h.d2 = d2; h.b0 = (T)0; h.b1 = R::sub((T)1, t); h.b2 = t; }
+    d2 = mq_segment<T>(p, c, a, t);
+    if (d2 < h.d2) { h.d2 = d2; h.b0 = t; h.b1 = (T)0; h.b2 = R::sub((T)1, t); }
+    return h;
+}
+
+// n / d for an edge parameter: d >= n >= 0 here, and d = 0 only when n = 0 too.
+template <typename T>
+__device__ __forceinline__ T mq_ratio(T n, T d) { return d > (T)0 ? mq_div<T>(n, d) : (T)0; }
+
+// Ericson's closest point on triangle abc, regions in his order: vertex A, vertex B, edge AB, vertex C, edge AC,
+// edge BC, interior.  The interior is taken only when s = (va + vb) + vc > 0 and v = vb / s, w = vc / s satisfy
+// v >= 0, w >= 0, v + w <= 1; otherwise, and for degenerate faces, the face is the union of its edges.
+template <typename T>
+__device__ __forceinline__ MqHit<T> closest_on_face(const T p[3], const T a[3], const T b[3], const T c[3], bool degenerate) {
+    using R = Real<T>;
+    if (degenerate) return mq_edges<T>(p, a, b, c);
+    const T abx = R::sub(b[0], a[0]), aby = R::sub(b[1], a[1]), abz = R::sub(b[2], a[2]);
+    const T acx = R::sub(c[0], a[0]), acy = R::sub(c[1], a[1]), acz = R::sub(c[2], a[2]);
+    MqHit<T> h;
+    const T apx = R::sub(p[0], a[0]), apy = R::sub(p[1], a[1]), apz = R::sub(p[2], a[2]);
+    const T d1 = mq_dot<T>(abx, aby, abz, apx, apy, apz), d2 = mq_dot<T>(acx, acy, acz, apx, apy, apz);
+    if (d1 <= (T)0 && d2 <= (T)0) {
+        h.d2 = mq_d2<T>(p, a[0], a[1], a[2]); h.b0 = (T)1; h.b1 = (T)0; h.b2 = (T)0;
+        return h;
+    }
+    const T bpx = R::sub(p[0], b[0]), bpy = R::sub(p[1], b[1]), bpz = R::sub(p[2], b[2]);
+    const T d3 = mq_dot<T>(abx, aby, abz, bpx, bpy, bpz), d4 = mq_dot<T>(acx, acy, acz, bpx, bpy, bpz);
+    if (d3 >= (T)0 && d4 <= d3) {
+        h.d2 = mq_d2<T>(p, b[0], b[1], b[2]); h.b0 = (T)0; h.b1 = (T)1; h.b2 = (T)0;
+        return h;
+    }
+    const T vc = R::sub(R::mul(d1, d4), R::mul(d3, d2));
+    if (vc <= (T)0 && d1 >= (T)0 && d3 <= (T)0) {
+        const T v = mq_ratio<T>(d1, R::sub(d1, d3));
+        h.d2 = mq_d2<T>(p, R::add(a[0], R::mul(v, abx)), R::add(a[1], R::mul(v, aby)), R::add(a[2], R::mul(v, abz)));
+        h.b0 = R::sub((T)1, v); h.b1 = v; h.b2 = (T)0;
+        return h;
+    }
+    const T cpx = R::sub(p[0], c[0]), cpy = R::sub(p[1], c[1]), cpz = R::sub(p[2], c[2]);
+    const T d5 = mq_dot<T>(abx, aby, abz, cpx, cpy, cpz), d6 = mq_dot<T>(acx, acy, acz, cpx, cpy, cpz);
+    if (d6 >= (T)0 && d5 <= d6) {
+        h.d2 = mq_d2<T>(p, c[0], c[1], c[2]); h.b0 = (T)0; h.b1 = (T)0; h.b2 = (T)1;
+        return h;
+    }
+    const T vb = R::sub(R::mul(d5, d2), R::mul(d1, d6));
+    if (vb <= (T)0 && d2 >= (T)0 && d6 <= (T)0) {
+        const T w = mq_ratio<T>(d2, R::sub(d2, d6));
+        h.d2 = mq_d2<T>(p, R::add(a[0], R::mul(w, acx)), R::add(a[1], R::mul(w, acy)), R::add(a[2], R::mul(w, acz)));
+        h.b0 = R::sub((T)1, w); h.b1 = (T)0; h.b2 = w;
+        return h;
+    }
+    const T va = R::sub(R::mul(d3, d6), R::mul(d5, d4));
+    const T e43 = R::sub(d4, d3), e56 = R::sub(d5, d6);
+    if (va <= (T)0 && e43 >= (T)0 && e56 >= (T)0) {
+        const T w = mq_ratio<T>(e43, R::add(e43, e56));
+        const T bcx = R::sub(c[0], b[0]), bcy = R::sub(c[1], b[1]), bcz = R::sub(c[2], b[2]);
+        h.d2 = mq_d2<T>(p, R::add(b[0], R::mul(w, bcx)), R::add(b[1], R::mul(w, bcy)), R::add(b[2], R::mul(w, bcz)));
+        h.b0 = (T)0; h.b1 = R::sub((T)1, w); h.b2 = w;
+        return h;
+    }
+    const T s = R::add(R::add(va, vb), vc);
+    if (s > (T)0) {
+        const T v = mq_div<T>(vb, s), w = mq_div<T>(vc, s);
+        if (v >= (T)0 && w >= (T)0 && R::add(v, w) <= (T)1) {
+            h.d2 = mq_d2<T>(p, R::add(R::add(a[0], R::mul(abx, v)), R::mul(acx, w)),
+                            R::add(R::add(a[1], R::mul(aby, v)), R::mul(acy, w)),
+                            R::add(R::add(a[2], R::mul(abz, v)), R::mul(acz, w)));
+            h.b0 = R::sub(R::sub((T)1, v), w); h.b1 = v; h.b2 = w;
+            return h;
+        }
+    }
+    return mq_edges<T>(p, a, b, c);
+}
+
+// ---- traversal ------------------------------------------------------------------------------------------------------
+// Lower bound of |p - x|^2 over the fp32 box, rounded down throughout (p enters as [pl, ph] around its fp32 image).
+__device__ __forceinline__ float mq_box_lb(const float pl[3], const float ph[3], const float lo[3], const float hi[3]) {
+    float g[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) g[k] = fmaxf(0.f, fmaxf(__fsub_rd(lo[k], ph[k]), __fsub_rd(pl[k], hi[k])));
+    return __fadd_rd(__fadd_rd(__fmul_rd(g[0], g[0]), __fmul_rd(g[1], g[1])), __fmul_rd(g[2], g[2]));
+}
+// A box may be skipped only when no face in it can have a computed d^2 <= best (DESIGN.md §3): when
+// rd(L (1 - 2^-21)) > ru(ru32(best) + 2^-140).
+__device__ __forceinline__ bool mq_prune(float lb, float limit) { return __fmul_rd(lb, 1.f - 0x1p-21f) > limit; }
+template <typename T>
+__device__ __forceinline__ float mq_limit(T best) {
+    return __fadd_ru(sizeof(T) == 4 ? (float)best : __double2float_ru((double)best), 0x1p-140f);
+}
+
+template <typename T>
+__device__ __forceinline__ void mq_test_leaf(const Pt<T>* __restrict__ leaves, int leaf, const T p[3], T& best, long long& best_face,
+                                             T bb[3], float& limit) {
+    const Pt<T> A = leaves[3 * leaf], B = leaves[3 * leaf + 1], C = leaves[3 * leaf + 2];
+    const T a[3] = {A.x, A.y, A.z}, b[3] = {B.x, B.y, B.z}, c[3] = {C.x, C.y, C.z};
+    const MqHit<T> h = closest_on_face<T>(p, a, b, c, B.i != 0);
+    const long long face = (long long)A.i;
+    if (h.d2 < best || (h.d2 == best && face < best_face)) {
+        best = h.d2; best_face = face; bb[0] = h.b0; bb[1] = h.b1; bb[2] = h.b2;
+        limit = mq_limit<T>(best);
+    }
+}
+
+// Query i in input order.  Nothing is written when the tree is empty (every face invalid: the caller raises).
+// Per visit: one 64-byte node record; per face tested: three Pt<T> (48 B fp32, 96 B fp64).
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mq_query_kernel(const T* __restrict__ q, long long nq, long long m,
+                                                            const MqScratch* __restrict__ sc, const MqNode* __restrict__ nodes,
+                                                            const Pt<T>* __restrict__ leaves, T* __restrict__ out_d,
+                                                            void* __restrict__ out_fidx, int fidx_wide, T* __restrict__ out_bc) {
+    const long long n = m - (long long)sc->bad;
+    if (n < 1) return;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += (long long)gridDim.x * blockDim.x) {
+        const T p[3] = {q[3 * i], q[3 * i + 1], q[3 * i + 2]};
+        float pl[3], ph[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            pl[k] = sizeof(T) == 4 ? (float)p[k] : __double2float_rd((double)p[k]);
+            ph[k] = sizeof(T) == 4 ? (float)p[k] : __double2float_ru((double)p[k]);
+        }
+        T best = Real<T>::inf(), bb[3] = {(T)0, (T)0, (T)0};
+        long long best_face = -1;
+        float limit = __int_as_float(0x7f800000);
+        if (n == 1) {
+            mq_test_leaf<T>(leaves, 0, p, best, best_face, bb, limit);
+        } else {
+            int stack[kMqStack];
+            float stack_lb[kMqStack];
+            int sp = 0, node = 0;
+            while (true) {
+                const float4* np_ = reinterpret_cast<const float4*>(nodes + node);
+                const float4 q0 = __ldg(np_), q1 = __ldg(np_ + 1), q2 = __ldg(np_ + 2), q3 = __ldg(np_ + 3);
+                const float lo0[3] = {q0.x, q0.y, q0.z}, hi0[3] = {q0.w, q1.x, q1.y};
+                const float lo1[3] = {q1.z, q1.w, q2.x}, hi1[3] = {q2.y, q2.z, q2.w};
+                const int c0 = __float_as_int(q3.x), c1 = __float_as_int(q3.y);
+                const float l0 = mq_box_lb(pl, ph, lo0, hi0), l1 = mq_box_lb(pl, ph, lo1, hi1);
+                bool k0 = !mq_prune(l0, limit), k1 = !mq_prune(l1, limit);
+                if (k0 && c0 < 0) { mq_test_leaf<T>(leaves, ~c0, p, best, best_face, bb, limit); k0 = false; }
+                if (k1 && c1 < 0) { mq_test_leaf<T>(leaves, ~c1, p, best, best_face, bb, limit); k1 = false; }
+                if (k0 && k1) {
+                    const bool first0 = l0 <= l1;
+                    stack[sp] = first0 ? c1 : c0;
+                    stack_lb[sp] = first0 ? l1 : l0;
+                    ++sp;
+                    node = first0 ? c0 : c1;
+                    continue;
+                }
+                if (k0) { node = c0; continue; }
+                if (k1) { node = c1; continue; }
+                node = -1;
+                while (sp > 0) {
+                    --sp;
+                    if (!mq_prune(stack_lb[sp], limit)) { node = stack[sp]; break; }
+                }
+                if (node < 0) break;
+            }
+        }
+        // a non-finite query matches no face: it gets d = inf, fi = -1 (unspecified, DESIGN.md §7)
+        out_d[i] = Real<T>::root(best);
+        if (fidx_wide) ((long long*)out_fidx)[i] = best_face; else ((int*)out_fidx)[i] = (int)best_face;
+        out_bc[3 * i] = bb[0]; out_bc[3 * i + 1] = bb[1]; out_bc[3 * i + 2] = bb[2];
+    }
+}
+
+}  // namespace pcu

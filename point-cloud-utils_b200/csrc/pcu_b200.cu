@@ -33,6 +33,7 @@
 #include "dedup.cuh"
 #include "poisson.cuh"
 #include "meshsample.cuh"
+#include "meshquery.cuh"
 
 using namespace pcu;
 
@@ -1259,6 +1260,60 @@ int dedup_dispatch(pcu_b200_workspace* ws, const T* pts, long long n, double eps
     return dedup_device<T, int>(ws, pts, n, epsilon, (const int*)faces, nf, cols, out_pts, out_svi, out_svj, (int*)out_faces, out_counts, stream);
 }
 
+// ---- closest points on a mesh (closest_points_on_mesh, meshquery.cuh) --------------------------------------------
+// Tree over the valid faces, built per call, then one traversal per query.  The count of faces with a corner out of
+// range lands in *out_bad; the caller reads it (the call's one synchronisation) and raises when it is not zero.
+template <typename T>
+int closest_points_device(pcu_b200_workspace* ws, const T* p, long long np, const T* v, long long nv, const void* f, long long m,
+                          int fkind, T* out_d, void* out_fidx, T* out_bc, unsigned long long* out_bad, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (np < 0 || (np > 0 && !p)) return fail(PCU_B200_INVALID_ARGUMENT, "p must be an (n, 3) array");
+    if (!out_bad || (np > 0 && (!out_d || !out_fidx || !out_bc))) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
+    const long long inner = std::max<long long>(1, m - 1);
+    struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; MqScratch* sc;
+             MqNode* nodes; int* node_parent; int* leaf_parent; int* arrivals; Pt<T>* leaves; MqBox* boxes; } s;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        s.a = cv.take<MqRec>((size_t)m);
+        s.b = cv.take<MqRec>((size_t)m);
+        s.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
+        s.totals = cv.take<unsigned long long>(kSortBins);
+        s.base = cv.take<unsigned>(kSortBins);
+        s.constant = cv.take<int>(1);
+        s.sc = cv.take<MqScratch>(1);
+        s.nodes = cv.take<MqNode>((size_t)inner);
+        s.node_parent = cv.take<int>((size_t)inner);
+        s.leaf_parent = cv.take<int>((size_t)m);
+        s.arrivals = cv.take<int>((size_t)inner);
+        s.leaves = cv.take<Pt<T>>((size_t)3 * m);
+        s.boxes = cv.take<MqBox>((size_t)m);
+    }));
+    PCU_CUDA(cudaMemsetAsync(s.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
+    PCU_CUDA(cudaMemsetAsync(s.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
+    PCU_CUDA(cudaMemsetAsync(&s.sc->bad, 0, sizeof(unsigned long long), stream));
+    PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
+    const unsigned fblocks = (unsigned)((m + kThreads - 1) / kThreads);
+    PCU_LAUNCH((mq_bounds_kernel<T>), (unsigned)std::min<long long>(fblocks, (long long)ws->sm_count * 8), kThreads, stream,
+               v, nv, f, fkind, m, s.sc);
+    PCU_LAUNCH((mq_codes_kernel<T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)s.sc, s.a);
+    MqRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records<MqRec>(s.a, s.b, m, 1, s.hist, s.totals, s.base, s.constant, stream, &sorted));
+    PCU_LAUNCH((mq_leaves_kernel<T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)s.sc, (const MqRec*)sorted,
+               s.leaves, s.boxes);
+    PCU_LAUNCH(mq_nodes_kernel, fblocks, kThreads, stream, (const MqRec*)sorted, m, (const MqScratch*)s.sc, s.nodes, s.node_parent,
+               s.leaf_parent);
+    PCU_LAUNCH(mq_refit_kernel, fblocks, kThreads, stream, m, (const MqScratch*)s.sc, s.nodes, (const int*)s.node_parent,
+               (const int*)s.leaf_parent, (const MqBox*)s.boxes, s.arrivals);
+    PCU_CUDA(cudaMemcpyAsync(out_bad, &s.sc->bad, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
+    if (np == 0) return PCU_B200_OK;
+    const unsigned qblocks = (unsigned)std::min<long long>((np + kThreads - 1) / kThreads, (long long)ws->sm_count * 64);
+    PCU_LAUNCH((mq_query_kernel<T>), qblocks, kThreads, stream, p, np, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
+               (const Pt<T>*)s.leaves, out_d, out_fidx, (fkind & 1), out_bc);
+    return PCU_B200_OK;
+}
+
 // ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
 inline unsigned blocks_for(long long n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
@@ -1913,6 +1968,18 @@ int pcu_b200_interpolate_barycentric_f64(pcu_b200_workspace* ws, const void* f, 
                                          int64_t nv, int64_t dim, double* out, uint64_t* out_bad, void* stream) {
     return interpolate_device<double>(ws, f, nf, f_kind, fi, n, fi_kind, bc, bc_is_f64, attribute, attribute_is_f64, nv, dim, out,
                                       (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_closest_points_on_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
+                                        int64_t nf, int f_kind, float* out_d, void* out_fidx, float* out_bc, uint64_t* out_bad,
+                                        void* stream) {
+    return closest_points_device<float>(ws, p, np, v, nv, f, nf, f_kind, out_d, out_fidx, out_bc, (unsigned long long*)out_bad,
+                                        (cudaStream_t)stream);
+}
+int pcu_b200_closest_points_on_mesh_f64(pcu_b200_workspace* ws, const double* p, int64_t np, const double* v, int64_t nv, const void* f,
+                                        int64_t nf, int f_kind, double* out_d, void* out_fidx, double* out_bc, uint64_t* out_bad,
+                                        void* stream) {
+    return closest_points_device<double>(ws, p, np, v, nv, f, nf, f_kind, out_d, out_fidx, out_bc, (unsigned long long*)out_bad,
+                                         (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,
