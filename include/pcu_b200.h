@@ -398,6 +398,30 @@ int pcu_b200_closest_points_on_mesh_f64(pcu_b200_workspace* ws, const double* p,
                                         int64_t nf, int f_kind, double* out_d, void* out_fidx, double* out_bc, uint64_t* out_bad,
                                         void* stream);
 
+/* ---- winding numbers and signed distances to a mesh -------------------------------------------------------------
+ * Replace triangle_soup_fast_winding_number (src/fast_winding_numbers.cpp) and signed_distance_to_mesh
+ * (src/signed_distance.cpp), libigl's fast winding numbers (Barill et al. 2018).  Both build the tree of the closest-point
+ * query over the valid faces, with Barill's order-2 far-field data on every node (DESIGN.md §3, csrc/winding.cuh).
+ *   fast_winding_number: out_w[i] (nq rows) is the winding number at q_i, evaluated in fp32 with an fp64 sum; a node
+ *     whose centre is more than accuracy_scale times its radius from q_i contributes its expansion.  accuracy_scale
+ *     must be positive (the library's functions use 2); +inf evaluates every face exactly.  The result is a function of
+ *     (v, f, q_i) alone.
+ *   signed_distance_to_mesh: out_fidx (int32) and out_bc are those of closest_points_on_mesh; out_s[i] =
+ *     fl(fl(1 - 2|w_i|) d_i), w_i the winding number at accuracy_scale 2.  Queries whose squared distance lies outside
+ *     libigl's band of (lower_bound, upper_bound) get out_s = NaN, out_fidx = nf + 1, out_bc = NaN.
+ * Faces with a corner outside [0, nv) are left out and counted in *out_bad (device uint64); when it is not zero the
+ * outputs are unspecified.  Every pointer is a DEVICE pointer and the call is stream-ordered. */
+int pcu_b200_fast_winding_number_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                     const float* q, int64_t nq, double accuracy_scale, float* out_w, uint64_t* out_bad, void* stream);
+int pcu_b200_fast_winding_number_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                     const double* q, int64_t nq, double accuracy_scale, double* out_w, uint64_t* out_bad, void* stream);
+int pcu_b200_signed_distance_to_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
+                                         int64_t nf, int f_kind, float lower_bound, float upper_bound, float* out_s, int32_t* out_fidx,
+                                         float* out_bc, uint64_t* out_bad, void* stream);
+int pcu_b200_signed_distance_to_mesh_f64(pcu_b200_workspace* ws, const double* p, int64_t np, const double* v, int64_t nv, const void* f,
+                                         int64_t nf, int f_kind, float lower_bound, float upper_bound, double* out_s, int32_t* out_fidx,
+                                         double* out_bc, uint64_t* out_bad, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

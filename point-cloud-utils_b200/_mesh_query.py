@@ -1,5 +1,6 @@
-"""closest_points_on_mesh -- the reference's name, arguments and outputs (the reference's src/closest_point_on_mesh.cpp),
-computed by csrc/meshquery.cuh.
+"""closest_points_on_mesh, triangle_soup_fast_winding_number and signed_distance_to_mesh -- the reference's names,
+arguments and outputs (the reference's src/closest_point_on_mesh.cpp, src/fast_winding_numbers.cpp and
+src/signed_distance.cpp), computed by csrc/meshquery.cuh and csrc/winding.cuh.
 
 Input forms and validation follow _mesh_sampling.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
@@ -20,6 +21,21 @@ def _validate_points(p, v, f):
     if len(p.shape) != 2 or p.shape[1] != 3:
         raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). Got points.shape =%s."
                          % (tuple(p.shape),))
+
+
+def _upload(form, arrays, device):
+    """Contiguous CUDA tensors of the inputs, on the device of the call."""
+    from . import _same_device
+    if form == "cuda":
+        _same_device(arrays[0], device)
+        return [a.detach().contiguous() for a in arrays]
+    return _to_device(arrays, device)
+
+
+def _raise_bad(bad):
+    nbad = int(bad.item())
+    if nbad:
+        raise ValueError("Invalid face indices: %d faces have a corner outside [0, #v)" % nbad)
 
 
 def closest_points_on_mesh(p, v, f, *, device=None):
@@ -63,11 +79,7 @@ def closest_points_on_mesh(p, v, f, *, device=None):
         _same_device(p, device)
         return (torch.zeros(0, dtype=p.dtype, device=p.device), torch.zeros(0, dtype=f.dtype, device=p.device),
                 torch.zeros((0, 3), dtype=p.dtype, device=p.device))
-    if form == "cuda":
-        _same_device(p, device)
-        pt, vt, ft = p.detach().contiguous(), v.detach().contiguous(), f.detach().contiguous()
-    else:
-        pt, vt, ft = _to_device([p, v, f], device)
+    pt, vt, ft = _upload(form, [p, v, f], device)
     dev, stream = _call_args(pt)
     d = torch.empty(n, dtype=pt.dtype, device=pt.device)
     fidx = torch.empty(n, dtype=ft.dtype, device=pt.device)
@@ -76,9 +88,122 @@ def closest_points_on_mesh(p, v, f, *, device=None):
     _pcu_internal._closest_points_on_mesh_device(pt.dtype == torch.float64, pt.data_ptr(), n, vt.data_ptr(), int(vt.shape[0]),
                                                  ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], d.data_ptr(),
                                                  fidx.data_ptr(), bc.data_ptr(), bad.data_ptr(), dev, stream)
-    nbad = int(bad.item())
-    if nbad:
-        raise ValueError("Invalid face indices: %d faces have a corner outside [0, #v)" % nbad)
+    _raise_bad(bad)
     if form == "numpy":
         return (d.cpu().numpy(),) + _back(fidx, bc, f, form)
     return d, fidx, bc
+
+
+def _validate_nonempty_points(p):
+    """validate_point_cloud(p, false) (src/common/common.h:58-74): zero rows are an error."""
+    if len(p.shape) == 2 and p.shape[0] == 0:
+        raise ValueError("Invalid input point cloud with zero points: points must have shape (n, 3) (n > 0). Got points.shape "
+                         "=%s." % (tuple(p.shape),))
+    if len(p.shape) != 2 or p.shape[1] != 3:
+        raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). Got points.shape =%s."
+                         % (tuple(p.shape),))
+
+
+def triangle_soup_fast_winding_number(v, f, p, *, device=None):
+    """
+    Compute a consistent inside/outside field given a triangle soup and evaluate that field
+    at a set of query points
+
+    Args:
+        v: (#v, 3)-shaped array of mesh vertex positions (float32 / float64)
+        f: (#f, 3)-shaped array of mesh face indexes into v (int32 / int64 / uint32 / uint64)
+        p: (#p, 3)-shaped array of query positions at which to evaluate the winding number field (v's dtype, #p > 0)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        w : a (#p,)-shaped array of winding numbers (v's dtype): about 1 inside and 0 outside a closed mesh whose faces
+            are oriented outwards, -1 inside when they are oriented inwards, k inside k nested shells
+
+    Mirrors the reference's src/fast_winding_numbers.cpp (libigl's fast winding numbers, Barill et al. 2018) and, like
+    libigl, evaluates the field in fp32 whatever v's dtype: corners and queries are rounded to fp32, every face near the
+    query contributes its exact solid angle, and a group of faces whose area-weighted centre is more than twice their
+    radius away contributes Barill's order-2 far-field expansion instead.  The terms are summed in fp64 in a fixed order,
+    so the result depends only on (v, f, p_i) (DESIGN.md §3).
+    Divergence: a face corner outside [0, #v) raises ValueError (the reference reads out of bounds).
+    """
+    form = _form([v, f, p], ["v", "f", "p"])
+    if _dtype_name(v) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected one of ['float32', 'float64']." % _dtype_name(v))
+    if _dtype_name(f) not in _INDEX_KINDS:
+        raise ValueError("Invalid scalar type (%s) for argument 'f'. Expected one of %s." % (_dtype_name(f), list(_INDEX_KINDS)))
+    if _dtype_name(p) != _dtype_name(v):
+        raise ValueError("Invalid scalar type (%s) for argument 'p'. Expected it to match argument 'v' which is of type %s."
+                         % (_dtype_name(p), _dtype_name(v)))
+    _validate_mesh(v, f, tuple(_INDEX_KINDS))
+    _validate_nonempty_points(p)
+    torch = _torch()
+    if form == "cpu":
+        return torch.from_numpy(triangle_soup_fast_winding_number(v.detach().numpy(), f.detach().numpy(), p.detach().numpy(),
+                                                                  device=device))
+    vt, ft, pt = _upload(form, [v, f, p], device)
+    n = int(pt.shape[0])
+    dev, stream = _call_args(pt)
+    w = torch.empty(n, dtype=pt.dtype, device=pt.device)
+    bad = torch.empty(1, dtype=torch.int64, device=pt.device)
+    _pcu_internal._fast_winding_number_device(pt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
+                                              int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], pt.data_ptr(), n, 2.0, w.data_ptr(),
+                                              bad.data_ptr(), dev, stream)
+    _raise_bad(bad)
+    return w.cpu().numpy() if form == "numpy" else w
+
+
+def signed_distance_to_mesh(p, v, f, lower_bound=-float("inf"), upper_bound=float("inf"), *, device=None):
+    """
+    Computes signed distances of a point cloud with respect to a Mesh using Fast Winding Numbers
+
+    Args:
+        p : (#p, 3)-shaped array point cloud (float32 / float64, #p > 0)
+        v : (#v, 3)-shaped array of mesh vertex positions (p's dtype)
+        f : (#f, 3)-shaped array of mesh face indexes into v (int32 / int64 / uint32 / uint64)
+        lower_bound : the lower end of the band of distances to compute (rounded to float32), -inf by default
+        upper_bound : the upper end of the band of distances to compute (rounded to float32), +inf by default
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        s : a (#p,)-shaped array of signed distances (p's dtype): negative inside, positive outside
+        fi : a (#p,)-shaped int32 array of indices of the closest face
+        bc : a (#p, 3)-shaped array of barycentric coordinates of the closest point on that face (p's dtype)
+
+    Mirrors the reference's src/signed_distance.cpp (libigl's signed_distance with the fast-winding-number sign).
+    fi and bc are exactly those of `closest_points_on_mesh(p, v, f)`, and s = sigma * d with d that function's
+    distance and sigma = 1 - 2|w|, w exactly `triangle_soup_fast_winding_number(v, f, p)`.  sigma is libigl's continuous
+    factor, not a sign: it is about -1 inside and +1 outside a closed, consistently oriented mesh, and -3 inside two
+    nested shells (|w| = 2), as in libigl.  With max_abs = max(-lower_bound, upper_bound), a query whose squared distance
+    is at least max_abs^2, or below max(max_abs - (upper_bound - lower_bound), 0)^2, is out of the band: s = NaN,
+    fi = #f + 1 and bc = NaN (DESIGN.md §3).  The default bounds give no band.
+    Divergences: out of the band, bc is NaN (libigl reads face #f + 1 out of bounds); a face corner outside [0, #v)
+    raises ValueError (the reference reads out of bounds).
+    """
+    import numpy as np
+    form = _form([p, v, f], ["p", "v", "f"])
+    if _dtype_name(p) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s) for argument 'p'. Expected one of ['float32', 'float64']." % _dtype_name(p))
+    if _dtype_name(v) != _dtype_name(p):
+        raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected it to match argument 'p' which is of type %s."
+                         % (_dtype_name(v), _dtype_name(p)))
+    _validate_mesh(v, f, tuple(_INDEX_KINDS))
+    _validate_nonempty_points(p)
+    lower, upper = float(np.float32(lower_bound)), float(np.float32(upper_bound))
+    torch = _torch()
+    if form == "cpu":
+        out = signed_distance_to_mesh(p.detach().numpy(), v.detach().numpy(), f.detach().numpy(), lower, upper, device=device)
+        return tuple(torch.from_numpy(o) for o in out)
+    pt, vt, ft = _upload(form, [p, v, f], device)
+    n = int(pt.shape[0])
+    dev, stream = _call_args(pt)
+    s = torch.empty(n, dtype=pt.dtype, device=pt.device)
+    fidx = torch.empty(n, dtype=torch.int32, device=pt.device)
+    bc = torch.empty((n, 3), dtype=pt.dtype, device=pt.device)
+    bad = torch.empty(1, dtype=torch.int64, device=pt.device)
+    _pcu_internal._signed_distance_to_mesh_device(pt.dtype == torch.float64, pt.data_ptr(), n, vt.data_ptr(), int(vt.shape[0]),
+                                                  ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], lower, upper,
+                                                  s.data_ptr(), fidx.data_ptr(), bc.data_ptr(), bad.data_ptr(), dev, stream)
+    _raise_bad(bad)
+    if form == "numpy":
+        return s.cpu().numpy(), fidx.cpu().numpy(), bc.cpu().numpy()
+    return s, fidx, bc

@@ -559,6 +559,31 @@ void closest_points_on_mesh_device(bool is_f64, uintptr_t p, int64_t np, uintptr
     });
 }
 
+// Winding numbers (triangle_soup_fast_winding_number, _mesh_query.py); accuracy_scale: the far-field threshold.
+void fast_winding_number_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t q, int64_t nq,
+                                double accuracy_scale, uintptr_t out_w, uintptr_t out_bad, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_fast_winding_number_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (const double*)q, nq,
+                                                         accuracy_scale, (double*)out_w, (uint64_t*)out_bad, (void*)stream)
+                      : pcu_b200_fast_winding_number_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (const float*)q, nq,
+                                                         accuracy_scale, (float*)out_w, (uint64_t*)out_bad, (void*)stream);
+    });
+}
+
+// Signed distances (signed_distance_to_mesh, _mesh_query.py); the bounds are float, as the reference binding's are.
+void signed_distance_to_mesh_device(bool is_f64, uintptr_t p, int64_t np, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind,
+                                    float lower_bound, float upper_bound, uintptr_t out_s, uintptr_t out_fidx, uintptr_t out_bc,
+                                    uintptr_t out_bad, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_signed_distance_to_mesh_f64(ws, (const double*)p, np, (const double*)v, nv, (const void*)f, nf, f_kind,
+                                                             lower_bound, upper_bound, (double*)out_s, (int32_t*)out_fidx,
+                                                             (double*)out_bc, (uint64_t*)out_bad, (void*)stream)
+                      : pcu_b200_signed_distance_to_mesh_f32(ws, (const float*)p, np, (const float*)v, nv, (const void*)f, nf, f_kind,
+                                                             lower_bound, upper_bound, (float*)out_s, (int32_t*)out_fidx,
+                                                             (float*)out_bc, (uint64_t*)out_bad, (void*)stream);
+    });
+}
+
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
@@ -950,6 +975,8 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_mesh_area_device", &mesh_area_device);
     mod.def("_sample_mesh_random_device", &sample_mesh_random_device);
     mod.def("_closest_points_on_mesh_device", &closest_points_on_mesh_device);
+    mod.def("_fast_winding_number_device", &fast_winding_number_device);
+    mod.def("_signed_distance_to_mesh_device", &signed_distance_to_mesh_device);
     mod.def("_sample_mesh_poisson_disk_device", &sample_mesh_poisson_disk_device);
     mod.def("_interpolate_barycentric_device", &interpolate_barycentric_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,

@@ -125,20 +125,10 @@ __global__ void __launch_bounds__(kThreads) mq_codes_kernel(const T* __restrict_
     *reinterpret_cast<ulonglong2*>(recs + t) = make_ulonglong2(code, (unsigned long long)t);   // {key[0], idx}
 }
 
-// Leaf i (i < valid = m - bad): its face's corners as three Pt<T> (lane i: face id in the first, 1 for a degenerate
-// face in the second) and its box.
+// A face is degenerate when D = (e1.e1)(e2.e2) - (e1.e2)^2 is not positive (DESIGN.md §3), in T from the corners.
 template <typename T>
-__global__ void __launch_bounds__(kThreads) mq_leaves_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f,
-                                                             int fkind, long long m, const MqScratch* __restrict__ sc,
-                                                             const MqRec* __restrict__ sorted, Pt<T>* __restrict__ leaves,
-                                                             MqBox* __restrict__ boxes) {
+__device__ __forceinline__ bool mq_degenerate(const double a[3], const double b[3], const double c[3]) {
     using R = Real<T>;
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m - (long long)sc->bad) return;
-    const long long t = (long long)sorted[i].idx;
-    double a[3], b[3], c[3];
-    mq_corners<T>(v, nv, f, fkind, t, a, b, c);
-    boxes[i] = mq_face_box<T>(a, b, c);
     const T ax = (T)a[0], ay = (T)a[1], az = (T)a[2];
     const T e1x = R::sub((T)b[0], ax), e1y = R::sub((T)b[1], ay), e1z = R::sub((T)b[2], az);
     const T e2x = R::sub((T)c[0], ax), e2y = R::sub((T)c[1], ay), e2z = R::sub((T)c[2], az);
@@ -146,9 +136,25 @@ __global__ void __launch_bounds__(kThreads) mq_leaves_kernel(const T* __restrict
     const T d11 = R::add(R::add(R::mul(e2x, e2x), R::mul(e2y, e2y)), R::mul(e2z, e2z));
     const T d01 = R::add(R::add(R::mul(e1x, e2x), R::mul(e1y, e2y)), R::mul(e1z, e2z));
     const T D = R::sub(R::mul(d00, d11), R::mul(d01, d01));
+    return !(D > (T)0);
+}
+
+// Leaf i (i < valid = m - bad): its face's corners as three Pt<T> (lane i: face id in the first, 1 for a degenerate
+// face in the second) and its box.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mq_leaves_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f,
+                                                             int fkind, long long m, const MqScratch* __restrict__ sc,
+                                                             const MqRec* __restrict__ sorted, Pt<T>* __restrict__ leaves,
+                                                             MqBox* __restrict__ boxes) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m - (long long)sc->bad) return;
+    const long long t = (long long)sorted[i].idx;
+    double a[3], b[3], c[3];
+    mq_corners<T>(v, nv, f, fkind, t, a, b, c);
+    boxes[i] = mq_face_box<T>(a, b, c);
     Pt<T> pa, pb, pc;
-    pa.x = ax; pa.y = ay; pa.z = az; pa.i = (typename Real<T>::index_t)t;
-    pb.x = (T)b[0]; pb.y = (T)b[1]; pb.z = (T)b[2]; pb.i = D > (T)0 ? 0 : 1;
+    pa.x = (T)a[0]; pa.y = (T)a[1]; pa.z = (T)a[2]; pa.i = (typename Real<T>::index_t)t;
+    pb.x = (T)b[0]; pb.y = (T)b[1]; pb.z = (T)b[2]; pb.i = mq_degenerate<T>(a, b, c) ? 1 : 0;
     pc.x = (T)c[0]; pc.y = (T)c[1]; pc.z = (T)c[2]; pc.i = 0;
     leaves[3 * i] = pa; leaves[3 * i + 1] = pb; leaves[3 * i + 2] = pc;
 }

@@ -33,7 +33,7 @@
 #include "dedup.cuh"
 #include "poisson.cuh"
 #include "meshsample.cuh"
-#include "meshquery.cuh"
+#include "winding.cuh"
 
 using namespace pcu;
 
@@ -1260,21 +1260,27 @@ int dedup_dispatch(pcu_b200_workspace* ws, const T* pts, long long n, double eps
     return dedup_device<T, int>(ws, pts, n, epsilon, (const int*)faces, nf, cols, out_pts, out_svi, out_svj, (int*)out_faces, out_counts, stream);
 }
 
-// ---- closest points on a mesh (closest_points_on_mesh, meshquery.cuh) --------------------------------------------
-// Tree over the valid faces, built per call, then one traversal per query.  The count of faces with a corner out of
-// range lands in *out_bad; the caller reads it (the call's one synchronisation) and raises when it is not zero.
+// ---- closest points, winding numbers and signed distances on a mesh (meshquery.cuh, winding.cuh) ---------------------
+// The tree over the valid faces, built per call by the one builder below, then one traversal per query.  The count of
+// faces with a corner out of range lands in *out_bad; the caller reads it (the call's one synchronisation) and raises
+// when it is not zero.
 template <typename T>
-int closest_points_device(pcu_b200_workspace* ws, const T* p, long long np, const T* v, long long nv, const void* f, long long m,
-                          int fkind, T* out_d, void* out_fidx, T* out_bc, unsigned long long* out_bad, cudaStream_t stream) {
-    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
-    PCU_TRY(mesh_check(v, nv, f, m, fkind));
-    if (np < 0 || (np > 0 && !p)) return fail(PCU_B200_INVALID_ARGUMENT, "p must be an (n, 3) array");
-    if (!out_bad || (np > 0 && (!out_d || !out_fidx || !out_bc))) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
-    PCU_ON_DEVICE(ws);
+struct MeshTree {
+    MqScratch* sc;
+    MqNode* nodes;
+    Pt<T>* leaves;
+    WnNode* wn;   // far-field data per node (with `moments` only)
+};
+
+// Carves the tree from the arena and enqueues its build: bounds, codes, sort, leaves, nodes, refit and, with `moments`,
+// the centre, radius and moment passes of winding.cuh.  The caller has checked the mesh and made the device current.
+template <typename T>
+int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, bool moments,
+                    unsigned long long* out_bad, cudaStream_t stream, MeshTree<T>& tree) {
     const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
     const long long inner = std::max<long long>(1, m - 1);
     struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; MqScratch* sc;
-             MqNode* nodes; int* node_parent; int* leaf_parent; int* arrivals; Pt<T>* leaves; MqBox* boxes; } s;
+             MqNode* nodes; int* node_parent; int* leaf_parent; int* arrivals; Pt<T>* leaves; MqBox* boxes; WnNode* wn; } s;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
         s.a = cv.take<MqRec>((size_t)m);
         s.b = cv.take<MqRec>((size_t)m);
@@ -1289,6 +1295,7 @@ int closest_points_device(pcu_b200_workspace* ws, const T* p, long long np, cons
         s.arrivals = cv.take<int>((size_t)inner);
         s.leaves = cv.take<Pt<T>>((size_t)3 * m);
         s.boxes = cv.take<MqBox>((size_t)m);
+        s.wn = moments ? cv.take<WnNode>((size_t)inner) : nullptr;
     }));
     PCU_CUDA(cudaMemsetAsync(s.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
     PCU_CUDA(cudaMemsetAsync(s.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
@@ -1306,11 +1313,85 @@ int closest_points_device(pcu_b200_workspace* ws, const T* p, long long np, cons
                s.leaf_parent);
     PCU_LAUNCH(mq_refit_kernel, fblocks, kThreads, stream, m, (const MqScratch*)s.sc, s.nodes, (const int*)s.node_parent,
                (const int*)s.leaf_parent, (const MqBox*)s.boxes, s.arrivals);
+    if (moments) {
+        PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
+        PCU_LAUNCH((wn_centres_kernel<T>), fblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
+                   (const int*)s.node_parent, (const int*)s.leaf_parent, (const Pt<T>*)s.leaves, s.wn, s.arrivals);
+        PCU_LAUNCH((wn_radius_kernel<T>), fblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const int*)s.node_parent,
+                   (const int*)s.leaf_parent, (const Pt<T>*)s.leaves, s.wn);
+        PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
+        PCU_LAUNCH((wn_moments_kernel<T>), fblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
+                   (const int*)s.node_parent, (const int*)s.leaf_parent, (const Pt<T>*)s.leaves, s.wn, s.arrivals);
+    }
     PCU_CUDA(cudaMemcpyAsync(out_bad, &s.sc->bad, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
+    tree = MeshTree<T>{s.sc, s.nodes, s.leaves, s.wn};
+    return PCU_B200_OK;
+}
+
+inline unsigned query_blocks(pcu_b200_workspace* ws, long long nq) {
+    return (unsigned)std::min<long long>((nq + kThreads - 1) / kThreads, (long long)ws->sm_count * 64);
+}
+
+template <typename T>
+int closest_points_device(pcu_b200_workspace* ws, const T* p, long long np, const T* v, long long nv, const void* f, long long m,
+                          int fkind, T* out_d, void* out_fidx, T* out_bc, unsigned long long* out_bad, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (np < 0 || (np > 0 && !p)) return fail(PCU_B200_INVALID_ARGUMENT, "p must be an (n, 3) array");
+    if (!out_bad || (np > 0 && (!out_d || !out_fidx || !out_bc))) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    MeshTree<T> t;
+    PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, false, out_bad, stream, t));
     if (np == 0) return PCU_B200_OK;
-    const unsigned qblocks = (unsigned)std::min<long long>((np + kThreads - 1) / kThreads, (long long)ws->sm_count * 64);
-    PCU_LAUNCH((mq_query_kernel<T>), qblocks, kThreads, stream, p, np, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
-               (const Pt<T>*)s.leaves, out_d, out_fidx, (fkind & 1), out_bc);
+    PCU_LAUNCH((mq_query_kernel<T>), query_blocks(ws, np), kThreads, stream, p, np, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
+               (const Pt<T>*)t.leaves, out_d, out_fidx, (fkind & 1), out_bc);
+    return PCU_B200_OK;
+}
+
+// Winding numbers at q with far-field threshold beta (DESIGN.md §3; beta = inf: every face exactly).
+template <typename T>
+int winding_number_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, const T* q,
+                          long long nq, double beta, T* out_w, unsigned long long* out_bad, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (nq < 0 || (nq > 0 && !q)) return fail(PCU_B200_INVALID_ARGUMENT, "q must be an (n, 3) array");
+    if (!(beta > 0.0)) return fail(PCU_B200_INVALID_ARGUMENT, "accuracy_scale must be positive (got %g)", beta);
+    if (!out_bad || (nq > 0 && !out_w)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    MeshTree<T> t;
+    PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, true, out_bad, stream, t));
+    if (nq == 0) return PCU_B200_OK;
+    PCU_LAUNCH((wn_query_kernel<T>), query_blocks(ws, nq), kThreads, stream, q, nq, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
+               (const WnNode*)t.wn, (const Pt<T>*)t.leaves, (float)beta, out_w);
+    return PCU_B200_OK;
+}
+
+// Signed distances (libigl's fast-winding-number sign): the closest-point walk, then sd_sign_kernel on the same tree.
+// The band is libigl's, computed in T from the fp32 bounds; max(a, b) is a < b ? b : a, so NaN (the defaults give
+// inf - inf) disables the lower limit.
+template <typename T>
+int signed_distance_device(pcu_b200_workspace* ws, const T* p, long long np, const T* v, long long nv, const void* f, long long m,
+                           int fkind, float lower_bound, float upper_bound, T* out_s, int* out_fidx, T* out_bc,
+                           unsigned long long* out_bad, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (np < 0 || (np > 0 && !p)) return fail(PCU_B200_INVALID_ARGUMENT, "p must be an (n, 3) array");
+    if (!out_bad || (np > 0 && (!out_s || !out_fidx || !out_bc))) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    if (m >= INT_MAX) return fail(PCU_B200_INVALID_ARGUMENT, "signed distance returns int32 face indices: at most 2^31 - 2 faces");
+    PCU_ON_DEVICE(ws);
+    const auto larger = [](T a, T b) { return a < b ? b : a; };
+    const T lo = (T)lower_bound, hi = (T)upper_bound;
+    const T max_abs = larger(-lo, hi);
+    const T up = max_abs * max_abs;
+    const T low_root = larger(max_abs - (hi - lo), (T)0);
+    const T low = low_root * low_root;
+    MeshTree<T> t;
+    PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, true, out_bad, stream, t));
+    if (np == 0) return PCU_B200_OK;
+    PCU_LAUNCH((mq_query_kernel<T>), query_blocks(ws, np), kThreads, stream, p, np, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
+               (const Pt<T>*)t.leaves, out_s, (void*)out_fidx, 0, out_bc);
+    PCU_LAUNCH((sd_sign_kernel<T>), query_blocks(ws, np), kThreads, stream, p, np, v, nv, f, fkind, m, (const MqScratch*)t.sc,
+               (const MqNode*)t.nodes, (const WnNode*)t.wn, (const Pt<T>*)t.leaves, 2.f, up, low, out_s, out_fidx, out_bc);
     return PCU_B200_OK;
 }
 
@@ -1980,6 +2061,29 @@ int pcu_b200_closest_points_on_mesh_f64(pcu_b200_workspace* ws, const double* p,
                                         void* stream) {
     return closest_points_device<double>(ws, p, np, v, nv, f, nf, f_kind, out_d, out_fidx, out_bc, (unsigned long long*)out_bad,
                                          (cudaStream_t)stream);
+}
+
+int pcu_b200_fast_winding_number_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                     const float* q, int64_t nq, double accuracy_scale, float* out_w, uint64_t* out_bad, void* stream) {
+    return winding_number_device<float>(ws, v, nv, f, nf, f_kind, q, nq, accuracy_scale, out_w, (unsigned long long*)out_bad,
+                                        (cudaStream_t)stream);
+}
+int pcu_b200_fast_winding_number_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                     const double* q, int64_t nq, double accuracy_scale, double* out_w, uint64_t* out_bad, void* stream) {
+    return winding_number_device<double>(ws, v, nv, f, nf, f_kind, q, nq, accuracy_scale, out_w, (unsigned long long*)out_bad,
+                                         (cudaStream_t)stream);
+}
+int pcu_b200_signed_distance_to_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
+                                         int64_t nf, int f_kind, float lower_bound, float upper_bound, float* out_s, int32_t* out_fidx,
+                                         float* out_bc, uint64_t* out_bad, void* stream) {
+    return signed_distance_device<float>(ws, p, np, v, nv, f, nf, f_kind, lower_bound, upper_bound, out_s, out_fidx, out_bc,
+                                         (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_signed_distance_to_mesh_f64(pcu_b200_workspace* ws, const double* p, int64_t np, const double* v, int64_t nv, const void* f,
+                                         int64_t nf, int f_kind, float lower_bound, float upper_bound, double* out_s, int32_t* out_fidx,
+                                         double* out_bc, uint64_t* out_bad, void* stream) {
+    return signed_distance_device<double>(ws, p, np, v, nv, f, nf, f_kind, lower_bound, upper_bound, out_s, out_fidx, out_bc,
+                                          (unsigned long long*)out_bad, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,
