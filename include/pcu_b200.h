@@ -422,6 +422,43 @@ int pcu_b200_signed_distance_to_mesh_f64(pcu_b200_workspace* ws, const double* p
                                          int64_t nf, int f_kind, float lower_bound, float upper_bound, double* out_s, int32_t* out_fidx,
                                          double* out_bc, uint64_t* out_bad, void* stream);
 
+/* ---- rays against a mesh -----------------------------------------------------------------------------------------
+ * Replace ray_mesh_intersection and RayMeshIntersector (src/ray_mesh_intersection.cpp, one Embree ray at a time).  For
+ * each ray i (n rays, n >= 0) with origin o[i * o_stride .. + 3] (o_stride 0: one origin for every ray, 3: one per ray)
+ * and direction d[3 i .. 3 i + 3]: out_fidx[i], out_bc[i, 0:3] and out_t[i] of the face that minimises (t, face index)
+ * lexicographically over the faces hit with near < t <= far, by the watertight test of Woop, Benthin and Wald (JCGT
+ * 2013) in fp32 on the fp32-rounded corners, origin and direction, both sides of a face counting (DESIGN.md §3,
+ * csrc/raycast.cuh).  bc = (fl((1 - b1) - b2 in fp64), b1, b2), t in units of |d|.  A ray that hits nothing, and a
+ * ray whose origin or direction is zero or not finite, gets out_fidx = -1, out_t = +inf and out_bc = 0.
+ *   ray_mesh_intersection: builds the tree of the closest-point query for the call; out_fidx has f's width (4 bytes for
+ *     I32 / U32, 8 for I64 / U64).  Faces with a corner outside [0, nv) are left out and counted in *out_bad (device
+ *     uint64); when it is not zero the outputs are unspecified.
+ *   mesh_prepare: builds that tree once into a private device block (*out_mesh) and counts the bad faces in *out_bad as
+ *     above (a handle whose count is not zero should be destroyed).  pcu_b200_mesh_destroy synchronises the device;
+ *     pcu_b200_mesh_size is the face count.
+ *   ray_mesh_intersection_prepared: rays against a prepared mesh of either precision (the suffix is the rays'); out_fidx
+ *     is int32.  Results equal ray_mesh_intersection's on the same mesh.
+ * Every array pointer is a DEVICE pointer and the calls are stream-ordered. */
+typedef struct pcu_b200_mesh pcu_b200_mesh;
+int pcu_b200_ray_mesh_intersection_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                       const float* o, int o_stride, const float* d, int64_t n, float near, float far, void* out_fidx,
+                                       float* out_bc, float* out_t, uint64_t* out_bad, void* stream);
+int pcu_b200_ray_mesh_intersection_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                       const double* o, int o_stride, const double* d, int64_t n, float near, float far, void* out_fidx,
+                                       double* out_bc, double* out_t, uint64_t* out_bad, void* stream);
+int pcu_b200_mesh_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                              pcu_b200_mesh** out_mesh, uint64_t* out_bad, void* stream);
+int pcu_b200_mesh_prepare_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                              pcu_b200_mesh** out_mesh, uint64_t* out_bad, void* stream);
+int pcu_b200_mesh_destroy(pcu_b200_mesh* mesh);
+int64_t pcu_b200_mesh_size(const pcu_b200_mesh* mesh);
+int pcu_b200_ray_mesh_intersection_prepared_f32(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, const float* o, int o_stride,
+                                                const float* d, int64_t n, float near, float far, int32_t* out_fidx, float* out_bc,
+                                                float* out_t, void* stream);
+int pcu_b200_ray_mesh_intersection_prepared_f64(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, const double* o, int o_stride,
+                                                const double* d, int64_t n, float near, float far, int32_t* out_fidx, double* out_bc,
+                                                double* out_t, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

@@ -1,0 +1,237 @@
+"""ray_mesh_intersection and RayMeshIntersector -- the reference's names, arguments and outputs (the reference's
+src/ray_mesh_intersection.cpp and point_cloud_utils/_ray_mesh_intersector.py), computed by csrc/raycast.cuh on the tree
+of csrc/meshquery.cuh.
+
+Input forms and validation follow _mesh_query.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
+out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
+import numpy as np
+
+from . import _pcu_internal
+from ._mesh_query import _raise_bad, _upload
+from ._mesh_sampling import _INDEX_KINDS, _call_args, _dtype_name, _form, _to_device, _torch, _validate_mesh
+
+
+def _matrix_shape(a):
+    """The (rows, cols) the reference's Eigen binding sees: a 1-D array of n elements is an (n, 1) column."""
+    s = tuple(a.shape)
+    return (s[0], 1) if len(s) == 1 else (s if len(s) == 2 else (int(np.prod(s)), 1))
+
+
+def _validate_rays(ray_o, ray_d):
+    """src/ray_mesh_intersection.cpp:117-135: a 3-element ray_o is one origin for every ray, else the row counts must
+    match and ray_o must have 3 columns; ray_d must have 3 columns.  Returns (single origin, number of rays)."""
+    single = int(np.prod(tuple(ray_o.shape))) == 3
+    (orows, ocols), (drows, dcols) = _matrix_shape(ray_o), _matrix_shape(ray_d)
+    if not single and orows != drows:
+        raise ValueError("ray_o and ray_d must have the same number of rows (one ray origin per ray direction). "
+                         "(Note: ray_o can have one row to use the same origin for all directions)")
+    if not single and ocols != 3:
+        raise ValueError("Invalid shape for ray_o must have shape (N, 3) but got (%d, %d)." % (orows, ocols))
+    if dcols != 3:
+        raise ValueError("Invalid shape for ray_d must have shape (N, 3) but got (%d, %d)." % (drows, dcols))
+    return single, drows
+
+
+def _check_float(x, name):
+    if _dtype_name(x) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of ['float32', 'float64']." % (_dtype_name(x), name))
+
+
+def _check_match(x, name, ref, ref_name):
+    if _dtype_name(x) != _dtype_name(ref):
+        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected it to match argument '%s' which is of type %s."
+                         % (_dtype_name(x), name, ref_name, _dtype_name(ref)))
+
+
+def _bounds(ray_near, ray_far):
+    """The reference hands both to Embree as float."""
+    return float(np.float32(ray_near)), float(np.float32(ray_far))
+
+
+def _empty(form, fdt, dt, device):
+    """Zero rays: empty outputs, no launch."""
+    if form == "numpy":
+        return np.zeros(0, dtype=fdt), np.zeros((0, 3), dtype=dt), np.zeros(0, dtype=dt)
+    torch = _torch()
+    return (torch.zeros(0, dtype=fdt, device=device), torch.zeros((0, 3), dtype=dt, device=device),
+            torch.zeros(0, dtype=dt, device=device))
+
+
+def _outputs(n, fidx_dtype, rt):
+    torch = _torch()
+    return (torch.empty(n, dtype=fidx_dtype, device=rt.device), torch.empty((n, 3), dtype=rt.dtype, device=rt.device),
+            torch.empty(n, dtype=rt.dtype, device=rt.device))
+
+
+def _origins(ot, single):
+    """(origins, o_stride) of a contiguous ray_o: a single origin is its 3 elements in order, with stride 0."""
+    return (ot.reshape(3), 0) if single else (ot, 3)
+
+
+def ray_mesh_intersection(v, f, ray_o, ray_d, ray_near=0.0, ray_far=np.inf, *, device=None):
+    """
+    Compute intersection between a set of rays and a triangle mesh
+
+    Args:
+        v : \\#v by 3 array of vertex positions (each row is a vertex) (float32 / float64)
+        f : \\#f by 3 Matrix of face (triangle) indices (int32 / int64 / uint32 / uint64)
+        ray_o : array of shape (#rays, 3) of ray origins (one per row) or a single array of shape (3,) to use (v's dtype)
+        ray_d : array of shape (#rays, 3) of ray directions (one per row) (v's dtype)
+        ray_near : an optional floating point value indicating the distance along each ray to start searching (default 0.0)
+        ray_far : an optional floating point value indicating the maximum distance along each ray to search (default inf)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        f_id : an array of shape (#rays,) representing the face id hit by each ray (f's dtype; -1 cast to it on a miss)
+        bc : an array of shape (#rays, 3) where each row is the barycentric coordinates within each face of the ray
+             intersection (v's dtype; 0 on a miss)
+        t : the distance along each ray to the intersection, in units of |ray_d| (v's dtype; inf on a miss)
+
+    Mirrors the reference's src/ray_mesh_intersection.cpp (Embree).  The result is a pure function of (v, f, o_i, d_i,
+    ray_near, ray_far), defined in DESIGN.md §3: everything is rounded to float32 as the reference does, every face is
+    tested with the watertight test of Woop, Benthin and Wald (2013) on both of its sides, and the chosen face is the
+    lexicographic minimum of (t, face index) over the faces hit with ray_near < t <= ray_far.  bc = (1 - b1 - b2, b1, b2).
+    Divergences: Embree's choice among tied faces and its arithmetic are not reproduced; a face corner outside [0, #v)
+    raises ValueError (the reference reads out of bounds); a 3-element ray_o of any shape is taken in element order (the
+    reference reads ray_o(0, 0), ray_o(1, 0), ray_o(2, 0)); a zero or non-finite origin or direction misses.
+    """
+    form = _form([v, f, ray_o, ray_d], ["v", "f", "ray_o", "ray_d"])
+    _check_float(v, "v")
+    if _dtype_name(f) not in _INDEX_KINDS:
+        raise ValueError("Invalid scalar type (%s) for argument 'f'. Expected one of %s." % (_dtype_name(f), list(_INDEX_KINDS)))
+    _check_match(ray_o, "ray_o", v, "v")
+    _check_match(ray_d, "ray_d", v, "v")
+    single, n = _validate_rays(ray_o, ray_d)
+    _validate_mesh(v, f, tuple(_INDEX_KINDS))
+    near, far = _bounds(ray_near, ray_far)
+    torch = _torch()
+    if form == "cpu":
+        out = ray_mesh_intersection(v.detach().numpy(), f.detach().numpy(), ray_o.detach().numpy(), ray_d.detach().numpy(),
+                                    near, far, device=device)
+        return tuple(torch.from_numpy(o) for o in out)
+    if n == 0:
+        if form == "cuda":
+            from . import _same_device
+            _same_device(v, device)
+        return _empty(form, f.dtype, v.dtype, v.device if form == "cuda" else None)
+    vt, ft, ot, dt = _upload(form, [v, f, ray_o, ray_d], device)
+    ot, o_stride = _origins(ot, single)
+    dt = dt.reshape(n, 3)
+    dev, stream = _call_args(vt)
+    fidx, bc, t = _outputs(n, ft.dtype, vt)
+    bad = torch.empty(1, dtype=torch.int64, device=vt.device)
+    _pcu_internal._ray_mesh_intersection_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
+                                                int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], ot.data_ptr(), o_stride,
+                                                dt.data_ptr(), n, near, far, fidx.data_ptr(), bc.data_ptr(), t.data_ptr(),
+                                                bad.data_ptr(), dev, stream)
+    _raise_bad(bad)
+    if form == "numpy":
+        return fidx.cpu().numpy().view(f.dtype), bc.cpu().numpy(), t.cpu().numpy()
+    return fidx, bc, t
+
+
+class RayMeshIntersector:
+    """
+    Class used to find the intersection between rays and a triangle mesh.
+
+    The mesh's tree is built once, on the GPU, when the object is made; every `intersect_rays` call only casts its
+    rays.  The results are those of `ray_mesh_intersection(mesh_v, mesh_f, ...)` (f_id as int32).  `close()` (or garbage
+    collection) frees the device memory.
+    """
+
+    def __init__(self, mesh_v, mesh_f, *, device=None):
+        """
+        Create a RayMeshIntersector object which can be used to do ray/mesh queries with a triangle mesh.
+
+        Args:
+          mesh_v : \\#v by 3 array of vertex positions (each row is a vertex) (float32 / float64)
+          mesh_f : \\#f by 3 Matrix of face (triangle) indices (int32 / int64 / uint32 / uint64)
+          device : (keyword only, not in the reference) the GPU of a numpy mesh, see `k_nearest_neighbors`; a mesh of
+                   CUDA tensors stays on its device.
+
+        Divergence: a face corner outside [0, #v) raises ValueError (the reference validates nothing here).
+        """
+        self._handle = 0
+        form = _form([mesh_v, mesh_f], ["mesh_v", "mesh_f"])
+        _validate_mesh(mesh_v, mesh_f, tuple(_INDEX_KINDS))
+        self.v = mesh_v
+        self.f = mesh_f
+        torch = _torch()
+        if form == "cuda":
+            from . import _same_device
+            _same_device(mesh_v, device)
+            vt, ft = (a.detach().contiguous() for a in (mesh_v, mesh_f))
+        else:
+            arrays = [mesh_v, mesh_f] if form == "numpy" else [mesh_v.detach().numpy(), mesh_f.detach().numpy()]
+            vt, ft = _to_device(arrays, device)
+        dev, stream = _call_args(vt)
+        bad = torch.empty(1, dtype=torch.int64, device=vt.device)
+        handle = _pcu_internal._mesh_prepare_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
+                                                    int(ft.shape[0]), _INDEX_KINDS[_dtype_name(mesh_f)], bad.data_ptr(), dev,
+                                                    stream)
+        try:
+            _raise_bad(bad)      # also waits for the build, so calls on any stream may use the tree
+        except ValueError:
+            _pcu_internal._mesh_destroy(handle)
+            raise
+        self._handle, self.device_index = handle, dev
+
+    def close(self):
+        if self._handle:
+            _pcu_internal._mesh_destroy(self._handle)
+            self._handle = 0
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:   # interpreter shutdown
+            pass
+
+    def intersect_rays(self, ray_o, ray_d, ray_near=0.0, ray_far=np.inf):
+        """
+        Compute intersection between a set of rays and the triangle mesh enclosed in this class
+
+        Args:
+          ray_o : array of shape (\\#rays, 3) of ray origins (one per row) or a single array of shape (3,) to use
+                  (float32 / float64)
+          ray_d : array of shape (\\#rays, 3) of ray directions (one per row) (ray_o's dtype)
+          ray_near : an optional floating point value indicating the distance along each ray to start searching (default 0.0)
+          ray_far : an optional floating point value indicating the maximum distance along each ray to search (default inf)
+
+        Returns:
+          f_id : an array of shape (#rays,) representing the face id hit by each ray (int32; -1 on a miss)
+          bc : an array of shape (#rays, 3) where each row is the barycentric coordinates within each face of the ray
+               intersection (ray_o's dtype)
+          t : the distance along each ray to the intersection (ray_o's dtype; inf on a miss)
+
+        Rays given as CUDA tensors must live on the mesh's device; numpy arrays and CPU tensors are copied there.
+        """
+        if not self._handle:
+            raise ValueError("the RayMeshIntersector has been closed")
+        form = _form([ray_o, ray_d], ["ray_o", "ray_d"])
+        _check_float(ray_o, "ray_o")
+        _check_match(ray_d, "ray_d", ray_o, "ray_o")
+        single, n = _validate_rays(ray_o, ray_d)
+        near, far = _bounds(ray_near, ray_far)
+        torch = _torch()
+        if form == "cpu":
+            out = self.intersect_rays(ray_o.detach().numpy(), ray_d.detach().numpy(), near, far)
+            return tuple(torch.from_numpy(o) for o in out)
+        if form == "cuda" and (ray_o.device.index or 0) != self.device_index:
+            raise ValueError("the rays live on %s, the mesh on cuda:%d" % (ray_o.device, self.device_index))
+        if n == 0:
+            return _empty(form, np.int32 if form == "numpy" else torch.int32, ray_o.dtype,
+                          ray_o.device if form == "cuda" else None)
+        if form == "cuda":
+            ot, dt = (a.detach().contiguous() for a in (ray_o, ray_d))
+        else:
+            ot, dt = _to_device([ray_o, ray_d], self.device_index)
+        ot, o_stride = _origins(ot, single)
+        dt = dt.reshape(n, 3)
+        dev, stream = _call_args(dt)
+        fidx, bc, t = _outputs(n, torch.int32, dt)
+        _pcu_internal._ray_mesh_prepared_device(dt.dtype == torch.float64, self._handle, ot.data_ptr(), o_stride, dt.data_ptr(),
+                                                n, near, far, fidx.data_ptr(), bc.data_ptr(), t.data_ptr(), dev, stream)
+        if form == "numpy":
+            return fidx.cpu().numpy(), bc.cpu().numpy(), t.cpu().numpy()
+        return fidx, bc, t

@@ -584,6 +584,48 @@ void signed_distance_to_mesh_device(bool is_f64, uintptr_t p, int64_t np, uintpt
     });
 }
 
+// Rays against a mesh (ray_mesh_intersection, _ray_mesh.py); o_stride 0: one origin; out_fidx has f's width.
+void ray_mesh_intersection_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t o, int o_stride,
+                                  uintptr_t d, int64_t n, float near, float far, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_t,
+                                  uintptr_t out_bad, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_ray_mesh_intersection_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (const double*)o, o_stride,
+                                                           (const double*)d, n, near, far, (void*)out_fidx, (double*)out_bc,
+                                                           (double*)out_t, (uint64_t*)out_bad, (void*)stream)
+                      : pcu_b200_ray_mesh_intersection_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (const float*)o, o_stride,
+                                                           (const float*)d, n, near, far, (void*)out_fidx, (float*)out_bc,
+                                                           (float*)out_t, (uint64_t*)out_bad, (void*)stream);
+    });
+}
+// A prepared mesh (RayMeshIntersector); out_bad: one device uint64, the faces with a corner out of range.
+uintptr_t mesh_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out_bad, int device,
+                              uintptr_t stream) {
+    pcu_b200_mesh* mesh = nullptr;
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_mesh_prepare_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, &mesh, (uint64_t*)out_bad,
+                                                  (void*)stream)
+                      : pcu_b200_mesh_prepare_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, &mesh, (uint64_t*)out_bad,
+                                                  (void*)stream);
+    });
+    return (uintptr_t)mesh;
+}
+void mesh_destroy(uintptr_t mesh) {
+    py::gil_scoped_release nogil;
+    pcu_b200_mesh_destroy((pcu_b200_mesh*)mesh);
+}
+// Rays of precision is_f64 against a prepared mesh of either precision; out_fidx is int32.
+void ray_mesh_prepared_device(bool is_f64, uintptr_t mesh, uintptr_t o, int o_stride, uintptr_t d, int64_t n, float near, float far,
+                              uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_t, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_ray_mesh_intersection_prepared_f64(ws, (const pcu_b200_mesh*)mesh, (const double*)o, o_stride,
+                                                                    (const double*)d, n, near, far, (int32_t*)out_fidx,
+                                                                    (double*)out_bc, (double*)out_t, (void*)stream)
+                      : pcu_b200_ray_mesh_intersection_prepared_f32(ws, (const pcu_b200_mesh*)mesh, (const float*)o, o_stride,
+                                                                    (const float*)d, n, near, far, (int32_t*)out_fidx,
+                                                                    (float*)out_bc, (float*)out_t, (void*)stream);
+    });
+}
+
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
@@ -978,6 +1020,10 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_fast_winding_number_device", &fast_winding_number_device);
     mod.def("_signed_distance_to_mesh_device", &signed_distance_to_mesh_device);
     mod.def("_sample_mesh_poisson_disk_device", &sample_mesh_poisson_disk_device);
+    mod.def("_ray_mesh_intersection_device", &ray_mesh_intersection_device);
+    mod.def("_mesh_prepare_device", &mesh_prepare_device);
+    mod.def("_mesh_destroy", &mesh_destroy);
+    mod.def("_ray_mesh_prepared_device", &ray_mesh_prepared_device);
     mod.def("_interpolate_barycentric_device", &interpolate_barycentric_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);

@@ -34,6 +34,7 @@
 #include "poisson.cuh"
 #include "meshsample.cuh"
 #include "winding.cuh"
+#include "raycast.cuh"
 
 using namespace pcu;
 
@@ -242,6 +243,18 @@ struct pcu_b200_cloud {
     int leaf = 0;                // > 0: the block also holds the reference-tree replica built with this leaf size
     KdReplayBuffers<float> kd32{};
     KdReplayBuffers<double> kd64{};
+};
+// A mesh whose tree is built once (pcu_b200_mesh_prepare_*): the tree's header, nodes and leaves (carve_mesh_tree, no
+// far-field data) live in one private device block.
+struct pcu_b200_mesh {
+    int device = 0;
+    int is_f64 = 0;
+    long long nf = 0;
+    unsigned char* block = nullptr;
+    size_t bytes = 0;
+    MqScratch* sc = nullptr;
+    MqNode* nodes = nullptr;
+    const void* leaves = nullptr;   // Pt<float> or Pt<double> by is_f64
 };
 template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
@@ -1272,15 +1285,27 @@ struct MeshTree {
     WnNode* wn;   // far-field data per node (with `moments` only)
 };
 
-// Carves the tree from the arena and enqueues its build: bounds, codes, sort, leaves, nodes, refit and, with `moments`,
-// the centre, radius and moment passes of winding.cuh.  The caller has checked the mesh and made the device current.
+// The arrays a built tree is queried through: the header, the nodes, the leaves and, with `moments`, the far-field data.
+template <typename T>
+void carve_mesh_tree(Carver& cv, long long m, bool moments, MeshTree<T>& t) {
+    const long long inner = std::max<long long>(1, m - 1);
+    t.sc = cv.take<MqScratch>(1);
+    t.nodes = cv.take<MqNode>((size_t)inner);
+    t.leaves = cv.take<Pt<T>>((size_t)3 * m);
+    t.wn = moments ? cv.take<WnNode>((size_t)inner) : nullptr;
+}
+
+// Carves the build's temporaries from the arena, the tree itself (carve_mesh_tree) from `keep` or, when it is null, from
+// the arena too, and enqueues the build: bounds, codes, sort, leaves, nodes, refit and, with `moments`, the centre,
+// radius and moment passes of winding.cuh.  The caller has checked the mesh and made the device current.
 template <typename T>
 int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, bool moments,
-                    unsigned long long* out_bad, cudaStream_t stream, MeshTree<T>& tree) {
+                    unsigned long long* out_bad, cudaStream_t stream, MeshTree<T>& tree, unsigned char* keep = nullptr) {
     const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
     const long long inner = std::max<long long>(1, m - 1);
     struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; MqScratch* sc;
              MqNode* nodes; int* node_parent; int* leaf_parent; int* arrivals; Pt<T>* leaves; MqBox* boxes; WnNode* wn; } s;
+    MeshTree<T> kept;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
         s.a = cv.take<MqRec>((size_t)m);
         s.b = cv.take<MqRec>((size_t)m);
@@ -1288,15 +1313,14 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
         s.totals = cv.take<unsigned long long>(kSortBins);
         s.base = cv.take<unsigned>(kSortBins);
         s.constant = cv.take<int>(1);
-        s.sc = cv.take<MqScratch>(1);
-        s.nodes = cv.take<MqNode>((size_t)inner);
         s.node_parent = cv.take<int>((size_t)inner);
         s.leaf_parent = cv.take<int>((size_t)m);
         s.arrivals = cv.take<int>((size_t)inner);
-        s.leaves = cv.take<Pt<T>>((size_t)3 * m);
         s.boxes = cv.take<MqBox>((size_t)m);
-        s.wn = moments ? cv.take<WnNode>((size_t)inner) : nullptr;
+        if (!keep) carve_mesh_tree<T>(cv, m, moments, kept);
     }));
+    if (keep) carve_at(keep, [&](Carver& cv) { carve_mesh_tree<T>(cv, m, moments, kept); });
+    s.sc = kept.sc; s.nodes = kept.nodes; s.leaves = kept.leaves; s.wn = kept.wn;
     PCU_CUDA(cudaMemsetAsync(s.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
     PCU_CUDA(cudaMemsetAsync(s.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
     PCU_CUDA(cudaMemsetAsync(&s.sc->bad, 0, sizeof(unsigned long long), stream));
@@ -1393,6 +1417,83 @@ int signed_distance_device(pcu_b200_workspace* ws, const T* p, long long np, con
     PCU_LAUNCH((sd_sign_kernel<T>), query_blocks(ws, np), kThreads, stream, p, np, v, nv, f, fkind, m, (const MqScratch*)t.sc,
                (const MqNode*)t.nodes, (const WnNode*)t.wn, (const Pt<T>*)t.leaves, 2.f, up, low, out_s, out_fidx, out_bc);
     return PCU_B200_OK;
+}
+
+// ---- rays against a mesh (raycast.cuh) --------------------------------------------------------------------------------
+// One launch over the rays of a built tree.  o_stride: 0 (one origin for every ray) or 3.  near and far are fp32
+// (DESIGN.md §3); out_fidx holds 8-byte indices when fidx_wide, else 4-byte ones.
+template <typename TR, typename TM>
+int cast_rays(pcu_b200_workspace* ws, const MqScratch* sc, const MqNode* nodes, const Pt<TM>* leaves, long long m, const TR* o,
+              int o_stride, const TR* d, long long n, float near, float far, void* out_fidx, int fidx_wide, TR* out_bc, TR* out_t,
+              cudaStream_t stream) {
+    if (n == 0) return PCU_B200_OK;
+    PCU_LAUNCH((rc_query_kernel<TR, TM>), query_blocks(ws, n), kThreads, stream, o, o_stride, d, n, near, far, m, sc, nodes, leaves,
+               out_fidx, fidx_wide, out_bc, out_t);
+    return PCU_B200_OK;
+}
+
+int check_rays(const void* o, int o_stride, const void* d, long long n) {
+    if (o_stride != 0 && o_stride != 3) return fail(PCU_B200_INVALID_ARGUMENT, "o_stride must be 0 (one origin) or 3 (got %d)", o_stride);
+    if (n < 0 || (n > 0 && (!o || !d))) return fail(PCU_B200_INVALID_ARGUMENT, "ray_o and ray_d must be (n, 3) arrays");
+    return PCU_B200_OK;
+}
+
+// The tree of the closest-point query, built for this call, then one thread per ray.
+template <typename T>
+int ray_mesh_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, const T* o, int o_stride,
+                    const T* d, long long n, float near, float far, void* out_fidx, T* out_bc, T* out_t, unsigned long long* out_bad,
+                    cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    PCU_TRY(check_rays(o, o_stride, d, n));
+    if (!out_bad || (n > 0 && (!out_fidx || !out_bc || !out_t))) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    MeshTree<T> t;
+    PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, false, out_bad, stream, t));
+    return cast_rays<T, T>(ws, t.sc, t.nodes, t.leaves, m, o, o_stride, d, n, near, far, out_fidx, fkind & 1, out_bc, out_t, stream);
+}
+
+// Builds the tree once into a private block; *out_bad gets the count of faces with a corner out of range.
+template <typename T>
+int mesh_prepare_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, pcu_b200_mesh** out,
+                        unsigned long long* out_bad, cudaStream_t stream) {
+    if (!ws || !out || !out_bad) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    PCU_ON_DEVICE(ws);
+    MeshTree<T> t;
+    const size_t bytes = carve_at(nullptr, [&](Carver& cv) { carve_mesh_tree<T>(cv, m, false, t); });
+    pcu_b200_mesh* h = new (std::nothrow) pcu_b200_mesh();
+    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
+    h->device = ws->device; h->is_f64 = sizeof(T) == 8 ? 1 : 0; h->nf = m; h->bytes = bytes;
+    cudaError_t e = cudaMalloc((void**)&h->block, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        delete h;
+        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMalloc of %zu bytes for a prepared mesh failed: %s", bytes, cudaGetErrorString(e));
+    }
+    const int st = build_mesh_tree<T>(ws, v, nv, f, m, fkind, false, out_bad, stream, t, h->block);
+    if (st != PCU_B200_OK) { cudaFree(h->block); delete h; return st; }
+    h->sc = t.sc; h->nodes = t.nodes; h->leaves = t.leaves;
+    *out = h;
+    return PCU_B200_OK;
+}
+
+// Rays of precision TR against a prepared mesh of either precision; face indices as int32.
+template <typename TR>
+int ray_mesh_prepared_device(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, const TR* o, int o_stride, const TR* d, long long n,
+                             float near, float far, int* out_fidx, TR* out_bc, TR* out_t, cudaStream_t stream) {
+    if (!ws || !mesh) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (mesh->device != ws->device)
+        return fail(PCU_B200_INVALID_ARGUMENT, "the mesh lives on device %d, the workspace on device %d", mesh->device, ws->device);
+    PCU_TRY(check_rays(o, o_stride, d, n));
+    if (n > 0 && (!out_fidx || !out_bc || !out_t)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    if (mesh->is_f64)
+        return cast_rays<TR, double>(ws, mesh->sc, mesh->nodes, (const Pt<double>*)mesh->leaves, mesh->nf, o, o_stride, d, n, near, far,
+                                     out_fidx, 0, out_bc, out_t, stream);
+    return cast_rays<TR, float>(ws, mesh->sc, mesh->nodes, (const Pt<float>*)mesh->leaves, mesh->nf, o, o_stride, d, n, near, far,
+                                out_fidx, 0, out_bc, out_t, stream);
 }
 
 // ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
@@ -2084,6 +2185,46 @@ int pcu_b200_signed_distance_to_mesh_f64(pcu_b200_workspace* ws, const double* p
                                          double* out_bc, uint64_t* out_bad, void* stream) {
     return signed_distance_device<double>(ws, p, np, v, nv, f, nf, f_kind, lower_bound, upper_bound, out_s, out_fidx, out_bc,
                                           (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+
+int pcu_b200_ray_mesh_intersection_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                       const float* o, int o_stride, const float* d, int64_t n, float near, float far, void* out_fidx,
+                                       float* out_bc, float* out_t, uint64_t* out_bad, void* stream) {
+    return ray_mesh_device<float>(ws, v, nv, f, nf, f_kind, o, o_stride, d, n, near, far, out_fidx, out_bc, out_t,
+                                  (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_ray_mesh_intersection_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                       const double* o, int o_stride, const double* d, int64_t n, float near, float far, void* out_fidx,
+                                       double* out_bc, double* out_t, uint64_t* out_bad, void* stream) {
+    return ray_mesh_device<double>(ws, v, nv, f, nf, f_kind, o, o_stride, d, n, near, far, out_fidx, out_bc, out_t,
+                                   (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                              pcu_b200_mesh** out_mesh, uint64_t* out_bad, void* stream) {
+    return mesh_prepare_device<float>(ws, v, nv, f, nf, f_kind, out_mesh, (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_prepare_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                              pcu_b200_mesh** out_mesh, uint64_t* out_bad, void* stream) {
+    return mesh_prepare_device<double>(ws, v, nv, f, nf, f_kind, out_mesh, (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_destroy(pcu_b200_mesh* mesh) {
+    if (!mesh) return PCU_B200_OK;
+    DeviceGuard guard(mesh->device);
+    cudaDeviceSynchronize();          // calls that use the mesh may still be queued
+    if (mesh->block) cudaFree(mesh->block);
+    delete mesh;
+    return PCU_B200_OK;
+}
+int64_t pcu_b200_mesh_size(const pcu_b200_mesh* mesh) { return mesh ? mesh->nf : 0; }
+int pcu_b200_ray_mesh_intersection_prepared_f32(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, const float* o, int o_stride,
+                                                const float* d, int64_t n, float near, float far, int32_t* out_fidx, float* out_bc,
+                                                float* out_t, void* stream) {
+    return ray_mesh_prepared_device<float>(ws, mesh, o, o_stride, d, n, near, far, out_fidx, out_bc, out_t, (cudaStream_t)stream);
+}
+int pcu_b200_ray_mesh_intersection_prepared_f64(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, const double* o, int o_stride,
+                                                const double* d, int64_t n, float near, float far, int32_t* out_fidx, double* out_bc,
+                                                double* out_t, void* stream) {
+    return ray_mesh_prepared_device<double>(ws, mesh, o, o_stride, d, n, near, far, out_fidx, out_bc, out_t, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,

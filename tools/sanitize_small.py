@@ -48,6 +48,13 @@ step("normals ball, capped, fp64", lambda: pcu.estimate_point_cloud_normals_ball
 step("voxel down-sampling", lambda: pcu.downsample_point_cloud_on_voxel_grid(0.05, x, x.astype(np.float64)))
 step("deduplicate points", lambda: pcu.deduplicate_point_cloud(np.concatenate([x, x[:500]]), 1e-6))
 step("deduplicate mesh fp64", lambda: pcu.deduplicate_mesh_vertices(np.concatenate([x, x[:500]]).astype(np.float64), rng.integers(0, n, (3000, 3)).astype(np.int64), 0.0))
+mv = rng.normal(size=(200, 3)); mf = rng.integers(0, 200, (300, 3))
+ro = rng.normal(size=(500, 3)) * 3
+step("ray mesh intersection", lambda: pcu.ray_mesh_intersection(mv, mf, ro, -ro))
+step("ray mesh intersection, one origin fp32", lambda: pcu.ray_mesh_intersection(mv.astype(np.float32), mf, np.zeros(3, np.float32), ro.astype(np.float32)))
+isect = step("prepare a mesh for rays", lambda: pcu.RayMeshIntersector(mv.astype(np.float32), mf))
+step("rays against a prepared mesh (fp64 rays)", lambda: isect.intersect_rays(ro, -ro))
+isect.close()
 pts_i = rng.integers(-1000, 1000, (n, 3)).astype(np.int32)
 codes = step("morton encode", lambda: pcu.morton_encode(pts_i))
 step("morton decode", lambda: pcu.morton_decode(codes))
