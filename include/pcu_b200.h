@@ -415,6 +415,16 @@ int pcu_b200_fast_winding_number_f32(pcu_b200_workspace* ws, const float* v, int
                                      const float* q, int64_t nq, double accuracy_scale, float* out_w, uint64_t* out_bad, void* stream);
 int pcu_b200_fast_winding_number_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
                                      const double* q, int64_t nq, double accuracy_scale, double* out_w, uint64_t* out_bad, void* stream);
+/* Replaces point_cloud_fast_winding_number (src/fast_winding_numbers.cpp): the winding number of the oriented point
+ * cloud (p, n, a) (np points; p and n (np, 3), a np values) at the nq queries q, out_w[i] (nq rows).  Each point
+ * contributes the dipole a_i n_i . (p_i - q) / |p_i - q|^3 (n used as given, not normalised); the same tree, far field
+ * and fp64 sum as fast_winding_number, over the points (DESIGN.md §3).  accuracy_scale as there: positive, 2 in the
+ * library's function, +inf evaluates every point exactly.  np = 0 gives out_w = 0.  np and nq are below 2^31 - 1.
+ * Every pointer is a DEVICE pointer and the call is stream-ordered. */
+int pcu_b200_point_cloud_fast_winding_number_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* a, int64_t np,
+                                                 const float* q, int64_t nq, double accuracy_scale, float* out_w, void* stream);
+int pcu_b200_point_cloud_fast_winding_number_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* a, int64_t np,
+                                                 const double* q, int64_t nq, double accuracy_scale, double* out_w, void* stream);
 int pcu_b200_signed_distance_to_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
                                          int64_t nf, int f_kind, float lower_bound, float upper_bound, float* out_s, int32_t* out_fidx,
                                          float* out_bc, uint64_t* out_bad, void* stream);

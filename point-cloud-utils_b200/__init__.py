@@ -41,7 +41,8 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "morton_encode", "morton_decode", "morton_add", "morton_subtract", "morton_knn", "pairwise_distances", "sinkhorn",
            "earth_movers_distance", "downsample_point_cloud_on_voxel_grid", "downsample_point_cloud_poisson_disk",
            "sample_mesh_random", "sample_mesh_poisson_disk", "interpolate_barycentric_coords", "closest_points_on_mesh",
-           "triangle_soup_fast_winding_number", "signed_distance_to_mesh", "ray_mesh_intersection", "RayMeshIntersector",
+           "triangle_soup_fast_winding_number", "point_cloud_fast_winding_number", "signed_distance_to_mesh",
+           "ray_mesh_intersection", "RayMeshIntersector",
            "deduplicate_point_cloud",
            "deduplicate_mesh_vertices", "prepare_cloud", "pinned_empty", "PreparedCloud", "device_count",
            "current_device", "launch_count"]
@@ -772,7 +773,8 @@ from ._sinkhorn import pairwise_distances, sinkhorn, earth_movers_distance  # no
 from ._dedup import deduplicate_point_cloud, deduplicate_mesh_vertices  # noqa: E402  (N2: duplicate removal)
 from ._poisson import downsample_point_cloud_poisson_disk  # noqa: E402  (Poisson-disk downsampling)
 from ._mesh_sampling import sample_mesh_random, sample_mesh_poisson_disk, interpolate_barycentric_coords  # noqa: E402
-from ._mesh_query import closest_points_on_mesh, triangle_soup_fast_winding_number, signed_distance_to_mesh  # noqa: E402
+from ._mesh_query import (closest_points_on_mesh, triangle_soup_fast_winding_number,  # noqa: E402
+                          point_cloud_fast_winding_number, signed_distance_to_mesh)
 from ._ray_mesh import ray_mesh_intersection, RayMeshIntersector  # noqa: E402
 
 

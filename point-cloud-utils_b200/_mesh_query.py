@@ -1,6 +1,6 @@
-"""closest_points_on_mesh, triangle_soup_fast_winding_number and signed_distance_to_mesh -- the reference's names,
-arguments and outputs (the reference's src/closest_point_on_mesh.cpp, src/fast_winding_numbers.cpp and
-src/signed_distance.cpp), computed by csrc/meshquery.cuh and csrc/winding.cuh.
+"""closest_points_on_mesh, triangle_soup_fast_winding_number, point_cloud_fast_winding_number and signed_distance_to_mesh
+-- the reference's names, arguments and outputs (the reference's src/closest_point_on_mesh.cpp,
+src/fast_winding_numbers.cpp and src/signed_distance.cpp), computed by csrc/meshquery.cuh and csrc/winding.cuh.
 
 Input forms and validation follow _mesh_sampling.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
@@ -149,6 +149,71 @@ def triangle_soup_fast_winding_number(v, f, p, *, device=None):
                                               int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], pt.data_ptr(), n, 2.0, w.data_ptr(),
                                               bad.data_ptr(), dev, stream)
     _raise_bad(bad)
+    return w.cpu().numpy() if form == "numpy" else w
+
+
+def _validate_point_cloud_normals(p, n):
+    """validate_point_cloud_normals(p, n) (src/common/common.h:78-109): zero points are allowed."""
+    ps, ns = tuple(p.shape), tuple(n.shape)
+    if len(ps) != 2 or ps[1] != 3:
+        raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). Got points.shape =%s." % (ps,))
+    if len(ns) != 2 or ns[1] != 3:
+        raise ValueError("Invalid shape for normals: must have shape (n, 3) (n > 0). Got normals.shape =%s." % (ns,))
+    if ns[0] != ps[0]:
+        raise ValueError("Invalid input point cloud. Number of normals must match number of points. Got points.shape =%s and "
+                         "normals.shape = %d, %d" % (ps, ns[0], ns[1]))
+
+
+def point_cloud_fast_winding_number(p, n, a, q, *, device=None):
+    """
+    Compute a consistent inside/outside field given a point cloud and evaluate that field
+    at a set of query points
+
+    Args:
+        p : (#p, 3)-shaped array of points (float32 / float64)
+        n : (#p, 3)-shaped array of point normals at p (p's dtype), used as given (not normalised)
+        a : array of #p point areas (p's dtype), of any shape with #p elements, e.g. (#p,) or (#p, 1)
+        q : (#q, 3)-shaped array of query positions at which to evaluate the winding number field (p's dtype, #q > 0)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        w : a (#q,)-shaped array of winding numbers (p's dtype): about 1 inside and 0 outside a closed surface sampled with
+            outward normals and areas that sum to its area, -1 inside with inward normals
+
+    Mirrors the reference's src/fast_winding_numbers.cpp (libigl's fast winding numbers for point clouds, Barill et al.
+    2018).  Point i contributes the dipole a_i n_i . (p_i - q) / |p_i - q|^3 / 4 pi, evaluated in fp32 whatever p's dtype:
+    points and queries are rounded to fp32, a_i n_i is formed in p's dtype and rounded to fp32, every point near the query
+    contributes its exact term (none when the query is on the point), and a group of points whose |a|-weighted centre is
+    more than twice their radius away contributes Barill's order-2 far-field expansion instead.  The terms are summed in
+    fp64 in a fixed order, so the result depends only on (p, n, a, q_i) (DESIGN.md §3).
+    Divergences: a of any shape with exactly #p elements is accepted and any other size raises ValueError (the reference
+    reads a short vector out of bounds); #p = 0 gives w = 0 for every query.
+    """
+    form = _form([p, n, a, q], ["p", "n", "a", "q"])
+    if _dtype_name(p) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s) for argument 'p'. Expected one of ['float32', 'float64']." % _dtype_name(p))
+    for x, name in ((n, "n"), (a, "a"), (q, "q")):
+        if _dtype_name(x) != _dtype_name(p):
+            raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected it to match argument 'p' which is of type %s."
+                             % (_dtype_name(x), name, _dtype_name(p)))
+    _validate_point_cloud_normals(p, n)
+    _validate_nonempty_points(q)
+    na = 1
+    for s in a.shape:
+        na *= int(s)
+    if na != int(p.shape[0]):
+        raise ValueError("Invalid shape for areas: a must have #p = %d elements, e.g. shape (#p,) or (#p, 1). Got a.shape =%s."
+                         % (int(p.shape[0]), tuple(a.shape)))
+    torch = _torch()
+    if form == "cpu":
+        return torch.from_numpy(point_cloud_fast_winding_number(p.detach().numpy(), n.detach().numpy(), a.detach().numpy(),
+                                                                q.detach().numpy(), device=device))
+    pt, nt, at, qt = _upload(form, [p, n, a, q], device)
+    m, nq = int(pt.shape[0]), int(qt.shape[0])
+    dev, stream = _call_args(qt)
+    w = torch.empty(nq, dtype=qt.dtype, device=qt.device)
+    _pcu_internal._point_cloud_fast_winding_number_device(qt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), at.data_ptr(), m,
+                                                          qt.data_ptr(), nq, 2.0, w.data_ptr(), dev, stream)
     return w.cpu().numpy() if form == "numpy" else w
 
 

@@ -570,6 +570,17 @@ void fast_winding_number_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t 
     });
 }
 
+// Winding numbers of an oriented point cloud (point_cloud_fast_winding_number, _mesh_query.py); a holds np values.
+void point_cloud_fast_winding_number_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t a, int64_t np, uintptr_t q, int64_t nq,
+                                            double accuracy_scale, uintptr_t out_w, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_point_cloud_fast_winding_number_f64(ws, (const double*)p, (const double*)n, (const double*)a, np,
+                                                                     (const double*)q, nq, accuracy_scale, (double*)out_w, (void*)stream)
+                      : pcu_b200_point_cloud_fast_winding_number_f32(ws, (const float*)p, (const float*)n, (const float*)a, np,
+                                                                     (const float*)q, nq, accuracy_scale, (float*)out_w, (void*)stream);
+    });
+}
+
 // Signed distances (signed_distance_to_mesh, _mesh_query.py); the bounds are float, as the reference binding's are.
 void signed_distance_to_mesh_device(bool is_f64, uintptr_t p, int64_t np, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind,
                                     float lower_bound, float upper_bound, uintptr_t out_s, uintptr_t out_fidx, uintptr_t out_bc,
@@ -1018,6 +1029,7 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_sample_mesh_random_device", &sample_mesh_random_device);
     mod.def("_closest_points_on_mesh_device", &closest_points_on_mesh_device);
     mod.def("_fast_winding_number_device", &fast_winding_number_device);
+    mod.def("_point_cloud_fast_winding_number_device", &point_cloud_fast_winding_number_device);
     mod.def("_signed_distance_to_mesh_device", &signed_distance_to_mesh_device);
     mod.def("_sample_mesh_poisson_disk_device", &sample_mesh_poisson_disk_device);
     mod.def("_ray_mesh_intersection_device", &ray_mesh_intersection_device);

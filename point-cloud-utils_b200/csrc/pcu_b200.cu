@@ -1390,6 +1390,69 @@ int winding_number_device(pcu_b200_workspace* ws, const T* v, long long nv, cons
     return PCU_B200_OK;
 }
 
+// Winding numbers of the oriented cloud (p, n, a) at q with far-field threshold beta (DESIGN.md §3, point clouds): the
+// tree of winding.cuh over the points, built per call from the arena, then one thread per query.  No points: w = 0.
+template <typename T>
+int point_winding_number_device(pcu_b200_workspace* ws, const T* p, const T* n, const T* a, long long m, const T* q, long long nq,
+                                double beta, T* out_w, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (m < 0 || (m > 0 && (!p || !n || !a))) return fail(PCU_B200_INVALID_ARGUMENT, "p, n and a must be (n, 3), (n, 3) and (n,) arrays");
+    if (m >= INT_MAX) return fail(PCU_B200_INVALID_ARGUMENT, "point cloud winding numbers: at most 2^31 - 2 points, got %lld", m);
+    if (nq < 0 || (nq > 0 && !q)) return fail(PCU_B200_INVALID_ARGUMENT, "q must be an (n, 3) array");
+    if (nq >= INT_MAX) return fail(PCU_B200_INVALID_ARGUMENT, "point cloud winding numbers: at most 2^31 - 2 queries, got %lld", nq);
+    if (!(beta > 0.0)) return fail(PCU_B200_INVALID_ARGUMENT, "accuracy_scale must be positive (got %g)", beta);
+    if (nq > 0 && !out_w) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    if (nq == 0) return PCU_B200_OK;
+    if (m == 0) {
+        PCU_TRY(adopt_stream(ws, stream));
+        PCU_CUDA(cudaMemsetAsync(out_w, 0, (size_t)nq * sizeof(T), stream));   // +0.0 in either precision
+        return PCU_B200_OK;
+    }
+    const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
+    const long long inner = std::max<long long>(1, m - 1);
+    struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; MqScratch* sc;
+             MqNode* nodes; int* node_parent; int* leaf_parent; int* arrivals; WnPoint* leaves; WnNode* wn; } s;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        s.a = cv.take<MqRec>((size_t)m);
+        s.b = cv.take<MqRec>((size_t)m);
+        s.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
+        s.totals = cv.take<unsigned long long>(kSortBins);
+        s.base = cv.take<unsigned>(kSortBins);
+        s.constant = cv.take<int>(1);
+        s.sc = cv.take<MqScratch>(1);
+        s.nodes = cv.take<MqNode>((size_t)inner);
+        s.node_parent = cv.take<int>((size_t)inner);
+        s.leaf_parent = cv.take<int>((size_t)m);
+        s.arrivals = cv.take<int>((size_t)inner);
+        s.leaves = cv.take<WnPoint>((size_t)m);
+        s.wn = cv.take<WnNode>((size_t)inner);
+    }));
+    PCU_CUDA(cudaMemsetAsync(s.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
+    PCU_CUDA(cudaMemsetAsync(s.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
+    PCU_CUDA(cudaMemsetAsync(&s.sc->bad, 0, sizeof(unsigned long long), stream));
+    PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
+    const unsigned pblocks = (unsigned)((m + kThreads - 1) / kThreads);
+    PCU_LAUNCH((wn_point_bounds_kernel<T>), (unsigned)std::min<long long>(pblocks, (long long)ws->sm_count * 8), kThreads, stream,
+               p, m, s.sc);
+    PCU_LAUNCH((wn_point_codes_kernel<T>), pblocks, kThreads, stream, p, m, (const MqScratch*)s.sc, s.a);
+    MqRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records<MqRec>(s.a, s.b, m, 1, s.hist, s.totals, s.base, s.constant, stream, &sorted));
+    PCU_LAUNCH((wn_point_leaves_kernel<T>), pblocks, kThreads, stream, p, n, a, m, (const MqRec*)sorted, s.leaves);
+    PCU_LAUNCH(mq_nodes_kernel, pblocks, kThreads, stream, (const MqRec*)sorted, m, (const MqScratch*)s.sc, s.nodes, s.node_parent,
+               s.leaf_parent);
+    PCU_LAUNCH(wn_point_centres_kernel, pblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
+               (const int*)s.node_parent, (const int*)s.leaf_parent, (const WnPoint*)s.leaves, s.wn, s.arrivals);
+    PCU_LAUNCH(wn_point_radius_kernel, pblocks, kThreads, stream, m, (const int*)s.node_parent, (const int*)s.leaf_parent,
+               (const WnPoint*)s.leaves, s.wn);
+    PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
+    PCU_LAUNCH(wn_point_moments_kernel, pblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
+               (const int*)s.node_parent, (const int*)s.leaf_parent, (const WnPoint*)s.leaves, s.wn, s.arrivals);
+    PCU_LAUNCH((wn_point_query_kernel<T>), query_blocks(ws, nq), kThreads, stream, q, nq, m, (const MqNode*)s.nodes, (const WnNode*)s.wn,
+               (const WnPoint*)s.leaves, (float)beta, out_w);
+    return PCU_B200_OK;
+}
+
 // Signed distances (libigl's fast-winding-number sign): the closest-point walk, then sd_sign_kernel on the same tree.
 // The band is libigl's, computed in T from the fp32 bounds; max(a, b) is a < b ? b : a, so NaN (the defaults give
 // inf - inf) disables the lower limit.
@@ -2173,6 +2236,14 @@ int pcu_b200_fast_winding_number_f64(pcu_b200_workspace* ws, const double* v, in
                                      const double* q, int64_t nq, double accuracy_scale, double* out_w, uint64_t* out_bad, void* stream) {
     return winding_number_device<double>(ws, v, nv, f, nf, f_kind, q, nq, accuracy_scale, out_w, (unsigned long long*)out_bad,
                                          (cudaStream_t)stream);
+}
+int pcu_b200_point_cloud_fast_winding_number_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* a, int64_t np,
+                                                 const float* q, int64_t nq, double accuracy_scale, float* out_w, void* stream) {
+    return point_winding_number_device<float>(ws, p, n, a, np, q, nq, accuracy_scale, out_w, (cudaStream_t)stream);
+}
+int pcu_b200_point_cloud_fast_winding_number_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* a, int64_t np,
+                                                 const double* q, int64_t nq, double accuracy_scale, double* out_w, void* stream) {
+    return point_winding_number_device<double>(ws, p, n, a, np, q, nq, accuracy_scale, out_w, (cudaStream_t)stream);
 }
 int pcu_b200_signed_distance_to_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
                                          int64_t nf, int f_kind, float lower_bound, float upper_bound, float* out_s, int32_t* out_fidx,

@@ -55,6 +55,9 @@ step("ray mesh intersection, one origin fp32", lambda: pcu.ray_mesh_intersection
 isect = step("prepare a mesh for rays", lambda: pcu.RayMeshIntersector(mv.astype(np.float32), mf))
 step("rays against a prepared mesh (fp64 rays)", lambda: isect.intersect_rays(ro, -ro))
 isect.close()
+cn = rng.normal(size=(n, 3)); ca = rng.random(n)
+step("point cloud winding numbers", lambda: pcu.point_cloud_fast_winding_number(v, cn, ca, ro))
+step("point cloud winding numbers fp32", lambda: pcu.point_cloud_fast_winding_number(v.astype(np.float32), cn.astype(np.float32), ca.astype(np.float32), ro.astype(np.float32)))
 pts_i = rng.integers(-1000, 1000, (n, 3)).astype(np.int32)
 codes = step("morton encode", lambda: pcu.morton_encode(pts_i))
 step("morton decode", lambda: pcu.morton_decode(codes))
