@@ -5,37 +5,19 @@ src/fast_winding_numbers.cpp and src/signed_distance.cpp), computed by csrc/mesh
 Input forms and validation follow _mesh_sampling.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
 from . import _pcu_internal
-from ._mesh_sampling import _INDEX_KINDS, _back, _call_args, _dtype_name, _form, _to_device, _torch, _validate_mesh
+from ._mesh_sampling import (_INDEX_KINDS, _back, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form,
+                             _raise_bad, _torch, _upload, _validate_mesh)
 
 
 def _validate_points(p, v, f):
     """The binding's dtype checks (npe_arg(v, npe_matches(p)) among them), then validate_point_cloud(p), which allows
     zero rows (src/common/common.h).  validate_mesh follows."""
-    if _dtype_name(p) not in ("float32", "float64"):
-        raise ValueError("Invalid scalar type (%s) for argument 'p'. Expected one of ['float32', 'float64']." % _dtype_name(p))
-    if _dtype_name(v) != _dtype_name(p):
-        raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected it to match argument 'p' which is of type %s."
-                         % (_dtype_name(v), _dtype_name(p)))
-    if _dtype_name(f) not in _INDEX_KINDS:
-        raise ValueError("Invalid scalar type (%s) for argument 'f'. Expected one of %s." % (_dtype_name(f), list(_INDEX_KINDS)))
+    _check_float(p, "p")
+    _check_match(v, "v", p, "p")
+    _check_index(f, "f", _INDEX_KINDS)
     if len(p.shape) != 2 or p.shape[1] != 3:
         raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). Got points.shape =%s."
                          % (tuple(p.shape),))
-
-
-def _upload(form, arrays, device):
-    """Contiguous CUDA tensors of the inputs, on the device of the call."""
-    from . import _same_device
-    if form == "cuda":
-        _same_device(arrays[0], device)
-        return [a.detach().contiguous() for a in arrays]
-    return _to_device(arrays, device)
-
-
-def _raise_bad(bad):
-    nbad = int(bad.item())
-    if nbad:
-        raise ValueError("Invalid face indices: %d faces have a corner outside [0, #v)" % nbad)
 
 
 def closest_points_on_mesh(p, v, f, *, device=None):
@@ -127,13 +109,9 @@ def triangle_soup_fast_winding_number(v, f, p, *, device=None):
     Divergence: a face corner outside [0, #v) raises ValueError (the reference reads out of bounds).
     """
     form = _form([v, f, p], ["v", "f", "p"])
-    if _dtype_name(v) not in ("float32", "float64"):
-        raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected one of ['float32', 'float64']." % _dtype_name(v))
-    if _dtype_name(f) not in _INDEX_KINDS:
-        raise ValueError("Invalid scalar type (%s) for argument 'f'. Expected one of %s." % (_dtype_name(f), list(_INDEX_KINDS)))
-    if _dtype_name(p) != _dtype_name(v):
-        raise ValueError("Invalid scalar type (%s) for argument 'p'. Expected it to match argument 'v' which is of type %s."
-                         % (_dtype_name(p), _dtype_name(v)))
+    _check_float(v, "v")
+    _check_index(f, "f", _INDEX_KINDS)
+    _check_match(p, "p", v, "v")
     _validate_mesh(v, f, tuple(_INDEX_KINDS))
     _validate_nonempty_points(p)
     torch = _torch()
@@ -190,12 +168,9 @@ def point_cloud_fast_winding_number(p, n, a, q, *, device=None):
     reads a short vector out of bounds); #p = 0 gives w = 0 for every query.
     """
     form = _form([p, n, a, q], ["p", "n", "a", "q"])
-    if _dtype_name(p) not in ("float32", "float64"):
-        raise ValueError("Invalid scalar type (%s) for argument 'p'. Expected one of ['float32', 'float64']." % _dtype_name(p))
+    _check_float(p, "p")
     for x, name in ((n, "n"), (a, "a"), (q, "q")):
-        if _dtype_name(x) != _dtype_name(p):
-            raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected it to match argument 'p' which is of type %s."
-                             % (_dtype_name(x), name, _dtype_name(p)))
+        _check_match(x, name, p, "p")
     _validate_point_cloud_normals(p, n)
     _validate_nonempty_points(q)
     na = 1
@@ -246,11 +221,8 @@ def signed_distance_to_mesh(p, v, f, lower_bound=-float("inf"), upper_bound=floa
     """
     import numpy as np
     form = _form([p, v, f], ["p", "v", "f"])
-    if _dtype_name(p) not in ("float32", "float64"):
-        raise ValueError("Invalid scalar type (%s) for argument 'p'. Expected one of ['float32', 'float64']." % _dtype_name(p))
-    if _dtype_name(v) != _dtype_name(p):
-        raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected it to match argument 'p' which is of type %s."
-                         % (_dtype_name(v), _dtype_name(p)))
+    _check_float(p, "p")
+    _check_match(v, "v", p, "p")
     _validate_mesh(v, f, tuple(_INDEX_KINDS))
     _validate_nonempty_points(p)
     lower, upper = float(np.float32(lower_bound)), float(np.float32(upper_bound))

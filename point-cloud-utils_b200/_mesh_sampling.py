@@ -50,12 +50,26 @@ def _form(arrays, names):
     return "numpy"
 
 
+def _check_float(x, name):
+    if _dtype_name(x) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of ['float32', 'float64']." % (_dtype_name(x), name))
+
+
+def _check_index(x, name, kinds):
+    if _dtype_name(x) not in kinds:
+        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of %s." % (_dtype_name(x), name, list(kinds)))
+
+
+def _check_match(x, name, ref, ref_name):
+    if _dtype_name(x) != _dtype_name(ref):
+        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected it to match argument '%s' which is of type %s."
+                         % (_dtype_name(x), name, ref_name, _dtype_name(ref)))
+
+
 def _validate_mesh(v, f, face_dtypes):
     """The binding's dtype checks, then validate_mesh (src/common/common.h:131-148)."""
-    if _dtype_name(v) not in ("float32", "float64"):
-        raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected one of ['float32', 'float64']." % _dtype_name(v))
-    if _dtype_name(f) not in face_dtypes:
-        raise ValueError("Invalid scalar type (%s) for argument 'f'. Expected one of %s." % (_dtype_name(f), list(face_dtypes)))
+    _check_float(v, "v")
+    _check_index(f, "f", face_dtypes)
     vs, fs = tuple(v.shape), tuple(f.shape)
     if len(vs) != 2 or len(fs) != 2:
         raise ValueError("Only 3D inputs are supported: v and f must have shape (n, 3) and (m, 3) (n, m > 0). Got v.shape ="
@@ -79,9 +93,25 @@ def _to_device(arrays, device):
             for a in arrays]
 
 
+def _upload(form, arrays, device):
+    """Contiguous CUDA tensors of the inputs, on the device of the call."""
+    from . import _same_device
+    if form == "cuda":
+        _same_device(arrays[0], device)
+        return [a.detach().contiguous() for a in arrays]
+    return _to_device(arrays, device)
+
+
 def _call_args(t):
     torch = _torch()
     return t.device.index or 0, torch.cuda.current_stream(t.device).cuda_stream
+
+
+def _raise_bad(bad):
+    """Raises for a count (a device tensor or a host scalar) of faces with a corner out of range."""
+    nbad = int(bad.item())
+    if nbad:
+        raise ValueError("Invalid face indices: %d faces have a corner outside [0, #v)" % nbad)
 
 
 def _read_area(area):
@@ -89,9 +119,7 @@ def _read_area(area):
     host = area.cpu().numpy()
     W = int(host[:1].view(_np.uint64)[0])
     S = float(host[1:2].view(_np.float64)[0])
-    bad = int(host[2])
-    if bad:
-        raise ValueError("Invalid face indices: %d faces have a corner outside [0, #v)" % bad)
+    _raise_bad(host[2])
     if W == 0:
         raise ValueError("Mesh has zero area")
     return W, S
@@ -124,7 +152,6 @@ def sample_mesh_random(v, f, num_samples, random_seed=0, *, device=None):
     j) ^ seed).  Faces of zero area are never drawn.
     Divergence: a face corner outside [0, #v) raises ValueError (the reference reads out of bounds).
     """
-    from . import _same_device
     form = _form([v, f], ["v", "f"])
     _validate_mesh(v, f, ("int32", "int64", "uint32", "uint64"))
     if int(num_samples) <= 0:
@@ -135,11 +162,7 @@ def sample_mesh_random(v, f, num_samples, random_seed=0, *, device=None):
     if form == "cpu":
         out = sample_mesh_random(v.detach().numpy(), f.detach().numpy(), n, seed, device=device)
         return tuple(torch.from_numpy(o) for o in out)
-    if form == "cuda":
-        _same_device(v, device)
-        vt, ft = v.detach().contiguous(), f.detach().contiguous()
-    else:
-        vt, ft = _to_device([v, f], device)
+    vt, ft = _upload(form, [v, f], device)
     dev, stream = _call_args(vt)
     kind = _INDEX_KINDS[_dtype_name(f)]
     fidx = torch.empty(n, dtype=ft.dtype, device=vt.device)
@@ -197,7 +220,6 @@ def sample_mesh_poisson_disk(v, f, num_samples, radius=0.0, use_geodesic_distanc
     Divergences: distances are Euclidean between dense positions (the reference's are too: it does not use geodesics);
     a face corner outside [0, #v) raises ValueError.
     """
-    from . import _same_device
     form = _form([v, f], ["v", "f"])
     _validate_mesh(v, f, ("int32", "int64"))
     num_samples, radius = int(num_samples), float(radius)
@@ -215,11 +237,7 @@ def sample_mesh_poisson_disk(v, f, num_samples, radius=0.0, use_geodesic_distanc
         out = sample_mesh_poisson_disk(v.detach().numpy(), f.detach().numpy(), num_samples, radius, use_geodesic_distance,
                                        best_choice_sampling, seed, sample_num_tolerance, oversampling_factor, device=device)
         return tuple(torch.from_numpy(o) for o in out)
-    if form == "cuda":
-        _same_device(v, device)
-        vt, ft = v.detach().contiguous(), f.detach().contiguous()
-    else:
-        vt, ft = _to_device([v, f], device)
+    vt, ft = _upload(form, [v, f], device)
     dev, stream = _call_args(vt)
     is_f64, nv, nf, kind = vt.dtype == torch.float64, int(vt.shape[0]), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)]
     area = torch.empty(3, dtype=torch.int64, device=vt.device)
@@ -256,12 +274,11 @@ def interpolate_barycentric_coords(f, fi, bc, attribute, *, device=None):
     Divergence: attribute must be 2-D; a 1-D attribute raises ValueError (numpy's broadcasting makes the reference's
     result an unrelated (#attribs, 3) array).
     """
-    from . import _same_device
     form = _form([f, fi, bc, attribute], ["f", "fi", "bc", "attribute"])
-    for x, name, ok in ((f, "f", _INDEX_KINDS), (fi, "fi", _INDEX_KINDS), (bc, "bc", ("float32", "float64")),
-                        (attribute, "attribute", ("float32", "float64"))):
-        if _dtype_name(x) not in ok:
-            raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of %s." % (_dtype_name(x), name, list(ok)))
+    _check_index(f, "f", _INDEX_KINDS)
+    _check_index(fi, "fi", _INDEX_KINDS)
+    _check_float(bc, "bc")
+    _check_float(attribute, "attribute")
     if attribute.ndim != 2:
         raise ValueError("attribute must have shape (#vertices, dim), got %s" % (tuple(attribute.shape),))
     if f.ndim != 2 or f.shape[1] != 3:
@@ -281,14 +298,11 @@ def interpolate_barycentric_coords(f, fi, bc, attribute, *, device=None):
             raise IndexError("index out of bounds for attribute with %d rows" % nv)
         if n == 0 or dim == 0:
             return _np.zeros((n, dim), dtype=_np.float64 if out_f64 else _np.float32)
-        ft, fit, bct, at = _to_device([f, fi, bc, attribute], device)
-    else:
-        _same_device(f, device)
-        if n == 0 or dim == 0:
-            return torch.zeros((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=f.device)
-        if nf == 0 or nv == 0:
-            raise IndexError("index out of bounds: f has %d rows and attribute %d" % (nf, nv))
-        ft, fit, bct, at = (x.detach().contiguous() for x in (f, fi, bc, attribute))
+    ft, fit, bct, at = _upload(form, [f, fi, bc, attribute], device)
+    if n == 0 or dim == 0:
+        return torch.zeros((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=ft.device)
+    if nf == 0 or nv == 0:
+        raise IndexError("index out of bounds: f has %d rows and attribute %d" % (nf, nv))
     dev, stream = _call_args(ft)
     out = torch.empty((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=ft.device)
     bad = torch.empty(1, dtype=torch.int64, device=ft.device)

@@ -7,8 +7,8 @@ out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's 
 import numpy as np
 
 from . import _pcu_internal
-from ._mesh_query import _raise_bad, _upload
-from ._mesh_sampling import _INDEX_KINDS, _call_args, _dtype_name, _form, _to_device, _torch, _validate_mesh
+from ._mesh_sampling import (_INDEX_KINDS, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form, _raise_bad,
+                             _torch, _upload, _validate_mesh)
 
 
 def _matrix_shape(a):
@@ -30,17 +30,6 @@ def _validate_rays(ray_o, ray_d):
     if dcols != 3:
         raise ValueError("Invalid shape for ray_d must have shape (N, 3) but got (%d, %d)." % (drows, dcols))
     return single, drows
-
-
-def _check_float(x, name):
-    if _dtype_name(x) not in ("float32", "float64"):
-        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of ['float32', 'float64']." % (_dtype_name(x), name))
-
-
-def _check_match(x, name, ref, ref_name):
-    if _dtype_name(x) != _dtype_name(ref):
-        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected it to match argument '%s' which is of type %s."
-                         % (_dtype_name(x), name, ref_name, _dtype_name(ref)))
 
 
 def _bounds(ray_near, ray_far):
@@ -97,8 +86,7 @@ def ray_mesh_intersection(v, f, ray_o, ray_d, ray_near=0.0, ray_far=np.inf, *, d
     """
     form = _form([v, f, ray_o, ray_d], ["v", "f", "ray_o", "ray_d"])
     _check_float(v, "v")
-    if _dtype_name(f) not in _INDEX_KINDS:
-        raise ValueError("Invalid scalar type (%s) for argument 'f'. Expected one of %s." % (_dtype_name(f), list(_INDEX_KINDS)))
+    _check_index(f, "f", _INDEX_KINDS)
     _check_match(ray_o, "ray_o", v, "v")
     _check_match(ray_d, "ray_d", v, "v")
     single, n = _validate_rays(ray_o, ray_d)
@@ -157,13 +145,8 @@ class RayMeshIntersector:
         self.v = mesh_v
         self.f = mesh_f
         torch = _torch()
-        if form == "cuda":
-            from . import _same_device
-            _same_device(mesh_v, device)
-            vt, ft = (a.detach().contiguous() for a in (mesh_v, mesh_f))
-        else:
-            arrays = [mesh_v, mesh_f] if form == "numpy" else [mesh_v.detach().numpy(), mesh_f.detach().numpy()]
-            vt, ft = _to_device(arrays, device)
+        arrays = [mesh_v.detach().numpy(), mesh_f.detach().numpy()] if form == "cpu" else [mesh_v, mesh_f]
+        vt, ft = _upload(form, arrays, device)
         dev, stream = _call_args(vt)
         bad = torch.empty(1, dtype=torch.int64, device=vt.device)
         handle = _pcu_internal._mesh_prepare_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
@@ -222,10 +205,7 @@ class RayMeshIntersector:
         if n == 0:
             return _empty(form, np.int32 if form == "numpy" else torch.int32, ray_o.dtype,
                           ray_o.device if form == "cuda" else None)
-        if form == "cuda":
-            ot, dt = (a.detach().contiguous() for a in (ray_o, ray_d))
-        else:
-            ot, dt = _to_device([ray_o, ray_d], self.device_index)
+        ot, dt = _upload(form, [ray_o, ray_d], self.device_index)
         ot, o_stride = _origins(ot, single)
         dt = dt.reshape(n, 3)
         dev, stream = _call_args(dt)

@@ -9,16 +9,23 @@
 //                      d = sqrt(d^2) rounded once, bc the chosen face's coordinates.
 // So neither the tree's shape, nor the sort, nor thread scheduling can change a result.
 //
-// The tree is a linear BVH (Karras 2012) built per call over the valid faces:
-//   mq_bounds_kernel    scene box of the face boxes, count of faces with a corner out of range
-//   mq_codes_kernel     63-bit Morton code of each face's box centre over the scene box (invalid faces: ~0, last)
-//   (sort.cuh)          stable radix sort of (code, face): equal codes stay in face order
-//   mq_leaves_kernel    corners packed in leaf order (face id and degeneracy in the spare lanes), leaf boxes
+// The tree is a linear BVH (Karras 2012), built per call by one sequence over either leaf kind L:
+//   faces   L = Pt<T>, three per leaf (corners, face id, degeneracy); a face with a corner out of range is invalid: it is
+//           counted in MqScratch::bad and sorts last, out of the tree; leaves have boxes and the nodes are refit
+//   points  L = WnPoint (point_cloud_fast_winding_number, winding.cuh), one per leaf, always valid; no boxes, no refit
+// The passes:
+//   mq_bounds_kernel    scene box of the leaves' boxes (a point's box is the point), count of invalid faces
+//   mq_codes_kernel     63-bit Morton code of each face's box centre or each fp32 point over the scene box (invalid
+//                       faces: ~0, last)
+//   (sort.cuh)          stable radix sort of (code, leaf): equal codes stay in input order
+//   mq_leaves_kernel    corners packed in leaf order (face id and degeneracy in the spare lanes), leaf boxes; points:
+//                       wn_point_leaves_kernel
 //   mq_nodes_kernel     Karras's internal nodes; equal codes are split by position (delta = 64 + clz(i ^ j))
-//   mq_refit_kernel     bottom-up boxes with per-node arrival counters: the second child to arrive writes both
+//   mq_refit_kernel     faces: bottom-up boxes with per-node arrival counters: the second child to arrive writes both
 //                       children's boxes into the parent (one 64-byte record per visit)
 //   mq_query_kernel     one thread per query: nearer child first, the other pushed; pruning with the margin of §3.
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "meshsample.cuh"
 #include "morton.cuh"
@@ -42,10 +49,27 @@ struct __align__(16) MqNode {
 };
 struct MqBox { float lo[3], hi[3]; };
 
+// A point leaf of point_cloud_fast_winding_number, one per input point in tree order: the point, its weight |a| and
+// an = a n (fp32, an rounded once from T), 32 bytes whatever the input precision.
+struct __align__(16) WnPoint {
+    float p[3], w;
+    float an[3], pad;
+};
+static_assert(sizeof(WnPoint) == 32, "two float4 per point");
+
+template <typename L>
+constexpr bool kPointLeaf = std::is_same<L, WnPoint>::value;
+
 struct MqScratch {
     int scene[6];                 // ordered-int images of the scene box (min x y z, max x y z)
     unsigned long long bad;       // faces with a corner out of range: left out of the tree, counted for the caller
 };
+
+// Leaves in the tree: m less the invalid faces, counted by mq_bounds_kernel (a point tree has none).
+template <typename L>
+__device__ __forceinline__ long long mq_tree_size(long long m, const MqScratch* sc) {
+    return kPointLeaf<L> ? m : m - (long long)sc->bad;
+}
 
 __device__ __forceinline__ int mq_ord(float x) { const int b = __float_as_int(x); return b >= 0 ? b : b ^ 0x7fffffff; }
 __device__ __forceinline__ float mq_unord(int b) { return __int_as_float(b >= 0 ? b : b ^ 0x7fffffff); }
@@ -77,15 +101,47 @@ __device__ __forceinline__ MqBox mq_face_box(const double a[3], const double b[3
     return bx;
 }
 
-template <typename T>
+// Leaf t of the input in fp64: a face's three corners (false when one is out of range), or the point in a (v holds the
+// points; nv, f and fkind are unused).
+template <typename L, typename T>
+__device__ __forceinline__ bool mq_leaf_corners(const T* v, long long nv, const void* f, int fkind, long long t, double a[3],
+                                                double b[3], double c[3]) {
+    if constexpr (kPointLeaf<L>) {
+        load_vertex<T>(v, t, a);
+        return true;
+    } else {
+        return mq_corners<T>(v, nv, f, fkind, t, a, b, c);
+    }
+}
+
+// The leaf's fp32 box: a face's widened box, or the point's fp32 image as both corners.
+template <typename L, typename T>
+__device__ __forceinline__ MqBox mq_leaf_box(const double a[3], const double b[3], const double c[3]) {
+    if constexpr (kPointLeaf<L>) {
+        MqBox bx;
+        for (int k = 0; k < 3; ++k) bx.lo[k] = bx.hi[k] = (float)a[k];
+        return bx;
+    } else {
+        return mq_face_box<T>(a, b, c);
+    }
+}
+
+// Coordinate k of the point a leaf's Morton code is taken at: a face's box centre, or the point itself (not
+// 0.5 lo + 0.5 hi, which rounds a subnormal point and so could reorder the leaves).
+template <typename L>
+__device__ __forceinline__ float mq_code_point(const MqBox& bx, int k) {
+    return kPointLeaf<L> ? bx.lo[k] : 0.5f * bx.lo[k] + 0.5f * bx.hi[k];
+}
+
+template <typename L, typename T>
 __global__ void __launch_bounds__(kThreads) mq_bounds_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f,
                                                              int fkind, long long m, MqScratch* __restrict__ sc) {
     int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
     unsigned long long bad = 0;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < m; t += (long long)gridDim.x * blockDim.x) {
         double a[3], b[3], c[3];
-        if (!mq_corners<T>(v, nv, f, fkind, t, a, b, c)) { ++bad; continue; }
-        const MqBox bx = mq_face_box<T>(a, b, c);
+        if (!mq_leaf_corners<L, T>(v, nv, f, fkind, t, a, b, c)) { ++bad; continue; }
+        const MqBox bx = mq_leaf_box<L, T>(a, b, c);
         for (int k = 0; k < 3; ++k) { lo[k] = min(lo[k], mq_ord(bx.lo[k])); hi[k] = max(hi[k], mq_ord(bx.hi[k])); }
     }
     for (int o = 16; o > 0; o >>= 1) {
@@ -93,7 +149,7 @@ __global__ void __launch_bounds__(kThreads) mq_bounds_kernel(const T* __restrict
             lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
             hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
         }
-        bad += __shfl_xor_sync(0xffffffffu, bad, o);
+        if constexpr (!kPointLeaf<L>) bad += __shfl_xor_sync(0xffffffffu, bad, o);
     }
     if ((threadIdx.x & 31) == 0) {
         for (int k = 0; k < 3; ++k) { atomicMin(&sc->scene[k], lo[k]); atomicMax(&sc->scene[3 + k], hi[k]); }
@@ -101,8 +157,8 @@ __global__ void __launch_bounds__(kThreads) mq_bounds_kernel(const T* __restrict
     }
 }
 
-// Record t = (code of face t, t).  The box centre is quantised to 21 bits per axis over the scene box.
-template <typename T>
+// Record t = (code of leaf t, t): its code point (mq_code_point) quantised to 21 bits per axis over the scene box.
+template <typename L, typename T>
 __global__ void __launch_bounds__(kThreads) mq_codes_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f,
                                                             int fkind, long long m, const MqScratch* __restrict__ sc,
                                                             MqRec* __restrict__ recs) {
@@ -110,14 +166,14 @@ __global__ void __launch_bounds__(kThreads) mq_codes_kernel(const T* __restrict_
     if (t >= m) return;
     unsigned long long code = ~0ull;
     double a[3], b[3], c[3];
-    if (mq_corners<T>(v, nv, f, fkind, t, a, b, c)) {
-        const MqBox bx = mq_face_box<T>(a, b, c);
+    if (mq_leaf_corners<L, T>(v, nv, f, fkind, t, a, b, c)) {
+        const MqBox bx = mq_leaf_box<L, T>(a, b, c);
         code = 0;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             const float slo = mq_unord(sc->scene[k]), shi = mq_unord(sc->scene[3 + k]);
             const float ext = shi - slo;
-            const float centre = 0.5f * bx.lo[k] + 0.5f * bx.hi[k];
+            const float centre = mq_code_point<L>(bx, k);
             const float s = ext > 0.f ? __fdividef(centre - slo, ext) * 2097152.f : 0.f;   // only orders the leaves
             code |= morton_split21((int)fminf(fmaxf(s, 0.f), 2097151.f)) << k;   // NaN -> 0
         }

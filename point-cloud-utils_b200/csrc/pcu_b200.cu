@@ -1273,39 +1273,44 @@ int dedup_dispatch(pcu_b200_workspace* ws, const T* pts, long long n, double eps
     return dedup_device<T, int>(ws, pts, n, epsilon, (const int*)faces, nf, cols, out_pts, out_svi, out_svj, (int*)out_faces, out_counts, stream);
 }
 
-// ---- closest points, winding numbers and signed distances on a mesh (meshquery.cuh, winding.cuh) ---------------------
-// The tree over the valid faces, built per call by the one builder below, then one traversal per query.  The count of
-// faces with a corner out of range lands in *out_bad; the caller reads it (the call's one synchronisation) and raises
-// when it is not zero.
-template <typename T>
+// ---- closest points, winding numbers and signed distances on a mesh or a point cloud (meshquery.cuh, winding.cuh) ----
+// The tree over the valid faces, or over the points, built per call by the one builder below, then one traversal per
+// query.  The count of faces with a corner out of range lands in *out_bad; the caller reads it (the call's one
+// synchronisation) and raises when it is not zero.
+template <typename L>
 struct MeshTree {
     MqScratch* sc;
     MqNode* nodes;
-    Pt<T>* leaves;
+    L* leaves;
     WnNode* wn;   // far-field data per node (with `moments` only)
 };
 
 // The arrays a built tree is queried through: the header, the nodes, the leaves and, with `moments`, the far-field data.
-template <typename T>
-void carve_mesh_tree(Carver& cv, long long m, bool moments, MeshTree<T>& t) {
+template <typename L>
+void carve_mesh_tree(Carver& cv, long long m, bool moments, MeshTree<L>& t) {
     const long long inner = std::max<long long>(1, m - 1);
     t.sc = cv.take<MqScratch>(1);
     t.nodes = cv.take<MqNode>((size_t)inner);
-    t.leaves = cv.take<Pt<T>>((size_t)3 * m);
+    t.leaves = cv.take<L>((size_t)(kPointLeaf<L> ? 1 : 3) * m);
     t.wn = moments ? cv.take<WnNode>((size_t)inner) : nullptr;
 }
 
 // Carves the build's temporaries from the arena, the tree itself (carve_mesh_tree) from `keep` or, when it is null, from
-// the arena too, and enqueues the build: bounds, codes, sort, leaves, nodes, refit and, with `moments`, the centre,
-// radius and moment passes of winding.cuh.  The caller has checked the mesh and made the device current.
-template <typename T>
+// the arena too, and enqueues the build over the leaf kind L (meshquery.cuh): bounds, codes, sort, leaves, nodes, for
+// faces the refit and, with `moments`, the centre, radius and moment passes of winding.cuh.  Face leaves (L = Pt<T>)
+// are built from the mesh (v, nv, f, fkind) and the count of invalid faces lands in *out_bad; point leaves (L = WnPoint)
+// from the points v, normals n and areas a, always with moments.  The caller has checked the input and made the device
+// current.
+template <typename T, typename L>
 int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, bool moments,
-                    unsigned long long* out_bad, cudaStream_t stream, MeshTree<T>& tree, unsigned char* keep = nullptr) {
+                    unsigned long long* out_bad, cudaStream_t stream, MeshTree<L>& tree, unsigned char* keep = nullptr,
+                    const T* n = nullptr, const T* a = nullptr) {
+    constexpr bool points = kPointLeaf<L>;
     const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
     const long long inner = std::max<long long>(1, m - 1);
-    struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; MqScratch* sc;
-             MqNode* nodes; int* node_parent; int* leaf_parent; int* arrivals; Pt<T>* leaves; MqBox* boxes; WnNode* wn; } s;
-    MeshTree<T> kept;
+    struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant;
+             int* node_parent; int* leaf_parent; int* arrivals; MqBox* boxes; } s;
+    MeshTree<L> t;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
         s.a = cv.take<MqRec>((size_t)m);
         s.b = cv.take<MqRec>((size_t)m);
@@ -1316,39 +1321,44 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
         s.node_parent = cv.take<int>((size_t)inner);
         s.leaf_parent = cv.take<int>((size_t)m);
         s.arrivals = cv.take<int>((size_t)inner);
-        s.boxes = cv.take<MqBox>((size_t)m);
-        if (!keep) carve_mesh_tree<T>(cv, m, moments, kept);
+        s.boxes = points ? nullptr : cv.take<MqBox>((size_t)m);
+        if (!keep) carve_mesh_tree<L>(cv, m, moments, t);
     }));
-    if (keep) carve_at(keep, [&](Carver& cv) { carve_mesh_tree<T>(cv, m, moments, kept); });
-    s.sc = kept.sc; s.nodes = kept.nodes; s.leaves = kept.leaves; s.wn = kept.wn;
-    PCU_CUDA(cudaMemsetAsync(s.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
-    PCU_CUDA(cudaMemsetAsync(s.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
-    PCU_CUDA(cudaMemsetAsync(&s.sc->bad, 0, sizeof(unsigned long long), stream));
-    PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
+    if (keep) carve_at(keep, [&](Carver& cv) { carve_mesh_tree<L>(cv, m, moments, t); });
+    PCU_CUDA(cudaMemsetAsync(t.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
+    PCU_CUDA(cudaMemsetAsync(t.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
+    PCU_CUDA(cudaMemsetAsync(&t.sc->bad, 0, sizeof(unsigned long long), stream));
     const unsigned fblocks = (unsigned)((m + kThreads - 1) / kThreads);
-    PCU_LAUNCH((mq_bounds_kernel<T>), (unsigned)std::min<long long>(fblocks, (long long)ws->sm_count * 8), kThreads, stream,
-               v, nv, f, fkind, m, s.sc);
-    PCU_LAUNCH((mq_codes_kernel<T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)s.sc, s.a);
+    PCU_LAUNCH((mq_bounds_kernel<L, T>), (unsigned)std::min<long long>(fblocks, (long long)ws->sm_count * 8), kThreads, stream,
+               v, nv, f, fkind, m, t.sc);
+    PCU_LAUNCH((mq_codes_kernel<L, T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)t.sc, s.a);
     MqRec* sorted = nullptr;
     PCU_TRY(radix_sort_records<MqRec>(s.a, s.b, m, 1, s.hist, s.totals, s.base, s.constant, stream, &sorted));
-    PCU_LAUNCH((mq_leaves_kernel<T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)s.sc, (const MqRec*)sorted,
-               s.leaves, s.boxes);
-    PCU_LAUNCH(mq_nodes_kernel, fblocks, kThreads, stream, (const MqRec*)sorted, m, (const MqScratch*)s.sc, s.nodes, s.node_parent,
+    if constexpr (points)
+        PCU_LAUNCH((wn_point_leaves_kernel<T>), fblocks, kThreads, stream, v, n, a, m, (const MqRec*)sorted, t.leaves);
+    else
+        PCU_LAUNCH((mq_leaves_kernel<T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)t.sc, (const MqRec*)sorted,
+                   t.leaves, s.boxes);
+    PCU_LAUNCH(mq_nodes_kernel, fblocks, kThreads, stream, (const MqRec*)sorted, m, (const MqScratch*)t.sc, t.nodes, s.node_parent,
                s.leaf_parent);
-    PCU_LAUNCH(mq_refit_kernel, fblocks, kThreads, stream, m, (const MqScratch*)s.sc, s.nodes, (const int*)s.node_parent,
-               (const int*)s.leaf_parent, (const MqBox*)s.boxes, s.arrivals);
+    if constexpr (!points) {
+        PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
+        PCU_LAUNCH(mq_refit_kernel, fblocks, kThreads, stream, m, (const MqScratch*)t.sc, t.nodes, (const int*)s.node_parent,
+                   (const int*)s.leaf_parent, (const MqBox*)s.boxes, s.arrivals);
+    }
     if (moments) {
         PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
-        PCU_LAUNCH((wn_centres_kernel<T>), fblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
-                   (const int*)s.node_parent, (const int*)s.leaf_parent, (const Pt<T>*)s.leaves, s.wn, s.arrivals);
-        PCU_LAUNCH((wn_radius_kernel<T>), fblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const int*)s.node_parent,
-                   (const int*)s.leaf_parent, (const Pt<T>*)s.leaves, s.wn);
+        PCU_LAUNCH((wn_centres_kernel<L>), fblocks, kThreads, stream, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
+                   (const int*)s.node_parent, (const int*)s.leaf_parent, (const L*)t.leaves, t.wn, s.arrivals);
+        PCU_LAUNCH((wn_radius_kernel<L>), fblocks, kThreads, stream, m, (const MqScratch*)t.sc, (const int*)s.node_parent,
+                   (const int*)s.leaf_parent, (const L*)t.leaves, t.wn);
         PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
-        PCU_LAUNCH((wn_moments_kernel<T>), fblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
-                   (const int*)s.node_parent, (const int*)s.leaf_parent, (const Pt<T>*)s.leaves, s.wn, s.arrivals);
+        PCU_LAUNCH((wn_moments_kernel<L>), fblocks, kThreads, stream, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
+                   (const int*)s.node_parent, (const int*)s.leaf_parent, (const L*)t.leaves, t.wn, s.arrivals);
     }
-    PCU_CUDA(cudaMemcpyAsync(out_bad, &s.sc->bad, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
-    tree = MeshTree<T>{s.sc, s.nodes, s.leaves, s.wn};
+    if constexpr (!points)
+        PCU_CUDA(cudaMemcpyAsync(out_bad, &t.sc->bad, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
+    tree = t;
     return PCU_B200_OK;
 }
 
@@ -1364,7 +1374,7 @@ int closest_points_device(pcu_b200_workspace* ws, const T* p, long long np, cons
     if (np < 0 || (np > 0 && !p)) return fail(PCU_B200_INVALID_ARGUMENT, "p must be an (n, 3) array");
     if (!out_bad || (np > 0 && (!out_d || !out_fidx || !out_bc))) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    MeshTree<T> t;
+    MeshTree<Pt<T>> t;
     PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, false, out_bad, stream, t));
     if (np == 0) return PCU_B200_OK;
     PCU_LAUNCH((mq_query_kernel<T>), query_blocks(ws, np), kThreads, stream, p, np, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
@@ -1382,16 +1392,17 @@ int winding_number_device(pcu_b200_workspace* ws, const T* v, long long nv, cons
     if (!(beta > 0.0)) return fail(PCU_B200_INVALID_ARGUMENT, "accuracy_scale must be positive (got %g)", beta);
     if (!out_bad || (nq > 0 && !out_w)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    MeshTree<T> t;
+    MeshTree<Pt<T>> t;
     PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, true, out_bad, stream, t));
     if (nq == 0) return PCU_B200_OK;
-    PCU_LAUNCH((wn_query_kernel<T>), query_blocks(ws, nq), kThreads, stream, q, nq, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
+    PCU_LAUNCH((wn_query_kernel<T, Pt<T>>), query_blocks(ws, nq), kThreads, stream, q, nq, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
                (const WnNode*)t.wn, (const Pt<T>*)t.leaves, (float)beta, out_w);
     return PCU_B200_OK;
 }
 
 // Winding numbers of the oriented cloud (p, n, a) at q with far-field threshold beta (DESIGN.md §3, point clouds): the
-// tree of winding.cuh over the points, built per call from the arena, then one thread per query.  No points: w = 0.
+// tree over the points (build_mesh_tree with point leaves), built per call from the arena, then one thread per query.
+// No points: w = 0.
 template <typename T>
 int point_winding_number_device(pcu_b200_workspace* ws, const T* p, const T* n, const T* a, long long m, const T* q, long long nq,
                                 double beta, T* out_w, cudaStream_t stream) {
@@ -1409,47 +1420,10 @@ int point_winding_number_device(pcu_b200_workspace* ws, const T* p, const T* n, 
         PCU_CUDA(cudaMemsetAsync(out_w, 0, (size_t)nq * sizeof(T), stream));   // +0.0 in either precision
         return PCU_B200_OK;
     }
-    const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
-    const long long inner = std::max<long long>(1, m - 1);
-    struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; MqScratch* sc;
-             MqNode* nodes; int* node_parent; int* leaf_parent; int* arrivals; WnPoint* leaves; WnNode* wn; } s;
-    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
-        s.a = cv.take<MqRec>((size_t)m);
-        s.b = cv.take<MqRec>((size_t)m);
-        s.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
-        s.totals = cv.take<unsigned long long>(kSortBins);
-        s.base = cv.take<unsigned>(kSortBins);
-        s.constant = cv.take<int>(1);
-        s.sc = cv.take<MqScratch>(1);
-        s.nodes = cv.take<MqNode>((size_t)inner);
-        s.node_parent = cv.take<int>((size_t)inner);
-        s.leaf_parent = cv.take<int>((size_t)m);
-        s.arrivals = cv.take<int>((size_t)inner);
-        s.leaves = cv.take<WnPoint>((size_t)m);
-        s.wn = cv.take<WnNode>((size_t)inner);
-    }));
-    PCU_CUDA(cudaMemsetAsync(s.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
-    PCU_CUDA(cudaMemsetAsync(s.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
-    PCU_CUDA(cudaMemsetAsync(&s.sc->bad, 0, sizeof(unsigned long long), stream));
-    PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
-    const unsigned pblocks = (unsigned)((m + kThreads - 1) / kThreads);
-    PCU_LAUNCH((wn_point_bounds_kernel<T>), (unsigned)std::min<long long>(pblocks, (long long)ws->sm_count * 8), kThreads, stream,
-               p, m, s.sc);
-    PCU_LAUNCH((wn_point_codes_kernel<T>), pblocks, kThreads, stream, p, m, (const MqScratch*)s.sc, s.a);
-    MqRec* sorted = nullptr;
-    PCU_TRY(radix_sort_records<MqRec>(s.a, s.b, m, 1, s.hist, s.totals, s.base, s.constant, stream, &sorted));
-    PCU_LAUNCH((wn_point_leaves_kernel<T>), pblocks, kThreads, stream, p, n, a, m, (const MqRec*)sorted, s.leaves);
-    PCU_LAUNCH(mq_nodes_kernel, pblocks, kThreads, stream, (const MqRec*)sorted, m, (const MqScratch*)s.sc, s.nodes, s.node_parent,
-               s.leaf_parent);
-    PCU_LAUNCH(wn_point_centres_kernel, pblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
-               (const int*)s.node_parent, (const int*)s.leaf_parent, (const WnPoint*)s.leaves, s.wn, s.arrivals);
-    PCU_LAUNCH(wn_point_radius_kernel, pblocks, kThreads, stream, m, (const int*)s.node_parent, (const int*)s.leaf_parent,
-               (const WnPoint*)s.leaves, s.wn);
-    PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
-    PCU_LAUNCH(wn_point_moments_kernel, pblocks, kThreads, stream, m, (const MqScratch*)s.sc, (const MqNode*)s.nodes,
-               (const int*)s.node_parent, (const int*)s.leaf_parent, (const WnPoint*)s.leaves, s.wn, s.arrivals);
-    PCU_LAUNCH((wn_point_query_kernel<T>), query_blocks(ws, nq), kThreads, stream, q, nq, m, (const MqNode*)s.nodes, (const WnNode*)s.wn,
-               (const WnPoint*)s.leaves, (float)beta, out_w);
+    MeshTree<WnPoint> t;
+    PCU_TRY(build_mesh_tree<T>(ws, p, 0, nullptr, m, 0, true, nullptr, stream, t, nullptr, n, a));
+    PCU_LAUNCH((wn_query_kernel<T, WnPoint>), query_blocks(ws, nq), kThreads, stream, q, nq, m, (const MqScratch*)t.sc,
+               (const MqNode*)t.nodes, (const WnNode*)t.wn, (const WnPoint*)t.leaves, (float)beta, out_w);
     return PCU_B200_OK;
 }
 
@@ -1472,7 +1446,7 @@ int signed_distance_device(pcu_b200_workspace* ws, const T* p, long long np, con
     const T up = max_abs * max_abs;
     const T low_root = larger(max_abs - (hi - lo), (T)0);
     const T low = low_root * low_root;
-    MeshTree<T> t;
+    MeshTree<Pt<T>> t;
     PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, true, out_bad, stream, t));
     if (np == 0) return PCU_B200_OK;
     PCU_LAUNCH((mq_query_kernel<T>), query_blocks(ws, np), kThreads, stream, p, np, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
@@ -1511,7 +1485,7 @@ int ray_mesh_device(pcu_b200_workspace* ws, const T* v, long long nv, const void
     PCU_TRY(check_rays(o, o_stride, d, n));
     if (!out_bad || (n > 0 && (!out_fidx || !out_bc || !out_t))) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    MeshTree<T> t;
+    MeshTree<Pt<T>> t;
     PCU_TRY(build_mesh_tree<T>(ws, v, nv, f, m, fkind, false, out_bad, stream, t));
     return cast_rays<T, T>(ws, t.sc, t.nodes, t.leaves, m, o, o_stride, d, n, near, far, out_fidx, fkind & 1, out_bc, out_t, stream);
 }
@@ -1524,8 +1498,8 @@ int mesh_prepare_device(pcu_b200_workspace* ws, const T* v, long long nv, const 
     *out = nullptr;
     PCU_TRY(mesh_check(v, nv, f, m, fkind));
     PCU_ON_DEVICE(ws);
-    MeshTree<T> t;
-    const size_t bytes = carve_at(nullptr, [&](Carver& cv) { carve_mesh_tree<T>(cv, m, false, t); });
+    MeshTree<Pt<T>> t;
+    const size_t bytes = carve_at(nullptr, [&](Carver& cv) { carve_mesh_tree(cv, m, false, t); });
     pcu_b200_mesh* h = new (std::nothrow) pcu_b200_mesh();
     if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
     h->device = ws->device; h->is_f64 = sizeof(T) == 8 ? 1 : 0; h->nf = m; h->bytes = bytes;

@@ -3,21 +3,21 @@
 // libigl's fast_winding_number and signed_distance).
 //
 // The field is defined in DESIGN.md §3 (winding number), after Barill et al. 2018, "Fast Winding Numbers for Soups and
-// Clouds", evaluated in fp32 as libigl does:
-//   leaf           one face, always exact: its signed solid angle in fp32 (wn_leaf_omega)
+// Clouds", evaluated in fp32 as libigl does.  The tree's leaves are faces (Pt<T>) or, for point_cloud_fast_winding_number
+// (the same section of DESIGN.md), points (WnPoint, filled by wn_point_leaves_kernel); every pass below serves both
+// leaf kinds, which differ only where noted:
+//   leaf           always exact: a face's signed solid angle or a point's dipole term, in fp32 (wn_leaf_omega)
 //   internal node  when |q - P| > beta r, the order-2 far-field expansion about its area-weighted centre P (wn_far),
-//                  and its subtree is not entered; otherwise child 0's subtree, then child 1's
-//   query          the terms summed in fp64 in that fixed order, w = fp32(sum / 4 pi): a function of (v, f, q) alone
+//                  and its subtree is not entered; otherwise child 0's subtree, then child 1's.  A point tree's node of
+//                  radius 0 is always entered.
+//   query          the terms summed in fp64 in that fixed order, w = fp32(sum / 4 pi): a function of the leaves and q
 //
 //   wn_centres_kernel   bottom-up over the existing topology (as mq_refit_kernel): each node's area and centre P
-//   wn_radius_kernel    every leaf climbs to the root and raises each ancestor's r to the farthest of its corners
+//   wn_radius_kernel    every leaf climbs to the root and raises each ancestor's r to the farthest of its points
 //   wn_moments_kernel   bottom-up again: the second child to arrive at a node shifts both children's moments to the
 //                       node's P, child 0 then child 1, and writes them in units of the node's r
 //   wn_query_kernel     one thread per query
 //   sd_sign_kernel      signed distance after mq_query_kernel: the band on d^2, then sigma = 1 - 2|w| and s = sigma d
-//
-// point_cloud_fast_winding_number (the same section of DESIGN.md) runs the three build passes on point leaves
-// (WnPoint, one per point; the wn_point_* kernels at the end) and a walk whose leaf term is a dipole (wn_dipole).
 #pragma once
 #include "meshquery.cuh"
 
@@ -89,14 +89,6 @@ __device__ __forceinline__ WnRec wn_leaf_rec(const Pt<T>* __restrict__ leaves, i
     return r;
 }
 
-// A point leaf of point_cloud_fast_winding_number, one per input point in tree order: the point, its weight |a| and
-// an = a n (fp32, an rounded once from T), 32 bytes whatever the input precision.
-struct __align__(16) WnPoint {
-    float p[3], w;
-    float an[3], pad;
-};
-static_assert(sizeof(WnPoint) == 32, "two float4 per point");
-
 // One point's moments about the point itself: N = an, A = |a|, M = 0, Q = 0.
 __device__ __forceinline__ WnRec wn_leaf_rec(const WnPoint* __restrict__ leaves, int j) {
     const float4* s = reinterpret_cast<const float4*>(leaves + j);
@@ -111,8 +103,17 @@ __device__ __forceinline__ WnRec wn_leaf_rec(const WnPoint* __restrict__ leaves,
     return r;
 }
 
-// The build passes below serve both leaf kinds (L = Pt<T>, three per face, or WnPoint); wn_leaf_rec is the one thing
-// they read from a leaf.
+// The fp32 points of leaf j that bound its ancestors' radii: a face's three corners, or the point.
+template <typename T>
+__device__ __forceinline__ void wn_leaf_points(const Pt<T>* __restrict__ leaves, int j, float (&c)[3][3]) {
+    wn_leaf_corners<T>(leaves, j, c[0], c[1], c[2]);
+}
+__device__ __forceinline__ void wn_leaf_points(const WnPoint* __restrict__ leaves, int j, float (&c)[1][3]) {
+    const float4 x = *reinterpret_cast<const float4*>(leaves + j);
+    c[0][0] = x.x; c[0][1] = x.y; c[0][2] = x.z;
+}
+
+// The build passes below read a leaf only through wn_leaf_rec and wn_leaf_points.
 // Child c of a node, its area and centre: a leaf's own, or an internal node's as stored (written by other threads of
 // this launch).
 template <typename L>
@@ -174,9 +175,10 @@ __device__ __forceinline__ void wn_shift_add(const WnRec& r, const double P[3], 
 // (their midpoint when both have zero area; a leaf's centre is its centroid, or its point), in fp64 rounded to fp32.
 // r is left 0 for wn_radius_kernel.  `arrivals` starts at 0.
 template <typename L>
-__device__ __forceinline__ void wn_centres_climb(long long m, const MqScratch* __restrict__ sc, const MqNode* __restrict__ nodes,
-                                                 const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
-                                                 const L* __restrict__ leaves, WnNode* wn, int* __restrict__ arrivals) {
+__global__ void __launch_bounds__(kThreads) wn_centres_kernel(long long m, const MqScratch* __restrict__ sc,
+                                                              const MqNode* __restrict__ nodes, const int* __restrict__ node_parent,
+                                                              const int* __restrict__ leaf_parent, const L* __restrict__ leaves,
+                                                              WnNode* wn, int* __restrict__ arrivals) {
     const long long n = m - (long long)sc->bad;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (n < 2 || i >= n) return;
@@ -199,19 +201,20 @@ __device__ __forceinline__ void wn_centres_climb(long long m, const MqScratch* _
     }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kThreads) wn_centres_kernel(long long m, const MqScratch* __restrict__ sc,
-                                                              const MqNode* __restrict__ nodes, const int* __restrict__ node_parent,
-                                                              const int* __restrict__ leaf_parent, const Pt<T>* __restrict__ leaves,
-                                                              WnNode* wn, int* __restrict__ arrivals) {
-    wn_centres_climb(m, sc, nodes, node_parent, leaf_parent, leaves, wn, arrivals);
-}
-
-// r of every ancestor of a leaf, from the leaf's K fp32 points c (a face's corners, or one point), starting at `node`:
-// the largest distance from the ancestor's P to one of them, in fp64 rounded up, then up to fp32; the maximum over the
-// subtree's leaves is the same whatever order the atomics land in.
-template <int K>
-__device__ __forceinline__ void wn_radius_climb(int node, const int* __restrict__ node_parent, const float (&c)[K][3], WnNode* wn) {
+// r of every ancestor of leaf i, from the leaf's K fp32 points c (wn_leaf_points): the largest distance from the
+// ancestor's P to one of them, in fp64 rounded up, then up to fp32; the maximum over the subtree's leaves is the same
+// whatever order the atomics land in.
+template <typename L>
+__global__ void __launch_bounds__(kThreads) wn_radius_kernel(long long m, const MqScratch* __restrict__ sc,
+                                                             const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
+                                                             const L* __restrict__ leaves, WnNode* wn) {
+    constexpr int K = kPointLeaf<L> ? 1 : 3;
+    const long long n = mq_tree_size<L>(m, sc);
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (n < 2 || i >= n) return;
+    float c[K][3];
+    wn_leaf_points(leaves, (int)i, c);
+    int node = leaf_parent[i];
     while (true) {
         float* rec = reinterpret_cast<float*>(wn + node);
         double d2 = 0.0;
@@ -232,25 +235,14 @@ __device__ __forceinline__ void wn_radius_climb(int node, const int* __restrict_
     }
 }
 
-template <typename T>
-__global__ void __launch_bounds__(kThreads) wn_radius_kernel(long long m, const MqScratch* __restrict__ sc,
-                                                             const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
-                                                             const Pt<T>* __restrict__ leaves, WnNode* wn) {
-    const long long n = m - (long long)sc->bad;
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (n < 2 || i >= n) return;
-    float c[3][3];
-    wn_leaf_corners<T>(leaves, (int)i, c[0], c[1], c[2]);
-    wn_radius_climb<3>(leaf_parent[i], node_parent, c, wn);
-}
-
 // The same climb after wn_radius_kernel (`arrivals` cleared again): the second arrival shifts both children's moments,
 // child 0 then child 1, to the node's P in fp64 (an internal child's taken back from units of its own r), so what a
 // node stores does not depend on which child arrived last, and writes them in units of the node's r.
 template <typename L>
-__device__ __forceinline__ void wn_moments_climb(long long m, const MqScratch* __restrict__ sc, const MqNode* __restrict__ nodes,
-                                                 const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
-                                                 const L* __restrict__ leaves, WnNode* wn, int* __restrict__ arrivals) {
+__global__ void __launch_bounds__(kThreads) wn_moments_kernel(long long m, const MqScratch* __restrict__ sc,
+                                                              const MqNode* __restrict__ nodes, const int* __restrict__ node_parent,
+                                                              const int* __restrict__ leaf_parent, const L* __restrict__ leaves,
+                                                              WnNode* wn, int* __restrict__ arrivals) {
     const long long n = m - (long long)sc->bad;
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (n < 2 || i >= n) return;
@@ -268,7 +260,7 @@ __device__ __forceinline__ void wn_moments_climb(long long m, const MqScratch* _
         wn_shift_add(r0, P, N, M, S);
         wn_shift_add(r1, P, N, M, S);
         // a node of radius 0 has every corner at P, so its moments are 0; a node of coincident points has N != 0, which
-        // these units cannot hold: the point walk never takes its far field (wn_point_eval)
+        // these units cannot hold: the point walk never takes its far field (wn_walk)
         const double i1 = head.w > 0.f ? 1.0 / (double)head.w : 0.0, i2 = i1 * i1, i3 = i2 * i1, i4 = i2 * i2;
         p[1] = make_float4((float)(N[0] * i2), (float)(N[1] * i2), (float)(N[2] * i2), (float)(r0.A + r1.A));
         p[2] = make_float4((float)(M[0] * i3), (float)(M[1] * i3), (float)(M[2] * i3), (float)(M[3] * i3));
@@ -278,14 +270,6 @@ __device__ __forceinline__ void wn_moments_climb(long long m, const MqScratch* _
         if (node == 0) return;
         node = node_parent[node];
     }
-}
-
-template <typename T>
-__global__ void __launch_bounds__(kThreads) wn_moments_kernel(long long m, const MqScratch* __restrict__ sc,
-                                                              const MqNode* __restrict__ nodes, const int* __restrict__ node_parent,
-                                                              const int* __restrict__ leaf_parent, const Pt<T>* __restrict__ leaves,
-                                                              WnNode* wn, int* __restrict__ arrivals) {
-    wn_moments_climb(m, sc, nodes, node_parent, leaf_parent, leaves, wn, arrivals);
 }
 
 // The signed solid angle of leaf j seen from q, in fp32 with every operation rounded on its own (van Oosterom and
@@ -317,6 +301,24 @@ __device__ __forceinline__ float wn_leaf_omega(const Pt<T>* __restrict__ leaves,
     return R::mul(2.f, atan2f(det, den));
 }
 
+// The dipole term of point j seen from q, Omega = an.d / |d|^3 with d = p - q, in fp32 with every operation rounded on
+// its own, in this order:
+//   d_k = p_k - q_k,  d2 = (dx dx + dy dy) + dz dz,  l = sqrt(d2),  t = ((an_x dx + an_y dy) + an_z dz) / l,
+//   Omega = t / d2,
+// and 0 when d2 = 0 (a query on the point).  Scaling p and q by 2^k and a by 2^2k scales d and l by 2^k, t by 2^2k and
+// d2 by 2^2k, each exactly where nothing over- or underflows, so Omega keeps its bits.  The intermediate t is of the
+// size of an, so only Omega itself can leave the fp32 range.
+__device__ __forceinline__ float wn_leaf_omega(const WnPoint* __restrict__ leaves, int j, const float q[3]) {
+    using R = Real<float>;
+    const float4* s = reinterpret_cast<const float4*>(leaves + j);
+    const float4 x = __ldg(s), an = __ldg(s + 1);
+    const float dx = R::sub(x.x, q[0]), dy = R::sub(x.y, q[1]), dz = R::sub(x.z, q[2]);
+    const float d2 = mq_dot<float>(dx, dy, dz, dx, dy, dz);
+    if (d2 == 0.f) return 0.f;
+    const float t = __fdiv_rn(mq_dot<float>(an.x, an.y, an.z, dx, dy, dz), R::root(d2));
+    return __fdiv_rn(t, d2);
+}
+
 // The order-2 expansion of a node's solid angle, d = P - q, |d|^2 = d2 (Taylor expansion of y / |y|^3 about d):
 //   N.d / |d|^3 + tr(M) / |d|^3 - 3 d.M.d / |d|^5 - (9/2) c.d / |d|^5 + (15/2) Q[d, d, d] / |d|^7,  c_k = sum_i Q_iik,
 // evaluated as (N'.u) k^2 + (tr M' - 3 u.M'.u) k^3 + ((15/2) Q'[u, u, u] - (9/2) c'.u) k^4 with the unit direction
@@ -342,27 +344,27 @@ __device__ __forceinline__ float wn_far(const WnNode* __restrict__ node, float d
     return (t0 + t1) + t2;
 }
 
-// w at q (fp32): the walk of the header, child 0 first, at most one node pushed per level (kMqStack holds the deepest
-// path).  Not inlined, so the winding-number and the signed-distance kernels run the very same code and get the same
-// bits.
-template <typename T>
-__device__ __noinline__ float wn_eval(const float q[3], long long n, const MqNode* __restrict__ nodes, const WnNode* __restrict__ wn,
-                                      const Pt<T>* __restrict__ leaves, float beta) {
+// w at q (fp32) for a tree of n leaves: the walk of the header, child 0 first, at most one node pushed per level
+// (kMqStack holds the deepest path).  In a point tree a node of radius 0 (every point of its subtree at P, its N not
+// held by WnNode's units) is always opened.
+template <typename L>
+__device__ __forceinline__ float wn_walk(const float q[3], long long n, const MqNode* __restrict__ nodes, const WnNode* __restrict__ wn,
+                                         const L* __restrict__ leaves, float beta) {
     double acc = 0.0;
     if (n == 1) {
-        acc = (double)wn_leaf_omega<T>(leaves, 0, q);
+        acc = (double)wn_leaf_omega(leaves, 0, q);
     } else {
         int stack[kMqStack];
         int sp = 0, x = 0;
         while (true) {
             if (x < 0) {
-                acc += (double)wn_leaf_omega<T>(leaves, ~x, q);
+                acc += (double)wn_leaf_omega(leaves, ~x, q);
             } else {
                 const float4 pr = __ldg(reinterpret_cast<const float4*>(wn + x));
                 const float dx = pr.x - q[0], dy = pr.y - q[1], dz = pr.z - q[2];
                 const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
                 const float br = beta * pr.w;   // beta = inf, r = 0: NaN, never far
-                if (d2 > br * br) {
+                if ((!kPointLeaf<L> || pr.w > 0.f) && d2 > br * br) {
                     acc += (double)wn_far(wn + x, dx, dy, dz, d2, pr.w);
                 } else {
                     const int2 c = __ldg(reinterpret_cast<const int2*>(&nodes[x].c0));
@@ -378,23 +380,36 @@ __device__ __noinline__ float wn_eval(const float q[3], long long n, const MqNod
     return __double2float_rn(__ddiv_rn(acc, 4.0 * 3.141592653589793));
 }
 
+// The face walk is not inlined, so the winding-number and the signed-distance kernels run the very same code and get the
+// same bits; the point walk is inlined into wn_query_kernel.
+template <typename T>
+__device__ __noinline__ float wn_eval(const float q[3], long long n, const MqNode* __restrict__ nodes, const WnNode* __restrict__ wn,
+                                      const Pt<T>* __restrict__ leaves, float beta) {
+    return wn_walk(q, n, nodes, wn, leaves, beta);
+}
+__device__ __forceinline__ float wn_eval(const float q[3], long long n, const MqNode* __restrict__ nodes, const WnNode* __restrict__ wn,
+                                         const WnPoint* __restrict__ leaves, float beta) {
+    return wn_walk(q, n, nodes, wn, leaves, beta);
+}
+
 template <typename T>
 __device__ __forceinline__ void wn_query_point(const T* q, long long i, float out[3]) {
     out[0] = (float)q[3 * i]; out[1] = (float)q[3 * i + 1]; out[2] = (float)q[3 * i + 2];
 }
 
-// Query i in input order; nothing is written when the tree is empty (every face invalid: the caller raises).
-template <typename T>
+// Query i in input order; nothing is written when a face tree is empty (every face invalid: the caller raises).  A point
+// tree is never empty (the caller handles m = 0 without one).
+template <typename T, typename L>
 __global__ void __launch_bounds__(kThreads) wn_query_kernel(const T* __restrict__ q, long long nq, long long m,
                                                             const MqScratch* __restrict__ sc, const MqNode* __restrict__ nodes,
-                                                            const WnNode* __restrict__ wn, const Pt<T>* __restrict__ leaves,
+                                                            const WnNode* __restrict__ wn, const L* __restrict__ leaves,
                                                             float beta, T* __restrict__ out_w) {
-    const long long n = m - (long long)sc->bad;
-    if (n < 1) return;
+    const long long n = mq_tree_size<L>(m, sc);
+    if (!kPointLeaf<L> && n < 1) return;
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += (long long)gridDim.x * blockDim.x) {
         float p[3];
         wn_query_point<T>(q, i, p);
-        out_w[i] = (T)wn_eval<T>(p, n, nodes, wn, leaves, beta);
+        out_w[i] = (T)wn_eval(p, n, nodes, wn, leaves, beta);
     }
 }
 
@@ -436,47 +451,8 @@ __global__ void __launch_bounds__(kThreads) sd_sign_kernel(const T* __restrict__
 }
 
 // ---- oriented point clouds (point_cloud_fast_winding_number, DESIGN.md §3) -------------------------------------------
-// The same tree over the m points: scene box and Morton codes of the fp32 points, the sort, WnPoint leaves in tree
-// order, mq_nodes_kernel (sc->bad is 0), no box refit (the walk reads no boxes), then the centre, radius and moment
-// passes above on point leaves, and a walk whose leaf term is a dipole.
-template <typename T>
-__global__ void __launch_bounds__(kThreads) wn_point_bounds_kernel(const T* __restrict__ p, long long m, MqScratch* __restrict__ sc) {
-    int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < m; i += (long long)gridDim.x * blockDim.x) {
-        float x[3];
-        wn_query_point<T>(p, i, x);
-        for (int k = 0; k < 3; ++k) { lo[k] = min(lo[k], mq_ord(x[k])); hi[k] = max(hi[k], mq_ord(x[k])); }
-    }
-    for (int o = 16; o > 0; o >>= 1)
-        for (int k = 0; k < 3; ++k) {
-            lo[k] = min(lo[k], __shfl_xor_sync(0xffffffffu, lo[k], o));
-            hi[k] = max(hi[k], __shfl_xor_sync(0xffffffffu, hi[k], o));
-        }
-    if ((threadIdx.x & 31) == 0)
-        for (int k = 0; k < 3; ++k) { atomicMin(&sc->scene[k], lo[k]); atomicMax(&sc->scene[3 + k], hi[k]); }
-}
-
-// Record i = (code of point i, i): the fp32 point quantised to 21 bits per axis over the scene box, as in
-// mq_codes_kernel (kept apart so that the face kernel's code stays as it is).
-template <typename T>
-__global__ void __launch_bounds__(kThreads) wn_point_codes_kernel(const T* __restrict__ p, long long m, const MqScratch* __restrict__ sc,
-                                                                  MqRec* __restrict__ recs) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    float x[3];
-    wn_query_point<T>(p, i, x);
-    unsigned long long code = 0;
-#pragma unroll
-    for (int k = 0; k < 3; ++k) {
-        const float slo = mq_unord(sc->scene[k]), shi = mq_unord(sc->scene[3 + k]);
-        const float ext = shi - slo;
-        const float s = ext > 0.f ? __fdividef(x[k] - slo, ext) * 2097152.f : 0.f;   // only orders the leaves
-        code |= morton_split21((int)fminf(fmaxf(s, 0.f), 2097151.f)) << k;   // NaN -> 0
-    }
-    *reinterpret_cast<ulonglong2*>(recs + i) = make_ulonglong2(code, (unsigned long long)i);   // {key[0], idx}
-}
-
-// Leaf i: the fp32 point, |a| and an_k = fl32(fl_T(a n_k)).  a is read as a flat array of m values.
+// The leaves pass of a point tree, in place of mq_leaves_kernel.  Leaf i: the fp32 point, |a| and an_k = fl32(fl_T(a n_k)).
+// a is read as a flat array of m values.
 template <typename T>
 __global__ void __launch_bounds__(kThreads) wn_point_leaves_kernel(const T* __restrict__ p, const T* __restrict__ nrm, const T* __restrict__ a,
                                                                    long long m, const MqRec* __restrict__ sorted, WnPoint* __restrict__ leaves) {
@@ -491,94 +467,6 @@ __global__ void __launch_bounds__(kThreads) wn_point_leaves_kernel(const T* __re
     float4* s = reinterpret_cast<float4*>(leaves + i);
     s[0] = make_float4(x[0], x[1], x[2], fabsf((float)ai));
     s[1] = make_float4(an0, an1, an2, 0.f);
-}
-
-__global__ void __launch_bounds__(kThreads) wn_point_centres_kernel(long long m, const MqScratch* __restrict__ sc,
-                                                                    const MqNode* __restrict__ nodes, const int* __restrict__ node_parent,
-                                                                    const int* __restrict__ leaf_parent, const WnPoint* __restrict__ leaves,
-                                                                    WnNode* wn, int* __restrict__ arrivals) {
-    wn_centres_climb(m, sc, nodes, node_parent, leaf_parent, leaves, wn, arrivals);
-}
-
-__global__ void __launch_bounds__(kThreads) wn_point_radius_kernel(long long m, const int* __restrict__ node_parent,
-                                                                   const int* __restrict__ leaf_parent, const WnPoint* __restrict__ leaves,
-                                                                   WnNode* wn) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (m < 2 || i >= m) return;
-    const float4 x = *reinterpret_cast<const float4*>(leaves + i);
-    const float c[1][3] = {{x.x, x.y, x.z}};
-    wn_radius_climb<1>(leaf_parent[i], node_parent, c, wn);
-}
-
-__global__ void __launch_bounds__(kThreads) wn_point_moments_kernel(long long m, const MqScratch* __restrict__ sc,
-                                                                    const MqNode* __restrict__ nodes, const int* __restrict__ node_parent,
-                                                                    const int* __restrict__ leaf_parent, const WnPoint* __restrict__ leaves,
-                                                                    WnNode* wn, int* __restrict__ arrivals) {
-    wn_moments_climb(m, sc, nodes, node_parent, leaf_parent, leaves, wn, arrivals);
-}
-
-// The dipole term of point j seen from q, Omega = an.d / |d|^3 with d = p - q, in fp32 with every operation rounded on
-// its own, in this order:
-//   d_k = p_k - q_k,  d2 = (dx dx + dy dy) + dz dz,  l = sqrt(d2),  t = ((an_x dx + an_y dy) + an_z dz) / l,
-//   Omega = t / d2,
-// and 0 when d2 = 0 (a query on the point).  Scaling p and q by 2^k and a by 2^2k scales d and l by 2^k, t by 2^2k and
-// d2 by 2^2k, each exactly where nothing over- or underflows, so Omega keeps its bits.  The intermediate t is of the
-// size of an, so only Omega itself can leave the fp32 range.
-__device__ __forceinline__ float wn_dipole(const WnPoint* __restrict__ leaves, int j, const float q[3]) {
-    using R = Real<float>;
-    const float4* s = reinterpret_cast<const float4*>(leaves + j);
-    const float4 x = __ldg(s), an = __ldg(s + 1);
-    const float dx = R::sub(x.x, q[0]), dy = R::sub(x.y, q[1]), dz = R::sub(x.z, q[2]);
-    const float d2 = mq_dot<float>(dx, dy, dz, dx, dy, dz);
-    if (d2 == 0.f) return 0.f;
-    const float t = __fdiv_rn(mq_dot<float>(an.x, an.y, an.z, dx, dy, dz), R::root(d2));
-    return __fdiv_rn(t, d2);
-}
-
-// w at q for a point tree of n leaves: the walk of wn_eval with the dipole as the leaf term, except that a node of
-// radius 0 (every point of its subtree at P, its N not held by WnNode's units) is always opened.
-__device__ __forceinline__ float wn_point_eval(const float q[3], long long n, const MqNode* __restrict__ nodes,
-                                               const WnNode* __restrict__ wn, const WnPoint* __restrict__ leaves, float beta) {
-    double acc = 0.0;
-    if (n == 1) {
-        acc = (double)wn_dipole(leaves, 0, q);
-    } else {
-        int stack[kMqStack];
-        int sp = 0, x = 0;
-        while (true) {
-            if (x < 0) {
-                acc += (double)wn_dipole(leaves, ~x, q);
-            } else {
-                const float4 pr = __ldg(reinterpret_cast<const float4*>(wn + x));
-                const float dx = pr.x - q[0], dy = pr.y - q[1], dz = pr.z - q[2];
-                const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
-                const float br = beta * pr.w;   // beta = inf, r = 0: NaN, never far
-                if (pr.w > 0.f && d2 > br * br) {
-                    acc += (double)wn_far(wn + x, dx, dy, dz, d2, pr.w);
-                } else {
-                    const int2 c = __ldg(reinterpret_cast<const int2*>(&nodes[x].c0));
-                    stack[sp++] = c.y;
-                    x = c.x;
-                    continue;
-                }
-            }
-            if (sp == 0) break;
-            x = stack[--sp];
-        }
-    }
-    return __double2float_rn(__ddiv_rn(acc, 4.0 * 3.141592653589793));
-}
-
-// Query i in input order, against a tree of m >= 1 points.
-template <typename T>
-__global__ void __launch_bounds__(kThreads) wn_point_query_kernel(const T* __restrict__ q, long long nq, long long m,
-                                                                  const MqNode* __restrict__ nodes, const WnNode* __restrict__ wn,
-                                                                  const WnPoint* __restrict__ leaves, float beta, T* __restrict__ out_w) {
-    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nq; i += (long long)gridDim.x * blockDim.x) {
-        float x[3];
-        wn_query_point<T>(q, i, x);
-        out_w[i] = (T)wn_point_eval(x, m, nodes, wn, leaves, beta);
-    }
 }
 
 }  // namespace pcu
