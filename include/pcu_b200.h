@@ -496,8 +496,11 @@ int pcu_b200_voxel_downsample_f64(pcu_b200_workspace* ws, const double* points, 
  *   sinkhorn: weights a (nb, n), b (nb, m), costs M (nb, n, m), eps, max_iters, stop_thresh -> plan out_P (nb, n, m);
  *             out_cost (nb) fp64 = sum_ij P * M per batch or NULL; out_iters: device int32 or NULL.  The log-domain
  *             iteration of the reference, its convergence test evaluated on the device (no host synchronisation).
- * Floating point: element-wise expressions in the arrays' precision and the reference's order, the two reductions in
- * fp64 -- agreement with numpy to rounding (tests/test_sinkhorn.py states the tolerances). */
+ * Any number of rows and batches.  Floating point: pairwise norm kinds 0-4 equal numpy bit for bit (the same rounded
+ * operations, sums in numpy's pairwise order, NaN propagated); kind 5 evaluates pow in fp64, within a few ulp of numpy.
+ * Sinkhorn: element-wise expressions in the arrays' precision and the reference's order, the two reductions in fp64
+ * -- agreement with numpy to rounding; the iteration count is the reference's, a NaN change never counting as
+ * converged (tests/test_dense_metrics.py states the tolerances). */
 int pcu_b200_pairwise_distances_f32(pcu_b200_workspace* ws, const float* a, const float* b, int64_t nb, int64_t n, int64_t m, int d,
                                     int norm_kind, double p, float* out, void* stream);
 int pcu_b200_pairwise_distances_f64(pcu_b200_workspace* ws, const double* a, const double* b, int64_t nb, int64_t n, int64_t m, int d,

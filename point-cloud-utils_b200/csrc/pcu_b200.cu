@@ -1683,6 +1683,10 @@ int voxel_downsample_dispatch(pcu_b200_workspace* ws, const T* pts, long long n,
 }
 
 // ---- dense pairwise distances, Sinkhorn (SURVEY.md 8f N4) ------------------------------------------------
+// gridDim.y and gridDim.z stop at 65535: the dense kernels take rows and batches there, so larger problems are
+// launched in chunks of that many, the pointers offset to each chunk's first row or batch.
+constexpr long long kMaxGridYZ = 65535;
+
 template <typename T>
 int pairwise_device(pcu_b200_workspace* ws, const T* a, const T* b, long long nb, long long n, long long m, int d, int norm_kind,
                     double p, T* out, cudaStream_t stream) {
@@ -1690,9 +1694,13 @@ int pairwise_device(pcu_b200_workspace* ws, const T* a, const T* b, long long nb
     if (!a || !b || !out) return fail(PCU_B200_INVALID_ARGUMENT, "null pointer");
     if (nb <= 0 || n <= 0 || m <= 0 || d <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid shape: a and b must be [m, n, d] or [n, d] with positive sizes");
     if (norm_kind < kNorm2 || norm_kind > kNormP) return fail(PCU_B200_INVALID_ARGUMENT, "unknown norm");
-    if (nb > 65535 || n > 65535) return fail(PCU_B200_INVALID_ARGUMENT, "pairwise_distances: at most 65535 batches and rows per launch");
     PCU_ON_DEVICE(ws);
-    PCU_LAUNCH((pairwise_kernel<T>), dim3(blocks_for(m), (unsigned)n, (unsigned)nb), kThreads, stream, a, b, n, m, d, norm_kind, p, out);
+    for (long long b0 = 0; b0 < nb; b0 += kMaxGridYZ)
+        for (long long i0 = 0; i0 < n; i0 += kMaxGridYZ) {
+            const dim3 grid(blocks_for(m), (unsigned)std::min(n - i0, kMaxGridYZ), (unsigned)std::min(nb - b0, kMaxGridYZ));
+            PCU_LAUNCH((pairwise_kernel<T>), grid, kThreads, stream, a + (b0 * n + i0) * d, b + b0 * m * d, n, m, d, norm_kind, p,
+                       out + (b0 * n + i0) * m);
+        }
     return PCU_B200_OK;
 }
 
@@ -1705,7 +1713,6 @@ int sinkhorn_device(pcu_b200_workspace* ws, const T* a, const T* b, const T* M, 
     if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
     if (!a || !b || !M || !out_P) return fail(PCU_B200_INVALID_ARGUMENT, "null pointer");
     if (nb <= 0 || n <= 0 || m <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Got unexpected shape for M, should be [nb, m, n] with positive sizes");
-    if (nb > 65535 || n > 65535) return fail(PCU_B200_INVALID_ARGUMENT, "sinkhorn: at most 65535 batches and rows per launch");
     if (max_iters < 0) return fail(PCU_B200_INVALID_ARGUMENT, "max_iters must be >= 0");
     PCU_ON_DEVICE(ws);
     T *u, *v; double *eu, *ev; int* flags;
@@ -1722,11 +1729,24 @@ int sinkhorn_device(pcu_b200_workspace* ws, const T* a, const T* b, const T* M, 
     if (out_cost) PCU_CUDA(cudaMemsetAsync(out_cost, 0, sizeof(double) * nb, stream));
     const T e = (T)eps;
     for (int it = 0; it < max_iters; ++it) {
-        PCU_LAUNCH((sinkhorn_half_kernel<T, false>), dim3((unsigned)n, (unsigned)nb), kThreads, stream, M, a, v, u, n, m, e, eu, flags);
-        PCU_LAUNCH((sinkhorn_half_kernel<T, true>), dim3((unsigned)((m + 31) / 32), (unsigned)nb), kThreads, stream, M, b, u, v, m, n, e, ev, flags);
+        for (long long b0 = 0; b0 < nb; b0 += kMaxGridYZ) {
+            const unsigned nbc = (unsigned)std::min(nb - b0, kMaxGridYZ);
+            PCU_LAUNCH((sinkhorn_half_kernel<T, false>), dim3((unsigned)n, nbc), kThreads, stream, M + b0 * n * m, a + b0 * n, v + b0 * m,
+                       u + b0 * n, n, m, e, eu + b0, flags);
+        }
+        for (long long b0 = 0; b0 < nb; b0 += kMaxGridYZ) {
+            const unsigned nbc = (unsigned)std::min(nb - b0, kMaxGridYZ);
+            PCU_LAUNCH((sinkhorn_half_kernel<T, true>), dim3((unsigned)((m + 31) / 32), nbc), kThreads, stream, M + b0 * n * m, b + b0 * m,
+                       u + b0 * n, v + b0 * m, m, n, e, ev + b0, flags);
+        }
         PCU_LAUNCH(sinkhorn_check_kernel, 1, kThreads, stream, eu, ev, nb, stop_thresh, flags, flags + 1);
     }
-    PCU_LAUNCH((sinkhorn_plan_kernel<T>), dim3(blocks_for(m), (unsigned)n, (unsigned)nb), kThreads, stream, M, u, v, n, m, e, out_P, out_cost);
+    for (long long b0 = 0; b0 < nb; b0 += kMaxGridYZ)
+        for (long long i0 = 0; i0 < n; i0 += kMaxGridYZ) {
+            const dim3 grid(blocks_for(m), (unsigned)std::min(n - i0, kMaxGridYZ), (unsigned)std::min(nb - b0, kMaxGridYZ));
+            PCU_LAUNCH((sinkhorn_plan_kernel<T>), grid, kThreads, stream, M + (b0 * n + i0) * m, u + b0 * n + i0, v + b0 * m, n, m, e,
+                       out_P + (b0 * n + i0) * m, out_cost ? out_cost + b0 : nullptr);
+        }
     if (out_iters) PCU_CUDA(cudaMemcpyAsync(out_iters, flags + 1, sizeof(int), cudaMemcpyDeviceToDevice, stream));
     return PCU_B200_OK;
 }

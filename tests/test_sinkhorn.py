@@ -1,10 +1,12 @@
 """Dense metrics (SURVEY.md 8f, N4; /root/reference/point_cloud_utils/_sinkhorn.py:4-156): pairwise_distances,
 sinkhorn, earth_movers_distance.  The golden vectors were produced by the reference's own numpy code
 (oracle/make_golden_sinkhorn.py).  CPU: the restatement reproduces them bit for bit.  GPU: the kernels agree with
-them within the stated tolerances -- pairwise p = 2 / 1 / inf / -inf / 0 exactly (same rounded operations), general
-p to 4 ulp (pow); the Sinkhorn plan to 2e-3 relative in float32 and 1e-9 in float64 (the potentials enter the plan
-divided by eps, which amplifies the rounding of the two reductions -- numpy sums pairwise in the array's precision,
-the kernels accumulate in fp64 -- by 1 / eps)."""
+them within the stated tolerances -- pairwise p = 2 / 1 / inf / -inf / 0 exactly (same rounded operations, summed in
+numpy's pairwise order, which for these d = 3 goldens is a plain sequential sum), general p to a relative 5e-7 /
+1e-15 (pow is evaluated in fp64 on the device, in the array's precision by numpy); the Sinkhorn plan to 2e-3 relative
+in float32 and 1e-9 in float64 (the potentials enter the plan divided by eps, which amplifies the rounding of the two
+reductions -- numpy sums pairwise in the array's precision, the kernels accumulate in fp64 -- by 1 / eps).
+tests/test_dense_metrics.py covers d >= 8, non-finite inputs, edge shapes and the iteration count."""
 import numpy as np
 import pytest
 
