@@ -11,7 +11,7 @@
 
 namespace pcu {
 
-constexpr int kMaxRing = 2;   // rings the in-kernel slow path walks before a query goes to the pyramid descent
+constexpr int kMaxRing = 2;   // rings the far pass examines before a query goes to the pyramid descent
 
 // Per-thread table of the 9 rows (fixed y, z; three x-adjacent cells = one contiguous run of the
 // sorted dataset) of a query's 3 x 3 x 3 neighbourhood, nearest rows first.  Indexed [row][thread]
@@ -92,6 +92,57 @@ __device__ __forceinline__ bool warp_ring_search(const GridHeader<T>& g, const C
         if (xa == 0 && ya == 0 && za == 0 && xb == g.dim[0] - 1 && yb == g.dim[1] - 1 && zb == g.dim[2] - 1) return true;
     }
     return false;
+}
+
+// Warp-cooperative search of ONE query's whole (2r + 1)^3 window of cells in a single round: one (y, z) row per
+// lane, each row's x-run [cx - r, cx + r] (x-adjacent cells are one contiguous run of the sorted dataset) scanned
+// whole with four candidate loads in flight, then one merge and one check of the window's wall bound.  The window
+// is the union of rings 0 .. r and no row is skipped, so what it settles is exactly what warp_ring_search settles
+// with r rings (DESIGN.md "why the grid search is exact"), in one dependent round instead of r + 1.  Returns true
+// when the bound closed or the window covers the grid; all lanes return the same best.
+template <typename T>
+__device__ __forceinline__ bool warp_window_search(const GridHeader<T>& g, const Cloud<T>& dc, const Pt<T>& q, int lane,
+                                                   int r, Best1<T>& best) {
+    using R = Real<T>;
+    const int st = g.stride;
+    const int cx = cell_of<T>(q.x, g.origin[0], g.inv_h, g.dim[0]);
+    const int cy = cell_of<T>(q.y, g.origin[1], g.inv_h, g.dim[1]);
+    const int cz = cell_of<T>(q.z, g.origin[2], g.inv_h, g.dim[2]);
+    const int xa = max(cx - r, 0), xb = min(cx + r, g.dim[0] - 1);
+    const int ya = max(cy - r, 0), yb = min(cy + r, g.dim[1] - 1);
+    const int za = max(cz - r, 0), zb = min(cz + r, g.dim[2] - 1);
+    // the window's wall bound first, so that its loads are in flight while the rows are scanned
+    T lb = sq_gap<T>(q.x, dc.wall_lo[xa]);
+    lb = R::vmin(lb, sq_gap<T>(q.x, dc.wall_hi[xb + 1]));
+    lb = R::vmin(lb, sq_gap<T>(q.y, dc.wall_lo[st + ya]));
+    lb = R::vmin(lb, sq_gap<T>(q.y, dc.wall_hi[st + yb + 1]));
+    lb = R::vmin(lb, sq_gap<T>(q.z, dc.wall_lo[2 * st + za]));
+    lb = R::vmin(lb, sq_gap<T>(q.z, dc.wall_hi[2 * st + zb + 1]));
+    best.d = R::inf(); best.i = no_index<T>(); best.tie = false;
+    const int ny = yb - ya + 1, nrows = ny * (zb - za + 1);
+    for (int idx = lane; idx < nrows; idx += 32) {
+        const int z = za + idx / ny, y = ya + idx % ny;
+        const unsigned base = (unsigned)((z * g.dim[1] + y) * g.dim[0]);
+        const unsigned a = dc.cell_start[base + xa], b = dc.cell_start[base + xb + 1];
+        for (unsigned j = a; j < b; j += 4) {
+            Pt<T> p[4];
+#pragma unroll
+            for (int u = 0; u < 4; ++u) p[u] = load_pt<T>(dc.sorted + min(j + u, b - 1));
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                offer1_select<T>(best, dist2<T>(q.x, q.y, q.z, p[u].x, p[u].y, p[u].z), p[u].i, j + u < b);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        Best1<T> other;
+        other.d = __shfl_xor_sync(0xffffffffu, best.d, o);
+        other.i = __shfl_xor_sync(0xffffffffu, best.i, o);
+        other.tie = __shfl_xor_sync(0xffffffffu, (int)best.tie, o) != 0;
+        merge_best<T>(best, other);
+    }
+    return best.d < lb ||
+           (xa == 0 && ya == 0 && za == 0 && xb == g.dim[0] - 1 && yb == g.dim[1] - 1 && zb == g.dim[2] - 1);
 }
 
 // Main pass: one thread per (cell-sorted) query.
@@ -224,8 +275,8 @@ __global__ void __launch_bounds__(kThreads, sizeof(T) == 4 ? 6 : 4) nn1_kernel(c
         if (!settled) sw.far_list[atomicAdd(sw.counters, 1u)] = (unsigned)t;
     }
     double sum = 0.0, sumsq = 0.0;
-    MaxCand<T> mc; mc.d2 = (T)-1; mc.q = 0xffffffffu; mc.pos = 0u;
-    finish_query1<T, kOut, kStats>(sw, active && settled, best, row, (unsigned)t, sum, sumsq, mc);
+    MaxCand<T> mc = no_max<T>();
+    finish_query1<T, kOut, kStats>(sw, active && settled, best, row, (unsigned)t, kWitnessUnknown, sum, sumsq, mc);
     if (kStats) block_reduce_stats<T>(sum, sumsq, mc, sw.partial + blockIdx.x);
 }
 
@@ -235,7 +286,9 @@ template <typename T> __device__ void conclude_sweep(const Sweep<T>& sw, const C
 template <typename T> __device__ __forceinline__ SweepPartial<T> load_partial(const SweepPartial<T>* src);
 
 // Slow pass for the queries the 3 x 3 x 3 neighbourhood could not settle (empty surroundings): one
-// WARP per query (warp_ring_search); what even kMaxRing rings cannot settle goes to the very-far list.
+// WARP per query, which scans the kMaxRing window in one round (warp_window_search; rings 0 and 1 alone cannot
+// settle such a query, the main pass has just found so); what the window cannot settle goes to the very-far list.
+// Every query it answers carries its witness (neighbour, tie flag) into the statistics.
 // Its CTAs also fold the main pass's per-block statistics partials into their own (slot s belongs to
 // CTA s mod gridDim), so the CTA that finishes last has only far_blocks partials left to combine: if the
 // very-far list is empty -- the rule on overlapping clouds -- it concludes the sweep right here
@@ -253,16 +306,16 @@ __global__ void __launch_bounds__(kThreads) nn1_far_kernel(const __grid_constant
     const unsigned warps_total = gridDim.x * (kThreads / 32);
     if (blockIdx.x == 0 && threadIdx.x == 0) publish_far_hint<T>(dc, n_far, qc.n);
     double sum = 0.0, sumsq = 0.0;
-    MaxCand<T> mc; mc.d2 = (T)-1; mc.q = 0xffffffffu; mc.pos = 0u;
+    MaxCand<T> mc = no_max<T>();
     if (n_far > 0) {
         const GridHeader<T> g = *dc.grid;
         for (unsigned f = blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); f < n_far; f += warps_total) {
             const unsigned qt = sw.far_list[f];
             const Pt<T> q = load_pt<T>(qc.sorted + qt);
             Best1<T> best;
-            const bool ok = warp_ring_search<T>(g, dc, q, lane, best);
+            const bool ok = warp_window_search<T>(g, dc, q, lane, kMaxRing, best);
             if (!ok && lane == 0) sw.vfar_list[atomicAdd(sw.counters + 2, 1u)] = qt;
-            finish_query1<T, kOut, kStats>(sw, ok && lane == 0, best, (long long)q.i, qt, sum, sumsq, mc);
+            finish_query1<T, kOut, kStats>(sw, ok && lane == 0, best, (long long)q.i, qt, witness_word<T>(best), sum, sumsq, mc);
         }
     }
     if (kStats) {
@@ -270,7 +323,7 @@ __global__ void __launch_bounds__(kThreads) nn1_far_kernel(const __grid_constant
         for (int s = blockIdx.x + threadIdx.x * gridDim.x; s < main_used; s += gridDim.x * blockDim.x) {
             const SweepPartial<T> p = load_partial<T>(sw.partial + s);
             sum += p.sum; sumsq += p.sumsq;
-            MaxCand<T> c; c.d2 = p.max_d2; c.q = p.arg_q; c.pos = p.arg_pos;
+            MaxCand<T> c; c.d2 = p.max_d2; c.q = p.arg_q; c.pos = p.arg_pos; c.nn = p.arg_nn;
             take_max<T>(mc, c);
         }
         block_reduce_stats<T>(sum, sumsq, mc, sw.partial + sw.main_blocks + blockIdx.x);
@@ -294,7 +347,7 @@ template <typename T>
 __device__ __forceinline__ SweepPartial<T> load_partial(const SweepPartial<T>* src) {
     SweepPartial<T> p;
     p.sum = __ldcg(&src->sum); p.sumsq = __ldcg(&src->sumsq); p.max_d2 = __ldcg(&src->max_d2);
-    p.arg_q = __ldcg(&src->arg_q); p.arg_pos = __ldcg(&src->arg_pos);
+    p.arg_q = __ldcg(&src->arg_q); p.arg_pos = __ldcg(&src->arg_pos); p.arg_nn = __ldcg(&src->arg_nn);
     return p;
 }
 
@@ -303,11 +356,11 @@ __device__ __forceinline__ SweepPartial<T> load_partial(const SweepPartial<T>* s
 template <typename T>
 __device__ __forceinline__ void finalize_sweep(const Sweep<T>& sw, SweepPartial<T>* result /* shared */, int total) {
     double sum = 0.0, sumsq = 0.0;
-    MaxCand<T> mc; mc.d2 = (T)-1; mc.q = 0xffffffffu; mc.pos = 0u;
+    MaxCand<T> mc = no_max<T>();
     for (int s = threadIdx.x; s < total; s += blockDim.x) {
         const SweepPartial<T> p = load_partial<T>(sw.partial + sw.main_blocks + s);
         sum += p.sum; sumsq += p.sumsq;
-        MaxCand<T> c; c.d2 = p.max_d2; c.q = p.arg_q; c.pos = p.arg_pos;
+        MaxCand<T> c; c.d2 = p.max_d2; c.q = p.arg_q; c.pos = p.arg_pos; c.nn = p.arg_nn;
         take_max<T>(mc, c);
     }
     block_reduce_stats<T>(sum, sumsq, mc, result);

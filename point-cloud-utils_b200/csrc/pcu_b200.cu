@@ -394,6 +394,7 @@ struct PlanSpec {
     pcu_b200_nn_stats* stats = nullptr;   // caller's device buffer, or null -> carved from the arena
     T* value_out = nullptr;               // per-pair Chamfer values (nsweeps == 2), or null
     long long replay_points = 0;
+    int sm_count = 0;                     // the device's SMs (prepare_plan): sizes the far pass
 };
 
 // Scratch layout of one call.  Every per-cloud / per-sweep buffer is an array over the batch with
@@ -447,8 +448,8 @@ struct Plan {
         max_n = std::max(sp.n, sp.m);
         max_cap = 0;
         max_bbox_blocks = 1;
-        // far pass: a fixed number of CTAs per sweep (warp-stride loop over the far list)
-        far_blocks = (int)std::max<long long>(4, 296 / std::max<long long>(1, B * sp.nsweeps));
+        // far pass (warp-stride loop over the far list): two CTAs per SM over all sweeps, at least four per sweep
+        far_blocks = (int)std::max<long long>(4, 2LL * sp.sm_count / std::max<long long>(1, B * sp.nsweeps));
         // zeroed region first: cell counters and sweep counters
         const size_t zero_from = cv.off;
         for (int s = 0; s < 2; ++s) {
@@ -619,6 +620,7 @@ void apply_grid_feedback(pcu_b200_workspace* ws, PlanSpec<T>& spec) {
 template <typename T>
 int prepare_plan(pcu_b200_workspace* ws, Plan<T>& plan, PlanSpec<T>& spec, cudaStream_t stream) {
     apply_grid_feedback(ws, spec);
+    spec.sm_count = ws->sm_count;
     return carve_scratch(ws, kArena, stream, [&](Carver& cv) { plan.layout(cv, spec); });
 }
 

@@ -113,10 +113,12 @@ __device__ __forceinline__ void load_shapes(const Cloud<T>& dc, GridHeader<T>& g
 
 // Last step of a statistics sweep, run by ONE CTA once every partial of the sweep is in memory: folds the
 // `nparts` per-CTA partials of the slow passes (which carry the main pass's partials, folded in by
-// nn1_far_kernel) into the caller's pcu_b200_nn_stats, recovers the Hausdorff witness -- the neighbour of
-// the one query that attains the maximum, and whether it was decided by tie order: a single warp repeats
-// that query's search with full bookkeeping -- and, for a bidirectional call, lets the sweep that
-// finishes second write the pair's Chamfer value.
+// nn1_far_kernel) into the caller's pcu_b200_nn_stats, takes the Hausdorff witness -- the neighbour of the
+// one query that attains the maximum, and whether it was decided by tie order -- and, for a bidirectional
+// call, lets the sweep that finishes second write the pair's Chamfer value.
+// A maximum answered by the far or the very-far pass carries its witness.  One answered by the main pass
+// was settled inside its 3 x 3 x 3 cells, so a single warp finds the witness in one round over their 9 rows;
+// the ring walk and the pyramid descent stay behind that round for whatever it cannot settle.
 template <typename T>
 __device__ void conclude_sweep(const Sweep<T>& sw, const Cloud<T>& qc, const Cloud<T>& dc, int nparts) {
     using R = Real<T>;
@@ -127,17 +129,23 @@ __device__ void conclude_sweep(const Sweep<T>& sw, const Cloud<T>& qc, const Clo
     if (threadIdx.x == 0) wg = *dc.grid;
     __syncthreads();
     if (threadIdx.x < 32 && result.max_d2 >= (T)0) {
-        const Pt<T> wq = load_pt<T>(qc.sorted + result.arg_pos);
         Best1<T> wb; wb.d = R::inf(); wb.i = no_index<T>(); wb.tie = false;
-        const bool ok = warp_ring_search<T>(wg, dc, wq, threadIdx.x, wb);
-        if (!ok) {   // beyond the rings: the pyramid exists (this query was on the very-far list)
-            wb.d = R::inf(); wb.i = no_index<T>(); wb.tie = false;
-            for (int w = threadIdx.x; w < (int)(sizeof(PyramidShape) / sizeof(int)); w += 32)
-                reinterpret_cast<int*>(&wps)[w] = reinterpret_cast<const int*>(dc.shape)[w];
-            __syncwarp();
-            if (threadIdx.x == 0)
-                pyramid_descend<T>(wg, wps, dc, wq, [&]() { return wb.d; },
-                                   [&](unsigned a, unsigned b) { scan_run1<T>(dc.sorted, a, b, wq.x, wq.y, wq.z, wb); });
+        if (result.arg_nn != kWitnessUnknown) {
+            const unsigned nn = result.arg_nn & kWitnessNone;
+            wb.i = nn == kWitnessNone ? no_index<T>() : (typename Real<T>::index_t)nn;
+            wb.tie = (result.arg_nn >> 31) != 0u;
+        } else {
+            const Pt<T> wq = load_pt<T>(qc.sorted + result.arg_pos);
+            if (!warp_window_search<T>(wg, dc, wq, threadIdx.x, 1, wb) && !warp_ring_search<T>(wg, dc, wq, threadIdx.x, wb)) {
+                // beyond the rings: the pyramid exists (this query was on the very-far list)
+                wb.d = R::inf(); wb.i = no_index<T>(); wb.tie = false;
+                for (int w = threadIdx.x; w < (int)(sizeof(PyramidShape) / sizeof(int)); w += 32)
+                    reinterpret_cast<int*>(&wps)[w] = reinterpret_cast<const int*>(dc.shape)[w];
+                __syncwarp();
+                if (threadIdx.x == 0)
+                    pyramid_descend<T>(wg, wps, dc, wq, [&]() { return wb.d; },
+                                       [&](unsigned a, unsigned b) { scan_run1<T>(dc.sorted, a, b, wq.x, wq.y, wq.z, wb); });
+            }
         }
         if (threadIdx.x == 0) {
             pcu_b200_nn_stats st;
@@ -199,7 +207,7 @@ __global__ void __launch_bounds__(kThreads) nn1_vfar_kernel(const __grid_constan
     const Cloud<T> qc = clouds[sw.qcloud];
     const Cloud<T> dc = clouds[sw.dcloud];
     double sum = 0.0, sumsq = 0.0;
-    MaxCand<T> mc; mc.d2 = (T)-1; mc.q = 0xffffffffu; mc.pos = 0u;
+    MaxCand<T> mc = no_max<T>();
     {
         __shared__ GridHeader<T> g;
         __shared__ PyramidShape ps;
@@ -210,7 +218,7 @@ __global__ void __launch_bounds__(kThreads) nn1_vfar_kernel(const __grid_constan
             Best1<T> best; best.d = R::inf(); best.i = no_index<T>(); best.tie = false;
             pyramid_descend<T>(g, ps, dc, q, [&]() { return best.d; },
                                [&](unsigned a, unsigned b) { scan_run1<T>(dc.sorted, a, b, q.x, q.y, q.z, best); });
-            finish_query1<T, kOut, kStats>(sw, true, best, (long long)q.i, sw.vfar_list[f], sum, sumsq, mc);
+            finish_query1<T, kOut, kStats>(sw, true, best, (long long)q.i, sw.vfar_list[f], witness_word<T>(best), sum, sumsq, mc);
         }
     }
     if (kStats) {

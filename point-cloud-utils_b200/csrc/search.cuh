@@ -24,6 +24,7 @@ struct SweepPartial {
     T max_d2;
     unsigned arg_q;     // caller-order row of the query attaining max_d2 (first one)
     unsigned arg_pos;   // its position in cell order (the witness search starts from there)
+    unsigned arg_nn;    // its witness word (witness_word) when the pass that answered it knew it, else kWitnessUnknown
 };
 
 // One query-cloud -> dataset-cloud direction.
@@ -70,6 +71,17 @@ struct Best1 {
 template <typename T> __device__ __forceinline__ typename Real<T>::index_t no_index();
 template <> __device__ __forceinline__ int32_t no_index<float>() { return 0x7fffffff; }
 template <> __device__ __forceinline__ long long no_index<double>() { return 0x7fffffffffffffffLL; }
+
+// The Hausdorff witness of one answered query in one word: the neighbour's index in bits 0-30 (clouds hold fewer
+// than 2^31 points; kWitnessNone when no point was found) and, in bit 31, whether tie order decided it.  A Best1
+// without a neighbour never has its tie flag set, so no witness word equals kWitnessUnknown, which the main
+// statistics pass writes: it tracks distances only.
+constexpr unsigned kWitnessUnknown = 0xffffffffu;
+constexpr unsigned kWitnessNone = 0x7fffffffu;
+template <typename T>
+__device__ __forceinline__ unsigned witness_word(const Best1<T>& b) {
+    return (b.i == no_index<T>() ? kWitnessNone : (unsigned)b.i) | (b.tie ? 0x80000000u : 0u);
+}
 
 template <typename T>
 __device__ __forceinline__ void offer1(Best1<T>& b, T d, typename Real<T>::index_t i) {
@@ -160,10 +172,17 @@ struct MaxCand {
     T d2;           // -1: neutral element
     unsigned q;     // caller-order row (clouds are limited to 2^31 - 1 points)
     unsigned pos;   // position in cell order
+    unsigned nn;    // witness word of the query, or kWitnessUnknown
 };
 template <typename T>
+__device__ __forceinline__ MaxCand<T> no_max() {
+    MaxCand<T> mc; mc.d2 = (T)-1; mc.q = 0xffffffffu; mc.pos = 0u; mc.nn = kWitnessUnknown;
+    return mc;
+}
+template <typename T>
 __device__ __forceinline__ void take_max(MaxCand<T>& a, const MaxCand<T>& b) {
-    // larger distance wins; equal distance -> lower query row (Eigen maxCoeff: first maximum)
+    // larger distance wins; equal distance -> lower query row (Eigen maxCoeff: first maximum); the witness
+    // travels with the winner
     if (b.d2 > a.d2 || (b.d2 == a.d2 && b.q < a.q)) a = b;
 }
 
@@ -176,6 +195,7 @@ __device__ __forceinline__ MaxCand<T> warp_take_max(MaxCand<T> mc) {
         other.d2 = __shfl_xor_sync(0xffffffffu, mc.d2, o);
         other.q = __shfl_xor_sync(0xffffffffu, mc.q, o);
         other.pos = __shfl_xor_sync(0xffffffffu, mc.pos, o);
+        other.nn = __shfl_xor_sync(0xffffffffu, mc.nn, o);
         take_max<T>(mc, other);
     }
     return mc;
@@ -197,6 +217,7 @@ __device__ __forceinline__ MaxCand<float> warp_take_max<float>(MaxCand<float> mc
     out.d2 = __uint_as_float(top);
     out.q = first;
     out.pos = __shfl_sync(0xffffffffu, mc.pos, src);
+    out.nn = __shfl_sync(0xffffffffu, mc.nn, src);
     return out;
 }
 
@@ -219,7 +240,7 @@ __device__ __forceinline__ void block_reduce_stats(double sum, double sumsq, Max
             take_max<T>(mc, s_mc[i]);
         }
         SweepPartial<T> p;
-        p.sum = sum; p.sumsq = sumsq; p.max_d2 = mc.d2; p.arg_q = mc.q; p.arg_pos = mc.pos;
+        p.sum = sum; p.sumsq = sumsq; p.max_d2 = mc.d2; p.arg_q = mc.q; p.arg_pos = mc.pos; p.arg_nn = mc.nn;
         *out = p;
     }
 }
@@ -227,10 +248,11 @@ __device__ __forceinline__ void block_reduce_stats(double sum, double sumsq, Max
 // kOut: write the query's neighbour to the caller's arrays.  kStats: fold its distance into the fused
 // statistics.  In the statistics-only sweeps the hot loop tracks the minimum distance and nothing else:
 // the only index the scalar metrics ever need is the neighbour of the ONE query that attains the
-// Hausdorff maximum, and that is recovered afterwards by one warp (last CTA of the pyramid pass).
+// Hausdorff maximum.  The slow passes know it and carry it with the maximum (`witness`: witness_word(best));
+// the main pass passes kWitnessUnknown and conclude_sweep recovers it with one warp.
 template <typename T, bool kOut, bool kStats>
 __device__ __forceinline__ void finish_query1(const Sweep<T>& sw, bool have, const Best1<T>& best, long long row,
-                                              unsigned pos, double& sum, double& sumsq, MaxCand<T>& mc) {
+                                              unsigned pos, unsigned witness, double& sum, double& sumsq, MaxCand<T>& mc) {
     using R = Real<T>;
     if (!have) return;
     const T root = R::root(best.d);
@@ -243,7 +265,7 @@ __device__ __forceinline__ void finish_query1(const Sweep<T>& sw, bool have, con
     if (kStats) {
         sum += (double)root;
         sumsq += (double)best.d;
-        MaxCand<T> c; c.d2 = best.d; c.q = (unsigned)row; c.pos = pos;
+        MaxCand<T> c; c.d2 = best.d; c.q = (unsigned)row; c.pos = pos; c.nn = witness;
         take_max<T>(mc, c);
     }
 }
