@@ -469,6 +469,44 @@ int pcu_b200_ray_mesh_intersection_prepared_f64(pcu_b200_workspace* ws, const pc
                                                 const double* d, int64_t n, float near, float far, int32_t* out_fidx, double* out_bc,
                                                 double* out_t, void* stream);
 
+/* ---- rays against surfels -----------------------------------------------------------------------------------------
+ * Replace ray_surfel_intersection, RaySurfelIntersector and pointcloud_surfel_geometry (src/ray_point_cloud_intersection.cpp,
+ * "circle" geometry).  Point i (np points, 0 <= np < 2^31 - 1) is a disk of radius r[i] around p[i] facing n[i], drawn
+ * as a fan of s = subdivs triangles (4 <= s <= 2^24): rim vertex j at angle theta_j = 2 pi j / s in the reference's
+ * basis, computed in fp32 op by op, with fl32(cos theta_j) and fl32(sin theta_j) from the C library (DESIGN.md §3).
+ * For each ray (as for rays against a mesh): out_pid[i] (int32) and out_t[i] of the point that minimises (t, point id)
+ * over the fan triangles hit with near < t <= far, by the same fp32 watertight test.  Misses, invalid rays, np = 0 and
+ * points whose fan has a non-finite coordinate (a zero normal, non-finite p or r) give pid = -1, t = +inf.
+ *   ray_surfel_intersection: builds the surfel tree for the call.
+ *   surfel_prepare: builds it once into a private device block (*out_surfels, a pcu_b200_mesh handle freed by
+ *     pcu_b200_mesh_destroy; pcu_b200_mesh_size is np).
+ *   ray_surfel_intersection_prepared: rays of either precision (the suffix is the rays') against prepared surfels of
+ *     either precision.  Results equal ray_surfel_intersection's on the same input.
+ *   pointcloud_surfel_geometry: the fans as a mesh: out_v ((s + 1) np rows, rim j of point i at i (s + 1) + j, the
+ *     centre at i (s + 1) + s) in p's precision, and out_f (s np rows (centre, rim j, rim (j + 1) mod s)) int32;
+ *     (s + 1) np must be below 2^31 - 1.
+ * Every array pointer is a DEVICE pointer and the calls are stream-ordered. */
+int pcu_b200_ray_surfel_intersection_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* r, int64_t np, int subdivs,
+                                         const float* o, int o_stride, const float* d, int64_t nr, float near, float far, int32_t* out_pid,
+                                         float* out_t, void* stream);
+int pcu_b200_ray_surfel_intersection_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np, int subdivs,
+                                         const double* o, int o_stride, const double* d, int64_t nr, float near, float far, int32_t* out_pid,
+                                         double* out_t, void* stream);
+int pcu_b200_surfel_prepare_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* r, int64_t np, int subdivs,
+                                pcu_b200_mesh** out_surfels, void* stream);
+int pcu_b200_surfel_prepare_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np, int subdivs,
+                                pcu_b200_mesh** out_surfels, void* stream);
+int pcu_b200_ray_surfel_intersection_prepared_f32(pcu_b200_workspace* ws, const pcu_b200_mesh* surfels, const float* o, int o_stride,
+                                                  const float* d, int64_t nr, float near, float far, int32_t* out_pid, float* out_t,
+                                                  void* stream);
+int pcu_b200_ray_surfel_intersection_prepared_f64(pcu_b200_workspace* ws, const pcu_b200_mesh* surfels, const double* o, int o_stride,
+                                                  const double* d, int64_t nr, float near, float far, int32_t* out_pid, double* out_t,
+                                                  void* stream);
+int pcu_b200_pointcloud_surfel_geometry_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* r, int64_t np, int subdivs,
+                                            float* out_v, int32_t* out_f, void* stream);
+int pcu_b200_pointcloud_surfel_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np,
+                                            int subdivs, double* out_v, int32_t* out_f, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

@@ -637,6 +637,51 @@ void ray_mesh_prepared_device(bool is_f64, uintptr_t mesh, uintptr_t o, int o_st
     });
 }
 
+// Rays against surfels (ray_surfel_intersection, _ray_surfel.py); r holds np radii in p's dtype; out_pid is int32.
+void ray_surfel_intersection_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t r, int64_t np, int subdivs, uintptr_t o,
+                                    int o_stride, uintptr_t d, int64_t nr, float near, float far, uintptr_t out_pid, uintptr_t out_t,
+                                    int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_ray_surfel_intersection_f64(ws, (const double*)p, (const double*)n, (const double*)r, np, subdivs,
+                                                             (const double*)o, o_stride, (const double*)d, nr, near, far,
+                                                             (int32_t*)out_pid, (double*)out_t, (void*)stream)
+                      : pcu_b200_ray_surfel_intersection_f32(ws, (const float*)p, (const float*)n, (const float*)r, np, subdivs,
+                                                             (const float*)o, o_stride, (const float*)d, nr, near, far,
+                                                             (int32_t*)out_pid, (float*)out_t, (void*)stream);
+    });
+}
+// Prepared surfels (RaySurfelIntersector); freed by _mesh_destroy.
+uintptr_t surfel_prepare_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t r, int64_t np, int subdivs, int device, uintptr_t stream) {
+    pcu_b200_mesh* h = nullptr;
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_surfel_prepare_f64(ws, (const double*)p, (const double*)n, (const double*)r, np, subdivs, &h, (void*)stream)
+                      : pcu_b200_surfel_prepare_f32(ws, (const float*)p, (const float*)n, (const float*)r, np, subdivs, &h, (void*)stream);
+    });
+    return (uintptr_t)h;
+}
+// Rays of precision is_f64 against prepared surfels of either precision.
+void ray_surfel_prepared_device(bool is_f64, uintptr_t surfels, uintptr_t o, int o_stride, uintptr_t d, int64_t nr, float near, float far,
+                                uintptr_t out_pid, uintptr_t out_t, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_ray_surfel_intersection_prepared_f64(ws, (const pcu_b200_mesh*)surfels, (const double*)o, o_stride,
+                                                                      (const double*)d, nr, near, far, (int32_t*)out_pid, (double*)out_t,
+                                                                      (void*)stream)
+                      : pcu_b200_ray_surfel_intersection_prepared_f32(ws, (const pcu_b200_mesh*)surfels, (const float*)o, o_stride,
+                                                                      (const float*)d, nr, near, far, (int32_t*)out_pid, (float*)out_t,
+                                                                      (void*)stream);
+    });
+}
+// pointcloud_surfel_geometry: out_v ((subdivs + 1) np, 3) in p's dtype, out_f (subdivs np, 3) int32.
+void surfel_geometry_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t r, int64_t np, int subdivs, uintptr_t out_v, uintptr_t out_f,
+                            int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_pointcloud_surfel_geometry_f64(ws, (const double*)p, (const double*)n, (const double*)r, np, subdivs,
+                                                                (double*)out_v, (int32_t*)out_f, (void*)stream)
+                      : pcu_b200_pointcloud_surfel_geometry_f32(ws, (const float*)p, (const float*)n, (const float*)r, np, subdivs,
+                                                                (float*)out_v, (int32_t*)out_f, (void*)stream);
+    });
+}
+
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
@@ -1036,6 +1081,10 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_mesh_prepare_device", &mesh_prepare_device);
     mod.def("_mesh_destroy", &mesh_destroy);
     mod.def("_ray_mesh_prepared_device", &ray_mesh_prepared_device);
+    mod.def("_ray_surfel_intersection_device", &ray_surfel_intersection_device);
+    mod.def("_surfel_prepare_device", &surfel_prepare_device);
+    mod.def("_ray_surfel_prepared_device", &ray_surfel_prepared_device);
+    mod.def("_surfel_geometry_device", &surfel_geometry_device);
     mod.def("_interpolate_barycentric_device", &interpolate_barycentric_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);

@@ -13,6 +13,8 @@
 //   faces   L = Pt<T>, three per leaf (corners, face id, degeneracy); a face with a corner out of range is invalid: it is
 //           counted in MqScratch::bad and sorts last, out of the tree; leaves have boxes and the nodes are refit
 //   points  L = WnPoint (point_cloud_fast_winding_number, winding.cuh), one per leaf, always valid; no boxes, no refit
+//   surfels L = SfWord (ray_surfel_intersection, raycast.cuh), a whole fp32 fan per leaf (sf_fan); a fan with a
+//           non-finite coordinate is invalid, counted and left out as a face is; leaves have boxes and the nodes are refit
 // The passes:
 //   mq_bounds_kernel    scene box of the leaves' boxes (a point's box is the point), count of invalid faces
 //   mq_codes_kernel     63-bit Morton code of each face's box centre or each fp32 point over the scene box (invalid
@@ -59,6 +61,114 @@ static_assert(sizeof(WnPoint) == 32, "two float4 per point");
 
 template <typename L>
 constexpr bool kPointLeaf = std::is_same<L, WnPoint>::value;
+
+// 16 bytes of a surfel leaf of ray_surfel_intersection (raycast.cuh).  Leaf l is sf_words(s) words from word
+// l sf_words(s): its fan's s + 1 fp32 vertices (the centre, then rim 0 .. s - 1), x y z each, zero-padded to whole
+// words (96 B at s = 7); its point id lives in MeshTree::ids.  A surfel whose fan has a non-finite coordinate is
+// counted in MqScratch::bad and sorts last, out of the tree, as an invalid face does.
+struct __align__(16) SfWord { float x[4]; };
+
+template <typename L>
+constexpr bool kSurfelLeaf = std::is_same<L, SfWord>::value;
+
+__host__ __device__ __forceinline__ long long sf_words(int s) { return (3ll * (s + 1) + 3) / 4; }
+
+// What a surfel fan is computed from: normals and radii (T, as the points), s and the table cs[2 j] = fl32(cos
+// theta_j), cs[2 j + 1] = fl32(sin theta_j), computed on the host (DESIGN.md §3, ray-surfel casting).  During a tree
+// build `boxes` holds each surfel's box in input order: mq_bounds_kernel writes it (lo[0] = NaN for a non-finite
+// fan) and mq_codes_kernel reads it, so the fan is not computed again there.
+struct SfSrc {
+    const void* n;
+    const void* r;
+    const float* cs;
+    MqBox* boxes;
+    int s;
+};
+
+// Moves the host-computed table (and the SfSrc record, for the bounds and codes passes) to the device through kernel
+// parameters, so no host buffer is copied: each launch writes `count` <= kSfChunk values of the table at `dst` and,
+// when `dst_src` is set, the record there.
+constexpr int kSfChunk = 960;
+struct SfUpload {
+    SfSrc* dst_src;
+    SfSrc src;
+    float* dst;
+    int count;
+    float v[kSfChunk];
+};
+static_assert(sizeof(SfUpload) <= 4096, "within the kernel parameter limit");
+
+__global__ void __launch_bounds__(kThreads) sf_upload_kernel(const SfUpload u) {
+    for (int k = threadIdx.x; k < u.count; k += blockDim.x) u.dst[k] = u.v[k];
+    if (threadIdx.x == 0 && u.dst_src) *u.dst_src = u.src;
+}
+
+template <typename C> __device__ __forceinline__ C sf_div(C a, C b);
+template <> __device__ __forceinline__ float sf_div<float>(float a, float b) { return __fdiv_rn(a, b); }
+template <> __device__ __forceinline__ double sf_div<double>(double a, double b) { return __ddiv_rn(a, b); }
+
+// a x b, each product and difference rounded on its own.
+template <typename C>
+__device__ __forceinline__ void sf_cross(const C a[3], const C b[3], C out[3]) {
+    using R = Real<C>;
+    out[0] = R::sub(R::mul(a[1], b[2]), R::mul(a[2], b[1]));
+    out[1] = R::sub(R::mul(a[2], b[0]), R::mul(a[0], b[2]));
+    out[2] = R::sub(R::mul(a[0], b[1]), R::mul(a[1], b[0]));
+}
+
+// a / |a|, |a| = sqrt((a0^2 + a1^2) + a2^2).
+template <typename C>
+__device__ __forceinline__ void sf_unit(C a[3]) {
+    using R = Real<C>;
+    const C l = R::root(R::add(R::add(R::mul(a[0], a[0]), R::mul(a[1], a[1])), R::mul(a[2], a[2])));
+    for (int k = 0; k < 3; ++k) a[k] = sf_div<C>(a[k], l);
+}
+
+// Surfel i's fan in the compute precision C (float for rays, T for pointcloud_surfel_geometry): emit(j, x, y, z) for
+// rim vertex j = 0 .. s - 1, then emit(s, p_i) for the centre.  The reference's local_basis and generate_splat_geometry
+// op by op (DESIGN.md §3): n^ = n / |n|; right = n^ x e_x when | |(0 n^_x + 1 n^_y) + 0 n^_z| - 1 | < 1e-5 (in fp64),
+// else n^ x e_y; right and up = n^ x right normalised; x0 = fl32(r_i c_j), y0 = fl32(r_i s_j) with the products in T;
+// row k = ((right_k x0 + up_k y0) + n^_k 0) + p_k.
+template <typename T, typename C, typename F>
+__device__ __forceinline__ void sf_fan(const T* __restrict__ p, const SfSrc& src, long long i, F&& emit) {
+    using R = Real<C>;
+    const T* n = (const T*)src.n;
+    C nh[3] = {(C)n[3 * i], (C)n[3 * i + 1], (C)n[3 * i + 2]};
+    const C c[3] = {(C)p[3 * i], (C)p[3 * i + 1], (C)p[3 * i + 2]};
+    sf_unit<C>(nh);
+    const C dot = R::add(R::add(R::mul((C)0, nh[0]), R::mul((C)1, nh[1])), R::mul((C)0, nh[2]));
+    const bool near_y = fabs((double)fabs(dot) - 1.0) < 1e-5;
+    const C axis[3] = {near_y ? (C)1 : (C)0, near_y ? (C)0 : (C)1, (C)0};
+    C right[3], up[3];
+    sf_cross<C>(nh, axis, right);
+    sf_unit<C>(right);
+    sf_cross<C>(nh, right, up);
+    sf_unit<C>(up);
+    const T ri = ((const T*)src.r)[i];
+    for (int j = 0; j < src.s; ++j) {
+        const float x0 = (float)Real<T>::mul(ri, (T)src.cs[2 * j]), y0 = (float)Real<T>::mul(ri, (T)src.cs[2 * j + 1]);
+        C v[3];
+#pragma unroll
+        for (int k = 0; k < 3; ++k)
+            v[k] = R::add(R::add(R::add(R::mul(right[k], (C)x0), R::mul(up[k], (C)y0)), R::mul(nh[k], (C)0)), c[k]);
+        emit(j, v[0], v[1], v[2]);
+    }
+    emit(src.s, c[0], c[1], c[2]);
+}
+
+// The surfel's fp32 box (the min / max of its fan's vertices); false when a fan coordinate is not finite.
+template <typename T>
+__device__ __forceinline__ bool sf_box(const T* __restrict__ p, const SfSrc& src, long long i, MqBox& bx) {
+    const float inf = __int_as_float(0x7f800000);
+    bool finite = true;
+    for (int k = 0; k < 3; ++k) { bx.lo[k] = inf; bx.hi[k] = -inf; }
+    sf_fan<T, float>(p, src, i, [&](int, float x, float y, float z) {
+        finite = finite && isfinite(x) && isfinite(y) && isfinite(z);
+        bx.lo[0] = fminf(bx.lo[0], x); bx.lo[1] = fminf(bx.lo[1], y); bx.lo[2] = fminf(bx.lo[2], z);
+        bx.hi[0] = fmaxf(bx.hi[0], x); bx.hi[1] = fmaxf(bx.hi[1], y); bx.hi[2] = fmaxf(bx.hi[2], z);
+    });
+    return finite;
+}
 
 struct MqScratch {
     int scene[6];                 // ordered-int images of the scene box (min x y z, max x y z)
@@ -139,6 +249,16 @@ __global__ void __launch_bounds__(kThreads) mq_bounds_kernel(const T* __restrict
     int lo[3] = {INT_MAX, INT_MAX, INT_MAX}, hi[3] = {INT_MIN, INT_MIN, INT_MIN};
     unsigned long long bad = 0;
     for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < m; t += (long long)gridDim.x * blockDim.x) {
+        if constexpr (kSurfelLeaf<L>) {   // v: the points, f: their SfSrc in device memory
+            const SfSrc& src = *(const SfSrc*)f;
+            MqBox bx;
+            const bool finite = sf_box<T>(v, src, t, bx);
+            if (!finite) bx.lo[0] = __int_as_float(0x7fffffff);
+            src.boxes[t] = bx;
+            if (!finite) { ++bad; continue; }
+            for (int k = 0; k < 3; ++k) { lo[k] = min(lo[k], mq_ord(bx.lo[k])); hi[k] = max(hi[k], mq_ord(bx.hi[k])); }
+            continue;
+        }
         double a[3], b[3], c[3];
         if (!mq_leaf_corners<L, T>(v, nv, f, fkind, t, a, b, c)) { ++bad; continue; }
         const MqBox bx = mq_leaf_box<L, T>(a, b, c);
@@ -166,8 +286,14 @@ __global__ void __launch_bounds__(kThreads) mq_codes_kernel(const T* __restrict_
     if (t >= m) return;
     unsigned long long code = ~0ull;
     double a[3], b[3], c[3];
-    if (mq_leaf_corners<L, T>(v, nv, f, fkind, t, a, b, c)) {
-        const MqBox bx = mq_leaf_box<L, T>(a, b, c);
+    MqBox sb;
+    bool surfel = false;
+    if constexpr (kSurfelLeaf<L>) {   // v: the points, f: their SfSrc; the box mq_bounds_kernel stored
+        sb = ((const SfSrc*)f)->boxes[t];
+        surfel = !isnan(sb.lo[0]);
+    }
+    if (kSurfelLeaf<L> ? surfel : mq_leaf_corners<L, T>(v, nv, f, fkind, t, a, b, c)) {
+        const MqBox bx = kSurfelLeaf<L> ? sb : mq_leaf_box<L, T>(a, b, c);
         code = 0;
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
@@ -213,6 +339,50 @@ __global__ void __launch_bounds__(kThreads) mq_leaves_kernel(const T* __restrict
     pb.x = (T)b[0]; pb.y = (T)b[1]; pb.z = (T)b[2]; pb.i = mq_degenerate<T>(a, b, c) ? 1 : 0;
     pc.x = (T)c[0]; pc.y = (T)c[1]; pc.z = (T)c[2]; pc.i = 0;
     leaves[3 * i] = pa; leaves[3 * i + 1] = pb; leaves[3 * i + 2] = pc;
+}
+
+// Surfel leaf i (i < m - bad): its fan in fp32 (layout at SfWord), its point id and its box.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) sf_leaves_kernel(const T* __restrict__ p, const SfSrc src, long long m,
+                                                             const MqScratch* __restrict__ sc, const MqRec* __restrict__ sorted,
+                                                             SfWord* __restrict__ leaves, int* __restrict__ ids,
+                                                             MqBox* __restrict__ boxes) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m - (long long)sc->bad) return;
+    const long long t = (long long)sorted[i].idx;
+    const long long words = sf_words(src.s);
+    float* out = reinterpret_cast<float*>(leaves + i * words);
+    MqBox bx;
+    for (int k = 0; k < 3; ++k) { bx.lo[k] = __int_as_float(0x7f800000); bx.hi[k] = -bx.lo[k]; }
+    sf_fan<T, float>(p, src, t, [&](int j, float x, float y, float z) {   // the fan once: the leaf and its box (sf_box's)
+        const int at = j == src.s ? 0 : 3 * (j + 1);
+        out[at] = x; out[at + 1] = y; out[at + 2] = z;
+        bx.lo[0] = fminf(bx.lo[0], x); bx.lo[1] = fminf(bx.lo[1], y); bx.lo[2] = fminf(bx.lo[2], z);
+        bx.hi[0] = fmaxf(bx.hi[0], x); bx.hi[1] = fmaxf(bx.hi[1], y); bx.hi[2] = fmaxf(bx.hi[2], z);
+    });
+    for (long long k = 3ll * (src.s + 1); k < 4 * words; ++k) out[k] = 0.f;
+    ids[i] = (int)t;
+    boxes[i] = bx;
+}
+
+// pointcloud_surfel_geometry: surfel i's s + 1 vertices at rows i (s + 1) .. (rim j at + j, the centre at + s), in T
+// (the reference's mixed precision: basis and vertices in T, x0 and y0 in fp32), and its s faces (centre, rim j,
+// rim (j + 1) mod s) at rows i s + j.  One thread per point.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) sf_geometry_kernel(const T* __restrict__ p, const SfSrc src, long long m,
+                                                               T* __restrict__ out_v, int* __restrict__ out_f) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m) return;
+    const int s = src.s;
+    const long long base = i * (s + 1);
+    sf_fan<T, T>(p, src, i, [&](int j, T x, T y, T z) {
+        T* o = out_v + 3 * (base + j);
+        o[0] = x; o[1] = y; o[2] = z;
+    });
+    for (int j = 0; j < s; ++j) {
+        int* o = out_f + 3 * (i * s + j);
+        o[0] = (int)(base + s); o[1] = (int)(base + j); o[2] = (int)(base + (j + 1) % s);
+    }
 }
 
 __device__ __forceinline__ int mq_delta(const MqRec* __restrict__ recs, long long n, long long i, unsigned long long ci, long long j) {

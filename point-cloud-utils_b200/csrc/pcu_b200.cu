@@ -9,6 +9,7 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
+#include <cmath>
 #include <cstring>
 #include <functional>
 #include <new>
@@ -244,17 +245,19 @@ struct pcu_b200_cloud {
     KdReplayBuffers<float> kd32{};
     KdReplayBuffers<double> kd64{};
 };
-// A mesh whose tree is built once (pcu_b200_mesh_prepare_*): the tree's header, nodes and leaves (carve_mesh_tree, no
-// far-field data) live in one private device block.
+// A mesh whose tree is built once (pcu_b200_mesh_prepare_*), or a point cloud's surfels (pcu_b200_surfel_prepare_*):
+// the tree's header, nodes and leaves (carve_mesh_tree, no far-field data) live in one private device block.
 struct pcu_b200_mesh {
     int device = 0;
     int is_f64 = 0;
-    long long nf = 0;
+    long long nf = 0;               // faces, or points
+    int subdivs = 0;                // > 0: a surfel tree of fans of this many triangles (leaves SfWord, ids)
     unsigned char* block = nullptr;
     size_t bytes = 0;
     MqScratch* sc = nullptr;
     MqNode* nodes = nullptr;
-    const void* leaves = nullptr;   // Pt<float> or Pt<double> by is_f64
+    const void* leaves = nullptr;   // Pt<float> or Pt<double> by is_f64, or SfWord
+    const int* ids = nullptr;       // surfels: the point id of each leaf
 };
 template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
@@ -1285,33 +1288,71 @@ struct MeshTree {
     MqNode* nodes;
     L* leaves;
     WnNode* wn;   // far-field data per node (with `moments` only)
+    int* ids;     // surfel leaves: the point id of each leaf
 };
 
-// The arrays a built tree is queried through: the header, the nodes, the leaves and, with `moments`, the far-field data.
+// The arrays a built tree is queried through: the header, the nodes, the leaves, with `moments` the far-field data and
+// for surfels (fans of `subdivs` triangles) the leaves' point ids.
 template <typename L>
-void carve_mesh_tree(Carver& cv, long long m, bool moments, MeshTree<L>& t) {
+void carve_mesh_tree(Carver& cv, long long m, bool moments, MeshTree<L>& t, int subdivs = 0) {
     const long long inner = std::max<long long>(1, m - 1);
     t.sc = cv.take<MqScratch>(1);
     t.nodes = cv.take<MqNode>((size_t)inner);
-    t.leaves = cv.take<L>((size_t)(kPointLeaf<L> ? 1 : 3) * m);
+    t.leaves = cv.take<L>((size_t)(kSurfelLeaf<L> ? sf_words(subdivs) : (kPointLeaf<L> ? 1 : 3)) * m);
     t.wn = moments ? cv.take<WnNode>((size_t)inner) : nullptr;
+    t.ids = kSurfelLeaf<L> ? cv.take<int>((size_t)m) : nullptr;
+}
+
+// The surfel table of DESIGN.md §3: theta_j = ((float)j / ((float)(s + 1) - 1)) (float)pi 2 in fp32, as the reference
+// computes it, then cs[2 j] = fl32(cos theta_j) and cs[2 j + 1] = fl32(sin theta_j) from the C library in fp64.
+void surfel_table(int s, float* cs) {
+    const float den = (float)(s + 1) - 1.0f;
+    for (int j = 0; j < s; ++j) {
+        const float theta = ((float)j / den) * (float)M_PI * 2.0f;
+        cs[2 * j] = (float)std::cos((double)theta);
+        cs[2 * j + 1] = (float)std::sin((double)theta);
+    }
+}
+
+// Bytes of a surfel source record in device memory: the SfSrc, then its table.
+size_t surfel_src_bytes(int s) { return align_up(sizeof(SfSrc)) + sizeof(float) * 2 * (size_t)s; }
+
+// Writes the SfSrc of (n, r, s, boxes) and its table to `dev` (surfel_src_bytes(s) bytes of device memory) in the order
+// of `stream`, through the parameters of sf_upload_kernel (no host buffer is copied, so nothing synchronises), and
+// returns the record as the kernels take it by value.
+int upload_surfel_src(unsigned char* dev, const void* n, const void* r, int s, MqBox* boxes, cudaStream_t stream, SfSrc& src) {
+    std::vector<float> cs(2 * (size_t)s);
+    surfel_table(s, cs.data());
+    src.n = n; src.r = r; src.s = s; src.boxes = boxes;
+    src.cs = reinterpret_cast<const float*>(dev + align_up(sizeof(SfSrc)));
+    SfUpload u;
+    u.src = src;
+    for (size_t at = 0; at < cs.size(); at += kSfChunk) {
+        u.dst_src = at == 0 ? reinterpret_cast<SfSrc*>(dev) : nullptr;
+        u.dst = const_cast<float*>(src.cs) + at;
+        u.count = (int)std::min<size_t>(kSfChunk, cs.size() - at);
+        std::memcpy(u.v, cs.data() + at, sizeof(float) * u.count);
+        PCU_LAUNCH(sf_upload_kernel, 1, kThreads, stream, u);
+    }
+    return PCU_B200_OK;
 }
 
 // Carves the build's temporaries from the arena, the tree itself (carve_mesh_tree) from `keep` or, when it is null, from
 // the arena too, and enqueues the build over the leaf kind L (meshquery.cuh): bounds, codes, sort, leaves, nodes, for
 // faces the refit and, with `moments`, the centre, radius and moment passes of winding.cuh.  Face leaves (L = Pt<T>)
 // are built from the mesh (v, nv, f, fkind) and the count of invalid faces lands in *out_bad; point leaves (L = WnPoint)
-// from the points v, normals n and areas a, always with moments.  The caller has checked the input and made the device
-// current.
+// from the points v, normals n and areas a, always with moments; surfel leaves (L = SfWord) from the points v, normals
+// n, radii a and `subdivs`, without moments, their non-finite fans counted in the header only.  The caller has checked
+// the input (m >= 1) and made the device current.
 template <typename T, typename L>
 int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, bool moments,
                     unsigned long long* out_bad, cudaStream_t stream, MeshTree<L>& tree, unsigned char* keep = nullptr,
-                    const T* n = nullptr, const T* a = nullptr) {
-    constexpr bool points = kPointLeaf<L>;
+                    const T* n = nullptr, const T* a = nullptr, int subdivs = 0) {
+    constexpr bool points = kPointLeaf<L>, surfels = kSurfelLeaf<L>;
     const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
     const long long inner = std::max<long long>(1, m - 1);
     struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant;
-             int* node_parent; int* leaf_parent; int* arrivals; MqBox* boxes; } s;
+             int* node_parent; int* leaf_parent; int* arrivals; MqBox* boxes; unsigned char* src; MqBox* in_boxes; } s;
     MeshTree<L> t;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
         s.a = cv.take<MqRec>((size_t)m);
@@ -1324,9 +1365,16 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
         s.leaf_parent = cv.take<int>((size_t)m);
         s.arrivals = cv.take<int>((size_t)inner);
         s.boxes = points ? nullptr : cv.take<MqBox>((size_t)m);
-        if (!keep) carve_mesh_tree<L>(cv, m, moments, t);
+        s.src = surfels ? cv.take<unsigned char>(surfel_src_bytes(subdivs)) : nullptr;
+        s.in_boxes = surfels ? cv.take<MqBox>((size_t)m) : nullptr;
+        if (!keep) carve_mesh_tree<L>(cv, m, moments, t, subdivs);
     }));
-    if (keep) carve_at(keep, [&](Carver& cv) { carve_mesh_tree<L>(cv, m, moments, t); });
+    if (keep) carve_at(keep, [&](Carver& cv) { carve_mesh_tree<L>(cv, m, moments, t, subdivs); });
+    SfSrc src{};
+    if constexpr (surfels) {   // the bounds and codes passes find the surfels' normals, radii and table through f
+        PCU_TRY(upload_surfel_src(s.src, n, a, subdivs, s.in_boxes, stream, src));
+        f = s.src;
+    }
     PCU_CUDA(cudaMemsetAsync(t.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
     PCU_CUDA(cudaMemsetAsync(t.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
     PCU_CUDA(cudaMemsetAsync(&t.sc->bad, 0, sizeof(unsigned long long), stream));
@@ -1338,6 +1386,9 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
     PCU_TRY(radix_sort_records<MqRec>(s.a, s.b, m, 1, s.hist, s.totals, s.base, s.constant, stream, &sorted));
     if constexpr (points)
         PCU_LAUNCH((wn_point_leaves_kernel<T>), fblocks, kThreads, stream, v, n, a, m, (const MqRec*)sorted, t.leaves);
+    else if constexpr (surfels)
+        PCU_LAUNCH((sf_leaves_kernel<T>), fblocks, kThreads, stream, v, src, m, (const MqScratch*)t.sc, (const MqRec*)sorted,
+                   t.leaves, t.ids, s.boxes);
     else
         PCU_LAUNCH((mq_leaves_kernel<T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)t.sc, (const MqRec*)sorted,
                    t.leaves, s.boxes);
@@ -1348,7 +1399,7 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
         PCU_LAUNCH(mq_refit_kernel, fblocks, kThreads, stream, m, (const MqScratch*)t.sc, t.nodes, (const int*)s.node_parent,
                    (const int*)s.leaf_parent, (const MqBox*)s.boxes, s.arrivals);
     }
-    if (moments) {
+    if constexpr (!surfels) if (moments) {   // surfel trees carry no far field
         PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
         PCU_LAUNCH((wn_centres_kernel<L>), fblocks, kThreads, stream, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
                    (const int*)s.node_parent, (const int*)s.leaf_parent, (const L*)t.leaves, t.wn, s.arrivals);
@@ -1358,7 +1409,7 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
         PCU_LAUNCH((wn_moments_kernel<L>), fblocks, kThreads, stream, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
                    (const int*)s.node_parent, (const int*)s.leaf_parent, (const L*)t.leaves, t.wn, s.arrivals);
     }
-    if constexpr (!points)
+    if constexpr (!points && !surfels)
         PCU_CUDA(cudaMemcpyAsync(out_bad, &t.sc->bad, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
     tree = t;
     return PCU_B200_OK;
@@ -1525,6 +1576,7 @@ int ray_mesh_prepared_device(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, 
     if (!ws || !mesh) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
     if (mesh->device != ws->device)
         return fail(PCU_B200_INVALID_ARGUMENT, "the mesh lives on device %d, the workspace on device %d", mesh->device, ws->device);
+    if (mesh->subdivs) return fail(PCU_B200_INVALID_ARGUMENT, "the handle holds surfels, not a mesh");
     PCU_TRY(check_rays(o, o_stride, d, n));
     if (n > 0 && (!out_fidx || !out_bc || !out_t)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
@@ -1533,6 +1585,107 @@ int ray_mesh_prepared_device(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, 
                                      out_fidx, 0, out_bc, out_t, stream);
     return cast_rays<TR, float>(ws, mesh->sc, mesh->nodes, (const Pt<float>*)mesh->leaves, mesh->nf, o, o_stride, d, n, near, far,
                                 out_fidx, 0, out_bc, out_t, stream);
+}
+
+// ---- rays against surfels (raycast.cuh) ------------------------------------------------------------------------------
+// The largest subdivs: theta_j's fp32 quotient j / s is then exact in its numerator and denominator.
+constexpr int kMaxSubdivs = 1 << 24;
+
+int check_surfels(const void* p, const void* n, const void* r, long long m, int subdivs) {
+    if (m < 0 || (m > 0 && (!p || !n || !r))) return fail(PCU_B200_INVALID_ARGUMENT, "p, n and r must be (n, 3), (n, 3) and (n,) arrays");
+    if (m >= INT_MAX) return fail(PCU_B200_INVALID_ARGUMENT, "surfels: at most 2^31 - 2 points, got %lld", m);
+    if (subdivs < 4 || subdivs > kMaxSubdivs)
+        return fail(PCU_B200_INVALID_ARGUMENT, "subdivs must be in [4, 2^24] (got %d)", subdivs);
+    return PCU_B200_OK;
+}
+
+// One launch over the rays of a built surfel tree (m = 0: no tree, every ray misses).
+template <typename TR>
+int cast_surfel_rays(pcu_b200_workspace* ws, const MqScratch* sc, const MqNode* nodes, const SfWord* leaves, const int* ids, long long m,
+                     int subdivs, const TR* o, int o_stride, const TR* d, long long n, float near, float far, int* out_pid, TR* out_t,
+                     cudaStream_t stream) {
+    if (n == 0) return PCU_B200_OK;
+    PCU_LAUNCH((rs_query_kernel<TR>), query_blocks(ws, n), kThreads, stream, o, o_stride, d, n, near, far, m, subdivs, sc, nodes,
+               leaves, ids, out_pid, out_t);
+    return PCU_B200_OK;
+}
+
+// The surfel tree of (p, n, r, subdivs), built for this call, then one thread per ray.
+template <typename T>
+int ray_surfel_device(pcu_b200_workspace* ws, const T* p, const T* nrm, const T* r, long long m, int subdivs, const T* o, int o_stride,
+                      const T* d, long long n, float near, float far, int* out_pid, T* out_t, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(check_surfels(p, nrm, r, m, subdivs));
+    PCU_TRY(check_rays(o, o_stride, d, n));
+    if (n > 0 && (!out_pid || !out_t)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    if (n == 0) return PCU_B200_OK;
+    MeshTree<SfWord> t{};
+    if (m > 0) PCU_TRY(build_mesh_tree<T>(ws, p, 0, nullptr, m, 0, false, nullptr, stream, t, nullptr, nrm, r, subdivs));
+    return cast_surfel_rays<T>(ws, t.sc, t.nodes, t.leaves, t.ids, m, subdivs, o, o_stride, d, n, near, far, out_pid, out_t, stream);
+}
+
+// Builds the surfel tree once into a private block (no block for m = 0).
+template <typename T>
+int surfel_prepare_device(pcu_b200_workspace* ws, const T* p, const T* nrm, const T* r, long long m, int subdivs, pcu_b200_mesh** out,
+                          cudaStream_t stream) {
+    if (!ws || !out) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    PCU_TRY(check_surfels(p, nrm, r, m, subdivs));
+    PCU_ON_DEVICE(ws);
+    MeshTree<SfWord> t{};
+    const size_t bytes = m > 0 ? carve_at(nullptr, [&](Carver& cv) { carve_mesh_tree(cv, m, false, t, subdivs); }) : 0;
+    pcu_b200_mesh* h = new (std::nothrow) pcu_b200_mesh();
+    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
+    h->device = ws->device; h->is_f64 = sizeof(T) == 8 ? 1 : 0; h->nf = m; h->subdivs = subdivs; h->bytes = bytes;
+    if (m > 0) {
+        cudaError_t e = cudaMalloc((void**)&h->block, bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            delete h;
+            return fail(PCU_B200_OUT_OF_MEMORY, "cudaMalloc of %zu bytes for prepared surfels failed: %s", bytes, cudaGetErrorString(e));
+        }
+        const int st = build_mesh_tree<T>(ws, p, 0, nullptr, m, 0, false, nullptr, stream, t, h->block, nrm, r, subdivs);
+        if (st != PCU_B200_OK) { cudaFree(h->block); delete h; return st; }
+        h->sc = t.sc; h->nodes = t.nodes; h->leaves = t.leaves; h->ids = t.ids;
+    }
+    *out = h;
+    return PCU_B200_OK;
+}
+
+// Rays of precision TR against prepared surfels of either precision (the leaves are fp32 either way).
+template <typename TR>
+int ray_surfel_prepared_device(pcu_b200_workspace* ws, const pcu_b200_mesh* h, const TR* o, int o_stride, const TR* d, long long n,
+                               float near, float far, int* out_pid, TR* out_t, cudaStream_t stream) {
+    if (!ws || !h) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (h->device != ws->device)
+        return fail(PCU_B200_INVALID_ARGUMENT, "the surfels live on device %d, the workspace on device %d", h->device, ws->device);
+    if (!h->subdivs) return fail(PCU_B200_INVALID_ARGUMENT, "the handle holds a mesh, not surfels");
+    PCU_TRY(check_rays(o, o_stride, d, n));
+    if (n > 0 && (!out_pid || !out_t)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    return cast_surfel_rays<TR>(ws, h->sc, h->nodes, (const SfWord*)h->leaves, h->ids, h->nf, h->subdivs, o, o_stride, d, n, near, far,
+                                out_pid, out_t, stream);
+}
+
+// pointcloud_surfel_geometry: (s + 1) m vertices in T and s m int32 faces.
+template <typename T>
+int surfel_geometry_device(pcu_b200_workspace* ws, const T* p, const T* nrm, const T* r, long long m, int subdivs, T* out_v,
+                           int* out_f, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(check_surfels(p, nrm, r, m, subdivs));
+    if (m * (long long)(subdivs + 1) >= INT_MAX)
+        return fail(PCU_B200_INVALID_ARGUMENT, "surfel geometry: int32 faces index at most 2^31 - 2 vertices, got %lld points of %d",
+                    m, subdivs + 1);
+    if (m > 0 && (!out_v || !out_f)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    if (m == 0) return PCU_B200_OK;
+    unsigned char* dev = nullptr;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { dev = cv.take<unsigned char>(surfel_src_bytes(subdivs)); }));
+    SfSrc src{};
+    PCU_TRY(upload_surfel_src(dev, nrm, r, subdivs, nullptr, stream, src));
+    PCU_LAUNCH((sf_geometry_kernel<T>), (unsigned)((m + kThreads - 1) / kThreads), kThreads, stream, p, src, m, out_v, out_f);
+    return PCU_B200_OK;
 }
 
 // ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
@@ -2292,6 +2445,43 @@ int pcu_b200_ray_mesh_intersection_prepared_f64(pcu_b200_workspace* ws, const pc
                                                 const double* d, int64_t n, float near, float far, int32_t* out_fidx, double* out_bc,
                                                 double* out_t, void* stream) {
     return ray_mesh_prepared_device<double>(ws, mesh, o, o_stride, d, n, near, far, out_fidx, out_bc, out_t, (cudaStream_t)stream);
+}
+
+int pcu_b200_ray_surfel_intersection_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* r, int64_t np, int subdivs,
+                                         const float* o, int o_stride, const float* d, int64_t nr, float near, float far, int32_t* out_pid,
+                                         float* out_t, void* stream) {
+    return ray_surfel_device<float>(ws, p, n, r, np, subdivs, o, o_stride, d, nr, near, far, out_pid, out_t, (cudaStream_t)stream);
+}
+int pcu_b200_ray_surfel_intersection_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np, int subdivs,
+                                         const double* o, int o_stride, const double* d, int64_t nr, float near, float far, int32_t* out_pid,
+                                         double* out_t, void* stream) {
+    return ray_surfel_device<double>(ws, p, n, r, np, subdivs, o, o_stride, d, nr, near, far, out_pid, out_t, (cudaStream_t)stream);
+}
+int pcu_b200_surfel_prepare_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* r, int64_t np, int subdivs,
+                                pcu_b200_mesh** out_surfels, void* stream) {
+    return surfel_prepare_device<float>(ws, p, n, r, np, subdivs, out_surfels, (cudaStream_t)stream);
+}
+int pcu_b200_surfel_prepare_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np, int subdivs,
+                                pcu_b200_mesh** out_surfels, void* stream) {
+    return surfel_prepare_device<double>(ws, p, n, r, np, subdivs, out_surfels, (cudaStream_t)stream);
+}
+int pcu_b200_ray_surfel_intersection_prepared_f32(pcu_b200_workspace* ws, const pcu_b200_mesh* surfels, const float* o, int o_stride,
+                                                  const float* d, int64_t nr, float near, float far, int32_t* out_pid, float* out_t,
+                                                  void* stream) {
+    return ray_surfel_prepared_device<float>(ws, surfels, o, o_stride, d, nr, near, far, out_pid, out_t, (cudaStream_t)stream);
+}
+int pcu_b200_ray_surfel_intersection_prepared_f64(pcu_b200_workspace* ws, const pcu_b200_mesh* surfels, const double* o, int o_stride,
+                                                  const double* d, int64_t nr, float near, float far, int32_t* out_pid, double* out_t,
+                                                  void* stream) {
+    return ray_surfel_prepared_device<double>(ws, surfels, o, o_stride, d, nr, near, far, out_pid, out_t, (cudaStream_t)stream);
+}
+int pcu_b200_pointcloud_surfel_geometry_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* r, int64_t np, int subdivs,
+                                            float* out_v, int32_t* out_f, void* stream) {
+    return surfel_geometry_device<float>(ws, p, n, r, np, subdivs, out_v, out_f, (cudaStream_t)stream);
+}
+int pcu_b200_pointcloud_surfel_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np,
+                                            int subdivs, double* out_v, int32_t* out_f, void* stream) {
+    return surfel_geometry_device<double>(ws, p, n, r, np, subdivs, out_v, out_f, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,

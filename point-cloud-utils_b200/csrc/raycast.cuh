@@ -1,5 +1,6 @@
 // raycast.cuh -- rays against a triangle mesh (ray_mesh_intersection / RayMeshIntersector of the reference,
-// src/ray_mesh_intersection.cpp, one Embree ray at a time).
+// src/ray_mesh_intersection.cpp, one Embree ray at a time), and rays against surfels (ray_surfel_intersection /
+// RaySurfelIntersector, src/ray_point_cloud_intersection.cpp: the same test on each point's fan, rs_query_kernel below).
 //
 // The result is defined exactly (DESIGN.md §3, ray casting) as a pure function of (v, f, o_i, d_i, near, far):
 //   rounding          corners, origin, direction, near and far are rounded to fp32 whatever the input precision
@@ -83,9 +84,99 @@ __device__ __forceinline__ bool rc_box(const RcRay& r, const float lo[3], const 
     return enter <= exit && zhi > near;
 }
 
+// Largest |coordinate| of the scene box, which covers every leaf's box.
+__device__ __forceinline__ float rc_scene(const MqScratch* __restrict__ sc) {
+    float scene = 0.f;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) scene = fmaxf(scene, fabsf(mq_unord(sc->scene[k])));
+    return scene;
+}
+
+// Ray (oi, di) rounded to fp32 and its constants as rc_query_kernel sets them up; false for a zero or non-finite origin or direction.
+template <typename TR>
+__device__ __forceinline__ bool rc_ray(const TR* oi, const TR* di, float scene, RcRay& r) {
+    float dir[3];
+    bool valid = true;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        r.o[k] = (float)oi[k];
+        dir[k] = (float)di[k];
+        valid = valid && isfinite(r.o[k]) && isfinite(dir[k]);
+    }
+    valid = valid && (dir[0] != 0.f || dir[1] != 0.f || dir[2] != 0.f);
+    if (!valid) return false;
+    r.kz = 0;
+    if (fabsf(dir[1]) > fabsf(dir[r.kz])) r.kz = 1;
+    if (fabsf(dir[2]) > fabsf(dir[r.kz])) r.kz = 2;
+    r.kx = r.kz == 2 ? 0 : r.kz + 1;
+    r.ky = r.kx == 2 ? 0 : r.kx + 1;
+    const float dz = rc_pick(dir, r.kz);
+    if (dz < 0.f) { const int s = r.kx; r.kx = r.ky; r.ky = s; }
+    r.sx = __fdiv_rn(rc_pick(dir, r.kx), dz);
+    r.sy = __fdiv_rn(rc_pick(dir, r.ky), dz);
+    r.sz = __fdiv_rn(1.f, dz);
+    const float R = __fadd_ru(fmaxf(fabsf(r.o[0]), fmaxf(fabsf(r.o[1]), fabsf(r.o[2]))), scene);
+    r.delta = __fmul_ru(R, 0x1p-20f);
+    const float R19 = __fmul_ru(R, 0x1p-19f);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const float ad = fabsf(dir[k]);
+        r.mode[k] = ad == 0.f ? 0 : (ad < 0x1p-100f ? 1 : 2);
+        r.inv[k] = __fdiv_rn(1.f, dir[k]);
+        r.m[k] = __fdiv_ru(R19, ad);
+    }
+    return true;
+}
+
+// The walk of rc_query_kernel (which keeps its own copy, unchanged) over a tree of n >= 1 leaves: leaf(l) for every leaf whose box rc_box keeps with its lower bound not past
+// best, which leaf() may lower; nearer child first, the other pushed with its bound.
+template <typename F>
+__device__ __forceinline__ void rc_walk(const RcRay& r, const MqNode* __restrict__ nodes, long long n, float near, const float& best,
+                                        F&& leaf) {
+    if (n == 1) {
+        leaf(0);
+        return;
+    }
+    int stack[kMqStack];
+    float stack_lb[kMqStack];
+    int sp = 0, node = 0;
+    while (true) {
+        const float4* np_ = reinterpret_cast<const float4*>(nodes + node);
+        const float4 q0 = __ldg(np_), q1 = __ldg(np_ + 1), q2 = __ldg(np_ + 2), q3 = __ldg(np_ + 3);
+        const float lo0[3] = {q0.x, q0.y, q0.z}, hi0[3] = {q0.w, q1.x, q1.y};
+        const float lo1[3] = {q1.z, q1.w, q2.x}, hi1[3] = {q2.y, q2.z, q2.w};
+        const int c0 = __float_as_int(q3.x), c1 = __float_as_int(q3.y);
+        float l0, l1;
+        bool k0 = rc_box(r, lo0, hi0, near, l0) && !(l0 > best);
+        bool k1 = rc_box(r, lo1, hi1, near, l1) && !(l1 > best);
+        if (k0 && c0 < 0) { leaf(~c0); k0 = false; }
+        if (k1 && c1 < 0) { leaf(~c1); k1 = false; }
+        k0 = k0 && !(l0 > best);
+        k1 = k1 && !(l1 > best);
+        if (k0 && k1) {
+            const bool first0 = l0 <= l1;
+            stack[sp] = first0 ? c1 : c0;
+            stack_lb[sp] = first0 ? l1 : l0;
+            ++sp;
+            node = first0 ? c0 : c1;
+            continue;
+        }
+        if (k0) { node = c0; continue; }
+        if (k1) { node = c1; continue; }
+        node = -1;
+        while (sp > 0) {
+            --sp;
+            if (!(stack_lb[sp] > best)) { node = stack[sp]; break; }
+        }
+        if (node < 0) break;
+    }
+}
+
 // Ray i: origin o + i * o_stride (o_stride 0: one origin for every ray), direction d + 3 i.  fidx_wide: 8-byte face
 // indices (f's width), else 4-byte.  Misses get fidx = -1, t = +inf, bc = 0.  Nothing is written when the tree is
 // empty (every face invalid: the caller raises).  Per visit one 64-byte node; per face tested three Pt<TM>.
+// rc_ray and rc_walk above repeat this kernel's ray setup and walk for rs_query_kernel; a change to either must be
+// made in both places (this kernel keeps its own copy so that its code stays as it was).
 template <typename TR, typename TM>
 __global__ void __launch_bounds__(kThreads) rc_query_kernel(const TR* __restrict__ o, int o_stride, const TR* __restrict__ d,
                                                             long long nr, float near, float far, long long m,
@@ -186,6 +277,47 @@ __global__ void __launch_bounds__(kThreads) rc_query_kernel(const TR* __restrict
         out_bc[3 * i] = hit ? (TR)__dsub_rn(__dsub_rn(1.0, (double)bb1), (double)bb2) : (TR)0;
         out_bc[3 * i + 1] = hit ? (TR)bb1 : (TR)0;
         out_bc[3 * i + 2] = hit ? (TR)bb2 : (TR)0;
+    }
+}
+
+// Rays against surfels (ray_surfel_intersection, DESIGN.md §3): the walk of rc_query_kernel over a surfel tree of
+// m points (meshquery.cuh, leaves SfWord of s-triangle fans).  At a leaf the s triangles (centre, rim j, rim
+// (j + 1) mod s) are tested with rc_face, each triangle loading its three corners (L1 hits after the first), so no
+// corner stays live across triangles.  The first hit by (t, point id) wins.  Misses, an empty tree (m = 0, or every fan non-finite) and invalid rays give pid = -1, t = +inf.  Per visit
+// one 64-byte node; per surfel tested sf_words(s) 16-byte words and one id.
+template <typename TR>
+__global__ void __launch_bounds__(kThreads) rs_query_kernel(const TR* __restrict__ o, int o_stride, const TR* __restrict__ d,
+                                                            long long nr, float near, float far, long long m, int s,
+                                                              const MqScratch* __restrict__ sc, const MqNode* __restrict__ nodes,
+                                                              const SfWord* __restrict__ leaves, const int* __restrict__ ids,
+                                                            int* __restrict__ out_pid, TR* __restrict__ out_t) {
+    const long long n = m > 0 ? m - (long long)sc->bad : 0;
+    const float scene = n > 0 ? rc_scene(sc) : 0.f;
+    const long long words = sf_words(s);
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nr; i += (long long)gridDim.x * blockDim.x) {
+        RcRay r;
+        float best = far;
+        int best_pid = INT_MAX;
+        if (n > 0 && rc_ray<TR>(o + (long long)o_stride * i, d + 3 * i, scene, r)) {
+            rc_walk(r, nodes, n, near, best, [&](int l) {
+                const float* q = reinterpret_cast<const float*>(leaves + (long long)l * words);
+                const int pid = __ldg(ids + l);
+                for (int j = 0; j < s; ++j) {   // every corner reloaded (L1 hits): nothing held across triangles
+                    const float* u = q + 3 * (j + 1);
+                    const float* w = q + (j + 1 < s ? 3 * (j + 2) : 3);
+                    const float centre[3] = {__ldg(q), __ldg(q + 1), __ldg(q + 2)};
+                    const float a[3] = {__ldg(u), __ldg(u + 1), __ldg(u + 2)}, b[3] = {__ldg(w), __ldg(w + 1), __ldg(w + 2)};
+                    float t, b1, b2;
+                    if (rc_face(r, centre, a, b, near, t, b1, b2) && (t < best || (t == best && pid < best_pid))) {
+                        best = t;
+                        best_pid = pid;
+                    }
+                }
+            });
+        }
+        const bool hit = best_pid != INT_MAX;
+        out_pid[i] = hit ? best_pid : -1;
+        out_t[i] = hit ? (TR)best : (TR)__int_as_float(0x7f800000);
     }
 }
 

@@ -55,6 +55,12 @@ step("ray mesh intersection, one origin fp32", lambda: pcu.ray_mesh_intersection
 isect = step("prepare a mesh for rays", lambda: pcu.RayMeshIntersector(mv.astype(np.float32), mf))
 step("rays against a prepared mesh (fp64 rays)", lambda: isect.intersect_rays(ro, -ro))
 isect.close()
+sp, sn = rng.normal(size=(300, 3)), rng.normal(size=(300, 3))
+step("ray surfel intersection", lambda: pcu.ray_surfel_intersection(sp, sn, ro, -ro, 0.3, 7))
+step("surfel geometry fp32", lambda: pcu.pointcloud_surfel_geometry(sp.astype(np.float32), sn.astype(np.float32), 0.3, 5))
+surf = step("prepare surfels for rays", lambda: pcu.RaySurfelIntersector(sp.astype(np.float32), sn.astype(np.float32), 0.3))
+step("rays against prepared surfels (fp64 rays)", lambda: surf.intersect_rays(ro, -ro))
+surf.close()
 cn = rng.normal(size=(n, 3)); ca = rng.random(n)
 step("point cloud winding numbers", lambda: pcu.point_cloud_fast_winding_number(v, cn, ca, ro))
 step("point cloud winding numbers fp32", lambda: pcu.point_cloud_fast_winding_number(v.astype(np.float32), cn.astype(np.float32), ca.astype(np.float32), ro.astype(np.float32)))
