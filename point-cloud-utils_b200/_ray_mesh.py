@@ -7,8 +7,8 @@ out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's 
 import numpy as np
 
 from . import _pcu_internal
-from ._mesh_sampling import (_INDEX_KINDS, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form, _raise_bad,
-                             _torch, _upload, _validate_mesh)
+from ._mesh_sampling import (_INDEX_KINDS, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form, _is_tensor,
+                             _raise_bad, _torch, _upload, _validate_mesh)
 
 
 def _matrix_shape(a):
@@ -37,24 +37,35 @@ def _bounds(ray_near, ray_far):
     return float(np.float32(ray_near)), float(np.float32(ray_far))
 
 
-def _empty(form, fdt, dt, device):
-    """Zero rays: empty outputs, no launch."""
-    if form == "numpy":
-        return np.zeros(0, dtype=fdt), np.zeros((0, 3), dtype=dt), np.zeros(0, dtype=dt)
-    torch = _torch()
-    return (torch.zeros(0, dtype=fdt, device=device), torch.zeros((0, 3), dtype=dt, device=device),
-            torch.zeros(0, dtype=dt, device=device))
-
-
-def _outputs(n, fidx_dtype, rt):
-    torch = _torch()
-    return (torch.empty(n, dtype=fidx_dtype, device=rt.device), torch.empty((n, 3), dtype=rt.dtype, device=rt.device),
-            torch.empty(n, dtype=rt.dtype, device=rt.device))
-
-
 def _origins(ot, single):
     """(origins, o_stride) of a contiguous ray_o: a single origin is its 3 elements in order, with stride 0."""
     return (ot.reshape(3), 0) if single else (ot, 3)
+
+
+def _cast(form, scene, ray_o, ray_d, single, n, device, outs, call):
+    """From validated inputs to the returned arrays.  `scene` holds the arrays that are uploaded with the rays (none for a
+    prepared tree); `outs` gives one (shape after #rays, dtype name) per output, None standing for the rays' dtype;
+    call(scene tensors, origins, o_stride, directions, outputs, device index, stream) makes the native call on
+    contiguous CUDA tensors.  CPU tensors go through numpy, and zero rays return empty outputs without a launch."""
+    torch = _torch()
+    if form == "cpu":
+        out = _cast("numpy", [a.detach().numpy() if _is_tensor(a) else a for a in scene], ray_o.detach().numpy(),
+                    ray_d.detach().numpy(), single, n, device, outs, call)
+        return tuple(torch.from_numpy(o) for o in out)
+    outs = [(tail, name or _dtype_name(ray_d)) for tail, name in outs]
+    if n == 0:
+        if form == "numpy":
+            return tuple(np.zeros((0,) + tail, dtype=name) for tail, name in outs)
+        from . import _same_device
+        _same_device(ray_d, device)
+        return tuple(torch.zeros((0,) + tail, dtype=getattr(torch, name), device=ray_d.device) for tail, name in outs)
+    *scene, ot, dt = _upload(form, list(scene) + [ray_o, ray_d], device)
+    ot, o_stride = _origins(ot, single)
+    dt = dt.reshape(n, 3)
+    dev, stream = _call_args(dt)
+    out = tuple(torch.empty((n,) + tail, dtype=getattr(torch, name), device=dt.device) for tail, name in outs)
+    call(scene, ot, o_stride, dt, out, dev, stream)
+    return tuple(o.cpu().numpy() for o in out) if form == "numpy" else out
 
 
 def ray_mesh_intersection(v, f, ray_o, ray_d, ray_near=0.0, ray_far=np.inf, *, device=None):
@@ -93,32 +104,58 @@ def ray_mesh_intersection(v, f, ray_o, ray_d, ray_near=0.0, ray_far=np.inf, *, d
     _validate_mesh(v, f, tuple(_INDEX_KINDS))
     near, far = _bounds(ray_near, ray_far)
     torch = _torch()
-    if form == "cpu":
-        out = ray_mesh_intersection(v.detach().numpy(), f.detach().numpy(), ray_o.detach().numpy(), ray_d.detach().numpy(),
-                                    near, far, device=device)
-        return tuple(torch.from_numpy(o) for o in out)
-    if n == 0:
-        if form == "cuda":
-            from . import _same_device
-            _same_device(v, device)
-        return _empty(form, f.dtype, v.dtype, v.device if form == "cuda" else None)
-    vt, ft, ot, dt = _upload(form, [v, f, ray_o, ray_d], device)
-    ot, o_stride = _origins(ot, single)
-    dt = dt.reshape(n, 3)
-    dev, stream = _call_args(vt)
-    fidx, bc, t = _outputs(n, ft.dtype, vt)
-    bad = torch.empty(1, dtype=torch.int64, device=vt.device)
-    _pcu_internal._ray_mesh_intersection_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
-                                                int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], ot.data_ptr(), o_stride,
-                                                dt.data_ptr(), n, near, far, fidx.data_ptr(), bc.data_ptr(), t.data_ptr(),
-                                                bad.data_ptr(), dev, stream)
-    _raise_bad(bad)
-    if form == "numpy":
-        return fidx.cpu().numpy().view(f.dtype), bc.cpu().numpy(), t.cpu().numpy()
-    return fidx, bc, t
+    # numpy and CPU inputs: f_id travels as the signed type of f's width, as f does, and is viewed back as f's dtype
+    fdt = _dtype_name(f) if form == "cuda" else _dtype_name(f).replace("u", "")
+
+    def call(scene, ot, o_stride, dt, out, dev, stream):
+        vt, ft = scene
+        bad = torch.empty(1, dtype=torch.int64, device=vt.device)
+        _pcu_internal._ray_mesh_intersection_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
+                                                    int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], ot.data_ptr(), o_stride,
+                                                    dt.data_ptr(), n, near, far, *(o.data_ptr() for o in out), bad.data_ptr(),
+                                                    dev, stream)
+        _raise_bad(bad)
+
+    fidx, bc, t = _cast(form, [v, f], ray_o, ray_d, single, n, device, [((), fdt), ((3,), None), ((), None)], call)
+    return fidx.view(f.dtype), bc, t
 
 
-class RayMeshIntersector:
+class _Prepared:
+    """A tree built once and held through a native handle: what RayMeshIntersector and RaySurfelIntersector share.
+    `_what` names the tree in messages; __init__ sets `_handle` and `device_index`."""
+    _handle = 0
+
+    def close(self):
+        if self._handle:
+            _pcu_internal._mesh_destroy(self._handle)
+            self._handle = 0
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:   # interpreter shutdown
+            pass
+
+    def _intersect(self, native, outs, ray_o, ray_d, ray_near, ray_far):
+        """intersect_rays: the checks in the order their errors win, then `native` on the handle, outputs as `outs`."""
+        if not self._handle:
+            raise ValueError("the %s has been closed" % type(self).__name__)
+        form = _form([ray_o, ray_d], ["ray_o", "ray_d"])
+        _check_float(ray_o, "ray_o")
+        _check_match(ray_d, "ray_d", ray_o, "ray_o")
+        single, n = _validate_rays(ray_o, ray_d)
+        near, far = _bounds(ray_near, ray_far)
+        if form == "cuda" and (ray_o.device.index or 0) != self.device_index:
+            raise ValueError("the rays live on %s, %s on cuda:%d" % (ray_o.device, self._what, self.device_index))
+
+        def call(_, ot, o_stride, dt, out, dev, stream):
+            native(dt.dtype == _torch().float64, self._handle, ot.data_ptr(), o_stride, dt.data_ptr(), n, near, far,
+                   *(o.data_ptr() for o in out), dev, stream)
+
+        return _cast(form, [], ray_o, ray_d, single, n, self.device_index, outs, call)
+
+
+class RayMeshIntersector(_Prepared):
     """
     Class used to find the intersection between rays and a triangle mesh.
 
@@ -126,6 +163,7 @@ class RayMeshIntersector:
     rays.  The results are those of `ray_mesh_intersection(mesh_v, mesh_f, ...)` (f_id as int32).  `close()` (or garbage
     collection) frees the device memory.
     """
+    _what = "the mesh"
 
     def __init__(self, mesh_v, mesh_f, *, device=None):
         """
@@ -139,7 +177,6 @@ class RayMeshIntersector:
 
         Divergence: a face corner outside [0, #v) raises ValueError (the reference validates nothing here).
         """
-        self._handle = 0
         form = _form([mesh_v, mesh_f], ["mesh_v", "mesh_f"])
         _validate_mesh(mesh_v, mesh_f, tuple(_INDEX_KINDS))
         self.v = mesh_v
@@ -158,17 +195,6 @@ class RayMeshIntersector:
             _pcu_internal._mesh_destroy(handle)
             raise
         self._handle, self.device_index = handle, dev
-
-    def close(self):
-        if self._handle:
-            _pcu_internal._mesh_destroy(self._handle)
-            self._handle = 0
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:   # interpreter shutdown
-            pass
 
     def intersect_rays(self, ray_o, ray_d, ray_near=0.0, ray_far=np.inf):
         """
@@ -189,29 +215,5 @@ class RayMeshIntersector:
 
         Rays given as CUDA tensors must live on the mesh's device; numpy arrays and CPU tensors are copied there.
         """
-        if not self._handle:
-            raise ValueError("the RayMeshIntersector has been closed")
-        form = _form([ray_o, ray_d], ["ray_o", "ray_d"])
-        _check_float(ray_o, "ray_o")
-        _check_match(ray_d, "ray_d", ray_o, "ray_o")
-        single, n = _validate_rays(ray_o, ray_d)
-        near, far = _bounds(ray_near, ray_far)
-        torch = _torch()
-        if form == "cpu":
-            out = self.intersect_rays(ray_o.detach().numpy(), ray_d.detach().numpy(), near, far)
-            return tuple(torch.from_numpy(o) for o in out)
-        if form == "cuda" and (ray_o.device.index or 0) != self.device_index:
-            raise ValueError("the rays live on %s, the mesh on cuda:%d" % (ray_o.device, self.device_index))
-        if n == 0:
-            return _empty(form, np.int32 if form == "numpy" else torch.int32, ray_o.dtype,
-                          ray_o.device if form == "cuda" else None)
-        ot, dt = _upload(form, [ray_o, ray_d], self.device_index)
-        ot, o_stride = _origins(ot, single)
-        dt = dt.reshape(n, 3)
-        dev, stream = _call_args(dt)
-        fidx, bc, t = _outputs(n, torch.int32, dt)
-        _pcu_internal._ray_mesh_prepared_device(dt.dtype == torch.float64, self._handle, ot.data_ptr(), o_stride, dt.data_ptr(),
-                                                n, near, far, fidx.data_ptr(), bc.data_ptr(), t.data_ptr(), dev, stream)
-        if form == "numpy":
-            return fidx.cpu().numpy(), bc.cpu().numpy(), t.cpu().numpy()
-        return fidx, bc, t
+        return self._intersect(_pcu_internal._ray_mesh_prepared_device, [((), "int32"), ((3,), None), ((), None)], ray_o, ray_d,
+                               ray_near, ray_far)

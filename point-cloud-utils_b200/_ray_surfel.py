@@ -7,8 +7,8 @@ out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's 
 import numpy as np
 
 from . import _pcu_internal
-from ._mesh_sampling import _call_args, _check_float, _check_match, _form, _is_tensor, _torch, _upload
-from ._ray_mesh import _bounds, _matrix_shape, _origins, _validate_rays
+from ._mesh_sampling import _call_args, _check_float, _check_match, _dtype_name, _form, _is_tensor, _torch, _upload
+from ._ray_mesh import _Prepared, _bounds, _cast, _matrix_shape, _validate_rays
 
 _MAX_SUBDIVS = 2 ** 24
 
@@ -20,7 +20,7 @@ def _validate_radius(p, r):
         if np.isscalar(r):
             r = r * np.ones(p.shape[0])
         elif isinstance(r, (list, tuple)):
-            r = np.array(r).astype(_numpy_dtype(p))
+            r = np.array(r).astype(_dtype_name(p))
         else:
             raise ValueError("Argument r must be a scalar or numpy array with the same number of rows as p")
     if r.shape[0] != p.shape[0]:
@@ -30,10 +30,6 @@ def _validate_radius(p, r):
     if len(r.shape) != 1:
         raise ValueError("Invalid shape for argument r, must have shape (N,) or (N, 1)")
     return r
-
-
-def _numpy_dtype(x):
-    return np.dtype(str(x.dtype).replace("torch.", ""))
 
 
 def _validate_surfels(p, n, subdivs):
@@ -64,20 +60,7 @@ def _radius_like(r, p, form):
         r = r if _is_tensor(r) else torch.from_numpy(np.ascontiguousarray(r))
         return r.to(device=p.device, dtype=p.dtype).contiguous()
     r = r.detach().cpu().numpy() if _is_tensor(r) else r
-    return np.ascontiguousarray(np.asarray(r).astype(_numpy_dtype(p)))
-
-
-def _misses(form, n, dt, device):
-    """Zero rays: empty outputs, no launch."""
-    if form == "numpy":
-        return np.zeros(n, dtype=np.int32), np.zeros(n, dtype=dt)
-    torch = _torch()
-    return torch.zeros(n, dtype=torch.int32, device=device), torch.zeros(n, dtype=dt, device=device)
-
-
-def _cast_outputs(n, rt):
-    torch = _torch()
-    return torch.empty(n, dtype=torch.int32, device=rt.device), torch.empty(n, dtype=rt.dtype, device=rt.device)
+    return np.ascontiguousarray(np.asarray(r).astype(_dtype_name(p)))
 
 
 def ray_surfel_intersection(p, n, ray_o, ray_d, r=0.1, subdivs=4, ray_near=0.0, ray_far=np.inf, *, device=None):
@@ -121,30 +104,17 @@ def ray_surfel_intersection(p, n, ray_o, ray_d, r=0.1, subdivs=4, ray_near=0.0, 
     subdivs = _validate_surfels(p, n, subdivs)
     near, far = _bounds(ray_near, ray_far)
     torch = _torch()
-    if form == "cpu":
-        out = ray_surfel_intersection(p.detach().numpy(), n.detach().numpy(), ray_o.detach().numpy(), ray_d.detach().numpy(),
-                                      _radius_like(r, p, "cpu"), subdivs, near, far, device=device)
-        return tuple(torch.from_numpy(o) for o in out)
-    r = _radius_like(r, p, form)
-    if nr == 0:
-        if form == "cuda":
-            from . import _same_device
-            _same_device(p, device)
-        return _misses(form, 0, p.dtype, p.device if form == "cuda" else None)
-    pt, nt, ot, dt, rt = _upload(form, [p, n, ray_o, ray_d, r], device)
-    ot, o_stride = _origins(ot, single)
-    dt = dt.reshape(nr, 3)
-    dev, stream = _call_args(dt)
-    pid, t = _cast_outputs(nr, dt)
-    _pcu_internal._ray_surfel_intersection_device(dt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), rt.data_ptr(),
-                                                  int(pt.shape[0]), subdivs, ot.data_ptr(), o_stride, dt.data_ptr(), nr,
-                                                  near, far, pid.data_ptr(), t.data_ptr(), dev, stream)
-    if form == "numpy":
-        return pid.cpu().numpy(), t.cpu().numpy()
-    return pid, t
+
+    def call(scene, ot, o_stride, dt, out, dev, stream):
+        pt, nt, rt = scene
+        _pcu_internal._ray_surfel_intersection_device(dt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), rt.data_ptr(),
+                                                      int(pt.shape[0]), subdivs, ot.data_ptr(), o_stride, dt.data_ptr(), nr,
+                                                      near, far, *(o.data_ptr() for o in out), dev, stream)
+
+    return _cast(form, [p, n, _radius_like(r, p, form)], ray_o, ray_d, single, nr, device, [((), "int32"), ((), None)], call)
 
 
-class RaySurfelIntersector:
+class RaySurfelIntersector(_Prepared):
     """
     Class used to find the intersection between rays and a point cloud converted to surfels (i.e. a point cloud
     represented as circles centered at each point and oriented perpendicularly to each normal).
@@ -153,6 +123,7 @@ class RaySurfelIntersector:
     rays.  The results are those of `ray_surfel_intersection(p, n, ray_o, ray_d, r, subdivs, ...)`.  `close()` (or
     garbage collection) frees the device memory.
     """
+    _what = "the surfels"
 
     def __init__(self, p, n, r=0.1, subdivs=7, *, device=None):
         """
@@ -170,7 +141,6 @@ class RaySurfelIntersector:
 
         Divergence: r is cast to p's dtype (the reference hands a float64 r to its float32 binding, which refuses it).
         """
-        self._handle = 0
         r = _validate_radius(p, r)
         form = _form([p, n], ["p", "n"])
         _check_float(p, "v")
@@ -190,17 +160,6 @@ class RaySurfelIntersector:
         torch.cuda.current_stream(pt.device).synchronize()    # calls on any stream may use the tree
         self._handle, self.device_index = handle, dev
 
-    def close(self):
-        if self._handle:
-            _pcu_internal._mesh_destroy(self._handle)
-            self._handle = 0
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:   # interpreter shutdown
-            pass
-
     def intersect_rays(self, ray_o, ray_d, ray_near=0.0, ray_far=np.inf):
         """
         Compute intersection between a set of rays and the point cloud converted to circular patches oriented with the
@@ -219,31 +178,8 @@ class RaySurfelIntersector:
 
         Rays given as CUDA tensors must live on the cloud's device; numpy arrays and CPU tensors are copied there.
         """
-        if not self._handle:
-            raise ValueError("the RaySurfelIntersector has been closed")
-        form = _form([ray_o, ray_d], ["ray_o", "ray_d"])
-        _check_float(ray_o, "ray_o")
-        _check_match(ray_d, "ray_d", ray_o, "ray_o")
-        single, nr = _validate_rays(ray_o, ray_d)
-        near, far = _bounds(ray_near, ray_far)
-        torch = _torch()
-        if form == "cpu":
-            out = self.intersect_rays(ray_o.detach().numpy(), ray_d.detach().numpy(), near, far)
-            return tuple(torch.from_numpy(o) for o in out)
-        if form == "cuda" and (ray_o.device.index or 0) != self.device_index:
-            raise ValueError("the rays live on %s, the surfels on cuda:%d" % (ray_o.device, self.device_index))
-        if nr == 0:
-            return _misses(form, 0, ray_o.dtype, ray_o.device if form == "cuda" else None)
-        ot, dt = _upload(form, [ray_o, ray_d], self.device_index)
-        ot, o_stride = _origins(ot, single)
-        dt = dt.reshape(nr, 3)
-        dev, stream = _call_args(dt)
-        pid, t = _cast_outputs(nr, dt)
-        _pcu_internal._ray_surfel_prepared_device(dt.dtype == torch.float64, self._handle, ot.data_ptr(), o_stride,
-                                                  dt.data_ptr(), nr, near, far, pid.data_ptr(), t.data_ptr(), dev, stream)
-        if form == "numpy":
-            return pid.cpu().numpy(), t.cpu().numpy()
-        return pid, t
+        return self._intersect(_pcu_internal._ray_surfel_prepared_device, [((), "int32"), ((), None)], ray_o, ray_d, ray_near,
+                               ray_far)
 
 
 def pointcloud_surfel_geometry(p, n, r=0.1, subdivs=7, *, device=None):

@@ -1528,6 +1528,45 @@ int check_rays(const void* o, int o_stride, const void* d, long long n) {
     return PCU_B200_OK;
 }
 
+// What every cast against a handle checks first: the handle is there, lives on the workspace's device and holds the
+// kind of tree the caller casts against, and the rays are well formed.
+int check_cast(pcu_b200_workspace* ws, const pcu_b200_mesh* h, bool want_surfels, const void* o, int o_stride, const void* d,
+               long long n) {
+    if (!ws || !h) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (h->device != ws->device)
+        return fail(PCU_B200_INVALID_ARGUMENT, "the %s on device %d, the workspace on device %d", want_surfels ? "surfels live" : "mesh lives",
+                    h->device, ws->device);
+    if ((h->subdivs != 0) != want_surfels)
+        return fail(PCU_B200_INVALID_ARGUMENT, "the handle holds %s", want_surfels ? "a mesh, not surfels" : "surfels, not a mesh");
+    return check_rays(o, o_stride, d, n);
+}
+
+// A new handle for a tree of m leaves L (fans of `subdivs` triangles for surfels, else 0) over coordinates T, built once
+// into a private block: sizes the block, allocates handle and block, runs build(block, tree) and frees both if that
+// fails.  m = 0 (surfels only): a handle without a block, which every ray misses.  `what` names the block when
+// cudaMalloc fails.
+template <typename T, typename L, typename Build>
+int prepare_tree(pcu_b200_workspace* ws, const char* what, long long m, int subdivs, pcu_b200_mesh** out, Build&& build) {
+    MeshTree<L> t{};
+    const size_t bytes = m > 0 ? carve_at(nullptr, [&](Carver& cv) { carve_mesh_tree(cv, m, false, t, subdivs); }) : 0;
+    pcu_b200_mesh* h = new (std::nothrow) pcu_b200_mesh();
+    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
+    h->device = ws->device; h->is_f64 = sizeof(T) == 8 ? 1 : 0; h->nf = m; h->subdivs = subdivs; h->bytes = bytes;
+    if (m > 0) {
+        cudaError_t e = cudaMalloc((void**)&h->block, bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            delete h;
+            return fail(PCU_B200_OUT_OF_MEMORY, "cudaMalloc of %zu bytes for %s failed: %s", bytes, what, cudaGetErrorString(e));
+        }
+        const int st = build(h->block, t);
+        if (st != PCU_B200_OK) { cudaFree(h->block); delete h; return st; }
+        h->sc = t.sc; h->nodes = t.nodes; h->leaves = t.leaves; h->ids = t.ids;
+    }
+    *out = h;
+    return PCU_B200_OK;
+}
+
 // The tree of the closest-point query, built for this call, then one thread per ray.
 template <typename T>
 int ray_mesh_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, const T* o, int o_stride,
@@ -1551,33 +1590,16 @@ int mesh_prepare_device(pcu_b200_workspace* ws, const T* v, long long nv, const 
     *out = nullptr;
     PCU_TRY(mesh_check(v, nv, f, m, fkind));
     PCU_ON_DEVICE(ws);
-    MeshTree<Pt<T>> t;
-    const size_t bytes = carve_at(nullptr, [&](Carver& cv) { carve_mesh_tree(cv, m, false, t); });
-    pcu_b200_mesh* h = new (std::nothrow) pcu_b200_mesh();
-    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
-    h->device = ws->device; h->is_f64 = sizeof(T) == 8 ? 1 : 0; h->nf = m; h->bytes = bytes;
-    cudaError_t e = cudaMalloc((void**)&h->block, bytes);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        delete h;
-        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMalloc of %zu bytes for a prepared mesh failed: %s", bytes, cudaGetErrorString(e));
-    }
-    const int st = build_mesh_tree<T>(ws, v, nv, f, m, fkind, false, out_bad, stream, t, h->block);
-    if (st != PCU_B200_OK) { cudaFree(h->block); delete h; return st; }
-    h->sc = t.sc; h->nodes = t.nodes; h->leaves = t.leaves;
-    *out = h;
-    return PCU_B200_OK;
+    return prepare_tree<T, Pt<T>>(ws, "a prepared mesh", m, 0, out, [&](unsigned char* block, MeshTree<Pt<T>>& t) {
+        return build_mesh_tree<T>(ws, v, nv, f, m, fkind, false, out_bad, stream, t, block);
+    });
 }
 
 // Rays of precision TR against a prepared mesh of either precision; face indices as int32.
 template <typename TR>
 int ray_mesh_prepared_device(pcu_b200_workspace* ws, const pcu_b200_mesh* mesh, const TR* o, int o_stride, const TR* d, long long n,
                              float near, float far, int* out_fidx, TR* out_bc, TR* out_t, cudaStream_t stream) {
-    if (!ws || !mesh) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
-    if (mesh->device != ws->device)
-        return fail(PCU_B200_INVALID_ARGUMENT, "the mesh lives on device %d, the workspace on device %d", mesh->device, ws->device);
-    if (mesh->subdivs) return fail(PCU_B200_INVALID_ARGUMENT, "the handle holds surfels, not a mesh");
-    PCU_TRY(check_rays(o, o_stride, d, n));
+    PCU_TRY(check_cast(ws, mesh, false, o, o_stride, d, n));
     if (n > 0 && (!out_fidx || !out_bc || !out_t)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
     if (mesh->is_f64)
@@ -1599,18 +1621,7 @@ int check_surfels(const void* p, const void* n, const void* r, long long m, int 
     return PCU_B200_OK;
 }
 
-// One launch over the rays of a built surfel tree (m = 0: no tree, every ray misses).
-template <typename TR>
-int cast_surfel_rays(pcu_b200_workspace* ws, const MqScratch* sc, const MqNode* nodes, const SfWord* leaves, const int* ids, long long m,
-                     int subdivs, const TR* o, int o_stride, const TR* d, long long n, float near, float far, int* out_pid, TR* out_t,
-                     cudaStream_t stream) {
-    if (n == 0) return PCU_B200_OK;
-    PCU_LAUNCH((rs_query_kernel<TR>), query_blocks(ws, n), kThreads, stream, o, o_stride, d, n, near, far, m, subdivs, sc, nodes,
-               leaves, ids, out_pid, out_t);
-    return PCU_B200_OK;
-}
-
-// The surfel tree of (p, n, r, subdivs), built for this call, then one thread per ray.
+// The surfel tree of (p, n, r, subdivs), built for this call, then one thread per ray (m = 0: no tree, every ray misses).
 template <typename T>
 int ray_surfel_device(pcu_b200_workspace* ws, const T* p, const T* nrm, const T* r, long long m, int subdivs, const T* o, int o_stride,
                       const T* d, long long n, float near, float far, int* out_pid, T* out_t, cudaStream_t stream) {
@@ -1622,7 +1633,9 @@ int ray_surfel_device(pcu_b200_workspace* ws, const T* p, const T* nrm, const T*
     if (n == 0) return PCU_B200_OK;
     MeshTree<SfWord> t{};
     if (m > 0) PCU_TRY(build_mesh_tree<T>(ws, p, 0, nullptr, m, 0, false, nullptr, stream, t, nullptr, nrm, r, subdivs));
-    return cast_surfel_rays<T>(ws, t.sc, t.nodes, t.leaves, t.ids, m, subdivs, o, o_stride, d, n, near, far, out_pid, out_t, stream);
+    PCU_LAUNCH((rs_query_kernel<T>), query_blocks(ws, n), kThreads, stream, o, o_stride, d, n, near, far, m, subdivs,
+               (const MqScratch*)t.sc, (const MqNode*)t.nodes, (const SfWord*)t.leaves, (const int*)t.ids, out_pid, out_t);
+    return PCU_B200_OK;
 }
 
 // Builds the surfel tree once into a private block (no block for m = 0).
@@ -1633,39 +1646,22 @@ int surfel_prepare_device(pcu_b200_workspace* ws, const T* p, const T* nrm, cons
     *out = nullptr;
     PCU_TRY(check_surfels(p, nrm, r, m, subdivs));
     PCU_ON_DEVICE(ws);
-    MeshTree<SfWord> t{};
-    const size_t bytes = m > 0 ? carve_at(nullptr, [&](Carver& cv) { carve_mesh_tree(cv, m, false, t, subdivs); }) : 0;
-    pcu_b200_mesh* h = new (std::nothrow) pcu_b200_mesh();
-    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
-    h->device = ws->device; h->is_f64 = sizeof(T) == 8 ? 1 : 0; h->nf = m; h->subdivs = subdivs; h->bytes = bytes;
-    if (m > 0) {
-        cudaError_t e = cudaMalloc((void**)&h->block, bytes);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            delete h;
-            return fail(PCU_B200_OUT_OF_MEMORY, "cudaMalloc of %zu bytes for prepared surfels failed: %s", bytes, cudaGetErrorString(e));
-        }
-        const int st = build_mesh_tree<T>(ws, p, 0, nullptr, m, 0, false, nullptr, stream, t, h->block, nrm, r, subdivs);
-        if (st != PCU_B200_OK) { cudaFree(h->block); delete h; return st; }
-        h->sc = t.sc; h->nodes = t.nodes; h->leaves = t.leaves; h->ids = t.ids;
-    }
-    *out = h;
-    return PCU_B200_OK;
+    return prepare_tree<T, SfWord>(ws, "prepared surfels", m, subdivs, out, [&](unsigned char* block, MeshTree<SfWord>& t) {
+        return build_mesh_tree<T>(ws, p, 0, nullptr, m, 0, false, nullptr, stream, t, block, nrm, r, subdivs);
+    });
 }
 
 // Rays of precision TR against prepared surfels of either precision (the leaves are fp32 either way).
 template <typename TR>
 int ray_surfel_prepared_device(pcu_b200_workspace* ws, const pcu_b200_mesh* h, const TR* o, int o_stride, const TR* d, long long n,
                                float near, float far, int* out_pid, TR* out_t, cudaStream_t stream) {
-    if (!ws || !h) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
-    if (h->device != ws->device)
-        return fail(PCU_B200_INVALID_ARGUMENT, "the surfels live on device %d, the workspace on device %d", h->device, ws->device);
-    if (!h->subdivs) return fail(PCU_B200_INVALID_ARGUMENT, "the handle holds a mesh, not surfels");
-    PCU_TRY(check_rays(o, o_stride, d, n));
+    PCU_TRY(check_cast(ws, h, true, o, o_stride, d, n));
     if (n > 0 && (!out_pid || !out_t)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    return cast_surfel_rays<TR>(ws, h->sc, h->nodes, (const SfWord*)h->leaves, h->ids, h->nf, h->subdivs, o, o_stride, d, n, near, far,
-                                out_pid, out_t, stream);
+    if (n == 0) return PCU_B200_OK;
+    PCU_LAUNCH((rs_query_kernel<TR>), query_blocks(ws, n), kThreads, stream, o, o_stride, d, n, near, far, h->nf, h->subdivs,
+               (const MqScratch*)h->sc, (const MqNode*)h->nodes, (const SfWord*)h->leaves, h->ids, out_pid, out_t);
+    return PCU_B200_OK;
 }
 
 // pointcloud_surfel_geometry: (s + 1) m vertices in T and s m int32 faces.

@@ -92,19 +92,23 @@ __device__ __forceinline__ float rc_scene(const MqScratch* __restrict__ sc) {
     return scene;
 }
 
-// Ray (oi, di) rounded to fp32 and its constants as rc_query_kernel sets them up; false for a zero or non-finite origin or direction.
+// Ray (oi, di) rounded to fp32 into o and dir; false for a zero or non-finite origin or direction.
 template <typename TR>
-__device__ __forceinline__ bool rc_ray(const TR* oi, const TR* di, float scene, RcRay& r) {
-    float dir[3];
+__device__ __forceinline__ bool rc_round(const TR* oi, const TR* di, float o[3], float dir[3]) {
     bool valid = true;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-        r.o[k] = (float)oi[k];
+        o[k] = (float)oi[k];
         dir[k] = (float)di[k];
-        valid = valid && isfinite(r.o[k]) && isfinite(dir[k]);
+        valid = valid && isfinite(o[k]) && isfinite(dir[k]);
     }
-    valid = valid && (dir[0] != 0.f || dir[1] != 0.f || dir[2] != 0.f);
-    if (!valid) return false;
+    return valid && (dir[0] != 0.f || dir[1] != 0.f || dir[2] != 0.f);
+}
+
+// The constants of a valid ray (r.o, dir).  Where a kernel calls it decides its register allocation (nvcc 12.9,
+// sm_90a): rc_query_kernel calls it inside the branch that walks, since set up ahead of that branch it spills;
+// rs_query_kernel sets up ahead, which is how it reaches 64 registers and its measured speed (DESIGN.md §4).
+__device__ __forceinline__ void rc_ray(const float dir[3], float scene, RcRay& r) {
     r.kz = 0;
     if (fabsf(dir[1]) > fabsf(dir[r.kz])) r.kz = 1;
     if (fabsf(dir[2]) > fabsf(dir[r.kz])) r.kz = 2;
@@ -125,10 +129,9 @@ __device__ __forceinline__ bool rc_ray(const TR* oi, const TR* di, float scene, 
         r.inv[k] = __fdiv_rn(1.f, dir[k]);
         r.m[k] = __fdiv_ru(R19, ad);
     }
-    return true;
 }
 
-// The walk of rc_query_kernel (which keeps its own copy, unchanged) over a tree of n >= 1 leaves: leaf(l) for every leaf whose box rc_box keeps with its lower bound not past
+// The walk over a tree of n >= 1 leaves: leaf(l) for every leaf whose box rc_box keeps with its lower bound not past
 // best, which leaf() may lower; nearer child first, the other pushed with its bound.
 template <typename F>
 __device__ __forceinline__ void rc_walk(const RcRay& r, const MqNode* __restrict__ nodes, long long n, float near, const float& best,
@@ -175,8 +178,6 @@ __device__ __forceinline__ void rc_walk(const RcRay& r, const MqNode* __restrict
 // Ray i: origin o + i * o_stride (o_stride 0: one origin for every ray), direction d + 3 i.  fidx_wide: 8-byte face
 // indices (f's width), else 4-byte.  Misses get fidx = -1, t = +inf, bc = 0.  Nothing is written when the tree is
 // empty (every face invalid: the caller raises).  Per visit one 64-byte node; per face tested three Pt<TM>.
-// rc_ray and rc_walk above repeat this kernel's ray setup and walk for rs_query_kernel; a change to either must be
-// made in both places (this kernel keeps its own copy so that its code stays as it was).
 template <typename TR, typename TM>
 __global__ void __launch_bounds__(kThreads) rc_query_kernel(const TR* __restrict__ o, int o_stride, const TR* __restrict__ d,
                                                             long long nr, float near, float far, long long m,
@@ -185,45 +186,15 @@ __global__ void __launch_bounds__(kThreads) rc_query_kernel(const TR* __restrict
                                                             int fidx_wide, TR* __restrict__ out_bc, TR* __restrict__ out_t) {
     const long long n = m - (long long)sc->bad;
     if (n < 1) return;
-    float scene = 0.f;   // largest |coordinate| of the scene box
-#pragma unroll
-    for (int k = 0; k < 6; ++k) scene = fmaxf(scene, fabsf(mq_unord(sc->scene[k])));
+    const float scene = rc_scene(sc);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nr; i += (long long)gridDim.x * blockDim.x) {
-        const TR* oi = o + (long long)o_stride * i;
         RcRay r;
         float dir[3];
-        bool valid = true;
-#pragma unroll
-        for (int k = 0; k < 3; ++k) {
-            r.o[k] = (float)oi[k];
-            dir[k] = (float)d[3 * i + k];
-            valid = valid && isfinite(r.o[k]) && isfinite(dir[k]);
-        }
-        valid = valid && (dir[0] != 0.f || dir[1] != 0.f || dir[2] != 0.f);
         float best = far, bb1 = 0.f, bb2 = 0.f;
         long long best_face = LLONG_MAX;
-        if (valid) {
-            r.kz = 0;
-            if (fabsf(dir[1]) > fabsf(dir[r.kz])) r.kz = 1;
-            if (fabsf(dir[2]) > fabsf(dir[r.kz])) r.kz = 2;
-            r.kx = r.kz == 2 ? 0 : r.kz + 1;
-            r.ky = r.kx == 2 ? 0 : r.kx + 1;
-            const float dz = rc_pick(dir, r.kz);
-            if (dz < 0.f) { const int s = r.kx; r.kx = r.ky; r.ky = s; }
-            r.sx = __fdiv_rn(rc_pick(dir, r.kx), dz);
-            r.sy = __fdiv_rn(rc_pick(dir, r.ky), dz);
-            r.sz = __fdiv_rn(1.f, dz);
-            const float R = __fadd_ru(fmaxf(fabsf(r.o[0]), fmaxf(fabsf(r.o[1]), fabsf(r.o[2]))), scene);
-            r.delta = __fmul_ru(R, 0x1p-20f);
-            const float R19 = __fmul_ru(R, 0x1p-19f);
-#pragma unroll
-            for (int k = 0; k < 3; ++k) {
-                const float ad = fabsf(dir[k]);
-                r.mode[k] = ad == 0.f ? 0 : (ad < 0x1p-100f ? 1 : 2);
-                r.inv[k] = __fdiv_rn(1.f, dir[k]);
-                r.m[k] = __fdiv_ru(R19, ad);
-            }
-            auto leaf = [&](int l) {
+        if (rc_round<TR>(o + (long long)o_stride * i, d + 3 * i, r.o, dir)) {
+            rc_ray(dir, scene, r);
+            rc_walk(r, nodes, n, near, best, [&](int l) {
                 const Pt<TM> A = leaves[3 * l], B = leaves[3 * l + 1], C = leaves[3 * l + 2];
                 const float a[3] = {(float)A.x, (float)A.y, (float)A.z}, b[3] = {(float)B.x, (float)B.y, (float)B.z},
                             c[3] = {(float)C.x, (float)C.y, (float)C.z};
@@ -231,44 +202,7 @@ __global__ void __launch_bounds__(kThreads) rc_query_kernel(const TR* __restrict
                 if (!rc_face(r, a, b, c, near, t, b1, b2)) return;
                 const long long face = (long long)A.i;
                 if (t < best || (t == best && face < best_face)) { best = t; best_face = face; bb1 = b1; bb2 = b2; }
-            };
-            if (n == 1) {
-                leaf(0);
-            } else {
-                int stack[kMqStack];
-                float stack_lb[kMqStack];
-                int sp = 0, node = 0;
-                while (true) {
-                    const float4* np_ = reinterpret_cast<const float4*>(nodes + node);
-                    const float4 q0 = __ldg(np_), q1 = __ldg(np_ + 1), q2 = __ldg(np_ + 2), q3 = __ldg(np_ + 3);
-                    const float lo0[3] = {q0.x, q0.y, q0.z}, hi0[3] = {q0.w, q1.x, q1.y};
-                    const float lo1[3] = {q1.z, q1.w, q2.x}, hi1[3] = {q2.y, q2.z, q2.w};
-                    const int c0 = __float_as_int(q3.x), c1 = __float_as_int(q3.y);
-                    float l0, l1;
-                    bool k0 = rc_box(r, lo0, hi0, near, l0) && !(l0 > best);
-                    bool k1 = rc_box(r, lo1, hi1, near, l1) && !(l1 > best);
-                    if (k0 && c0 < 0) { leaf(~c0); k0 = false; }
-                    if (k1 && c1 < 0) { leaf(~c1); k1 = false; }
-                    k0 = k0 && !(l0 > best);
-                    k1 = k1 && !(l1 > best);
-                    if (k0 && k1) {
-                        const bool first0 = l0 <= l1;
-                        stack[sp] = first0 ? c1 : c0;
-                        stack_lb[sp] = first0 ? l1 : l0;
-                        ++sp;
-                        node = first0 ? c0 : c1;
-                        continue;
-                    }
-                    if (k0) { node = c0; continue; }
-                    if (k1) { node = c1; continue; }
-                    node = -1;
-                    while (sp > 0) {
-                        --sp;
-                        if (!(stack_lb[sp] > best)) { node = stack[sp]; break; }
-                    }
-                    if (node < 0) break;
-                }
-            }
+            });
         }
         const bool hit = best_face != LLONG_MAX;
         if (fidx_wide) ((long long*)out_fidx)[i] = hit ? best_face : -1ll;
@@ -298,7 +232,13 @@ __global__ void __launch_bounds__(kThreads) rs_query_kernel(const TR* __restrict
         RcRay r;
         float best = far;
         int best_pid = INT_MAX;
-        if (n > 0 && rc_ray<TR>(o + (long long)o_stride * i, d + 3 * i, scene, r)) {
+        const auto ahead = [&]() {   // the setup ahead of the walk's branch, dir scoped to it (see rc_ray)
+            float dir[3];
+            if (!rc_round<TR>(o + (long long)o_stride * i, d + 3 * i, r.o, dir)) return false;
+            rc_ray(dir, scene, r);
+            return true;
+        };
+        if (n > 0 && ahead()) {
             rc_walk(r, nodes, n, near, best, [&](int l) {
                 const float* q = reinterpret_cast<const float*>(leaves + (long long)l * words);
                 const int pid = __ldg(ids + l);
