@@ -507,6 +507,35 @@ int pcu_b200_pointcloud_surfel_geometry_f32(pcu_b200_workspace* ws, const float*
 int pcu_b200_pointcloud_surfel_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np,
                                             int subdivs, double* out_v, int32_t* out_f, void* stream);
 
+/* ---- marching cubes on a sparse voxel grid and the grid's boundary ---------------------------------------------------
+ * Replace marching_cubes_sparse_voxel_grid (src/marching_cubes.cpp:35-85) and sparse_voxel_grid_boundary
+ * (src/sparse_voxel_grid.cpp:463-522).  The marching-cubes result is defined in DESIGN.md §3: one vertex per distinct
+ * unordered pair of corner indices on a crossing edge, numbered by first appearance (cube by cube, edge by edge), each
+ * interpolated in the coordinates' precision T from that first edge; faces cube by cube in the generated case table's
+ * order.  The suffix is T; scalars are float or double (scalars_f64), cube_idx is (m, 8) of kind idx_kind, 16-byte
+ * aligned; 1 <= n < 2^31 - 1, m >= 1.
+ *   marching_cubes_prepare: classifies the cubes, synchronises `stream` to read the crossing-edge and face counts, then
+ *     numbers the vertices and synchronises again to read their count.  *out_counts = {#v, #f} (host int64).  A cube
+ *     corner outside [0, n), 2^32 or more crossing edges, or more vertices than idx_kind can index fail with
+ *     PCU_B200_INVALID_ARGUMENT.  *out_mc (a handle; scalars, coords and cube_idx must stay alive until emit) is freed
+ *     by marching_cubes_destroy, stream-ordered on the stream it was prepared on.
+ *   marching_cubes_emit: writes out_v (#v, 3) in T and out_f (#f, 3) of idx_kind's width; stream-ordered.
+ *   sparse_voxel_grid_boundary: grid (n, 3) int32 (idx_kind I32) or int64 (I64), n >= 1; out_idx (capacity n, int64)
+ *     receives the boundary voxels' rows in ascending order, out_counts[0] (device int64) their number and
+ *     out_counts[1] the rows with a coordinate outside [INT32_MIN + 1, INT32_MAX - 1] (then the output is unspecified).
+ * Every array pointer is a DEVICE pointer. */
+typedef struct pcu_b200_marching_cubes pcu_b200_marching_cubes;
+int pcu_b200_marching_cubes_prepare_f32(pcu_b200_workspace* ws, const void* scalars, int scalars_f64, const float* coords, int64_t n,
+                                        const void* cube_idx, int64_t m, int idx_kind, double isovalue, pcu_b200_marching_cubes** out_mc,
+                                        int64_t out_counts[2], void* stream);
+int pcu_b200_marching_cubes_prepare_f64(pcu_b200_workspace* ws, const void* scalars, int scalars_f64, const double* coords, int64_t n,
+                                        const void* cube_idx, int64_t m, int idx_kind, double isovalue, pcu_b200_marching_cubes** out_mc,
+                                        int64_t out_counts[2], void* stream);
+int pcu_b200_marching_cubes_emit(pcu_b200_workspace* ws, const pcu_b200_marching_cubes* mc, void* out_v, void* out_f, void* stream);
+int pcu_b200_marching_cubes_destroy(pcu_b200_marching_cubes* mc);
+int pcu_b200_sparse_voxel_grid_boundary(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, int64_t* out_idx,
+                                        int64_t* out_counts, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

@@ -682,6 +682,38 @@ void surfel_geometry_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t r, 
     });
 }
 
+// Marching cubes (marching_cubes_sparse_voxel_grid, _sparse_voxels.py): classifies and numbers the vertices (two
+// synchronisations of `stream`), returns (handle, #v, #f); _marching_cubes_emit writes v and f; _marching_cubes_destroy.
+py::tuple marching_cubes_prepare_device(bool t_f64, uintptr_t scalars, bool s_f64, uintptr_t coords, int64_t n, uintptr_t idx, int64_t m,
+                                        int idx_kind, double isovalue, int device, uintptr_t stream) {
+    pcu_b200_marching_cubes* mc = nullptr;
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return t_f64 ? pcu_b200_marching_cubes_prepare_f64(ws, (const void*)scalars, s_f64, (const double*)coords, n, (const void*)idx, m,
+                                                           idx_kind, isovalue, &mc, counts, (void*)stream)
+                     : pcu_b200_marching_cubes_prepare_f32(ws, (const void*)scalars, s_f64, (const float*)coords, n, (const void*)idx, m,
+                                                           idx_kind, isovalue, &mc, counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)mc, counts[0], counts[1]);
+}
+void marching_cubes_emit_device(uintptr_t mc, uintptr_t out_v, uintptr_t out_f, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_marching_cubes_emit(ws, (const pcu_b200_marching_cubes*)mc, (void*)out_v, (void*)out_f, (void*)stream);
+    });
+}
+void marching_cubes_destroy(uintptr_t mc) {
+    py::gil_scoped_release nogil;
+    pcu_b200_marching_cubes_destroy((pcu_b200_marching_cubes*)mc);
+}
+// sparse_voxel_grid_boundary: out_idx (capacity n) int64, out_counts: two device int64 {boundary rows, rows out of range}.
+void sparse_voxel_grid_boundary_device(uintptr_t grid, int64_t n, int idx_kind, uintptr_t out_idx, uintptr_t out_counts, int device,
+                                       uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_sparse_voxel_grid_boundary(ws, (const void*)grid, n, idx_kind, (int64_t*)out_idx, (int64_t*)out_counts,
+                                                   (void*)stream);
+    });
+}
+
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
@@ -1086,6 +1118,10 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_ray_surfel_prepared_device", &ray_surfel_prepared_device);
     mod.def("_surfel_geometry_device", &surfel_geometry_device);
     mod.def("_interpolate_barycentric_device", &interpolate_barycentric_device);
+    mod.def("_marching_cubes_prepare_device", &marching_cubes_prepare_device);
+    mod.def("_marching_cubes_emit_device", &marching_cubes_emit_device);
+    mod.def("_marching_cubes_destroy", &marching_cubes_destroy);
+    mod.def("_sparse_voxel_grid_boundary_device", &sparse_voxel_grid_boundary_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),

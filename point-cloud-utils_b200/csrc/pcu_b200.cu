@@ -36,6 +36,7 @@
 #include "meshsample.cuh"
 #include "winding.cuh"
 #include "raycast.cuh"
+#include "sparse_voxels.cuh"
 
 using namespace pcu;
 
@@ -258,6 +259,30 @@ struct pcu_b200_mesh {
     MqNode* nodes = nullptr;
     const void* leaves = nullptr;   // Pt<float> or Pt<double> by is_f64, or SfWord
     const int* ids = nullptr;       // surfels: the point id of each leaf
+};
+// Marching cubes between pcu_b200_marching_cubes_prepare_* and _emit: the inputs, the cube block (case bytes, tile
+// offsets, counts; sized by m) and the slot block (run of every slot, vertex id of every run, owner flags; sized by the
+// slot count), both allocated and freed in the order of `stream`.
+struct pcu_b200_marching_cubes {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    int t_f64 = 0, s_f64 = 0, width = 4;   // coordinates, scalars, bytes per cube index
+    const void* scalars = nullptr;
+    const void* coords = nullptr;
+    const void* idx = nullptr;
+    long long n = 0, m = 0;
+    double iso = 0.0;                       // T(S(isovalue)), exactly
+    long long slots = 0, faces = 0, verts = 0;
+    unsigned char* cube_block = nullptr;
+    unsigned char* slot_block = nullptr;
+    unsigned char* cases = nullptr;
+    unsigned* tile_sum = nullptr;
+    unsigned long long* tile_slot0 = nullptr;
+    unsigned long long* tile_face0 = nullptr;
+    McCounts* counts = nullptr;
+    unsigned* slot_run = nullptr;
+    unsigned* run_vid = nullptr;
+    unsigned char* owner = nullptr;
 };
 template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
@@ -1196,12 +1221,13 @@ int interpolate_device(pcu_b200_workspace* ws, const void* f, long long m, int f
 }
 
 // ---- duplicate removal (SURVEY.md 8f N2, src/remove_duplicates.cpp) ----------------------------------------
-// Stable LSD radix sort of `n` records between two buffers; returns the buffer holding the sorted records.
+// Stable LSD radix sort of `n` records between two buffers; returns the buffer holding the sorted records.  key_bits > 0:
+// only the low key_bits bits of each key word can be non-zero, and the passes over the bytes above them are skipped.
 template <typename Rec>
 int radix_sort_records(Rec* a, Rec* b, long long n, int words, unsigned* hist, unsigned long long* totals, unsigned* base, int* constant,
-                       cudaStream_t stream, Rec** sorted) {
+                       cudaStream_t stream, Rec** sorted, int key_bits = 0) {
     const unsigned ntiles = (unsigned)((n + kSortTile - 1) / kSortTile);
-    const int bits = (int)sizeof(a->key[0]) * 8;
+    const int bits = key_bits > 0 ? key_bits : (int)sizeof(a->key[0]) * 8;
     Rec *in = a, *out = b;
     for (int w = words - 1; w >= 0; --w)          // least significant word first
         for (int shift = 0; shift < bits; shift += 8) {
@@ -1684,8 +1710,212 @@ int surfel_geometry_device(pcu_b200_workspace* ws, const T* p, const T* nrm, con
     return PCU_B200_OK;
 }
 
-// ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
+// ---- marching cubes and the boundary of a sparse voxel grid (sparse_voxels.cuh) ------------------------------------
 inline unsigned blocks_for(long long n) { return (unsigned)((n + kThreads - 1) / kThreads); }
+
+int mc_free(pcu_b200_marching_cubes* h) {
+    if (h->cube_block) cudaFreeAsync(h->cube_block, h->stream);
+    if (h->slot_block) cudaFreeAsync(h->slot_block, h->stream);
+    delete h;
+    return PCU_B200_OK;
+}
+
+int mc_alloc(unsigned char*& block, size_t bytes, cudaStream_t stream) {
+    const cudaError_t e = cudaMallocAsync((void**)&block, bytes, stream);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        block = nullptr;
+        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMallocAsync of %zu bytes for marching cubes failed: %s", bytes, cudaGetErrorString(e));
+    }
+    return PCU_B200_OK;
+}
+
+int mc_read_counts(pcu_b200_marching_cubes* h, McCounts& out) {
+    PCU_CUDA(cudaMemcpyAsync(&out, h->counts, sizeof(McCounts), cudaMemcpyDeviceToHost, h->stream));
+    PCU_CUDA(cudaStreamSynchronize(h->stream));
+    return PCU_B200_OK;
+}
+
+// Classify + scan, read the counts (first synchronisation), then the slot records, their sort, the runs and the owners'
+// vertex ids, and read the vertex count (second synchronisation).
+template <typename T, typename S, int W>
+int mc_build(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t stream) {
+    const long long m = h->m, tiles = (m + kThreads - 1) / kThreads;
+    PCU_CUDA(cudaMemsetAsync(h->counts, 0, sizeof(McCounts), stream));
+    PCU_LAUNCH((mc_classify_kernel<T, S, W>), (unsigned)tiles, kThreads, stream, (const S*)h->scalars, h->n, h->idx, m, (T)h->iso,
+               h->cases, h->tile_sum, h->counts);
+    PCU_LAUNCH(mc_tiles_kernel, 1, 1024, stream, (const unsigned*)h->tile_sum, tiles, h->tile_slot0, h->tile_face0, h->counts);
+    McCounts c;
+    PCU_TRY(mc_read_counts(h, c));
+    if (c.bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid cube_indices: %llu cubes have a corner outside [0, %lld)", c.bad, h->n);
+    if (c.slots >= (1ull << 32))
+        return fail(PCU_B200_INVALID_ARGUMENT, "marching cubes: at most 2^32 - 1 crossing edges are supported, got %llu", c.slots);
+    h->slots = (long long)c.slots;
+    h->faces = (long long)c.faces;
+    const long long ns = h->slots;
+    if (ns == 0) return PCU_B200_OK;
+    const long long nblocks = (ns + kThreads - 1) / kThreads;
+    PCU_TRY(mc_alloc(h->slot_block, carve_at(nullptr, [&](Carver& cv) {
+        cv.take<unsigned>((size_t)ns); cv.take<unsigned>((size_t)ns); cv.take<unsigned char>((size_t)ns); }), stream));
+    carve_at(h->slot_block, [&](Carver& cv) {
+        h->slot_run = cv.take<unsigned>((size_t)ns);
+        h->run_vid = cv.take<unsigned>((size_t)ns);
+        h->owner = cv.take<unsigned char>((size_t)ns);
+    });
+    const unsigned ntiles = (unsigned)((ns + kSortTile - 1) / kSortTile);
+    struct { McRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; unsigned char* head;
+             unsigned* counts; unsigned* ocounts; long long* owners; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.a = cv.take<McRec>((size_t)ns);
+        sc.b = cv.take<McRec>((size_t)ns);
+        sc.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
+        sc.totals = cv.take<unsigned long long>(kSortBins);
+        sc.base = cv.take<unsigned>(kSortBins);
+        sc.constant = cv.take<int>(1);
+        sc.head = cv.take<unsigned char>((size_t)ns);
+        sc.counts = cv.take<unsigned>((size_t)nblocks);
+        sc.ocounts = cv.take<unsigned>((size_t)nblocks);
+        sc.owners = cv.take<long long>(1);
+    }));
+    int b = 1;                                       // bits of the largest corner index, n - 1
+    while (b < 31 && ((h->n - 1) >> b) != 0) ++b;
+    PCU_LAUNCH((mc_slots_kernel<W>), (unsigned)tiles, kThreads, stream, h->idx, (const unsigned char*)h->cases, m,
+               (const unsigned long long*)h->tile_slot0, (const unsigned long long*)h->tile_face0, b, sc.a);
+    McRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records<McRec>(sc.a, sc.b, ns, 1, sc.hist, sc.totals, sc.base, sc.constant, stream, &sorted, 2 * b));
+    PCU_LAUNCH(mc_heads_kernel, (unsigned)nblocks, kThreads, stream, (const McRec*)sorted, ns, sc.head);
+    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)sc.head, ns, sc.counts);
+    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.counts, nblocks, &h->counts->verts);
+    PCU_LAUNCH(mc_runs_kernel, (unsigned)nblocks, kThreads, stream, (const McRec*)sorted, ns, (const unsigned char*)sc.head,
+               (const unsigned*)sc.counts, h->slot_run, h->owner);
+    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)h->owner, ns, sc.ocounts);
+    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.ocounts, nblocks, sc.owners);
+    PCU_LAUNCH(mc_owner_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)h->owner, ns, (const unsigned*)sc.ocounts,
+               (const unsigned*)h->slot_run, h->run_vid);
+    PCU_TRY(mc_read_counts(h, c));
+    h->verts = c.verts;
+    return PCU_B200_OK;
+}
+
+template <typename T, typename S>
+int mc_build_width(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t stream) {
+    return h->width == 8 ? mc_build<T, S, 8>(ws, h, stream) : mc_build<T, S, 4>(ws, h, stream);
+}
+
+template <typename T>
+int marching_cubes_prepare_device(pcu_b200_workspace* ws, const void* scalars, int s_f64, const T* coords, long long n, const void* idx,
+                                  long long m, int kind, double isovalue, pcu_b200_marching_cubes** out, long long* out_counts,
+                                  cudaStream_t stream) {
+    if (!ws || !out || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    if (!scalars || !coords || !idx) return fail(PCU_B200_INVALID_ARGUMENT, "null input pointer");
+    if (n <= 0 || n >= 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "marching cubes: n must be in [1, 2^31 - 2], got %lld", n);
+    if (m <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid cube_indices has zero rows!");
+    if (kind < kIdxI32 || kind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown index kind %d", kind);
+    if ((uintptr_t)idx % 16 != 0) return fail(PCU_B200_INVALID_ARGUMENT, "cube_idx must be 16-byte aligned");
+    if ((m + kThreads - 1) / kThreads > 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "too many cubes (%lld)", m);
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    pcu_b200_marching_cubes* h = new (std::nothrow) pcu_b200_marching_cubes();
+    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
+    h->device = ws->device; h->stream = stream; h->t_f64 = sizeof(T) == 8; h->s_f64 = s_f64 != 0; h->width = (kind & 1) ? 8 : 4;
+    h->scalars = scalars; h->coords = coords; h->idx = idx; h->n = n; h->m = m;
+    h->iso = s_f64 ? (double)(T)isovalue : (double)(T)(float)isovalue;
+    const long long tiles = (m + kThreads - 1) / kThreads;
+    const auto carve = [&](Carver& cv) {
+        h->cases = cv.take<unsigned char>((size_t)m);
+        h->tile_sum = cv.take<unsigned>((size_t)tiles);
+        h->tile_slot0 = cv.take<unsigned long long>((size_t)tiles);
+        h->tile_face0 = cv.take<unsigned long long>((size_t)tiles);
+        h->counts = cv.take<McCounts>(1);
+    };
+    int st = mc_alloc(h->cube_block, carve_at(nullptr, carve), stream);
+    if (st == PCU_B200_OK) {
+        carve_at(h->cube_block, carve);
+        st = h->s_f64 ? mc_build_width<T, double>(ws, h, stream) : mc_build_width<T, float>(ws, h, stream);
+    }
+    if (st == PCU_B200_OK) {
+        const long long most = kind == kIdxI32 ? (1ll << 31) : kind == kIdxU32 ? (1ll << 32) : LLONG_MAX;
+        if (h->verts > most) st = fail(PCU_B200_INVALID_ARGUMENT, "marching cubes: %lld vertices cannot be indexed by cube_indices' dtype",
+                                       h->verts);
+    }
+    if (st != PCU_B200_OK) { mc_free(h); return st; }
+    out_counts[0] = h->verts;
+    out_counts[1] = h->faces;
+    *out = h;
+    return PCU_B200_OK;
+}
+
+template <typename T, typename S>
+int mc_emit_launch(const pcu_b200_marching_cubes* h, void* out_v, void* out_f, cudaStream_t stream) {
+    const unsigned tiles = (unsigned)((h->m + kThreads - 1) / kThreads);
+    if (h->width == 8)
+        PCU_LAUNCH((mc_emit_kernel<T, S, 8>), tiles, kThreads, stream, (const S*)h->scalars, (const T*)h->coords, h->idx,
+                   (const unsigned char*)h->cases, h->m, (const unsigned long long*)h->tile_slot0,
+                   (const unsigned long long*)h->tile_face0, (T)h->iso, (const unsigned*)h->slot_run, (const unsigned*)h->run_vid,
+                   (const unsigned char*)h->owner, (T*)out_v, out_f);
+    else
+        PCU_LAUNCH((mc_emit_kernel<T, S, 4>), tiles, kThreads, stream, (const S*)h->scalars, (const T*)h->coords, h->idx,
+                   (const unsigned char*)h->cases, h->m, (const unsigned long long*)h->tile_slot0,
+                   (const unsigned long long*)h->tile_face0, (T)h->iso, (const unsigned*)h->slot_run, (const unsigned*)h->run_vid,
+                   (const unsigned char*)h->owner, (T*)out_v, out_f);
+    return PCU_B200_OK;
+}
+
+int marching_cubes_emit_device(pcu_b200_workspace* ws, const pcu_b200_marching_cubes* h, void* out_v, void* out_f, cudaStream_t stream) {
+    if (!ws || !h) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (h->device != ws->device) return fail(PCU_B200_INVALID_ARGUMENT, "the marching-cubes handle lives on device %d, the workspace on %d",
+                                             h->device, ws->device);
+    if (h->slots == 0) return PCU_B200_OK;
+    if (!out_v || (h->faces > 0 && !out_f)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    if (h->t_f64) return h->s_f64 ? mc_emit_launch<double, double>(h, out_v, out_f, stream) : mc_emit_launch<double, float>(h, out_v, out_f, stream);
+    return h->s_f64 ? mc_emit_launch<float, double>(h, out_v, out_f, stream) : mc_emit_launch<float, float>(h, out_v, out_f, stream);
+}
+
+// Codes, their sort, the six-neighbour lookups, the ordered compaction.  out_counts (device): {boundary rows, bad rows}.
+template <typename I>
+int svb_device(pcu_b200_workspace* ws, const I* g, long long n, long long* out_idx, long long* out_counts, cudaStream_t stream) {
+    const long long nblocks = (n + kThreads - 1) / kThreads;
+    const unsigned ntiles = (unsigned)((n + kSortTile - 1) / kSortTile);
+    struct { McRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; unsigned char* keep;
+             unsigned* counts; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.a = cv.take<McRec>((size_t)n);
+        sc.b = cv.take<McRec>((size_t)n);
+        sc.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
+        sc.totals = cv.take<unsigned long long>(kSortBins);
+        sc.base = cv.take<unsigned>(kSortBins);
+        sc.constant = cv.take<int>(1);
+        sc.keep = cv.take<unsigned char>((size_t)n);
+        sc.counts = cv.take<unsigned>((size_t)nblocks);
+    }));
+    PCU_CUDA(cudaMemsetAsync(out_counts, 0, 2 * sizeof(long long), stream));
+    PCU_LAUNCH((svb_codes_kernel<I>), (unsigned)nblocks, kThreads, stream, g, n, sc.a, (unsigned long long*)(out_counts + 1));
+    McRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records<McRec>(sc.a, sc.b, n, 1, sc.hist, sc.totals, sc.base, sc.constant, stream, &sorted));
+    PCU_LAUNCH((svb_flag_kernel<I>), (unsigned)nblocks, kThreads, stream, g, n, (const McRec*)sorted, sc.keep);
+    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)sc.keep, n, sc.counts);
+    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.counts, nblocks, out_counts);
+    PCU_LAUNCH(svb_emit_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)sc.keep, n, (const unsigned*)sc.counts, out_idx);
+    return PCU_B200_OK;
+}
+
+int sparse_voxel_grid_boundary_device(pcu_b200_workspace* ws, const void* g, long long n, int kind, long long* out_idx,
+                                      long long* out_counts, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!g || n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid grid_coordinates has zero rows!");
+    if (n >= 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "sparse_voxel_grid_boundary: at most 2^31 - 2 voxels, got %lld", n);
+    if (kind != kIdxI32 && kind != kIdxI64)
+        return fail(PCU_B200_INVALID_ARGUMENT, "Invalid vertex leads to an overflow integer. Perhaps grid_size is too small.");
+    if (!out_idx || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    return kind == kIdxI64 ? svb_device<long long>(ws, (const long long*)g, n, out_idx, out_counts, stream)
+                           : svb_device<int>(ws, (const int*)g, n, out_idx, out_counts, stream);
+}
+
+// ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
 
 template <typename I>
 int morton_encode_device(pcu_b200_workspace* ws, const I* pts, long long n, unsigned long long* out_codes, cudaStream_t stream) {
@@ -2478,6 +2708,31 @@ int pcu_b200_pointcloud_surfel_geometry_f32(pcu_b200_workspace* ws, const float*
 int pcu_b200_pointcloud_surfel_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np,
                                             int subdivs, double* out_v, int32_t* out_f, void* stream) {
     return surfel_geometry_device<double>(ws, p, n, r, np, subdivs, out_v, out_f, (cudaStream_t)stream);
+}
+
+int pcu_b200_marching_cubes_prepare_f32(pcu_b200_workspace* ws, const void* scalars, int scalars_f64, const float* coords, int64_t n,
+                                        const void* cube_idx, int64_t m, int idx_kind, double isovalue, pcu_b200_marching_cubes** out_mc,
+                                        int64_t out_counts[2], void* stream) {
+    return marching_cubes_prepare_device<float>(ws, scalars, scalars_f64, coords, n, cube_idx, m, idx_kind, isovalue, out_mc,
+                                                (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_marching_cubes_prepare_f64(pcu_b200_workspace* ws, const void* scalars, int scalars_f64, const double* coords, int64_t n,
+                                        const void* cube_idx, int64_t m, int idx_kind, double isovalue, pcu_b200_marching_cubes** out_mc,
+                                        int64_t out_counts[2], void* stream) {
+    return marching_cubes_prepare_device<double>(ws, scalars, scalars_f64, coords, n, cube_idx, m, idx_kind, isovalue, out_mc,
+                                                 (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_marching_cubes_emit(pcu_b200_workspace* ws, const pcu_b200_marching_cubes* mc, void* out_v, void* out_f, void* stream) {
+    return marching_cubes_emit_device(ws, mc, out_v, out_f, (cudaStream_t)stream);
+}
+int pcu_b200_marching_cubes_destroy(pcu_b200_marching_cubes* mc) {
+    if (!mc) return PCU_B200_OK;
+    DeviceGuard guard(mc->device);
+    return mc_free(mc);
+}
+int pcu_b200_sparse_voxel_grid_boundary(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, int64_t* out_idx,
+                                        int64_t* out_counts, void* stream) {
+    return sparse_voxel_grid_boundary_device(ws, grid, n, idx_kind, (long long*)out_idx, (long long*)out_counts, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,

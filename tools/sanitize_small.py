@@ -64,6 +64,14 @@ surf.close()
 cn = rng.normal(size=(n, 3)); ca = rng.random(n)
 step("point cloud winding numbers", lambda: pcu.point_cloud_fast_winding_number(v, cn, ca, ro))
 step("point cloud winding numbers fp32", lambda: pcu.point_cloud_fast_winding_number(v.astype(np.float32), cn.astype(np.float32), ca.astype(np.float32), ro.astype(np.float32)))
+ax = np.linspace(-1, 1, 12)
+gz, gy, gx = np.meshgrid(ax, ax, ax, indexing="ij")
+gc = np.stack([gx.ravel(), gy.ravel(), gz.ravel()], 1)
+cb = np.arange(12 ** 3).reshape(12, 12, 12)[:-1, :-1, :-1].ravel()[:, None] + np.array([0, 1, 13, 12, 144, 145, 157, 156])
+step("marching cubes", lambda: pcu.marching_cubes_sparse_voxel_grid(np.linalg.norm(gc, axis=1) - 0.6, gc, cb, 0.0))
+step("marching cubes fp32 / uint32", lambda: pcu.marching_cubes_sparse_voxel_grid(
+    (np.linalg.norm(gc, axis=1) - 0.6).astype(np.float32), gc.astype(np.float32), cb.astype(np.uint32), 0.0))
+step("sparse voxel grid boundary", lambda: pcu.sparse_voxel_grid_boundary(rng.integers(-10, 10, (n, 3)).astype(np.int32)))
 pts_i = rng.integers(-1000, 1000, (n, 3)).astype(np.int32)
 codes = step("morton encode", lambda: pcu.morton_encode(pts_i))
 step("morton decode", lambda: pcu.morton_decode(codes))
