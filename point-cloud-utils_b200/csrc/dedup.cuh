@@ -16,9 +16,10 @@
 // (tests/test_examples.py:509-531: SV[SVJ] == V, V[SVI] == SV) holds either way.
 //
 // Pipeline: keys (order-preserving integer image of the rounded coordinates) -> radix sort (sort.cuh) -> run heads
-// -> ordered compaction (the keep_* kernels of normals.cuh) -> emit.
+// -> ordered compaction (compact.cuh) -> emit.
 #pragma once
 #include "common.cuh"
+#include "compact.cuh"
 #include "sort.cuh"
 
 namespace pcu {
@@ -72,17 +73,10 @@ template <typename T, typename Rec>
 __global__ void __launch_bounds__(kThreads) dedup_emit_kernel(const Rec* __restrict__ recs, long long n, const unsigned char* __restrict__ head,
                                                               const unsigned* __restrict__ block_offset, const T* __restrict__ pts,
                                                               T* __restrict__ out_pts, int* __restrict__ svi, int* __restrict__ svj) {
-    __shared__ unsigned warp_sum[kThreads / 32];
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned mine = i < n ? head[i] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
+    const unsigned uid = keep_rank<true>(mine, block_offset) - 1u;   // heads up to and including this row
     if (i >= n) return;
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
-    const unsigned uid = before + __popc(ballot & ((2u << lane) - 1u)) - 1u;   // heads up to and including this lane
     const long long row = (long long)recs[i].idx;
     svj[row] = (int)uid;
     if (mine) {
@@ -117,17 +111,10 @@ template <typename I>
 __global__ void __launch_bounds__(kThreads) dedup_faces_emit_kernel(const I* __restrict__ faces, long long nf, int cols,
                                                                     const int* __restrict__ svj, const unsigned char* __restrict__ keep,
                                                                     const unsigned* __restrict__ block_offset, I* __restrict__ out_faces) {
-    __shared__ unsigned warp_sum[kThreads / 32];
     const long long f = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned mine = f < nf ? keep[f] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
+    const unsigned dst = keep_rank(mine, block_offset);
     if (!mine) return;
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
-    const unsigned dst = before + __popc(ballot & ((1u << lane) - 1u));
     for (int c = 0; c < cols; ++c) out_faces[(size_t)dst * cols + c] = (I)svj[faces[f * cols + c]];
 }
 

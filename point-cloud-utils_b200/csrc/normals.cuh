@@ -14,6 +14,7 @@
 // view directions the reference's sign is whatever its SVD happens to return).
 #pragma once
 #include "common.cuh"
+#include "compact.cuh"
 
 namespace pcu {
 
@@ -274,38 +275,17 @@ __global__ void __launch_bounds__(kThreads) normals_ball_kernel(Cloud<T> cl, con
     keep[row] = ok ? 1 : 0;
 }
 
-// Order-preserving compaction of the kept points (the reference's single-thread loop appends in index order,
-// :267-279): per-block counts, one block turns them into offsets, every block scatters its kept rows.
-__global__ void __launch_bounds__(kThreads) keep_count_kernel(const unsigned char* __restrict__ keep, long long n, unsigned* __restrict__ block_count) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned mine = i < n ? keep[i] : 0u;
-    const unsigned total = __syncthreads_count((int)mine);
-    if (threadIdx.x == 0) block_count[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024) keep_offsets_kernel(unsigned* __restrict__ block_count, long long nblocks, long long* __restrict__ out_count) {
-    // nblocks = ceil(n / kThreads) with n < 2^31 rows: fits 32 bits
-    const unsigned kept = block_scan_rounds<1024>(
-        (unsigned)nblocks, [&](unsigned b) { return block_count[b]; }, [&](unsigned b, unsigned ex, unsigned) { block_count[b] = ex; });
-    if (threadIdx.x == 0) *out_count = (long long)kept;
-}
-
+// The kept points and their normals in index order (the reference's single-thread loop appends in that order,
+// :267-279), after keep_count / keep_offsets of compact.cuh.
 template <typename T>
 __global__ void __launch_bounds__(kThreads) keep_scatter_kernel(const unsigned char* __restrict__ keep, long long n,
                                                                 const unsigned* __restrict__ block_offset,
                                                                 const T* __restrict__ normals, long long* __restrict__ out_idx,
                                                                 T* __restrict__ out_normals) {
-    __shared__ unsigned warp_sum[kThreads / 32];
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned mine = i < n ? keep[i] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
+    const unsigned pos = keep_rank(mine, block_offset);
     if (mine) {
-        const unsigned pos = before + __popc(ballot & ((1u << lane) - 1u));
         out_idx[pos] = i;
         out_normals[3ll * pos] = normals[3 * i];
         out_normals[3ll * pos + 1] = normals[3 * i + 1];

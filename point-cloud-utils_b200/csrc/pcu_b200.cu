@@ -27,6 +27,7 @@
 #include "topk.cuh"
 #include "pyramid.cuh"
 #include "kdreplay.cuh"
+#include "compact.cuh"
 #include "normals.cuh"
 #include "morton.cuh"
 #include "sinkhorn.cuh"
@@ -44,6 +45,9 @@ namespace {
 
 thread_local std::string g_error;
 std::atomic<long long> g_launches{0};
+
+// Blocks of kThreads threads for one thread per row.
+inline unsigned blocks_for(long long n) { return (unsigned)((n + kThreads - 1) / kThreads); }
 
 int fail(int status, const char* fmt, ...) {
     char buf[512];
@@ -911,6 +915,20 @@ int resolve_witness_device(pcu_b200_workspace* ws, const T* query, long long n, 
     return PCU_B200_OK;
 }
 
+// ---- ordered compaction (compact.cuh) --------------------------------------------------------------
+// Words of the block-count buffer that compacting n flags takes: one per block of keep_count_kernel.
+inline size_t keep_count_words(long long n) { return blocks_for(n); }
+
+// Enqueues the first two steps of compact.cuh over n flags: the kept rows of every block into `counts`
+// (keep_count_words(n) words), scanned in place into the blocks' offsets, and the total into *out_count (device memory).
+// The caller's emit kernel follows, with blocks_for(n) blocks of kThreads threads.
+int enqueue_keep_offsets(const unsigned char* keep, long long n, unsigned* counts, long long* out_count, cudaStream_t stream) {
+    const unsigned nblocks = blocks_for(n);
+    PCU_LAUNCH(keep_count_kernel, nblocks, kThreads, stream, keep, n, counts);
+    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, counts, (long long)nblocks, out_count);
+    return PCU_B200_OK;
+}
+
 // ---- normals from k nearest neighbours (SURVEY.md 8f N1) -------------------------------------------
 // Self-query top-k (the point itself is its own first neighbour, as in the reference), plane fit, optional
 // orientation / filtering by view directions, order-preserving compaction of the kept points.
@@ -924,20 +942,18 @@ int normals_knn_device(pcu_b200_workspace* ws, const T* points, long long n, con
         return fail(PCU_B200_INVALID_ARGUMENT, "Invalid point set with zero elements: points must have shape (n, 3) (got %lld rows)", n);
     if (!out_idx || !out_normals || !out_count) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
-    const long long nblocks = (n + kThreads - 1) / kThreads;
     long long* nn_idx; T *nn_dist, *dense; unsigned char* keep; unsigned* counts;
     PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
         nn_idx = cv.take<long long>((size_t)n * k);
         nn_dist = cv.take<T>((size_t)n * k);
         dense = cv.take<T>((size_t)3 * n);
         keep = cv.take<unsigned char>((size_t)n);
-        counts = cv.take<unsigned>((size_t)nblocks);
+        counts = cv.take<unsigned>(keep_count_words(n));
     }));
     PCU_TRY(knn_device<T>(ws, points, n, points, n, k, 1, nn_dist, nn_idx, nullptr, stream));
-    PCU_LAUNCH((normals_knn_kernel<T>), (unsigned)nblocks, kThreads, stream, points, n, nn_idx, k, view_dirs, drop_angle_threshold, dense, keep);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, keep, n, counts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, counts, nblocks, out_count);
-    PCU_LAUNCH((keep_scatter_kernel<T>), (unsigned)nblocks, kThreads, stream, keep, n, counts, dense, out_idx, out_normals);
+    PCU_LAUNCH((normals_knn_kernel<T>), blocks_for(n), kThreads, stream, points, n, nn_idx, k, view_dirs, drop_angle_threshold, dense, keep);
+    PCU_TRY(enqueue_keep_offsets(keep, n, counts, out_count, stream));
+    PCU_LAUNCH((keep_scatter_kernel<T>), blocks_for(n), kThreads, stream, keep, n, counts, dense, out_idx, out_normals);
     return PCU_B200_OK;
 }
 
@@ -986,12 +1002,11 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
     const double reach = std::sqrt((double)(T)o->radius);     // the search radius is a squared distance (normals.cuh)
     Plan<T> plan;
     PCU_TRY(single_cloud_plan<T>(ws, points, n, 0.5 * reach, plan, stream));
-    const long long nblocks = (n + kThreads - 1) / kThreads;
     T* dense; unsigned char* keep; unsigned* counts;
     PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
         dense = cv.take<T>((size_t)3 * n);
         keep = cv.take<unsigned char>((size_t)n);
-        counts = cv.take<unsigned>((size_t)nblocks);
+        counts = cv.take<unsigned>(keep_count_words(n));
     }));
     mark(ws, 0, stream);
     mark(ws, 1, stream);
@@ -1001,11 +1016,10 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
     bp.min_pts = o->min_pts_per_ball; bp.max_pts = o->max_pts_per_ball;
     bp.weight_kind = o->weight_function; bp.seed = o->seed;
     PCU_LAUNCH((cell_order_kernel<T>), (unsigned)std::min<long long>(((long long)plan.cv.v[0].cell_cap + kThreads - 1) / kThreads, (long long)ws->sm_count * 64), kThreads, stream, plan.cv.v[0]);
-    PCU_LAUNCH((normals_ball_kernel<T>), (unsigned)nblocks, kThreads, stream, plan.cv.v[0], view_dirs, bp, dense, keep);
+    PCU_LAUNCH((normals_ball_kernel<T>), blocks_for(n), kThreads, stream, plan.cv.v[0], view_dirs, bp, dense, keep);
     mark(ws, 6, stream);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, keep, n, counts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, counts, nblocks, out_count);
-    PCU_LAUNCH((keep_scatter_kernel<T>), (unsigned)nblocks, kThreads, stream, keep, n, counts, dense, out_idx, out_normals);
+    PCU_TRY(enqueue_keep_offsets(keep, n, counts, out_count, stream));
+    PCU_LAUNCH((keep_scatter_kernel<T>), blocks_for(n), kThreads, stream, keep, n, counts, dense, out_idx, out_normals);
     mark(ws, 7, stream);
     mark(ws, 8, stream);
     return PCU_B200_OK;
@@ -1015,7 +1029,7 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
 // The cloud is binned once (cells no finer than half the radius, as for the ball normals), then ONE cooperative launch
 // runs every selection round of poisson.cuh with grid barriers between them -- the number of rounds depends on the
 // data, and a barrier keeps that decision on the device without a launch per possible round -- and the kept rows are
-// compacted in ascending order like the normals' kept points.
+// compacted in ascending order (compact.cuh).
 template <typename T>
 int poisson_grid_blocks(int device, int sm_count, long long n, unsigned* out_blocks) {
     constexpr int kMaxDevices = 64;   // co-residency limit of the cooperative launch, cached per device
@@ -1051,7 +1065,6 @@ int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, do
     PCU_TRY(single_cloud_plan<T>(ws, points, n, 0.5 * (double)r, plan, stream));
     unsigned blocks = 1;
     PCU_TRY(poisson_grid_blocks<T>(ws->device, ws->sm_count, n, &blocks));
-    const long long nblocks = (n + kThreads - 1) / kThreads;
     PoissonScratch s; unsigned* counts;
     PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
         s.ring = cv.take<unsigned>(4);
@@ -1059,7 +1072,7 @@ int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, do
         s.keep = cv.take<unsigned char>((size_t)n);
         s.list[0] = cv.take<unsigned>((size_t)n);
         s.list[1] = cv.take<unsigned>((size_t)n);
-        counts = cv.take<unsigned>((size_t)nblocks);
+        counts = cv.take<unsigned>(keep_count_words(n));
     }));
     PCU_CUDA(cudaMemsetAsync(s.ring, 0, (size_t)((unsigned char*)s.list[0] - (unsigned char*)s.ring), stream));   // ring, state, keep
     mark(ws, 0, stream);
@@ -1071,9 +1084,8 @@ int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, do
     PCU_CUDA(cudaLaunchCooperativeKernel((void*)poisson_rounds_kernel<T>, dim3(blocks), dim3(kThreads), args, 0, stream));
     g_launches.fetch_add(1, std::memory_order_relaxed);
     mark(ws, 6, stream);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, s.keep, n, counts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, counts, nblocks, out_count);
-    PCU_LAUNCH(keep_scatter_rows_kernel, (unsigned)nblocks, kThreads, stream, s.keep, n, counts, out_idx);
+    PCU_TRY(enqueue_keep_offsets(s.keep, n, counts, out_count, stream));
+    PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(n), kThreads, stream, (const unsigned char*)s.keep, n, (const unsigned*)counts, out_idx);
     mark(ws, 7, stream);
     mark(ws, 8, stream);
     return PCU_B200_OK;
@@ -1220,28 +1232,48 @@ int interpolate_device(pcu_b200_workspace* ws, const void* f, long long m, int f
     }
 }
 
-// ---- duplicate removal (SURVEY.md 8f N2, src/remove_duplicates.cpp) ----------------------------------------
-// Stable LSD radix sort of `n` records between two buffers; returns the buffer holding the sorted records.  key_bits > 0:
-// only the low key_bits bits of each key word can be non-zero, and the passes over the bytes above them are skipped.
+// ---- radix sort of records (sort.cuh) ----------------------------------------------------------------------
+// The buffers of one sort of n records.  The caller writes the records to `a`.
 template <typename Rec>
-int radix_sort_records(Rec* a, Rec* b, long long n, int words, unsigned* hist, unsigned long long* totals, unsigned* base, int* constant,
-                       cudaStream_t stream, Rec** sorted, int key_bits = 0) {
-    const unsigned ntiles = (unsigned)((n + kSortTile - 1) / kSortTile);
-    const int bits = key_bits > 0 ? key_bits : (int)sizeof(a->key[0]) * 8;
-    Rec *in = a, *out = b;
+struct SortScratch {
+    Rec *a, *b;                    // the sort's two record buffers
+    unsigned* hist;                // [bin][tile] digit counts
+    unsigned long long* totals;    // per bin
+    unsigned* base;                // per bin
+    int* constant;                 // the pass's digit is the same in every record
+    static unsigned tiles(long long n) { return (unsigned)((n + kSortTile - 1) / kSortTile); }
+    void carve(Carver& cv, long long n) {
+        a = cv.take<Rec>((size_t)n);
+        b = cv.take<Rec>((size_t)n);
+        hist = cv.take<unsigned>((size_t)kSortBins * tiles(n));
+        totals = cv.take<unsigned long long>(kSortBins);
+        base = cv.take<unsigned>(kSortBins);
+        constant = cv.take<int>(1);
+    }
+};
+
+// Stable LSD radix sort of the `n` records in s.a between the two buffers; returns the buffer holding the sorted records.
+// key_bits > 0: only the low key_bits bits of each key word can be non-zero, and the passes over the bytes above them
+// are skipped.
+template <typename Rec>
+int radix_sort_records(const SortScratch<Rec>& s, long long n, int words, cudaStream_t stream, Rec** sorted, int key_bits = 0) {
+    const unsigned ntiles = SortScratch<Rec>::tiles(n);
+    const int bits = key_bits > 0 ? key_bits : (int)sizeof(s.a->key[0]) * 8;
+    Rec *in = s.a, *out = s.b;
     for (int w = words - 1; w >= 0; --w)          // least significant word first
         for (int shift = 0; shift < bits; shift += 8) {
-            PCU_LAUNCH((sort_hist_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, n, w, shift, hist, ntiles);
-            PCU_LAUNCH(sort_scan_rows, kSortBins, kSortThreads, stream, hist, ntiles, totals);
-            PCU_LAUNCH(sort_scan_bins, 1, kSortBins, stream, (const unsigned long long*)totals, n, base, constant);
-            PCU_LAUNCH((sort_scatter_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, out, n, w, shift, (const unsigned*)hist, ntiles,
-                       (const unsigned*)base, (const int*)constant);
+            PCU_LAUNCH((sort_hist_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, n, w, shift, s.hist, ntiles);
+            PCU_LAUNCH(sort_scan_rows, kSortBins, kSortThreads, stream, s.hist, ntiles, s.totals);
+            PCU_LAUNCH(sort_scan_bins, 1, kSortBins, stream, (const unsigned long long*)s.totals, n, s.base, s.constant);
+            PCU_LAUNCH((sort_scatter_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, out, n, w, shift, (const unsigned*)s.hist,
+                       ntiles, (const unsigned*)s.base, (const int*)s.constant);
             std::swap(in, out);
         }
     *sorted = in;
     return PCU_B200_OK;
 }
 
+// ---- duplicate removal (SURVEY.md 8f N2, src/remove_duplicates.cpp) ----------------------------------------
 // faces == nullptr: points only.  out_pts (n, 3), out_svi (n) and out_faces (nf, cols) are sized for the worst case;
 // out_counts[0] = unique points, [1] = surviving faces, [2] = faces with a corner out of range (an error for the caller).
 template <typename T, typename I>
@@ -1256,39 +1288,28 @@ int dedup_device(pcu_b200_workspace* ws, const T* pts, long long n, double epsil
         return fail(PCU_B200_INVALID_ARGUMENT, "faces must be an (m, c) array with 1 <= c <= 16");
     if (nf >= 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "too many faces (%lld)", nf);
     PCU_ON_DEVICE(ws);
-    const long long nblocks = (n + kThreads - 1) / kThreads;
-    const long long fblocks = faces ? (nf + kThreads - 1) / kThreads : 0;
-    const unsigned ntiles = (unsigned)((n + kSortTile - 1) / kSortTile);
-    struct { Rec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; unsigned char* head;
-             unsigned* counts; unsigned char* fkeep; unsigned* fcounts; unsigned* bad; } sc;
+    struct { SortScratch<Rec> sort; unsigned char* head; unsigned* counts; unsigned char* fkeep; unsigned* fcounts; unsigned* bad; } sc;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
-        sc.a = cv.take<Rec>((size_t)n);
-        sc.b = cv.take<Rec>((size_t)n);
-        sc.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
-        sc.totals = cv.take<unsigned long long>(kSortBins);
-        sc.base = cv.take<unsigned>(kSortBins);
-        sc.constant = cv.take<int>(1);
+        sc.sort.carve(cv, n);
         sc.head = cv.take<unsigned char>((size_t)n);
-        sc.counts = cv.take<unsigned>((size_t)nblocks);
+        sc.counts = cv.take<unsigned>(keep_count_words(n));
         sc.fkeep = cv.take<unsigned char>((size_t)std::max<long long>(1, nf));
-        sc.fcounts = cv.take<unsigned>((size_t)std::max<long long>(1, fblocks));
+        sc.fcounts = cv.take<unsigned>(std::max<size_t>(1, faces ? keep_count_words(nf) : 0));
         sc.bad = cv.take<unsigned>(1);
     }));
     PCU_CUDA(cudaMemsetAsync(out_counts, 0, 3 * sizeof(long long), stream));
-    PCU_LAUNCH((dedup_keys_kernel<T>), (unsigned)nblocks, kThreads, stream, pts, n, (T)epsilon, sc.a);
+    PCU_LAUNCH((dedup_keys_kernel<T>), blocks_for(n), kThreads, stream, pts, n, (T)epsilon, sc.sort.a);
     Rec* sorted = nullptr;
-    PCU_TRY(radix_sort_records<Rec>(sc.a, sc.b, n, 3, sc.hist, sc.totals, sc.base, sc.constant, stream, &sorted));
-    PCU_LAUNCH((dedup_heads_kernel<Rec>), (unsigned)nblocks, kThreads, stream, (const Rec*)sorted, n, sc.head);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)sc.head, n, sc.counts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.counts, nblocks, out_counts);
-    PCU_LAUNCH((dedup_emit_kernel<T, Rec>), (unsigned)nblocks, kThreads, stream, (const Rec*)sorted, n, (const unsigned char*)sc.head,
+    PCU_TRY(radix_sort_records(sc.sort, n, 3, stream, &sorted));
+    PCU_LAUNCH((dedup_heads_kernel<Rec>), blocks_for(n), kThreads, stream, (const Rec*)sorted, n, sc.head);
+    PCU_TRY(enqueue_keep_offsets(sc.head, n, sc.counts, out_counts, stream));
+    PCU_LAUNCH((dedup_emit_kernel<T, Rec>), blocks_for(n), kThreads, stream, (const Rec*)sorted, n, (const unsigned char*)sc.head,
                (const unsigned*)sc.counts, pts, out_pts, out_svi, out_svj);
     if (faces != nullptr && nf > 0) {
         PCU_CUDA(cudaMemsetAsync(sc.bad, 0, sizeof(unsigned), stream));
-        PCU_LAUNCH((dedup_faces_flag_kernel<I>), (unsigned)fblocks, kThreads, stream, faces, nf, cols, n, (const int*)out_svj, sc.fkeep, sc.bad);
-        PCU_LAUNCH(keep_count_kernel, (unsigned)fblocks, kThreads, stream, (const unsigned char*)sc.fkeep, nf, sc.fcounts);
-        PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.fcounts, fblocks, out_counts + 1);
-        PCU_LAUNCH((dedup_faces_emit_kernel<I>), (unsigned)fblocks, kThreads, stream, faces, nf, cols, (const int*)out_svj,
+        PCU_LAUNCH((dedup_faces_flag_kernel<I>), blocks_for(nf), kThreads, stream, faces, nf, cols, n, (const int*)out_svj, sc.fkeep, sc.bad);
+        PCU_TRY(enqueue_keep_offsets(sc.fkeep, nf, sc.fcounts, out_counts + 1, stream));
+        PCU_LAUNCH((dedup_faces_emit_kernel<I>), blocks_for(nf), kThreads, stream, faces, nf, cols, (const int*)out_svj,
                    (const unsigned char*)sc.fkeep, (const unsigned*)sc.fcounts, out_faces);
         PCU_LAUNCH(widen_counter_kernel, 1, 1, stream, sc.bad, out_counts + 2);
     }
@@ -1375,18 +1396,11 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
                     unsigned long long* out_bad, cudaStream_t stream, MeshTree<L>& tree, unsigned char* keep = nullptr,
                     const T* n = nullptr, const T* a = nullptr, int subdivs = 0) {
     constexpr bool points = kPointLeaf<L>, surfels = kSurfelLeaf<L>;
-    const unsigned ntiles = (unsigned)((m + kSortTile - 1) / kSortTile);
     const long long inner = std::max<long long>(1, m - 1);
-    struct { MqRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant;
-             int* node_parent; int* leaf_parent; int* arrivals; MqBox* boxes; unsigned char* src; MqBox* in_boxes; } s;
+    struct { SortScratch<MqRec> sort; int* node_parent; int* leaf_parent; int* arrivals; MqBox* boxes; unsigned char* src; MqBox* in_boxes; } s;
     MeshTree<L> t;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
-        s.a = cv.take<MqRec>((size_t)m);
-        s.b = cv.take<MqRec>((size_t)m);
-        s.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
-        s.totals = cv.take<unsigned long long>(kSortBins);
-        s.base = cv.take<unsigned>(kSortBins);
-        s.constant = cv.take<int>(1);
+        s.sort.carve(cv, m);
         s.node_parent = cv.take<int>((size_t)inner);
         s.leaf_parent = cv.take<int>((size_t)m);
         s.arrivals = cv.take<int>((size_t)inner);
@@ -1404,12 +1418,12 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
     PCU_CUDA(cudaMemsetAsync(t.sc->scene, 0x7f, 3 * sizeof(int), stream));       // min: the image of a huge float
     PCU_CUDA(cudaMemsetAsync(t.sc->scene + 3, 0x80, 3 * sizeof(int), stream));   // max: the image of a huge negative one
     PCU_CUDA(cudaMemsetAsync(&t.sc->bad, 0, sizeof(unsigned long long), stream));
-    const unsigned fblocks = (unsigned)((m + kThreads - 1) / kThreads);
+    const unsigned fblocks = blocks_for(m);
     PCU_LAUNCH((mq_bounds_kernel<L, T>), (unsigned)std::min<long long>(fblocks, (long long)ws->sm_count * 8), kThreads, stream,
                v, nv, f, fkind, m, t.sc);
-    PCU_LAUNCH((mq_codes_kernel<L, T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)t.sc, s.a);
+    PCU_LAUNCH((mq_codes_kernel<L, T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)t.sc, s.sort.a);
     MqRec* sorted = nullptr;
-    PCU_TRY(radix_sort_records<MqRec>(s.a, s.b, m, 1, s.hist, s.totals, s.base, s.constant, stream, &sorted));
+    PCU_TRY(radix_sort_records(s.sort, m, 1, stream, &sorted));
     if constexpr (points)
         PCU_LAUNCH((wn_point_leaves_kernel<T>), fblocks, kThreads, stream, v, n, a, m, (const MqRec*)sorted, t.leaves);
     else if constexpr (surfels)
@@ -1711,8 +1725,6 @@ int surfel_geometry_device(pcu_b200_workspace* ws, const T* p, const T* nrm, con
 }
 
 // ---- marching cubes and the boundary of a sparse voxel grid (sparse_voxels.cuh) ------------------------------------
-inline unsigned blocks_for(long long n) { return (unsigned)((n + kThreads - 1) / kThreads); }
-
 int mc_free(pcu_b200_marching_cubes* h) {
     if (h->cube_block) cudaFreeAsync(h->cube_block, h->stream);
     if (h->slot_block) cudaFreeAsync(h->slot_block, h->stream);
@@ -1740,11 +1752,12 @@ int mc_read_counts(pcu_b200_marching_cubes* h, McCounts& out) {
 // vertex ids, and read the vertex count (second synchronisation).
 template <typename T, typename S, int W>
 int mc_build(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t stream) {
-    const long long m = h->m, tiles = (m + kThreads - 1) / kThreads;
+    const long long m = h->m;
+    const unsigned tiles = blocks_for(m);
     PCU_CUDA(cudaMemsetAsync(h->counts, 0, sizeof(McCounts), stream));
-    PCU_LAUNCH((mc_classify_kernel<T, S, W>), (unsigned)tiles, kThreads, stream, (const S*)h->scalars, h->n, h->idx, m, (T)h->iso,
+    PCU_LAUNCH((mc_classify_kernel<T, S, W>), tiles, kThreads, stream, (const S*)h->scalars, h->n, h->idx, m, (T)h->iso,
                h->cases, h->tile_sum, h->counts);
-    PCU_LAUNCH(mc_tiles_kernel, 1, 1024, stream, (const unsigned*)h->tile_sum, tiles, h->tile_slot0, h->tile_face0, h->counts);
+    PCU_LAUNCH(mc_tiles_kernel, 1, 1024, stream, (const unsigned*)h->tile_sum, (long long)tiles, h->tile_slot0, h->tile_face0, h->counts);
     McCounts c;
     PCU_TRY(mc_read_counts(h, c));
     if (c.bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid cube_indices: %llu cubes have a corner outside [0, %lld)", c.bad, h->n);
@@ -1754,7 +1767,6 @@ int mc_build(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t st
     h->faces = (long long)c.faces;
     const long long ns = h->slots;
     if (ns == 0) return PCU_B200_OK;
-    const long long nblocks = (ns + kThreads - 1) / kThreads;
     PCU_TRY(mc_alloc(h->slot_block, carve_at(nullptr, [&](Carver& cv) {
         cv.take<unsigned>((size_t)ns); cv.take<unsigned>((size_t)ns); cv.take<unsigned char>((size_t)ns); }), stream));
     carve_at(h->slot_block, [&](Carver& cv) {
@@ -1762,35 +1774,26 @@ int mc_build(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t st
         h->run_vid = cv.take<unsigned>((size_t)ns);
         h->owner = cv.take<unsigned char>((size_t)ns);
     });
-    const unsigned ntiles = (unsigned)((ns + kSortTile - 1) / kSortTile);
-    struct { McRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; unsigned char* head;
-             unsigned* counts; unsigned* ocounts; long long* owners; } sc;
+    struct { SortScratch<McRec> sort; unsigned char* head; unsigned* counts; unsigned* ocounts; long long* owners; } sc;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
-        sc.a = cv.take<McRec>((size_t)ns);
-        sc.b = cv.take<McRec>((size_t)ns);
-        sc.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
-        sc.totals = cv.take<unsigned long long>(kSortBins);
-        sc.base = cv.take<unsigned>(kSortBins);
-        sc.constant = cv.take<int>(1);
+        sc.sort.carve(cv, ns);
         sc.head = cv.take<unsigned char>((size_t)ns);
-        sc.counts = cv.take<unsigned>((size_t)nblocks);
-        sc.ocounts = cv.take<unsigned>((size_t)nblocks);
+        sc.counts = cv.take<unsigned>(keep_count_words(ns));
+        sc.ocounts = cv.take<unsigned>(keep_count_words(ns));
         sc.owners = cv.take<long long>(1);
     }));
     int b = 1;                                       // bits of the largest corner index, n - 1
     while (b < 31 && ((h->n - 1) >> b) != 0) ++b;
-    PCU_LAUNCH((mc_slots_kernel<W>), (unsigned)tiles, kThreads, stream, h->idx, (const unsigned char*)h->cases, m,
-               (const unsigned long long*)h->tile_slot0, (const unsigned long long*)h->tile_face0, b, sc.a);
+    PCU_LAUNCH((mc_slots_kernel<W>), tiles, kThreads, stream, h->idx, (const unsigned char*)h->cases, m,
+               (const unsigned long long*)h->tile_slot0, (const unsigned long long*)h->tile_face0, b, sc.sort.a);
     McRec* sorted = nullptr;
-    PCU_TRY(radix_sort_records<McRec>(sc.a, sc.b, ns, 1, sc.hist, sc.totals, sc.base, sc.constant, stream, &sorted, 2 * b));
-    PCU_LAUNCH(mc_heads_kernel, (unsigned)nblocks, kThreads, stream, (const McRec*)sorted, ns, sc.head);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)sc.head, ns, sc.counts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.counts, nblocks, &h->counts->verts);
-    PCU_LAUNCH(mc_runs_kernel, (unsigned)nblocks, kThreads, stream, (const McRec*)sorted, ns, (const unsigned char*)sc.head,
+    PCU_TRY(radix_sort_records(sc.sort, ns, 1, stream, &sorted, 2 * b));
+    PCU_LAUNCH(mc_heads_kernel, blocks_for(ns), kThreads, stream, (const McRec*)sorted, ns, sc.head);
+    PCU_TRY(enqueue_keep_offsets(sc.head, ns, sc.counts, &h->counts->verts, stream));
+    PCU_LAUNCH(mc_runs_kernel, blocks_for(ns), kThreads, stream, (const McRec*)sorted, ns, (const unsigned char*)sc.head,
                (const unsigned*)sc.counts, h->slot_run, h->owner);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)h->owner, ns, sc.ocounts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.ocounts, nblocks, sc.owners);
-    PCU_LAUNCH(mc_owner_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)h->owner, ns, (const unsigned*)sc.ocounts,
+    PCU_TRY(enqueue_keep_offsets(h->owner, ns, sc.ocounts, sc.owners, stream));
+    PCU_LAUNCH(mc_owner_kernel, blocks_for(ns), kThreads, stream, (const unsigned char*)h->owner, ns, (const unsigned*)sc.ocounts,
                (const unsigned*)h->slot_run, h->run_vid);
     PCU_TRY(mc_read_counts(h, c));
     h->verts = c.verts;
@@ -1846,20 +1849,18 @@ int marching_cubes_prepare_device(pcu_b200_workspace* ws, const void* scalars, i
     return PCU_B200_OK;
 }
 
-template <typename T, typename S>
+template <typename T, typename S, int W>
 int mc_emit_launch(const pcu_b200_marching_cubes* h, void* out_v, void* out_f, cudaStream_t stream) {
-    const unsigned tiles = (unsigned)((h->m + kThreads - 1) / kThreads);
-    if (h->width == 8)
-        PCU_LAUNCH((mc_emit_kernel<T, S, 8>), tiles, kThreads, stream, (const S*)h->scalars, (const T*)h->coords, h->idx,
-                   (const unsigned char*)h->cases, h->m, (const unsigned long long*)h->tile_slot0,
-                   (const unsigned long long*)h->tile_face0, (T)h->iso, (const unsigned*)h->slot_run, (const unsigned*)h->run_vid,
-                   (const unsigned char*)h->owner, (T*)out_v, out_f);
-    else
-        PCU_LAUNCH((mc_emit_kernel<T, S, 4>), tiles, kThreads, stream, (const S*)h->scalars, (const T*)h->coords, h->idx,
-                   (const unsigned char*)h->cases, h->m, (const unsigned long long*)h->tile_slot0,
-                   (const unsigned long long*)h->tile_face0, (T)h->iso, (const unsigned*)h->slot_run, (const unsigned*)h->run_vid,
-                   (const unsigned char*)h->owner, (T*)out_v, out_f);
+    PCU_LAUNCH((mc_emit_kernel<T, S, W>), blocks_for(h->m), kThreads, stream, (const S*)h->scalars, (const T*)h->coords, h->idx,
+               (const unsigned char*)h->cases, h->m, (const unsigned long long*)h->tile_slot0,
+               (const unsigned long long*)h->tile_face0, (T)h->iso, (const unsigned*)h->slot_run, (const unsigned*)h->run_vid,
+               (const unsigned char*)h->owner, (T*)out_v, out_f);
     return PCU_B200_OK;
+}
+
+template <typename T, typename S>
+int mc_emit_width(const pcu_b200_marching_cubes* h, void* out_v, void* out_f, cudaStream_t stream) {
+    return h->width == 8 ? mc_emit_launch<T, S, 8>(h, out_v, out_f, stream) : mc_emit_launch<T, S, 4>(h, out_v, out_f, stream);
 }
 
 int marching_cubes_emit_device(pcu_b200_workspace* ws, const pcu_b200_marching_cubes* h, void* out_v, void* out_f, cudaStream_t stream) {
@@ -1870,35 +1871,26 @@ int marching_cubes_emit_device(pcu_b200_workspace* ws, const pcu_b200_marching_c
     if (!out_v || (h->faces > 0 && !out_f)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
     PCU_TRY(adopt_stream(ws, stream));
-    if (h->t_f64) return h->s_f64 ? mc_emit_launch<double, double>(h, out_v, out_f, stream) : mc_emit_launch<double, float>(h, out_v, out_f, stream);
-    return h->s_f64 ? mc_emit_launch<float, double>(h, out_v, out_f, stream) : mc_emit_launch<float, float>(h, out_v, out_f, stream);
+    if (h->t_f64) return h->s_f64 ? mc_emit_width<double, double>(h, out_v, out_f, stream) : mc_emit_width<double, float>(h, out_v, out_f, stream);
+    return h->s_f64 ? mc_emit_width<float, double>(h, out_v, out_f, stream) : mc_emit_width<float, float>(h, out_v, out_f, stream);
 }
 
 // Codes, their sort, the six-neighbour lookups, the ordered compaction.  out_counts (device): {boundary rows, bad rows}.
 template <typename I>
 int svb_device(pcu_b200_workspace* ws, const I* g, long long n, long long* out_idx, long long* out_counts, cudaStream_t stream) {
-    const long long nblocks = (n + kThreads - 1) / kThreads;
-    const unsigned ntiles = (unsigned)((n + kSortTile - 1) / kSortTile);
-    struct { McRec *a, *b; unsigned* hist; unsigned long long* totals; unsigned* base; int* constant; unsigned char* keep;
-             unsigned* counts; } sc;
+    struct { SortScratch<McRec> sort; unsigned char* keep; unsigned* counts; } sc;
     PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
-        sc.a = cv.take<McRec>((size_t)n);
-        sc.b = cv.take<McRec>((size_t)n);
-        sc.hist = cv.take<unsigned>((size_t)kSortBins * ntiles);
-        sc.totals = cv.take<unsigned long long>(kSortBins);
-        sc.base = cv.take<unsigned>(kSortBins);
-        sc.constant = cv.take<int>(1);
+        sc.sort.carve(cv, n);
         sc.keep = cv.take<unsigned char>((size_t)n);
-        sc.counts = cv.take<unsigned>((size_t)nblocks);
+        sc.counts = cv.take<unsigned>(keep_count_words(n));
     }));
     PCU_CUDA(cudaMemsetAsync(out_counts, 0, 2 * sizeof(long long), stream));
-    PCU_LAUNCH((svb_codes_kernel<I>), (unsigned)nblocks, kThreads, stream, g, n, sc.a, (unsigned long long*)(out_counts + 1));
+    PCU_LAUNCH((svb_codes_kernel<I>), blocks_for(n), kThreads, stream, g, n, sc.sort.a, (unsigned long long*)(out_counts + 1));
     McRec* sorted = nullptr;
-    PCU_TRY(radix_sort_records<McRec>(sc.a, sc.b, n, 1, sc.hist, sc.totals, sc.base, sc.constant, stream, &sorted));
-    PCU_LAUNCH((svb_flag_kernel<I>), (unsigned)nblocks, kThreads, stream, g, n, (const McRec*)sorted, sc.keep);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)sc.keep, n, sc.counts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, sc.counts, nblocks, out_counts);
-    PCU_LAUNCH(svb_emit_kernel, (unsigned)nblocks, kThreads, stream, (const unsigned char*)sc.keep, n, (const unsigned*)sc.counts, out_idx);
+    PCU_TRY(radix_sort_records(sc.sort, n, 1, stream, &sorted));
+    PCU_LAUNCH((svb_flag_kernel<I>), blocks_for(n), kThreads, stream, g, n, (const McRec*)sorted, sc.keep);
+    PCU_TRY(enqueue_keep_offsets(sc.keep, n, sc.counts, out_counts, stream));
+    PCU_LAUNCH(keep_rows_kernel<long long>, blocks_for(n), kThreads, stream, (const unsigned char*)sc.keep, n, (const unsigned*)sc.counts, out_idx);
     return PCU_B200_OK;
 }
 
@@ -2030,7 +2022,6 @@ int voxel_downsample_device(pcu_b200_workspace* ws, const T* pts, long long n, c
         if (g.size[a] * (T)2147483647 < (T)max_bound[a] - g.min_bound[a]) return fail(PCU_B200_INVALID_ARGUMENT, "Voxel size is too small");
     }
     PCU_ON_DEVICE(ws);
-    const long long nblocks = (n + kThreads - 1) / kThreads;
     unsigned slots = 64;
     while ((long long)slots < 2 * n) slots <<= 1;     // load factor <= 1/2
     int *table, *slot_of; VoxelAcc* acc; double* attr_sum; unsigned char* keep; unsigned* counts;
@@ -2040,15 +2031,14 @@ int voxel_downsample_device(pcu_b200_workspace* ws, const T* pts, long long n, c
         slot_of = cv.take<int>((size_t)n);
         attr_sum = cv.take<double>((size_t)slots * (attr_cols > 0 ? attr_cols : 0) + 1);
         keep = cv.take<unsigned char>((size_t)n);
-        counts = cv.take<unsigned>((size_t)nblocks);
+        counts = cv.take<unsigned>(keep_count_words(n));
     }));
-    PCU_LAUNCH(voxel_init_kernel, (slots + kThreads - 1) / kThreads, kThreads, stream, table, acc, slots);
+    PCU_LAUNCH(voxel_init_kernel, blocks_for(slots), kThreads, stream, table, acc, slots);
     if (attr_cols > 0) PCU_CUDA(cudaMemsetAsync(attr_sum, 0, sizeof(double) * (size_t)slots * attr_cols, stream));
-    PCU_LAUNCH((voxel_insert_kernel<T, A>), (unsigned)nblocks, kThreads, stream, pts, n, g, table, slots, acc, slot_of, attr, attr_cols, attr_sum);
-    PCU_LAUNCH(voxel_flag_kernel, (unsigned)nblocks, kThreads, stream, slot_of, acc, n, min_points, keep);
-    PCU_LAUNCH(keep_count_kernel, (unsigned)nblocks, kThreads, stream, keep, n, counts);
-    PCU_LAUNCH(keep_offsets_kernel, 1, 1024, stream, counts, nblocks, out_rows);
-    PCU_LAUNCH((voxel_emit_kernel<T, A>), (unsigned)nblocks, kThreads, stream, keep, n, counts, slot_of, acc, attr_sum, attr_cols, out_pts, out_attr, out_counts);
+    PCU_LAUNCH((voxel_insert_kernel<T, A>), blocks_for(n), kThreads, stream, pts, n, g, table, slots, acc, slot_of, attr, attr_cols, attr_sum);
+    PCU_LAUNCH(voxel_flag_kernel, blocks_for(n), kThreads, stream, slot_of, acc, n, min_points, keep);
+    PCU_TRY(enqueue_keep_offsets(keep, n, counts, out_rows, stream));
+    PCU_LAUNCH((voxel_emit_kernel<T, A>), blocks_for(n), kThreads, stream, keep, n, counts, slot_of, acc, attr_sum, attr_cols, out_pts, out_attr, out_counts);
     return PCU_B200_OK;
 }
 

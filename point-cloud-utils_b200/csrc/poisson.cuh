@@ -98,20 +98,4 @@ __global__ void __launch_bounds__(kThreads) poisson_rounds_kernel(Cloud<T> cl, T
     if (gtid == 0 && rounds_out != nullptr) *rounds_out = round;
 }
 
-// The kept rows in ascending order as int32 (keep_count_kernel / keep_offsets_kernel of normals.cuh give the offsets).
-__global__ void __launch_bounds__(kThreads) keep_scatter_rows_kernel(const unsigned char* __restrict__ keep, long long n,
-                                                                     const unsigned* __restrict__ block_offset,
-                                                                     int* __restrict__ out_idx) {
-    __shared__ unsigned warp_sum[kThreads / 32];
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned mine = i < n ? keep[i] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
-    if (mine) out_idx[before + __popc(ballot & ((1u << lane) - 1u))] = (int)i;
-}
-
 }  // namespace pcu

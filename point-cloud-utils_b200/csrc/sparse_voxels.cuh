@@ -18,6 +18,7 @@
 // (morton_add2, in the reference's offset order) is not among them.  Integer work only.
 #pragma once
 #include "common.cuh"
+#include "compact.cuh"
 #include "morton.cuh"
 #include "sort.cuh"
 #include "mc_tables.h"
@@ -154,18 +155,12 @@ __global__ void __launch_bounds__(kThreads) mc_heads_kernel(const McRec* __restr
 __global__ void __launch_bounds__(kThreads) mc_runs_kernel(const McRec* __restrict__ recs, long long ns, const unsigned char* __restrict__ head,
                                                            const unsigned* __restrict__ block_offset, unsigned* __restrict__ slot_run,
                                                            unsigned char* __restrict__ owner) {
-    __shared__ unsigned warp_sum[kThreads / 32];
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned mine = i < ns ? head[i] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
+    const unsigned run = keep_rank<true>(mine, block_offset) - 1u;
     if (i >= ns) return;
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
     const unsigned long long slot = recs[i].idx;
-    slot_run[slot] = before + __popc(ballot & ((2u << lane) - 1u)) - 1u;
+    slot_run[slot] = run;
     owner[slot] = (unsigned char)mine;
 }
 
@@ -173,17 +168,10 @@ __global__ void __launch_bounds__(kThreads) mc_runs_kernel(const McRec* __restri
 __global__ void __launch_bounds__(kThreads) mc_owner_kernel(const unsigned char* __restrict__ owner, long long ns,
                                                             const unsigned* __restrict__ block_offset, const unsigned* __restrict__ slot_run,
                                                             unsigned* __restrict__ run_vid) {
-    __shared__ unsigned warp_sum[kThreads / 32];
     const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned mine = s < ns ? owner[s] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
-    if (!mine) return;
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
-    run_vid[slot_run[s]] = before + __popc(ballot & ((1u << lane) - 1u));
+    const unsigned vid = keep_rank(mine, block_offset);
+    if (mine) run_vid[slot_run[s]] = vid;
 }
 
 template <typename T> __device__ __forceinline__ T mc_div(T a, T b);
@@ -277,22 +265,6 @@ __global__ void __launch_bounds__(kThreads) svb_flag_kernel(const I* __restrict_
         boundary = lo == n || __ldg(&sorted[lo].key[0]) != q;
     }
     keep[i] = boundary ? 1 : 0;
-}
-
-// After keep_count / keep_offsets: the kept rows in ascending order, as int64.
-__global__ void __launch_bounds__(kThreads) svb_emit_kernel(const unsigned char* __restrict__ keep, long long n,
-                                                            const unsigned* __restrict__ block_offset, long long* __restrict__ out_idx) {
-    __shared__ unsigned warp_sum[kThreads / 32];
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned mine = i < n ? keep[i] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
-    if (!mine) return;
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
-    out_idx[before + __popc(ballot & ((1u << lane) - 1u))] = i;
 }
 
 }  // namespace pcu

@@ -17,6 +17,7 @@
 // output row is emitted by an ordered compaction.
 #pragma once
 #include "common.cuh"
+#include "compact.cuh"
 
 namespace pcu {
 
@@ -100,23 +101,16 @@ __global__ void __launch_bounds__(kThreads) voxel_flag_kernel(const int* __restr
     keep[i] = (a.first == (int)i && a.count >= min_points) ? 1 : 0;
 }
 
-// pass 3 (after keep_count / keep_offsets of normals.cuh): ordered scatter of the means
+// pass 3 (after keep_count / keep_offsets of compact.cuh): ordered scatter of the means
 template <typename T, typename A>
 __global__ void __launch_bounds__(kThreads) voxel_emit_kernel(const unsigned char* __restrict__ keep, long long n,
                                                               const unsigned* __restrict__ block_offset, const int* __restrict__ slot_of,
                                                               const VoxelAcc* __restrict__ acc, const double* __restrict__ attr_sum, int c,
                                                               T* __restrict__ out_pts, A* __restrict__ out_attr, int* __restrict__ out_count) {
-    __shared__ unsigned warp_sum[kThreads / 32];
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const unsigned mine = i < n ? keep[i] : 0u;
-    const unsigned ballot = __ballot_sync(0xffffffffu, mine != 0u);
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    if (lane == 0) warp_sum[w] = __popc(ballot);
-    __syncthreads();
-    unsigned before = block_offset[blockIdx.x];
-    for (int j = 0; j < w; ++j) before += warp_sum[j];
+    const unsigned pos = keep_rank(mine, block_offset);
     if (mine) {
-        const unsigned pos = before + __popc(ballot & ((1u << lane) - 1u));
         const int h = slot_of[i];
         const VoxelAcc a = acc[h];
         const double cnt = (double)a.count;
