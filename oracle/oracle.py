@@ -306,12 +306,17 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
 # ---- voxel-grid down-sampling (src/sample_point_cloud.cpp:163-244, point_cloud_utils/__init__.py:123-200) ----
 def voxel_indices(points, voxel_size, min_bound):
     """:201-206 -- int(floor((p - min_bound) / voxel_size)) per axis, in the cloud's precision (the binding casts the
-    double arguments to the cloud's scalar type first, :346-354)."""
+    double arguments to the cloud's scalar type first, :346-354).  int(...) is the conversion the reference's x86-64
+    build performs (cvttss2si / cvttsd2si): a value outside [-2^31, 2^31), +-inf and NaN all give INT_MIN.  The rule is
+    applied here explicitly rather than left to numpy's cast of such values, which is platform behaviour."""
     points = np.asarray(points)
     t = points.dtype.type
     size = np.array([t(v) for v in voxel_size], dtype=points.dtype)
     lo = np.array([t(v) for v in min_bound], dtype=points.dtype)
-    return np.floor((points - lo) / size).astype(np.int32)
+    with np.errstate(invalid="ignore", over="ignore"):      # inf - inf, finite / tiny: the quotient is what it is
+        f = np.floor((points - lo) / size)
+    fits = (f >= -2147483648.0) & (f < 2147483648.0)         # False for NaN
+    return np.where(fits, f, -2147483648.0).astype(np.int32)
 
 
 def downsample_point_cloud_on_voxel_grid(voxel_size, points, *attribs, min_bound=None, max_bound=None, min_points_per_voxel=1,

@@ -855,7 +855,10 @@ def downsample_point_cloud_on_voxel_grid(voxel_size, points, *args, min_bound=No
     Mirrors /root/reference/point_cloud_utils/__init__.py:123-200 and /root/reference/src/sample_point_cloud.cpp:163-244.
     Voxel membership, the set of output voxels and their sizes are the reference's exactly; rows come in the order of each
     voxel's first input point (the reference's order is that of a std::unordered_map walk, i.e. unspecified); means are
-    accumulated in fp64 (the reference sums in the array's precision).
+    accumulated in fp64 (the reference sums in the array's precision): within one float32 ulp of the exact mean of the
+    voxel's points for float32 outputs, within the fp64 summation bound for float64 ones.  A point whose index along an
+    axis does not fit an int32 -- far outside explicit bounds, +-inf or NaN -- gets index INT_MIN (-2^31) on that axis,
+    as in the reference, so all such points of one axis share that layer of the grid.
     """
     is_np = isinstance(points, _np.ndarray)
     if not is_np and not _is_tensor(points):

@@ -7,10 +7,14 @@
 // attribute array) to the output.
 //
 // What is exact: the voxel of every point (same rounded subtraction, division and floor), hence the set of occupied
-// voxels, the point count of each and the number of output rows.  What differs, and is stated: the reference walks a
-// std::unordered_map, so its output ORDER is whatever libstdc++'s hash table iteration yields -- here voxels come out
+// voxels, the point count of each and the number of output rows.  That includes points whose quotient does not fit an
+// int -- far outside explicit bounds, +-inf, NaN: the reference's int(...) on x86-64 gives INT_MIN for all of them, so
+// on such an axis they share the INT_MIN layer of the grid here too.  What differs, and is stated: the reference walks
+// a std::unordered_map, so its output ORDER is whatever libstdc++'s hash table iteration yields -- here voxels come out
 // in the order of their first point in the input; and the reference sums in the cloud's precision point after point
-// where this kernel accumulates in fp64 (atomics), so means agree to the rounding of the reference's own float sums.
+// where this kernel accumulates in fp64 (atomics), so the means are within one float32 ulp of the exact mean of the
+// voxel's points for float32 outputs, and within the fp64 summation bound for float64 ones
+// (tests/test_voxel_grid_edges.py), rather than equal to the reference's rounded float sums.
 //
 // No sort: a hash table of point indices (open addressing, 32-bit CAS; a slot's key is the voxel of the point it
 // holds, recomputed when probing) groups the points; per voxel an atomicMin keeps its first point, which is where the
@@ -34,7 +38,10 @@ __device__ __forceinline__ void voxel_of(const VoxelGrid<T>& g, const T* __restr
     for (int a = 0; a < 3; ++a) {
         const T c = sizeof(T) == 4 ? (T)__fdiv_rn((float)R::sub(p[a], g.min_bound[a]), (float)g.size[a])
                                    : (T)__ddiv_rn((double)R::sub(p[a], g.min_bound[a]), (double)g.size[a]);
-        v[a] = (int)floor((double)c);     // floor of a T value is exact in double; int(...) as in the reference
+        // floor of a T value is exact in double.  int(...) as the reference's x86-64 build converts: a value outside
+        // the int range, +-inf and NaN all give INT_MIN (a plain cast here would saturate, and turn NaN into 0)
+        const double f = floor((double)c);
+        v[a] = (f >= -2147483648.0 && f < 2147483648.0) ? (int)f : INT_MIN;
     }
 }
 
