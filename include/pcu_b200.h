@@ -536,6 +536,39 @@ int pcu_b200_marching_cubes_destroy(pcu_b200_marching_cubes* mc);
 int pcu_b200_sparse_voxel_grid_boundary(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, int64_t* out_idx,
                                         int64_t* out_counts, void* stream);
 
+/* ---- triangle-mesh voxelization and 3-D flood fill -----------------------------------------------------------------
+ * Replace voxelize_triangle_mesh and flood_fill_3d (the reference's point_cloud_utils/_voxels.py,
+ * src/voxelize_triangle_mesh.cpp, src/flood_fill_3d.cpp).  Results defined in DESIGN.md §3.
+ *   voxelize_prepare: v (nv, 3) in the suffix's type, f (nf, 3) of kind f_kind, voxel_size > 0 and voxel_origin (host
+ *     arrays of 3).  Voxel (i, j, k) is the box centred at origin + (i, j, k) * size with half-size size / 2; a face
+ *     keeps the voxels of its index bounds [floor((min - o) / s), ceil((max - o) / s)] (x included over the whole
+ *     range) that the reference's triBoxOverlap accepts, in fp64 operation for operation.  Synchronises `stream`
+ *     twice: once to read the accepted count (which sizes the code buffer), once to read the number of distinct
+ *     voxels.  *out_counts = {distinct voxels n, accepted (face, voxel) pairs} (host int64).  A corner outside [0, nv), a non-finite vertex, index bounds outside [INT32_MIN, INT32_MAX - 1], a
+ *     candidate total that overflows int64, 2^31 - 1 or more accepted (face, voxel) pairs, or none at all fail with
+ *     PCU_B200_INVALID_ARGUMENT.  *out_vx (v and f need not outlive prepare) is freed by voxelize_destroy,
+ *     stream-ordered on the stream it was prepared on.
+ *   voxelize_emit: writes out_ijk (n, 3) int32: morton_decode of the distinct 64-bit Morton codes of the kept
+ *     voxels, in ascending code order (coordinates alias beyond 21 bits as in the reference's morton_encode).
+ *   flood_fill_3d: grid (w, h, d) C-ordered of grid_kind, w h d < 2^31, seed inside the grid.  out (same shape and
+ *     type) = grid with fill_value (converted as the reference's x86 build converts a double: integers truncate, NaN
+ *     or out of range give INT_MIN of the type) written over the seed's component among the voxels equal to the
+ *     seed's value, linear index o adjacent to o +- 1, o +- d, o +- h d inside [0, w h d) (so steps past the y and z
+ *     faces wrap, as in the reference).  fill == seed value: out is a copy.  Stream-ordered, no synchronisation.
+ * Every array pointer is a DEVICE pointer. */
+typedef struct pcu_b200_voxelize pcu_b200_voxelize;
+enum pcu_b200_grid_kind { PCU_B200_GRID_I32 = 0, PCU_B200_GRID_I64 = 1, PCU_B200_GRID_F32 = 2, PCU_B200_GRID_F64 = 3 };
+int pcu_b200_voxelize_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                  const double voxel_size[3], const double voxel_origin[3], pcu_b200_voxelize** out_vx,
+                                  int64_t out_counts[2], void* stream);
+int pcu_b200_voxelize_prepare_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                  const double voxel_size[3], const double voxel_origin[3], pcu_b200_voxelize** out_vx,
+                                  int64_t out_counts[2], void* stream);
+int pcu_b200_voxelize_emit(pcu_b200_workspace* ws, const pcu_b200_voxelize* vx, int32_t* out_ijk, void* stream);
+int pcu_b200_voxelize_destroy(pcu_b200_voxelize* vx);
+int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t seed_x,
+                           int64_t seed_y, int64_t seed_z, double fill_value, void* out, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

@@ -714,6 +714,38 @@ void sparse_voxel_grid_boundary_device(uintptr_t grid, int64_t n, int idx_kind, 
     });
 }
 
+// Voxelization (voxelize_triangle_mesh, _voxels.py): tests and sorts (two synchronisations of `stream`), returns
+// (handle, n, accepted (face, voxel) pairs); _voxelize_emit writes the (n, 3) int32 voxels; _voxelize_destroy.
+py::tuple voxelize_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, std::vector<double> size,
+                                  std::vector<double> origin, int device, uintptr_t stream) {
+    if (size.size() != 3 || origin.size() != 3) throw py::value_error("Invalid shape");
+    pcu_b200_voxelize* vx = nullptr;
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_voxelize_prepare_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, size.data(), origin.data(), &vx,
+                                                      counts, (void*)stream)
+                      : pcu_b200_voxelize_prepare_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, size.data(), origin.data(), &vx,
+                                                      counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)vx, counts[0], counts[1]);
+}
+void voxelize_emit_device(uintptr_t vx, uintptr_t out, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_voxelize_emit(ws, (const pcu_b200_voxelize*)vx, (int32_t*)out, (void*)stream);
+    });
+}
+void voxelize_destroy(uintptr_t vx) {
+    py::gil_scoped_release nogil;
+    pcu_b200_voxelize_destroy((pcu_b200_voxelize*)vx);
+}
+// flood_fill_3d: grid and out (w, h, d) C-ordered of grid_kind (pcu_b200_grid_kind); no synchronisation.
+void flood_fill_3d_device(uintptr_t grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t sx, int64_t sy, int64_t sz,
+                          double fill_value, uintptr_t out, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_flood_fill_3d(ws, (const void*)grid, grid_kind, w, h, d, sx, sy, sz, fill_value, (void*)out, (void*)stream);
+    });
+}
+
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
@@ -1122,6 +1154,10 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_marching_cubes_emit_device", &marching_cubes_emit_device);
     mod.def("_marching_cubes_destroy", &marching_cubes_destroy);
     mod.def("_sparse_voxel_grid_boundary_device", &sparse_voxel_grid_boundary_device);
+    mod.def("_voxelize_prepare_device", &voxelize_prepare_device);
+    mod.def("_voxelize_emit_device", &voxelize_emit_device);
+    mod.def("_voxelize_destroy", &voxelize_destroy);
+    mod.def("_flood_fill_3d_device", &flood_fill_3d_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),

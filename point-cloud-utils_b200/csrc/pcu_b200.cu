@@ -38,6 +38,7 @@
 #include "winding.cuh"
 #include "raycast.cuh"
 #include "sparse_voxels.cuh"
+#include "voxelize.cuh"
 
 using namespace pcu;
 
@@ -287,6 +288,17 @@ struct pcu_b200_marching_cubes {
     unsigned* slot_run = nullptr;
     unsigned* run_vid = nullptr;
     unsigned char* owner = nullptr;
+};
+// Voxelization between pcu_b200_voxelize_prepare_* and _emit: the sorted codes, their run heads and the heads' block
+// offsets, in one block allocated and freed in the order of `stream`.
+struct pcu_b200_voxelize {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    long long recs = 0, n = 0;              // accepted (face, voxel) pairs; distinct voxels
+    unsigned char* block = nullptr;
+    const McRec* sorted = nullptr;
+    unsigned char* head = nullptr;
+    unsigned* offsets = nullptr;
 };
 template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
@@ -1907,6 +1919,171 @@ int sparse_voxel_grid_boundary_device(pcu_b200_workspace* ws, const void* g, lon
                            : svb_device<int>(ws, (const int*)g, n, out_idx, out_counts, stream);
 }
 
+// ---- triangle-mesh voxelization and 3-D flood fill (voxelize.cuh) ------------------------------------------------
+int vx_free(pcu_b200_voxelize* h) {
+    if (h->block) cudaFreeAsync(h->block, h->stream);
+    delete h;
+    return PCU_B200_OK;
+}
+
+// Persistent CTAs of vx_test_kernel: enough to fill every SM (the kernel holds 16-32 KB of shared memory per CTA).
+inline unsigned vx_test_blocks(const pcu_b200_workspace* ws) { return (unsigned)ws->sm_count * 6u; }
+
+// Bounds, scan and the counting pass; read the counts (first synchronisation); the code records, sized by the accepted
+// count, their sort and run heads; read the number of distinct codes (second synchronisation).
+template <typename T>
+int vx_build(pcu_b200_workspace* ws, pcu_b200_voxelize* h, const T* v, long long nv, const void* f, long long m, int fkind,
+             const VxGeom& g, cudaStream_t stream) {
+    const long long tiles = (m + kThreads - 1) / kThreads;
+    struct { VxFace* faces; unsigned long long* local; unsigned long long* tile; VxCounts* counts; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.faces = cv.take<VxFace>((size_t)m);
+        sc.local = cv.take<unsigned long long>((size_t)m);
+        sc.tile = cv.take<unsigned long long>((size_t)tiles);
+        sc.counts = cv.take<VxCounts>(1);
+    }));
+    PCU_CUDA(cudaMemsetAsync(sc.counts, 0, sizeof(VxCounts), stream));
+    PCU_LAUNCH((vx_bounds_kernel<T>), (unsigned)tiles, kThreads, stream, v, nv, f, fkind, m, g, sc.faces, sc.local, sc.tile, sc.counts);
+    PCU_LAUNCH(vx_tiles_kernel, 1, 1024, stream, sc.tile, tiles, sc.counts);
+    PCU_LAUNCH((vx_test_kernel<T, false>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
+               (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, (McRec*)nullptr);
+    VxCounts c;
+    PCU_CUDA(cudaMemcpyAsync(&c, sc.counts, sizeof(VxCounts), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    if (c.bad_corner) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", c.bad_corner);
+    if (c.bad_bounds)
+        return fail(PCU_B200_INVALID_ARGUMENT, "voxelize_triangle_mesh: %llu faces have a non-finite vertex or voxel index bounds outside "
+                    "[-2^31, 2^31 - 2]", c.bad_bounds);
+    if (!(c.cand_d < kVxMaxCandidates))
+        return fail(PCU_B200_INVALID_ARGUMENT, "voxelize_triangle_mesh: %.6g candidate voxels overflow a 64-bit count", c.cand_d);
+    if (c.accepted >= 0x7fffffffull)
+        return fail(PCU_B200_INVALID_ARGUMENT, "voxelize_triangle_mesh: at most 2^31 - 2 (face, voxel) overlaps are supported, got %llu",
+                    c.accepted);
+    const long long na = (long long)c.accepted;
+    h->recs = na;
+    if (na == 0) return fail(PCU_B200_INVALID_ARGUMENT, "pts must be an array of shape [n, 3] but got an empty array");
+    struct { SortScratch<McRec> sort; unsigned char* head; unsigned* counts; } hb;
+    const auto carve = [&](Carver& cv) {
+        hb.sort.carve(cv, na);
+        hb.head = cv.take<unsigned char>((size_t)na);
+        hb.counts = cv.take<unsigned>(keep_count_words(na));
+    };
+    const size_t bytes = carve_at(nullptr, carve);
+    const cudaError_t e = cudaMallocAsync((void**)&h->block, bytes, stream);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        h->block = nullptr;
+        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMallocAsync of %zu bytes for voxelization failed: %s", bytes, cudaGetErrorString(e));
+    }
+    carve_at(h->block, carve);
+    PCU_LAUNCH((vx_test_kernel<T, true>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
+               (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, hb.sort.a);
+    McRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(hb.sort, na, 1, stream, &sorted));
+    PCU_LAUNCH(mc_heads_kernel, blocks_for(na), kThreads, stream, (const McRec*)sorted, na, hb.head);
+    PCU_TRY(enqueue_keep_offsets(hb.head, na, hb.counts, &sc.counts->unique, stream));
+    PCU_CUDA(cudaMemcpyAsync(&c, sc.counts, sizeof(VxCounts), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    h->n = c.unique;
+    h->sorted = sorted;
+    h->head = hb.head;
+    h->offsets = hb.counts;
+    return PCU_B200_OK;
+}
+
+template <typename T>
+int voxelize_prepare_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, const double size[3],
+                            const double origin[3], pcu_b200_voxelize** out, long long* out_counts, cudaStream_t stream) {
+    if (!ws || !out || !out_counts || !size || !origin) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    if (!v || !f) return fail(PCU_B200_INVALID_ARGUMENT, "null input pointer");
+    if (nv <= 0 || m <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid input mesh with zero elements");
+    if (m >= 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "voxelize_triangle_mesh: at most 2^31 - 2 faces are supported, got %lld", m);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    // as in the reference, a NaN size passes here (it makes every face's bounds non-finite)
+    if (size[0] <= 0.0 || size[1] <= 0.0 || size[2] <= 0.0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid voxel size");
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    VxGeom g;
+    for (int k = 0; k < 3; ++k) { g.o[k] = origin[k]; g.s[k] = size[k]; g.h[k] = size[k] / 2; }
+    pcu_b200_voxelize* h = new (std::nothrow) pcu_b200_voxelize();
+    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
+    h->device = ws->device;
+    h->stream = stream;
+    const int st = vx_build<T>(ws, h, v, nv, f, m, fkind, g, stream);
+    if (st != PCU_B200_OK) { vx_free(h); return st; }
+    out_counts[0] = h->n;
+    out_counts[1] = h->recs;
+    *out = h;
+    return PCU_B200_OK;
+}
+
+int voxelize_emit_device(pcu_b200_workspace* ws, const pcu_b200_voxelize* h, int32_t* out_ijk, cudaStream_t stream) {
+    if (!ws || !h || !out_ijk) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (h->device != ws->device) return fail(PCU_B200_INVALID_ARGUMENT, "the voxelization handle lives on device %d, the workspace on %d",
+                                             h->device, ws->device);
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_LAUNCH(vx_decode_kernel, blocks_for(h->recs), kThreads, stream, h->sorted, h->recs, (const unsigned char*)h->head,
+               (const unsigned*)h->offsets, (int*)out_ijk);
+    return PCU_B200_OK;
+}
+
+// (T)fill_value as the reference's x86 build converts a double: cvttsd2si for the integers (truncation toward zero; NaN
+// and values whose truncation is out of range give the "integer indefinite" INT_MIN), round to nearest for float.
+template <typename T>
+T ff_cast(double x) {
+    if constexpr (std::is_same<T, int>::value) return (x > -2147483649.0 && x < 2147483648.0) ? (int)x : INT32_MIN;
+    else if constexpr (std::is_same<T, long long>::value) return (x >= -0x1p63 && x < 0x1p63) ? (long long)x : LLONG_MIN;
+    else return (T)x;
+}
+
+// Tiles of at most kFfTileMax voxels, sides powers of two: up to 32 along z, then up to 256 / tz along y, the rest along
+// x, each no larger than the grid needs.
+inline int ff_log2_cover(long long n, int cap_log2) {
+    int l = 0;
+    while (l < cap_log2 && (1ll << l) < n) ++l;
+    return l;
+}
+
+template <typename T>
+int ff_device(pcu_b200_workspace* ws, const T* grid, long long w, long long h, long long d, long long seed, double fill, T* out,
+              cudaStream_t stream) {
+    FfShape s;
+    s.w = w; s.h = h; s.d = d; s.n = w * h * d; s.seed = seed;
+    s.lz = ff_log2_cover(d, 5);
+    s.ly = ff_log2_cover(h, 8 - s.lz);
+    s.lx = ff_log2_cover(w, 10 - s.lz - s.ly);
+    s.tz_n = (unsigned)((d + (1ll << s.lz) - 1) >> s.lz);
+    s.ty_n = (unsigned)((h + (1ll << s.ly) - 1) >> s.ly);
+    const long long tx_n = (w + (1ll << s.lx) - 1) >> s.lx;
+    const long long tiles = tx_n * s.ty_n * s.tz_n;
+    int* P = nullptr;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { P = cv.take<int>((size_t)s.n); }));
+    PCU_LAUNCH((ff_tile_kernel<T>), (unsigned)tiles, kThreads, stream, grid, s, P);
+    PCU_LAUNCH((ff_cross_kernel<T>), (unsigned)tiles, kThreads, stream, grid, s, P);
+    PCU_LAUNCH((ff_out_kernel<T>), blocks_for(s.n), kThreads, stream, grid, s.n, seed, ff_cast<T>(fill), P, out);
+    return PCU_B200_OK;
+}
+
+int flood_fill_3d_device(pcu_b200_workspace* ws, const void* grid, int kind, long long w, long long h, long long d, long long sx,
+                         long long sy, long long sz, double fill, void* out, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!grid || !out) return fail(PCU_B200_INVALID_ARGUMENT, "null pointer");
+    if (sx < 0 || sx >= w || sy < 0 || sy >= h || sz < 0 || sz >= d) return fail(PCU_B200_INVALID_ARGUMENT, "seed point must be inside grid");
+    if (w > 0x7fffffffLL || h > 0x7fffffffLL || d > 0x7fffffffLL || w * h > 0x7fffffffLL || w * h * d > 0x7fffffffLL)
+        return fail(PCU_B200_INVALID_ARGUMENT, "flood_fill_3d: grids of at most 2^31 - 1 voxels are supported, got %lld x %lld x %lld", w, h, d);
+    PCU_ON_DEVICE(ws);
+    const long long seed = (sx * h + sy) * d + sz;
+    switch (kind) {
+        case PCU_B200_GRID_I32: return ff_device<int>(ws, (const int*)grid, w, h, d, seed, fill, (int*)out, stream);
+        case PCU_B200_GRID_I64: return ff_device<long long>(ws, (const long long*)grid, w, h, d, seed, fill, (long long*)out, stream);
+        case PCU_B200_GRID_F32: return ff_device<float>(ws, (const float*)grid, w, h, d, seed, fill, (float*)out, stream);
+        case PCU_B200_GRID_F64: return ff_device<double>(ws, (const double*)grid, w, h, d, seed, fill, (double*)out, stream);
+        default: return fail(PCU_B200_INVALID_ARGUMENT, "unknown grid kind %d", kind);
+    }
+}
+
 // ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
 
 template <typename I>
@@ -2723,6 +2900,31 @@ int pcu_b200_marching_cubes_destroy(pcu_b200_marching_cubes* mc) {
 int pcu_b200_sparse_voxel_grid_boundary(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, int64_t* out_idx,
                                         int64_t* out_counts, void* stream) {
     return sparse_voxel_grid_boundary_device(ws, grid, n, idx_kind, (long long*)out_idx, (long long*)out_counts, (cudaStream_t)stream);
+}
+
+int pcu_b200_voxelize_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                  const double voxel_size[3], const double voxel_origin[3], pcu_b200_voxelize** out_vx,
+                                  int64_t out_counts[2], void* stream) {
+    return voxelize_prepare_device<float>(ws, v, nv, f, nf, f_kind, voxel_size, voxel_origin, out_vx, (long long*)out_counts,
+                                          (cudaStream_t)stream);
+}
+int pcu_b200_voxelize_prepare_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                  const double voxel_size[3], const double voxel_origin[3], pcu_b200_voxelize** out_vx,
+                                  int64_t out_counts[2], void* stream) {
+    return voxelize_prepare_device<double>(ws, v, nv, f, nf, f_kind, voxel_size, voxel_origin, out_vx, (long long*)out_counts,
+                                           (cudaStream_t)stream);
+}
+int pcu_b200_voxelize_emit(pcu_b200_workspace* ws, const pcu_b200_voxelize* vx, int32_t* out_ijk, void* stream) {
+    return voxelize_emit_device(ws, vx, out_ijk, (cudaStream_t)stream);
+}
+int pcu_b200_voxelize_destroy(pcu_b200_voxelize* vx) {
+    if (!vx) return PCU_B200_OK;
+    DeviceGuard guard(vx->device);
+    return vx_free(vx);
+}
+int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t seed_x,
+                           int64_t seed_y, int64_t seed_z, double fill_value, void* out, void* stream) {
+    return flood_fill_3d_device(ws, grid, grid_kind, w, h, d, seed_x, seed_y, seed_z, fill_value, out, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,
