@@ -569,6 +569,47 @@ int pcu_b200_voxelize_destroy(pcu_b200_voxelize* vx);
 int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t seed_x,
                            int64_t seed_y, int64_t seed_z, double fill_value, void* out, void* stream);
 
+/* ---- mesh topology: connected components and vertex removal ----------------------------------------------------------
+ * Replace connected_components, remove_mesh_vertices and remove_unreferenced_mesh_vertices (the reference's
+ * src/connected_components.cpp, src/remove_mesh_vertices.cpp, src/remove_unreferenced_mesh_vertices.cpp).  Results
+ * defined in DESIGN.md §3.  Index arrays are of kind f_kind (pcu_b200_index_kind); outputs of "f's width" are int32
+ * for the 32-bit kinds and int64 for the 64-bit ones (unsigned kinds share the bits).
+ *   connected_components_prepare: f (nf, f_cols), 1 <= nf < 2^31 - 1, f_cols >= 1.  The graph's vertices are [0, n),
+ *     n = max(f) + 1; corner j of every row is joined to corner j + 1.  Component j is the j-th in ascending order of
+ *     its smallest vertex.  Synchronises `stream` twice: once to read max(f) (which sizes the buffers), once to read the
+ *     component count k.  *out_counts = {n, k} (host int64).  An entry of f that is negative or above 2^31 - 2 fails with
+ *     PCU_B200_INVALID_ARGUMENT.  *out_cc (f need not outlive prepare) is freed by connected_components_destroy,
+ *     stream-ordered on the stream it was prepared on.
+ *   connected_components_emit: writes out_cv (n), out_nv (k), out_cf (nf) and out_nf (k) in f's width: the component of
+ *     every vertex, the vertices of every component, the component of every face (that of its first corner) and the
+ *     faces of every component.
+ *   remove_mesh_vertices: v (nv, 3) in the suffix's type, f (nf, 3) int32 or int64, mask (nv) bytes, nonzero = keep.
+ *     out_v (capacity nv rows) receives the kept vertices in input order, out_f (capacity nf rows, f's width) the faces
+ *     whose three corners are kept, re-indexed, in input order.  Synchronises `stream` once; *out_counts = {kept
+ *     vertices, kept faces} (host int64).
+ *   remove_unreferenced_mesh_vertices: v (nv, 3), f (nf, 3) of any index kind.  out_v (capacity nv rows) = v[J];
+ *     out_corr_v (capacity nv) = J, the vertices some corner names, ascending; out_corr_f (nv) = I, I[J[j]] = j and -1
+ *     (all ones for the unsigned kinds) elsewhere; out_f (nf, 3) = I[f]; all in f's width.  Synchronises `stream`
+ *     once; *out_count = #J (host int64).
+ *   For both removals 1 <= nv, nf < 2^31 - 1, and a corner outside [0, nv) fails with PCU_B200_INVALID_ARGUMENT.
+ * Every array pointer is a DEVICE pointer. */
+typedef struct pcu_b200_components pcu_b200_components;
+int pcu_b200_connected_components_prepare(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_cols, int f_kind,
+                                           pcu_b200_components** out_cc, int64_t out_counts[2], void* stream);
+int pcu_b200_connected_components_emit(pcu_b200_workspace* ws, const pcu_b200_components* cc, void* out_cv, void* out_nv, void* out_cf,
+                                        void* out_nf, void* stream);
+int pcu_b200_connected_components_destroy(pcu_b200_components* cc);
+int pcu_b200_remove_mesh_vertices_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                      const uint8_t* mask, float* out_v, void* out_f, int64_t out_counts[2], void* stream);
+int pcu_b200_remove_mesh_vertices_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                      const uint8_t* mask, double* out_v, void* out_f, int64_t out_counts[2], void* stream);
+int pcu_b200_remove_unreferenced_mesh_vertices_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                                   float* out_v, void* out_f, void* out_corr_v, void* out_corr_f, int64_t* out_count,
+                                                   void* stream);
+int pcu_b200_remove_unreferenced_mesh_vertices_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                                   double* out_v, void* out_f, void* out_corr_v, void* out_corr_f, int64_t* out_count,
+                                                   void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

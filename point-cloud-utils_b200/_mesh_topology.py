@@ -1,0 +1,176 @@
+"""connected_components, remove_mesh_vertices and remove_unreferenced_mesh_vertices -- the reference's names, arguments
+and outputs (the reference's src/connected_components.cpp, src/remove_mesh_vertices.cpp and
+src/remove_unreferenced_mesh_vertices.cpp), computed by csrc/mesh_topology.cuh.
+
+numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA torch tensors in -> CUDA tensors out;
+CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages and in its order, before any
+device call.  Shapes are the reference's through npe::move, which squeezes them as numpy does: an (m, 1) result is
+(m,), a single entry is a 0-d array and a single (1, 3) row is (3,)."""
+import numpy as np
+
+from . import _pcu_internal
+from ._mesh_sampling import _INDEX_KINDS, _call_args, _check_float, _check_index, _dtype_name, _form, _torch, _upload, _validate_mesh
+from ._ray_mesh import _matrix_shape
+
+_MAX_ROWS = 2 ** 31 - 1
+
+
+def _back(form, f, *outs):
+    """The outputs squeezed as npe::move squeezes them; numpy when the inputs were (index arrays viewed as f's dtype)."""
+    torch = _torch()
+    outs = [o.squeeze() for o in outs]
+    if form != "numpy":
+        return tuple(outs)
+    return tuple(o.cpu().numpy().view(f.dtype) if o.dtype in (torch.int32, torch.int64) else o.cpu().numpy() for o in outs)
+
+
+def _from_numpy(outs):
+    torch = _torch()
+    return tuple(torch.from_numpy(o) for o in outs)
+
+
+def connected_components(v, f, *, device=None):
+    """
+    Determine the connected components of a mesh
+
+    Args:
+      v : (#v, 3)-shaped array of mesh vertex positions (one vertex position per row)
+      f : (#f, 3)-shaped array of mesh face indexes into v (a row (fi, fj, fk) indicate the 3 vertices of a face)
+      device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+      cv : a (#vertices,)-shaped array of integer indexes (starting from 0) indicating which component each vertex belongs to. i.e. cv[i] is the component of the vertex v[i].
+      nv : the number of vertices in each connected component. i.e. nv[j] is the number of vertices in component j
+      cf : a (#faces,)-shaped array of integer indexes (starting from 0) indicating which component each face belongs to. i.e. cf[i] is the component of the face f[i].
+      nf : the number of faces in each connected component. i.e. nf[j] is the number of faces in component j
+
+    Dtypes: v float32 / float64 (checked, never read: the result depends on f alone), f int32 / int64 / uint32 / uint64
+    of shape (m, c), m, c >= 1 (a 1-D f is one column); all four outputs have f's dtype.  Defined in DESIGN.md §3 as
+    the reference computes it: the graph's vertices are [0, n) with n = max(f) + 1 (libigl's adjacency_matrix sizes it
+    so), not #v, so cv is shorter than #v when the last vertices are unreferenced and longer when f refers past #v;
+    the corners of a row are joined to each other (so edge lists and tets work), and every index no face names is a
+    component of one vertex.  Component j is the j-th in ascending order of its smallest vertex, the order in which the
+    reference starts its BFS runs; cf[i] = cv[f[i, 0]].  Shapes squeezed as npe::move squeezes them: one face gives a
+    0-d cf, one component 0-d nv and nf.
+    Divergences, where the reference is undefined: an f with zero rows or zero columns, a negative index or an index
+    above 2^31 - 2 raise ValueError.
+    """
+    form = _form([v, f], ["v", "f"])
+    _check_float(v, "v")
+    _check_index(f, "f", _INDEX_KINDS)
+    if len(f.shape) not in (1, 2):
+        raise ValueError("connected_components: f must be a 1-D or 2-D array, got shape %s" % (tuple(f.shape),))
+    rows, cols = _matrix_shape(f)
+    if rows == 0 or cols == 0:
+        raise ValueError("connected_components: f must have at least one row and one column, got shape %s" % (tuple(f.shape),))
+    if rows >= _MAX_ROWS:
+        raise ValueError("connected_components: at most 2^31 - 2 faces are supported, got %d" % rows)
+    torch = _torch()
+    if form == "cpu":
+        return _from_numpy(connected_components(v.detach().numpy(), f.detach().numpy(), device=device))
+    (ft,) = _upload(form, [f], device)
+    dev, stream = _call_args(ft)
+    handle, n, k = _pcu_internal._connected_components_prepare_device(ft.data_ptr(), rows, cols, _INDEX_KINDS[_dtype_name(f)], dev,
+                                                                       stream)
+    try:
+        cv = torch.empty(n, dtype=ft.dtype, device=ft.device)
+        nv = torch.empty(k, dtype=ft.dtype, device=ft.device)
+        cf = torch.empty(rows, dtype=ft.dtype, device=ft.device)
+        nf = torch.empty(k, dtype=ft.dtype, device=ft.device)
+        _pcu_internal._connected_components_emit_device(handle, cv.data_ptr(), nv.data_ptr(), cf.data_ptr(), nf.data_ptr(), dev, stream)
+    finally:
+        _pcu_internal._connected_components_destroy(handle)
+    return _back(form, f, cv, nv, cf, nf)
+
+
+def remove_mesh_vertices(v, f, mask, *, device=None):
+    """
+    Removes vertices specified by a mask from a triangle mesh and updates the face indices accordingly.
+
+    Args:
+        v : #v by 3 Matrix of mesh vertex 3D positions
+        f : #f by 3 Matrix of face (triangle) indices
+        mask: A boolean mask of shape (#v,) indicating which vertices to keep (True) or remove (False)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        v_out : (#v, 3)-shaped array of mesh vertices with the mask applied
+        f_out : (#f, 3)-shaped array of mesh faces corresponding to mesh with removed vertices
+
+    Dtypes: v float32 / float64, f int32 / int64, mask bool of shape (#v,) or (#v, 1); v_out has v's dtype, f_out f's.
+    As the reference computes it (src/remove_mesh_vertices.cpp): v_out holds the kept vertices in input order, f_out
+    the faces whose three corners are all kept, in input order, re-indexed to the new numbering.  Shapes squeezed as
+    npe::move squeezes them: one kept vertex gives v_out of shape (3,), one kept face f_out of shape (3,).
+    Divergence: a face corner outside [0, #v) raises ValueError (the reference reads out of bounds).
+    """
+    form = _form([v, f, mask], ["v", "f", "mask"])
+    _check_float(v, "v")
+    _check_index(f, "f", {"int32": 0, "int64": 1})
+    _check_index(mask, "mask", {"bool": 0})
+    _validate_mesh(v, f, _INDEX_KINDS)
+    mrows, mcols = _matrix_shape(mask)
+    if mrows != v.shape[0]:
+        raise ValueError("mask should have the same number of rows as v")
+    if mcols != 1:
+        raise ValueError("mask should have only one column")
+    nvert, nface = int(v.shape[0]), int(f.shape[0])
+    if nvert >= _MAX_ROWS or nface >= _MAX_ROWS:
+        raise ValueError("remove_mesh_vertices: at most 2^31 - 2 vertices and faces are supported, got %d and %d" % (nvert, nface))
+    torch = _torch()
+    if form == "cpu":
+        return _from_numpy(remove_mesh_vertices(v.detach().numpy(), f.detach().numpy(), mask.detach().numpy(), device=device))
+    vt, ft, mt = _upload(form, [v, f, mask.reshape(-1)], device)
+    dev, stream = _call_args(vt)
+    v_out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
+    f_out = torch.empty((nface, 3), dtype=ft.dtype, device=vt.device)
+    kv, kf = _pcu_internal._remove_mesh_vertices_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                                        _INDEX_KINDS[_dtype_name(f)], mt.data_ptr(), v_out.data_ptr(), f_out.data_ptr(),
+                                                        dev, stream)
+    return _back(form, f, v_out[:kv], f_out[:kf])
+
+
+def remove_unreferenced_mesh_vertices(v, f, *, device=None):
+    """
+    Removes the vertices of a triangle mesh that no face references.
+
+    Args:
+        v : (#v, 3)-shaped array of mesh vertex 3D positions
+        f : (#f, 3)-shaped array of face (triangle) indices
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        v_new : (#v_new, 3)-shaped array of mesh vertex positions without unreferenced vertices
+        f_new : (#f, 3)-shaped array of mesh faces indexing into v_new
+        correspondences_v : (#v_new,)-shaped array J of old vertex indices, so that v_new = v[J]
+        correspondences_f : (#v,)-shaped array I of new vertex indices, so that f_new = I[f]; -1 (converted to f's
+                            dtype, so all ones for uint32 / uint64) for the unreferenced vertices
+
+    Dtypes: v float32 / float64, f int32 / int64 / uint32 / uint64; the index outputs have f's dtype.  As the reference
+    computes it (igl::remove_unreferenced(V, F, NV, NF, I, J), returned as (NV, NF, J, I)): a vertex is referenced
+    when some face corner names it; J lists the referenced vertices in ascending order, and every face is kept.  The
+    reference's own docstring describes the two correspondence arrays otherwise ("(#v, 1)-shaped ... v_new =
+    correspondences_v[svi]", "(#f, 1)-shaped ... f_new = correspondences_f[svj]"); the shapes and meanings above are what
+    it returns.  Shapes squeezed as npe::move squeezes them: one referenced vertex gives v_new of shape (3,) and a 0-d
+    correspondences_v, one face f_new of shape (3,), one vertex a 0-d correspondences_f.
+    Divergence: a face corner outside [0, #v) raises ValueError, -1 included (libigl's handling of it depends on its
+    version).
+    """
+    form = _form([v, f], ["v", "f"])
+    _validate_mesh(v, f, _INDEX_KINDS)
+    nvert, nface = int(v.shape[0]), int(f.shape[0])
+    if nvert >= _MAX_ROWS or nface >= _MAX_ROWS:
+        raise ValueError("remove_unreferenced_mesh_vertices: at most 2^31 - 2 vertices and faces are supported, got %d and %d"
+                         % (nvert, nface))
+    torch = _torch()
+    if form == "cpu":
+        return _from_numpy(remove_unreferenced_mesh_vertices(v.detach().numpy(), f.detach().numpy(), device=device))
+    vt, ft = _upload(form, [v, f], device)
+    dev, stream = _call_args(vt)
+    v_out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
+    f_out = torch.empty((nface, 3), dtype=ft.dtype, device=vt.device)
+    corr_v = torch.empty(nvert, dtype=ft.dtype, device=vt.device)
+    corr_f = torch.empty(nvert, dtype=ft.dtype, device=vt.device)
+    kept = _pcu_internal._remove_unreferenced_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                                     _INDEX_KINDS[_dtype_name(f)], v_out.data_ptr(), f_out.data_ptr(), corr_v.data_ptr(),
+                                                     corr_f.data_ptr(), dev, stream)
+    return _back(form, f, v_out[:kept], f_out, corr_v[:kept], corr_f)

@@ -746,6 +746,57 @@ void flood_fill_3d_device(uintptr_t grid, int grid_kind, int64_t w, int64_t h, i
     });
 }
 
+// Connected components (connected_components, _mesh_topology.py): validates f and labels (two synchronisations of
+// `stream`), returns (handle, n = max(f) + 1, components); _connected_components_emit writes cv, nv, cf and nf in f's
+// width; _connected_components_destroy.
+py::tuple connected_components_prepare_device(uintptr_t f, int64_t nf, int f_cols, int f_kind, int device, uintptr_t stream) {
+    pcu_b200_components* cc = nullptr;
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_connected_components_prepare(ws, (const void*)f, nf, f_cols, f_kind, &cc, counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)cc, counts[0], counts[1]);
+}
+void connected_components_emit_device(uintptr_t cc, uintptr_t out_cv, uintptr_t out_nv, uintptr_t out_cf, uintptr_t out_nf, int device,
+                                      uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_connected_components_emit(ws, (const pcu_b200_components*)cc, (void*)out_cv, (void*)out_nv, (void*)out_cf,
+                                                  (void*)out_nf, (void*)stream);
+    });
+}
+void connected_components_destroy(uintptr_t cc) {
+    py::gil_scoped_release nogil;
+    pcu_b200_connected_components_destroy((pcu_b200_components*)cc);
+}
+// remove_mesh_vertices: out_v (capacity nv rows), out_f (capacity nf rows, f's width); one synchronisation; returns
+// (kept vertices, kept faces).
+py::tuple remove_mesh_vertices_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t mask,
+                                      uintptr_t out_v, uintptr_t out_f, int device, uintptr_t stream) {
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_remove_mesh_vertices_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (const uint8_t*)mask,
+                                                          (double*)out_v, (void*)out_f, counts, (void*)stream)
+                      : pcu_b200_remove_mesh_vertices_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (const uint8_t*)mask,
+                                                          (float*)out_v, (void*)out_f, counts, (void*)stream);
+    });
+    return py::make_tuple(counts[0], counts[1]);
+}
+// remove_unreferenced_mesh_vertices: out_v and out_corr_v (capacity nv rows), out_f (nf, 3) and out_corr_f (nv), the
+// index arrays in f's width; one synchronisation; returns the kept vertex count.
+int64_t remove_unreferenced_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out_v,
+                                   uintptr_t out_f, uintptr_t out_corr_v, uintptr_t out_corr_f, int device, uintptr_t stream) {
+    int64_t kept = 0;
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_remove_unreferenced_mesh_vertices_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (double*)out_v,
+                                                                       (void*)out_f, (void*)out_corr_v, (void*)out_corr_f, &kept,
+                                                                       (void*)stream)
+                      : pcu_b200_remove_unreferenced_mesh_vertices_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (float*)out_v,
+                                                                       (void*)out_f, (void*)out_corr_v, (void*)out_corr_f, &kept,
+                                                                       (void*)stream);
+    });
+    return kept;
+}
+
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
@@ -1158,6 +1209,11 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_voxelize_emit_device", &voxelize_emit_device);
     mod.def("_voxelize_destroy", &voxelize_destroy);
     mod.def("_flood_fill_3d_device", &flood_fill_3d_device);
+    mod.def("_connected_components_prepare_device", &connected_components_prepare_device);
+    mod.def("_connected_components_emit_device", &connected_components_emit_device);
+    mod.def("_connected_components_destroy", &connected_components_destroy);
+    mod.def("_remove_mesh_vertices_device", &remove_mesh_vertices_device);
+    mod.def("_remove_unreferenced_device", &remove_unreferenced_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),

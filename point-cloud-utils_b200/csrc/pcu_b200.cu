@@ -39,6 +39,7 @@
 #include "raycast.cuh"
 #include "sparse_voxels.cuh"
 #include "voxelize.cuh"
+#include "mesh_topology.cuh"
 
 using namespace pcu;
 
@@ -299,6 +300,20 @@ struct pcu_b200_voxelize {
     const McRec* sorted = nullptr;
     unsigned char* head = nullptr;
     unsigned* offsets = nullptr;
+};
+// Connected components between pcu_b200_connected_components_prepare and _emit: int32 labels and counts in one block
+// allocated and freed in the order of `stream` (cv over n = max(f) + 1 vertices, cf over m faces, nv and nf over
+// the k components, sized n).
+struct pcu_b200_components {
+    int device = 0;
+    cudaStream_t stream = nullptr;
+    int fkind = 0;
+    long long n = 0, m = 0, k = 0;
+    unsigned char* block = nullptr;
+    const int* cv = nullptr;
+    const int* cf = nullptr;
+    const int* nv = nullptr;
+    const int* nf = nullptr;
 };
 template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
@@ -2084,6 +2099,199 @@ int flood_fill_3d_device(pcu_b200_workspace* ws, const void* grid, int kind, lon
     }
 }
 
+// ---- mesh connected components and vertex removal (mesh_topology.cuh) ----------------------------------------------
+int cc_free(pcu_b200_components* h) {
+    if (h->block) cudaFreeAsync(h->block, h->stream);
+    delete h;
+    return PCU_B200_OK;
+}
+
+// Persistent CTAs of cc_validate_kernel.
+inline unsigned cc_validate_blocks(const pcu_b200_workspace* ws, long long total) {
+    return (unsigned)std::max(1ll, std::min((long long)ws->sm_count * 8, (total + kThreads - 1) / kThreads));
+}
+
+// Validate f and read max(f) (first synchronisation); the labels and counts in the handle's block; read the component
+// count (second synchronisation).
+int cc_build(pcu_b200_workspace* ws, pcu_b200_components* h, const void* f, long long m, int c, int fkind, cudaStream_t stream) {
+    CcCounts* rec = nullptr;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { rec = cv.take<CcCounts>(1); }));
+    PCU_CUDA(cudaMemsetAsync(rec, 0, sizeof(CcCounts), stream));
+    const long long total = m * c;
+    PCU_LAUNCH(cc_validate_kernel, cc_validate_blocks(ws, total), kThreads, stream, f, fkind, total, rec);
+    CcCounts hc;
+    PCU_CUDA(cudaMemcpyAsync(&hc, rec, sizeof(CcCounts), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    if (hc.bad)
+        return fail(PCU_B200_INVALID_ARGUMENT, "connected_components: %llu face indices are negative or above 2^31 - 2", hc.bad);
+    const long long n = (long long)hc.max_index + 1;
+    struct { int *P, *root, *rank, *nv, *nf, *cf; unsigned char* is_root; unsigned* counts; } b;
+    const auto carve = [&](Carver& cv) {
+        b.P = cv.take<int>((size_t)n);
+        b.root = cv.take<int>((size_t)n);
+        b.rank = cv.take<int>((size_t)n);
+        b.nv = cv.take<int>((size_t)n);
+        b.nf = cv.take<int>((size_t)n);
+        b.cf = cv.take<int>((size_t)m);
+        b.is_root = cv.take<unsigned char>((size_t)n);
+        b.counts = cv.take<unsigned>(keep_count_words(n));
+    };
+    const size_t bytes = carve_at(nullptr, carve);
+    const cudaError_t e = cudaMallocAsync((void**)&h->block, bytes, stream);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        h->block = nullptr;
+        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMallocAsync of %zu bytes for connected components failed: %s", bytes, cudaGetErrorString(e));
+    }
+    carve_at(h->block, carve);
+    PCU_CUDA(cudaMemsetAsync(b.nv, 0, sizeof(int) * (size_t)n, stream));
+    PCU_CUDA(cudaMemsetAsync(b.nf, 0, sizeof(int) * (size_t)n, stream));
+    PCU_LAUNCH(cc_init_kernel, blocks_for(n), kThreads, stream, b.P, n);
+    PCU_LAUNCH(cc_hook_kernel, blocks_for(m), kThreads, stream, f, fkind, m, c, b.P);
+    PCU_LAUNCH(cc_flatten_kernel, blocks_for(n), kThreads, stream, b.P, n, b.root, b.is_root);
+    PCU_TRY(enqueue_keep_offsets(b.is_root, n, b.counts, &rec->ncomp, stream));
+    PCU_LAUNCH(cc_rank_kernel, blocks_for(n), kThreads, stream, (const unsigned char*)b.is_root, n, (const unsigned*)b.counts, b.rank);
+    PCU_LAUNCH(cc_label_kernel, blocks_for(n), kThreads, stream, b.root, n, (const int*)b.rank, b.nv);
+    PCU_LAUNCH(cc_face_kernel, blocks_for(m), kThreads, stream, f, fkind, m, c, (const int*)b.root, b.cf, b.nf);
+    PCU_CUDA(cudaMemcpyAsync(&hc, rec, sizeof(CcCounts), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    h->n = n;
+    h->m = m;
+    h->k = hc.ncomp;
+    h->cv = b.root;
+    h->cf = b.cf;
+    h->nv = b.nv;
+    h->nf = b.nf;
+    return PCU_B200_OK;
+}
+
+int connected_components_prepare_device(pcu_b200_workspace* ws, const void* f, long long m, int c, int fkind, pcu_b200_components** out,
+                                        long long* out_counts, cudaStream_t stream) {
+    if (!ws || !out || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    if (!f) return fail(PCU_B200_INVALID_ARGUMENT, "null input pointer");
+    if (m <= 0 || c <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "connected_components: f must have at least one row and one column");
+    if (m >= 0x7fffffffLL || m * c >= (1ll << 40))
+        return fail(PCU_B200_INVALID_ARGUMENT, "connected_components: at most 2^31 - 2 faces are supported, got %lld x %d", m, c);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    pcu_b200_components* h = new (std::nothrow) pcu_b200_components();
+    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
+    h->device = ws->device;
+    h->stream = stream;
+    h->fkind = fkind;
+    const int st = cc_build(ws, h, f, m, c, fkind, stream);
+    if (st != PCU_B200_OK) { cc_free(h); return st; }
+    out_counts[0] = h->n;
+    out_counts[1] = h->k;
+    *out = h;
+    return PCU_B200_OK;
+}
+
+int connected_components_emit_device(pcu_b200_workspace* ws, const pcu_b200_components* h, void* out_cv, void* out_nv, void* out_cf,
+                                     void* out_nf, cudaStream_t stream) {
+    if (!ws || !h || !out_cv || !out_nv || !out_cf || !out_nf) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (h->device != ws->device)
+        return fail(PCU_B200_INVALID_ARGUMENT, "the components handle lives on device %d, the workspace on %d", h->device, ws->device);
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    const unsigned blocks = blocks_for(std::max(h->n, h->m));
+    if (h->fkind == kIdxI64 || h->fkind == kIdxU64)
+        PCU_LAUNCH(cc_emit_kernel<long long>, blocks, kThreads, stream, h->cv, h->n, h->cf, h->m, h->nv, h->nf, h->k, (long long*)out_cv,
+                   (long long*)out_cf, (long long*)out_nv, (long long*)out_nf);
+    else
+        PCU_LAUNCH(cc_emit_kernel<int>, blocks, kThreads, stream, h->cv, h->n, h->cf, h->m, h->nv, h->nf, h->k, (int*)out_cv, (int*)out_cf,
+                   (int*)out_nv, (int*)out_nf);
+    return PCU_B200_OK;
+}
+
+// Arguments shared by the two removals.
+int mt_check(const pcu_b200_workspace* ws, const void* v, long long nv, const void* f, long long m, int fkind) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!v || !f) return fail(PCU_B200_INVALID_ARGUMENT, "null input pointer");
+    if (nv <= 0 || m <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid input mesh with zero elements");
+    if (nv >= 0x7fffffffLL || m >= 0x7fffffffLL)
+        return fail(PCU_B200_INVALID_ARGUMENT, "at most 2^31 - 2 vertices and faces are supported, got %lld and %lld", nv, m);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    return PCU_B200_OK;
+}
+
+// Reads the removal's counts (the one synchronisation) and fails on a corner out of range.
+int mt_read(MtCounts* rec, MtCounts* host, cudaStream_t stream) {
+    PCU_CUDA(cudaMemcpyAsync(host, rec, sizeof(MtCounts), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    if (host->bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", host->bad);
+    return PCU_B200_OK;
+}
+
+template <typename T>
+int remove_mesh_vertices_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind,
+                                const unsigned char* mask, T* out_v, void* out_f, long long* out_counts, cudaStream_t stream) {
+    PCU_TRY(mt_check(ws, v, nv, f, m, fkind));
+    if (fkind != kIdxI32 && fkind != kIdxI64) return fail(PCU_B200_INVALID_ARGUMENT, "remove_mesh_vertices: f must be int32 or int64");
+    if (!mask || !out_v || !out_f || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    PCU_ON_DEVICE(ws);
+    struct { MtCounts* rec; int* remap; unsigned* vcounts; unsigned char* keep; unsigned* fcounts; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.rec = cv.take<MtCounts>(1);
+        sc.remap = cv.take<int>((size_t)nv);
+        sc.vcounts = cv.take<unsigned>(keep_count_words(nv));
+        sc.keep = cv.take<unsigned char>((size_t)m);
+        sc.fcounts = cv.take<unsigned>(keep_count_words(m));
+    }));
+    PCU_CUDA(cudaMemsetAsync(sc.rec, 0, sizeof(MtCounts), stream));
+    PCU_TRY(enqueue_keep_offsets(mask, nv, sc.vcounts, &sc.rec->kept_v, stream));
+    PCU_LAUNCH(rmv_vertex_kernel<T>, blocks_for(nv), kThreads, stream, v, nv, mask, (const unsigned*)sc.vcounts, out_v, sc.remap);
+    PCU_LAUNCH(rmv_face_flag_kernel, blocks_for(m), kThreads, stream, f, fkind, m, nv, (const int*)sc.remap, sc.keep, sc.rec);
+    PCU_TRY(enqueue_keep_offsets(sc.keep, m, sc.fcounts, &sc.rec->kept_f, stream));
+    if (fkind == kIdxI64)
+        PCU_LAUNCH(rmv_face_emit_kernel<long long>, blocks_for(m), kThreads, stream, f, fkind, m, nv, (const unsigned char*)sc.keep,
+                   (const unsigned*)sc.fcounts, (const int*)sc.remap, (long long*)out_f);
+    else
+        PCU_LAUNCH(rmv_face_emit_kernel<int>, blocks_for(m), kThreads, stream, f, fkind, m, nv, (const unsigned char*)sc.keep,
+                   (const unsigned*)sc.fcounts, (const int*)sc.remap, (int*)out_f);
+    MtCounts hc;
+    PCU_TRY(mt_read(sc.rec, &hc, stream));
+    out_counts[0] = hc.kept_v;
+    out_counts[1] = hc.kept_f;
+    return PCU_B200_OK;
+}
+
+template <typename T, typename I>
+int rur_launch(const T* v, long long nv, const void* f, long long m, int fkind, const unsigned char* used, const unsigned* vcounts,
+               T* out_v, void* out_f, void* out_j, void* out_i, cudaStream_t stream) {
+    PCU_LAUNCH((rur_vertex_kernel<T, I>), blocks_for(nv), kThreads, stream, v, nv, used, vcounts, out_v, (I*)out_j, (I*)out_i);
+    PCU_LAUNCH(rur_face_kernel<I>, blocks_for(3 * m), kThreads, stream, f, fkind, 3 * m, nv, (const I*)out_i, (I*)out_f);
+    return PCU_B200_OK;
+}
+
+template <typename T>
+int remove_unreferenced_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, T* out_v,
+                               void* out_f, void* out_j, void* out_i, long long* out_count, cudaStream_t stream) {
+    PCU_TRY(mt_check(ws, v, nv, f, m, fkind));
+    if (!out_v || !out_f || !out_j || !out_i || !out_count) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    PCU_ON_DEVICE(ws);
+    struct { MtCounts* rec; unsigned char* used; unsigned* vcounts; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.rec = cv.take<MtCounts>(1);
+        sc.used = cv.take<unsigned char>((size_t)nv);
+        sc.vcounts = cv.take<unsigned>(keep_count_words(nv));
+    }));
+    PCU_CUDA(cudaMemsetAsync(sc.rec, 0, sizeof(MtCounts), stream));
+    PCU_CUDA(cudaMemsetAsync(sc.used, 0, (size_t)nv, stream));
+    PCU_LAUNCH(rur_mark_kernel, blocks_for(m), kThreads, stream, f, fkind, m, nv, sc.used, sc.rec);
+    PCU_TRY(enqueue_keep_offsets(sc.used, nv, sc.vcounts, &sc.rec->kept_v, stream));
+    if (fkind == kIdxI64 || fkind == kIdxU64)
+        PCU_TRY((rur_launch<T, long long>(v, nv, f, m, fkind, sc.used, sc.vcounts, out_v, out_f, out_j, out_i, stream)));
+    else
+        PCU_TRY((rur_launch<T, int>(v, nv, f, m, fkind, sc.used, sc.vcounts, out_v, out_f, out_j, out_i, stream)));
+    MtCounts hc;
+    PCU_TRY(mt_read(sc.rec, &hc, stream));
+    *out_count = hc.kept_v;
+    return PCU_B200_OK;
+}
+
 // ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
 
 template <typename I>
@@ -2925,6 +3133,40 @@ int pcu_b200_voxelize_destroy(pcu_b200_voxelize* vx) {
 int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t seed_x,
                            int64_t seed_y, int64_t seed_z, double fill_value, void* out, void* stream) {
     return flood_fill_3d_device(ws, grid, grid_kind, w, h, d, seed_x, seed_y, seed_z, fill_value, out, (cudaStream_t)stream);
+}
+
+int pcu_b200_connected_components_prepare(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_cols, int f_kind,
+                                           pcu_b200_components** out_cc, int64_t out_counts[2], void* stream) {
+    return connected_components_prepare_device(ws, f, nf, f_cols, f_kind, out_cc, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_connected_components_emit(pcu_b200_workspace* ws, const pcu_b200_components* cc, void* out_cv, void* out_nv, void* out_cf,
+                                        void* out_nf, void* stream) {
+    return connected_components_emit_device(ws, cc, out_cv, out_nv, out_cf, out_nf, (cudaStream_t)stream);
+}
+int pcu_b200_connected_components_destroy(pcu_b200_components* cc) {
+    if (!cc) return PCU_B200_OK;
+    DeviceGuard guard(cc->device);
+    return cc_free(cc);
+}
+int pcu_b200_remove_mesh_vertices_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                      const uint8_t* mask, float* out_v, void* out_f, int64_t out_counts[2], void* stream) {
+    return remove_mesh_vertices_device<float>(ws, v, nv, f, nf, f_kind, mask, out_v, out_f, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_remove_mesh_vertices_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                      const uint8_t* mask, double* out_v, void* out_f, int64_t out_counts[2], void* stream) {
+    return remove_mesh_vertices_device<double>(ws, v, nv, f, nf, f_kind, mask, out_v, out_f, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_remove_unreferenced_mesh_vertices_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                                   float* out_v, void* out_f, void* out_corr_v, void* out_corr_f, int64_t* out_count,
+                                                   void* stream) {
+    return remove_unreferenced_device<float>(ws, v, nv, f, nf, f_kind, out_v, out_f, out_corr_v, out_corr_f, (long long*)out_count,
+                                             (cudaStream_t)stream);
+}
+int pcu_b200_remove_unreferenced_mesh_vertices_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                                   double* out_v, void* out_f, void* out_corr_v, void* out_corr_f, int64_t* out_count,
+                                                   void* stream) {
+    return remove_unreferenced_device<double>(ws, v, nv, f, nf, f_kind, out_v, out_f, out_corr_v, out_corr_f, (long long*)out_count,
+                                              (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,

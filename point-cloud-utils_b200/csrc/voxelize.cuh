@@ -19,7 +19,7 @@
 // the voxels equal to the seed's value, by union-find on int32 parents (parent <= index, roots are the smallest index
 // of their tree), in passes that do not depend on the region's shape:
 //   ff_tile_kernel     union-find in shared memory over a 3-D tile (z fastest): the +1, +d, +h d edges inside it
-//   ff_cross_kernel    the edges that leave a tile or wrap, united in global memory with atomicMin
+//   ff_cross_kernel    the edges that leave a tile or wrap, united in global memory with atomicMin (union_find.cuh)
 //   ff_out_kernel      out = fill where the voxel's root is the seed's, else the input value
 #pragma once
 #include "common.cuh"
@@ -28,6 +28,7 @@
 #include "morton.cuh"
 #include "sort.cuh"
 #include "sparse_voxels.cuh"
+#include "union_find.cuh"
 
 namespace pcu {
 
@@ -322,7 +323,7 @@ __device__ __forceinline__ FfVoxel ff_voxel(const FfShape& s, const FfTile& t, i
 template <typename T>
 __device__ __forceinline__ bool ff_eq(const T* __restrict__ grid, long long o, T sv) { return __ldg(grid + o) == sv; }
 
-// Parents are read through volatile loads: other threads (other SMs, for P) change them while a union runs.
+// Parents are read through volatile loads: other threads change them while a union runs.
 __device__ __forceinline__ int ff_find_shared(const int* lab, int x) {
     const volatile int* l = lab;
     while (l[x] != x) x = l[x];
@@ -341,29 +342,6 @@ __device__ __forceinline__ void ff_union_shared(int* lab, int a, int b) {
         a = old;
     }
 }
-// Root of x with path halving: every store points a voxel at an ancestor, so concurrent unions keep their meaning.
-__device__ __forceinline__ int ff_find(int* P, int x) {
-    volatile int* q = P;
-    while (true) {
-        const int p = q[x];
-        if (p == x) return x;
-        const int gp = q[p];
-        if (gp != p) q[x] = gp;
-        x = gp;
-    }
-}
-__device__ __forceinline__ void ff_union(int* P, int a, int b) {
-    while (true) {
-        a = ff_find(P, a);
-        b = ff_find(P, b);
-        if (a == b) return;
-        if (a < b) { const int t = a; a = b; b = t; }
-        const int old = atomicMin(&P[a], b);
-        if (old == a) return;
-        a = old;
-    }
-}
-
 // Tile-local components of the voxels equal to the seed's value; P[o] = the tile root's linear index (o for the others).
 template <typename T>
 __global__ void __launch_bounds__(kThreads) ff_tile_kernel(const T* __restrict__ grid, const __grid_constant__ FfShape s, int* __restrict__ P) {
@@ -413,9 +391,9 @@ __global__ void __launch_bounds__(kThreads) ff_cross_kernel(const T* __restrict_
         const bool ey = (p.iy == (1 << s.ly) - 1 || p.y == s.h - 1) && p.o + s.d < s.n;
         const bool ex = p.ix == (1 << s.lx) - 1 && p.x + 1 < s.w;
         if (!(ez || ey || ex) || !ff_eq(grid, p.o, sv)) continue;
-        if (ez && ff_eq(grid, p.o + 1, sv)) ff_union(P, (int)p.o, (int)(p.o + 1));
-        if (ey && ff_eq(grid, p.o + s.d, sv)) ff_union(P, (int)p.o, (int)(p.o + s.d));
-        if (ex && ff_eq(grid, p.o + s.h * s.d, sv)) ff_union(P, (int)p.o, (int)(p.o + s.h * s.d));
+        if (ez && ff_eq(grid, p.o + 1, sv)) uf_union(P, (int)p.o, (int)(p.o + 1));
+        if (ey && ff_eq(grid, p.o + s.d, sv)) uf_union(P, (int)p.o, (int)(p.o + s.d));
+        if (ex && ff_eq(grid, p.o + s.h * s.d, sv)) uf_union(P, (int)p.o, (int)(p.o + s.h * s.d));
     }
 }
 
@@ -426,12 +404,12 @@ __global__ void __launch_bounds__(kThreads) ff_out_kernel(const T* __restrict__ 
                                                           int* __restrict__ P, T* __restrict__ out) {
     __shared__ int s_root;
     const T sv = __ldg(grid + seed);
-    if (threadIdx.x == 0) s_root = ff_find(P, (int)seed);
+    if (threadIdx.x == 0) s_root = uf_find(P, (int)seed);
     __syncthreads();
     const long long o = (long long)blockIdx.x * kThreads + threadIdx.x;
     if (o >= n) return;
     const T x = __ldg(grid + o);
-    out[o] = (x == sv && !(fill == sv) && ff_find(P, (int)o) == s_root) ? fill : x;
+    out[o] = (x == sv && !(fill == sv) && uf_find(P, (int)o) == s_root) ? fill : x;
 }
 
 }  // namespace pcu

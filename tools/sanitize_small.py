@@ -71,7 +71,12 @@ cb = np.arange(12 ** 3).reshape(12, 12, 12)[:-1, :-1, :-1].ravel()[:, None] + np
 step("marching cubes", lambda: pcu.marching_cubes_sparse_voxel_grid(np.linalg.norm(gc, axis=1) - 0.6, gc, cb, 0.0))
 step("marching cubes fp32 / uint32", lambda: pcu.marching_cubes_sparse_voxel_grid(
     (np.linalg.norm(gc, axis=1) - 0.6).astype(np.float32), gc.astype(np.float32), cb.astype(np.uint32), 0.0))
-step("sparse voxel grid boundary", lambda: pcu.sparse_voxel_grid_boundary(rng.integers(-10, 10, (n, 3)).astype(np.int32)))
+tf = np.concatenate([mf[:, :2], mf[:, :2] + 205, rng.integers(0, 60, (40, 2)) + 400])
+step("connected components", lambda: pcu.connected_components(mv, np.concatenate([mf, mf + 205])))
+step("connected components uint64 edges", lambda: pcu.connected_components(mv.astype(np.float32), tf.astype(np.uint64)))
+step("remove mesh vertices", lambda: pcu.remove_mesh_vertices(mv, mf, rng.random(200) < 0.7))
+step("remove unreferenced vertices fp32 / uint32", lambda: pcu.remove_unreferenced_mesh_vertices(mv.astype(np.float32), mf[:50].astype(np.uint32)))
+step("sparse voxel grid boundary",lambda: pcu.sparse_voxel_grid_boundary(rng.integers(-10, 10, (n, 3)).astype(np.int32)))
 pts_i = rng.integers(-1000, 1000, (n, 3)).astype(np.int32)
 codes = step("morton encode", lambda: pcu.morton_encode(pts_i))
 step("morton decode", lambda: pcu.morton_decode(codes))
