@@ -610,6 +610,39 @@ int pcu_b200_remove_unreferenced_mesh_vertices_f64(pcu_b200_workspace* ws, const
                                                    double* out_v, void* out_f, void* out_corr_v, void* out_corr_f, int64_t* out_count,
                                                    void* stream);
 
+/* ---- mesh normals, face areas and Laplacian smoothing ------------------------------------------------------------
+ * Replace mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals and laplacian_smooth_mesh (the
+ * reference's src/face_areas.cpp, src/mesh_normals.cpp, src/smooth.cpp).  Results defined in DESIGN.md §3.  v (nv, 3)
+ * in the suffix's type, f (nf, 3) of kind f_kind (pcu_b200_index_kind); 1 <= nv <= 2^31 - 2, 1 <= nf <= 357913941.
+ * A face with a corner outside [0, nv) fails with PCU_B200_INVALID_ARGUMENT (the outputs are written nonetheless).
+ *   mesh_face_areas: out_areas (nf), the reference's formula in v's precision.  Synchronises `stream` once.
+ *   mesh_face_normals: out_n (nf, 3), unit normals from fp64, 0 for a face of zero area.  Synchronises once.
+ *   mesh_vertex_normals: out_n (nv, 3); weighting 0 uniform, 1 area, 2 angle.  Synchronises once.
+ *   laplacian_smooth_mesh: out_v (nv, 3); num_iters >= 0 (0 copies v and does not synchronise).  out_cg_iters and
+ *     out_residual (host, num_iters entries) receive every step's conjugate-gradient iterations and its largest
+ *     |r| / |b| at exit (<= 1e-12 when it converged; a step stops after max_cg_iters iterations).  Synchronises once
+ *     after assembling the Laplacian, once per 16 CG iterations of every step and, with use_cotan_weights, once at the
+ *     end.  Non-finite coordinates and (use_cotan_weights) a total area of 0 fail with PCU_B200_INVALID_ARGUMENT.
+ * Every array pointer is a DEVICE pointer unless stated otherwise. */
+int pcu_b200_mesh_face_areas_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, float* out_areas,
+                                 void* stream);
+int pcu_b200_mesh_face_areas_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, double* out_areas,
+                                 void* stream);
+int pcu_b200_mesh_face_normals_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, float* out_n,
+                                   void* stream);
+int pcu_b200_mesh_face_normals_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, double* out_n,
+                                   void* stream);
+int pcu_b200_mesh_vertex_normals_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, int weighting,
+                                     float* out_n, void* stream);
+int pcu_b200_mesh_vertex_normals_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, int weighting,
+                                     double* out_n, void* stream);
+int pcu_b200_laplacian_smooth_mesh_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, int num_iters,
+                                       double step_size, int use_cotan_weights, int max_cg_iters, float* out_v, int32_t* out_cg_iters,
+                                       double* out_residual, void* stream);
+int pcu_b200_laplacian_smooth_mesh_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, int num_iters,
+                                       double step_size, int use_cotan_weights, int max_cg_iters, double* out_v, int32_t* out_cg_iters,
+                                       double* out_residual, void* stream);
+
 /* ---- voxel-grid down-sampling (SURVEY.md 8f, N2) --------------------------------------------
  * Replaces downsample_point_cloud_voxel_grid_internal (src/sample_point_cloud.cpp:336-367, :163-244): every point
  * goes to voxel int(floor((p - min_bound) / voxel_size)) per axis, computed in the cloud's precision exactly like the

@@ -47,6 +47,7 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "marching_cubes_sparse_voxel_grid", "sparse_voxel_grid_boundary",
            "voxelize_triangle_mesh", "flood_fill_3d",
            "connected_components", "remove_mesh_vertices", "remove_unreferenced_mesh_vertices",
+           "mesh_face_areas", "estimate_mesh_face_normals", "estimate_mesh_vertex_normals", "laplacian_smooth_mesh",
            "deduplicate_point_cloud",
            "deduplicate_mesh_vertices", "prepare_cloud", "pinned_empty", "PreparedCloud", "device_count",
            "current_device", "launch_count"]
@@ -784,6 +785,7 @@ from ._ray_surfel import ray_surfel_intersection, RaySurfelIntersector, pointclo
 from ._sparse_voxels import marching_cubes_sparse_voxel_grid, sparse_voxel_grid_boundary  # noqa: E402
 from ._voxels import voxelize_triangle_mesh, flood_fill_3d  # noqa: E402
 from ._mesh_topology import connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices  # noqa: E402
+from ._mesh_geometry import mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals, laplacian_smooth_mesh  # noqa: E402
 
 
 def _voxel_internal(points, attrib, voxel_size, min_bound, max_bound, min_points_per_voxel, device, return_counts=False):

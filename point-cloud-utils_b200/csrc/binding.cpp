@@ -797,6 +797,50 @@ int64_t remove_unreferenced_device(bool is_f64, uintptr_t v, int64_t nv, uintptr
     return kept;
 }
 
+// mesh_face_areas (normal false) / estimate_mesh_face_normals (normal true): out (nf) or (nf, 3) in v's type; one
+// synchronisation.
+void mesh_face_device(bool is_f64, bool normal, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out, int device,
+                      uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        if (normal)
+            return is_f64 ? pcu_b200_mesh_face_normals_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (double*)out, (void*)stream)
+                          : pcu_b200_mesh_face_normals_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (float*)out, (void*)stream);
+        return is_f64 ? pcu_b200_mesh_face_areas_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (double*)out, (void*)stream)
+                      : pcu_b200_mesh_face_areas_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (float*)out, (void*)stream);
+    });
+}
+// estimate_mesh_vertex_normals: out (nv, 3) in v's type; weighting 0 uniform, 1 area, 2 angle; one synchronisation.
+void mesh_vertex_normals_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int weighting, uintptr_t out,
+                                int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_mesh_vertex_normals_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, weighting, (double*)out,
+                                                         (void*)stream)
+                      : pcu_b200_mesh_vertex_normals_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, weighting, (float*)out,
+                                                         (void*)stream);
+    });
+}
+// laplacian_smooth_mesh: out (nv, 3) in v's type; returns (CG iterations of every step, largest relative residual of
+// every step).
+py::tuple laplacian_smooth_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int num_iters, double step_size,
+                                  bool use_cotan_weights, int max_cg_iters, uintptr_t out, int device, uintptr_t stream) {
+    std::vector<int32_t> iters((size_t)std::max(num_iters, 0));
+    std::vector<double> residual(iters.size());
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_laplacian_smooth_mesh_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, num_iters, step_size,
+                                                           use_cotan_weights, max_cg_iters, (double*)out, iters.data(), residual.data(),
+                                                           (void*)stream)
+                      : pcu_b200_laplacian_smooth_mesh_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, num_iters, step_size,
+                                                           use_cotan_weights, max_cg_iters, (float*)out, iters.data(), residual.data(),
+                                                           (void*)stream);
+    });
+    py::list it, res;
+    for (size_t i = 0; i < iters.size(); ++i) {
+        it.append(iters[i]);
+        res.append(residual[i]);
+    }
+    return py::make_tuple(it, res);
+}
+
 // out is float64 when bc or attribute is (numpy's promotion), else float32; out_bad: one device uint64.
 void interpolate_barycentric_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t fi, int64_t n, int fi_kind, uintptr_t bc,
                                     bool bc_f64, uintptr_t attr, bool attr_f64, int64_t nv, int64_t dim, uintptr_t out,
@@ -1214,6 +1258,9 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_connected_components_destroy", &connected_components_destroy);
     mod.def("_remove_mesh_vertices_device", &remove_mesh_vertices_device);
     mod.def("_remove_unreferenced_device", &remove_unreferenced_device);
+    mod.def("_mesh_face_device", &mesh_face_device);
+    mod.def("_mesh_vertex_normals_device", &mesh_vertex_normals_device);
+    mod.def("_laplacian_smooth_device", &laplacian_smooth_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),

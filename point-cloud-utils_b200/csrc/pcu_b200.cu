@@ -40,6 +40,7 @@
 #include "sparse_voxels.cuh"
 #include "voxelize.cuh"
 #include "mesh_topology.cuh"
+#include "laplacian.cuh"
 
 using namespace pcu;
 
@@ -2292,6 +2293,244 @@ int remove_unreferenced_device(pcu_b200_workspace* ws, const T* v, long long nv,
     return PCU_B200_OK;
 }
 
+// ---- mesh normals, face areas and Laplacian smoothing (mesh_geometry.cuh, laplacian.cuh) ---------------------------
+// Arguments shared by the four entry points.  6 m records must fit int32 positions.
+int mg_check(const pcu_b200_workspace* ws, const void* v, long long nv, const void* f, long long m, int fkind, const void* out) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!v || !f || !out) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (nv <= 0 || m <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid input mesh with zero elements");
+    if (nv >= 0x7fffffffLL || m > 0x7fffffffLL / 6)
+        return fail(PCU_B200_INVALID_ARGUMENT, "at most 2^31 - 2 vertices and 357913941 faces are supported, got %lld and %lld", nv, m);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    return PCU_B200_OK;
+}
+
+// CTAs of the kernels that reduce (reduce_grid): a function of the row count alone, so the sums' order is too.
+inline unsigned mg_blocks(long long n) { return std::min<unsigned>(kMgBlocks, blocks_for(n)); }
+
+// Bits of the largest vertex index n - 1 (at least 1).
+inline int mg_index_bits(long long n) {
+    int b = 1;
+    while (b < 31 && ((n - 1) >> b) != 0) ++b;
+    return b;
+}
+
+// Reads the record (one synchronisation) and fails on a corner out of range.
+int mg_read(const MgRecord* rec, MgRecord* host, cudaStream_t stream) {
+    PCU_CUDA(cudaMemcpyAsync(host, rec, sizeof(MgRecord), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    if (host->bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", host->bad);
+    return PCU_B200_OK;
+}
+
+// One face pass over v (T = the type of v; double for the smoothing's fp64 iterate).
+template <typename T>
+int mg_face_pass(const T* v, long long nv, const void* f, int fkind, long long m, const FaceOut<T>& out, MgRecord* rec, cudaStream_t stream) {
+    PCU_LAUNCH(mg_face_kernel<T>, mg_blocks(m), kThreads, stream, v, nv, f, fkind, m, out, rec);
+    return PCU_B200_OK;
+}
+
+// The corner CSR of the nv vertices: first (nv + 1) and corner (3 m), through the stable sort of the corner records
+// (sort: scratch for at least 3 m records).
+int enqueue_incidence(const SortScratch<MgRec>& sort, const void* f, int fkind, long long m, long long nv, int* first, int* corner,
+                      cudaStream_t stream) {
+    const long long n = 3 * m;
+    PCU_LAUNCH(mg_corner_kernel, blocks_for(n), kThreads, stream, f, fkind, n, nv, sort.a);
+    MgRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(sort, n, 1, stream, &sorted, mg_index_bits(nv)));
+    PCU_LAUNCH(mg_rows_kernel, blocks_for(n + 1), kThreads, stream, (const MgRec*)sorted, n, nv, first, corner, 0);
+    return PCU_B200_OK;
+}
+
+// mesh_face_areas (normal == false) or estimate_mesh_face_normals (normal == true): one face pass, one synchronisation.
+template <typename T>
+int mesh_face_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, bool normal, T* out,
+                     cudaStream_t stream) {
+    PCU_TRY(mg_check(ws, v, nv, f, m, fkind, out));
+    PCU_ON_DEVICE(ws);
+    MgRecord* rec = nullptr;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { rec = cv.take<MgRecord>(1); }));
+    PCU_CUDA(cudaMemsetAsync(rec, 0, sizeof(MgRecord), stream));
+    FaceOut<T> o = {};
+    if (normal) o.normal = out; else o.area = out;
+    PCU_TRY(mg_face_pass<T>(v, nv, f, fkind, m, o, rec, stream));
+    MgRecord host;
+    return mg_read(rec, &host, stream);
+}
+
+// estimate_mesh_vertex_normals, weighting 0 uniform, 1 area, 2 angle: face pass, corner CSR, vertex pass; one
+// synchronisation.
+template <typename T>
+int vertex_normals_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, int weighting, T* out,
+                          cudaStream_t stream) {
+    PCU_TRY(mg_check(ws, v, nv, f, m, fkind, out));
+    if (weighting < 0 || weighting > 2) return fail(PCU_B200_INVALID_ARGUMENT, "unknown weighting %d", weighting);
+    PCU_ON_DEVICE(ws);
+    struct { MgRecord* rec; double *unit, *weight; SortScratch<MgRec> sort; int *first, *corner; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.rec = cv.take<MgRecord>(1);
+        sc.unit = cv.take<double>(3 * (size_t)m);
+        sc.weight = weighting ? cv.take<double>(3 * (size_t)m) : nullptr;
+        sc.sort.carve(cv, 3 * m);
+        sc.first = cv.take<int>((size_t)nv + 1);
+        sc.corner = cv.take<int>(3 * (size_t)m);
+    }));
+    PCU_CUDA(cudaMemsetAsync(sc.rec, 0, sizeof(MgRecord), stream));
+    FaceOut<T> o = {};
+    o.unit = sc.unit;
+    o.weight = sc.weight;
+    o.weighting = weighting;
+    PCU_TRY(mg_face_pass<T>(v, nv, f, fkind, m, o, sc.rec, stream));
+    PCU_TRY(enqueue_incidence(sc.sort, f, fkind, m, nv, sc.first, sc.corner, stream));
+    PCU_LAUNCH(mg_vertex_normal_kernel<T>, blocks_for(nv), kThreads, stream, (const int*)sc.first, (const int*)sc.corner, nv,
+               (const double*)sc.unit, (const double*)sc.weight, out);
+    MgRecord host;
+    return mg_read(sc.rec, &host, stream);
+}
+
+constexpr int kCgWindow = 16;   // CG iterations enqueued between two reads of the solver's record
+
+// The buffers of one smoothing call.
+struct LapScratch {
+    LapRecord* rec;
+    double *u, *r, *z, *p, *q, *mass, *halfcot, *dbla, *partial, *val, *diag;
+    SortScratch<MgRec> sort;
+    MgRec* rows;
+    unsigned char *head, *lone;
+    unsigned* counts;
+    int *col, *rowptr, *first, *corner;
+    void carve(Carver& cv, long long nv, long long m, bool cotan) {
+        const size_t n3 = 3 * (size_t)nv, e = 6 * (size_t)m;
+        rec = cv.take<LapRecord>(1);
+        u = cv.take<double>(n3); r = cv.take<double>(n3); z = cv.take<double>(n3); p = cv.take<double>(n3); q = cv.take<double>(n3);
+        mass = cotan ? cv.take<double>((size_t)nv) : nullptr;
+        halfcot = cv.take<double>(3 * (size_t)m);
+        dbla = cotan ? cv.take<double>((size_t)m) : nullptr;
+        partial = cv.take<double>((size_t)kMgBlocks * 9);
+        sort.carve(cv, (long long)e);
+        rows = cv.take<MgRec>(e);
+        head = cv.take<unsigned char>(e);
+        counts = cv.take<unsigned>(keep_count_words((long long)e));
+        col = cv.take<int>(e);
+        val = cv.take<double>(e);
+        rowptr = cv.take<int>((size_t)nv + 1);
+        diag = cv.take<double>((size_t)nv);
+        lone = cv.take<unsigned char>((size_t)nv);
+        first = cotan ? cv.take<int>((size_t)nv + 1) : nullptr;
+        corner = cotan ? cv.take<int>(3 * (size_t)m) : nullptr;
+    }
+};
+
+// Reads the record (one synchronisation).
+int lap_read(const LapRecord* rec, LapRecord* host, cudaStream_t stream) {
+    PCU_CUDA(cudaMemcpyAsync(host, rec, sizeof(LapRecord), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    if (host->mesh.zero_area) return fail(PCU_B200_INVALID_ARGUMENT, "laplacian_smooth_mesh: the mesh has zero total area");
+    return PCU_B200_OK;
+}
+
+// The cotangent Laplacian of u in the scratch's CSR; reads the record once (corners, finiteness, entries).
+int lap_assemble(LapScratch& s, const void* f, int fkind, long long m, long long nv, bool cotan, cudaStream_t stream) {
+    const long long e = 6 * m;
+    const int bits = mg_index_bits(nv);
+    FaceOut<double> o = {};
+    o.halfcot = s.halfcot;
+    PCU_TRY(mg_face_pass<double>(s.u, nv, f, fkind, m, o, &s.rec->mesh, stream));
+    PCU_LAUNCH(lap_edge_kernel, blocks_for(m), kThreads, stream, f, fkind, m, nv, bits, s.sort.a);
+    MgRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(s.sort, e, 1, stream, &sorted, 2 * bits));
+    PCU_LAUNCH(mc_heads_kernel, blocks_for(e), kThreads, stream, (const McRec*)sorted, e, s.head);
+    PCU_TRY(enqueue_keep_offsets(s.head, e, s.counts, &s.rec->mesh.nnz, stream));
+    PCU_LAUNCH(lap_entries_kernel, blocks_for(e), kThreads, stream, (const MgRec*)sorted, e, (const unsigned char*)s.head,
+               (const unsigned*)s.counts, (const double*)s.halfcot, bits, s.rows, s.col, s.val);
+    if (cotan) PCU_TRY(enqueue_incidence(s.sort, f, fkind, m, nv, s.first, s.corner, stream));
+    LapRecord host;
+    PCU_TRY(lap_read(s.rec, &host, stream));
+    if (host.mesh.bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", host.mesh.bad);
+    if (host.mesh.nonfinite)
+        return fail(PCU_B200_INVALID_ARGUMENT, "laplacian_smooth_mesh: v has %llu coordinates that are not finite", host.mesh.nonfinite);
+    PCU_LAUNCH(mg_rows_kernel, blocks_for(host.mesh.nnz + 1), kThreads, stream, (const MgRec*)s.rows, host.mesh.nnz, nv, s.rowptr,
+               (int*)nullptr, 0);
+    PCU_LAUNCH(lap_diag_kernel, blocks_for(nv), kThreads, stream, (const int*)s.rowptr, (const double*)s.val, nv, s.diag, s.lone);
+    return PCU_B200_OK;
+}
+
+// One CG solve of S u' = M u in place; reads the record once per window of kCgWindow iterations.  Returns the
+// iterations and the largest |r| / |b| of the three columns at exit.
+int lap_solve(const LapScratch& s, const LapSystem& sys, int max_iters, int* out_iters, double* out_residual, cudaStream_t stream) {
+    const long long n = sys.n;
+    const unsigned blocks = mg_blocks(n);
+    PCU_CUDA(cudaMemsetAsync(&s.rec->cg, 0, sizeof(CgState), stream));
+    PCU_LAUNCH(lap_cg_init_kernel, blocks, kThreads, stream, sys, (const double*)s.u, s.r, s.z, s.p, s.partial, s.rec);
+    LapRecord host;
+    for (;;) {
+        for (int k = 0; k < kCgWindow; ++k) {
+            PCU_LAUNCH(lap_cg_spmv_kernel, blocks, kThreads, stream, sys, (const double*)s.p, s.q, s.partial, s.rec);
+            PCU_LAUNCH(lap_cg_update_kernel, blocks, kThreads, stream, sys, s.u, s.r, s.z, (const double*)s.p, (const double*)s.q, s.partial,
+                       max_iters, s.rec);
+            PCU_LAUNCH(lap_cg_direction_kernel, blocks_for(3 * n), kThreads, stream, n, (const double*)s.z, s.p, (const LapRecord*)s.rec);
+        }
+        PCU_TRY(lap_read(s.rec, &host, stream));
+        if (host.cg.done) break;
+    }
+    double worst = 0.0;
+    for (int c = 0; c < 3; ++c) {
+        const double rr = host.cg.rr[c], bb = host.cg.bb[c];
+        const double rel = bb > 0.0 ? std::sqrt(rr / bb) : (rr > 0.0 ? HUGE_VAL : 0.0);
+        worst = std::max(worst, rel);
+    }
+    *out_iters = host.cg.iters;
+    *out_residual = worst;
+    return PCU_B200_OK;
+}
+
+// laplacian_smooth_mesh (src/smooth.cpp): out_iters / out_residual (host, num_iters entries) receive every step's CG
+// iterations and its largest relative residual at exit.
+template <typename T>
+int laplacian_smooth_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, int num_iters,
+                            double step_size, bool cotan, int max_cg_iters, T* out, int* out_iters, double* out_residual, cudaStream_t stream) {
+    PCU_TRY(mg_check(ws, v, nv, f, m, fkind, out));
+    if (num_iters < 0)
+        return fail(PCU_B200_INVALID_ARGUMENT, "Invalid value for argument num_iters in smooth_mesh_laplacian. Must be a positive integer or 0.");
+    if (max_cg_iters <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "max_cg_iters must be positive, got %d", max_cg_iters);
+    if (num_iters > 0 && (!out_iters || !out_residual)) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    PCU_ON_DEVICE(ws);
+    if (num_iters == 0) {
+        PCU_TRY(adopt_stream(ws, stream));
+        PCU_CUDA(cudaMemcpyAsync(out, v, 3 * (size_t)nv * sizeof(T), cudaMemcpyDeviceToDevice, stream));
+        return PCU_B200_OK;
+    }
+    LapScratch s;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { s.carve(cv, nv, m, cotan); }));
+    PCU_CUDA(cudaMemsetAsync(s.rec, 0, sizeof(LapRecord), stream));
+    PCU_LAUNCH(lap_load_kernel<T>, blocks_for(3 * nv), kThreads, stream, v, 3 * nv, s.u, &s.rec->mesh);
+    PCU_TRY(lap_assemble(s, f, fkind, m, nv, cotan, stream));
+    const LapSystem sys = {s.rowptr, s.col, s.val, s.diag, s.mass, cotan ? step_size * 1e-3 : step_size, nv};
+    for (int it = 0; it < num_iters; ++it) {
+        if (cotan) {
+            FaceOut<double> o = {};
+            o.dbla = s.dbla;
+            o.partial = s.partial;
+            PCU_TRY(mg_face_pass<double>(s.u, nv, f, fkind, m, o, &s.rec->mesh, stream));
+            PCU_LAUNCH(lap_mass_kernel, blocks_for(nv), kThreads, stream, (const int*)s.first, (const int*)s.corner, nv, (const double*)s.dbla,
+                       (const unsigned char*)s.lone, s.mass);
+        }
+        PCU_TRY(lap_solve(s, sys, max_cg_iters, out_iters + it, out_residual + it, stream));
+        if (cotan) {
+            FaceOut<double> o = {};
+            o.partial = s.partial;
+            PCU_TRY(mg_face_pass<double>(s.u, nv, f, fkind, m, o, &s.rec->mesh, stream));
+            PCU_LAUNCH(lap_rescale_kernel, blocks_for(3 * nv), kThreads, stream, s.u, nv, (const MgRecord*)&s.rec->mesh);
+        }
+    }
+    PCU_LAUNCH(lap_store_kernel<T>, blocks_for(3 * nv), kThreads, stream, (const double*)s.u, 3 * nv, out);
+    if (cotan) {
+        LapRecord host;
+        PCU_TRY(lap_read(s.rec, &host, stream));
+    }
+    return PCU_B200_OK;
+}
+
 // ---- Morton codes (SURVEY.md 8f N3) -------------------------------------------------------------------
 
 template <typename I>
@@ -3167,6 +3406,43 @@ int pcu_b200_remove_unreferenced_mesh_vertices_f64(pcu_b200_workspace* ws, const
                                                    void* stream) {
     return remove_unreferenced_device<double>(ws, v, nv, f, nf, f_kind, out_v, out_f, out_corr_v, out_corr_f, (long long*)out_count,
                                               (cudaStream_t)stream);
+}
+
+int pcu_b200_mesh_face_areas_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, float* out_areas,
+                                 void* stream) {
+    return mesh_face_device<float>(ws, v, nv, f, nf, f_kind, false, out_areas, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_face_areas_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, double* out_areas,
+                                 void* stream) {
+    return mesh_face_device<double>(ws, v, nv, f, nf, f_kind, false, out_areas, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_face_normals_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, float* out_n,
+                                   void* stream) {
+    return mesh_face_device<float>(ws, v, nv, f, nf, f_kind, true, out_n, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_face_normals_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, double* out_n,
+                                   void* stream) {
+    return mesh_face_device<double>(ws, v, nv, f, nf, f_kind, true, out_n, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_vertex_normals_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, int weighting,
+                                     float* out_n, void* stream) {
+    return vertex_normals_device<float>(ws, v, nv, f, nf, f_kind, weighting, out_n, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_vertex_normals_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, int weighting,
+                                     double* out_n, void* stream) {
+    return vertex_normals_device<double>(ws, v, nv, f, nf, f_kind, weighting, out_n, (cudaStream_t)stream);
+}
+int pcu_b200_laplacian_smooth_mesh_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, int num_iters,
+                                       double step_size, int use_cotan_weights, int max_cg_iters, float* out_v, int32_t* out_cg_iters,
+                                       double* out_residual, void* stream) {
+    return laplacian_smooth_device<float>(ws, v, nv, f, nf, f_kind, num_iters, step_size, use_cotan_weights != 0, max_cg_iters, out_v,
+                                          out_cg_iters, out_residual, (cudaStream_t)stream);
+}
+int pcu_b200_laplacian_smooth_mesh_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, int num_iters,
+                                       double step_size, int use_cotan_weights, int max_cg_iters, double* out_v, int32_t* out_cg_iters,
+                                       double* out_residual, void* stream) {
+    return laplacian_smooth_device<double>(ws, v, nv, f, nf, f_kind, num_iters, step_size, use_cotan_weights != 0, max_cg_iters, out_v,
+                                           out_cg_iters, out_residual, (cudaStream_t)stream);
 }
 
 int pcu_b200_deduplicate_f32(pcu_b200_workspace* ws, const float* points, int64_t n, double epsilon, const void* faces, int64_t n_faces,

@@ -76,6 +76,12 @@ step("connected components", lambda: pcu.connected_components(mv, np.concatenate
 step("connected components uint64 edges", lambda: pcu.connected_components(mv.astype(np.float32), tf.astype(np.uint64)))
 step("remove mesh vertices", lambda: pcu.remove_mesh_vertices(mv, mf, rng.random(200) < 0.7))
 step("remove unreferenced vertices fp32 / uint32", lambda: pcu.remove_unreferenced_mesh_vertices(mv.astype(np.float32), mf[:50].astype(np.uint32)))
+step("mesh face areas", lambda: pcu.mesh_face_areas(mv, mf))
+step("face normals fp32 / uint32", lambda: pcu.estimate_mesh_face_normals(mv.astype(np.float32), mf.astype(np.uint32)))
+step("vertex normals area", lambda: pcu.estimate_mesh_vertex_normals(mv, mf, "area"))
+step("vertex normals angle fp32", lambda: pcu.estimate_mesh_vertex_normals(mv.astype(np.float32), mf.astype(np.int32), "angle"))
+step("laplacian smoothing", lambda: pcu.laplacian_smooth_mesh(mv, mf, 2))
+step("laplacian smoothing cotan fp32", lambda: pcu.laplacian_smooth_mesh(mv.astype(np.float32), mf.astype(np.int32), 2, use_cotan_weights=True))
 step("sparse voxel grid boundary",lambda: pcu.sparse_voxel_grid_boundary(rng.integers(-10, 10, (n, 3)).astype(np.int32)))
 pts_i = rng.integers(-1000, 1000, (n, 3)).astype(np.int32)
 codes = step("morton encode", lambda: pcu.morton_encode(pts_i))
