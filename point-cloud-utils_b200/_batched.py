@@ -8,11 +8,7 @@ all-gather of the per-pair values when the caller wants them all.
 import numpy as _np
 
 from . import _pcu_internal
-
-
-def _torch():
-    import importlib
-    return importlib.import_module("torch")
+from ._call import _torch
 
 
 def batched_chamfer(x, y, max_points_per_leaf=10, return_sum=False, device=-1):

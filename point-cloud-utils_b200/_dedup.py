@@ -6,15 +6,7 @@ tensors in -> CUDA tensors out.  float32 / float64 points, int32 / int64 faces."
 import numpy as _np
 
 from . import _pcu_internal
-
-
-def _torch():
-    import importlib
-    return importlib.import_module("torch")
-
-
-def _is_tensor(x):
-    return type(x).__module__.startswith("torch")
+from ._call import _is_tensor, _torch
 
 
 def _run(points, faces, epsilon, device, pname, fname):

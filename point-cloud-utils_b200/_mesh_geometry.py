@@ -9,7 +9,7 @@ device call.  Shapes are the reference's through npe::move, which squeezes them 
 import warnings
 
 from . import _pcu_internal
-from ._mesh_sampling import _INDEX_KINDS, _call_args, _dtype_name, _form, _torch, _upload, _validate_mesh
+from ._call import _INDEX_KINDS, _dtype_name, _form, _run, _torch, _validate_mesh
 
 _SIGNED_KINDS = {"int32": 0, "int64": 1}
 _MAX_VERTICES = 2 ** 31 - 2
@@ -26,24 +26,18 @@ def _check_size(name, v, f):
     return nvert, nface
 
 
-def _back(form, out):
-    """The output squeezed as npe::move squeezes it; numpy when the inputs were."""
-    out = out.squeeze()
-    return out.cpu().numpy() if form == "numpy" else out
-
-
 def _face_pass(v, f, normal, device):
     form = _form([v, f], ["v", "f"])
     nvert, nface = _check_size("estimate_mesh_face_normals" if normal else "mesh_face_areas", v, f)
     torch = _torch()
-    if form == "cpu":
-        return torch.from_numpy(_face_pass(v.detach().numpy(), f.detach().numpy(), normal, device))
-    vt, ft = _upload(form, [v, f], device)
-    dev, stream = _call_args(vt)
-    out = torch.empty((nface, 3) if normal else (nface,), dtype=vt.dtype, device=vt.device)
-    _pcu_internal._mesh_face_device(vt.dtype == torch.float64, normal, vt.data_ptr(), nvert, ft.data_ptr(), nface,
-                                    _INDEX_KINDS[_dtype_name(f)], out.data_ptr(), dev, stream)
-    return _back(form, out)
+
+    def body(vt, ft, dev, stream):
+        out = torch.empty((nface, 3) if normal else (nface,), dtype=vt.dtype, device=vt.device)
+        _pcu_internal._mesh_face_device(vt.dtype == torch.float64, normal, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                        _INDEX_KINDS[_dtype_name(f)], out.data_ptr(), dev, stream)
+        return out
+
+    return _run(form, [v, f], device, body, squeeze=True)
 
 
 def mesh_face_areas(v, f, num_threads=-1, *, device=None):
@@ -119,14 +113,14 @@ def estimate_mesh_vertex_normals(v, f, weighting_type="uniform", *, device=None)
         raise ValueError("Invalid weighting_type must be one of 'uniform', 'angle', or 'area', but got '%s'" % (weighting_type,))
     nvert, nface = _check_size("estimate_mesh_vertex_normals", v, f)
     torch = _torch()
-    if form == "cpu":
-        return torch.from_numpy(estimate_mesh_vertex_normals(v.detach().numpy(), f.detach().numpy(), weighting_type, device=device))
-    vt, ft = _upload(form, [v, f], device)
-    dev, stream = _call_args(vt)
-    out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
-    _pcu_internal._mesh_vertex_normals_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
-                                              _INDEX_KINDS[_dtype_name(f)], _WEIGHTINGS[weighting_type], out.data_ptr(), dev, stream)
-    return _back(form, out)
+
+    def body(vt, ft, dev, stream):
+        out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
+        _pcu_internal._mesh_vertex_normals_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                                  _INDEX_KINDS[_dtype_name(f)], _WEIGHTINGS[weighting_type], out.data_ptr(), dev, stream)
+        return out
+
+    return _run(form, [v, f], device, body, squeeze=True)
 
 
 def _smooth(v, f, num_iters, step_size, use_cotan_weights, device):
@@ -140,21 +134,23 @@ def _smooth(v, f, num_iters, step_size, use_cotan_weights, device):
     torch = _torch()
     if num_iters == 0:
         return (v.copy() if form == "numpy" else v.detach().clone()).squeeze(), []
-    if form == "cpu":
-        out, iters = _smooth(v.detach().numpy(), f.detach().numpy(), num_iters, step_size, use_cotan_weights, device)
-        return torch.from_numpy(out), iters
-    vt, ft = _upload(form, [v, f], device)
-    dev, stream = _call_args(vt)
-    out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
-    iters, residual = _pcu_internal._laplacian_smooth_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
-                                                             _INDEX_KINDS[_dtype_name(f)], num_iters, float(step_size),
-                                                             bool(use_cotan_weights), int(_CG_MAX_ITERS), out.data_ptr(), dev, stream)
+    iters = residual = None
+
+    def body(vt, ft, dev, stream):
+        nonlocal iters, residual
+        out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
+        iters, residual = _pcu_internal._laplacian_smooth_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                                                 _INDEX_KINDS[_dtype_name(f)], num_iters, float(step_size),
+                                                                 bool(use_cotan_weights), int(_CG_MAX_ITERS), out.data_ptr(), dev, stream)
+        return out
+
+    out = _run(form, [v, f], device, body, squeeze=True)
     for step, (k, res) in enumerate(zip(iters, residual)):
         if not res <= _CG_TOL:
             warnings.warn("laplacian_smooth_mesh: the solve of step %d stopped after %d conjugate-gradient iterations at a relative "
                           "residual of %.3g (tolerance %g); its iterate is returned" % (step, k, res, _CG_TOL), RuntimeWarning,
                           stacklevel=3)
-    return _back(form, out), iters
+    return out, iters
 
 
 def laplacian_smooth_mesh(v, f, num_iters, step_size=0.1, use_cotan_weights=False, *, device=None):

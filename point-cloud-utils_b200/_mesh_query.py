@@ -2,11 +2,10 @@
 -- the reference's names, arguments and outputs (the reference's src/closest_point_on_mesh.cpp,
 src/fast_winding_numbers.cpp and src/signed_distance.cpp), computed by csrc/meshquery.cuh and csrc/winding.cuh.
 
-Input forms and validation follow _mesh_sampling.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
+Input forms and validation follow _call.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
 from . import _pcu_internal
-from ._mesh_sampling import (_INDEX_KINDS, _back, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form,
-                             _raise_bad, _torch, _upload, _validate_mesh)
+from ._call import _INDEX_KINDS, _check_float, _check_index, _check_match, _dtype_name, _form, _raise_bad, _run, _torch, _validate_mesh
 
 
 def _validate_points(p, v, f):
@@ -50,30 +49,28 @@ def closest_points_on_mesh(p, v, f, *, device=None):
     _validate_points(p, v, f)
     _validate_mesh(v, f, ("int32", "int64", "uint32", "uint64"))
     torch = _torch()
-    if form == "cpu":
-        out = closest_points_on_mesh(p.detach().numpy(), v.detach().numpy(), f.detach().numpy(), device=device)
-        return tuple(torch.from_numpy(o) for o in out)
     n = int(p.shape[0])
     if n == 0:
         if form == "numpy":
             import numpy as np
             return np.zeros(0, dtype=p.dtype), np.zeros(0, dtype=f.dtype), np.zeros((0, 3), dtype=p.dtype)
-        _same_device(p, device)
+        if form == "cuda":
+            _same_device(p, device)
         return (torch.zeros(0, dtype=p.dtype, device=p.device), torch.zeros(0, dtype=f.dtype, device=p.device),
                 torch.zeros((0, 3), dtype=p.dtype, device=p.device))
-    pt, vt, ft = _upload(form, [p, v, f], device)
-    dev, stream = _call_args(pt)
-    d = torch.empty(n, dtype=pt.dtype, device=pt.device)
-    fidx = torch.empty(n, dtype=ft.dtype, device=pt.device)
-    bc = torch.empty((n, 3), dtype=pt.dtype, device=pt.device)
-    bad = torch.empty(1, dtype=torch.int64, device=pt.device)
-    _pcu_internal._closest_points_on_mesh_device(pt.dtype == torch.float64, pt.data_ptr(), n, vt.data_ptr(), int(vt.shape[0]),
-                                                 ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], d.data_ptr(),
-                                                 fidx.data_ptr(), bc.data_ptr(), bad.data_ptr(), dev, stream)
-    _raise_bad(bad)
-    if form == "numpy":
-        return (d.cpu().numpy(),) + _back(fidx, bc, f, form)
-    return d, fidx, bc
+
+    def body(pt, vt, ft, dev, stream):
+        d = torch.empty(n, dtype=pt.dtype, device=pt.device)
+        fidx = torch.empty(n, dtype=ft.dtype, device=pt.device)
+        bc = torch.empty((n, 3), dtype=pt.dtype, device=pt.device)
+        bad = torch.empty(1, dtype=torch.int64, device=pt.device)
+        _pcu_internal._closest_points_on_mesh_device(pt.dtype == torch.float64, pt.data_ptr(), n, vt.data_ptr(), int(vt.shape[0]),
+                                                     ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], d.data_ptr(),
+                                                     fidx.data_ptr(), bc.data_ptr(), bad.data_ptr(), dev, stream)
+        _raise_bad(bad)
+        return d, fidx, bc
+
+    return _run(form, [p, v, f], device, body, index=(f, [1]))
 
 
 def _validate_nonempty_points(p):
@@ -115,19 +112,18 @@ def triangle_soup_fast_winding_number(v, f, p, *, device=None):
     _validate_mesh(v, f, tuple(_INDEX_KINDS))
     _validate_nonempty_points(p)
     torch = _torch()
-    if form == "cpu":
-        return torch.from_numpy(triangle_soup_fast_winding_number(v.detach().numpy(), f.detach().numpy(), p.detach().numpy(),
-                                                                  device=device))
-    vt, ft, pt = _upload(form, [v, f, p], device)
-    n = int(pt.shape[0])
-    dev, stream = _call_args(pt)
-    w = torch.empty(n, dtype=pt.dtype, device=pt.device)
-    bad = torch.empty(1, dtype=torch.int64, device=pt.device)
-    _pcu_internal._fast_winding_number_device(pt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
-                                              int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], pt.data_ptr(), n, 2.0, w.data_ptr(),
-                                              bad.data_ptr(), dev, stream)
-    _raise_bad(bad)
-    return w.cpu().numpy() if form == "numpy" else w
+
+    def body(vt, ft, pt, dev, stream):
+        n = int(pt.shape[0])
+        w = torch.empty(n, dtype=pt.dtype, device=pt.device)
+        bad = torch.empty(1, dtype=torch.int64, device=pt.device)
+        _pcu_internal._fast_winding_number_device(pt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
+                                                  int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], pt.data_ptr(), n, 2.0, w.data_ptr(),
+                                                  bad.data_ptr(), dev, stream)
+        _raise_bad(bad)
+        return w
+
+    return _run(form, [v, f, p], device, body)
 
 
 def _validate_point_cloud_normals(p, n):
@@ -180,16 +176,15 @@ def point_cloud_fast_winding_number(p, n, a, q, *, device=None):
         raise ValueError("Invalid shape for areas: a must have #p = %d elements, e.g. shape (#p,) or (#p, 1). Got a.shape =%s."
                          % (int(p.shape[0]), tuple(a.shape)))
     torch = _torch()
-    if form == "cpu":
-        return torch.from_numpy(point_cloud_fast_winding_number(p.detach().numpy(), n.detach().numpy(), a.detach().numpy(),
-                                                                q.detach().numpy(), device=device))
-    pt, nt, at, qt = _upload(form, [p, n, a, q], device)
-    m, nq = int(pt.shape[0]), int(qt.shape[0])
-    dev, stream = _call_args(qt)
-    w = torch.empty(nq, dtype=qt.dtype, device=qt.device)
-    _pcu_internal._point_cloud_fast_winding_number_device(qt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), at.data_ptr(), m,
-                                                          qt.data_ptr(), nq, 2.0, w.data_ptr(), dev, stream)
-    return w.cpu().numpy() if form == "numpy" else w
+
+    def body(pt, nt, at, qt, dev, stream):
+        m, nq = int(pt.shape[0]), int(qt.shape[0])
+        w = torch.empty(nq, dtype=qt.dtype, device=qt.device)
+        _pcu_internal._point_cloud_fast_winding_number_device(qt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), at.data_ptr(), m,
+                                                              qt.data_ptr(), nq, 2.0, w.data_ptr(), dev, stream)
+        return w
+
+    return _run(form, [p, n, a, q], device, body)
 
 
 def signed_distance_to_mesh(p, v, f, lower_bound=-float("inf"), upper_bound=float("inf"), *, device=None):
@@ -227,20 +222,17 @@ def signed_distance_to_mesh(p, v, f, lower_bound=-float("inf"), upper_bound=floa
     _validate_nonempty_points(p)
     lower, upper = float(np.float32(lower_bound)), float(np.float32(upper_bound))
     torch = _torch()
-    if form == "cpu":
-        out = signed_distance_to_mesh(p.detach().numpy(), v.detach().numpy(), f.detach().numpy(), lower, upper, device=device)
-        return tuple(torch.from_numpy(o) for o in out)
-    pt, vt, ft = _upload(form, [p, v, f], device)
-    n = int(pt.shape[0])
-    dev, stream = _call_args(pt)
-    s = torch.empty(n, dtype=pt.dtype, device=pt.device)
-    fidx = torch.empty(n, dtype=torch.int32, device=pt.device)
-    bc = torch.empty((n, 3), dtype=pt.dtype, device=pt.device)
-    bad = torch.empty(1, dtype=torch.int64, device=pt.device)
-    _pcu_internal._signed_distance_to_mesh_device(pt.dtype == torch.float64, pt.data_ptr(), n, vt.data_ptr(), int(vt.shape[0]),
-                                                  ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], lower, upper,
-                                                  s.data_ptr(), fidx.data_ptr(), bc.data_ptr(), bad.data_ptr(), dev, stream)
-    _raise_bad(bad)
-    if form == "numpy":
-        return s.cpu().numpy(), fidx.cpu().numpy(), bc.cpu().numpy()
-    return s, fidx, bc
+
+    def body(pt, vt, ft, dev, stream):
+        n = int(pt.shape[0])
+        s = torch.empty(n, dtype=pt.dtype, device=pt.device)
+        fidx = torch.empty(n, dtype=torch.int32, device=pt.device)
+        bc = torch.empty((n, 3), dtype=pt.dtype, device=pt.device)
+        bad = torch.empty(1, dtype=torch.int64, device=pt.device)
+        _pcu_internal._signed_distance_to_mesh_device(pt.dtype == torch.float64, pt.data_ptr(), n, vt.data_ptr(), int(vt.shape[0]),
+                                                      ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)], lower, upper,
+                                                      s.data_ptr(), fidx.data_ptr(), bc.data_ptr(), bad.data_ptr(), dev, stream)
+        _raise_bad(bad)
+        return s, fidx, bc
+
+    return _run(form, [p, v, f], device, body)

@@ -9,109 +9,13 @@ import math
 import numpy as _np
 
 from . import _pcu_internal
-
-_INDEX_KINDS = {"int32": 0, "int64": 1, "uint32": 2, "uint64": 3}
-
-
-def _torch():
-    import importlib
-    return importlib.import_module("torch")
-
-
-def _is_tensor(x):
-    return type(x).__module__.startswith("torch")
-
-
-def _dtype_name(x):
-    return str(x.dtype).replace("torch.", "")
+from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _raise_bad, _run, _torch, _validate_mesh
 
 
 def _seed(random_seed):
     """A 32-bit seed; 0 draws one from NumPy's global random state (the reference uses the time)."""
     seed = int(random_seed) & 0xFFFFFFFF
     return int(_np.random.randint(2 ** 31 - 1)) if seed == 0 else seed
-
-
-def _form(arrays, names):
-    """'numpy', 'cuda' or 'cpu' (CPU tensors) for a set of inputs that must all be of one form."""
-    tensors = [_is_tensor(a) for a in arrays]
-    if all(tensors):
-        cuda = [a.is_cuda for a in arrays]
-        if all(cuda):
-            if len({a.device for a in arrays}) != 1:
-                raise ValueError("%s must live on one device" % ", ".join(names))
-            return "cuda"
-        if not any(cuda):
-            return "cpu"
-        raise ValueError("%s must all be CUDA tensors or all CPU tensors" % ", ".join(names))
-    for a, name in zip(arrays, names):
-        if type(a) != _np.ndarray:
-            raise ValueError("Invalid type for %s, must be a NumPy array, but got %s." % (name, type(a)))
-    return "numpy"
-
-
-def _check_float(x, name):
-    if _dtype_name(x) not in ("float32", "float64"):
-        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of ['float32', 'float64']." % (_dtype_name(x), name))
-
-
-def _check_index(x, name, kinds):
-    if _dtype_name(x) not in kinds:
-        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of %s." % (_dtype_name(x), name, list(kinds)))
-
-
-def _check_match(x, name, ref, ref_name):
-    if _dtype_name(x) != _dtype_name(ref):
-        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected it to match argument '%s' which is of type %s."
-                         % (_dtype_name(x), name, ref_name, _dtype_name(ref)))
-
-
-def _validate_mesh(v, f, face_dtypes):
-    """The binding's dtype checks, then validate_mesh (src/common/common.h:131-148)."""
-    _check_float(v, "v")
-    _check_index(f, "f", face_dtypes)
-    vs, fs = tuple(v.shape), tuple(f.shape)
-    if len(vs) != 2 or len(fs) != 2:
-        raise ValueError("Only 3D inputs are supported: v and f must have shape (n, 3) and (m, 3) (n, m > 0). Got v.shape ="
-                         "%s, f.shape = %s." % (vs, fs))
-    if vs[0] == 0 or fs[0] == 0:
-        raise ValueError("Invalid input mesh with zero elements: v and f must have shape (n, 3) and (m, 3) (n, m > 0). Got "
-                         "v.shape =%s, f.shape = %s." % (vs, fs))
-    if vs[1] != 3 or fs[1] != 3:
-        raise ValueError("Only 3D inputs are supported: v and f must have shape (n, 3) and (m, 3) (n, m > 0). Got v.shape ="
-                         "%s, f.shape = %s." % (vs, fs))
-
-
-def _to_device(arrays, device):
-    """numpy arrays -> contiguous CUDA tensors on the device= of the call (one upload each).  Unsigned index arrays
-    travel as the signed type of their width (the kernels take the kind separately)."""
-    from . import _dev
-    torch = _torch()
-    dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
-    signed = {"uint32": _np.int32, "uint64": _np.int64}
-    return [torch.from_numpy(_np.ascontiguousarray(a).view(signed.get(a.dtype.name, a.dtype))).to(torch.device("cuda", dev))
-            for a in arrays]
-
-
-def _upload(form, arrays, device):
-    """Contiguous CUDA tensors of the inputs, on the device of the call."""
-    from . import _same_device
-    if form == "cuda":
-        _same_device(arrays[0], device)
-        return [a.detach().contiguous() for a in arrays]
-    return _to_device(arrays, device)
-
-
-def _call_args(t):
-    torch = _torch()
-    return t.device.index or 0, torch.cuda.current_stream(t.device).cuda_stream
-
-
-def _raise_bad(bad):
-    """Raises for a count (a device tensor or a host scalar) of faces with a corner out of range."""
-    nbad = int(bad.item())
-    if nbad:
-        raise ValueError("Invalid face indices: %d faces have a corner outside [0, #v)" % nbad)
 
 
 def _read_area(area):
@@ -123,10 +27,6 @@ def _read_area(area):
     if W == 0:
         raise ValueError("Mesh has zero area")
     return W, S
-
-
-def _back(fidx, bc, f, form):
-    return (fidx.cpu().numpy().view(f.dtype), bc.cpu().numpy()) if form == "numpy" else (fidx, bc)
 
 
 def sample_mesh_random(v, f, num_samples, random_seed=0, *, device=None):
@@ -159,20 +59,19 @@ def sample_mesh_random(v, f, num_samples, random_seed=0, *, device=None):
     n = int(num_samples)
     seed = _seed(random_seed)
     torch = _torch()
-    if form == "cpu":
-        out = sample_mesh_random(v.detach().numpy(), f.detach().numpy(), n, seed, device=device)
-        return tuple(torch.from_numpy(o) for o in out)
-    vt, ft = _upload(form, [v, f], device)
-    dev, stream = _call_args(vt)
-    kind = _INDEX_KINDS[_dtype_name(f)]
-    fidx = torch.empty(n, dtype=ft.dtype, device=vt.device)
-    bc = torch.empty((n, 3), dtype=vt.dtype, device=vt.device)
-    area = torch.empty(3, dtype=torch.int64, device=vt.device)
-    _pcu_internal._sample_mesh_random_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
-                                             int(ft.shape[0]), kind, n, seed, fidx.data_ptr(),
-                                             bc.data_ptr(), area.data_ptr(), dev, stream)
-    _read_area(area)
-    return _back(fidx, bc, f, form)
+
+    def body(vt, ft, dev, stream):
+        kind = _INDEX_KINDS[_dtype_name(f)]
+        fidx = torch.empty(n, dtype=ft.dtype, device=vt.device)
+        bc = torch.empty((n, 3), dtype=vt.dtype, device=vt.device)
+        area = torch.empty(3, dtype=torch.int64, device=vt.device)
+        _pcu_internal._sample_mesh_random_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),
+                                                 int(ft.shape[0]), kind, n, seed, fidx.data_ptr(),
+                                                 bc.data_ptr(), area.data_ptr(), dev, stream)
+        _read_area(area)
+        return fidx, bc
+
+    return _run(form, [v, f], device, body, index=(f, [0]))
 
 
 def dense_plan(W, S, num_samples, radius, oversampling_factor):
@@ -233,24 +132,22 @@ def sample_mesh_poisson_disk(v, f, num_samples, radius=0.0, use_geodesic_distanc
         raise ValueError("oversampling_factor must be >= 1.0 (got %r)" % (oversampling_factor,))
     seed = _seed(random_seed)
     torch = _torch()
-    if form == "cpu":
-        out = sample_mesh_poisson_disk(v.detach().numpy(), f.detach().numpy(), num_samples, radius, use_geodesic_distance,
-                                       best_choice_sampling, seed, sample_num_tolerance, oversampling_factor, device=device)
-        return tuple(torch.from_numpy(o) for o in out)
-    vt, ft = _upload(form, [v, f], device)
-    dev, stream = _call_args(vt)
-    is_f64, nv, nf, kind = vt.dtype == torch.float64, int(vt.shape[0]), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)]
-    area = torch.empty(3, dtype=torch.int64, device=vt.device)
-    _pcu_internal._mesh_area_device(is_f64, vt.data_ptr(), nv, ft.data_ptr(), nf, kind, area.data_ptr(), dev, stream)
-    W, S = _read_area(area)
-    r, n_dense = dense_plan(W, S, num_samples, radius, osf)
-    fidx = torch.empty(n_dense, dtype=ft.dtype, device=vt.device)
-    bc = torch.empty((n_dense, 3), dtype=vt.dtype, device=vt.device)
-    count = torch.empty(1, dtype=torch.int64, device=vt.device)
-    _pcu_internal._sample_mesh_poisson_disk_device(is_f64, vt.data_ptr(), nv, ft.data_ptr(), nf, kind, r, n_dense, seed,
-                                                   fidx.data_ptr(), bc.data_ptr(), count.data_ptr(), dev, stream)
-    m = int(count.item())
-    return _back(fidx[:m], bc[:m], f, form)
+
+    def body(vt, ft, dev, stream):
+        is_f64, nv, nf, kind = vt.dtype == torch.float64, int(vt.shape[0]), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)]
+        area = torch.empty(3, dtype=torch.int64, device=vt.device)
+        _pcu_internal._mesh_area_device(is_f64, vt.data_ptr(), nv, ft.data_ptr(), nf, kind, area.data_ptr(), dev, stream)
+        W, S = _read_area(area)
+        r, n_dense = dense_plan(W, S, num_samples, radius, osf)
+        fidx = torch.empty(n_dense, dtype=ft.dtype, device=vt.device)
+        bc = torch.empty((n_dense, 3), dtype=vt.dtype, device=vt.device)
+        count = torch.empty(1, dtype=torch.int64, device=vt.device)
+        _pcu_internal._sample_mesh_poisson_disk_device(is_f64, vt.data_ptr(), nv, ft.data_ptr(), nf, kind, r, n_dense, seed,
+                                                       fidx.data_ptr(), bc.data_ptr(), count.data_ptr(), dev, stream)
+        m = int(count.item())
+        return fidx[:m], bc[:m]
+
+    return _run(form, [v, f], device, body, index=(f, [0]))
 
 
 def interpolate_barycentric_coords(f, fi, bc, attribute, *, device=None):
@@ -288,28 +185,30 @@ def interpolate_barycentric_coords(f, fi, bc, attribute, *, device=None):
     torch = _torch()
     out_f64 = "float64" in (_dtype_name(bc), _dtype_name(attribute))
     n, dim, nv, nf = int(fi.shape[0]), int(attribute.shape[1]), int(attribute.shape[0]), int(f.shape[0])
-    if form == "cpu":
-        out = interpolate_barycentric_coords(f.detach().numpy(), fi.detach().numpy(), bc.detach().numpy(),
-                                             attribute.detach().numpy(), device=device)
-        return torch.from_numpy(out)
-    if form == "numpy":
-        corners = f[fi]                                   # numpy's own IndexError for fi out of range
+    if form != "cuda":
+        hf, hfi = (f, fi) if form == "numpy" else (f.detach().numpy(), fi.detach().numpy())
+        corners = hf[hfi]                                 # numpy's own IndexError for fi out of range
         if corners.size and (int(corners.max()) >= nv or (corners.dtype.kind == "i" and int(corners.min()) < -nv)):
             raise IndexError("index out of bounds for attribute with %d rows" % nv)
-        if n == 0 or dim == 0:
-            return _np.zeros((n, dim), dtype=_np.float64 if out_f64 else _np.float32)
-    ft, fit, bct, at = _upload(form, [f, fi, bc, attribute], device)
     if n == 0 or dim == 0:
-        return torch.zeros((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=ft.device)
-    if nf == 0 or nv == 0:
-        raise IndexError("index out of bounds: f has %d rows and attribute %d" % (nf, nv))
-    dev, stream = _call_args(ft)
-    out = torch.empty((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=ft.device)
-    bad = torch.empty(1, dtype=torch.int64, device=ft.device)
-    _pcu_internal._interpolate_barycentric_device(ft.data_ptr(), nf, _INDEX_KINDS[_dtype_name(f)], fit.data_ptr(), n,
-                                                  _INDEX_KINDS[_dtype_name(fi)], bct.data_ptr(), bct.dtype == torch.float64,
-                                                  at.data_ptr(), at.dtype == torch.float64, nv, dim, out.data_ptr(),
-                                                  bad.data_ptr(), dev, stream)
-    if int(bad.item()):
-        raise IndexError("index out of bounds: %d rows of fi name a face or a vertex out of range" % int(bad.item()))
-    return out.cpu().numpy() if form == "numpy" else out
+        if form == "numpy":
+            return _np.zeros((n, dim), dtype=_np.float64 if out_f64 else _np.float32)
+        if form == "cuda":
+            from . import _same_device
+            _same_device(f, device)
+        return torch.zeros((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=f.device)
+
+    def body(ft, fit, bct, at, dev, stream):
+        if nf == 0 or nv == 0:
+            raise IndexError("index out of bounds: f has %d rows and attribute %d" % (nf, nv))
+        out = torch.empty((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=ft.device)
+        bad = torch.empty(1, dtype=torch.int64, device=ft.device)
+        _pcu_internal._interpolate_barycentric_device(ft.data_ptr(), nf, _INDEX_KINDS[_dtype_name(f)], fit.data_ptr(), n,
+                                                      _INDEX_KINDS[_dtype_name(fi)], bct.data_ptr(), bct.dtype == torch.float64,
+                                                      at.data_ptr(), at.dtype == torch.float64, nv, dim, out.data_ptr(),
+                                                      bad.data_ptr(), dev, stream)
+        if int(bad.item()):
+            raise IndexError("index out of bounds: %d rows of fi name a face or a vertex out of range" % int(bad.item()))
+        return out
+
+    return _run(form, [f, fi, bc, attribute], device, body)

@@ -6,27 +6,10 @@ numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA t
 CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages and in its order, before any
 device call.  Shapes are the reference's through npe::move, which squeezes them as numpy does: an (m, 1) result is
 (m,), a single entry is a 0-d array and a single (1, 3) row is (3,)."""
-import numpy as np
-
 from . import _pcu_internal
-from ._mesh_sampling import _INDEX_KINDS, _call_args, _check_float, _check_index, _dtype_name, _form, _torch, _upload, _validate_mesh
-from ._ray_mesh import _matrix_shape
+from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _matrix_shape, _run, _torch, _validate_mesh
 
 _MAX_ROWS = 2 ** 31 - 1
-
-
-def _back(form, f, *outs):
-    """The outputs squeezed as npe::move squeezes them; numpy when the inputs were (index arrays viewed as f's dtype)."""
-    torch = _torch()
-    outs = [o.squeeze() for o in outs]
-    if form != "numpy":
-        return tuple(outs)
-    return tuple(o.cpu().numpy().view(f.dtype) if o.dtype in (torch.int32, torch.int64) else o.cpu().numpy() for o in outs)
-
-
-def _from_numpy(outs):
-    torch = _torch()
-    return tuple(torch.from_numpy(o) for o in outs)
 
 
 def connected_components(v, f, *, device=None):
@@ -66,21 +49,21 @@ def connected_components(v, f, *, device=None):
     if rows >= _MAX_ROWS:
         raise ValueError("connected_components: at most 2^31 - 2 faces are supported, got %d" % rows)
     torch = _torch()
-    if form == "cpu":
-        return _from_numpy(connected_components(v.detach().numpy(), f.detach().numpy(), device=device))
-    (ft,) = _upload(form, [f], device)
-    dev, stream = _call_args(ft)
-    handle, n, k = _pcu_internal._connected_components_prepare_device(ft.data_ptr(), rows, cols, _INDEX_KINDS[_dtype_name(f)], dev,
-                                                                       stream)
-    try:
-        cv = torch.empty(n, dtype=ft.dtype, device=ft.device)
-        nv = torch.empty(k, dtype=ft.dtype, device=ft.device)
-        cf = torch.empty(rows, dtype=ft.dtype, device=ft.device)
-        nf = torch.empty(k, dtype=ft.dtype, device=ft.device)
-        _pcu_internal._connected_components_emit_device(handle, cv.data_ptr(), nv.data_ptr(), cf.data_ptr(), nf.data_ptr(), dev, stream)
-    finally:
-        _pcu_internal._connected_components_destroy(handle)
-    return _back(form, f, cv, nv, cf, nf)
+
+    def body(ft, dev, stream):
+        handle, n, k = _pcu_internal._connected_components_prepare_device(ft.data_ptr(), rows, cols, _INDEX_KINDS[_dtype_name(f)], dev,
+                                                                           stream)
+        try:
+            cv = torch.empty(n, dtype=ft.dtype, device=ft.device)
+            nv = torch.empty(k, dtype=ft.dtype, device=ft.device)
+            cf = torch.empty(rows, dtype=ft.dtype, device=ft.device)
+            nf = torch.empty(k, dtype=ft.dtype, device=ft.device)
+            _pcu_internal._connected_components_emit_device(handle, cv.data_ptr(), nv.data_ptr(), cf.data_ptr(), nf.data_ptr(), dev, stream)
+        finally:
+            _pcu_internal._connected_components_destroy(handle)
+        return cv, nv, cf, nf
+
+    return _run(form, [f], device, body, index=(f, [0, 1, 2, 3]), squeeze=True)
 
 
 def remove_mesh_vertices(v, f, mask, *, device=None):
@@ -117,16 +100,16 @@ def remove_mesh_vertices(v, f, mask, *, device=None):
     if nvert >= _MAX_ROWS or nface >= _MAX_ROWS:
         raise ValueError("remove_mesh_vertices: at most 2^31 - 2 vertices and faces are supported, got %d and %d" % (nvert, nface))
     torch = _torch()
-    if form == "cpu":
-        return _from_numpy(remove_mesh_vertices(v.detach().numpy(), f.detach().numpy(), mask.detach().numpy(), device=device))
-    vt, ft, mt = _upload(form, [v, f, mask.reshape(-1)], device)
-    dev, stream = _call_args(vt)
-    v_out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
-    f_out = torch.empty((nface, 3), dtype=ft.dtype, device=vt.device)
-    kv, kf = _pcu_internal._remove_mesh_vertices_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
-                                                        _INDEX_KINDS[_dtype_name(f)], mt.data_ptr(), v_out.data_ptr(), f_out.data_ptr(),
-                                                        dev, stream)
-    return _back(form, f, v_out[:kv], f_out[:kf])
+
+    def body(vt, ft, mt, dev, stream):
+        v_out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
+        f_out = torch.empty((nface, 3), dtype=ft.dtype, device=vt.device)
+        kv, kf = _pcu_internal._remove_mesh_vertices_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                                            _INDEX_KINDS[_dtype_name(f)], mt.data_ptr(), v_out.data_ptr(), f_out.data_ptr(),
+                                                            dev, stream)
+        return v_out[:kv], f_out[:kf]
+
+    return _run(form, [v, f, mask.reshape(-1)], device, body, index=(f, [1]), squeeze=True)
 
 
 def remove_unreferenced_mesh_vertices(v, f, *, device=None):
@@ -162,15 +145,15 @@ def remove_unreferenced_mesh_vertices(v, f, *, device=None):
         raise ValueError("remove_unreferenced_mesh_vertices: at most 2^31 - 2 vertices and faces are supported, got %d and %d"
                          % (nvert, nface))
     torch = _torch()
-    if form == "cpu":
-        return _from_numpy(remove_unreferenced_mesh_vertices(v.detach().numpy(), f.detach().numpy(), device=device))
-    vt, ft = _upload(form, [v, f], device)
-    dev, stream = _call_args(vt)
-    v_out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
-    f_out = torch.empty((nface, 3), dtype=ft.dtype, device=vt.device)
-    corr_v = torch.empty(nvert, dtype=ft.dtype, device=vt.device)
-    corr_f = torch.empty(nvert, dtype=ft.dtype, device=vt.device)
-    kept = _pcu_internal._remove_unreferenced_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
-                                                     _INDEX_KINDS[_dtype_name(f)], v_out.data_ptr(), f_out.data_ptr(), corr_v.data_ptr(),
-                                                     corr_f.data_ptr(), dev, stream)
-    return _back(form, f, v_out[:kept], f_out, corr_v[:kept], corr_f)
+
+    def body(vt, ft, dev, stream):
+        v_out = torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device)
+        f_out = torch.empty((nface, 3), dtype=ft.dtype, device=vt.device)
+        corr_v = torch.empty(nvert, dtype=ft.dtype, device=vt.device)
+        corr_f = torch.empty(nvert, dtype=ft.dtype, device=vt.device)
+        kept = _pcu_internal._remove_unreferenced_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                                         _INDEX_KINDS[_dtype_name(f)], v_out.data_ptr(), f_out.data_ptr(), corr_v.data_ptr(),
+                                                         corr_f.data_ptr(), dev, stream)
+        return v_out[:kept], f_out, corr_v[:kept], corr_f
+
+    return _run(form, [v, f], device, body, index=(f, [1, 2, 3]), squeeze=True)

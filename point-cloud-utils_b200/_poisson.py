@@ -6,15 +6,7 @@ target-count search tries); CUDA torch tensors in -> CUDA int32 tensors out; CPU
 import numpy as _np
 
 from . import _pcu_internal
-
-
-def _torch():
-    import importlib
-    return importlib.import_module("torch")
-
-
-def _is_tensor(x):
-    return type(x).__module__.startswith("torch")
+from ._call import _is_tensor, _torch
 
 
 def target_search(sample, dtype, bbsize, target, tolerance):

@@ -2,19 +2,13 @@
 src/ray_mesh_intersection.cpp and point_cloud_utils/_ray_mesh_intersector.py), computed by csrc/raycast.cuh on the tree
 of csrc/meshquery.cuh.
 
-Input forms and validation follow _mesh_query.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
+Input forms and validation follow _call.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
 import numpy as np
 
 from . import _pcu_internal
-from ._mesh_sampling import (_INDEX_KINDS, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form, _is_tensor,
-                             _raise_bad, _torch, _upload, _validate_mesh)
-
-
-def _matrix_shape(a):
-    """The (rows, cols) the reference's Eigen binding sees: a 1-D array of n elements is an (n, 1) column."""
-    s = tuple(a.shape)
-    return (s[0], 1) if len(s) == 1 else (s if len(s) == 2 else (int(np.prod(s)), 1))
+from ._call import (_INDEX_KINDS, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form, _matrix_shape,
+                    _raise_bad, _run, _torch, _upload, _validate_mesh)
 
 
 def _validate_rays(ray_o, ray_d):
@@ -43,29 +37,29 @@ def _origins(ot, single):
 
 
 def _cast(form, scene, ray_o, ray_d, single, n, device, outs, call):
-    """From validated inputs to the returned arrays.  `scene` holds the arrays that are uploaded with the rays (none for a
-    prepared tree); `outs` gives one (shape after #rays, dtype name) per output, None standing for the rays' dtype;
-    call(scene tensors, origins, o_stride, directions, outputs, device index, stream) makes the native call on
-    contiguous CUDA tensors.  CPU tensors go through numpy, and zero rays return empty outputs without a launch."""
+    """_run for rays.  `scene` holds the arrays that are uploaded with the rays (none for a prepared tree); `outs` gives
+    one (shape after #rays, dtype name) per output, None standing for the rays' dtype; call(scene tensors, origins,
+    o_stride, directions, outputs, device index, stream) makes the native call on contiguous CUDA tensors.  Zero rays
+    return empty outputs without a launch."""
     torch = _torch()
-    if form == "cpu":
-        out = _cast("numpy", [a.detach().numpy() if _is_tensor(a) else a for a in scene], ray_o.detach().numpy(),
-                    ray_d.detach().numpy(), single, n, device, outs, call)
-        return tuple(torch.from_numpy(o) for o in out)
     outs = [(tail, name or _dtype_name(ray_d)) for tail, name in outs]
     if n == 0:
         if form == "numpy":
             return tuple(np.zeros((0,) + tail, dtype=name) for tail, name in outs)
-        from . import _same_device
-        _same_device(ray_d, device)
+        if form == "cuda":
+            from . import _same_device
+            _same_device(ray_d, device)
         return tuple(torch.zeros((0,) + tail, dtype=getattr(torch, name), device=ray_d.device) for tail, name in outs)
-    *scene, ot, dt = _upload(form, list(scene) + [ray_o, ray_d], device)
-    ot, o_stride = _origins(ot, single)
-    dt = dt.reshape(n, 3)
-    dev, stream = _call_args(dt)
-    out = tuple(torch.empty((n,) + tail, dtype=getattr(torch, name), device=dt.device) for tail, name in outs)
-    call(scene, ot, o_stride, dt, out, dev, stream)
-    return tuple(o.cpu().numpy() for o in out) if form == "numpy" else out
+
+    def body(*args):
+        *scene_t, ot, dt, dev, stream = args
+        ot, o_stride = _origins(ot, single)
+        dt = dt.reshape(n, 3)
+        out = tuple(torch.empty((n,) + tail, dtype=getattr(torch, name), device=dt.device) for tail, name in outs)
+        call(scene_t, ot, o_stride, dt, out, dev, stream)
+        return out
+
+    return _run(form, list(scene) + [ray_o, ray_d], device, body)
 
 
 def ray_mesh_intersection(v, f, ray_o, ray_d, ray_near=0.0, ray_far=np.inf, *, device=None):
@@ -182,8 +176,7 @@ class RayMeshIntersector(_Prepared):
         self.v = mesh_v
         self.f = mesh_f
         torch = _torch()
-        arrays = [mesh_v.detach().numpy(), mesh_f.detach().numpy()] if form == "cpu" else [mesh_v, mesh_f]
-        vt, ft = _upload(form, arrays, device)
+        vt, ft = _upload(form, [mesh_v, mesh_f], device)
         dev, stream = _call_args(vt)
         bad = torch.empty(1, dtype=torch.int64, device=vt.device)
         handle = _pcu_internal._mesh_prepare_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(),

@@ -2,13 +2,13 @@
 outputs (the reference's src/ray_point_cloud_intersection.cpp, point_cloud_utils/_ray_point_cloud_intersector.py and
 _point_cloud_geometry.py), computed by csrc/raycast.cuh on the surfel tree of csrc/meshquery.cuh.
 
-Input forms and validation follow _ray_mesh.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
+Input forms and validation follow _call.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
 import numpy as np
 
 from . import _pcu_internal
-from ._mesh_sampling import _call_args, _check_float, _check_match, _dtype_name, _form, _is_tensor, _torch, _upload
-from ._ray_mesh import _Prepared, _bounds, _cast, _matrix_shape, _validate_rays
+from ._call import _call_args, _check_float, _check_match, _dtype_name, _form, _is_tensor, _matrix_shape, _run, _torch, _upload
+from ._ray_mesh import _Prepared, _bounds, _cast, _validate_rays
 
 _MAX_SUBDIVS = 2 ** 24
 
@@ -151,9 +151,7 @@ class RaySurfelIntersector(_Prepared):
         self.r = r
         self.num_subdivs = subdivs
         torch = _torch()
-        arrays = [p.detach().numpy(), n.detach().numpy(), _radius_like(r, p, "cpu")] if form == "cpu" \
-            else [p, n, _radius_like(r, p, form)]
-        pt, nt, rt = _upload(form, arrays, device)
+        pt, nt, rt = _upload(form, [p, n, _radius_like(r, p, form)], device)
         dev, stream = _call_args(pt)
         handle = _pcu_internal._surfel_prepare_device(pt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), rt.data_ptr(),
                                                       int(pt.shape[0]), subdivs, dev, stream)
@@ -212,26 +210,23 @@ def pointcloud_surfel_geometry(p, n, r=0.1, subdivs=7, *, device=None):
     _check_match(n, "n", p, "v")
     subdivs = _validate_surfels(p, n, subdivs)
     torch = _torch()
-    if form == "cpu":
-        out = pointcloud_surfel_geometry(p.detach().numpy(), n.detach().numpy(), _radius_like(r, p, "cpu"), subdivs,
-                                         device=device)
-        return tuple(torch.from_numpy(o) for o in out)
     m = int(p.shape[0])
     if m == 0:
         if form == "numpy":
             return np.zeros((0, 3), dtype=p.dtype), np.zeros((0, 3), dtype=np.int32)
-        from . import _same_device
-        _same_device(p, device)
+        if form == "cuda":
+            from . import _same_device
+            _same_device(p, device)
         return torch.zeros((0, 3), dtype=p.dtype, device=p.device), torch.zeros((0, 3), dtype=torch.int32, device=p.device)
     if m * (subdivs + 1) >= 2 ** 31 - 1:
         raise ValueError("pointcloud_surfel_geometry: int32 faces index at most 2^31 - 2 vertices, got %d points of %d"
                          % (m, subdivs + 1))
-    pt, nt, rt = _upload(form, [p, n, _radius_like(r, p, form)], device)
-    dev, stream = _call_args(pt)
-    v = torch.empty((m * (subdivs + 1), 3), dtype=pt.dtype, device=pt.device)
-    f = torch.empty((m * subdivs, 3), dtype=torch.int32, device=pt.device)
-    _pcu_internal._surfel_geometry_device(pt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), rt.data_ptr(), m, subdivs,
-                                          v.data_ptr(), f.data_ptr(), dev, stream)
-    if form == "numpy":
-        return v.cpu().numpy(), f.cpu().numpy()
-    return v, f
+
+    def body(pt, nt, rt, dev, stream):
+        v = torch.empty((m * (subdivs + 1), 3), dtype=pt.dtype, device=pt.device)
+        f = torch.empty((m * subdivs, 3), dtype=torch.int32, device=pt.device)
+        _pcu_internal._surfel_geometry_device(pt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), rt.data_ptr(), m, subdivs,
+                                              v.data_ptr(), f.data_ptr(), dev, stream)
+        return v, f
+
+    return _run(form, [p, n, _radius_like(r, p, form)], device, body)

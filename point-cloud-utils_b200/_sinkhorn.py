@@ -8,13 +8,9 @@ import math
 import numpy as _np
 
 from . import _pcu_internal
+from ._call import _torch
 
 _NORM2, _NORM1, _NORMINF, _NORMNEGINF, _NORM0, _NORMP = range(6)
-
-
-def _torch():
-    import importlib
-    return importlib.import_module("torch")
 
 
 def _norm_kind(p):

@@ -4,8 +4,7 @@ reference's src/marching_cubes.cpp and src/sparse_voxel_grid.cpp), computed by c
 numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA torch tensors in -> CUDA tensors out;
 CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
 from . import _pcu_internal
-from ._mesh_sampling import _INDEX_KINDS, _call_args, _check_float, _check_index, _dtype_name, _form, _torch, _upload
-from ._ray_mesh import _matrix_shape
+from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _matrix_shape, _run, _torch
 
 _MAX_ROWS = 2 ** 31 - 1
 _OVERFLOW = "Invalid vertex leads to an overflow integer. Perhaps grid_size is too small."
@@ -84,27 +83,23 @@ def marching_cubes_sparse_voxel_grid(grid_scalars, grid_coordinates, cube_indice
     n, m = _validate_marching_cubes(grid_scalars, grid_coordinates, cube_indices)
     isovalue = float(isovalue)
     torch = _torch()
-    if form == "cpu":
-        out = marching_cubes_sparse_voxel_grid(grid_scalars.detach().numpy(), grid_coordinates.detach().numpy(),
-                                               cube_indices.detach().numpy(), isovalue, device=device)
-        return tuple(torch.from_numpy(o) for o in out)
-    st, ct, it = _upload(form, [grid_scalars.reshape(n), grid_coordinates, cube_indices], device)
-    it = _aligned(it)
-    dev, stream = _call_args(ct)
-    handle, nv, nf = _pcu_internal._marching_cubes_prepare_device(
-        ct.dtype == torch.float64, st.data_ptr(), st.dtype == torch.float64, ct.data_ptr(), n, it.data_ptr(), m,
-        _INDEX_KINDS[_dtype_name(cube_indices)], isovalue, dev, stream)
-    try:
-        if nv == 0:
-            raise ValueError("No level set found for isovalue %f" % isovalue)
-        v = torch.empty((nv, 3), dtype=ct.dtype, device=ct.device)
-        f = torch.empty((nf, 3), dtype=it.dtype, device=ct.device)
-        _pcu_internal._marching_cubes_emit_device(handle, v.data_ptr(), f.data_ptr(), dev, stream)
-    finally:
-        _pcu_internal._marching_cubes_destroy(handle)
-    if form == "numpy":
-        return v.cpu().numpy(), f.cpu().numpy().view(cube_indices.dtype)
-    return v, f
+
+    def body(st, ct, it, dev, stream):
+        it = _aligned(it)
+        handle, nv, nf = _pcu_internal._marching_cubes_prepare_device(
+            ct.dtype == torch.float64, st.data_ptr(), st.dtype == torch.float64, ct.data_ptr(), n, it.data_ptr(), m,
+            _INDEX_KINDS[_dtype_name(cube_indices)], isovalue, dev, stream)
+        try:
+            if nv == 0:
+                raise ValueError("No level set found for isovalue %f" % isovalue)
+            v = torch.empty((nv, 3), dtype=ct.dtype, device=ct.device)
+            f = torch.empty((nf, 3), dtype=it.dtype, device=ct.device)
+            _pcu_internal._marching_cubes_emit_device(handle, v.data_ptr(), f.data_ptr(), dev, stream)
+        finally:
+            _pcu_internal._marching_cubes_destroy(handle)
+        return v, f
+
+    return _run(form, [grid_scalars.reshape(n), grid_coordinates, cube_indices], device, body, index=(cube_indices, [1]))
 
 
 def sparse_voxel_grid_boundary(grid_coordinates, *, device=None):
@@ -137,16 +132,15 @@ def sparse_voxel_grid_boundary(grid_coordinates, *, device=None):
     if rows >= _MAX_ROWS:
         raise ValueError("sparse_voxel_grid_boundary: at most 2^31 - 2 voxels are supported, got %d" % rows)
     torch = _torch()
-    if form == "cpu":
-        return torch.from_numpy(sparse_voxel_grid_boundary(grid_coordinates.detach().numpy(), device=device))
-    (gt,) = _upload(form, [grid_coordinates], device)
-    dev, stream = _call_args(gt)
-    out = torch.empty(rows, dtype=torch.int64, device=gt.device)
-    counts = torch.empty(2, dtype=torch.int64, device=gt.device)
-    _pcu_internal._sparse_voxel_grid_boundary_device(gt.data_ptr(), rows, _INDEX_KINDS[_dtype_name(grid_coordinates)],
-                                                     out.data_ptr(), counts.data_ptr(), dev, stream)
-    found, bad = (int(c) for c in counts.cpu().numpy())
-    if bad:
-        raise ValueError(_OVERFLOW)
-    res = out[:found].reshape(found, 1).squeeze()        # the reference's (m, 1) result through npe::move's squeeze
-    return res.cpu().numpy() if form == "numpy" else res
+
+    def body(gt, dev, stream):
+        out = torch.empty(rows, dtype=torch.int64, device=gt.device)
+        counts = torch.empty(2, dtype=torch.int64, device=gt.device)
+        _pcu_internal._sparse_voxel_grid_boundary_device(gt.data_ptr(), rows, _INDEX_KINDS[_dtype_name(grid_coordinates)],
+                                                         out.data_ptr(), counts.data_ptr(), dev, stream)
+        found, bad = (int(c) for c in counts.cpu().numpy())
+        if bad:
+            raise ValueError(_OVERFLOW)
+        return out[:found].reshape(found, 1)        # the reference's (m, 1) result, squeezed as npe::move squeezes it
+
+    return _run(form, [grid_coordinates], device, body, squeeze=True)

@@ -7,7 +7,7 @@ device call."""
 import numpy as np
 
 from . import _pcu_internal
-from ._mesh_sampling import _INDEX_KINDS, _call_args, _check_index, _dtype_name, _form, _torch, _upload, _validate_mesh
+from ._call import _INDEX_KINDS, _check_index, _dtype_name, _form, _run, _torch, _validate_mesh
 
 _GRID_KINDS = {"int32": 0, "int64": 1, "float32": 2, "float64": 3}
 _MAX_VOXELS = 2 ** 31
@@ -69,14 +69,14 @@ def flood_fill_3d(grid, start_coord, fill_value, *, device=None):
         raise ValueError("flood_fill_3d: grids of at most 2^31 - 1 voxels are supported, got %d x %d x %d" % (w, h, d))
     fill = float(fill_value)
     torch = _torch()
-    if form == "cpu":
-        return torch.from_numpy(flood_fill_3d(grid.detach().numpy(), start_coord, fill, device=device))
-    (gt,) = _upload(form, [grid], device)
-    dev, stream = _call_args(gt)
-    out = torch.empty_like(gt)
-    _pcu_internal._flood_fill_3d_device(gt.data_ptr(), _GRID_KINDS[_dtype_name(grid)], w, h, d, int(start_coord[0]),
-                                        int(start_coord[1]), int(start_coord[2]), fill, out.data_ptr(), dev, stream)
-    return out.cpu().numpy() if form == "numpy" else out
+
+    def body(gt, dev, stream):
+        out = torch.empty_like(gt)
+        _pcu_internal._flood_fill_3d_device(gt.data_ptr(), _GRID_KINDS[_dtype_name(grid)], w, h, d, int(start_coord[0]),
+                                            int(start_coord[1]), int(start_coord[2]), fill, out.data_ptr(), dev, stream)
+        return out
+
+    return _run(form, [grid], device, body)
 
 
 def voxelize_triangle_mesh(v, f, voxel_size, voxel_origin, *, device=None):
@@ -118,17 +118,16 @@ def voxelize_triangle_mesh(v, f, voxel_size, voxel_origin, *, device=None):
     if voxel_size[0] <= 0.0 or voxel_size[1] <= 0.0 or voxel_size[2] <= 0.0:
         raise ValueError("Invalid voxel size")
     torch = _torch()
-    if form == "cpu":
-        return torch.from_numpy(voxelize_triangle_mesh(v.detach().numpy(), f.detach().numpy(), voxel_size, voxel_origin,
-                                                       device=device))
-    vt, ft = _upload(form, [v, f], device)
-    dev, stream = _call_args(vt)
-    handle, n, _ = _pcu_internal._voxelize_prepare_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]),
-                                                          ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)],
-                                                          voxel_size.tolist(), voxel_origin.tolist(), dev, stream)
-    try:
-        ijk = torch.empty((n, 3), dtype=torch.int32, device=vt.device)
-        _pcu_internal._voxelize_emit_device(handle, ijk.data_ptr(), dev, stream)
-    finally:
-        _pcu_internal._voxelize_destroy(handle)
-    return ijk.cpu().numpy() if form == "numpy" else ijk
+
+    def body(vt, ft, dev, stream):
+        handle, n, _ = _pcu_internal._voxelize_prepare_device(vt.dtype == torch.float64, vt.data_ptr(), int(vt.shape[0]),
+                                                              ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)],
+                                                              voxel_size.tolist(), voxel_origin.tolist(), dev, stream)
+        try:
+            ijk = torch.empty((n, 3), dtype=torch.int32, device=vt.device)
+            _pcu_internal._voxelize_emit_device(handle, ijk.data_ptr(), dev, stream)
+        finally:
+            _pcu_internal._voxelize_destroy(handle)
+        return ijk
+
+    return _run(form, [v, f], device, body)

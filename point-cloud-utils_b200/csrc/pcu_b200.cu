@@ -267,12 +267,17 @@ struct pcu_b200_mesh {
     const void* leaves = nullptr;   // Pt<float> or Pt<double> by is_f64, or SfWord
     const int* ids = nullptr;       // surfels: the point id of each leaf
 };
-// Marching cubes between pcu_b200_marching_cubes_prepare_* and _emit: the inputs, the cube block (case bytes, tile
-// offsets, counts; sized by m) and the slot block (run of every slot, vertex id of every run, owner flags; sized by the
-// slot count), both allocated and freed in the order of `stream`.
-struct pcu_b200_marching_cubes {
+// What the stream-ordered handles below share: the device and stream they were prepared on.  Deleting a handle releases
+// its blocks in the order of that stream.
+struct StreamHandle {
     int device = 0;
     cudaStream_t stream = nullptr;
+    void release(unsigned char* block) const { if (block) cudaFreeAsync(block, stream); }
+};
+// Marching cubes between pcu_b200_marching_cubes_prepare_* and _emit: the inputs, the cube block (case bytes, tile
+// offsets, counts; sized by m) and the slot block (run of every slot, vertex id of every run, owner flags; sized by the
+// slot count).
+struct pcu_b200_marching_cubes : StreamHandle {
     int t_f64 = 0, s_f64 = 0, width = 4;   // coordinates, scalars, bytes per cube index
     const void* scalars = nullptr;
     const void* coords = nullptr;
@@ -290,24 +295,21 @@ struct pcu_b200_marching_cubes {
     unsigned* slot_run = nullptr;
     unsigned* run_vid = nullptr;
     unsigned char* owner = nullptr;
+    ~pcu_b200_marching_cubes() { release(cube_block); release(slot_block); }
 };
 // Voxelization between pcu_b200_voxelize_prepare_* and _emit: the sorted codes, their run heads and the heads' block
-// offsets, in one block allocated and freed in the order of `stream`.
-struct pcu_b200_voxelize {
-    int device = 0;
-    cudaStream_t stream = nullptr;
+// offsets, in one block.
+struct pcu_b200_voxelize : StreamHandle {
     long long recs = 0, n = 0;              // accepted (face, voxel) pairs; distinct voxels
     unsigned char* block = nullptr;
     const McRec* sorted = nullptr;
     unsigned char* head = nullptr;
     unsigned* offsets = nullptr;
+    ~pcu_b200_voxelize() { release(block); }
 };
 // Connected components between pcu_b200_connected_components_prepare and _emit: int32 labels and counts in one block
-// allocated and freed in the order of `stream` (cv over n = max(f) + 1 vertices, cf over m faces, nv and nf over
-// the k components, sized n).
-struct pcu_b200_components {
-    int device = 0;
-    cudaStream_t stream = nullptr;
+// (cv over n = max(f) + 1 vertices, cf over m faces, nv and nf over the k components, sized n).
+struct pcu_b200_components : StreamHandle {
     int fkind = 0;
     long long n = 0, m = 0, k = 0;
     unsigned char* block = nullptr;
@@ -315,6 +317,7 @@ struct pcu_b200_components {
     const int* cf = nullptr;
     const int* nv = nullptr;
     const int* nf = nullptr;
+    ~pcu_b200_components() { release(block); }
 };
 template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
@@ -1753,26 +1756,51 @@ int surfel_geometry_device(pcu_b200_workspace* ws, const T* p, const T* nrm, con
 }
 
 // ---- marching cubes and the boundary of a sparse voxel grid (sparse_voxels.cuh) ------------------------------------
-int mc_free(pcu_b200_marching_cubes* h) {
-    if (h->cube_block) cudaFreeAsync(h->cube_block, h->stream);
-    if (h->slot_block) cudaFreeAsync(h->slot_block, h->stream);
-    delete h;
+// Copies a count record to the host and waits for it: one synchronisation of `stream`.
+template <class R>
+int read_record(const R* dev, R* host, cudaStream_t stream) {
+    PCU_CUDA(cudaMemcpyAsync(host, dev, sizeof(R), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
     return PCU_B200_OK;
 }
 
-int mc_alloc(unsigned char*& block, size_t bytes, cudaStream_t stream) {
+// The failure of a call that found `bad` faces with a corner outside [0, #v).
+int bad_corners(unsigned long long bad) {
+    return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", bad);
+}
+
+// Whether face indices of this kind are 64 bits wide.
+inline bool wide_index(int kind) { return kind & 1; }
+
+// A handle's block, allocated in the order of `stream`; `what` names the handle's feature when that fails.
+int alloc_block(unsigned char*& block, size_t bytes, cudaStream_t stream, const char* what) {
     const cudaError_t e = cudaMallocAsync((void**)&block, bytes, stream);
     if (e != cudaSuccess) {
         cudaGetLastError();
         block = nullptr;
-        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMallocAsync of %zu bytes for marching cubes failed: %s", bytes, cudaGetErrorString(e));
+        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMallocAsync of %zu bytes for %s failed: %s", bytes, what, cudaGetErrorString(e));
     }
     return PCU_B200_OK;
 }
 
-int mc_read_counts(pcu_b200_marching_cubes* h, McCounts& out) {
-    PCU_CUDA(cudaMemcpyAsync(&out, h->counts, sizeof(McCounts), cudaMemcpyDeviceToHost, h->stream));
-    PCU_CUDA(cudaStreamSynchronize(h->stream));
+// A new handle H on the workspace's device and `stream`: runs build(h), deletes the handle if that fails and
+// publishes it in *out if it succeeds.
+template <class H, class Build>
+int prepare_handle(pcu_b200_workspace* ws, cudaStream_t stream, H** out, Build&& build) {
+    H* h = new (std::nothrow) H();
+    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
+    h->device = ws->device;
+    h->stream = stream;
+    const int st = build(h);
+    if (st != PCU_B200_OK) { delete h; return st; }
+    *out = h;
+    return PCU_B200_OK;
+}
+
+// An emit runs on the device its handle was prepared on; `what` names the handle.
+int check_handle_device(const pcu_b200_workspace* ws, const StreamHandle* h, const char* what) {
+    if (h->device != ws->device)
+        return fail(PCU_B200_INVALID_ARGUMENT, "the %s handle lives on device %d, the workspace on %d", what, h->device, ws->device);
     return PCU_B200_OK;
 }
 
@@ -1787,7 +1815,7 @@ int mc_build(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t st
                h->cases, h->tile_sum, h->counts);
     PCU_LAUNCH(mc_tiles_kernel, 1, 1024, stream, (const unsigned*)h->tile_sum, (long long)tiles, h->tile_slot0, h->tile_face0, h->counts);
     McCounts c;
-    PCU_TRY(mc_read_counts(h, c));
+    PCU_TRY(read_record(h->counts, &c, stream));
     if (c.bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid cube_indices: %llu cubes have a corner outside [0, %lld)", c.bad, h->n);
     if (c.slots >= (1ull << 32))
         return fail(PCU_B200_INVALID_ARGUMENT, "marching cubes: at most 2^32 - 1 crossing edges are supported, got %llu", c.slots);
@@ -1795,8 +1823,8 @@ int mc_build(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t st
     h->faces = (long long)c.faces;
     const long long ns = h->slots;
     if (ns == 0) return PCU_B200_OK;
-    PCU_TRY(mc_alloc(h->slot_block, carve_at(nullptr, [&](Carver& cv) {
-        cv.take<unsigned>((size_t)ns); cv.take<unsigned>((size_t)ns); cv.take<unsigned char>((size_t)ns); }), stream));
+    PCU_TRY(alloc_block(h->slot_block, carve_at(nullptr, [&](Carver& cv) {
+        cv.take<unsigned>((size_t)ns); cv.take<unsigned>((size_t)ns); cv.take<unsigned char>((size_t)ns); }), stream, "marching cubes"));
     carve_at(h->slot_block, [&](Carver& cv) {
         h->slot_run = cv.take<unsigned>((size_t)ns);
         h->run_vid = cv.take<unsigned>((size_t)ns);
@@ -1823,7 +1851,7 @@ int mc_build(pcu_b200_workspace* ws, pcu_b200_marching_cubes* h, cudaStream_t st
     PCU_TRY(enqueue_keep_offsets(h->owner, ns, sc.ocounts, sc.owners, stream));
     PCU_LAUNCH(mc_owner_kernel, blocks_for(ns), kThreads, stream, (const unsigned char*)h->owner, ns, (const unsigned*)sc.ocounts,
                (const unsigned*)h->slot_run, h->run_vid);
-    PCU_TRY(mc_read_counts(h, c));
+    PCU_TRY(read_record(h->counts, &c, stream));
     h->verts = c.verts;
     return PCU_B200_OK;
 }
@@ -1847,33 +1875,28 @@ int marching_cubes_prepare_device(pcu_b200_workspace* ws, const void* scalars, i
     if ((m + kThreads - 1) / kThreads > 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "too many cubes (%lld)", m);
     PCU_ON_DEVICE(ws);
     PCU_TRY(adopt_stream(ws, stream));
-    pcu_b200_marching_cubes* h = new (std::nothrow) pcu_b200_marching_cubes();
-    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
-    h->device = ws->device; h->stream = stream; h->t_f64 = sizeof(T) == 8; h->s_f64 = s_f64 != 0; h->width = (kind & 1) ? 8 : 4;
-    h->scalars = scalars; h->coords = coords; h->idx = idx; h->n = n; h->m = m;
-    h->iso = s_f64 ? (double)(T)isovalue : (double)(T)(float)isovalue;
-    const long long tiles = (m + kThreads - 1) / kThreads;
-    const auto carve = [&](Carver& cv) {
-        h->cases = cv.take<unsigned char>((size_t)m);
-        h->tile_sum = cv.take<unsigned>((size_t)tiles);
-        h->tile_slot0 = cv.take<unsigned long long>((size_t)tiles);
-        h->tile_face0 = cv.take<unsigned long long>((size_t)tiles);
-        h->counts = cv.take<McCounts>(1);
-    };
-    int st = mc_alloc(h->cube_block, carve_at(nullptr, carve), stream);
-    if (st == PCU_B200_OK) {
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_marching_cubes* h) -> int {
+        h->t_f64 = sizeof(T) == 8; h->s_f64 = s_f64 != 0; h->width = wide_index(kind) ? 8 : 4;
+        h->scalars = scalars; h->coords = coords; h->idx = idx; h->n = n; h->m = m;
+        h->iso = s_f64 ? (double)(T)isovalue : (double)(T)(float)isovalue;
+        const long long tiles = (m + kThreads - 1) / kThreads;
+        const auto carve = [&](Carver& cv) {
+            h->cases = cv.take<unsigned char>((size_t)m);
+            h->tile_sum = cv.take<unsigned>((size_t)tiles);
+            h->tile_slot0 = cv.take<unsigned long long>((size_t)tiles);
+            h->tile_face0 = cv.take<unsigned long long>((size_t)tiles);
+            h->counts = cv.take<McCounts>(1);
+        };
+        PCU_TRY(alloc_block(h->cube_block, carve_at(nullptr, carve), stream, "marching cubes"));
         carve_at(h->cube_block, carve);
-        st = h->s_f64 ? mc_build_width<T, double>(ws, h, stream) : mc_build_width<T, float>(ws, h, stream);
-    }
-    if (st == PCU_B200_OK) {
+        PCU_TRY((h->s_f64 ? mc_build_width<T, double>(ws, h, stream) : mc_build_width<T, float>(ws, h, stream)));
         const long long most = kind == kIdxI32 ? (1ll << 31) : kind == kIdxU32 ? (1ll << 32) : LLONG_MAX;
-        if (h->verts > most) st = fail(PCU_B200_INVALID_ARGUMENT, "marching cubes: %lld vertices cannot be indexed by cube_indices' dtype",
-                                       h->verts);
-    }
-    if (st != PCU_B200_OK) { mc_free(h); return st; }
-    out_counts[0] = h->verts;
-    out_counts[1] = h->faces;
-    *out = h;
+        if (h->verts > most)
+            return fail(PCU_B200_INVALID_ARGUMENT, "marching cubes: %lld vertices cannot be indexed by cube_indices' dtype", h->verts);
+        return PCU_B200_OK;
+    }));
+    out_counts[0] = (*out)->verts;
+    out_counts[1] = (*out)->faces;
     return PCU_B200_OK;
 }
 
@@ -1893,8 +1916,7 @@ int mc_emit_width(const pcu_b200_marching_cubes* h, void* out_v, void* out_f, cu
 
 int marching_cubes_emit_device(pcu_b200_workspace* ws, const pcu_b200_marching_cubes* h, void* out_v, void* out_f, cudaStream_t stream) {
     if (!ws || !h) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
-    if (h->device != ws->device) return fail(PCU_B200_INVALID_ARGUMENT, "the marching-cubes handle lives on device %d, the workspace on %d",
-                                             h->device, ws->device);
+    PCU_TRY(check_handle_device(ws, h, "marching-cubes"));
     if (h->slots == 0) return PCU_B200_OK;
     if (!out_v || (h->faces > 0 && !out_f)) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
     PCU_ON_DEVICE(ws);
@@ -1936,12 +1958,6 @@ int sparse_voxel_grid_boundary_device(pcu_b200_workspace* ws, const void* g, lon
 }
 
 // ---- triangle-mesh voxelization and 3-D flood fill (voxelize.cuh) ------------------------------------------------
-int vx_free(pcu_b200_voxelize* h) {
-    if (h->block) cudaFreeAsync(h->block, h->stream);
-    delete h;
-    return PCU_B200_OK;
-}
-
 // Persistent CTAs of vx_test_kernel: enough to fill every SM (the kernel holds 16-32 KB of shared memory per CTA).
 inline unsigned vx_test_blocks(const pcu_b200_workspace* ws) { return (unsigned)ws->sm_count * 6u; }
 
@@ -1964,9 +1980,8 @@ int vx_build(pcu_b200_workspace* ws, pcu_b200_voxelize* h, const T* v, long long
     PCU_LAUNCH((vx_test_kernel<T, false>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
                (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, (McRec*)nullptr);
     VxCounts c;
-    PCU_CUDA(cudaMemcpyAsync(&c, sc.counts, sizeof(VxCounts), cudaMemcpyDeviceToHost, stream));
-    PCU_CUDA(cudaStreamSynchronize(stream));
-    if (c.bad_corner) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", c.bad_corner);
+    PCU_TRY(read_record(sc.counts, &c, stream));
+    if (c.bad_corner) return bad_corners(c.bad_corner);
     if (c.bad_bounds)
         return fail(PCU_B200_INVALID_ARGUMENT, "voxelize_triangle_mesh: %llu faces have a non-finite vertex or voxel index bounds outside "
                     "[-2^31, 2^31 - 2]", c.bad_bounds);
@@ -1984,13 +1999,7 @@ int vx_build(pcu_b200_workspace* ws, pcu_b200_voxelize* h, const T* v, long long
         hb.head = cv.take<unsigned char>((size_t)na);
         hb.counts = cv.take<unsigned>(keep_count_words(na));
     };
-    const size_t bytes = carve_at(nullptr, carve);
-    const cudaError_t e = cudaMallocAsync((void**)&h->block, bytes, stream);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        h->block = nullptr;
-        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMallocAsync of %zu bytes for voxelization failed: %s", bytes, cudaGetErrorString(e));
-    }
+    PCU_TRY(alloc_block(h->block, carve_at(nullptr, carve), stream, "voxelization"));
     carve_at(h->block, carve);
     PCU_LAUNCH((vx_test_kernel<T, true>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
                (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, hb.sort.a);
@@ -1998,8 +2007,7 @@ int vx_build(pcu_b200_workspace* ws, pcu_b200_voxelize* h, const T* v, long long
     PCU_TRY(radix_sort_records(hb.sort, na, 1, stream, &sorted));
     PCU_LAUNCH(mc_heads_kernel, blocks_for(na), kThreads, stream, (const McRec*)sorted, na, hb.head);
     PCU_TRY(enqueue_keep_offsets(hb.head, na, hb.counts, &sc.counts->unique, stream));
-    PCU_CUDA(cudaMemcpyAsync(&c, sc.counts, sizeof(VxCounts), cudaMemcpyDeviceToHost, stream));
-    PCU_CUDA(cudaStreamSynchronize(stream));
+    PCU_TRY(read_record(sc.counts, &c, stream));
     h->n = c.unique;
     h->sorted = sorted;
     h->head = hb.head;
@@ -2022,22 +2030,15 @@ int voxelize_prepare_device(pcu_b200_workspace* ws, const T* v, long long nv, co
     PCU_TRY(adopt_stream(ws, stream));
     VxGeom g;
     for (int k = 0; k < 3; ++k) { g.o[k] = origin[k]; g.s[k] = size[k]; g.h[k] = size[k] / 2; }
-    pcu_b200_voxelize* h = new (std::nothrow) pcu_b200_voxelize();
-    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
-    h->device = ws->device;
-    h->stream = stream;
-    const int st = vx_build<T>(ws, h, v, nv, f, m, fkind, g, stream);
-    if (st != PCU_B200_OK) { vx_free(h); return st; }
-    out_counts[0] = h->n;
-    out_counts[1] = h->recs;
-    *out = h;
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_voxelize* h) { return vx_build<T>(ws, h, v, nv, f, m, fkind, g, stream); }));
+    out_counts[0] = (*out)->n;
+    out_counts[1] = (*out)->recs;
     return PCU_B200_OK;
 }
 
 int voxelize_emit_device(pcu_b200_workspace* ws, const pcu_b200_voxelize* h, int32_t* out_ijk, cudaStream_t stream) {
     if (!ws || !h || !out_ijk) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
-    if (h->device != ws->device) return fail(PCU_B200_INVALID_ARGUMENT, "the voxelization handle lives on device %d, the workspace on %d",
-                                             h->device, ws->device);
+    PCU_TRY(check_handle_device(ws, h, "voxelization"));
     PCU_ON_DEVICE(ws);
     PCU_TRY(adopt_stream(ws, stream));
     PCU_LAUNCH(vx_decode_kernel, blocks_for(h->recs), kThreads, stream, h->sorted, h->recs, (const unsigned char*)h->head,
@@ -2101,12 +2102,6 @@ int flood_fill_3d_device(pcu_b200_workspace* ws, const void* grid, int kind, lon
 }
 
 // ---- mesh connected components and vertex removal (mesh_topology.cuh) ----------------------------------------------
-int cc_free(pcu_b200_components* h) {
-    if (h->block) cudaFreeAsync(h->block, h->stream);
-    delete h;
-    return PCU_B200_OK;
-}
-
 // Persistent CTAs of cc_validate_kernel.
 inline unsigned cc_validate_blocks(const pcu_b200_workspace* ws, long long total) {
     return (unsigned)std::max(1ll, std::min((long long)ws->sm_count * 8, (total + kThreads - 1) / kThreads));
@@ -2121,8 +2116,7 @@ int cc_build(pcu_b200_workspace* ws, pcu_b200_components* h, const void* f, long
     const long long total = m * c;
     PCU_LAUNCH(cc_validate_kernel, cc_validate_blocks(ws, total), kThreads, stream, f, fkind, total, rec);
     CcCounts hc;
-    PCU_CUDA(cudaMemcpyAsync(&hc, rec, sizeof(CcCounts), cudaMemcpyDeviceToHost, stream));
-    PCU_CUDA(cudaStreamSynchronize(stream));
+    PCU_TRY(read_record(rec, &hc, stream));
     if (hc.bad)
         return fail(PCU_B200_INVALID_ARGUMENT, "connected_components: %llu face indices are negative or above 2^31 - 2", hc.bad);
     const long long n = (long long)hc.max_index + 1;
@@ -2137,13 +2131,7 @@ int cc_build(pcu_b200_workspace* ws, pcu_b200_components* h, const void* f, long
         b.is_root = cv.take<unsigned char>((size_t)n);
         b.counts = cv.take<unsigned>(keep_count_words(n));
     };
-    const size_t bytes = carve_at(nullptr, carve);
-    const cudaError_t e = cudaMallocAsync((void**)&h->block, bytes, stream);
-    if (e != cudaSuccess) {
-        cudaGetLastError();
-        h->block = nullptr;
-        return fail(PCU_B200_OUT_OF_MEMORY, "cudaMallocAsync of %zu bytes for connected components failed: %s", bytes, cudaGetErrorString(e));
-    }
+    PCU_TRY(alloc_block(h->block, carve_at(nullptr, carve), stream, "connected components"));
     carve_at(h->block, carve);
     PCU_CUDA(cudaMemsetAsync(b.nv, 0, sizeof(int) * (size_t)n, stream));
     PCU_CUDA(cudaMemsetAsync(b.nf, 0, sizeof(int) * (size_t)n, stream));
@@ -2154,8 +2142,7 @@ int cc_build(pcu_b200_workspace* ws, pcu_b200_components* h, const void* f, long
     PCU_LAUNCH(cc_rank_kernel, blocks_for(n), kThreads, stream, (const unsigned char*)b.is_root, n, (const unsigned*)b.counts, b.rank);
     PCU_LAUNCH(cc_label_kernel, blocks_for(n), kThreads, stream, b.root, n, (const int*)b.rank, b.nv);
     PCU_LAUNCH(cc_face_kernel, blocks_for(m), kThreads, stream, f, fkind, m, c, (const int*)b.root, b.cf, b.nf);
-    PCU_CUDA(cudaMemcpyAsync(&hc, rec, sizeof(CcCounts), cudaMemcpyDeviceToHost, stream));
-    PCU_CUDA(cudaStreamSynchronize(stream));
+    PCU_TRY(read_record(rec, &hc, stream));
     h->n = n;
     h->m = m;
     h->k = hc.ncomp;
@@ -2177,28 +2164,23 @@ int connected_components_prepare_device(pcu_b200_workspace* ws, const void* f, l
     if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
     PCU_ON_DEVICE(ws);
     PCU_TRY(adopt_stream(ws, stream));
-    pcu_b200_components* h = new (std::nothrow) pcu_b200_components();
-    if (!h) return fail(PCU_B200_OUT_OF_MEMORY, "out of host memory");
-    h->device = ws->device;
-    h->stream = stream;
-    h->fkind = fkind;
-    const int st = cc_build(ws, h, f, m, c, fkind, stream);
-    if (st != PCU_B200_OK) { cc_free(h); return st; }
-    out_counts[0] = h->n;
-    out_counts[1] = h->k;
-    *out = h;
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_components* h) {
+        h->fkind = fkind;
+        return cc_build(ws, h, f, m, c, fkind, stream);
+    }));
+    out_counts[0] = (*out)->n;
+    out_counts[1] = (*out)->k;
     return PCU_B200_OK;
 }
 
 int connected_components_emit_device(pcu_b200_workspace* ws, const pcu_b200_components* h, void* out_cv, void* out_nv, void* out_cf,
                                      void* out_nf, cudaStream_t stream) {
     if (!ws || !h || !out_cv || !out_nv || !out_cf || !out_nf) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
-    if (h->device != ws->device)
-        return fail(PCU_B200_INVALID_ARGUMENT, "the components handle lives on device %d, the workspace on %d", h->device, ws->device);
+    PCU_TRY(check_handle_device(ws, h, "components"));
     PCU_ON_DEVICE(ws);
     PCU_TRY(adopt_stream(ws, stream));
     const unsigned blocks = blocks_for(std::max(h->n, h->m));
-    if (h->fkind == kIdxI64 || h->fkind == kIdxU64)
+    if (wide_index(h->fkind))
         PCU_LAUNCH(cc_emit_kernel<long long>, blocks, kThreads, stream, h->cv, h->n, h->cf, h->m, h->nv, h->nf, h->k, (long long*)out_cv,
                    (long long*)out_cf, (long long*)out_nv, (long long*)out_nf);
     else
@@ -2215,14 +2197,6 @@ int mt_check(const pcu_b200_workspace* ws, const void* v, long long nv, const vo
     if (nv >= 0x7fffffffLL || m >= 0x7fffffffLL)
         return fail(PCU_B200_INVALID_ARGUMENT, "at most 2^31 - 2 vertices and faces are supported, got %lld and %lld", nv, m);
     if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
-    return PCU_B200_OK;
-}
-
-// Reads the removal's counts (the one synchronisation) and fails on a corner out of range.
-int mt_read(MtCounts* rec, MtCounts* host, cudaStream_t stream) {
-    PCU_CUDA(cudaMemcpyAsync(host, rec, sizeof(MtCounts), cudaMemcpyDeviceToHost, stream));
-    PCU_CUDA(cudaStreamSynchronize(stream));
-    if (host->bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", host->bad);
     return PCU_B200_OK;
 }
 
@@ -2246,14 +2220,15 @@ int remove_mesh_vertices_device(pcu_b200_workspace* ws, const T* v, long long nv
     PCU_LAUNCH(rmv_vertex_kernel<T>, blocks_for(nv), kThreads, stream, v, nv, mask, (const unsigned*)sc.vcounts, out_v, sc.remap);
     PCU_LAUNCH(rmv_face_flag_kernel, blocks_for(m), kThreads, stream, f, fkind, m, nv, (const int*)sc.remap, sc.keep, sc.rec);
     PCU_TRY(enqueue_keep_offsets(sc.keep, m, sc.fcounts, &sc.rec->kept_f, stream));
-    if (fkind == kIdxI64)
+    if (wide_index(fkind))
         PCU_LAUNCH(rmv_face_emit_kernel<long long>, blocks_for(m), kThreads, stream, f, fkind, m, nv, (const unsigned char*)sc.keep,
                    (const unsigned*)sc.fcounts, (const int*)sc.remap, (long long*)out_f);
     else
         PCU_LAUNCH(rmv_face_emit_kernel<int>, blocks_for(m), kThreads, stream, f, fkind, m, nv, (const unsigned char*)sc.keep,
                    (const unsigned*)sc.fcounts, (const int*)sc.remap, (int*)out_f);
     MtCounts hc;
-    PCU_TRY(mt_read(sc.rec, &hc, stream));
+    PCU_TRY(read_record(sc.rec, &hc, stream));
+    if (hc.bad) return bad_corners(hc.bad);
     out_counts[0] = hc.kept_v;
     out_counts[1] = hc.kept_f;
     return PCU_B200_OK;
@@ -2283,12 +2258,13 @@ int remove_unreferenced_device(pcu_b200_workspace* ws, const T* v, long long nv,
     PCU_CUDA(cudaMemsetAsync(sc.used, 0, (size_t)nv, stream));
     PCU_LAUNCH(rur_mark_kernel, blocks_for(m), kThreads, stream, f, fkind, m, nv, sc.used, sc.rec);
     PCU_TRY(enqueue_keep_offsets(sc.used, nv, sc.vcounts, &sc.rec->kept_v, stream));
-    if (fkind == kIdxI64 || fkind == kIdxU64)
+    if (wide_index(fkind))
         PCU_TRY((rur_launch<T, long long>(v, nv, f, m, fkind, sc.used, sc.vcounts, out_v, out_f, out_j, out_i, stream)));
     else
         PCU_TRY((rur_launch<T, int>(v, nv, f, m, fkind, sc.used, sc.vcounts, out_v, out_f, out_j, out_i, stream)));
     MtCounts hc;
-    PCU_TRY(mt_read(sc.rec, &hc, stream));
+    PCU_TRY(read_record(sc.rec, &hc, stream));
+    if (hc.bad) return bad_corners(hc.bad);
     *out_count = hc.kept_v;
     return PCU_B200_OK;
 }
@@ -2313,14 +2289,6 @@ inline int mg_index_bits(long long n) {
     int b = 1;
     while (b < 31 && ((n - 1) >> b) != 0) ++b;
     return b;
-}
-
-// Reads the record (one synchronisation) and fails on a corner out of range.
-int mg_read(const MgRecord* rec, MgRecord* host, cudaStream_t stream) {
-    PCU_CUDA(cudaMemcpyAsync(host, rec, sizeof(MgRecord), cudaMemcpyDeviceToHost, stream));
-    PCU_CUDA(cudaStreamSynchronize(stream));
-    if (host->bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", host->bad);
-    return PCU_B200_OK;
 }
 
 // One face pass over v (T = the type of v; double for the smoothing's fp64 iterate).
@@ -2355,7 +2323,8 @@ int mesh_face_device(pcu_b200_workspace* ws, const T* v, long long nv, const voi
     if (normal) o.normal = out; else o.area = out;
     PCU_TRY(mg_face_pass<T>(v, nv, f, fkind, m, o, rec, stream));
     MgRecord host;
-    return mg_read(rec, &host, stream);
+    PCU_TRY(read_record(rec, &host, stream));
+    return host.bad ? bad_corners(host.bad) : PCU_B200_OK;
 }
 
 // estimate_mesh_vertex_normals, weighting 0 uniform, 1 area, 2 angle: face pass, corner CSR, vertex pass; one
@@ -2385,7 +2354,8 @@ int vertex_normals_device(pcu_b200_workspace* ws, const T* v, long long nv, cons
     PCU_LAUNCH(mg_vertex_normal_kernel<T>, blocks_for(nv), kThreads, stream, (const int*)sc.first, (const int*)sc.corner, nv,
                (const double*)sc.unit, (const double*)sc.weight, out);
     MgRecord host;
-    return mg_read(sc.rec, &host, stream);
+    PCU_TRY(read_record(sc.rec, &host, stream));
+    return host.bad ? bad_corners(host.bad) : PCU_B200_OK;
 }
 
 constexpr int kCgWindow = 16;   // CG iterations enqueued between two reads of the solver's record
@@ -2421,10 +2391,9 @@ struct LapScratch {
     }
 };
 
-// Reads the record (one synchronisation).
+// Reads the record (one synchronisation) and fails on a mesh of zero total area.
 int lap_read(const LapRecord* rec, LapRecord* host, cudaStream_t stream) {
-    PCU_CUDA(cudaMemcpyAsync(host, rec, sizeof(LapRecord), cudaMemcpyDeviceToHost, stream));
-    PCU_CUDA(cudaStreamSynchronize(stream));
+    PCU_TRY(read_record(rec, host, stream));
     if (host->mesh.zero_area) return fail(PCU_B200_INVALID_ARGUMENT, "laplacian_smooth_mesh: the mesh has zero total area");
     return PCU_B200_OK;
 }
@@ -2446,7 +2415,7 @@ int lap_assemble(LapScratch& s, const void* f, int fkind, long long m, long long
     if (cotan) PCU_TRY(enqueue_incidence(s.sort, f, fkind, m, nv, s.first, s.corner, stream));
     LapRecord host;
     PCU_TRY(lap_read(s.rec, &host, stream));
-    if (host.mesh.bad) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", host.mesh.bad);
+    if (host.mesh.bad) return bad_corners(host.mesh.bad);
     if (host.mesh.nonfinite)
         return fail(PCU_B200_INVALID_ARGUMENT, "laplacian_smooth_mesh: v has %llu coordinates that are not finite", host.mesh.nonfinite);
     PCU_LAUNCH(mg_rows_kernel, blocks_for(host.mesh.nnz + 1), kThreads, stream, (const MgRec*)s.rows, host.mesh.nnz, nv, s.rowptr,
@@ -3342,7 +3311,8 @@ int pcu_b200_marching_cubes_emit(pcu_b200_workspace* ws, const pcu_b200_marching
 int pcu_b200_marching_cubes_destroy(pcu_b200_marching_cubes* mc) {
     if (!mc) return PCU_B200_OK;
     DeviceGuard guard(mc->device);
-    return mc_free(mc);
+    delete mc;
+    return PCU_B200_OK;
 }
 int pcu_b200_sparse_voxel_grid_boundary(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, int64_t* out_idx,
                                         int64_t* out_counts, void* stream) {
@@ -3367,7 +3337,8 @@ int pcu_b200_voxelize_emit(pcu_b200_workspace* ws, const pcu_b200_voxelize* vx, 
 int pcu_b200_voxelize_destroy(pcu_b200_voxelize* vx) {
     if (!vx) return PCU_B200_OK;
     DeviceGuard guard(vx->device);
-    return vx_free(vx);
+    delete vx;
+    return PCU_B200_OK;
 }
 int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t seed_x,
                            int64_t seed_y, int64_t seed_z, double fill_value, void* out, void* stream) {
@@ -3385,7 +3356,8 @@ int pcu_b200_connected_components_emit(pcu_b200_workspace* ws, const pcu_b200_co
 int pcu_b200_connected_components_destroy(pcu_b200_components* cc) {
     if (!cc) return PCU_B200_OK;
     DeviceGuard guard(cc->device);
-    return cc_free(cc);
+    delete cc;
+    return PCU_B200_OK;
 }
 int pcu_b200_remove_mesh_vertices_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
                                       const uint8_t* mask, float* out_v, void* out_f, int64_t out_counts[2], void* stream) {
