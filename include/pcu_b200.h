@@ -592,6 +592,11 @@ int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_ki
  *     (all ones for the unsigned kinds) elsewhere; out_f (nf, 3) = I[f]; all in f's width.  Synchronises `stream`
  *     once; *out_count = #J (host int64).
  *   For both removals 1 <= nv, nf < 2^31 - 1, and a corner outside [0, nv) fails with PCU_B200_INVALID_ARGUMENT.
+ *   orient_mesh_faces (the reference's src/orient_mesh_faces.cpp, libigl's bfs_orient): f (nf, 3) of any index kind,
+ *     1 <= nf <= 2^30 - 1.  Ids are only compared for equality, so every value is legal.  out_f (nf, 3) receives the
+ *     rows, consistently oriented within each patch (faces joined by edges that no third face has), and
+ *     out_components (nf) each face's patch, patch j being the j-th in ascending order of its smallest face; both in
+ *     f's width.  Never synchronises `stream`.
  * Every array pointer is a DEVICE pointer. */
 typedef struct pcu_b200_components pcu_b200_components;
 int pcu_b200_connected_components_prepare(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_cols, int f_kind,
@@ -609,6 +614,8 @@ int pcu_b200_remove_unreferenced_mesh_vertices_f32(pcu_b200_workspace* ws, const
 int pcu_b200_remove_unreferenced_mesh_vertices_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
                                                    double* out_v, void* out_f, void* out_corr_v, void* out_corr_f, int64_t* out_count,
                                                    void* stream);
+int pcu_b200_orient_mesh_faces(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, void* out_f, void* out_components,
+                               void* stream);
 
 /* ---- mesh normals, face areas and Laplacian smoothing ------------------------------------------------------------
  * Replace mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals and laplacian_smooth_mesh (the

@@ -1,6 +1,7 @@
-"""connected_components, remove_mesh_vertices and remove_unreferenced_mesh_vertices -- the reference's names, arguments
-and outputs (the reference's src/connected_components.cpp, src/remove_mesh_vertices.cpp and
-src/remove_unreferenced_mesh_vertices.cpp), computed by csrc/mesh_topology.cuh.
+"""connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices and orient_mesh_faces -- the
+reference's names, arguments and outputs (the reference's src/connected_components.cpp, src/remove_mesh_vertices.cpp,
+src/remove_unreferenced_mesh_vertices.cpp and src/orient_mesh_faces.cpp), computed by csrc/mesh_topology.cuh and
+csrc/orient.cuh.
 
 numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA torch tensors in -> CUDA tensors out;
 CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages and in its order, before any
@@ -157,3 +158,54 @@ def remove_unreferenced_mesh_vertices(v, f, *, device=None):
         return v_out[:kept], f_out, corr_v[:kept], corr_f
 
     return _run(form, [v, f], device, body, index=(f, [1, 2, 3]), squeeze=True)
+
+
+_MAX_ORIENT_FACES = 2 ** 30 - 1
+
+
+def orient_mesh_faces(f, weighting_type="uniform", *, device=None):
+    """
+    Consistently orient faces of a mesh within each connected component
+
+    Args:
+        f : (#f, 3)-shaped NumPy array of face (triangle) indices
+        weighting_type : accepted for the reference's signature and ignored (the reference never reads it)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        oriented_faces  : (#f, 3)-shaped NumPy array of faces which are consistently oriented
+        face_components : (#f,)-shaped NumPy array of connected component ids (i.e. face_components[i] is the component id of facef[i])
+
+    Dtypes: f int32 / int64 / uint32 / uint64; both outputs have f's dtype.  Defined in DESIGN.md §3 as libigl's
+    bfs_orient computes it: two faces are adjacent when they share an undirected edge that no third face has, and the
+    components are the patches this adjacency connects, numbered in ascending order of their smallest face.  Each patch
+    is walked breadth-first from its smallest face, which is never flipped; a neighbour is reversed ((a, b, c) becomes
+    (c, b, a)) whenever one of its directed edges equals one of the current face's.  Ids are only compared for
+    equality, never used as indices, so any value (negative ones included) is legal and no vertex array is needed.
+    Shapes squeezed as npe::move squeezes them: one face gives oriented_faces of shape (3,) and a 0-d face_components.
+    A CUDA-tensor call never synchronises the host.
+    Divergence: more than 2^30 - 1 faces raise ValueError.
+    """
+    form = _form([f], ["f"])
+    _check_index(f, "f", _INDEX_KINDS)
+    if len(f.shape) not in (1, 2):
+        raise ValueError("orient_mesh_faces: f must be a 1-D or 2-D array, got shape %s" % (tuple(f.shape),))
+    rows, cols = _matrix_shape(f)
+    if rows == 0:
+        raise ValueError("Invalid input faces with zero elements: f must have shape (n, 3) where n > 0. Got f.shape =(%d, %d)."
+                         % (rows, cols))
+    if cols != 3:
+        raise ValueError("Only triangle inputs are supported: f must have shape (n, 3) where n > 0. Got f.shape =(%d, %d)."
+                         % (rows, cols))
+    if rows > _MAX_ORIENT_FACES:
+        raise ValueError("orient_mesh_faces: at most 2^30 - 1 faces are supported, got %d" % rows)
+    torch = _torch()
+
+    def body(ft, dev, stream):
+        out_f = torch.empty((rows, 3), dtype=ft.dtype, device=ft.device)
+        out_c = torch.empty(rows, dtype=ft.dtype, device=ft.device)
+        _pcu_internal._orient_mesh_faces_device(ft.data_ptr(), rows, _INDEX_KINDS[_dtype_name(f)], out_f.data_ptr(), out_c.data_ptr(),
+                                                dev, stream)
+        return out_f, out_c
+
+    return _run(form, [f], device, body, index=(f, [0, 1]), squeeze=True)

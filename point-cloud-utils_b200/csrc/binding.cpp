@@ -796,6 +796,12 @@ int64_t remove_unreferenced_device(bool is_f64, uintptr_t v, int64_t nv, uintptr
     });
     return kept;
 }
+// orient_mesh_faces: out_f (nf, 3) and out_components (nf) in f's width; no synchronisation.
+void orient_mesh_faces_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t out_f, uintptr_t out_components, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_orient_mesh_faces(ws, (const void*)f, nf, f_kind, (void*)out_f, (void*)out_components, (void*)stream);
+    });
+}
 
 // mesh_face_areas (normal false) / estimate_mesh_face_normals (normal true): out (nf) or (nf, 3) in v's type; one
 // synchronisation.
@@ -1258,6 +1264,7 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_connected_components_destroy", &connected_components_destroy);
     mod.def("_remove_mesh_vertices_device", &remove_mesh_vertices_device);
     mod.def("_remove_unreferenced_device", &remove_unreferenced_device);
+    mod.def("_orient_mesh_faces_device", &orient_mesh_faces_device);
     mod.def("_mesh_face_device", &mesh_face_device);
     mod.def("_mesh_vertex_normals_device", &mesh_vertex_normals_device);
     mod.def("_laplacian_smooth_device", &laplacian_smooth_device);

@@ -40,6 +40,7 @@
 #include "sparse_voxels.cuh"
 #include "voxelize.cuh"
 #include "mesh_topology.cuh"
+#include "orient.cuh"
 #include "laplacian.cuh"
 
 using namespace pcu;
@@ -2269,6 +2270,51 @@ int remove_unreferenced_device(pcu_b200_workspace* ws, const T* v, long long nv,
     return PCU_B200_OK;
 }
 
+// ---- consistent face orientation (orient.cuh) ----------------------------------------------------------------------
+// K = the half-edge records' word, I = f's width.  Every buffer is sized by m: no synchronisation.
+template <typename K, typename I>
+int orient_launch(pcu_b200_workspace* ws, const void* f, long long m, int fkind, I* out_f, I* out_c, cudaStream_t stream) {
+    using Rec = OmRec<K>;
+    const long long n = 3 * m;
+    struct { SortScratch<Rec> sort; int *P, *nb, *root, *rank, *next; unsigned char *flag, *enq; unsigned* counts; long long* seeds; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.sort.carve(cv, n);
+        sc.P = cv.take<int>(2 * (size_t)m);
+        sc.nb = cv.take<int>((size_t)n);
+        sc.root = cv.take<int>((size_t)m);
+        sc.rank = cv.take<int>((size_t)m);
+        sc.next = cv.take<int>((size_t)m);
+        sc.flag = cv.take<unsigned char>((size_t)m);
+        sc.enq = cv.take<unsigned char>((size_t)m);
+        sc.counts = cv.take<unsigned>(keep_count_words(m));
+        sc.seeds = cv.take<long long>(1);
+    }));
+    PCU_CUDA(cudaMemsetAsync(sc.nb, 0xff, sizeof(int) * (size_t)n, stream));
+    PCU_CUDA(cudaMemsetAsync(sc.enq, 0, (size_t)m, stream));
+    PCU_LAUNCH(om_records_kernel<K>, blocks_for(m), kThreads, stream, f, fkind, m, sc.sort.a, sc.P);
+    Rec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(sc.sort, n, 2, stream, &sorted));
+    PCU_LAUNCH(om_runs_kernel<K>, blocks_for(n), kThreads, stream, (const Rec*)sorted, n, m, f, fkind, sc.nb, sc.P);
+    PCU_LAUNCH(om_flatten_kernel, blocks_for(m), kThreads, stream, sc.P, m, sc.root, sc.flag);
+    PCU_TRY(enqueue_keep_offsets(sc.flag, m, sc.counts, sc.seeds, stream));
+    PCU_LAUNCH(cc_rank_kernel, blocks_for(m), kThreads, stream, (const unsigned char*)sc.flag, m, (const unsigned*)sc.counts, sc.rank);
+    PCU_LAUNCH(om_emit_kernel<I>, blocks_for(m), kThreads, stream, (const I*)f, m, (const int*)sc.root, (const int*)sc.rank, out_f, out_c);
+    PCU_LAUNCH(om_replay_kernel<I>, blocks_for(m), kThreads, stream, (const unsigned char*)sc.flag, m, (const int*)sc.nb, sc.enq, sc.next,
+               out_f);
+    return PCU_B200_OK;
+}
+
+int orient_mesh_faces_device(pcu_b200_workspace* ws, const void* f, long long m, int fkind, void* out_f, void* out_c, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!f || !out_f || !out_c) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (m <= 0 || m > kOmMaxFaces)
+        return fail(PCU_B200_INVALID_ARGUMENT, "orient_mesh_faces: between 1 and 2^30 - 1 faces are supported, got %lld", m);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    PCU_ON_DEVICE(ws);
+    return wide_index(fkind) ? orient_launch<unsigned long long, long long>(ws, f, m, fkind, (long long*)out_f, (long long*)out_c, stream)
+                             : orient_launch<unsigned, int>(ws, f, m, fkind, (int*)out_f, (int*)out_c, stream);
+}
+
 // ---- mesh normals, face areas and Laplacian smoothing (mesh_geometry.cuh, laplacian.cuh) ---------------------------
 // Arguments shared by the four entry points.  6 m records must fit int32 positions.
 int mg_check(const pcu_b200_workspace* ws, const void* v, long long nv, const void* f, long long m, int fkind, const void* out) {
@@ -3378,6 +3424,10 @@ int pcu_b200_remove_unreferenced_mesh_vertices_f64(pcu_b200_workspace* ws, const
                                                    void* stream) {
     return remove_unreferenced_device<double>(ws, v, nv, f, nf, f_kind, out_v, out_f, out_corr_v, out_corr_f, (long long*)out_count,
                                               (cudaStream_t)stream);
+}
+int pcu_b200_orient_mesh_faces(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, void* out_f, void* out_components,
+                               void* stream) {
+    return orient_mesh_faces_device(ws, f, nf, f_kind, out_f, out_components, (cudaStream_t)stream);
 }
 
 int pcu_b200_mesh_face_areas_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, float* out_areas,

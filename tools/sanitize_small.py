@@ -76,6 +76,8 @@ step("connected components", lambda: pcu.connected_components(mv, np.concatenate
 step("connected components uint64 edges", lambda: pcu.connected_components(mv.astype(np.float32), tf.astype(np.uint64)))
 step("remove mesh vertices", lambda: pcu.remove_mesh_vertices(mv, mf, rng.random(200) < 0.7))
 step("remove unreferenced vertices fp32 / uint32", lambda: pcu.remove_unreferenced_mesh_vertices(mv.astype(np.float32), mf[:50].astype(np.uint32)))
+step("orient mesh faces", lambda: pcu.orient_mesh_faces(np.concatenate([mf, mf[::-1, ::-1] + 205])))
+step("orient mesh faces uint64, repeated corners (replayed)", lambda: pcu.orient_mesh_faces(rng.integers(0, 12, (60, 3)).astype(np.uint64)))
 step("mesh face areas", lambda: pcu.mesh_face_areas(mv, mf))
 step("face normals fp32 / uint32", lambda: pcu.estimate_mesh_face_normals(mv.astype(np.float32), mf.astype(np.uint32)))
 step("vertex normals area", lambda: pcu.estimate_mesh_vertex_normals(mv, mf, "area"))
