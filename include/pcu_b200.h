@@ -536,6 +536,48 @@ int pcu_b200_marching_cubes_destroy(pcu_b200_marching_cubes* mc);
 int pcu_b200_sparse_voxel_grid_boundary(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, int64_t* out_idx,
                                         int64_t* out_counts, void* stream);
 
+/* ---- sparse voxel grids: from points, dilation, erosion, hex mesh; voxel cube meshes --------------------------------
+ * Replace sparse_voxel_grid_from_pointcloud, dilate_sparse_voxel_grid, erode_sparse_voxel_grid and
+ * sparse_voxel_grid_to_hex_mesh (the reference's src/sparse_voxel_grid.cpp:78-460) and voxel_grid_geometry
+ * (src/mesh_for_voxels.cpp).  Results, and the three divergences from the reference's bindings (all 26 neighbours,
+ * per-axis half voxel, shape check), are defined in DESIGN.md §3.  Voxels are identified by 64-bit Morton codes of
+ * their int32 coordinates; grids are int32 (idx_kind I32) or int64 (I64) rows, n >= 1; a coordinate outside
+ * [INT32_MIN + 1, INT32_MAX - 1] (and any unsigned grid) fails with PCU_B200_INVALID_ARGUMENT and the reference's
+ * message "Invalid vertex leads to an overflow integer. ...".
+ *   sparse_grid_from_points: points (n, 3) in the suffix's type, n < 2^31 - 1, voxel_size and origin host arrays of 3;
+ *     voxel index round((p - o) / s) per axis in fp64.  Synchronises `stream` once; *out_counts = {distinct voxels u,
+ *     n} (host int64).
+ *   sparse_grid_dilate_prepare: one dilation round of an (n, 3) grid, n <= 82 595 524 (26 n flags are ranked in 32
+ *     bits).  Synchronises `stream` once; *out_counts = {rows of the result, new rows}.  grid must stay alive until emit.
+ *   sparse_grid_hex_prepare: the hex mesh of an (n, 3) grid, n < 2^28; vertices in double (vertices_f64) or float.
+ *     Synchronises `stream` once; *out_counts = {#v, 8 n}.
+ *   sparse_grid_emit: from points: out_rows (u, 3) int32 grid, out_index (n) int64 point_to_vox; dilation: out_rows
+ *     (n + new, 3) of the grid's kind (the input rows, then the new ones), out_index unused; hex mesh: out_rows (#v, 3)
+ *     vertices, out_index (n, 8) int64 cubes.  Stream-ordered.
+ *   sparse_grid_destroy: frees a prepared handle, stream-ordered on the stream it was prepared on.
+ *   sparse_grid_erode: one erosion round of an (n, 3) grid, n < 2^31 - 1: out_grid (capacity n rows, the grid's kind)
+ *     receives the kept rows in order, out_counts[0] (device int64) their number and out_counts[1] the rows out of
+ *     range (then the output is unspecified).  Stream-ordered, no synchronisation.
+ *   voxel_grid_geometry: ijk (n, 3) of any index kind, 1 <= n <= 2^28, voxel_size > 0 (NaN passes, as in the
+ *     reference); out_v (8 n, 3) float and out_f (12 n, 3) int32.  Stream-ordered, no synchronisation.
+ * Every array pointer is a DEVICE pointer. */
+typedef struct pcu_b200_sparse_grid pcu_b200_sparse_grid;
+int pcu_b200_sparse_grid_from_points_f32(pcu_b200_workspace* ws, const float* points, int64_t n, const double voxel_size[3],
+                                         const double origin[3], pcu_b200_sparse_grid** out_grid, int64_t out_counts[2], void* stream);
+int pcu_b200_sparse_grid_from_points_f64(pcu_b200_workspace* ws, const double* points, int64_t n, const double voxel_size[3],
+                                         const double origin[3], pcu_b200_sparse_grid** out_grid, int64_t out_counts[2], void* stream);
+int pcu_b200_sparse_grid_dilate_prepare(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, pcu_b200_sparse_grid** out_grid,
+                                        int64_t out_counts[2], void* stream);
+int pcu_b200_sparse_grid_hex_prepare(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, const double voxel_size[3],
+                                     const double origin[3], int vertices_f64, pcu_b200_sparse_grid** out_grid, int64_t out_counts[2],
+                                     void* stream);
+int pcu_b200_sparse_grid_emit(pcu_b200_workspace* ws, const pcu_b200_sparse_grid* sg, void* out_rows, int64_t* out_index, void* stream);
+int pcu_b200_sparse_grid_destroy(pcu_b200_sparse_grid* sg);
+int pcu_b200_sparse_grid_erode(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, void* out_grid, int64_t* out_counts,
+                               void* stream);
+int pcu_b200_voxel_grid_geometry(pcu_b200_workspace* ws, const void* ijk, int64_t n, int idx_kind, const double voxel_size[3],
+                                 const double voxel_origin[3], double gap_fraction, float* out_v, int32_t* out_f, void* stream);
+
 /* ---- triangle-mesh voxelization and 3-D flood fill -----------------------------------------------------------------
  * Replace voxelize_triangle_mesh and flood_fill_3d (the reference's point_cloud_utils/_voxels.py,
  * src/voxelize_triangle_mesh.cpp, src/flood_fill_3d.cpp).  Results defined in DESIGN.md §3.

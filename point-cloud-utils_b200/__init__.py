@@ -45,7 +45,9 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "ray_mesh_intersection", "RayMeshIntersector",
            "ray_surfel_intersection", "RaySurfelIntersector", "pointcloud_surfel_geometry",
            "marching_cubes_sparse_voxel_grid", "sparse_voxel_grid_boundary",
-           "voxelize_triangle_mesh", "flood_fill_3d",
+           "sparse_voxel_grid_from_pointcloud", "dilate_sparse_voxel_grid", "erode_sparse_voxel_grid",
+           "sparse_voxel_grid_to_hex_mesh",
+           "voxelize_triangle_mesh", "flood_fill_3d", "voxel_grid_geometry",
            "connected_components", "remove_mesh_vertices", "remove_unreferenced_mesh_vertices", "orient_mesh_faces",
            "mesh_face_areas", "estimate_mesh_face_normals", "estimate_mesh_vertex_normals", "laplacian_smooth_mesh",
            "deduplicate_point_cloud",
@@ -783,7 +785,9 @@ from ._mesh_query import (closest_points_on_mesh, triangle_soup_fast_winding_num
 from ._ray_mesh import ray_mesh_intersection, RayMeshIntersector  # noqa: E402
 from ._ray_surfel import ray_surfel_intersection, RaySurfelIntersector, pointcloud_surfel_geometry  # noqa: E402
 from ._sparse_voxels import marching_cubes_sparse_voxel_grid, sparse_voxel_grid_boundary  # noqa: E402
-from ._voxels import voxelize_triangle_mesh, flood_fill_3d  # noqa: E402
+from ._sparse_voxels import (sparse_voxel_grid_from_pointcloud, dilate_sparse_voxel_grid, erode_sparse_voxel_grid,  # noqa: E402
+                             sparse_voxel_grid_to_hex_mesh)
+from ._voxels import voxelize_triangle_mesh, flood_fill_3d, voxel_grid_geometry  # noqa: E402
 from ._mesh_topology import (connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices,  # noqa: E402
                              orient_mesh_faces)
 from ._mesh_geometry import mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals, laplacian_smooth_mesh  # noqa: E402

@@ -1,5 +1,7 @@
-"""voxelize_triangle_mesh and flood_fill_3d -- the reference's names, arguments and outputs (the reference's
-point_cloud_utils/_voxels.py, src/voxelize_triangle_mesh.cpp and src/flood_fill_3d.cpp), computed by csrc/voxelize.cuh.
+"""voxelize_triangle_mesh, flood_fill_3d and voxel_grid_geometry -- the reference's names, arguments and outputs (the
+reference's point_cloud_utils/_voxels.py, src/voxelize_triangle_mesh.cpp, src/flood_fill_3d.cpp,
+point_cloud_utils/_point_cloud_geometry.py and src/mesh_for_voxels.cpp), computed by csrc/voxelize.cuh and
+csrc/sparse_voxels.cuh.
 
 numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA torch tensors in -> CUDA tensors out;
 CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages and in its order, before any
@@ -7,10 +9,11 @@ device call."""
 import numpy as np
 
 from . import _pcu_internal
-from ._call import _INDEX_KINDS, _check_index, _dtype_name, _form, _run, _torch, _validate_mesh
+from ._call import _INDEX_KINDS, _check_index, _dtype_name, _form, _matrix_shape, _run, _torch, _validate_mesh
 
 _GRID_KINDS = {"int32": 0, "int64": 1, "float32": 2, "float64": 3}
 _MAX_VOXELS = 2 ** 31
+_MAX_CUBES = 2 ** 28                      # voxel_grid_geometry's int32 faces index 8 vertices per voxel
 
 
 def _coord3d_to_array(coord, dtype=np.float64):
@@ -131,3 +134,58 @@ def voxelize_triangle_mesh(v, f, voxel_size, voxel_origin, *, device=None):
         return ijk
 
     return _run(form, [v, f], device, body)
+
+
+def voxel_grid_geometry(ijk, voxel_size=np.array((1., 1., 1.)), voxel_origin=np.array((0., 0., 0.)), gap_fraction=0.0, *,
+                        device=None):
+    """
+    Generate a triangle mesh of cubes for voxel coordinates ijk. The [0, 0, 0] voxel has its
+    low corner at voxel_origin and each voxel has voxel_size.
+
+    Args:
+        ijk np.ndarray: [num_voxels, 3] array of integer voxel coordinates
+        voxel_size: Float or triple representing the size of each voxel.
+                    Defaults to np.array((1., 1., 1.)).
+        voxel_origin: Low corner of the [0, 0, 0] voxel. Defaults to np.array((0., 0., 0.)).
+        gap_fraction: Fraction of a voxel to leave as a gap between voxels (default 0.0)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        v: Numpy array of vertices for the cube mesh
+        f: Numpy array of faces for the cube mesh
+
+    Dtypes: ijk int32 / int64 / uint32 / uint64; v float32 (8 n, 3), f int32 (12 n, 3).  Bit for bit the reference's
+    (src/mesh_for_voxels.cpp): voxel i contributes 8 vertices and 12 faces in the order of the reference's tables;
+    component k of table corner c (0 or 1) is float((((c * (1 - gap) + 0.5 gap) + ijk_k) * s_k) + o_k), each
+    operation rounded in fp64 (uint64 indices convert as unsigned), and face j of voxel i is the table's face j plus
+    8 i.  The origin is therefore the LOW corner of voxel (0, 0, 0), as the reference's code computes it (its
+    description says the centre): cubes drawn for voxelize_triangle_mesh's output with the same origin, which centres
+    voxel (i, j, k) at o + (i, j, k) s, sit half a voxel off.  A voxel size <= 0 raises ValueError("Voxel size must be
+    positive") (NaN passes, as in the reference).  At most 2^28 voxels (the int32 face indices overflow beyond).
+    """
+    voxel_origin = _coord3d_to_array(voxel_origin, dtype=np.float64)
+    voxel_size = _number_or_coord3d_to_array(voxel_size, dtype=np.float64)
+    form = _form([ijk], ["ijk"])
+    _check_index(ijk, "ijk", _INDEX_KINDS)
+    gap_fraction = float(gap_fraction)
+    rows, cols = _matrix_shape(ijk)
+    if rows == 0:
+        raise ValueError("Invalid input point cloud with zero points: points must have shape (n, 3) (n > 0). "
+                         "Got points.shape =(%d, %d)." % (rows, cols))
+    if cols != 3:
+        raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). "
+                         "Got points.shape =(%d, %d)." % (rows, cols))
+    if voxel_size[0] <= 0.0 or voxel_size[1] <= 0.0 or voxel_size[2] <= 0.0:
+        raise ValueError("Voxel size must be positive")
+    if rows > _MAX_CUBES:
+        raise ValueError("voxel_grid_geometry: at most 2^28 voxels are supported, got %d" % rows)
+    torch = _torch()
+
+    def body(it, dev, stream):
+        v = torch.empty((8 * rows, 3), dtype=torch.float32, device=it.device)
+        f = torch.empty((12 * rows, 3), dtype=torch.int32, device=it.device)
+        _pcu_internal._voxel_grid_geometry_device(it.data_ptr(), rows, _INDEX_KINDS[_dtype_name(ijk)], voxel_size.tolist(),
+                                                  voxel_origin.tolist(), gap_fraction, v.data_ptr(), f.data_ptr(), dev, stream)
+        return v, f
+
+    return _run(form, [ijk], device, body, squeeze=True)

@@ -714,6 +714,65 @@ void sparse_voxel_grid_boundary_device(uintptr_t grid, int64_t n, int idx_kind, 
     });
 }
 
+// Sparse voxel grids (_sparse_voxels.py): one code-set handle, prepared from points, by a dilation round or from a grid's
+// cube corners (one synchronisation of `stream` each), returns (handle, rows, records); _sparse_grid_emit writes the
+// outputs; _sparse_grid_destroy.
+py::tuple sparse_grid_from_points_device(bool is_f64, uintptr_t points, int64_t n, std::vector<double> size, std::vector<double> origin,
+                                         int device, uintptr_t stream) {
+    if (size.size() != 3 || origin.size() != 3) throw py::value_error("Invalid shape");
+    pcu_b200_sparse_grid* sg = nullptr;
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_sparse_grid_from_points_f64(ws, (const double*)points, n, size.data(), origin.data(), &sg, counts, (void*)stream)
+                      : pcu_b200_sparse_grid_from_points_f32(ws, (const float*)points, n, size.data(), origin.data(), &sg, counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)sg, counts[0], counts[1]);
+}
+py::tuple sparse_grid_dilate_prepare_device(uintptr_t grid, int64_t n, int idx_kind, int device, uintptr_t stream) {
+    pcu_b200_sparse_grid* sg = nullptr;
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_sparse_grid_dilate_prepare(ws, (const void*)grid, n, idx_kind, &sg, counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)sg, counts[0], counts[1]);
+}
+py::tuple sparse_grid_hex_prepare_device(uintptr_t grid, int64_t n, int idx_kind, std::vector<double> size, std::vector<double> origin,
+                                         bool vertices_f64, int device, uintptr_t stream) {
+    if (size.size() != 3 || origin.size() != 3) throw py::value_error("Invalid shape");
+    pcu_b200_sparse_grid* sg = nullptr;
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_sparse_grid_hex_prepare(ws, (const void*)grid, n, idx_kind, size.data(), origin.data(), vertices_f64 ? 1 : 0, &sg,
+                                                counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)sg, counts[0], counts[1]);
+}
+void sparse_grid_emit_device(uintptr_t sg, uintptr_t out_rows, uintptr_t out_index, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_sparse_grid_emit(ws, (const pcu_b200_sparse_grid*)sg, (void*)out_rows, (int64_t*)out_index, (void*)stream);
+    });
+}
+void sparse_grid_destroy(uintptr_t sg) {
+    py::gil_scoped_release nogil;
+    pcu_b200_sparse_grid_destroy((pcu_b200_sparse_grid*)sg);
+}
+// erode_sparse_voxel_grid: out_grid (capacity n rows, the grid's kind), out_counts: two device int64 {kept rows, rows out
+// of range}.
+void sparse_grid_erode_device(uintptr_t grid, int64_t n, int idx_kind, uintptr_t out_grid, uintptr_t out_counts, int device, uintptr_t stream) {
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_sparse_grid_erode(ws, (const void*)grid, n, idx_kind, (void*)out_grid, (int64_t*)out_counts, (void*)stream);
+    });
+}
+// voxel_grid_geometry (_voxels.py): out_v (8 n, 3) float32, out_f (12 n, 3) int32; no synchronisation.
+void voxel_grid_geometry_device(uintptr_t ijk, int64_t n, int idx_kind, std::vector<double> size, std::vector<double> origin, double gap,
+                                uintptr_t out_v, uintptr_t out_f, int device, uintptr_t stream) {
+    if (size.size() != 3 || origin.size() != 3) throw py::value_error("Invalid shape");
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_voxel_grid_geometry(ws, (const void*)ijk, n, idx_kind, size.data(), origin.data(), gap, (float*)out_v,
+                                            (int32_t*)out_f, (void*)stream);
+    });
+}
+
 // Voxelization (voxelize_triangle_mesh, _voxels.py): tests and sorts (two synchronisations of `stream`), returns
 // (handle, n, accepted (face, voxel) pairs); _voxelize_emit writes the (n, 3) int32 voxels; _voxelize_destroy.
 py::tuple voxelize_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, std::vector<double> size,
@@ -1255,6 +1314,13 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_marching_cubes_emit_device", &marching_cubes_emit_device);
     mod.def("_marching_cubes_destroy", &marching_cubes_destroy);
     mod.def("_sparse_voxel_grid_boundary_device", &sparse_voxel_grid_boundary_device);
+    mod.def("_sparse_grid_from_points_device", &sparse_grid_from_points_device);
+    mod.def("_sparse_grid_dilate_prepare_device", &sparse_grid_dilate_prepare_device);
+    mod.def("_sparse_grid_hex_prepare_device", &sparse_grid_hex_prepare_device);
+    mod.def("_sparse_grid_emit_device", &sparse_grid_emit_device);
+    mod.def("_sparse_grid_destroy", &sparse_grid_destroy);
+    mod.def("_sparse_grid_erode_device", &sparse_grid_erode_device);
+    mod.def("_voxel_grid_geometry_device", &voxel_grid_geometry_device);
     mod.def("_voxelize_prepare_device", &voxelize_prepare_device);
     mod.def("_voxelize_emit_device", &voxelize_emit_device);
     mod.def("_voxelize_destroy", &voxelize_destroy);

@@ -320,6 +320,25 @@ struct pcu_b200_components : StreamHandle {
     const int* nf = nullptr;
     ~pcu_b200_components() { release(block); }
 };
+// A sparse voxel grid's code set between pcu_b200_sparse_grid_*_prepare and pcu_b200_sparse_grid_emit: the sorted code
+// records, their run heads, the heads' block offsets and the count record, in one block.  Prepared from points, by a
+// dilation round or from a grid's cube corners; the mode says what emit writes.
+struct SvgCounts { long long rows; unsigned long long bad; };
+struct pcu_b200_sparse_grid : StreamHandle {
+    int mode = 0;                           // SvgMode
+    int out_kind = 0;                       // dilation: the grid's index kind; hex mesh: vertices in double (1) or float (0)
+    const void* grid = nullptr;             // dilation: the input rows, which emit copies ahead of the new ones
+    long long n = 0;                        // input rows (points or voxels)
+    long long recs = 0;                     // sorted records
+    long long rows = 0;                     // distinct codes: grid rows, new rows or vertices
+    SvgPlace place{};
+    unsigned char* block = nullptr;
+    const McRec* sorted = nullptr;
+    unsigned char* head = nullptr;          // nullptr: the records are distinct already (dilation)
+    unsigned* offsets = nullptr;
+    SvgCounts* counts = nullptr;
+    ~pcu_b200_sparse_grid() { release(block); }
+};
 template <typename T> KdReplayBuffers<T>& cloud_tree(pcu_b200_cloud* c);
 template <> KdReplayBuffers<float>& cloud_tree<float>(pcu_b200_cloud* c) { return c->kd32; }
 template <> KdReplayBuffers<double>& cloud_tree<double>(pcu_b200_cloud* c) { return c->kd64; }
@@ -1958,6 +1977,232 @@ int sparse_voxel_grid_boundary_device(pcu_b200_workspace* ws, const void* g, lon
                            : svb_device<int>(ws, (const int*)g, n, out_idx, out_counts, stream);
 }
 
+// ---- sparse voxel grids and voxel cube meshes (sparse_voxels.cuh) -------------------------------------------------
+enum SvgMode { kSvgPoints = 0, kSvgDilate = 1, kSvgHex = 2 };
+// Dilation ranks 26 flags per voxel, the hex mesh 8 corners per voxel, in 32 bits (compact.cuh: fewer than 2^31 rows);
+// voxel_grid_geometry's int32 faces index 8 n vertices.
+constexpr long long kSvgMaxDilate = (0x7ffffffeLL) / 26;   // 82 595 524
+constexpr long long kSvgMaxHex = (0x7ffffffeLL) / 8;       // 2^28 - 1
+constexpr long long kVgMaxVoxels = 1LL << 28;
+
+int svg_overflow() {
+    return fail(PCU_B200_INVALID_ARGUMENT, "Invalid vertex leads to an overflow integer. Perhaps grid_size is too small.");
+}
+
+// The handle's block for `recs` records: sort scratch, run heads (unless the records are distinct), block offsets, the
+// count record.  The caller writes the records into sort.a.
+int svg_alloc(pcu_b200_sparse_grid* h, long long recs, bool heads, SortScratch<McRec>& sort, cudaStream_t stream) {
+    h->recs = recs;
+    const auto carve = [&](Carver& cv) {
+        sort.carve(cv, recs);
+        h->head = heads ? cv.take<unsigned char>((size_t)recs) : nullptr;
+        h->offsets = cv.take<unsigned>(keep_count_words(recs));
+        h->counts = cv.take<SvgCounts>(1);
+    };
+    PCU_TRY(alloc_block(h->block, carve_at(nullptr, carve), stream, "sparse voxel grid"));
+    carve_at(h->block, carve);
+    PCU_CUDA(cudaMemsetAsync(h->counts, 0, sizeof(SvgCounts), stream));
+    return PCU_B200_OK;
+}
+
+// Sorts the records, numbers their runs (the count of distinct codes into h->counts->rows) and, when read, reads the
+// count record: one synchronisation of `stream`.
+int svg_sort_runs(pcu_b200_sparse_grid* h, const SortScratch<McRec>& sort, bool read, cudaStream_t stream) {
+    McRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(sort, h->recs, 1, stream, &sorted));
+    h->sorted = sorted;
+    if (h->head) {
+        PCU_LAUNCH(mc_heads_kernel, blocks_for(h->recs), kThreads, stream, (const McRec*)sorted, h->recs, h->head);
+        PCU_TRY(enqueue_keep_offsets(h->head, h->recs, h->offsets, &h->counts->rows, stream));
+    }
+    if (!read) return PCU_B200_OK;
+    SvgCounts c;
+    PCU_TRY(read_record(h->counts, &c, stream));
+    if (c.bad) return svg_overflow();
+    h->rows = c.rows;
+    return PCU_B200_OK;
+}
+
+// A grid argument of the sparse-grid entry points: int32 or int64 (unsigned grids fail the reference's range check).
+int svg_check_grid(const void* g, long long n, int kind, long long most, const char* what) {
+    if (!g || n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid grid_coordinates has zero rows!");
+    if (n > most) return fail(PCU_B200_INVALID_ARGUMENT, "%s: at most %lld voxels are supported, got %lld", what, most, n);
+    if (kind != kIdxI32 && kind != kIdxI64) return svg_overflow();
+    return PCU_B200_OK;
+}
+
+template <typename T>
+int svg_points_prepare(pcu_b200_workspace* ws, const T* p, long long n, const double size[3], const double origin[3],
+                       pcu_b200_sparse_grid** out, long long* out_counts, cudaStream_t stream) {
+    if (!ws || !out || !out_counts || !size || !origin) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    if (!p || n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid points has zero rows!");
+    if (n >= 0x7fffffffLL)
+        return fail(PCU_B200_INVALID_ARGUMENT, "sparse_voxel_grid_from_pointcloud: at most 2^31 - 2 points are supported, got %lld", n);
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_sparse_grid* h) -> int {
+        h->mode = kSvgPoints; h->n = n;
+        for (int a = 0; a < 3; ++a) { h->place.g[a] = size[a]; h->place.o[a] = origin[a]; }
+        SortScratch<McRec> sort;
+        PCU_TRY(svg_alloc(h, n, true, sort, stream));
+        PCU_LAUNCH((svg_point_codes_kernel<T>), blocks_for(n), kThreads, stream, p, n, h->place, sort.a, &h->counts->bad);
+        return svg_sort_runs(h, sort, true, stream);
+    }));
+    out_counts[0] = (*out)->rows;
+    out_counts[1] = (*out)->recs;
+    return PCU_B200_OK;
+}
+
+// One dilation round: the input's codes and their sort, the owned missing neighbours' flags and their count (read:
+// one synchronisation), then the owned codes, compacted and sorted.
+template <typename I>
+int svg_dilate_build(pcu_b200_workspace* ws, pcu_b200_sparse_grid* h, const I* g, long long n, cudaStream_t stream) {
+    const long long slots = 26 * n;
+    struct { SortScratch<McRec> sort; unsigned char* flag; unsigned* counts; SvgCounts* rec; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.sort.carve(cv, n);
+        sc.flag = cv.take<unsigned char>((size_t)slots);
+        sc.counts = cv.take<unsigned>(keep_count_words(slots));
+        sc.rec = cv.take<SvgCounts>(1);
+    }));
+    PCU_CUDA(cudaMemsetAsync(sc.rec, 0, sizeof(SvgCounts), stream));
+    PCU_LAUNCH((svb_codes_kernel<I>), blocks_for(n), kThreads, stream, g, n, sc.sort.a, &sc.rec->bad);
+    McRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(sc.sort, n, 1, stream, &sorted));
+    PCU_LAUNCH(svg_dilate_flag_kernel, blocks_for(n), kThreads, stream, (const McRec*)sorted, n, sc.flag);
+    PCU_TRY(enqueue_keep_offsets(sc.flag, slots, sc.counts, &sc.rec->rows, stream));
+    SvgCounts c;
+    PCU_TRY(read_record(sc.rec, &c, stream));
+    if (c.bad) return svg_overflow();
+    h->rows = c.rows;
+    if (c.rows == 0) return PCU_B200_OK;
+    SortScratch<McRec> sort;
+    PCU_TRY(svg_alloc(h, c.rows, false, sort, stream));
+    PCU_LAUNCH(svg_dilate_write_kernel, blocks_for(slots), kThreads, stream, (const McRec*)sorted, n, (const unsigned char*)sc.flag,
+               (const unsigned*)sc.counts, sort.a);
+    return svg_sort_runs(h, sort, false, stream);
+}
+
+int svg_dilate_prepare(pcu_b200_workspace* ws, const void* g, long long n, int kind, pcu_b200_sparse_grid** out, long long* out_counts,
+                       cudaStream_t stream) {
+    if (!ws || !out || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    PCU_TRY(svg_check_grid(g, n, kind, kSvgMaxDilate, "dilate_sparse_voxel_grid"));
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_sparse_grid* h) -> int {
+        h->mode = kSvgDilate; h->n = n; h->grid = g; h->out_kind = kind;
+        return kind == kIdxI64 ? svg_dilate_build<long long>(ws, h, (const long long*)g, n, stream)
+                               : svg_dilate_build<int>(ws, h, (const int*)g, n, stream);
+    }));
+    out_counts[0] = n + (*out)->rows;
+    out_counts[1] = (*out)->recs;
+    return PCU_B200_OK;
+}
+
+int svg_hex_prepare(pcu_b200_workspace* ws, const void* g, long long n, int kind, const double size[3], const double origin[3], int v_f64,
+                    pcu_b200_sparse_grid** out, long long* out_counts, cudaStream_t stream) {
+    if (!ws || !out || !out_counts || !size || !origin) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    PCU_TRY(svg_check_grid(g, n, kind, kSvgMaxHex, "sparse_voxel_grid_to_hex_mesh"));
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_sparse_grid* h) -> int {
+        h->mode = kSvgHex; h->n = n; h->out_kind = v_f64 != 0;
+        for (int a = 0; a < 3; ++a) { h->place.g[a] = size[a]; h->place.o[a] = origin[a]; }
+        SortScratch<McRec> sort;
+        PCU_TRY(svg_alloc(h, 8 * n, true, sort, stream));
+        if (kind == kIdxI64) PCU_LAUNCH((svg_corners_kernel<long long>), blocks_for(n), kThreads, stream, (const long long*)g, n, sort.a, &h->counts->bad);
+        else PCU_LAUNCH((svg_corners_kernel<int>), blocks_for(n), kThreads, stream, (const int*)g, n, sort.a, &h->counts->bad);
+        return svg_sort_runs(h, sort, true, stream);
+    }));
+    out_counts[0] = (*out)->rows;
+    out_counts[1] = (*out)->recs;
+    return PCU_B200_OK;
+}
+
+template <typename O>
+int svg_decode_launch(const pcu_b200_sparse_grid* h, void* out, cudaStream_t stream) {
+    PCU_LAUNCH(svg_decode_kernel<O>, blocks_for(h->recs), kThreads, stream, h->sorted, h->recs, (const unsigned char*)h->head,
+               (const unsigned*)h->offsets, h->place, (O*)out);
+    return PCU_B200_OK;
+}
+
+// From points: out_rows (rows, 3) int32, out_index (n) int64 point_to_vox.  Dilation: out_rows (n + rows, 3) of the
+// grid's kind, the input rows then the new ones.  Hex mesh: out_rows (rows, 3) vertices, out_index (n, 8) int64 cubes.
+int svg_emit(pcu_b200_workspace* ws, const pcu_b200_sparse_grid* h, void* out_rows, int64_t* out_index, cudaStream_t stream) {
+    if (!ws || !h || !out_rows || (h->mode != kSvgDilate && !out_index)) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    PCU_TRY(check_handle_device(ws, h, "sparse voxel grid"));
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    if (h->mode == kSvgDilate) {
+        const size_t width = h->out_kind == kIdxI64 ? 8 : 4;
+        PCU_CUDA(cudaMemcpyAsync(out_rows, h->grid, (size_t)h->n * 3 * width, cudaMemcpyDeviceToDevice, stream));
+        if (h->rows == 0) return PCU_B200_OK;
+        unsigned char* tail = (unsigned char*)out_rows + (size_t)h->n * 3 * width;
+        return h->out_kind == kIdxI64 ? svg_decode_launch<long long>(h, tail, stream) : svg_decode_launch<int>(h, tail, stream);
+    }
+    if (h->mode == kSvgPoints) PCU_TRY(svg_decode_launch<int>(h, out_rows, stream));
+    else PCU_TRY(h->out_kind ? svg_decode_launch<double>(h, out_rows, stream) : svg_decode_launch<float>(h, out_rows, stream));
+    PCU_LAUNCH(svg_rank_kernel, blocks_for(h->recs), kThreads, stream, h->sorted, h->recs, (const unsigned char*)h->head,
+               (const unsigned*)h->offsets, (long long*)out_index);
+    return PCU_B200_OK;
+}
+
+// Erosion: codes, their sort, the 26-neighbour test, the ordered copy of the kept rows.  out_counts (device):
+// {kept rows, rows out of range}.
+template <typename I>
+int svg_erode_device(pcu_b200_workspace* ws, const I* g, long long n, I* out, long long* out_counts, cudaStream_t stream) {
+    struct { SortScratch<McRec> sort; unsigned char* keep; unsigned* counts; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.sort.carve(cv, n);
+        sc.keep = cv.take<unsigned char>((size_t)n);
+        sc.counts = cv.take<unsigned>(keep_count_words(n));
+    }));
+    PCU_CUDA(cudaMemsetAsync(out_counts, 0, 2 * sizeof(long long), stream));
+    PCU_LAUNCH((svb_codes_kernel<I>), blocks_for(n), kThreads, stream, g, n, sc.sort.a, (unsigned long long*)(out_counts + 1));
+    McRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(sc.sort, n, 1, stream, &sorted));
+    PCU_LAUNCH((svg_erode_flag_kernel<I>), blocks_for(n), kThreads, stream, g, n, (const McRec*)sorted, sc.keep);
+    PCU_TRY(enqueue_keep_offsets(sc.keep, n, sc.counts, out_counts, stream));
+    PCU_LAUNCH((svg_keep_voxels_kernel<I>), blocks_for(n), kThreads, stream, g, (const unsigned char*)sc.keep, n, (const unsigned*)sc.counts, out);
+    return PCU_B200_OK;
+}
+
+int svg_erode(pcu_b200_workspace* ws, const void* g, long long n, int kind, void* out, long long* out_counts, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(svg_check_grid(g, n, kind, 0x7ffffffeLL, "erode_sparse_voxel_grid"));
+    if (!out || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    return kind == kIdxI64 ? svg_erode_device<long long>(ws, (const long long*)g, n, (long long*)out, out_counts, stream)
+                           : svg_erode_device<int>(ws, (const int*)g, n, (int*)out, out_counts, stream);
+}
+
+int voxel_grid_geometry_device(pcu_b200_workspace* ws, const void* ijk, long long n, int kind, const double size[3], const double origin[3],
+                               double gap, float* out_v, int32_t* out_f, cudaStream_t stream) {
+    if (!ws || !size || !origin) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (!ijk || n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid input point cloud with zero points");
+    if (n > kVgMaxVoxels) return fail(PCU_B200_INVALID_ARGUMENT, "voxel_grid_geometry: at most 2^28 voxels are supported, got %lld", n);
+    if (kind < kIdxI32 || kind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown index kind %d", kind);
+    // as in the reference, a NaN size passes here
+    if (size[0] <= 0.0 || size[1] <= 0.0 || size[2] <= 0.0) return fail(PCU_B200_INVALID_ARGUMENT, "Voxel size must be positive");
+    if (!out_v || !out_f) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    VgGeom g;
+    for (int k = 0; k < 3; ++k) { g.s[k] = size[k]; g.o[k] = origin[k]; }
+    g.keep = 1.0 - gap;
+    g.shift = 0.5 * gap;
+    const unsigned blocks = blocks_for(12 * n);
+    switch (kind) {
+        case kIdxI32: PCU_LAUNCH(vg_geometry_kernel<int>, blocks, kThreads, stream, (const int*)ijk, n, g, out_v, out_f); break;
+        case kIdxI64: PCU_LAUNCH(vg_geometry_kernel<long long>, blocks, kThreads, stream, (const long long*)ijk, n, g, out_v, out_f); break;
+        case kIdxU32: PCU_LAUNCH(vg_geometry_kernel<unsigned>, blocks, kThreads, stream, (const unsigned*)ijk, n, g, out_v, out_f); break;
+        default: PCU_LAUNCH(vg_geometry_kernel<unsigned long long>, blocks, kThreads, stream, (const unsigned long long*)ijk, n, g, out_v, out_f);
+    }
+    return PCU_B200_OK;
+}
+
 // ---- triangle-mesh voxelization and 3-D flood fill (voxelize.cuh) ------------------------------------------------
 // Persistent CTAs of vx_test_kernel: enough to fill every SM (the kernel holds 16-32 KB of shared memory per CTA).
 inline unsigned vx_test_blocks(const pcu_b200_workspace* ws) { return (unsigned)ws->sm_count * 6u; }
@@ -3363,6 +3608,41 @@ int pcu_b200_marching_cubes_destroy(pcu_b200_marching_cubes* mc) {
 int pcu_b200_sparse_voxel_grid_boundary(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, int64_t* out_idx,
                                         int64_t* out_counts, void* stream) {
     return sparse_voxel_grid_boundary_device(ws, grid, n, idx_kind, (long long*)out_idx, (long long*)out_counts, (cudaStream_t)stream);
+}
+
+int pcu_b200_sparse_grid_from_points_f32(pcu_b200_workspace* ws, const float* points, int64_t n, const double voxel_size[3],
+                                         const double origin[3], pcu_b200_sparse_grid** out_grid, int64_t out_counts[2], void* stream) {
+    return svg_points_prepare<float>(ws, points, n, voxel_size, origin, out_grid, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_sparse_grid_from_points_f64(pcu_b200_workspace* ws, const double* points, int64_t n, const double voxel_size[3],
+                                         const double origin[3], pcu_b200_sparse_grid** out_grid, int64_t out_counts[2], void* stream) {
+    return svg_points_prepare<double>(ws, points, n, voxel_size, origin, out_grid, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_sparse_grid_dilate_prepare(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, pcu_b200_sparse_grid** out_grid,
+                                        int64_t out_counts[2], void* stream) {
+    return svg_dilate_prepare(ws, grid, n, idx_kind, out_grid, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_sparse_grid_hex_prepare(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, const double voxel_size[3],
+                                     const double origin[3], int vertices_f64, pcu_b200_sparse_grid** out_grid, int64_t out_counts[2],
+                                     void* stream) {
+    return svg_hex_prepare(ws, grid, n, idx_kind, voxel_size, origin, vertices_f64, out_grid, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_sparse_grid_emit(pcu_b200_workspace* ws, const pcu_b200_sparse_grid* sg, void* out_rows, int64_t* out_index, void* stream) {
+    return svg_emit(ws, sg, out_rows, out_index, (cudaStream_t)stream);
+}
+int pcu_b200_sparse_grid_destroy(pcu_b200_sparse_grid* sg) {
+    if (!sg) return PCU_B200_OK;
+    DeviceGuard guard(sg->device);
+    delete sg;
+    return PCU_B200_OK;
+}
+int pcu_b200_sparse_grid_erode(pcu_b200_workspace* ws, const void* grid, int64_t n, int idx_kind, void* out_grid, int64_t* out_counts,
+                               void* stream) {
+    return svg_erode(ws, grid, n, idx_kind, out_grid, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_voxel_grid_geometry(pcu_b200_workspace* ws, const void* ijk, int64_t n, int idx_kind, const double voxel_size[3],
+                                 const double voxel_origin[3], double gap_fraction, float* out_v, int32_t* out_f, void* stream) {
+    return voxel_grid_geometry_device(ws, ijk, n, idx_kind, voxel_size, voxel_origin, gap_fraction, out_v, out_f, (cudaStream_t)stream);
 }
 
 int pcu_b200_voxelize_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,

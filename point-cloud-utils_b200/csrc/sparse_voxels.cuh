@@ -16,7 +16,21 @@
 // sparse_voxel_grid_boundary (src/sparse_voxel_grid.cpp:463-522): Morton codes of the voxels (the reference's
 // safe_cast range check first), sorted; a voxel is on the boundary when one of its six face neighbours' codes
 // (morton_add2, in the reference's offset order) is not among them.  Integer work only.
+//
+// Sparse voxel grids (sparse_voxel_grid_from_pointcloud, dilate / erode_sparse_voxel_grid,
+// sparse_voxel_grid_to_hex_mesh; the reference's src/sparse_voxel_grid.cpp:78-460) and voxel_grid_geometry
+// (src/mesh_for_voxels.cpp): results defined in DESIGN.md §3.  Each builds a set of code records and sorts it with
+// sort.cuh; run heads (mc_heads_kernel) and the compaction of compact.cuh number the distinct codes:
+//   svg_point_codes_kernel  {code, point} of every point (fp64 quantisation, range check)
+//   svg_dilate_flag_kernel  per sorted voxel and neighbour offset: the missing neighbours this voxel owns
+//   svg_dilate_write_kernel the owned neighbours' codes, compacted (already distinct; sorted afterwards)
+//   svg_erode_flag_kernel   per voxel: all 26 neighbours present; svg_keep_voxels_kernel copies the kept rows
+//   svg_corners_kernel      {corner code, 8 i + k} of every cube corner
+//   svg_decode_kernel       distinct codes -> integer rows or hex vertices
+//   svg_rank_kernel         run rank of every record scattered to its index (point_to_vox, cubes)
+//   vg_geometry_kernel      the cube mesh of every voxel (no sort; sizes known in advance)
 #pragma once
+#include <type_traits>
 #include "common.cuh"
 #include "compact.cuh"
 #include "morton.cuh"
@@ -246,6 +260,20 @@ __global__ void __launch_bounds__(kThreads) svb_codes_kernel(const I* __restrict
     store_rec(recs + i, r);
 }
 
+// std::lower_bound of code q in the n sorted codes, and the reference's vector_binsearch test on it.
+__device__ __forceinline__ long long svb_lower_bound(const McRec* __restrict__ sorted, long long n, unsigned long long q) {
+    long long lo = 0, hi = n;
+    while (lo < hi) {
+        const long long mid = lo + ((hi - lo) >> 1);
+        if (__ldg(&sorted[mid].key[0]) < q) lo = mid + 1; else hi = mid;
+    }
+    return lo;
+}
+__device__ __forceinline__ bool svb_missing(const McRec* __restrict__ sorted, long long n, unsigned long long q) {
+    const long long lo = svb_lower_bound(sorted, n, q);
+    return lo == n || __ldg(&sorted[lo].key[0]) != q;
+}
+
 // keep[i] = 1 when one of voxel i's six face neighbours (+x, -x, +y, -y, +z, -z: the reference's order) is missing
 template <typename I>
 __global__ void __launch_bounds__(kThreads) svb_flag_kernel(const I* __restrict__ g, long long n, const McRec* __restrict__ sorted,
@@ -257,14 +285,197 @@ __global__ void __launch_bounds__(kThreads) svb_flag_kernel(const I* __restrict_
     for (int o = 0; o < 6 && !boundary; ++o) {
         const int d = (o & 1) ? -1 : 1, a = o >> 1;
         const unsigned long long q = morton_add2(code, morton_encode3(a == 0 ? d : 0, a == 1 ? d : 0, a == 2 ? d : 0));
-        long long lo = 0, hi = n;                 // std::lower_bound
-        while (lo < hi) {
-            const long long mid = lo + ((hi - lo) >> 1);
-            if (__ldg(&sorted[mid].key[0]) < q) lo = mid + 1; else hi = mid;
-        }
-        boundary = lo == n || __ldg(&sorted[lo].key[0]) != q;
+        boundary = svb_missing(sorted, n, q);
     }
     keep[i] = boundary ? 1 : 0;
+}
+
+// ---- sparse voxel grids: from points, dilation, erosion, hex mesh; voxel cube meshes ------------------------------
+// Definitions in DESIGN.md §3.  A voxel is its 64-bit Morton code (morton.cuh); "sorted" is ascending code order.
+// The 26 neighbour offsets, x slowest then y then z (the reference's table order without its three repeats):
+// o in [0, 26) is cell c = o + (o >= 13) of the 3 x 3 x 3 block, offset (c / 9 - 1, c / 3 % 3 - 1, c % 3 - 1).
+__device__ __forceinline__ int svg_axis(int o, int a) {
+    const int c = o + (o >= 13 ? 1 : 0);
+    return (a == 0 ? c / 9 : a == 1 ? c / 3 % 3 : c % 3) - 1;
+}
+__device__ __forceinline__ unsigned long long svg_offset(int o) {
+    return morton_encode3(svg_axis(o, 0), svg_axis(o, 1), svg_axis(o, 2));
+}
+
+// The scaling of the point quantisation and of the hex vertices (host values, passed by value).
+struct SvgPlace { double g[3], o[3]; };
+
+// Per point: round((double(p) - o) / g) per axis (each operation rounded in fp64, C round: half away from zero), the
+// reference's safe_cast<double, int32_t> (NaN passes it and converts to INT32_MIN, as x86-64 cvttsd2si does), its
+// code as the record {code, point}.  *bad counts points with a coordinate outside [INT32_MIN + 1, INT32_MAX - 1].
+template <typename T>
+__global__ void __launch_bounds__(kThreads) svg_point_codes_kernel(const T* __restrict__ p, long long n, SvgPlace pl,
+                                                                   McRec* __restrict__ recs, unsigned long long* __restrict__ bad) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    int c[3];
+    bool out = false;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const double r = round(__ddiv_rn(__dsub_rn((double)p[3 * i + a], pl.o[a]), pl.g[a]));
+        out = out || r > 2147483646.0 || r < -2147483647.0;
+        c[a] = isnan(r) ? INT_MIN : (int)r;
+    }
+    if (out) atomicAdd(bad, 1ull);
+    McRec rec;
+    rec.key[0] = morton_encode3(c[0], c[1], c[2]);
+    rec.idx = (unsigned long long)i;
+    store_rec(recs + i, rec);
+}
+
+// Dilation, one thread per sorted voxel code j (duplicates after the first flag nothing): flag[o n + j] = 1 when
+// neighbour q = code + offset o is missing from the grid and this voxel owns it, i.e. no earlier offset o' < o reaches
+// q from a voxel of the grid (q - offset o' = code + offset o - offset o' present).  Every missing neighbour is thus
+// flagged exactly once, and the flagged codes are already distinct.
+__global__ void __launch_bounds__(kThreads) svg_dilate_flag_kernel(const McRec* __restrict__ sorted, long long n,
+                                                                   unsigned char* __restrict__ flag) {
+    const long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (j >= n) return;
+    const unsigned long long code = __ldg(&sorted[j].key[0]);
+    const bool first = j == 0 || __ldg(&sorted[j - 1].key[0]) != code;
+#pragma unroll 1
+    for (int o = 0; o < 26; ++o) {
+        bool owned = false;
+        if (first && svb_missing(sorted, n, morton_add2(code, svg_offset(o)))) {
+            owned = true;
+#pragma unroll 1
+            for (int e = 0; e < o && owned; ++e) {
+                const unsigned long long d = morton_encode3(svg_axis(o, 0) - svg_axis(e, 0), svg_axis(o, 1) - svg_axis(e, 1),
+                                                            svg_axis(o, 2) - svg_axis(e, 2));
+                owned = svb_missing(sorted, n, morton_add2(code, d));
+            }
+        }
+        flag[o * n + j] = owned ? 1 : 0;
+    }
+}
+
+// After keep_count / keep_offsets over the 26 n flags: every flagged slot o n + j writes the record {code_j + offset
+// o, rank} at its rank.
+__global__ void __launch_bounds__(kThreads) svg_dilate_write_kernel(const McRec* __restrict__ sorted, long long n,
+                                                                    const unsigned char* __restrict__ flag,
+                                                                    const unsigned* __restrict__ block_offset, McRec* __restrict__ recs) {
+    const long long s = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool mine = s < 26 * n && flag[s];
+    const unsigned pos = keep_rank(mine, block_offset);
+    if (!mine) return;
+    const long long o = s / n, j = s - o * n;
+    McRec rec;
+    rec.key[0] = morton_add2(__ldg(&sorted[j].key[0]), svg_offset((int)o));
+    rec.idx = pos;
+    store_rec(recs + pos, rec);
+}
+
+// Erosion: keep[i] = 1 when all 26 neighbours of voxel i are in the grid.
+template <typename I>
+__global__ void __launch_bounds__(kThreads) svg_erode_flag_kernel(const I* __restrict__ g, long long n, const McRec* __restrict__ sorted,
+                                                                  unsigned char* __restrict__ keep) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const unsigned long long code = svb_code<I>(g, i);
+    bool all = true;
+#pragma unroll 1
+    for (int o = 0; o < 26 && all; ++o) all = !svb_missing(sorted, n, morton_add2(code, svg_offset(o)));
+    keep[i] = all ? 1 : 0;
+}
+
+// The kept rows of g, verbatim and in order.
+template <typename I>
+__global__ void __launch_bounds__(kThreads) svg_keep_voxels_kernel(const I* __restrict__ g, const unsigned char* __restrict__ keep,
+                                                                   long long n, const unsigned* __restrict__ block_offset,
+                                                                   I* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const bool mine = i < n && keep[i];
+    const unsigned pos = keep_rank(mine, block_offset);
+    if (!mine) return;
+    out[3ull * pos] = g[3 * i]; out[3ull * pos + 1] = g[3 * i + 1]; out[3ull * pos + 2] = g[3 * i + 2];
+}
+
+// Hex mesh: the 8 corner records {code + corner offset, 8 i + k} of voxel i, corners (0,0,0) (1,0,0) (1,1,0) (0,1,0)
+// (0,0,1) (1,0,1) (1,1,1) (0,1,1) (marching_cubes_sparse_voxel_grid's order); *bad as in svb_codes_kernel.
+template <typename I>
+__global__ void __launch_bounds__(kThreads) svg_corners_kernel(const I* __restrict__ g, long long n, McRec* __restrict__ recs,
+                                                               unsigned long long* __restrict__ bad) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    if (!svb_fits((long long)g[3 * i]) || !svb_fits((long long)g[3 * i + 1]) || !svb_fits((long long)g[3 * i + 2])) atomicAdd(bad, 1ull);
+    const unsigned long long code = svb_code<I>(g, i);
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        McRec rec;
+        rec.key[0] = morton_add2(code, morton_encode3(((k + 1) >> 1) & 1, (k >> 1) & 1, k >> 2));
+        rec.idx = 8ull * i + k;
+        store_rec(recs + 8 * i + k, rec);
+    }
+}
+
+// After keep_count / keep_offsets over the run heads of the sorted records: each head writes its decoded code as row
+// rank(head) of out -- integer rows (O = int or long long), or hex vertices (O = float or double):
+// ((double)c * g + o) - 0.5 * g per axis, each operation rounded in fp64, then one rounding to O.  head == nullptr:
+// every record is a head (codes already distinct), rows in record order.
+template <typename O>
+__global__ void __launch_bounds__(kThreads) svg_decode_kernel(const McRec* __restrict__ recs, long long n, const unsigned char* __restrict__ head,
+                                                              const unsigned* __restrict__ block_offset, SvgPlace pl, O* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    bool mine = i < n;
+    unsigned long long pos = (unsigned long long)i;
+    if (head) {
+        mine = mine && head[i];
+        pos = keep_rank(mine, block_offset);
+    }
+    if (!mine) return;
+    int c[3];
+    morton_decode3(recs[i].key[0], c[0], c[1], c[2]);
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        if constexpr (std::is_floating_point<O>::value)
+            out[3 * pos + a] = (O)__dsub_rn(__dadd_rn(__dmul_rn((double)c[a], pl.g[a]), pl.o[a]), __dmul_rn(0.5, pl.g[a]));
+        else
+            out[3 * pos + a] = (O)c[a];
+    }
+}
+
+// After keep_count / keep_offsets over the run heads: each record's run (distinct codes at or before it, minus one)
+// scattered to its index: point_to_vox[point], or cubes[8 i + k].
+__global__ void __launch_bounds__(kThreads) svg_rank_kernel(const McRec* __restrict__ recs, long long n, const unsigned char* __restrict__ head,
+                                                            const unsigned* __restrict__ block_offset, long long* __restrict__ out) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    const unsigned run = keep_rank<true>(i < n && head[i], block_offset) - 1u;
+    if (i < n) out[recs[i].idx] = (long long)run;
+}
+
+// voxel_grid_geometry (the reference's src/mesh_for_voxels.cpp generate_cube_mesh): thread t writes vertex row t
+// (t < 8 n) and face row t (t < 12 n).  Vertex row 8 i + c, component k: float((((tbl_ck * (1 - gap) + 0.5 gap)
+// + (double)ijk_ik) * s_k) + o_k), each operation rounded in fp64; face row 12 i + f: the table's face f plus 8 i.
+struct VgGeom { double s[3], o[3], keep, shift; };   // keep = 1 - gap, shift = 0.5 gap (as the reference computes them)
+__constant__ unsigned char kVgCorner[8] = {4, 5, 6, 7, 0, 1, 2, 3};   // bit 0: x, bit 1: y, bit 2: z of each table corner
+__constant__ unsigned char kVgFaces[36] = {2, 7, 6, 2, 3, 7, 0, 4, 5, 0, 5, 1, 0, 2, 6, 0, 6, 4,
+                                           1, 7, 3, 1, 5, 7, 0, 3, 2, 0, 1, 3, 4, 6, 7, 4, 7, 5};
+template <typename I>
+__global__ void __launch_bounds__(kThreads) vg_geometry_kernel(const I* __restrict__ ijk, long long n, VgGeom g, float* __restrict__ out_v,
+                                                               int* __restrict__ out_f) {
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < 8 * n) {
+        const long long i = t >> 3;
+        const unsigned corner = __ldg(&kVgCorner[t & 7]);
+#pragma unroll
+        for (int k = 0; k < 3; ++k) {
+            const double tbl = (double)((corner >> k) & 1u);
+            double x = __dadd_rn(__dmul_rn(tbl, g.keep), g.shift);
+            x = __dadd_rn(x, (double)ijk[3 * i + k]);
+            x = __dadd_rn(__dmul_rn(x, g.s[k]), g.o[k]);
+            out_v[3 * t + k] = __double2float_rn(x);
+        }
+    }
+    if (t < 12 * n) {
+        const long long i = t / 12, f = t - 12 * i;
+#pragma unroll
+        for (int k = 0; k < 3; ++k) out_f[3 * t + k] = (int)__ldg(&kVgFaces[3 * f + k]) + (int)(8 * i);
+    }
 }
 
 }  // namespace pcu
