@@ -68,11 +68,14 @@ typedef struct pcu_b200_workspace pcu_b200_workspace;
 
 /* Per-direction result of the fused k = 1 sweep (no per-point distance buffer is written). */
 typedef struct pcu_b200_nn_stats {
+    /* A query has a neighbour when some point's rounded d2 is below FLT_MAX / DBL_MAX (nanoflann's admission   */
+    /* rule); a query without one counts as d2_min = -1 in max_sq_dist and makes both sums +inf.                */
     double sum_dist;      /* sum over queries of sqrt(d2_min), accumulated in fp64                */
     double sum_sq_dist;   /* sum over queries of d2_min, accumulated in fp64                      */
-    double max_sq_dist;   /* largest d2_min (exact: the input-precision value widened to double)  */
+    double max_sq_dist;   /* largest d2_min (exact: the input-precision value widened to double); */
+                          /* -1 when no query has a neighbour                                      */
     int64_t argmax_query; /* first (lowest-index) query attaining it (Eigen maxCoeff, :221-223)   */
-    int64_t argmax_data;  /* its nearest neighbour in the dataset (:225)                          */
+    int64_t argmax_data;  /* its nearest neighbour in the dataset (:225); -1 when it has none     */
     int64_t n_queries;    /* n                                                                    */
     int64_t n_tied;       /* -1: the fused sweeps track distances only (ties only matter to witness_tied) */
     int64_t n_far;        /* queries that needed the ring-expansion slow path (diagnostic)        */

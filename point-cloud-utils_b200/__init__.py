@@ -181,6 +181,8 @@ def _stats_device(a, b, both, leaf):
 
 def _metric_value(max_sq, squared, dtype):
     d2 = dtype(max_sq)
+    if d2 == -1:   # no query found a neighbour: the reference's padded distance, not its root
+        return -1.0
     return float(d2 if squared else _np.sqrt(d2))
 
 
@@ -533,7 +535,13 @@ def chamfer_distance(x, y, return_index=False, p_norm=2, max_points_per_leaf=10,
     if _is_tensor(x):
         torch = _torch()
         if p_norm == 2:
-            cham = dists_x_to_y.mean() + dists_y_to_x.mean()
+            # A row without neighbour (index -1, distance -1.0) takes the reference's term instead of its padding:
+            # numpy indexes the last point there, and its norm is sqrt((e0^2 + e1^2) + e2^2) in the input precision.
+            def wrapped(dists, corrs, data, queries):
+                e = data[-1] - queries
+                last = ((e[:, 0] * e[:, 0] + e[:, 1] * e[:, 1]) + e[:, 2] * e[:, 2]).sqrt()
+                return torch.where(corrs.reshape(-1) < 0, last, dists.reshape(-1))
+            cham = wrapped(dists_x_to_y, corrs_x_to_y, y, x).mean() + wrapped(dists_y_to_x, corrs_y_to_x, x, y).mean()
         else:
             cham = torch.linalg.vector_norm(x[corrs_y_to_x.reshape(-1)] - y, ord=p_norm, dim=-1).mean() + \
                    torch.linalg.vector_norm(y[corrs_x_to_y.reshape(-1)] - x, ord=p_norm, dim=-1).mean()

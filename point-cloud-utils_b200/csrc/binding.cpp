@@ -331,6 +331,7 @@ pcu_b200_nn_stats one_sided_numpy(const py::array& s_in, const py::array& t_in, 
 template <typename T>
 T metric_value(double max_sq, bool squared) {
     const T d2 = (T)max_sq;  // exact: max_sq is the input-precision value widened
+    if (d2 == (T)-1) return d2;  // no query found a neighbour: the reference's padded distance, not its root
     return squared ? d2 : (T)std::sqrt(d2);  // correctly rounded sqrt in the input precision (:84-88)
 }
 

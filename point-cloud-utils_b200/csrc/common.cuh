@@ -33,6 +33,7 @@ template <> struct Real<float> {
     static __device__ __forceinline__ float add(float a, float b) { return __fadd_rn(a, b); }
     static __device__ __forceinline__ float root(float a) { return __fsqrt_rn(a); }
     static __device__ __forceinline__ float inf() { return __int_as_float(0x7f800000); }
+    static __device__ __forceinline__ float largest() { return __int_as_float(0x7f7fffff); }   // FLT_MAX
     static __device__ __forceinline__ float vmax(float a, float b) { return fmaxf(a, b); }
     static __device__ __forceinline__ float vmin(float a, float b) { return fminf(a, b); }
     static __device__ __forceinline__ bits_t bits(float a) { return __float_as_uint(a); }
@@ -49,6 +50,7 @@ template <> struct Real<double> {
     static __device__ __forceinline__ double add(double a, double b) { return __dadd_rn(a, b); }
     static __device__ __forceinline__ double root(double a) { return __dsqrt_rn(a); }
     static __device__ __forceinline__ double inf() { return __longlong_as_double(0x7ff0000000000000LL); }
+    static __device__ __forceinline__ double largest() { return __longlong_as_double(0x7fefffffffffffffLL); }   // DBL_MAX
     static __device__ __forceinline__ double vmax(double a, double b) { return fmax(a, b); }
     static __device__ __forceinline__ double vmin(double a, double b) { return fmin(a, b); }
     static __device__ __forceinline__ bits_t bits(double a) { return (bits_t)__double_as_longlong(a); }

@@ -52,7 +52,7 @@ __device__ __forceinline__ bool warp_ring_search(const GridHeader<T>& g, const C
     const int cx = cell_of<T>(q.x, g.origin[0], g.inv_h, g.dim[0]);
     const int cy = cell_of<T>(q.y, g.origin[1], g.inv_h, g.dim[1]);
     const int cz = cell_of<T>(q.z, g.origin[2], g.inv_h, g.dim[2]);
-    best.d = R::inf(); best.i = no_index<T>(); best.tie = false;
+    best.d = R::largest(); best.i = no_index<T>(); best.tie = false;
     for (int r = 0; r <= kMaxRing; ++r) {
         const int xa = max(cx - r, 0), xb = min(cx + r, g.dim[0] - 1);
         const int ya = max(cy - r, 0), yb = min(cy + r, g.dim[1] - 1);
@@ -118,7 +118,7 @@ __device__ __forceinline__ bool warp_window_search(const GridHeader<T>& g, const
     lb = R::vmin(lb, sq_gap<T>(q.y, dc.wall_hi[st + yb + 1]));
     lb = R::vmin(lb, sq_gap<T>(q.z, dc.wall_lo[2 * st + za]));
     lb = R::vmin(lb, sq_gap<T>(q.z, dc.wall_hi[2 * st + zb + 1]));
-    best.d = R::inf(); best.i = no_index<T>(); best.tie = false;
+    best.d = R::largest(); best.i = no_index<T>(); best.tie = false;
     const int ny = yb - ya + 1, nrows = ny * (zb - za + 1);
     for (int idx = lane; idx < nrows; idx += 32) {
         const int z = za + idx / ny, y = ya + idx % ny;
@@ -169,7 +169,7 @@ __global__ void __launch_bounds__(kThreads, sizeof(T) == 4 ? 6 : 4) nn1_kernel(c
     const int tid = threadIdx.x;
     const long long t = (long long)blockIdx.x * blockDim.x + tid;
     const bool active = t < qc.n;
-    Best1<T> best; best.d = R::inf(); best.i = no_index<T>(); best.tie = false;
+    Best1<T> best; best.d = R::largest(); best.i = no_index<T>(); best.tie = false;
     bool settled = false;
     long long row = -1;
     if (active) {

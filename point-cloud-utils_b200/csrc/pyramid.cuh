@@ -129,7 +129,7 @@ __device__ void conclude_sweep(const Sweep<T>& sw, const Cloud<T>& qc, const Clo
     if (threadIdx.x == 0) wg = *dc.grid;
     __syncthreads();
     if (threadIdx.x < 32 && result.max_d2 >= (T)0) {
-        Best1<T> wb; wb.d = R::inf(); wb.i = no_index<T>(); wb.tie = false;
+        Best1<T> wb; wb.d = R::largest(); wb.i = no_index<T>(); wb.tie = false;
         if (result.arg_nn != kWitnessUnknown) {
             const unsigned nn = result.arg_nn & kWitnessNone;
             wb.i = nn == kWitnessNone ? no_index<T>() : (typename Real<T>::index_t)nn;
@@ -138,7 +138,7 @@ __device__ void conclude_sweep(const Sweep<T>& sw, const Cloud<T>& qc, const Clo
             const Pt<T> wq = load_pt<T>(qc.sorted + result.arg_pos);
             if (!warp_window_search<T>(wg, dc, wq, threadIdx.x, 1, wb) && !warp_ring_search<T>(wg, dc, wq, threadIdx.x, wb)) {
                 // beyond the rings: the pyramid exists (this query was on the very-far list)
-                wb.d = R::inf(); wb.i = no_index<T>(); wb.tie = false;
+                wb.d = R::largest(); wb.i = no_index<T>(); wb.tie = false;
                 for (int w = threadIdx.x; w < (int)(sizeof(PyramidShape) / sizeof(int)); w += 32)
                     reinterpret_cast<int*>(&wps)[w] = reinterpret_cast<const int*>(dc.shape)[w];
                 __syncwarp();
@@ -162,13 +162,14 @@ __device__ void conclude_sweep(const Sweep<T>& sw, const Cloud<T>& qc, const Clo
             *sw.stats = st;
         }
     } else if (threadIdx.x == 0 && !(result.max_d2 >= (T)0)) {
-        // no query produced a comparable distance (non-finite coordinates): the record is still written, with
-        // no witness, so that callers never decode uninitialised memory
+        // no query found a neighbour (max_d2 = -1 from the first such query, as in the reference's padded
+        // distances) or none produced a comparable distance (non-finite coordinates): the record is still
+        // written, with no witness, so that callers never decode uninitialised memory
         pcu_b200_nn_stats st;
         st.sum_dist = result.sum;
         st.sum_sq_dist = result.sumsq;
         st.max_sq_dist = (double)result.max_d2;
-        st.argmax_query = -1;
+        st.argmax_query = result.max_d2 == (T)-1 && result.arg_q != 0xffffffffu ? (long long)result.arg_q : -1;
         st.argmax_data = -1;
         st.n_queries = qc.n;
         st.n_tied = -1;
@@ -215,7 +216,7 @@ __global__ void __launch_bounds__(kThreads) nn1_vfar_kernel(const __grid_constan
         const unsigned step = gridDim.x * blockDim.x;
         for (unsigned f = blockIdx.x * blockDim.x + threadIdx.x; f < n_vfar; f += step) {
             const Pt<T> q = load_pt<T>(qc.sorted + sw.vfar_list[f]);
-            Best1<T> best; best.d = R::inf(); best.i = no_index<T>(); best.tie = false;
+            Best1<T> best; best.d = R::largest(); best.i = no_index<T>(); best.tie = false;
             pyramid_descend<T>(g, ps, dc, q, [&]() { return best.d; },
                                [&](unsigned a, unsigned b) { scan_run1<T>(dc.sorted, a, b, q.x, q.y, q.z, best); });
             finish_query1<T, kOut, kStats>(sw, true, best, (long long)q.i, sw.vfar_list[f], witness_word<T>(best), sum, sumsq, mc);
@@ -269,8 +270,8 @@ __global__ void __launch_bounds__(kThreads) knn_descend_kernel(const __grid_cons
         T* ld = sw.out_dist + row * k;
         long long* li = sw.out_idx + row * k;
         int have = 0;
-        T worst = R::inf();
-        long long worst_i = 0x7fffffffffffffffLL;
+        T worst = R::largest();   // nanoflann's KNNResultSet::init: a point at exactly this d^2 is never admitted
+        long long worst_i = -1;   // no index passes the tie clause below until the list is full
         T rej = R::inf();
         pyramid_descend<T>(g, ps, dc, q, [&]() { return worst; },
             [&](unsigned a, unsigned b) {

@@ -61,6 +61,10 @@ struct SweepsVal {
     __device__ __forceinline__ const Sweep<T>& operator[](int i) const { return v[i]; }
 };
 
+// The running nearest neighbour of one query.  d starts at the largest finite value, as nanoflann's KNNResultSet
+// does (init), so a point whose rounded d^2 is exactly that value or overflows to +inf is never admitted and
+// d < Real<T>::largest() holds exactly when a neighbour was found.  While d is still at its start value the tie
+// branch of the offers may record a point at that distance in i and tie; found1() ignores both then.
 template <typename T>
 struct Best1 {
     T d;
@@ -68,19 +72,22 @@ struct Best1 {
     bool tie;
 };
 
+template <typename T>
+__device__ __forceinline__ bool found1(const Best1<T>& b) { return b.d < Real<T>::largest(); }
+
 template <typename T> __device__ __forceinline__ typename Real<T>::index_t no_index();
 template <> __device__ __forceinline__ int32_t no_index<float>() { return 0x7fffffff; }
 template <> __device__ __forceinline__ long long no_index<double>() { return 0x7fffffffffffffffLL; }
 
 // The Hausdorff witness of one answered query in one word: the neighbour's index in bits 0-30 (clouds hold fewer
-// than 2^31 points; kWitnessNone when no point was found) and, in bit 31, whether tie order decided it.  A Best1
-// without a neighbour never has its tie flag set, so no witness word equals kWitnessUnknown, which the main
+// than 2^31 points; kWitnessNone when no point was found) and, in bit 31, whether tie order decided it.  A query
+// without a neighbour never gets the tie bit, so no witness word equals kWitnessUnknown, which the main
 // statistics pass writes: it tracks distances only.
 constexpr unsigned kWitnessUnknown = 0xffffffffu;
 constexpr unsigned kWitnessNone = 0x7fffffffu;
 template <typename T>
 __device__ __forceinline__ unsigned witness_word(const Best1<T>& b) {
-    return (b.i == no_index<T>() ? kWitnessNone : (unsigned)b.i) | (b.tie ? 0x80000000u : 0u);
+    return found1<T>(b) ? (unsigned)b.i | (b.tie ? 0x80000000u : 0u) : kWitnessNone;
 }
 
 template <typename T>
@@ -169,7 +176,7 @@ __device__ __forceinline__ bool expand_rings(const GridHeader<T>& g, const T* __
 // block-level reduction of the fused statistics
 template <typename T>
 struct MaxCand {
-    T d2;           // -1: neutral element
+    T d2;           // -1: neutral element (q = 0xffffffff) or a query without neighbour
     unsigned q;     // caller-order row (clouds are limited to 2^31 - 1 points)
     unsigned pos;   // position in cell order
     unsigned nn;    // witness word of the query, or kWitnessUnknown
@@ -200,21 +207,22 @@ __device__ __forceinline__ MaxCand<T> warp_take_max(MaxCand<T> mc) {
     }
     return mc;
 }
-// fp32: distances are >= 0, so their bit patterns order like the values and the hardware integer
-// reductions (REDUX) do the work: max of the distance bits, then min row among the lanes holding it.
+// fp32: the order-preserving image of the distances (>= 0, or -1 for a query without neighbour) lets the hardware
+// integer reductions (REDUX) do the work: max of the images, then min row among the lanes holding it.  The neutral
+// element (-1, row 0xffffffff) loses to every candidate; a NaN never wins.
 template <>
 __device__ __forceinline__ MaxCand<float> warp_take_max<float>(MaxCand<float> mc) {
-    const bool real = mc.d2 >= 0.f;   // the neutral element has d2 = -1
-    const unsigned bits = real ? __float_as_uint(mc.d2) : 0u;
+    const bool real = mc.d2 >= -1.f;
+    const unsigned bits = real ? ordered<float>(mc.d2) : 0u;
     const unsigned top = __reduce_max_sync(0xffffffffu, bits);
     const bool holds = real && bits == top;
     const unsigned row = holds ? mc.q : 0xffffffffu;
     const unsigned first = __reduce_min_sync(0xffffffffu, row);
     const unsigned who = __ballot_sync(0xffffffffu, holds && row == first);
-    if (who == 0u) return mc;         // nobody holds a real candidate: all lanes are neutral
+    if (who == 0u) return mc;         // every lane holds a NaN (non-finite coordinates)
     const int src = __ffs(who) - 1;
     MaxCand<float> out;
-    out.d2 = __uint_as_float(top);
+    out.d2 = unordered<float>(top);
     out.q = first;
     out.pos = __shfl_sync(0xffffffffu, mc.pos, src);
     out.nn = __shfl_sync(0xffffffffu, mc.nn, src);
@@ -250,22 +258,24 @@ __device__ __forceinline__ void block_reduce_stats(double sum, double sumsq, Max
 // the only index the scalar metrics ever need is the neighbour of the ONE query that attains the
 // Hausdorff maximum.  The slow passes know it and carry it with the maximum (`witness`: witness_word(best));
 // the main pass passes kWitnessUnknown and conclude_sweep recovers it with one warp.
+// A query without neighbour enters the Hausdorff maximum as -1, the distance the reference pads its row with, and
+// makes the distance sums (hence the Chamfer distance) +inf (DESIGN.md section 3).
 template <typename T, bool kOut, bool kStats>
 __device__ __forceinline__ void finish_query1(const Sweep<T>& sw, bool have, const Best1<T>& best, long long row,
                                               unsigned pos, unsigned witness, double& sum, double& sumsq, MaxCand<T>& mc) {
     using R = Real<T>;
     if (!have) return;
+    const bool found = found1<T>(best);
     const T root = R::root(best.d);
     if (kOut) {
-        const bool found = best.i != no_index<T>();
         sw.out_idx[row] = found ? (long long)best.i : -1;
         sw.out_dist[row] = found ? (sw.squared ? best.d : root) : (T)-1;
-        if (best.tie) sw.tie_list[atomicAdd(sw.counters + 1, 1u)] = row;
+        if (found && best.tie) sw.tie_list[atomicAdd(sw.counters + 1, 1u)] = row;
     }
     if (kStats) {
-        sum += (double)root;
-        sumsq += (double)best.d;
-        MaxCand<T> c; c.d2 = best.d; c.q = (unsigned)row; c.pos = pos; c.nn = witness;
+        sum += found ? (double)root : (double)R::inf();
+        sumsq += found ? (double)best.d : (double)R::inf();
+        MaxCand<T> c; c.d2 = found ? best.d : (T)-1; c.q = (unsigned)row; c.pos = pos; c.nn = witness;
         take_max<T>(mc, c);
     }
 }

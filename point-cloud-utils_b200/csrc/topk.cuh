@@ -22,9 +22,11 @@ __device__ __forceinline__ void knn_warp_one(const Sweep<T>& sw, const Cloud<T>&
     const int k = sw.k;
     const Pt<T> q = load_pt<T>(qc.sorted + t);
 
-    T dl = R::inf();
+    // empty slots and the k-th distance start at the largest finite value (nanoflann's KNNResultSet::init): a point
+    // at exactly that d^2, or at +inf, is never admitted, and the tie clause only applies once the list is full
+    T dl = R::largest();
     index_t il = no_index<T>();
-    T worst = R::inf();
+    T worst = R::largest();
     index_t worst_i = no_index<T>();
     T rej = R::inf();   // smallest distance that was turned away or pushed out (uniform across lanes)
     const unsigned kmask = k >= 32 ? 0xffffffffu : ((1u << k) - 1u);
@@ -41,7 +43,7 @@ __device__ __forceinline__ void knn_warp_one(const Sweep<T>& sw, const Cloud<T>&
                 d = dist2<T>(q.x, q.y, q.z, p.x, p.y, p.z);
                 pi = p.i;
             }
-            const bool pass = valid && (d < worst || (d == worst && pi < worst_i));
+            const bool pass = valid && (d < worst || (d == worst && pi < worst_i && worst_i != no_index<T>()));
             // distances that never enter the list still matter for the tie flag
             T turned = (valid && !pass) ? d : R::inf();
 #pragma unroll
@@ -53,7 +55,7 @@ __device__ __forceinline__ void knn_warp_one(const Sweep<T>& sw, const Cloud<T>&
                 mask &= mask - 1;
                 const T cd = __shfl_sync(0xffffffffu, d, src);
                 const index_t ci = __shfl_sync(0xffffffffu, pi, src);
-                if (!(cd < worst || (cd == worst && ci < worst_i))) { rej = R::vmin(rej, cd); continue; }
+                if (!(cd < worst || (cd == worst && ci < worst_i && worst_i != no_index<T>()))) { rej = R::vmin(rej, cd); continue; }
                 const bool before = (dl < cd) || (dl == cd && il < ci);
                 const int pos = __popc(__ballot_sync(0xffffffffu, before) & kmask);
                 const T pushed = __shfl_sync(0xffffffffu, dl, k - 1);
@@ -129,7 +131,9 @@ __global__ void __launch_bounds__(kThreads) knn_warp_kernel(const __grid_constan
 //
 // Slots: K = capacity (power of two >= k).  The K - k surplus slots are filled with a key that is
 // smaller than every real key, so they sit at the front of the ascending list for ever and the k-th
-// best is always slot K - 1 -- a compile-time register, no dynamic indexing.
+// best is always slot K - 1 -- a compile-time register, no dynamic indexing.  Empty slots hold a key at the
+// largest finite distance that no candidate at that distance (or at +inf) is less than: as in nanoflann's
+// KNNResultSet, only a point strictly nearer than the largest finite value is ever admitted.
 template <typename T> struct ListKey;
 template <> struct ListKey<float> {
     unsigned long long v;   // (distance bits << 32) | index : distances are >= +0, bits order like values
@@ -137,23 +141,23 @@ template <> struct ListKey<float> {
         ListKey k; k.v = ((unsigned long long)__float_as_uint(d) << 32) | (unsigned)i; return k;
     }
     static __device__ __forceinline__ ListKey dead() { ListKey k; k.v = 0ull; return k; }
-    static __device__ __forceinline__ ListKey empty() { ListKey k; k.v = ~0ull; return k; }
+    static __device__ __forceinline__ ListKey empty() { ListKey k; k.v = 0x7f7fffffull << 32; return k; }   // (FLT_MAX, 0)
     __device__ __forceinline__ bool less(const ListKey& o) const { return v < o.v; }
     __device__ __forceinline__ float dist() const { return __uint_as_float((unsigned)(v >> 32)); }
     __device__ __forceinline__ long long index() const { return (long long)(int)(unsigned)v; }
-    __device__ __forceinline__ bool is_empty() const { return v == ~0ull; }
+    __device__ __forceinline__ bool is_empty() const { return v == 0x7f7fffffull << 32; }
 };
 template <> struct ListKey<double> {
     double d; long long i;
     static __device__ __forceinline__ ListKey make(double d, long long i) { ListKey k; k.d = d; k.i = i; return k; }
     static __device__ __forceinline__ ListKey dead() { ListKey k; k.d = -1.0; k.i = -1; return k; }
-    static __device__ __forceinline__ ListKey empty() {
-        ListKey k; k.d = __longlong_as_double(0x7ff0000000000000LL); k.i = 0x7fffffffffffffffLL; return k;
+    static __device__ __forceinline__ ListKey empty() {   // (DBL_MAX, -1)
+        ListKey k; k.d = __longlong_as_double(0x7fefffffffffffffLL); k.i = -1; return k;
     }
     __device__ __forceinline__ bool less(const ListKey& o) const { return d < o.d || (d == o.d && i < o.i); }
     __device__ __forceinline__ double dist() const { return d; }
     __device__ __forceinline__ long long index() const { return i; }
-    __device__ __forceinline__ bool is_empty() const { return i == 0x7fffffffffffffffLL; }
+    __device__ __forceinline__ bool is_empty() const { return d == __longlong_as_double(0x7fefffffffffffffLL); }
 };
 
 template <typename T, int K>
