@@ -336,6 +336,25 @@ int pcu_b200_poisson_disk_f32(pcu_b200_workspace* ws, const float* points, int64
 int pcu_b200_poisson_disk_f64(pcu_b200_workspace* ws, const double* points, int64_t n, double radius, uint32_t seed,
                               int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream);
 
+/* ---- Voronoi cells in the unit cube / square and Lloyd relaxation ------------------------------
+ * Replace voronoi_centroids_unit_cube, lloyd_3d and lloyd_2d (src/lloyd.cpp:166-300), whose geogram restricted Voronoi
+ * diagram, initial sampling and HLBFGS Newton iterations are not available; the results are defined in DESIGN.md §3:
+ *   cell V_i = {x in [0,1]^dim : |x - c_i|^2 <= |x - c_j|^2 for every c_j != c_i}; seeds at one position share one cell,
+ *   owned by the lowest index.  Centroid row i = centroid of V_i when vol(V_i) > 1e-30, else c_i.  All fp64.
+ * pcu_b200_voronoi_centroids: centers (n, dim) and out_centroids (n, dim) are DEVICE pointers; centers must lie in
+ *   [0,1]^dim (outside it the rows are unspecified).  dim 2 or 3, 1 <= n <= 2^31 - 2.  out_moments (DEVICE, may be NULL):
+ *   (n, 5) per cell: volume, first moment about the seed (x, y, z; z = 0 in 2-D), second moment about the seed.
+ * pcu_b200_lloyd: the initial sample of (n, dim, seed), num_lloyd centroid steps, then at most num_newton L-BFGS steps on
+ *   the CVT energy; out_points (n, dim) DEVICE.  out_energy (HOST, num_newton + 1 doubles, may be NULL): the energy of
+ *   the starting point and of every accepted Newton step; out_newton_steps (HOST, may be NULL): accepted steps.
+ * out_passes (HOST, 3 int64, may be NULL): cells handled by the first pass, the longer-list pass and the all-seeds pass,
+ *   summed over every cell evaluation of the call.  Both calls synchronise `stream` (the fallback passes are sized on
+ *   the host; DESIGN.md §8). */
+int pcu_b200_voronoi_centroids(pcu_b200_workspace* ws, const double* centers, int64_t n, int dim, double* out_centroids,
+                               double* out_moments, int64_t* out_passes, void* stream);
+int pcu_b200_lloyd(pcu_b200_workspace* ws, int64_t n, int dim, uint32_t seed, int num_lloyd, int num_newton, double* out_points,
+                   double* out_energy, int32_t* out_newton_steps, int64_t* out_passes, void* stream);
+
 /* ---- mesh sampling and barycentric interpolation ----------------------------------------------
  * Replaces sample_mesh_random / sample_mesh_poisson_disk (src/sample_mesh.cpp) and interpolate_barycentric_coords
  * (point_cloud_utils/__init__.py:203-217).  The reference draws with std::rand and libigl; the samples here are pure

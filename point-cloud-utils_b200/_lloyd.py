@@ -1,0 +1,155 @@
+"""voronoi_centroids_unit_cube, lloyd_3d and lloyd_2d -- the reference's names, arguments, defaults and messages
+(the reference's src/lloyd.cpp:166-300), computed by csrc/voronoi.cuh.
+
+The reference computes its cells with geogram's restricted Voronoi diagram and relaxes with geogram's initial sampling
+and HLBFGS Newton iterations, none of which is available; DESIGN.md §3 defines the results exactly instead (cells,
+centroid rows, the initial sample, the Lloyd step and the L-BFGS Newton phase)."""
+import numpy as _np
+
+from . import _pcu_internal
+from ._call import _dtype_name, _is_tensor, _torch
+
+# Cells handled by each pass (first pass, longer neighbour lists, all seeds) in the last call of this module's functions,
+# in any thread (a plain module global, for tests and tools): the fallback passes are otherwise invisible.
+last_pass_counts = (0, 0, 0)
+# The CVT energy of the starting point and of every accepted Newton step of the last lloyd_3d / lloyd_2d call.
+last_newton_energies = []
+
+
+def _device_args(t):
+    torch = _torch()
+    return t.device.index or 0, torch.cuda.current_stream(t.device).cuda_stream
+
+
+def voronoi_centroids_unit_cube(centers, *, device=None):
+    """
+    Compute the centroids of a 3d voronoi diagram restricted to the unit cube [0, 1]^3
+
+    Args:
+      centers : A [n, 3] array where each row is a point in a voronoi diagram restricted to
+               the unit cube [0, 1]^3 (float32 / float64 numpy array, CUDA tensor or CPU tensor)
+      device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+      voronoi_ctrs : a [n, 3] float64 array of centroids where each row is the centroid of the corresponding voronoi
+                     cell in the input centers (a CUDA tensor for a CUDA tensor, a CPU tensor for a CPU tensor).
+
+    Row i is the centroid of {x in [0,1]^3 : |x - c_i| <= |x - c_j| for every c_j != c_i} when that cell's volume is
+    above 1e-30.  Seeds at one position share one cell, which the lowest index owns; every other row (an empty cell)
+    is the seed itself -- the reference leaves such rows uninitialised.
+    """
+    global last_pass_counts
+    from . import _dev, _same_device
+    torch = _torch()
+    tensor = _is_tensor(centers)
+    if not tensor and type(centers) != _np.ndarray:
+        raise ValueError("Invalid type for centers, must be a NumPy array, but got " + str(type(centers)) + ".")
+    if _dtype_name(centers) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s) for argument 'centers'. Expected one of ['float32', 'float64']."
+                         % _dtype_name(centers))
+    shape = tuple(centers.shape)
+    if len(shape) != 2 or shape[1] != 3:
+        raise ValueError("Invalid shape for centers, must be (n, 3) but got " + str(shape))
+    n = shape[0]
+    if tensor and not centers.is_cuda:
+        return torch.from_numpy(voronoi_centroids_unit_cube(centers.detach().numpy(), device=device))
+    if tensor:
+        _same_device(centers, device)
+        x = centers.detach().to(torch.float64).contiguous()
+        if n == 0:
+            return x.clone()
+        bad = bool(((x < 0) | (x > 1) | torch.isnan(x)).any().item())
+    else:
+        if n == 0:
+            return _np.zeros((0, 3), dtype=_np.float64)
+        host = _np.ascontiguousarray(centers, dtype=_np.float64)      # float32 widens exactly
+        bad = bool(((host < 0) | (host > 1) | _np.isnan(host)).any())
+    if bad:
+        raise ValueError("Centers of voronoi diagram must lie in the unit cube [0, 1]^3")
+    if not tensor:
+        dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
+        x = torch.from_numpy(host).to(torch.device("cuda", dev))
+    out = torch.empty_like(x)
+    last_pass_counts = tuple(_pcu_internal._voronoi_centroids_device(x.data_ptr(), n, 3, out.data_ptr(), 0, *_device_args(x)))
+    return out if tensor else out.cpu().numpy()
+
+
+def _cell_moments(centers, *, device=None):
+    """(centroid rows, moments) of a float64 numpy array of (n, 2) or (n, 3) seeds in the unit square / cube, n >= 1,
+    as numpy arrays; moments (n, 5): volume, first moment about the seed (x, y, z; z = 0 in 2-D) and second moment
+    about the seed of every cell.  Not part of the public interface: the cells the relaxations see, for tests."""
+    global last_pass_counts
+    from . import _dev
+    torch = _torch()
+    host = _np.ascontiguousarray(centers, dtype=_np.float64)
+    n, dim = host.shape
+    dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
+    x = torch.from_numpy(host).to(torch.device("cuda", dev))
+    out = torch.empty_like(x)
+    mom = torch.empty((n, 5), dtype=torch.float64, device=x.device)
+    last_pass_counts = tuple(_pcu_internal._voronoi_centroids_device(x.data_ptr(), n, dim, out.data_ptr(), mom.data_ptr(),
+                                                                     *_device_args(x)))
+    return out.cpu().numpy(), mom.cpu().numpy()
+
+
+def _lloyd(n, num_lloyd, num_newton, dim, device):
+    global last_pass_counts, last_newton_energies
+    from . import _dev
+    n = int(n)
+    if n <= 0:
+        raise ValueError("n must be a positive integer. Got n = %d" % n)
+    seed = int(_np.random.randint(2 ** 31 - 1))
+    torch = _torch()
+    dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
+    out = torch.empty((n, dim), dtype=torch.float64, device=torch.device("cuda", dev))
+    energies, passes = _pcu_internal._lloyd_device(n, dim, seed, int(num_lloyd), int(num_newton), out.data_ptr(),
+                                                   *_device_args(out))
+    last_pass_counts = tuple(passes)
+    last_newton_energies = list(energies)
+    return out.cpu().numpy()
+
+
+_LLOYD_DEFINITION = """
+    The initial sample is a pure function of (n, seed, dimension), the seed drawn as int(np.random.randint(2**31 - 1))
+    (seed NumPy for reproducible results); num_lloyd steps then move every point to its cell's centroid, and at most
+    num_newton L-BFGS steps (memory 7, Armijo backtracking inside the unit cube) decrease the CVT energy
+    sum_i int_{V_i} |y - x_i|^2 dy.  num_lloyd <= 0 / num_newton <= 0 skip their phase.  DESIGN.md §3 states the
+    definitions; geogram's initial sampling and HLBFGS, which the reference uses, cannot be reproduced.
+"""
+
+
+def lloyd_2d(n, num_lloyd=10, num_newton=10, *, device=None):
+    return _lloyd(n, num_lloyd, num_newton, 2, device)
+
+
+def lloyd_3d(n, num_lloyd=10, num_newton=10, *, device=None):
+    return _lloyd(n, num_lloyd, num_newton, 3, device)
+
+
+lloyd_2d.__doc__ = """
+    Generate n samples in the unit square, [0, 1]^2 using Lloyd's algorithm
+    (https://en.wikipedia.org/wiki/Lloyd%27s_algorithm).
+
+    Args:
+      n : The number of 2d point samples to generate
+      num_lloyd : The number of Lloyd iterations to do (default 10)
+      num_newton : The number of Newton iterations to do when computing Voronoi diagrams (default 10)
+      device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+      lloyd_points : a (n, 2)-shaped float64 numpy array of point samples in the unit square [0, 1]^2
+""" + _LLOYD_DEFINITION
+
+lloyd_3d.__doc__ = """
+    Generate n samples in the unit cube, [0, 1]^3 using Lloyd's algorithm
+    (https://en.wikipedia.org/wiki/Lloyd%27s_algorithm).
+
+    Args:
+      n : The number of 3d point samples to generate
+      num_lloyd : The number of Lloyd iterations to do (default 10)
+      num_newton : The number of Newton iterations to do when computing Voronoi diagrams (default 10)
+      device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+      lloyd_pts : a (n, 3)-shaped float64 numpy array of point samples in the unit cube [0, 1]^3
+""" + _LLOYD_DEFINITION

@@ -24,6 +24,7 @@
 #include <stdexcept>
 #include <string>
 #include <tuple>
+#include <vector>
 
 #include "../../include/pcu_b200.h"
 
@@ -511,6 +512,30 @@ void poisson_disk_device(bool is_f64, uintptr_t points, int64_t n, double radius
                       : pcu_b200_poisson_disk_f32(ws, (const float*)points, n, radius, seed, (int32_t*)out_idx,
                                                   (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream);
     });
+}
+
+// Voronoi centroids of device seeds (n, dim) fp64 -> device out (and the cells' moments, (n, 5), when out_moments is
+// not 0); returns the cells each pass handled.
+py::tuple voronoi_centroids_device(uintptr_t centers, int64_t n, int dim, uintptr_t out, uintptr_t out_moments, int device,
+                                   uintptr_t stream) {
+    int64_t passes[3] = {0, 0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_voronoi_centroids(ws, (const double*)centers, n, dim, (double*)out, (double*)out_moments, passes,
+                                          (void*)stream);
+    });
+    return py::make_tuple(passes[0], passes[1], passes[2]);
+}
+
+// Lloyd relaxation into device out (n, dim) fp64; returns (energies of the Newton phase, cells each pass handled).
+py::tuple lloyd_device(int64_t n, int dim, uint32_t seed, int num_lloyd, int num_newton, uintptr_t out, int device, uintptr_t stream) {
+    int64_t passes[3] = {0, 0, 0};
+    int32_t steps = 0;
+    std::vector<double> energy((size_t)std::max(num_newton, 0) + 1, 0.0);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_lloyd(ws, n, dim, seed, num_lloyd, num_newton, (double*)out, energy.data(), &steps, passes, (void*)stream);
+    });
+    energy.resize(num_newton > 0 ? (size_t)steps + 1 : 0);
+    return py::make_tuple(energy, py::make_tuple(passes[0], passes[1], passes[2]));
 }
 
 // Mesh sampling (sample_mesh_random / sample_mesh_poisson_disk, _mesh_sampling.py).  f_kind: 0 int32, 1 int64,
@@ -1295,6 +1320,8 @@ PYBIND11_MODULE(_pcu_internal, mod) {
             "Indices of the kept points and their unit normals (plane fit to the points in a ball around each point).");
     mod.def("_normals_ball_device", &normals_ball_device);
     mod.def("_poisson_disk_device", &poisson_disk_device);
+    mod.def("_voronoi_centroids_device", &voronoi_centroids_device);
+    mod.def("_lloyd_device", &lloyd_device);
     mod.def("_mesh_area_device", &mesh_area_device);
     mod.def("_sample_mesh_random_device", &sample_mesh_random_device);
     mod.def("_closest_points_on_mesh_device", &closest_points_on_mesh_device);

@@ -42,6 +42,7 @@
 #include "mesh_topology.cuh"
 #include "orient.cuh"
 #include "laplacian.cuh"
+#include "voronoi.cuh"
 
 using namespace pcu;
 
@@ -203,9 +204,12 @@ enum Scratch {
     kAux,     // intermediate results (normals, Poisson disk) that outlive a nested call's re-carving of the arena
     kMesh,    // the face CDF and dense samples of mesh Poisson-disk sampling, which outlive the point-cloud Poisson-disk
               // call it makes (that one re-carves the arena and aux)
+    kVorList, // the Voronoi cells' fallback passes (rows, queries, longer neighbour lists), sized once the first pass is done
+    kLloyd,   // the points, L-BFGS history and sync record of a Lloyd relaxation, which outlive every cell evaluation
     kScratchBlocks
 };
-static const char* const kScratchName[kScratchBlocks] = {"scratch", "staging", "intermediate scratch", "mesh-sampling scratch"};
+static const char* const kScratchName[kScratchBlocks] = {"scratch", "staging", "intermediate scratch", "mesh-sampling scratch",
+                                                         "Voronoi fallback scratch", "Lloyd scratch"};
 
 struct pcu_b200_workspace {
     int device = 0;
@@ -829,7 +833,8 @@ template <> const Cloud<double>& cloud_desc<double>(const pcu_b200_cloud* c) { r
 // ---- k nearest neighbours ---------------------------------------------------------------------
 template <typename T>
 int knn_device(pcu_b200_workspace* ws, const T* query, long long n, const T* dataset, long long m, int k, int squared,
-               T* out_dist, long long* out_idx, long long* out_n_tied, cudaStream_t stream, pcu_b200_cloud* prepared = nullptr) {
+               T* out_dist, long long* out_idx, long long* out_n_tied, cudaStream_t stream, pcu_b200_cloud* prepared = nullptr,
+               bool tie_replay = true) {
     if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
     if (k <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid value for k (%d) must be greater than 0.", k);
     if (prepared != nullptr) {
@@ -851,8 +856,11 @@ int knn_device(pcu_b200_workspace* ws, const T* query, long long n, const T* dat
     spec.out_dist = out_dist; spec.out_idx = out_idx;
     const int leaf = ws->opts.max_points_per_leaf > 0 ? ws->opts.max_points_per_leaf : 10;
     // a prepared cloud that owns the reference tree (same leaf size) spares the call the build
-    const bool own_tree = prepared != nullptr && prepared->leaf == leaf && ws->opts.disable_tie_replay == 0;
-    spec.replay_points = (ws->opts.disable_tie_replay == 1 || own_tree) ? 0 : m;
+    // tie_replay = false: callers to whom the order among equidistant neighbours does not matter (the Voronoi cells)
+    // skip the replay without touching the workspace option
+    const bool replay = tie_replay && ws->opts.disable_tie_replay != 1;
+    const bool own_tree = replay && prepared != nullptr && prepared->leaf == leaf && ws->opts.disable_tie_replay == 0;
+    spec.replay_points = (!replay || own_tree) ? 0 : m;
     spec.prepared_second = prepared != nullptr;
     Plan<T> plan;
     PCU_TRY(prepare_plan(ws, plan, spec, stream));
@@ -891,7 +899,7 @@ int knn_device(pcu_b200_workspace* ws, const T* query, long long n, const T* dat
                                                       plan.args.sweep[0].counters + 1, n, out_dist, out_idx, stream, g_launches);
         if (rs != PCU_B200_OK) return fail(rs, "tie replay failed: %s", cudaGetErrorString(cudaGetLastError()));
         ws->replay_overflows = tree.overflows;
-    } else if (ws->opts.disable_tie_replay != 1) {
+    } else if (replay) {
         const int rs = enqueue_tie_replay<T>(plan.replay, query, dataset, m, k, squared, leaf, plan.args.sweep[0].tie_list,
                                              plan.args.sweep[0].counters + 1, n, out_dist, out_idx, ws->opts.disable_tie_replay, stream, g_launches);
         if (rs != PCU_B200_OK) return fail(rs, "tie replay failed: %s", cudaGetErrorString(cudaGetLastError()));
@@ -1787,6 +1795,195 @@ int read_record(const R* dev, R* host, cudaStream_t stream) {
 // The failure of a call that found `bad` faces with a corner outside [0, #v).
 int bad_corners(unsigned long long bad) {
     return fail(PCU_B200_INVALID_ARGUMENT, "Invalid face indices: %llu faces have a corner outside [0, #v)", bad);
+}
+
+// ---- Voronoi cells in the unit cube / square and Lloyd relaxation (voronoi.cuh) ----------------------------------
+// One evaluation of the cells of n seeds (fp64, (n, dim)):
+//   pass 1  the seeds' self k-NN (k = 64 in 3-D, 24 in 2-D; no tie replay: the order among equidistant neighbours
+//           cannot change a cell, and the certificate only reads the k-th distance), then every cell on the thread's
+//           stack at 96 (3-D) / 48 (2-D) vertices;
+//   pass 2  the cells pass 1 left uncertified, compacted in ascending order: their k-NN with k = 160 (3-D) / 64 (2-D),
+//           at 252 / 250 vertices;
+//   pass 3  what pass 2 left: its list, then every seed that can still cut the cell, with the cell in device memory at
+//           2 048 (3-D) / 1 024 (2-D) vertices; the cells that outgrow it are compacted and redone at twice the
+//           capacity, until every cell is certified.
+// The host reads the count after pass 1 (one synchronisation), after pass 2 when it ran, and after every round of
+// pass 3.  passes[p] += cells handled by pass p (pass 3: summed over its rounds).
+constexpr int kVorK1[2] = {24, 64}, kVorK2[2] = {64, 160};   // by dim - 2
+constexpr int kVorSmall[2] = {48, 96}, kVorLarge[2] = {250, 252};
+constexpr int kVorWide[2] = {1024, 2048};
+constexpr int kVorWideMax = 1 << 22;   // vertices of one cell: 150 MB of device memory in 3-D
+
+// pass 0, 1: the small and the large capacity on the stack
+template <int D>
+int vor_pass_launch(const VorPass& p, int pass, cudaStream_t stream) {
+    const unsigned blocks = (unsigned)((p.count + kVorThreads - 1) / kVorThreads);
+    if (pass == 0) PCU_LAUNCH((vor_clip_kernel<D, kVorSmall[D - 2]>), blocks, kVorThreads, stream, p);
+    else           PCU_LAUNCH((vor_clip_kernel<D, kVorLarge[D - 2]>), blocks, kVorThreads, stream, p);
+    return PCU_B200_OK;
+}
+
+template <int D>
+int vor_eval(pcu_b200_workspace* ws, const double* x, long long n, VorSync* sync, double** mom_out, long long* passes,
+             VorSync* seen, cudaStream_t stream) {
+    const int k1 = (int)std::min<long long>(kVorK1[D - 2], n), k2 = (int)std::min<long long>(kVorK2[D - 2], n);
+    double *x3 = nullptr, *mom, *d1; long long* i1; unsigned char* flag; unsigned* counts;
+    PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
+        if (D == 2) x3 = cv.take<double>((size_t)3 * n);
+        mom = cv.take<double>((size_t)kVorMoments * n);
+        d1 = cv.take<double>((size_t)k1 * n);
+        i1 = cv.take<long long>((size_t)k1 * n);
+        flag = cv.take<unsigned char>((size_t)n);
+        counts = cv.take<unsigned>(keep_count_words(n));
+    }));
+    if (D == 3) x3 = (double*)x;
+    else PCU_LAUNCH(vor_lift_kernel, blocks_for(n), kThreads, stream, x, n, x3);
+    *mom_out = mom;
+    PCU_TRY(knn_device<double>(ws, x3, n, x3, n, k1, 1, d1, i1, nullptr, stream, nullptr, false));
+    VorPass p{};
+    p.x = x; p.x3 = x3; p.n = n; p.count = n; p.nn_idx = i1; p.nn_d2 = d1; p.k = k1; p.list_is_all = k1 >= n;
+    p.mom = mom; p.uncert = flag;
+    PCU_TRY(vor_pass_launch<D>(p, 0, stream));
+    passes[0] += n;
+    PCU_TRY(enqueue_keep_offsets(flag, n, counts, &sync->count, stream));
+    PCU_TRY(read_record(sync, seen, stream));
+    const long long c1 = seen->count;
+    if (c1 == 0) return PCU_B200_OK;
+    int *rows, *sub[2]; double *q, *d2; long long* i2; unsigned char* flag2; unsigned* counts2;
+    PCU_TRY(carve_scratch(ws, kVorList, stream, [&](Carver& cv) {
+        rows = cv.take<int>((size_t)c1);
+        sub[0] = cv.take<int>((size_t)c1);
+        sub[1] = cv.take<int>((size_t)c1);
+        q = cv.take<double>((size_t)3 * c1);
+        d2 = cv.take<double>((size_t)k2 * c1);
+        i2 = cv.take<long long>((size_t)k2 * c1);
+        flag2 = cv.take<unsigned char>((size_t)c1);
+        counts2 = cv.take<unsigned>(keep_count_words(c1));
+    }));
+    PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(n), kThreads, stream, (const unsigned char*)flag, n, (const unsigned*)counts, rows);
+    PCU_LAUNCH(vor_gather_kernel, blocks_for(c1), kThreads, stream, (const double*)x3, (const int*)rows, c1, q);
+    PCU_TRY(knn_device<double>(ws, q, c1, x3, n, k2, 1, d2, i2, nullptr, stream, nullptr, false));
+    p.rows = rows; p.count = c1; p.nn_idx = i2; p.nn_d2 = d2; p.k = k2; p.list_is_all = k2 >= n; p.uncert = flag2;
+    PCU_TRY(vor_pass_launch<D>(p, 1, stream));
+    passes[1] += c1;
+    PCU_TRY(enqueue_keep_offsets(flag2, c1, counts2, &sync->count, stream));
+    PCU_TRY(read_record(sync, seen, stream));
+    long long cnt = seen->count;
+    if (cnt == 0) return PCU_B200_OK;
+    // the last resort; sub[r & 1]: the pass-2 entries of round r
+    PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(c1), kThreads, stream, (const unsigned char*)flag2, c1, (const unsigned*)counts2, sub[0]);
+    p.scan_all = 1; p.list_is_all = 0; p.uncert = flag2;
+    for (int V = kVorWide[D - 2], r = 0;; V *= 2, ++r) {
+        if (V > kVorWideMax)
+            return fail(PCU_B200_OUT_OF_MEMORY, "voronoi: %lld cells have more than %d vertices", cnt, kVorWideMax);
+        // the cells live in the arena: the k-NN searches, its only other users here, are enqueued already
+        PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+            p.cells = cv.take<unsigned char>((size_t)cnt * vor_cell_bytes<D>(V));
+        }));
+        p.sub = sub[r & 1]; p.count = cnt;
+        PCU_LAUNCH(vor_clip_wide_kernel<D>, (unsigned)((cnt + kVorThreads - 1) / kVorThreads), kVorThreads, stream, p, V);
+        passes[2] += cnt;
+        PCU_TRY(enqueue_keep_offsets(flag2, cnt, counts2, &sync->count, stream));
+        PCU_TRY(read_record(sync, seen, stream));
+        if (seen->count == 0) break;
+        PCU_LAUNCH(vor_keep_sub_kernel, blocks_for(cnt), kThreads, stream, (const unsigned char*)flag2, cnt, (const unsigned*)counts2,
+                   (const int*)sub[r & 1], sub[(r + 1) & 1]);
+        cnt = seen->count;
+    }
+    return PCU_B200_OK;
+}
+
+int vor_check(long long n, int dim) {
+    if (dim != 2 && dim != 3) return fail(PCU_B200_INVALID_ARGUMENT, "voronoi: dim must be 2 or 3, got %d", dim);
+    if (n > 0x7fffffffLL - 1) return fail(PCU_B200_INVALID_ARGUMENT, "voronoi: at most 2^31 - 2 seeds, got %lld", n);
+    return PCU_B200_OK;
+}
+
+template <int D>
+int voronoi_centroids_device(pcu_b200_workspace* ws, const double* x, long long n, double* out, double* out_moments,
+                             long long* passes, cudaStream_t stream) {
+    VorSync* sync;
+    PCU_TRY(carve_scratch(ws, kLloyd, stream, [&](Carver& cv) { sync = cv.take<VorSync>(1); }));
+    PCU_CUDA(cudaMemsetAsync(sync, 0, sizeof(VorSync), stream));
+    double* mom; VorSync seen;
+    PCU_TRY(vor_eval<D>(ws, x, n, sync, &mom, passes, &seen, stream));
+    PCU_LAUNCH(vor_centroid_kernel<D>, blocks_for(n), kThreads, stream, x, n, (const double*)mom, out);
+    if (out_moments)
+        PCU_CUDA(cudaMemcpyAsync(out_moments, mom, (size_t)n * kVorMoments * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    return PCU_B200_OK;
+}
+
+// Blocks of the cooperative L-BFGS step: at most 4 per SM, no more than the vectors need.
+int lbfgs_grid_blocks(const pcu_b200_workspace* ws, long long N, unsigned* out_blocks) {
+    int fit = 0;
+    PCU_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&fit, lbfgs_step_kernel, kThreads, 0));
+    if (fit < 1) return fail(PCU_B200_CUDA_ERROR, "lbfgs_step_kernel cannot be resident on this device");
+    const long long want = (N + kThreads - 1) / kThreads;
+    *out_blocks = (unsigned)std::max<long long>(1, std::min<long long>(want, (long long)std::min(4, fit) * ws->sm_count));
+    return PCU_B200_OK;
+}
+
+// The initial sample, num_lloyd Lloyd steps, then the Newton phase (L-BFGS, voronoi.cuh).  Synchronisations: those
+// of every cell evaluation (one, plus one per fallback pass or last-resort round that runs), one for the initial
+// L-BFGS state, one after every L-BFGS step (its verdict decides whether the trial point is evaluated), and one for
+// the energies at the end.
+template <int D>
+int lloyd_device(pcu_b200_workspace* ws, long long n, unsigned seed, int num_lloyd, int num_newton, double* out,
+                 double* energy_host, int* iters_host, long long* passes, cudaStream_t stream) {
+    const long long N = n * D;
+    const bool newton = num_newton > 0;
+    unsigned blocks = 1;
+    if (newton) PCU_TRY(lbfgs_grid_blocks(ws, N, &blocks));
+    double *x, *x_acc = nullptr, *g = nullptr, *p = nullptr, *S = nullptr, *Y = nullptr, *partial = nullptr, *energy = nullptr;
+    LbState* st = nullptr; VorSync* sync;
+    PCU_TRY(carve_scratch(ws, kLloyd, stream, [&](Carver& cv) {
+        sync = cv.take<VorSync>(1);
+        x = cv.take<double>((size_t)N);
+        if (newton) {
+            st = cv.take<LbState>(1);
+            energy = cv.take<double>((size_t)num_newton + 1);
+            partial = cv.take<double>((size_t)2 * blocks);
+            x_acc = cv.take<double>((size_t)N);
+            g = cv.take<double>((size_t)N);
+            p = cv.take<double>((size_t)N);
+            S = cv.take<double>((size_t)kLbSlots * N);
+            Y = cv.take<double>((size_t)kLbSlots * N);
+        }
+    }));
+    PCU_CUDA(cudaMemsetAsync(sync, 0, sizeof(VorSync), stream));
+    PCU_LAUNCH(lloyd_init_kernel, blocks_for(N), kThreads, stream, seed, N, x);
+    double* mom; VorSync seen;
+    for (int it = 0; it < num_lloyd; ++it) {
+        PCU_TRY(vor_eval<D>(ws, x, n, sync, &mom, passes, &seen, stream));
+        PCU_LAUNCH(vor_centroid_kernel<D>, blocks_for(n), kThreads, stream, (const double*)x, n, (const double*)mom, x);
+    }
+    if (!newton) {
+        PCU_CUDA(cudaMemcpyAsync(out, x, (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+        if (iters_host) *iters_host = 0;
+        return PCU_B200_OK;
+    }
+    LbState s0{};
+    s0.t = 1.0; s0.gamma = 1.0; s0.init = 1;
+    PCU_CUDA(cudaMemcpyAsync(st, &s0, sizeof(LbState), cudaMemcpyHostToDevice, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));   // s0 lives on this stack
+    LbArgs a{};
+    a.n = n; a.D = D; a.x_acc = x_acc; a.g = g; a.x_t = x; a.p = p; a.S = S; a.Y = Y; a.partial = partial;
+    a.st = st; a.sync = sync; a.energy = energy; a.num_newton = num_newton;
+    PCU_TRY(vor_eval<D>(ws, x, n, sync, &mom, passes, &seen, stream));
+    for (;;) {
+        a.mom = mom;
+        void* args[] = {(void*)&a};
+        PCU_CUDA(cudaLaunchCooperativeKernel((void*)lbfgs_step_kernel, dim3(blocks), dim3(kThreads), args, 0, stream));
+        g_launches.fetch_add(1, std::memory_order_relaxed);
+        PCU_TRY(read_record(sync, &seen, stream));   // the step's verdict: evaluate its trial point, or stop
+        if (seen.done) break;
+        PCU_TRY(vor_eval<D>(ws, x, n, sync, &mom, passes, &seen, stream));
+    }
+    PCU_CUDA(cudaMemcpyAsync(out, x_acc, (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    if (energy_host) PCU_CUDA(cudaMemcpyAsync(energy_host, energy, ((size_t)seen.iter + 1) * sizeof(double), cudaMemcpyDeviceToHost, stream));
+    PCU_CUDA(cudaStreamSynchronize(stream));
+    if (iters_host) *iters_host = seen.iter;
+    return PCU_B200_OK;
 }
 
 // Whether face indices of this kind are 64 bits wide.
@@ -3417,6 +3614,34 @@ int pcu_b200_poisson_disk_f32(pcu_b200_workspace* ws, const float* points, int64
 int pcu_b200_poisson_disk_f64(pcu_b200_workspace* ws, const double* points, int64_t n, double radius, uint32_t seed,
                               int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream) {
     return poisson_disk_device<double>(ws, points, n, radius, seed, out_idx, (long long*)out_count, out_rounds, (cudaStream_t)stream);
+}
+
+int pcu_b200_voronoi_centroids(pcu_b200_workspace* ws, const double* centers, int64_t n, int dim, double* out_centroids,
+                               double* out_moments, int64_t* out_passes, void* stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(vor_check(n, dim));
+    if (n <= 0 || !centers || !out_centroids) return fail(PCU_B200_INVALID_ARGUMENT, "voronoi: n >= 1 seeds and non-null pointers required");
+    PCU_ON_DEVICE(ws);
+    long long passes[3] = {0, 0, 0};
+    const int rs = dim == 3 ? voronoi_centroids_device<3>(ws, centers, n, out_centroids, out_moments, passes, (cudaStream_t)stream)
+                            : voronoi_centroids_device<2>(ws, centers, n, out_centroids, out_moments, passes, (cudaStream_t)stream);
+    if (out_passes) for (int i = 0; i < 3; ++i) out_passes[i] = passes[i];
+    return rs;
+}
+int pcu_b200_lloyd(pcu_b200_workspace* ws, int64_t n, int dim, uint32_t seed, int num_lloyd, int num_newton, double* out_points,
+                   double* out_energy, int32_t* out_newton_steps, int64_t* out_passes, void* stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(vor_check(n, dim));
+    if (n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "n must be a positive integer. Got n = %lld", (long long)n);
+    if (!out_points) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    long long passes[3] = {0, 0, 0};
+    int steps = 0;
+    const int rs = dim == 3 ? lloyd_device<3>(ws, n, seed, num_lloyd, num_newton, out_points, out_energy, &steps, passes, (cudaStream_t)stream)
+                            : lloyd_device<2>(ws, n, seed, num_lloyd, num_newton, out_points, out_energy, &steps, passes, (cudaStream_t)stream);
+    if (out_passes) for (int i = 0; i < 3; ++i) out_passes[i] = passes[i];
+    if (out_newton_steps) *out_newton_steps = steps;
+    return rs;
 }
 
 int pcu_b200_mesh_area_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
