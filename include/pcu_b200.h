@@ -430,7 +430,8 @@ int pcu_b200_closest_points_on_mesh_f64(pcu_b200_workspace* ws, const double* p,
  *     (v, f, q_i) alone.
  *   signed_distance_to_mesh: out_fidx (int32) and out_bc are those of closest_points_on_mesh; out_s[i] =
  *     fl(fl(1 - 2|w_i|) d_i), w_i the winding number at accuracy_scale 2.  Queries whose squared distance lies outside
- *     libigl's band of (lower_bound, upper_bound) get out_s = NaN, out_fidx = nf + 1, out_bc = NaN.
+ *     libigl's band of (lower_bound, upper_bound) get out_s = NaN, out_fidx = nf + 1, out_bc = NaN.  The bounds are
+ *     float, as the reference binding's are.
  * Faces with a corner outside [0, nv) are left out and counted in *out_bad (device uint64); when it is not zero the
  * outputs are unspecified.  Every pointer is a DEVICE pointer and the call is stream-ordered. */
 int pcu_b200_fast_winding_number_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,

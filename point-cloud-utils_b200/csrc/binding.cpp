@@ -1,15 +1,15 @@
-// binding.cpp -- pybind11 module `_pcu_internal`: the Python-facing mirror of the two bindings the
-// reference generates with numpyeigen for this path,
-//     k_nearest_neighbors           /root/reference/src/point_cloud_distance.cpp:123-164
-//     one_sided_hausdorff_distance  /root/reference/src/point_cloud_distance.cpp:186-234
-// with the same argument names, defaults, dtype rules (float32 / float64, both clouds alike),
-// shape rules ((n, 3), n > 0), error type (ValueError), int64 indices and squeezed outputs
-// (tests/test_examples.py:363-368).  All computation goes through the C ABI of libpcu_b200.so
-// (include/pcu_b200.h); there is no CPU implementation behind these functions.
-//
-// Besides the numpy entry points the module exposes raw-pointer variants (`*_device`) that the
-// Python package uses for CUDA torch tensors: the caller passes data_ptr()s and a stream handle,
-// nothing is copied and nothing synchronises.
+// binding.cpp -- pybind11 module `_pcu_internal`, the layer between the Python package and the C ABI of
+// libpcu_b200.so (include/pcu_b200.h).  All computation goes through that ABI; there is no CPU implementation
+// behind these functions.  The module has three kinds of functions:
+//   - numpy entry points, which run the library's host entry points.  Those named after the reference's numpyeigen
+//     bindings (k_nearest_neighbors, one_sided_hausdorff_distance, the normal estimators, the Morton-code functions)
+//     keep its argument names, defaults, dtype and shape rules, error type (ValueError), int64 indices and squeezed
+//     outputs; the underscored ones (_chamfer_stats, _cloud_prepare, ...) serve the Python package;
+//   - device entry points (`_*_device`), which the Python package uses for CUDA torch tensors: the caller passes
+//     data_ptr()s, a device and a stream handle; nothing is copied and nothing synchronises unless the C entry point
+//     says so.  Those that only forward to the C ABI are generated from the C signatures (Forward below); the rest
+//     build host arrays or option structs, or return handles, counts or vectors;
+//   - handle destroyers and diagnostics.
 #include <pybind11/pybind11.h>
 #include <pybind11/numpy.h>
 #include <pybind11/stl.h>
@@ -24,6 +24,8 @@
 #include <stdexcept>
 #include <string>
 #include <tuple>
+#include <type_traits>
+#include <utility>
 #include <vector>
 
 #include "../../include/pcu_b200.h"
@@ -211,6 +213,75 @@ void on_workspace(int device, uintptr_t key, int leaf, F&& call) {
     check(status);
 }
 
+// The _f32 or the _f64 entry point of a pair, for inputs of type T.
+template <typename T, class F32, class F64>
+auto pick(F32 f32, F64 f64) {
+    static_assert(std::is_same_v<T, float> || std::is_same_v<T, double>, "inputs are float or double");
+    if constexpr (std::is_same_v<T, float>) return f32;
+    else return f64;
+}
+
+// Device bindings that only forward to one C entry point int f(pcu_b200_workspace*, A..., void* stream), or to one of a
+// pair f_f32 / f_f64, are built from that signature.  The Python function takes ([is_f64,] A'..., [max_points_per_leaf,]
+// device, stream), A' being A with every pointer passed as an integer address; it runs f on the workspace of (device,
+// stream), with each address converted to f's own parameter type and stream passed on as f's stream.
+template <class F> struct CParams;
+template <class... A> struct CParams<int (*)(pcu_b200_workspace*, A...)> { using type = std::tuple<A...>; };
+template <class F, size_t I> using c_param_t = std::tuple_element_t<I, typename CParams<F>::type>;
+template <class F> constexpr size_t c_arity = std::tuple_size_v<typename CParams<F>::type>;
+template <class T> using py_param_t = std::conditional_t<std::is_pointer_v<T>, uintptr_t, T>;
+template <class T> T from_py(py_param_t<T> a) {
+    if constexpr (std::is_pointer_v<T>) return reinterpret_cast<T>(a);
+    else return a;
+}
+template <class A, class B> constexpr bool same_up_to_pointee = std::is_pointer_v<A> ? std::is_pointer_v<B> : std::is_same_v<A, B>;
+
+template <class F32, class F64, class = std::make_index_sequence<c_arity<F32> - 1>> struct Forward;
+template <class F32, class F64, size_t... I> struct Forward<F32, F64, std::index_sequence<I...>> {
+    static_assert(std::is_same_v<c_param_t<F32, sizeof...(I)>, void*>, "an entry point's last parameter is its stream");
+    static_assert(c_arity<F64> == c_arity<F32> && (same_up_to_pointee<c_param_t<F32, I>, c_param_t<F64, I>> && ...),
+                  "the _f32 and _f64 entry points differ only in pointer types");
+    F32 f32;
+    F64 f64;
+
+    void run(bool is_f64, int leaf, int device, uintptr_t stream, py_param_t<c_param_t<F32, I>>... a) const {
+        on_workspace(device, stream, leaf, [&](pcu_b200_workspace* ws) {
+            return is_f64 ? f64(ws, from_py<c_param_t<F64, I>>(a)..., (void*)stream)
+                          : f32(ws, from_py<c_param_t<F32, I>>(a)..., (void*)stream);
+        });
+    }
+    auto single() const {
+        return [e = *this](py_param_t<c_param_t<F32, I>>... a, int device, uintptr_t stream) {
+            e.run(false, kDefaultLeaf, device, stream, a...);
+        };
+    }
+    auto single_with_leaf() const {
+        return [e = *this](py_param_t<c_param_t<F32, I>>... a, int max_points_per_leaf, int device, uintptr_t stream) {
+            e.run(false, max_points_per_leaf, device, stream, a...);
+        };
+    }
+    auto pair() const {
+        return [e = *this](bool is_f64, py_param_t<c_param_t<F32, I>>... a, int device, uintptr_t stream) {
+            e.run(is_f64, kDefaultLeaf, device, stream, a...);
+        };
+    }
+    auto pair_with_leaf() const {
+        return [e = *this](bool is_f64, py_param_t<c_param_t<F32, I>>... a, int max_points_per_leaf, int device, uintptr_t stream) {
+            e.run(is_f64, max_points_per_leaf, device, stream, a...);
+        };
+    }
+};
+template <class F> Forward<F, F> forward_to(F f) { return {f, f}; }
+template <class F32, class F64> Forward<F32, F64> forward_to(F32 f32, F64 f64) { return {f32, f64}; }
+
+// Frees a handle with the library's destroy function f, without the GIL.
+template <class H> auto destroy(int (*f)(H*)) {
+    return [f](uintptr_t handle) {
+        py::gil_scoped_release nogil;
+        f(reinterpret_cast<H*>(handle));
+    };
+}
+
 enum class Dt { f32, f64 };
 
 Dt common_dtype(const py::array& a, const py::array& b, const char* na, const char* nb) {
@@ -279,11 +350,8 @@ py::tuple knn_numpy(const py::array& q_in, const py::array& d_in, int k, bool sq
     py::array_t<int64_t> corrs = result_array<int64_t>((py::ssize_t)n, (py::ssize_t)k);
     int64_t tied = 0;
     on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        if (sizeof(T) == 4)
-            return pcu_b200_knn_host_f32(ws, (const float*)q.data(), n, (const float*)d.data(), m, k, squared,
-                                         (float*)dists.mutable_data(), corrs.mutable_data(), &tied);
-        return pcu_b200_knn_host_f64(ws, (const double*)q.data(), n, (const double*)d.data(), m, k, squared,
-                                     (double*)dists.mutable_data(), corrs.mutable_data(), &tied);
+        return pick<T>(pcu_b200_knn_host_f32, pcu_b200_knn_host_f64)(ws, q.data(), n, d.data(), m, k, squared, dists.mutable_data(),
+                                                                      corrs.mutable_data(), &tied);
     });
     // npe::move hands the matrix to numpy and squeezes every size-1 dimension
     // (pinned for (n, 1) -> (n,) by tests/test_examples.py:363-368)
@@ -322,9 +390,7 @@ pcu_b200_nn_stats one_sided_numpy(const py::array& s_in, const py::array& t_in, 
     auto t = dense<T>(t_in);
     pcu_b200_nn_stats st{};
     on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        if (sizeof(T) == 4)
-            return pcu_b200_nn_stats_host_f32(ws, (const float*)s.data(), s.shape(0), (const float*)t.data(), t.shape(0), &st);
-        return pcu_b200_nn_stats_host_f64(ws, (const double*)s.data(), s.shape(0), (const double*)t.data(), t.shape(0), &st);
+        return pick<T>(pcu_b200_nn_stats_host_f32, pcu_b200_nn_stats_host_f64)(ws, s.data(), s.shape(0), t.data(), t.shape(0), &st);
     });
     return st;
 }
@@ -349,31 +415,25 @@ py::object one_sided_hausdorff_distance(const py::array& source, const py::array
     return py::float_(value);
 }
 
+template <typename T>
+py::tuple chamfer_numpy(const py::array& x_in, const py::array& y_in, int leaf, int device) {
+    auto x = dense<T>(x_in);
+    auto y = dense<T>(y_in);
+    pcu_b200_nn_stats st[2] = {};
+    T v = 0;
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
+        return pick<T>(pcu_b200_chamfer_host_f32, pcu_b200_chamfer_host_f64)(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v);
+    });
+    return py::make_tuple(py::dtype::of<T>().attr("type")(v), stats_to_dict(st[0]), stats_to_dict(st[1]));
+}
+
 // Fused bidirectional sweep on numpy inputs: (chamfer value in input precision, stats x->y, stats y->x)
 py::tuple chamfer_stats(const py::array& x_in, const py::array& y_in, int max_points_per_leaf, int device) {
     const Dt dt = common_dtype(x_in, y_in, "x", "y");
     check_shapes(x_in, y_in, "x", "y");
     const int dev = current_device_or_default(device);
-    pcu_b200_nn_stats st[2] = {};
-    py::object value;
-    if (dt == Dt::f32) {
-        auto x = dense<float>(x_in);
-        auto y = dense<float>(y_in);
-        float v = 0.f;
-        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-            return pcu_b200_chamfer_host_f32(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v);
-        });
-        value = py::module_::import("numpy").attr("float32")(v);
-    } else {
-        auto x = dense<double>(x_in);
-        auto y = dense<double>(y_in);
-        double v = 0.0;
-        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-            return pcu_b200_chamfer_host_f64(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v);
-        });
-        value = py::module_::import("numpy").attr("float64")(v);
-    }
-    return py::make_tuple(value, stats_to_dict(st[0]), stats_to_dict(st[1]));
+    return dt == Dt::f32 ? chamfer_numpy<float>(x_in, y_in, max_points_per_leaf, dev)
+                         : chamfer_numpy<double>(x_in, y_in, max_points_per_leaf, dev);
 }
 
 // validate_input of the reference (src/point_cloud_normals.cpp:25-42) plus the npe dtype rule
@@ -408,11 +468,8 @@ py::tuple normals_knn_numpy(const py::array& p_in, const py::array& v_in, int k,
     py::array_t<T> normals({(py::ssize_t)n, (py::ssize_t)3});
     int64_t kept = 0;
     on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        if (sizeof(T) == 4)
-            return pcu_b200_normals_knn_host_f32(ws, (const float*)pts.data(), n, has_dirs ? (const float*)dirs.data() : nullptr, k,
-                                                 drop_angle, idx.mutable_data(), (float*)normals.mutable_data(), &kept);
-        return pcu_b200_normals_knn_host_f64(ws, (const double*)pts.data(), n, has_dirs ? (const double*)dirs.data() : nullptr, k,
-                                             drop_angle, idx.mutable_data(), (double*)normals.mutable_data(), &kept);
+        return pick<T>(pcu_b200_normals_knn_host_f32, pcu_b200_normals_knn_host_f64)(
+            ws, pts.data(), n, has_dirs ? dirs.data() : nullptr, k, drop_angle, idx.mutable_data(), normals.mutable_data(), &kept);
     });
     idx.resize({(py::ssize_t)kept});
     normals.resize({(py::ssize_t)kept, (py::ssize_t)3});
@@ -429,18 +486,6 @@ py::tuple estimate_point_cloud_normals_knn_internal(const py::array& points, con
     const int dev = current_device_or_default(device);
     return dt == Dt::f32 ? normals_knn_numpy<float>(points, view_dirs, num_neighbors, max_points_per_leaf, drop_angle_threshold, dev)
                          : normals_knn_numpy<double>(points, view_dirs, num_neighbors, max_points_per_leaf, drop_angle_threshold, dev);
-}
-
-void normals_knn_device(bool is_f64, uintptr_t points, int64_t n, uintptr_t view_dirs, int k, double drop_angle,
-                        uintptr_t out_idx, uintptr_t out_normals, uintptr_t out_count, int max_points_per_leaf, int device,
-                        uintptr_t stream) {
-    if (k <= 0) throw py::value_error("Invalid number of neighbors (" + std::to_string(k) + ") must be greater than 0.");
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_normals_knn_f64(ws, (const double*)points, n, (const double*)view_dirs, k, drop_angle,
-                                                 (int64_t*)out_idx, (double*)out_normals, (int64_t*)out_count, (void*)stream)
-                      : pcu_b200_normals_knn_f32(ws, (const float*)points, n, (const float*)view_dirs, k, drop_angle,
-                                                 (int64_t*)out_idx, (float*)out_normals, (int64_t*)out_count, (void*)stream);
-    });
 }
 
 // estimate_point_cloud_normals_ball_internal (src/point_cloud_normals.cpp:303-370), argument order of the reference
@@ -469,11 +514,8 @@ py::tuple normals_ball_numpy(const py::array& p_in, const py::array& v_in, const
     py::array_t<T> normals({(py::ssize_t)n, (py::ssize_t)3});
     int64_t kept = 0;
     on_workspace(device, kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        if (sizeof(T) == 4)
-            return pcu_b200_normals_ball_host_f32(ws, (const float*)pts.data(), n, has_dirs ? (const float*)dirs.data() : nullptr, &o,
-                                                  idx.mutable_data(), (float*)normals.mutable_data(), &kept);
-        return pcu_b200_normals_ball_host_f64(ws, (const double*)pts.data(), n, has_dirs ? (const double*)dirs.data() : nullptr, &o,
-                                              idx.mutable_data(), (double*)normals.mutable_data(), &kept);
+        return pick<T>(pcu_b200_normals_ball_host_f32, pcu_b200_normals_ball_host_f64)(
+            ws, pts.data(), n, has_dirs ? dirs.data() : nullptr, &o, idx.mutable_data(), normals.mutable_data(), &kept);
     });
     idx.resize({(py::ssize_t)kept});
     normals.resize({(py::ssize_t)kept, (py::ssize_t)3});
@@ -503,17 +545,6 @@ void normals_ball_device(bool is_f64, uintptr_t points, int64_t n, uintptr_t vie
     });
 }
 
-// One Poisson-disk sample of a device cloud at one radius (the search over radii is in _poisson.py).
-void poisson_disk_device(bool is_f64, uintptr_t points, int64_t n, double radius, uint32_t seed, uintptr_t out_idx,
-                         uintptr_t out_count, uintptr_t out_rounds, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_poisson_disk_f64(ws, (const double*)points, n, radius, seed, (int32_t*)out_idx,
-                                                  (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream)
-                      : pcu_b200_poisson_disk_f32(ws, (const float*)points, n, radius, seed, (int32_t*)out_idx,
-                                                  (int64_t*)out_count, (int32_t*)out_rounds, (void*)stream);
-    });
-}
-
 // Voronoi centroids of device seeds (n, dim) fp64 -> device out (and the cells' moments, (n, 5), when out_moments is
 // not 0); returns the cells each pass handled.
 py::tuple voronoi_centroids_device(uintptr_t centers, int64_t n, int dim, uintptr_t out, uintptr_t out_moments, int device,
@@ -538,102 +569,6 @@ py::tuple lloyd_device(int64_t n, int dim, uint32_t seed, int num_lloyd, int num
     return py::make_tuple(energy, py::make_tuple(passes[0], passes[1], passes[2]));
 }
 
-// Mesh sampling (sample_mesh_random / sample_mesh_poisson_disk, _mesh_sampling.py).  f_kind: 0 int32, 1 int64,
-// 2 uint32, 3 uint64; out_area: 3 device words {W, S, faces with a corner out of range}.
-void mesh_area_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out_area, int device,
-                      uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_mesh_area_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (pcu_b200_mesh_area*)out_area,
-                                               (void*)stream)
-                      : pcu_b200_mesh_area_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (pcu_b200_mesh_area*)out_area,
-                                               (void*)stream);
-    });
-}
-
-void sample_mesh_random_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int64_t num_samples,
-                               uint32_t seed, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_area, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_sample_mesh_random_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
-                                                        (void*)out_fidx, (double*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream)
-                      : pcu_b200_sample_mesh_random_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, num_samples, seed,
-                                                        (void*)out_fidx, (float*)out_bc, (pcu_b200_mesh_area*)out_area, (void*)stream);
-    });
-}
-
-void sample_mesh_poisson_disk_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, double radius,
-                                     int64_t n_dense, uint32_t seed, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_count,
-                                     int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_sample_mesh_poisson_disk_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, radius, n_dense,
-                                                              seed, (void*)out_fidx, (double*)out_bc, (int64_t*)out_count, (void*)stream)
-                      : pcu_b200_sample_mesh_poisson_disk_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, radius, n_dense,
-                                                              seed, (void*)out_fidx, (float*)out_bc, (int64_t*)out_count, (void*)stream);
-    });
-}
-
-// Closest points on a mesh (closest_points_on_mesh, _mesh_query.py); out_bad: one device uint64, the faces with a
-// corner out of range.
-void closest_points_on_mesh_device(bool is_f64, uintptr_t p, int64_t np, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind,
-                                   uintptr_t out_d, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_bad, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_closest_points_on_mesh_f64(ws, (const double*)p, np, (const double*)v, nv, (const void*)f, nf, f_kind,
-                                                            (double*)out_d, (void*)out_fidx, (double*)out_bc, (uint64_t*)out_bad,
-                                                            (void*)stream)
-                      : pcu_b200_closest_points_on_mesh_f32(ws, (const float*)p, np, (const float*)v, nv, (const void*)f, nf, f_kind,
-                                                            (float*)out_d, (void*)out_fidx, (float*)out_bc, (uint64_t*)out_bad,
-                                                            (void*)stream);
-    });
-}
-
-// Winding numbers (triangle_soup_fast_winding_number, _mesh_query.py); accuracy_scale: the far-field threshold.
-void fast_winding_number_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t q, int64_t nq,
-                                double accuracy_scale, uintptr_t out_w, uintptr_t out_bad, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_fast_winding_number_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (const double*)q, nq,
-                                                         accuracy_scale, (double*)out_w, (uint64_t*)out_bad, (void*)stream)
-                      : pcu_b200_fast_winding_number_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (const float*)q, nq,
-                                                         accuracy_scale, (float*)out_w, (uint64_t*)out_bad, (void*)stream);
-    });
-}
-
-// Winding numbers of an oriented point cloud (point_cloud_fast_winding_number, _mesh_query.py); a holds np values.
-void point_cloud_fast_winding_number_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t a, int64_t np, uintptr_t q, int64_t nq,
-                                            double accuracy_scale, uintptr_t out_w, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_point_cloud_fast_winding_number_f64(ws, (const double*)p, (const double*)n, (const double*)a, np,
-                                                                     (const double*)q, nq, accuracy_scale, (double*)out_w, (void*)stream)
-                      : pcu_b200_point_cloud_fast_winding_number_f32(ws, (const float*)p, (const float*)n, (const float*)a, np,
-                                                                     (const float*)q, nq, accuracy_scale, (float*)out_w, (void*)stream);
-    });
-}
-
-// Signed distances (signed_distance_to_mesh, _mesh_query.py); the bounds are float, as the reference binding's are.
-void signed_distance_to_mesh_device(bool is_f64, uintptr_t p, int64_t np, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind,
-                                    float lower_bound, float upper_bound, uintptr_t out_s, uintptr_t out_fidx, uintptr_t out_bc,
-                                    uintptr_t out_bad, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_signed_distance_to_mesh_f64(ws, (const double*)p, np, (const double*)v, nv, (const void*)f, nf, f_kind,
-                                                             lower_bound, upper_bound, (double*)out_s, (int32_t*)out_fidx,
-                                                             (double*)out_bc, (uint64_t*)out_bad, (void*)stream)
-                      : pcu_b200_signed_distance_to_mesh_f32(ws, (const float*)p, np, (const float*)v, nv, (const void*)f, nf, f_kind,
-                                                             lower_bound, upper_bound, (float*)out_s, (int32_t*)out_fidx,
-                                                             (float*)out_bc, (uint64_t*)out_bad, (void*)stream);
-    });
-}
-
-// Rays against a mesh (ray_mesh_intersection, _ray_mesh.py); o_stride 0: one origin; out_fidx has f's width.
-void ray_mesh_intersection_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t o, int o_stride,
-                                  uintptr_t d, int64_t n, float near, float far, uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_t,
-                                  uintptr_t out_bad, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_ray_mesh_intersection_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (const double*)o, o_stride,
-                                                           (const double*)d, n, near, far, (void*)out_fidx, (double*)out_bc,
-                                                           (double*)out_t, (uint64_t*)out_bad, (void*)stream)
-                      : pcu_b200_ray_mesh_intersection_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (const float*)o, o_stride,
-                                                           (const float*)d, n, near, far, (void*)out_fidx, (float*)out_bc,
-                                                           (float*)out_t, (uint64_t*)out_bad, (void*)stream);
-    });
-}
 // A prepared mesh (RayMeshIntersector); out_bad: one device uint64, the faces with a corner out of range.
 uintptr_t mesh_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out_bad, int device,
                               uintptr_t stream) {
@@ -646,36 +581,7 @@ uintptr_t mesh_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f,
     });
     return (uintptr_t)mesh;
 }
-void mesh_destroy(uintptr_t mesh) {
-    py::gil_scoped_release nogil;
-    pcu_b200_mesh_destroy((pcu_b200_mesh*)mesh);
-}
-// Rays of precision is_f64 against a prepared mesh of either precision; out_fidx is int32.
-void ray_mesh_prepared_device(bool is_f64, uintptr_t mesh, uintptr_t o, int o_stride, uintptr_t d, int64_t n, float near, float far,
-                              uintptr_t out_fidx, uintptr_t out_bc, uintptr_t out_t, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_ray_mesh_intersection_prepared_f64(ws, (const pcu_b200_mesh*)mesh, (const double*)o, o_stride,
-                                                                    (const double*)d, n, near, far, (int32_t*)out_fidx,
-                                                                    (double*)out_bc, (double*)out_t, (void*)stream)
-                      : pcu_b200_ray_mesh_intersection_prepared_f32(ws, (const pcu_b200_mesh*)mesh, (const float*)o, o_stride,
-                                                                    (const float*)d, n, near, far, (int32_t*)out_fidx,
-                                                                    (float*)out_bc, (float*)out_t, (void*)stream);
-    });
-}
 
-// Rays against surfels (ray_surfel_intersection, _ray_surfel.py); r holds np radii in p's dtype; out_pid is int32.
-void ray_surfel_intersection_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t r, int64_t np, int subdivs, uintptr_t o,
-                                    int o_stride, uintptr_t d, int64_t nr, float near, float far, uintptr_t out_pid, uintptr_t out_t,
-                                    int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_ray_surfel_intersection_f64(ws, (const double*)p, (const double*)n, (const double*)r, np, subdivs,
-                                                             (const double*)o, o_stride, (const double*)d, nr, near, far,
-                                                             (int32_t*)out_pid, (double*)out_t, (void*)stream)
-                      : pcu_b200_ray_surfel_intersection_f32(ws, (const float*)p, (const float*)n, (const float*)r, np, subdivs,
-                                                             (const float*)o, o_stride, (const float*)d, nr, near, far,
-                                                             (int32_t*)out_pid, (float*)out_t, (void*)stream);
-    });
-}
 // Prepared surfels (RaySurfelIntersector); freed by _mesh_destroy.
 uintptr_t surfel_prepare_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t r, int64_t np, int subdivs, int device, uintptr_t stream) {
     pcu_b200_mesh* h = nullptr;
@@ -684,28 +590,6 @@ uintptr_t surfel_prepare_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t
                       : pcu_b200_surfel_prepare_f32(ws, (const float*)p, (const float*)n, (const float*)r, np, subdivs, &h, (void*)stream);
     });
     return (uintptr_t)h;
-}
-// Rays of precision is_f64 against prepared surfels of either precision.
-void ray_surfel_prepared_device(bool is_f64, uintptr_t surfels, uintptr_t o, int o_stride, uintptr_t d, int64_t nr, float near, float far,
-                                uintptr_t out_pid, uintptr_t out_t, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_ray_surfel_intersection_prepared_f64(ws, (const pcu_b200_mesh*)surfels, (const double*)o, o_stride,
-                                                                      (const double*)d, nr, near, far, (int32_t*)out_pid, (double*)out_t,
-                                                                      (void*)stream)
-                      : pcu_b200_ray_surfel_intersection_prepared_f32(ws, (const pcu_b200_mesh*)surfels, (const float*)o, o_stride,
-                                                                      (const float*)d, nr, near, far, (int32_t*)out_pid, (float*)out_t,
-                                                                      (void*)stream);
-    });
-}
-// pointcloud_surfel_geometry: out_v ((subdivs + 1) np, 3) in p's dtype, out_f (subdivs np, 3) int32.
-void surfel_geometry_device(bool is_f64, uintptr_t p, uintptr_t n, uintptr_t r, int64_t np, int subdivs, uintptr_t out_v, uintptr_t out_f,
-                            int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_pointcloud_surfel_geometry_f64(ws, (const double*)p, (const double*)n, (const double*)r, np, subdivs,
-                                                                (double*)out_v, (int32_t*)out_f, (void*)stream)
-                      : pcu_b200_pointcloud_surfel_geometry_f32(ws, (const float*)p, (const float*)n, (const float*)r, np, subdivs,
-                                                                (float*)out_v, (int32_t*)out_f, (void*)stream);
-    });
 }
 
 // Marching cubes (marching_cubes_sparse_voxel_grid, _sparse_voxels.py): classifies and numbers the vertices (two
@@ -721,23 +605,6 @@ py::tuple marching_cubes_prepare_device(bool t_f64, uintptr_t scalars, bool s_f6
                                                            idx_kind, isovalue, &mc, counts, (void*)stream);
     });
     return py::make_tuple((uintptr_t)mc, counts[0], counts[1]);
-}
-void marching_cubes_emit_device(uintptr_t mc, uintptr_t out_v, uintptr_t out_f, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_marching_cubes_emit(ws, (const pcu_b200_marching_cubes*)mc, (void*)out_v, (void*)out_f, (void*)stream);
-    });
-}
-void marching_cubes_destroy(uintptr_t mc) {
-    py::gil_scoped_release nogil;
-    pcu_b200_marching_cubes_destroy((pcu_b200_marching_cubes*)mc);
-}
-// sparse_voxel_grid_boundary: out_idx (capacity n) int64, out_counts: two device int64 {boundary rows, rows out of range}.
-void sparse_voxel_grid_boundary_device(uintptr_t grid, int64_t n, int idx_kind, uintptr_t out_idx, uintptr_t out_counts, int device,
-                                       uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_sparse_voxel_grid_boundary(ws, (const void*)grid, n, idx_kind, (int64_t*)out_idx, (int64_t*)out_counts,
-                                                   (void*)stream);
-    });
 }
 
 // Sparse voxel grids (_sparse_voxels.py): one code-set handle, prepared from points, by a dilation round or from a grid's
@@ -773,22 +640,6 @@ py::tuple sparse_grid_hex_prepare_device(uintptr_t grid, int64_t n, int idx_kind
     });
     return py::make_tuple((uintptr_t)sg, counts[0], counts[1]);
 }
-void sparse_grid_emit_device(uintptr_t sg, uintptr_t out_rows, uintptr_t out_index, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_sparse_grid_emit(ws, (const pcu_b200_sparse_grid*)sg, (void*)out_rows, (int64_t*)out_index, (void*)stream);
-    });
-}
-void sparse_grid_destroy(uintptr_t sg) {
-    py::gil_scoped_release nogil;
-    pcu_b200_sparse_grid_destroy((pcu_b200_sparse_grid*)sg);
-}
-// erode_sparse_voxel_grid: out_grid (capacity n rows, the grid's kind), out_counts: two device int64 {kept rows, rows out
-// of range}.
-void sparse_grid_erode_device(uintptr_t grid, int64_t n, int idx_kind, uintptr_t out_grid, uintptr_t out_counts, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_sparse_grid_erode(ws, (const void*)grid, n, idx_kind, (void*)out_grid, (int64_t*)out_counts, (void*)stream);
-    });
-}
 // voxel_grid_geometry (_voxels.py): out_v (8 n, 3) float32, out_f (12 n, 3) int32; no synchronisation.
 void voxel_grid_geometry_device(uintptr_t ijk, int64_t n, int idx_kind, std::vector<double> size, std::vector<double> origin, double gap,
                                 uintptr_t out_v, uintptr_t out_f, int device, uintptr_t stream) {
@@ -814,22 +665,6 @@ py::tuple voxelize_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_
     });
     return py::make_tuple((uintptr_t)vx, counts[0], counts[1]);
 }
-void voxelize_emit_device(uintptr_t vx, uintptr_t out, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_voxelize_emit(ws, (const pcu_b200_voxelize*)vx, (int32_t*)out, (void*)stream);
-    });
-}
-void voxelize_destroy(uintptr_t vx) {
-    py::gil_scoped_release nogil;
-    pcu_b200_voxelize_destroy((pcu_b200_voxelize*)vx);
-}
-// flood_fill_3d: grid and out (w, h, d) C-ordered of grid_kind (pcu_b200_grid_kind); no synchronisation.
-void flood_fill_3d_device(uintptr_t grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t sx, int64_t sy, int64_t sz,
-                          double fill_value, uintptr_t out, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_flood_fill_3d(ws, (const void*)grid, grid_kind, w, h, d, sx, sy, sz, fill_value, (void*)out, (void*)stream);
-    });
-}
 
 // Connected components (connected_components, _mesh_topology.py): validates f and labels (two synchronisations of
 // `stream`), returns (handle, n = max(f) + 1, components); _connected_components_emit writes cv, nv, cf and nf in f's
@@ -841,17 +676,6 @@ py::tuple connected_components_prepare_device(uintptr_t f, int64_t nf, int f_col
         return pcu_b200_connected_components_prepare(ws, (const void*)f, nf, f_cols, f_kind, &cc, counts, (void*)stream);
     });
     return py::make_tuple((uintptr_t)cc, counts[0], counts[1]);
-}
-void connected_components_emit_device(uintptr_t cc, uintptr_t out_cv, uintptr_t out_nv, uintptr_t out_cf, uintptr_t out_nf, int device,
-                                      uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_connected_components_emit(ws, (const pcu_b200_components*)cc, (void*)out_cv, (void*)out_nv, (void*)out_cf,
-                                                  (void*)out_nf, (void*)stream);
-    });
-}
-void connected_components_destroy(uintptr_t cc) {
-    py::gil_scoped_release nogil;
-    pcu_b200_connected_components_destroy((pcu_b200_components*)cc);
 }
 // remove_mesh_vertices: out_v (capacity nv rows), out_f (capacity nf rows, f's width); one synchronisation; returns
 // (kept vertices, kept faces).
@@ -881,12 +705,6 @@ int64_t remove_unreferenced_device(bool is_f64, uintptr_t v, int64_t nv, uintptr
     });
     return kept;
 }
-// orient_mesh_faces: out_f (nf, 3) and out_components (nf) in f's width; no synchronisation.
-void orient_mesh_faces_device(uintptr_t f, int64_t nf, int f_kind, uintptr_t out_f, uintptr_t out_components, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_orient_mesh_faces(ws, (const void*)f, nf, f_kind, (void*)out_f, (void*)out_components, (void*)stream);
-    });
-}
 
 // mesh_face_areas (normal false) / estimate_mesh_face_normals (normal true): out (nf) or (nf, 3) in v's type; one
 // synchronisation.
@@ -898,16 +716,6 @@ void mesh_face_device(bool is_f64, bool normal, uintptr_t v, int64_t nv, uintptr
                           : pcu_b200_mesh_face_normals_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (float*)out, (void*)stream);
         return is_f64 ? pcu_b200_mesh_face_areas_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, (double*)out, (void*)stream)
                       : pcu_b200_mesh_face_areas_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, (float*)out, (void*)stream);
-    });
-}
-// estimate_mesh_vertex_normals: out (nv, 3) in v's type; weighting 0 uniform, 1 area, 2 angle; one synchronisation.
-void mesh_vertex_normals_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int weighting, uintptr_t out,
-                                int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_mesh_vertex_normals_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, weighting, (double*)out,
-                                                         (void*)stream)
-                      : pcu_b200_mesh_vertex_normals_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, weighting, (float*)out,
-                                                         (void*)stream);
     });
 }
 // laplacian_smooth_mesh: out (nv, 3) in v's type; returns (CG iterations of every step, largest relative residual of
@@ -1024,6 +832,18 @@ py::array morton_knn(const py::array& codes_in, const py::array& qcodes_in, int 
 }
 
 // ---- prepared clouds (handles travel as integers; point-cloud-utils_b200/__init__.py wraps them in PreparedCloud) ----
+template <typename T>
+pcu_b200_cloud* cloud_prepare_numpy_t(const py::array& pts_in, int knn_k, int leaf, int device) {
+    auto p = dense<T>(pts_in);
+    pcu_b200_cloud* cloud = nullptr;
+    on_workspace(device, kHostKey, leaf > 0 ? leaf : kDefaultLeaf, [&](pcu_b200_workspace* ws) {   // leaf 0: the library's default
+        if (knn_k > 0)
+            return pick<T>(pcu_b200_cloud_prepare_knn_host_f32, pcu_b200_cloud_prepare_knn_host_f64)(ws, p.data(), p.shape(0), knn_k, leaf,
+                                                                                                     &cloud);
+        return pick<T>(pcu_b200_cloud_prepare_host_f32, pcu_b200_cloud_prepare_host_f64)(ws, p.data(), p.shape(0), &cloud);
+    });
+    return cloud;
+}
 uintptr_t cloud_prepare_numpy(const py::array& pts_in, int device, int knn_k, int leaf) {
     const bool f32 = pts_in.dtype().is(py::dtype::of<float>()), f64 = pts_in.dtype().is(py::dtype::of<double>());
     if (!f32 && !f64)
@@ -1031,22 +851,8 @@ uintptr_t cloud_prepare_numpy(const py::array& pts_in, int device, int knn_k, in
     if (pts_in.ndim() != 2 || pts_in.shape(1) != 3 || pts_in.shape(0) == 0)
         throw py::value_error("Only 3D inputs are supported: points must have shape (n, 3) with n > 0.");
     const int dev = current_device_or_default(device);
-    const int call_leaf = leaf > 0 ? leaf : kDefaultLeaf;   // a leaf size of 0 asks the library for its default
-    pcu_b200_cloud* cloud = nullptr;
-    if (f32) {
-        auto p = dense<float>(pts_in);
-        on_workspace(dev, kHostKey, call_leaf, [&](pcu_b200_workspace* ws) {
-            return knn_k > 0 ? pcu_b200_cloud_prepare_knn_host_f32(ws, p.data(), p.shape(0), knn_k, leaf, &cloud)
-                             : pcu_b200_cloud_prepare_host_f32(ws, p.data(), p.shape(0), &cloud);
-        });
-    } else {
-        auto p = dense<double>(pts_in);
-        on_workspace(dev, kHostKey, call_leaf, [&](pcu_b200_workspace* ws) {
-            return knn_k > 0 ? pcu_b200_cloud_prepare_knn_host_f64(ws, p.data(), p.shape(0), knn_k, leaf, &cloud)
-                             : pcu_b200_cloud_prepare_host_f64(ws, p.data(), p.shape(0), &cloud);
-        });
-    }
-    return (uintptr_t)cloud;
+    return (uintptr_t)(f32 ? cloud_prepare_numpy_t<float>(pts_in, knn_k, leaf, dev)
+                           : cloud_prepare_numpy_t<double>(pts_in, knn_k, leaf, dev));
 }
 uintptr_t cloud_prepare_device(bool is_f64, uintptr_t pts, int64_t n, int device, uintptr_t stream, int knn_k, int leaf) {
     pcu_b200_cloud* cloud = nullptr;
@@ -1059,10 +865,6 @@ uintptr_t cloud_prepare_device(bool is_f64, uintptr_t pts, int64_t n, int device
     });
     return (uintptr_t)cloud;
 }
-void cloud_destroy(uintptr_t cloud) {
-    py::gil_scoped_release nogil;
-    pcu_b200_cloud_destroy((pcu_b200_cloud*)cloud);
-}
 // k nearest neighbours of numpy points in a prepared cloud: (dists, corrs) like k_nearest_neighbors
 template <typename T>
 py::tuple knn_prepared_numpy_t(const py::array& q_in, pcu_b200_cloud* cloud, int k, bool squared, int leaf, int device) {
@@ -1072,11 +874,8 @@ py::tuple knn_prepared_numpy_t(const py::array& q_in, pcu_b200_cloud* cloud, int
     py::array_t<int64_t> corrs = result_array<int64_t>((py::ssize_t)n, (py::ssize_t)k);
     int64_t tied = 0;
     on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        if (sizeof(T) == 4)
-            return pcu_b200_knn_prepared_host_f32(ws, (const float*)q.data(), n, cloud, k, squared, (float*)dists.mutable_data(),
-                                                  corrs.mutable_data(), &tied);
-        return pcu_b200_knn_prepared_host_f64(ws, (const double*)q.data(), n, cloud, k, squared, (double*)dists.mutable_data(),
-                                              corrs.mutable_data(), &tied);
+        return pick<T>(pcu_b200_knn_prepared_host_f32, pcu_b200_knn_prepared_host_f64)(ws, q.data(), n, cloud, k, squared,
+                                                                                        dists.mutable_data(), corrs.mutable_data(), &tied);
     });
     return py::make_tuple(dists.attr("squeeze")(), corrs.attr("squeeze")());
 }
@@ -1093,17 +892,19 @@ py::tuple knn_prepared_numpy(const py::array& q_in, uintptr_t cloud, bool cloud_
     return f32 ? knn_prepared_numpy_t<float>(q_in, (pcu_b200_cloud*)cloud, k, squared, max_points_per_leaf, dev)
                : knn_prepared_numpy_t<double>(q_in, (pcu_b200_cloud*)cloud, k, squared, max_points_per_leaf, dev);
 }
-void knn_prepared_device(bool is_f64, uintptr_t query, int64_t n, uintptr_t cloud, int k, bool squared, uintptr_t out_dist,
-                         uintptr_t out_idx, uintptr_t out_n_tied, int max_points_per_leaf, int device, uintptr_t stream) {
-    if (k <= 0) throw py::value_error("Invalid value for k (" + std::to_string(k) + ") must be greater than 0.");
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_knn_prepared_f64(ws, (const double*)query, n, (pcu_b200_cloud*)cloud, k, squared, (double*)out_dist,
-                                                  (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream)
-                      : pcu_b200_knn_prepared_f32(ws, (const float*)query, n, (pcu_b200_cloud*)cloud, k, squared, (float*)out_dist,
-                                                  (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream);
-    });
-}
 
+template <typename T>
+py::tuple stats_prepared_numpy_t(const py::array& x_in, const pcu_b200_cloud* y, bool both, int leaf, int device) {
+    auto x = dense<T>(x_in);
+    pcu_b200_nn_stats st[2] = {};
+    T v = 0;
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
+        return both ? pick<T>(pcu_b200_chamfer_prepared_host_f32, pcu_b200_chamfer_prepared_host_f64)(ws, x.data(), x.shape(0), y, st, &v)
+                    : pick<T>(pcu_b200_nn_stats_prepared_host_f32, pcu_b200_nn_stats_prepared_host_f64)(ws, x.data(), x.shape(0), y, st);
+    });
+    if (both) return py::make_tuple(py::dtype::of<T>().attr("type")(v), stats_to_dict(st[0]), stats_to_dict(st[1]));
+    return py::make_tuple(py::none(), stats_to_dict(st[0]));
+}
 // fused sweep(s) of numpy points against a prepared cloud: (value or None, stats[, stats])
 py::tuple stats_prepared_numpy(const py::array& x_in, uintptr_t cloud, bool cloud_is_f64, bool both, int max_points_per_leaf, int device) {
     const bool f32 = x_in.dtype().is(py::dtype::of<float>()), f64 = x_in.dtype().is(py::dtype::of<double>());
@@ -1114,28 +915,9 @@ py::tuple stats_prepared_numpy(const py::array& x_in, uintptr_t cloud, bool clou
         throw py::value_error("Only 3D inputs are supported: points must have shape (n, 3).");
     if (x_in.shape(0) == 0) throw py::value_error("Invalid input set with zero elements: points must have shape (n, 3) with n > 0.");
     const int dev = current_device_or_default(device);
-    pcu_b200_nn_stats st[2] = {};
-    py::object value = py::none();
     auto* y = (const pcu_b200_cloud*)cloud;
-    if (f32) {
-        auto x = dense<float>(x_in);
-        float v = 0.f;
-        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-            return both ? pcu_b200_chamfer_prepared_host_f32(ws, x.data(), x.shape(0), y, st, &v)
-                        : pcu_b200_nn_stats_prepared_host_f32(ws, x.data(), x.shape(0), y, st);
-        });
-        if (both) value = py::module_::import("numpy").attr("float32")(v);
-    } else {
-        auto x = dense<double>(x_in);
-        double v = 0.0;
-        on_workspace(dev, kHostKey, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-            return both ? pcu_b200_chamfer_prepared_host_f64(ws, x.data(), x.shape(0), y, st, &v)
-                        : pcu_b200_nn_stats_prepared_host_f64(ws, x.data(), x.shape(0), y, st);
-        });
-        if (both) value = py::module_::import("numpy").attr("float64")(v);
-    }
-    if (both) return py::make_tuple(value, stats_to_dict(st[0]), stats_to_dict(st[1]));
-    return py::make_tuple(value, stats_to_dict(st[0]));
+    return f32 ? stats_prepared_numpy_t<float>(x_in, y, both, max_points_per_leaf, dev)
+               : stats_prepared_numpy_t<double>(x_in, y, both, max_points_per_leaf, dev);
 }
 void stats_prepared_device(bool is_f64, bool both, uintptr_t a, int64_t n, uintptr_t cloud, uintptr_t out_stats, uintptr_t out_value,
                            int max_points_per_leaf, int device, uintptr_t stream) {
@@ -1161,50 +943,6 @@ void voxel_downsample_device(bool is_f64, uintptr_t pts, int64_t n, uintptr_t at
                       : pcu_b200_voxel_downsample_f32(ws, (const float*)pts, n, (const void*)attr, attr_cols, attr_is_f64 ? 1 : 0,
                                                       size.data(), lo.data(), hi.data(), min_points, (float*)out_pts, (void*)out_attr,
                                                       (int32_t*)out_counts, (int64_t*)out_rows, (void*)stream);
-    });
-}
-
-void deduplicate_device(bool is_f64, uintptr_t pts, int64_t n, double epsilon, uintptr_t faces, int64_t nf, int cols, bool faces_i64,
-                        uintptr_t out_pts, uintptr_t out_svi, uintptr_t out_svj, uintptr_t out_faces, uintptr_t out_counts, int device,
-                        uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_deduplicate_f64(ws, (const double*)pts, n, epsilon, (const void*)faces, nf, cols, faces_i64 ? 1 : 0,
-                                                 (double*)out_pts, (int32_t*)out_svi, (int32_t*)out_svj, (void*)out_faces,
-                                                 (int64_t*)out_counts, (void*)stream)
-                      : pcu_b200_deduplicate_f32(ws, (const float*)pts, n, epsilon, (const void*)faces, nf, cols, faces_i64 ? 1 : 0,
-                                                 (float*)out_pts, (int32_t*)out_svi, (int32_t*)out_svj, (void*)out_faces,
-                                                 (int64_t*)out_counts, (void*)stream);
-    });
-}
-
-// ---- dense pairwise distances / Sinkhorn on device pointers (the Python layer owns the arrays) ----
-void pairwise_device(bool is_f64, uintptr_t a, uintptr_t b, int64_t nb, int64_t n, int64_t m, int d, int norm_kind, double p,
-                     uintptr_t out, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_pairwise_distances_f64(ws, (const double*)a, (const double*)b, nb, n, m, d, norm_kind, p, (double*)out, (void*)stream)
-                      : pcu_b200_pairwise_distances_f32(ws, (const float*)a, (const float*)b, nb, n, m, d, norm_kind, p, (float*)out, (void*)stream);
-    });
-}
-void sinkhorn_device(bool is_f64, uintptr_t a, uintptr_t b, uintptr_t M, int64_t nb, int64_t n, int64_t m, double eps, int max_iters,
-                     double stop_thresh, uintptr_t out_P, uintptr_t out_cost, uintptr_t out_iters, int device, uintptr_t stream) {
-    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_sinkhorn_f64(ws, (const double*)a, (const double*)b, (const double*)M, nb, n, m, eps, max_iters,
-                                              stop_thresh, (double*)out_P, (double*)out_cost, (int32_t*)out_iters, (void*)stream)
-                      : pcu_b200_sinkhorn_f32(ws, (const float*)a, (const float*)b, (const float*)M, nb, n, m, eps, max_iters,
-                                              stop_thresh, (float*)out_P, (double*)out_cost, (int32_t*)out_iters, (void*)stream);
-    });
-}
-
-// ---- raw device-pointer entry points (CUDA torch tensors) --------------------------------------
-void knn_device(bool is_f64, uintptr_t query, int64_t n, uintptr_t dataset, int64_t m, int k, bool squared,
-                uintptr_t out_dist, uintptr_t out_idx, uintptr_t out_n_tied, int max_points_per_leaf, int device,
-                uintptr_t stream) {
-    if (k <= 0) throw py::value_error("Invalid value for k (" + std::to_string(k) + ") must be greater than 0.");
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_knn_f64(ws, (const double*)query, n, (const double*)dataset, m, k, squared,
-                                         (double*)out_dist, (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream)
-                      : pcu_b200_knn_f32(ws, (const float*)query, n, (const float*)dataset, m, k, squared,
-                                         (float*)out_dist, (int64_t*)out_idx, (int64_t*)out_n_tied, (void*)stream);
     });
 }
 
@@ -1239,22 +977,6 @@ py::tuple batched_chamfer_numpy(const py::array& x_in, const py::array& y_in, in
     return py::make_tuple(out, sum);
 }
 
-void batched_chamfer_device(uintptr_t x, uintptr_t y, int64_t B, int64_t n, int64_t m, uintptr_t out_per_pair,
-                            uintptr_t out_sum, int max_points_per_leaf, int device, uintptr_t stream) {
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_batched_chamfer_f32(ws, (const float*)x, (const float*)y, B, n, m, (float*)out_per_pair, (double*)out_sum,
-                                            (void*)stream);
-    });
-}
-
-void batched_chamfer_stats_device(uintptr_t x, uintptr_t y, int64_t B, int64_t n, int64_t m, uintptr_t out_stats,
-                                  uintptr_t out_per_pair, int max_points_per_leaf, int device, uintptr_t stream) {
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        return pcu_b200_debug_batched_chamfer_stats_f32(ws, (const float*)x, (const float*)y, B, n, m, (pcu_b200_nn_stats*)out_stats,
-                                                        (float*)out_per_pair, (void*)stream);
-    });
-}
-
 template <typename T>
 py::dict debug_kd_tree_t(const py::array& pts_in, int leaf, int device) {
     auto pts = dense<T>(pts_in);
@@ -1264,13 +986,10 @@ py::dict debug_kd_tree_t(const py::array& pts_in, int leaf, int device) {
     py::array_t<T> lo(cap), hi(cap);
     int64_t nn = 0;
     on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        if (sizeof(T) == 4)
-            return pcu_b200_debug_kd_tree_f32(ws, (const float*)pts.data(), m, leaf, order.mutable_data(), cap, feat.mutable_data(),
-                                              (float*)lo.mutable_data(), (float*)hi.mutable_data(), first.mutable_data(),
-                                              last.mutable_data(), kid0.mutable_data(), kid1.mutable_data(), &nn);
-        return pcu_b200_debug_kd_tree_f64(ws, (const double*)pts.data(), m, leaf, order.mutable_data(), cap, feat.mutable_data(),
-                                          (double*)lo.mutable_data(), (double*)hi.mutable_data(), first.mutable_data(),
-                                          last.mutable_data(), kid0.mutable_data(), kid1.mutable_data(), &nn);
+        return pick<T>(pcu_b200_debug_kd_tree_f32, pcu_b200_debug_kd_tree_f64)(ws, pts.data(), m, leaf, order.mutable_data(), cap,
+                                                                                feat.mutable_data(), lo.mutable_data(), hi.mutable_data(),
+                                                                                first.mutable_data(), last.mutable_data(),
+                                                                                kid0.mutable_data(), kid1.mutable_data(), &nn);
     });
     py::dict d;
     d["order"] = order; d["feat"] = feat; d["div_lo"] = lo; d["div_hi"] = hi; d["first"] = first; d["last"] = last;
@@ -1284,14 +1003,6 @@ py::dict debug_kd_tree(const py::array& pts, int leaf, int device) {
     if (pts.dtype().is(py::dtype::of<float>())) return debug_kd_tree_t<float>(pts, leaf, dev);
     if (pts.dtype().is(py::dtype::of<double>())) return debug_kd_tree_t<double>(pts, leaf, dev);
     throw py::value_error("points must be float32 or float64");
-}
-
-void resolve_witness_device(bool is_f64, uintptr_t q, int64_t n, uintptr_t d, int64_t m, uintptr_t stats,
-                            int max_points_per_leaf, int device, uintptr_t stream) {
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        return is_f64 ? pcu_b200_resolve_witness_f64(ws, (const double*)q, n, (const double*)d, m, (pcu_b200_nn_stats*)stats, (void*)stream)
-                      : pcu_b200_resolve_witness_f32(ws, (const float*)q, n, (const float*)d, m, (pcu_b200_nn_stats*)stats, (void*)stream);
-    });
 }
 
 }  // namespace
@@ -1312,70 +1023,76 @@ PYBIND11_MODULE(_pcu_internal, mod) {
             py::arg("drop_angle_threshold") = 1.5707963267948966, py::arg("num_threads") = 0, py::arg("random_seed") = -1,
             py::arg("device") = -1,
             "Indices of the kept points and their unit normals (plane fit to the k nearest neighbours of each point).");
-    mod.def("_normals_knn_device", &normals_knn_device);
+    mod.def("_normals_knn_device", forward_to(pcu_b200_normals_knn_f32, pcu_b200_normals_knn_f64).pair_with_leaf());
     mod.def("estimate_point_cloud_normals_ball_internal", &estimate_point_cloud_normals_ball_internal, py::arg("points"),
             py::arg("view_dirs"), py::arg("radius"), py::arg("min_pts_per_ball"), py::arg("max_pts_per_ball") = -1,
             py::arg("drop_angle_threshold") = 1.5707963267948966, py::arg("max_points_per_leaf") = 10, py::arg("num_threads") = 0,
             py::arg("weight_function") = "constant", py::arg("random_seed") = -1, py::arg("device") = -1,
             "Indices of the kept points and their unit normals (plane fit to the points in a ball around each point).");
     mod.def("_normals_ball_device", &normals_ball_device);
-    mod.def("_poisson_disk_device", &poisson_disk_device);
+    mod.def("_poisson_disk_device", forward_to(pcu_b200_poisson_disk_f32, pcu_b200_poisson_disk_f64).pair());
     mod.def("_voronoi_centroids_device", &voronoi_centroids_device);
     mod.def("_lloyd_device", &lloyd_device);
-    mod.def("_mesh_area_device", &mesh_area_device);
-    mod.def("_sample_mesh_random_device", &sample_mesh_random_device);
-    mod.def("_closest_points_on_mesh_device", &closest_points_on_mesh_device);
-    mod.def("_fast_winding_number_device", &fast_winding_number_device);
-    mod.def("_point_cloud_fast_winding_number_device", &point_cloud_fast_winding_number_device);
-    mod.def("_signed_distance_to_mesh_device", &signed_distance_to_mesh_device);
-    mod.def("_sample_mesh_poisson_disk_device", &sample_mesh_poisson_disk_device);
-    mod.def("_ray_mesh_intersection_device", &ray_mesh_intersection_device);
+    mod.def("_mesh_area_device", forward_to(pcu_b200_mesh_area_f32, pcu_b200_mesh_area_f64).pair());
+    mod.def("_sample_mesh_random_device", forward_to(pcu_b200_sample_mesh_random_f32, pcu_b200_sample_mesh_random_f64).pair());
+    mod.def("_closest_points_on_mesh_device", forward_to(pcu_b200_closest_points_on_mesh_f32, pcu_b200_closest_points_on_mesh_f64).pair());
+    mod.def("_fast_winding_number_device", forward_to(pcu_b200_fast_winding_number_f32, pcu_b200_fast_winding_number_f64).pair());
+    mod.def("_point_cloud_fast_winding_number_device",
+            forward_to(pcu_b200_point_cloud_fast_winding_number_f32, pcu_b200_point_cloud_fast_winding_number_f64).pair());
+    mod.def("_signed_distance_to_mesh_device",
+            forward_to(pcu_b200_signed_distance_to_mesh_f32, pcu_b200_signed_distance_to_mesh_f64).pair());
+    mod.def("_sample_mesh_poisson_disk_device",
+            forward_to(pcu_b200_sample_mesh_poisson_disk_f32, pcu_b200_sample_mesh_poisson_disk_f64).pair());
+    mod.def("_ray_mesh_intersection_device", forward_to(pcu_b200_ray_mesh_intersection_f32, pcu_b200_ray_mesh_intersection_f64).pair());
     mod.def("_mesh_prepare_device", &mesh_prepare_device);
-    mod.def("_mesh_destroy", &mesh_destroy);
-    mod.def("_ray_mesh_prepared_device", &ray_mesh_prepared_device);
-    mod.def("_ray_surfel_intersection_device", &ray_surfel_intersection_device);
+    mod.def("_mesh_destroy", destroy(pcu_b200_mesh_destroy));
+    mod.def("_ray_mesh_prepared_device",
+            forward_to(pcu_b200_ray_mesh_intersection_prepared_f32, pcu_b200_ray_mesh_intersection_prepared_f64).pair());
+    mod.def("_ray_surfel_intersection_device",
+            forward_to(pcu_b200_ray_surfel_intersection_f32, pcu_b200_ray_surfel_intersection_f64).pair());
     mod.def("_surfel_prepare_device", &surfel_prepare_device);
-    mod.def("_ray_surfel_prepared_device", &ray_surfel_prepared_device);
-    mod.def("_surfel_geometry_device", &surfel_geometry_device);
+    mod.def("_ray_surfel_prepared_device",
+            forward_to(pcu_b200_ray_surfel_intersection_prepared_f32, pcu_b200_ray_surfel_intersection_prepared_f64).pair());
+    mod.def("_surfel_geometry_device", forward_to(pcu_b200_pointcloud_surfel_geometry_f32, pcu_b200_pointcloud_surfel_geometry_f64).pair());
     mod.def("_interpolate_barycentric_device", &interpolate_barycentric_device);
     mod.def("_marching_cubes_prepare_device", &marching_cubes_prepare_device);
-    mod.def("_marching_cubes_emit_device", &marching_cubes_emit_device);
-    mod.def("_marching_cubes_destroy", &marching_cubes_destroy);
-    mod.def("_sparse_voxel_grid_boundary_device", &sparse_voxel_grid_boundary_device);
+    mod.def("_marching_cubes_emit_device", forward_to(pcu_b200_marching_cubes_emit).single());
+    mod.def("_marching_cubes_destroy", destroy(pcu_b200_marching_cubes_destroy));
+    mod.def("_sparse_voxel_grid_boundary_device", forward_to(pcu_b200_sparse_voxel_grid_boundary).single());
     mod.def("_sparse_grid_from_points_device", &sparse_grid_from_points_device);
     mod.def("_sparse_grid_dilate_prepare_device", &sparse_grid_dilate_prepare_device);
     mod.def("_sparse_grid_hex_prepare_device", &sparse_grid_hex_prepare_device);
-    mod.def("_sparse_grid_emit_device", &sparse_grid_emit_device);
-    mod.def("_sparse_grid_destroy", &sparse_grid_destroy);
-    mod.def("_sparse_grid_erode_device", &sparse_grid_erode_device);
+    mod.def("_sparse_grid_emit_device", forward_to(pcu_b200_sparse_grid_emit).single());
+    mod.def("_sparse_grid_destroy", destroy(pcu_b200_sparse_grid_destroy));
+    mod.def("_sparse_grid_erode_device", forward_to(pcu_b200_sparse_grid_erode).single());
     mod.def("_voxel_grid_geometry_device", &voxel_grid_geometry_device);
     mod.def("_voxelize_prepare_device", &voxelize_prepare_device);
-    mod.def("_voxelize_emit_device", &voxelize_emit_device);
-    mod.def("_voxelize_destroy", &voxelize_destroy);
-    mod.def("_flood_fill_3d_device", &flood_fill_3d_device);
+    mod.def("_voxelize_emit_device", forward_to(pcu_b200_voxelize_emit).single());
+    mod.def("_voxelize_destroy", destroy(pcu_b200_voxelize_destroy));
+    mod.def("_flood_fill_3d_device", forward_to(pcu_b200_flood_fill_3d).single());
     mod.def("_connected_components_prepare_device", &connected_components_prepare_device);
-    mod.def("_connected_components_emit_device", &connected_components_emit_device);
-    mod.def("_connected_components_destroy", &connected_components_destroy);
+    mod.def("_connected_components_emit_device", forward_to(pcu_b200_connected_components_emit).single());
+    mod.def("_connected_components_destroy", destroy(pcu_b200_connected_components_destroy));
     mod.def("_remove_mesh_vertices_device", &remove_mesh_vertices_device);
     mod.def("_remove_unreferenced_device", &remove_unreferenced_device);
-    mod.def("_orient_mesh_faces_device", &orient_mesh_faces_device);
+    mod.def("_orient_mesh_faces_device", forward_to(pcu_b200_orient_mesh_faces).single());
     mod.def("_mesh_face_device", &mesh_face_device);
-    mod.def("_mesh_vertex_normals_device", &mesh_vertex_normals_device);
+    mod.def("_mesh_vertex_normals_device", forward_to(pcu_b200_mesh_vertex_normals_f32, pcu_b200_mesh_vertex_normals_f64).pair());
     mod.def("_laplacian_smooth_device", &laplacian_smooth_device);
     mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
             py::arg("max_points_per_leaf") = 10);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),
             py::arg("stream"), py::arg("knn_k") = 0, py::arg("max_points_per_leaf") = 10);
     mod.def("_knn_prepared", &knn_prepared_numpy);
-    mod.def("_knn_prepared_device", &knn_prepared_device);
-    mod.def("_cloud_destroy", &cloud_destroy);
+    mod.def("_knn_prepared_device", forward_to(pcu_b200_knn_prepared_f32, pcu_b200_knn_prepared_f64).pair_with_leaf());
+    mod.def("_cloud_destroy", destroy(pcu_b200_cloud_destroy));
     mod.def("_cloud_points", [](uintptr_t cloud) { return (uintptr_t)pcu_b200_cloud_points((const pcu_b200_cloud*)cloud); });
     mod.def("_stats_prepared", &stats_prepared_numpy);
     mod.def("_stats_prepared_device", &stats_prepared_device);
     mod.def("_voxel_downsample_device", &voxel_downsample_device);
-    mod.def("_deduplicate_device", &deduplicate_device);
-    mod.def("_pairwise_device", &pairwise_device);
-    mod.def("_sinkhorn_device", &sinkhorn_device);
+    mod.def("_deduplicate_device", forward_to(pcu_b200_deduplicate_f32, pcu_b200_deduplicate_f64).pair());
+    mod.def("_pairwise_device", forward_to(pcu_b200_pairwise_distances_f32, pcu_b200_pairwise_distances_f64).pair());
+    mod.def("_sinkhorn_device", forward_to(pcu_b200_sinkhorn_f32, pcu_b200_sinkhorn_f64).pair());
     mod.def("morton_encode", &morton_encode, py::arg("pts"), py::arg("num_threads") = -1, py::arg("device") = -1,
             "Encode n 3D integer points into Morton codes: (n, 3) int32 / int64 -> (n,) uint64.");
     mod.def("morton_decode", &morton_decode, py::arg("codes"), py::arg("num_threads") = -1, py::arg("device") = -1,
@@ -1393,11 +1110,11 @@ PYBIND11_MODULE(_pcu_internal, mod) {
             py::arg("device") = -1);
     mod.def("_batched_chamfer", &batched_chamfer_numpy, py::arg("x"), py::arg("y"), py::arg("max_points_per_leaf") = 10,
             py::arg("device") = -1);
-    mod.def("_batched_chamfer_device", &batched_chamfer_device);
-    mod.def("_batched_chamfer_stats_device", &batched_chamfer_stats_device);
-    mod.def("_knn_device", &knn_device);
+    mod.def("_batched_chamfer_device", forward_to(pcu_b200_batched_chamfer_f32).single_with_leaf());
+    mod.def("_batched_chamfer_stats_device", forward_to(pcu_b200_debug_batched_chamfer_stats_f32).single_with_leaf());
+    mod.def("_knn_device", forward_to(pcu_b200_knn_f32, pcu_b200_knn_f64).pair_with_leaf());
     mod.def("_stats_device", &stats_device);
-    mod.def("_resolve_witness_device", &resolve_witness_device);
+    mod.def("_resolve_witness_device", forward_to(pcu_b200_resolve_witness_f32, pcu_b200_resolve_witness_f64).pair_with_leaf());
     // diagnostics address a workspace by (device, stream); stream None = the numpy path's own workspace,
     // device < 0 = the device a call that names none would use
     auto key_of = [](const py::object& stream) { return stream.is_none() ? kHostKey : stream.cast<uintptr_t>(); };
