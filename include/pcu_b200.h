@@ -355,6 +355,28 @@ int pcu_b200_voronoi_centroids(pcu_b200_workspace* ws, const double* centers, in
 int pcu_b200_lloyd(pcu_b200_workspace* ws, int64_t n, int dim, uint32_t seed, int num_lloyd, int num_newton, double* out_points,
                    double* out_energy, int32_t* out_newton_steps, int64_t* out_passes, void* stream);
 
+/* ---- Voronoi cells restricted to a triangle mesh and Lloyd sampling of its surface -----------------------------
+ * Replace sample_mesh_lloyd (src/lloyd.cpp:357-401), whose geogram restricted Voronoi diagram and initial sampling are
+ * not available; the results are defined in DESIGN.md §3:
+ *   cell R_i = {y on the faces : |y - x_i|^2 <= |y - x_j|^2 for every x_j != x_i}; seeds at one position share one
+ *   cell, owned by the lowest index; faces of zero area contribute nothing; seeds need not lie on the faces.  All fp64.
+ * v (nv, 3), f (nf, 3) of index kind f_kind (pcu_b200_index_kind) and every array below are DEVICE pointers.
+ * pcu_b200_restricted_voronoi_moments: seeds (n, 3), 1 <= n <= 2^31 - 2; out_moments (n, 5) per cell: area, first
+ *   moment about the seed (x, y, z), second moment about the seed.  A face with a corner out of range fails the call.
+ * pcu_b200_sample_mesh_lloyd: the first num_samples samples of pcu_b200_sample_mesh_random_f64 at `seed` (their
+ *   positions fl((b0 a + b1 b) + b2 c)), num_lloyd centroid steps, then at most num_newton L-BFGS steps on the energy
+ *   sum_i int_{R_i} |y - x_i|^2 dA with no domain test; out_points (num_samples, 3).  out_energy (HOST, num_newton + 1
+ *   doubles, may be NULL) and out_newton_steps (HOST, may be NULL) as for pcu_b200_lloyd.  A face with a corner out of
+ *   range or a mesh of zero area fails the call (PCU_B200_INVALID_ARGUMENT).
+ * out_passes (HOST, 3 int64, may be NULL): (face, seed) pairs handled by the first pass, the longer-list pass and the
+ *   all-seeds pass, summed over every cell evaluation of the call.  Both calls synchronise `stream` (the pairs and the
+ *   fallback passes are sized on the host); too many pairs for device memory fail with PCU_B200_OUT_OF_MEMORY. */
+int pcu_b200_restricted_voronoi_moments(pcu_b200_workspace* ws, const double* seeds, int64_t n, const double* v, int64_t nv,
+                                        const void* f, int64_t nf, int f_kind, double* out_moments, int64_t* out_passes, void* stream);
+int pcu_b200_sample_mesh_lloyd(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                               int64_t num_samples, uint32_t seed, int num_lloyd, int num_newton, double* out_points,
+                               double* out_energy, int32_t* out_newton_steps, int64_t* out_passes, void* stream);
+
 /* ---- mesh sampling and barycentric interpolation ----------------------------------------------
  * Replaces sample_mesh_random / sample_mesh_poisson_disk (src/sample_mesh.cpp) and interpolate_barycentric_coords
  * (point_cloud_utils/__init__.py:203-217).  The reference draws with std::rand and libigl; the samples here are pure

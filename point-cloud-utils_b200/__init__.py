@@ -51,6 +51,7 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "connected_components", "remove_mesh_vertices", "remove_unreferenced_mesh_vertices", "orient_mesh_faces",
            "mesh_face_areas", "estimate_mesh_face_normals", "estimate_mesh_vertex_normals", "laplacian_smooth_mesh",
            "deduplicate_point_cloud", "voronoi_centroids_unit_cube", "lloyd_3d", "lloyd_2d",
+           "sample_mesh_lloyd",
            "deduplicate_mesh_vertices", "prepare_cloud", "pinned_empty", "PreparedCloud", "device_count",
            "current_device", "launch_count"]
 
@@ -787,7 +788,7 @@ def morton_knn(codes, qcodes, k, sort_dist=True, *, device=None):
 from ._sinkhorn import pairwise_distances, sinkhorn, earth_movers_distance  # noqa: E402  (N4: dense metrics)
 from ._dedup import deduplicate_point_cloud, deduplicate_mesh_vertices  # noqa: E402  (N2: duplicate removal)
 from ._poisson import downsample_point_cloud_poisson_disk  # noqa: E402  (Poisson-disk downsampling)
-from ._lloyd import voronoi_centroids_unit_cube, lloyd_3d, lloyd_2d  # noqa: E402  (Voronoi centroids, Lloyd relaxation)
+from ._lloyd import voronoi_centroids_unit_cube, lloyd_3d, lloyd_2d, sample_mesh_lloyd  # noqa: E402  (Voronoi, Lloyd)
 from ._mesh_sampling import sample_mesh_random, sample_mesh_poisson_disk, interpolate_barycentric_coords  # noqa: E402
 from ._mesh_query import (closest_points_on_mesh, triangle_soup_fast_winding_number,  # noqa: E402
                           point_cloud_fast_winding_number, signed_distance_to_mesh)

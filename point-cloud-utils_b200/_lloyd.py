@@ -1,18 +1,20 @@
-"""voronoi_centroids_unit_cube, lloyd_3d and lloyd_2d -- the reference's names, arguments, defaults and messages
-(the reference's src/lloyd.cpp:166-300), computed by csrc/voronoi.cuh.
+"""voronoi_centroids_unit_cube, lloyd_3d, lloyd_2d and sample_mesh_lloyd -- the reference's names, arguments, defaults
+and messages (the reference's src/lloyd.cpp:166-401), computed by csrc/voronoi.cuh and csrc/rvd.cuh.
 
 The reference computes its cells with geogram's restricted Voronoi diagram and relaxes with geogram's initial sampling
 and HLBFGS Newton iterations, none of which is available; DESIGN.md §3 defines the results exactly instead (cells,
-centroid rows, the initial sample, the Lloyd step and the L-BFGS Newton phase)."""
+restricted cells, centroid rows, the initial samples, the Lloyd step and the L-BFGS Newton phase)."""
 import numpy as _np
 
 from . import _pcu_internal
-from ._call import _dtype_name, _is_tensor, _torch
+from ._call import _INDEX_KINDS, _dtype_name, _form, _is_tensor, _run, _torch, _validate_mesh
 
-# Cells handled by each pass (first pass, longer neighbour lists, all seeds) in the last call of this module's functions,
-# in any thread (a plain module global, for tests and tools): the fallback passes are otherwise invisible.
+# Cells (for restricted cells: (face, seed) pairs) handled by each pass (first pass, longer neighbour lists, all seeds)
+# in the last call of this module's functions, in any thread (a plain module global, for tests and tools): the fallback
+# passes are otherwise invisible.
 last_pass_counts = (0, 0, 0)
-# The CVT energy of the starting point and of every accepted Newton step of the last lloyd_3d / lloyd_2d call.
+# The CVT energy of the starting point and of every accepted Newton step of the last lloyd_3d / lloyd_2d /
+# sample_mesh_lloyd call.
 last_newton_energies = []
 
 
@@ -153,3 +155,82 @@ lloyd_3d.__doc__ = """
     Returns:
       lloyd_pts : a (n, 3)-shaped float64 numpy array of point samples in the unit cube [0, 1]^3
 """ + _LLOYD_DEFINITION
+
+
+def _restricted_cell_moments(seeds, v, f, *, device=None):
+    """Moments (n, 5) of the cells of (n, 3) seeds restricted to the mesh (v, f), numpy arrays in and out (v float32 or
+    float64, widened exactly; f of any of the four index dtypes), n >= 1: area, first moment about the seed (x, y, z)
+    and second moment about the seed of every cell.  Not part of the public interface: the cells sample_mesh_lloyd
+    sees, for tests."""
+    global last_pass_counts
+    torch = _torch()
+    seeds = _np.ascontiguousarray(seeds, dtype=_np.float64)
+    _validate_mesh(v, f, tuple(_INDEX_KINDS))
+    n = seeds.shape[0]
+    result = {}
+
+    def body(vt, ft, st, dev, stream):
+        vt = vt.to(torch.float64).contiguous()
+        mom = torch.empty((n, 5), dtype=torch.float64, device=vt.device)
+        result["passes"] = _pcu_internal._restricted_voronoi_moments_device(
+            st.data_ptr(), n, vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(), int(ft.shape[0]), _INDEX_KINDS[_dtype_name(f)],
+            mom.data_ptr(), dev, stream)
+        return mom
+
+    mom = _run("numpy", [v, f, seeds], device, body)
+    last_pass_counts = tuple(result["passes"])
+    return mom
+
+
+def sample_mesh_lloyd(v, f, num_samples, num_lloyd=10, num_newton=10, return_mesh=False, *, device=None):
+    """
+    Sample points on a mesh surface using Lloyd's algorithm
+
+    Args:
+      v : (#v, 3)-shaped array of mesh vertex positions (float32 / float64)
+      f : (#f, 3)-shaped array of mesh face indices (int32 / int64 / uint32 / uint64)
+      num_samples : the number of samples to generate (> 0)
+      num_lloyd : the number of Lloyd iterations to do (default 10)
+      num_newton : the number of Newton iterations to do when computing Voronoi diagrams (default 10)
+      return_mesh : accepted and ignored, as in the reference (whose binding does not use it)
+      device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+      points : a (num_samples, 3)-shaped float64 array of samples (numpy for numpy inputs, a CUDA tensor for CUDA
+               tensors, a CPU tensor for CPU tensors)
+
+    All arithmetic is fp64 (float32 v is widened exactly first).  The cell of sample x_i is the part of the surface
+    nearer to x_i than to any other sample, R_i = {y on the faces : |y - x_i|^2 <= |y - x_j|^2 for every x_j != x_i}
+    (samples at one position share one cell, owned by the lowest index; faces of zero area contribute nothing).  The
+    initial sample is the first num_samples samples of sample_mesh_random on the fp64 vertices with the seed
+    int(np.random.randint(2**31 - 1)) (seed NumPy for reproducible results), at positions fl((b0 a + b1 b) + b2 c) per
+    axis; num_lloyd steps then move every point to its cell's centroid (a point whose cell has area <= 1e-30 stays),
+    and at most num_newton L-BFGS steps (memory 7, Armijo backtracking, no domain test) decrease the energy
+    sum_i int_{R_i} |y - x_i|^2 dA.  Centroids are not projected onto the surface: the centroid of a cell on a curved
+    surface lies slightly off it.  Two calls with the same NumPy state give bit-identical points.  DESIGN.md §3 states
+    the definitions; geogram's initial sampling and HLBFGS, which the reference uses, cannot be reproduced.
+    Divergence: a face corner outside [0, #v) raises ValueError (the reference reads out of bounds).
+    """
+    global last_pass_counts, last_newton_energies
+    form = _form([v, f], ["v", "f"])
+    _validate_mesh(v, f, tuple(_INDEX_KINDS))
+    n = int(num_samples)
+    if n <= 0:
+        raise ValueError("num_samples must be > 0")
+    seed = int(_np.random.randint(2 ** 31 - 1))
+    torch = _torch()
+    kind = _INDEX_KINDS[_dtype_name(f)]
+    result = {}
+
+    def body(vt, ft, dev, stream):
+        vt = vt.to(torch.float64).contiguous()
+        out = torch.empty((n, 3), dtype=torch.float64, device=vt.device)
+        result["energies"], result["passes"] = _pcu_internal._sample_mesh_lloyd_device(
+            vt.data_ptr(), int(vt.shape[0]), ft.data_ptr(), int(ft.shape[0]), kind, n, seed, int(num_lloyd), int(num_newton),
+            out.data_ptr(), dev, stream)
+        return out
+
+    out = _run(form, [v, f], device, body)
+    last_pass_counts = tuple(result["passes"])
+    last_newton_energies = list(result["energies"])
+    return out

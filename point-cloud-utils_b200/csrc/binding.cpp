@@ -569,6 +569,33 @@ py::tuple lloyd_device(int64_t n, int dim, uint32_t seed, int num_lloyd, int num
     return py::make_tuple(energy, py::make_tuple(passes[0], passes[1], passes[2]));
 }
 
+// Moments (n, 5) of the cells of device seeds (n, 3) restricted to a device mesh (fp64 v) into device out_moments;
+// returns the pairs each pass handled.
+py::tuple restricted_voronoi_moments_device(uintptr_t seeds, int64_t n, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind,
+                                            uintptr_t out_moments, int device, uintptr_t stream) {
+    int64_t passes[3] = {0, 0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_restricted_voronoi_moments(ws, (const double*)seeds, n, (const double*)v, nv, (const void*)f, nf, f_kind,
+                                                   (double*)out_moments, passes, (void*)stream);
+    });
+    return py::make_tuple(passes[0], passes[1], passes[2]);
+}
+
+// Lloyd sampling of a device mesh (fp64 v) into device out (num_samples, 3) fp64; returns (energies of the Newton
+// phase, pairs each pass handled).
+py::tuple sample_mesh_lloyd_device(uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int64_t num_samples, uint32_t seed,
+                                   int num_lloyd, int num_newton, uintptr_t out, int device, uintptr_t stream) {
+    int64_t passes[3] = {0, 0, 0};
+    int32_t steps = 0;
+    std::vector<double> energy((size_t)std::max(num_newton, 0) + 1, 0.0);
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_sample_mesh_lloyd(ws, (const double*)v, nv, (const void*)f, nf, f_kind, num_samples, seed, num_lloyd, num_newton,
+                                          (double*)out, energy.data(), &steps, passes, (void*)stream);
+    });
+    energy.resize(num_newton > 0 ? (size_t)steps + 1 : 0);
+    return py::make_tuple(energy, py::make_tuple(passes[0], passes[1], passes[2]));
+}
+
 // A prepared mesh (RayMeshIntersector); out_bad: one device uint64, the faces with a corner out of range.
 uintptr_t mesh_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t out_bad, int device,
                               uintptr_t stream) {
@@ -1033,6 +1060,8 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_poisson_disk_device", forward_to(pcu_b200_poisson_disk_f32, pcu_b200_poisson_disk_f64).pair());
     mod.def("_voronoi_centroids_device", &voronoi_centroids_device);
     mod.def("_lloyd_device", &lloyd_device);
+    mod.def("_restricted_voronoi_moments_device", &restricted_voronoi_moments_device);
+    mod.def("_sample_mesh_lloyd_device", &sample_mesh_lloyd_device);
     mod.def("_mesh_area_device", forward_to(pcu_b200_mesh_area_f32, pcu_b200_mesh_area_f64).pair());
     mod.def("_sample_mesh_random_device", forward_to(pcu_b200_sample_mesh_random_f32, pcu_b200_sample_mesh_random_f64).pair());
     mod.def("_closest_points_on_mesh_device", forward_to(pcu_b200_closest_points_on_mesh_f32, pcu_b200_closest_points_on_mesh_f64).pair());

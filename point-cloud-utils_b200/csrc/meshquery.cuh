@@ -15,6 +15,8 @@
 //   points  L = WnPoint (point_cloud_fast_winding_number, winding.cuh), one per leaf, always valid; no boxes, no refit
 //   surfels L = SfWord (ray_surfel_intersection, raycast.cuh), a whole fp32 fan per leaf (sf_fan); a fan with a
 //           non-finite coordinate is invalid, counted and left out as a face is; leaves have boxes and the nodes are refit
+//   balls   L = RvBall (sample_mesh_lloyd, rvd.cuh), one face's candidate ball per leaf; a ball without a radius is
+//           invalid, counted and left out as a face is; leaves have boxes and the nodes are refit
 // The passes:
 //   mq_bounds_kernel    scene box of the leaves' boxes (a point's box is the point), count of invalid faces
 //   mq_codes_kernel     63-bit Morton code of each face's box centre or each fp32 point over the scene box (invalid
@@ -72,6 +74,15 @@ template <typename L>
 constexpr bool kSurfelLeaf = std::is_same<L, SfWord>::value;
 
 __host__ __device__ __forceinline__ long long sf_words(int s) { return (3ll * (s + 1) + 3) / 4; }
+
+// A ball leaf of the restricted Voronoi pairs (rvd.cuh): a face's candidate ball, centre and radius in fp64.  The
+// build's input v is the (m, 4) array of balls; a ball whose radius is not >= 0 (NaN: a face that meets no cell) is
+// invalid, counted in MqScratch::bad and left out of the tree as an invalid face is.  The leaf's face id lives in
+// MeshTree::ids; its box is the ball's, rounded outward to fp32.
+struct __align__(16) RvBall { double c[3], r; };
+
+template <typename L>
+constexpr bool kBallLeaf = std::is_same<L, RvBall>::value;
 
 // What a surfel fan is computed from: normals and radii (T, as the points), s and the table cs[2 j] = fl32(cos
 // theta_j), cs[2 j + 1] = fl32(sin theta_j), computed on the host (DESIGN.md §3, ray-surfel casting).  During a tree
@@ -219,6 +230,10 @@ __device__ __forceinline__ bool mq_leaf_corners(const T* v, long long nv, const 
     if constexpr (kPointLeaf<L>) {
         load_vertex<T>(v, t, a);
         return true;
+    } else if constexpr (kBallLeaf<L>) {   // a: the centre, b[0]: the radius
+        const double* ball = (const double*)v + 4 * t;
+        a[0] = ball[0]; a[1] = ball[1]; a[2] = ball[2]; b[0] = ball[3];
+        return ball[3] >= 0.0;
     } else {
         return mq_corners<T>(v, nv, f, fkind, t, a, b, c);
     }
@@ -230,6 +245,13 @@ __device__ __forceinline__ MqBox mq_leaf_box(const double a[3], const double b[3
     if constexpr (kPointLeaf<L>) {
         MqBox bx;
         for (int k = 0; k < 3; ++k) bx.lo[k] = bx.hi[k] = (float)a[k];
+        return bx;
+    } else if constexpr (kBallLeaf<L>) {
+        MqBox bx;
+        for (int k = 0; k < 3; ++k) {
+            bx.lo[k] = __double2float_rd(__dsub_rd(a[k], b[0]));
+            bx.hi[k] = __double2float_ru(__dadd_ru(a[k], b[0]));
+        }
         return bx;
     } else {
         return mq_face_box<T>(a, b, c);
@@ -363,6 +385,23 @@ __global__ void __launch_bounds__(kThreads) sf_leaves_kernel(const T* __restrict
     for (long long k = 3ll * (src.s + 1); k < 4 * words; ++k) out[k] = 0.f;
     ids[i] = (int)t;
     boxes[i] = bx;
+}
+
+// Ball leaf i (i < m - bad): its ball, its face id and its box.
+__global__ void __launch_bounds__(kThreads) rv_ball_leaves_kernel(const double* __restrict__ balls, long long m,
+                                                                  const MqScratch* __restrict__ sc, const MqRec* __restrict__ sorted,
+                                                                  RvBall* __restrict__ leaves, int* __restrict__ ids,
+                                                                  MqBox* __restrict__ boxes) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= m - (long long)sc->bad) return;
+    const long long t = (long long)sorted[i].idx;
+    double a[3], b[3], c[3];
+    mq_leaf_corners<RvBall, double>(balls, 0, nullptr, 0, t, a, b, c);
+    RvBall r;
+    r.c[0] = a[0]; r.c[1] = a[1]; r.c[2] = a[2]; r.r = b[0];
+    leaves[i] = r;
+    ids[i] = (int)t;
+    boxes[i] = mq_leaf_box<RvBall, double>(a, b, c);
 }
 
 // pointcloud_surfel_geometry: surfel i's s + 1 vertices at rows i (s + 1) .. (rim j at + j, the centre at + s), in T

@@ -43,6 +43,7 @@
 #include "orient.cuh"
 #include "laplacian.cuh"
 #include "voronoi.cuh"
+#include "rvd.cuh"
 
 using namespace pcu;
 
@@ -206,10 +207,11 @@ enum Scratch {
               // call it makes (that one re-carves the arena and aux)
     kVorList, // the Voronoi cells' fallback passes (rows, queries, longer neighbour lists), sized once the first pass is done
     kLloyd,   // the points, L-BFGS history and sync record of a Lloyd relaxation, which outlive every cell evaluation
+    kRvd,     // the faces and the per-seed buffers of restricted Voronoi cells, which outlive every cell evaluation of a call
     kScratchBlocks
 };
 static const char* const kScratchName[kScratchBlocks] = {"scratch", "staging", "intermediate scratch", "mesh-sampling scratch",
-                                                         "Voronoi fallback scratch", "Lloyd scratch"};
+                                                         "Voronoi fallback scratch", "Lloyd scratch", "restricted Voronoi scratch"};
 
 struct pcu_b200_workspace {
     int device = 0;
@@ -1404,9 +1406,9 @@ void carve_mesh_tree(Carver& cv, long long m, bool moments, MeshTree<L>& t, int 
     const long long inner = std::max<long long>(1, m - 1);
     t.sc = cv.take<MqScratch>(1);
     t.nodes = cv.take<MqNode>((size_t)inner);
-    t.leaves = cv.take<L>((size_t)(kSurfelLeaf<L> ? sf_words(subdivs) : (kPointLeaf<L> ? 1 : 3)) * m);
+    t.leaves = cv.take<L>((size_t)(kSurfelLeaf<L> ? sf_words(subdivs) : (kPointLeaf<L> || kBallLeaf<L> ? 1 : 3)) * m);
     t.wn = moments ? cv.take<WnNode>((size_t)inner) : nullptr;
-    t.ids = kSurfelLeaf<L> ? cv.take<int>((size_t)m) : nullptr;
+    t.ids = kSurfelLeaf<L> || kBallLeaf<L> ? cv.take<int>((size_t)m) : nullptr;
 }
 
 // The surfel table of DESIGN.md §3: theta_j = ((float)j / ((float)(s + 1) - 1)) (float)pi 2 in fp32, as the reference
@@ -1448,7 +1450,8 @@ int upload_surfel_src(unsigned char* dev, const void* n, const void* r, int s, M
 // faces the refit and, with `moments`, the centre, radius and moment passes of winding.cuh.  Face leaves (L = Pt<T>)
 // are built from the mesh (v, nv, f, fkind) and the count of invalid faces lands in *out_bad; point leaves (L = WnPoint)
 // from the points v, normals n and areas a, always with moments; surfel leaves (L = SfWord) from the points v, normals
-// n, radii a and `subdivs`, without moments, their non-finite fans counted in the header only.  The caller has checked
+// n, radii a and `subdivs`, without moments, their non-finite fans counted in the header only; ball leaves (L = RvBall)
+// from the (m, 4) balls v, without moments, the balls without a radius counted in the header only.  The caller has checked
 // the input (m >= 1) and made the device current.
 template <typename T, typename L>
 int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, bool moments,
@@ -1488,6 +1491,9 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
     else if constexpr (surfels)
         PCU_LAUNCH((sf_leaves_kernel<T>), fblocks, kThreads, stream, v, src, m, (const MqScratch*)t.sc, (const MqRec*)sorted,
                    t.leaves, t.ids, s.boxes);
+    else if constexpr (kBallLeaf<L>)
+        PCU_LAUNCH(rv_ball_leaves_kernel, fblocks, kThreads, stream, (const double*)v, m, (const MqScratch*)t.sc, (const MqRec*)sorted,
+                   t.leaves, t.ids, s.boxes);
     else
         PCU_LAUNCH((mq_leaves_kernel<T>), fblocks, kThreads, stream, v, nv, f, fkind, m, (const MqScratch*)t.sc, (const MqRec*)sorted,
                    t.leaves, s.boxes);
@@ -1498,7 +1504,7 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
         PCU_LAUNCH(mq_refit_kernel, fblocks, kThreads, stream, m, (const MqScratch*)t.sc, t.nodes, (const int*)s.node_parent,
                    (const int*)s.leaf_parent, (const MqBox*)s.boxes, s.arrivals);
     }
-    if constexpr (!surfels) if (moments) {   // surfel trees carry no far field
+    if constexpr (!surfels && !kBallLeaf<L>) if (moments) {   // surfel and ball trees carry no far field
         PCU_CUDA(cudaMemsetAsync(s.arrivals, 0, (size_t)inner * sizeof(int), stream));
         PCU_LAUNCH((wn_centres_kernel<L>), fblocks, kThreads, stream, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
                    (const int*)s.node_parent, (const int*)s.leaf_parent, (const L*)t.leaves, t.wn, s.arrivals);
@@ -1508,7 +1514,7 @@ int build_mesh_tree(pcu_b200_workspace* ws, const T* v, long long nv, const void
         PCU_LAUNCH((wn_moments_kernel<L>), fblocks, kThreads, stream, m, (const MqScratch*)t.sc, (const MqNode*)t.nodes,
                    (const int*)s.node_parent, (const int*)s.leaf_parent, (const L*)t.leaves, t.wn, s.arrivals);
     }
-    if constexpr (!points && !surfels)
+    if constexpr (!points && !surfels && !kBallLeaf<L>)
         PCU_CUDA(cudaMemcpyAsync(out_bad, &t.sc->bad, sizeof(unsigned long long), cudaMemcpyDeviceToDevice, stream));
     tree = t;
     return PCU_B200_OK;
@@ -1823,10 +1829,97 @@ int vor_pass_launch(const VorPass& p, int pass, cudaStream_t stream) {
     return PCU_B200_OK;
 }
 
+// How the passes clip one kind of entry: the cells in the unit cube / square, or the (face, seed) pairs of restricted
+// cells (rvd.cuh).  k2: the longer lists of pass 2; wide: the first capacity of pass 3.
+template <int D>
+struct VorCube {
+    static constexpr int k2 = kVorK2[D - 2], wide = kVorWide[D - 2];
+    static int launch(const VorPass& p, int pass, cudaStream_t stream) { return vor_pass_launch<D>(p, pass, stream); }
+    static size_t cell_bytes(int V) { return vor_cell_bytes<D>(V); }
+    static int launch_wide(const VorPass& p, int V, cudaStream_t stream) {
+        PCU_LAUNCH(vor_clip_wide_kernel<D>, (unsigned)((p.count + kVorThreads - 1) / kVorThreads), kVorThreads, stream, p, V);
+        return PCU_B200_OK;
+    }
+};
+
+// Restricted pairs: the k-NN lists of a 2-D cell (a restricted cell is a surface patch), polygons of 16 / 64 vertices on
+// the stack, then 256 in device memory.
+constexpr int kRvK1 = 24, kRvK2 = 64, kRvSmall = 16, kRvLarge = 64, kRvWide = 256;
+struct VorRestricted {
+    static constexpr int k2 = kRvK2, wide = kRvWide;
+    static int launch(const VorPass& p, int pass, cudaStream_t stream) {
+        const unsigned blocks = (unsigned)((p.count + kVorThreads - 1) / kVorThreads);
+        if (pass == 0) PCU_LAUNCH(rv_clip_kernel<kRvSmall>, blocks, kVorThreads, stream, p);
+        else           PCU_LAUNCH(rv_clip_kernel<kRvLarge>, blocks, kVorThreads, stream, p);
+        return PCU_B200_OK;
+    }
+    static size_t cell_bytes(int V) { return poly_bytes(V); }
+    static int launch_wide(const VorPass& p, int V, cudaStream_t stream) {
+        PCU_LAUNCH(rv_clip_wide_kernel, (unsigned)((p.count + kVorThreads - 1) / kVorThreads), kVorThreads, stream, p, V);
+        return PCU_B200_OK;
+    }
+};
+
+// Passes 2 and 3 over the entries pass 1 (p, already enqueued over p.count entries) left uncertified in `flag`; `counts`
+// holds keep_count_words(p.count) words.
+template <class K>
+int vor_fallback(pcu_b200_workspace* ws, VorPass p, unsigned char* flag, unsigned* counts, VorSync* sync, long long* passes,
+                 VorSync* seen, cudaStream_t stream) {
+    const long long n = p.n, entries = p.count;
+    PCU_TRY(enqueue_keep_offsets(flag, entries, counts, &sync->count, stream));
+    PCU_TRY(read_record(sync, seen, stream));
+    const long long c1 = seen->count;
+    if (c1 == 0) return PCU_B200_OK;
+    const int k2 = (int)std::min<long long>(K::k2, n);
+    int *rows, *sub[2]; double *q, *d2; long long* i2; unsigned char* flag2; unsigned* counts2;
+    PCU_TRY(carve_scratch(ws, kVorList, stream, [&](Carver& cv) {
+        rows = cv.take<int>((size_t)c1);
+        sub[0] = cv.take<int>((size_t)c1);
+        sub[1] = cv.take<int>((size_t)c1);
+        q = cv.take<double>((size_t)3 * c1);
+        d2 = cv.take<double>((size_t)k2 * c1);
+        i2 = cv.take<long long>((size_t)k2 * c1);
+        flag2 = cv.take<unsigned char>((size_t)c1);
+        counts2 = cv.take<unsigned>(keep_count_words(c1));
+    }));
+    PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(entries), kThreads, stream, (const unsigned char*)flag, entries, (const unsigned*)counts, rows);
+    PCU_LAUNCH(vor_gather_kernel, blocks_for(c1), kThreads, stream, p.x3, (const int*)rows, c1, q, p.pair_seed);
+    PCU_TRY(knn_device<double>(ws, q, c1, p.x3, n, k2, 1, d2, i2, nullptr, stream, nullptr, false));
+    p.rows = rows; p.count = c1; p.nn_idx = i2; p.nn_d2 = d2; p.k = k2; p.list_is_all = k2 >= n; p.uncert = flag2;
+    p.list_of_seed = 0;
+    PCU_TRY(K::launch(p, 1, stream));
+    passes[1] += c1;
+    PCU_TRY(enqueue_keep_offsets(flag2, c1, counts2, &sync->count, stream));
+    PCU_TRY(read_record(sync, seen, stream));
+    long long cnt = seen->count;
+    if (cnt == 0) return PCU_B200_OK;
+    // the last resort; sub[r & 1]: the pass-2 entries of round r
+    PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(c1), kThreads, stream, (const unsigned char*)flag2, c1, (const unsigned*)counts2, sub[0]);
+    p.scan_all = 1; p.list_is_all = 0; p.uncert = flag2;
+    for (int V = K::wide, r = 0;; V *= 2, ++r) {
+        if (V > kVorWideMax)
+            return fail(PCU_B200_OUT_OF_MEMORY, "voronoi: %lld cells have more than %d vertices", cnt, kVorWideMax);
+        // the cells live in the arena: the k-NN searches, its only other users here, are enqueued already
+        PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+            p.cells = cv.take<unsigned char>((size_t)cnt * K::cell_bytes(V));
+        }));
+        p.sub = sub[r & 1]; p.count = cnt;
+        PCU_TRY(K::launch_wide(p, V, stream));
+        passes[2] += cnt;
+        PCU_TRY(enqueue_keep_offsets(flag2, cnt, counts2, &sync->count, stream));
+        PCU_TRY(read_record(sync, seen, stream));
+        if (seen->count == 0) break;
+        PCU_LAUNCH(vor_keep_sub_kernel, blocks_for(cnt), kThreads, stream, (const unsigned char*)flag2, cnt, (const unsigned*)counts2,
+                   (const int*)sub[r & 1], sub[(r + 1) & 1]);
+        cnt = seen->count;
+    }
+    return PCU_B200_OK;
+}
+
 template <int D>
 int vor_eval(pcu_b200_workspace* ws, const double* x, long long n, VorSync* sync, double** mom_out, long long* passes,
              VorSync* seen, cudaStream_t stream) {
-    const int k1 = (int)std::min<long long>(kVorK1[D - 2], n), k2 = (int)std::min<long long>(kVorK2[D - 2], n);
+    const int k1 = (int)std::min<long long>(kVorK1[D - 2], n);
     double *x3 = nullptr, *mom, *d1; long long* i1; unsigned char* flag; unsigned* counts;
     PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) {
         if (D == 2) x3 = cv.take<double>((size_t)3 * n);
@@ -1845,52 +1938,7 @@ int vor_eval(pcu_b200_workspace* ws, const double* x, long long n, VorSync* sync
     p.mom = mom; p.uncert = flag;
     PCU_TRY(vor_pass_launch<D>(p, 0, stream));
     passes[0] += n;
-    PCU_TRY(enqueue_keep_offsets(flag, n, counts, &sync->count, stream));
-    PCU_TRY(read_record(sync, seen, stream));
-    const long long c1 = seen->count;
-    if (c1 == 0) return PCU_B200_OK;
-    int *rows, *sub[2]; double *q, *d2; long long* i2; unsigned char* flag2; unsigned* counts2;
-    PCU_TRY(carve_scratch(ws, kVorList, stream, [&](Carver& cv) {
-        rows = cv.take<int>((size_t)c1);
-        sub[0] = cv.take<int>((size_t)c1);
-        sub[1] = cv.take<int>((size_t)c1);
-        q = cv.take<double>((size_t)3 * c1);
-        d2 = cv.take<double>((size_t)k2 * c1);
-        i2 = cv.take<long long>((size_t)k2 * c1);
-        flag2 = cv.take<unsigned char>((size_t)c1);
-        counts2 = cv.take<unsigned>(keep_count_words(c1));
-    }));
-    PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(n), kThreads, stream, (const unsigned char*)flag, n, (const unsigned*)counts, rows);
-    PCU_LAUNCH(vor_gather_kernel, blocks_for(c1), kThreads, stream, (const double*)x3, (const int*)rows, c1, q);
-    PCU_TRY(knn_device<double>(ws, q, c1, x3, n, k2, 1, d2, i2, nullptr, stream, nullptr, false));
-    p.rows = rows; p.count = c1; p.nn_idx = i2; p.nn_d2 = d2; p.k = k2; p.list_is_all = k2 >= n; p.uncert = flag2;
-    PCU_TRY(vor_pass_launch<D>(p, 1, stream));
-    passes[1] += c1;
-    PCU_TRY(enqueue_keep_offsets(flag2, c1, counts2, &sync->count, stream));
-    PCU_TRY(read_record(sync, seen, stream));
-    long long cnt = seen->count;
-    if (cnt == 0) return PCU_B200_OK;
-    // the last resort; sub[r & 1]: the pass-2 entries of round r
-    PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(c1), kThreads, stream, (const unsigned char*)flag2, c1, (const unsigned*)counts2, sub[0]);
-    p.scan_all = 1; p.list_is_all = 0; p.uncert = flag2;
-    for (int V = kVorWide[D - 2], r = 0;; V *= 2, ++r) {
-        if (V > kVorWideMax)
-            return fail(PCU_B200_OUT_OF_MEMORY, "voronoi: %lld cells have more than %d vertices", cnt, kVorWideMax);
-        // the cells live in the arena: the k-NN searches, its only other users here, are enqueued already
-        PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
-            p.cells = cv.take<unsigned char>((size_t)cnt * vor_cell_bytes<D>(V));
-        }));
-        p.sub = sub[r & 1]; p.count = cnt;
-        PCU_LAUNCH(vor_clip_wide_kernel<D>, (unsigned)((cnt + kVorThreads - 1) / kVorThreads), kVorThreads, stream, p, V);
-        passes[2] += cnt;
-        PCU_TRY(enqueue_keep_offsets(flag2, cnt, counts2, &sync->count, stream));
-        PCU_TRY(read_record(sync, seen, stream));
-        if (seen->count == 0) break;
-        PCU_LAUNCH(vor_keep_sub_kernel, blocks_for(cnt), kThreads, stream, (const unsigned char*)flag2, cnt, (const unsigned*)counts2,
-                   (const int*)sub[r & 1], sub[(r + 1) & 1]);
-        cnt = seen->count;
-    }
-    return PCU_B200_OK;
+    return vor_fallback<VorCube<D>>(ws, p, flag, counts, sync, passes, seen, stream);
 }
 
 int vor_check(long long n, int dim) {
@@ -1923,13 +1971,14 @@ int lbfgs_grid_blocks(const pcu_b200_workspace* ws, long long N, unsigned* out_b
     return PCU_B200_OK;
 }
 
-// The initial sample, num_lloyd Lloyd steps, then the Newton phase (L-BFGS, voronoi.cuh).  Synchronisations: those
-// of every cell evaluation (one, plus one per fallback pass or last-resort round that runs), one for the initial
-// L-BFGS state, one after every L-BFGS step (its verdict decides whether the trial point is evaluated), and one for
-// the energies at the end.
-template <int D>
-int lloyd_device(pcu_b200_workspace* ws, long long n, unsigned seed, int num_lloyd, int num_newton, double* out,
-                 double* energy_host, int* iters_host, long long* passes, cudaStream_t stream) {
+// The initial sample, num_lloyd Lloyd steps, then the Newton phase (L-BFGS, voronoi.cuh), for either kind of cell:
+// init(x) writes the (n, D) initial sample; eval(x, sync, &mom, &seen) evaluates the cells of x (their (n, 5) moments
+// into mom); cube: trial points must lie in the unit cube.  Synchronisations: those of init and of every cell evaluation,
+// one for the initial L-BFGS state, one after every L-BFGS step (its verdict decides whether the trial point is
+// evaluated), and one for the energies at the end.
+template <int D, class Init, class Eval>
+int lloyd_run(pcu_b200_workspace* ws, long long n, int cube, int num_lloyd, int num_newton, double* out, double* energy_host,
+              int* iters_host, cudaStream_t stream, Init&& init, Eval&& eval) {
     const long long N = n * D;
     const bool newton = num_newton > 0;
     unsigned blocks = 1;
@@ -1951,10 +2000,10 @@ int lloyd_device(pcu_b200_workspace* ws, long long n, unsigned seed, int num_llo
         }
     }));
     PCU_CUDA(cudaMemsetAsync(sync, 0, sizeof(VorSync), stream));
-    PCU_LAUNCH(lloyd_init_kernel, blocks_for(N), kThreads, stream, seed, N, x);
+    PCU_TRY(init(x));
     double* mom; VorSync seen;
     for (int it = 0; it < num_lloyd; ++it) {
-        PCU_TRY(vor_eval<D>(ws, x, n, sync, &mom, passes, &seen, stream));
+        PCU_TRY(eval((const double*)x, sync, &mom, &seen));
         PCU_LAUNCH(vor_centroid_kernel<D>, blocks_for(n), kThreads, stream, (const double*)x, n, (const double*)mom, x);
     }
     if (!newton) {
@@ -1968,8 +2017,8 @@ int lloyd_device(pcu_b200_workspace* ws, long long n, unsigned seed, int num_llo
     PCU_CUDA(cudaStreamSynchronize(stream));   // s0 lives on this stack
     LbArgs a{};
     a.n = n; a.D = D; a.x_acc = x_acc; a.g = g; a.x_t = x; a.p = p; a.S = S; a.Y = Y; a.partial = partial;
-    a.st = st; a.sync = sync; a.energy = energy; a.num_newton = num_newton;
-    PCU_TRY(vor_eval<D>(ws, x, n, sync, &mom, passes, &seen, stream));
+    a.st = st; a.sync = sync; a.energy = energy; a.num_newton = num_newton; a.cube = cube;
+    PCU_TRY(eval((const double*)x, sync, &mom, &seen));
     for (;;) {
         a.mom = mom;
         void* args[] = {(void*)&a};
@@ -1977,13 +2026,168 @@ int lloyd_device(pcu_b200_workspace* ws, long long n, unsigned seed, int num_llo
         g_launches.fetch_add(1, std::memory_order_relaxed);
         PCU_TRY(read_record(sync, &seen, stream));   // the step's verdict: evaluate its trial point, or stop
         if (seen.done) break;
-        PCU_TRY(vor_eval<D>(ws, x, n, sync, &mom, passes, &seen, stream));
+        PCU_TRY(eval((const double*)x, sync, &mom, &seen));
     }
     PCU_CUDA(cudaMemcpyAsync(out, x_acc, (size_t)N * sizeof(double), cudaMemcpyDeviceToDevice, stream));
     if (energy_host) PCU_CUDA(cudaMemcpyAsync(energy_host, energy, ((size_t)seen.iter + 1) * sizeof(double), cudaMemcpyDeviceToHost, stream));
     PCU_CUDA(cudaStreamSynchronize(stream));
     if (iters_host) *iters_host = seen.iter;
     return PCU_B200_OK;
+}
+
+// lloyd_3d / lloyd_2d: the counter-based initial sample of (n, D, seed) and the cube's cells.
+template <int D>
+int lloyd_device(pcu_b200_workspace* ws, long long n, unsigned seed, int num_lloyd, int num_newton, double* out,
+                 double* energy_host, int* iters_host, long long* passes, cudaStream_t stream) {
+    const long long N = n * D;
+    return lloyd_run<D>(
+        ws, n, 1, num_lloyd, num_newton, out, energy_host, iters_host, stream,
+        [&](double* x) -> int {
+            PCU_LAUNCH(lloyd_init_kernel, blocks_for(N), kThreads, stream, seed, N, x);
+            return PCU_B200_OK;
+        },
+        [&](const double* x, VorSync* sync, double** mom, VorSync* seen) -> int {
+            return vor_eval<D>(ws, x, n, sync, mom, passes, seen, stream);
+        });
+}
+
+// ---- Voronoi cells restricted to a triangle mesh and Lloyd sampling of its surface (rvd.cuh) ---------------------
+// One evaluation of the cells of n seeds x (fp64, (n, 3)) on the faces:
+//   the faces' candidate balls (a k = 1 search of the face centroids among the seeds), their tree, the pair count
+//   (one synchronisation sizes the pairs), the pairs, the seeds' self k-NN (k = 24, no tie replay), then pass 1 over
+//   every pair with the polygon on the stack at 16 vertices, and the fallback passes of the cube's cells (vor_fallback:
+//   k = 64 and 64 vertices, then every seed from 256 vertices in device memory up); finally each seed's pairs summed in
+//   order.  Synchronisations: the pair count, the count pass 1 leaves, and one per fallback pass or round that runs.
+//   passes[p] += pairs handled by pass p.
+struct RvScratch {
+    long long n = 0, m = 0;
+    int k1 = 1;
+    double *tri, *cen, *rad, *fd2, *balls, *sd2, *mom;
+    long long *fidx, *sidx, *start;
+    unsigned long long *local, *tiles, *bad;
+    VorSync* sync;
+    void carve(Carver& cv) {
+        tri = cv.take<double>((size_t)9 * m);
+        cen = cv.take<double>((size_t)3 * m);
+        rad = cv.take<double>((size_t)m);
+        fd2 = cv.take<double>((size_t)m);
+        fidx = cv.take<long long>((size_t)m);
+        balls = cv.take<double>((size_t)4 * m);
+        sd2 = cv.take<double>((size_t)k1 * n);
+        sidx = cv.take<long long>((size_t)k1 * n);
+        mom = cv.take<double>((size_t)kVorMoments * n);
+        start = cv.take<long long>((size_t)n);
+        local = cv.take<unsigned long long>((size_t)n);
+        tiles = cv.take<unsigned long long>((size_t)blocks_for(n));
+        bad = cv.take<unsigned long long>(1);
+        sync = cv.take<VorSync>(1);
+    }
+};
+
+int rv_check(pcu_b200_workspace* ws, const double* v, long long nv, const void* f, long long m, int fkind, long long n) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    PCU_TRY(mesh_check(v, nv, f, m, fkind));
+    if (n <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "num_samples must be > 0");
+    if (n > 0x7fffffffLL - 1) return fail(PCU_B200_INVALID_ARGUMENT, "restricted Voronoi: at most 2^31 - 2 seeds, got %lld", n);
+    return PCU_B200_OK;
+}
+
+// Carves the call's RvScratch and enqueues the per-face pass (corners, centroids, radii, faces out of range).
+int rv_prepare(pcu_b200_workspace* ws, RvScratch& r, const double* v, long long nv, const void* f, long long m, int fkind,
+               long long n, cudaStream_t stream) {
+    r.n = n; r.m = m; r.k1 = (int)std::min<long long>(kRvK1, n);
+    PCU_TRY(carve_scratch(ws, kRvd, stream, [&](Carver& cv) { r.carve(cv); }));
+    PCU_CUDA(cudaMemsetAsync(r.bad, 0, sizeof(unsigned long long), stream));
+    PCU_CUDA(cudaMemsetAsync(r.sync, 0, sizeof(VorSync), stream));
+    PCU_LAUNCH(rv_face_kernel, blocks_for(m), kThreads, stream, v, nv, f, fkind, m, r.tri, r.cen, r.rad, r.bad);
+    return PCU_B200_OK;
+}
+
+int rv_eval(pcu_b200_workspace* ws, const RvScratch& r, const double* x, VorSync* sync, double** mom_out, long long* passes,
+            VorSync* seen, cudaStream_t stream) {
+    const long long n = r.n, m = r.m;
+    *mom_out = r.mom;
+    PCU_TRY(knn_device<double>(ws, r.cen, m, x, n, 1, 1, r.fd2, r.fidx, nullptr, stream, nullptr, false));
+    PCU_LAUNCH(rv_ball_kernel, blocks_for(m), kThreads, stream, (const double*)r.cen, (const double*)r.rad, (const double*)r.fd2,
+               (const long long*)r.fidx, m, r.balls);
+    PCU_TRY(knn_device<double>(ws, x, n, x, n, r.k1, 1, r.sd2, r.sidx, nullptr, stream, nullptr, false));
+    MeshTree<RvBall> tree;   // in the arena, with its build's temporaries: nothing re-carves it before the pairs are out
+    PCU_TRY((build_mesh_tree<double, RvBall>)(ws, r.balls, m, nullptr, m, 0, false, nullptr, stream, tree));
+    const unsigned sb = blocks_for(n);
+    PCU_LAUNCH(rv_count_kernel, sb, kThreads, stream, x, n, m, (const MqScratch*)tree.sc, (const MqNode*)tree.nodes,
+               (const RvBall*)tree.leaves, (const int*)tree.ids, r.local, r.tiles);
+    PCU_LAUNCH(rv_tiles_kernel, 1, 1024, stream, r.tiles, (long long)sb, sync);
+    PCU_TRY(read_record(sync, seen, stream));
+    const long long P = seen->count;
+    if (P == 0) {   // every face has zero area
+        PCU_CUDA(cudaMemsetAsync(r.mom, 0, (size_t)n * kVorMoments * sizeof(double), stream));
+        return PCU_B200_OK;
+    }
+    int *pseed, *pface; double* pmom; unsigned char* flag; unsigned* counts;
+    const int rs = P > 0x7fffffffLL ? PCU_B200_OUT_OF_MEMORY : carve_scratch(ws, kAux, stream, [&](Carver& cv) {
+        pseed = cv.take<int>((size_t)P);
+        pface = cv.take<int>((size_t)P);
+        pmom = cv.take<double>((size_t)kVorMoments * P);
+        flag = cv.take<unsigned char>((size_t)P);
+        counts = cv.take<unsigned>(keep_count_words(P));
+    });
+    if (rs == PCU_B200_OUT_OF_MEMORY)
+        return fail(PCU_B200_OUT_OF_MEMORY, "restricted Voronoi: %lld (face, seed) pairs do not fit (%zu bytes of scratch, at most "
+                    "2^31 - 1 pairs)", P, (size_t)P * (8 + 8 * kVorMoments + 1));
+    PCU_TRY(rs);
+    PCU_LAUNCH(rv_emit_kernel, sb, kThreads, stream, x, n, m, (const MqScratch*)tree.sc, (const MqNode*)tree.nodes,
+               (const RvBall*)tree.leaves, (const int*)tree.ids, (const unsigned long long*)r.local, (const unsigned long long*)r.tiles,
+               r.start, pseed, pface);
+    VorPass p{};
+    p.x = x; p.x3 = x; p.n = n; p.count = P; p.nn_idx = r.sidx; p.nn_d2 = r.sd2; p.k = r.k1; p.list_is_all = r.k1 >= n;
+    p.list_of_seed = 1; p.mom = pmom; p.uncert = flag; p.pair_seed = pseed; p.pair_face = pface; p.tri = r.tri;
+    PCU_TRY(VorRestricted::launch(p, 0, stream));
+    passes[0] += P;
+    PCU_TRY(vor_fallback<VorRestricted>(ws, p, flag, counts, sync, passes, seen, stream));
+    PCU_LAUNCH(rv_reduce_kernel, sb, kThreads, stream, (const long long*)r.start, n, P, (const double*)pmom, r.mom);
+    return PCU_B200_OK;
+}
+
+int restricted_moments_device(pcu_b200_workspace* ws, const double* x, long long n, const double* v, long long nv, const void* f,
+                              long long m, int fkind, double* out_moments, long long* passes, cudaStream_t stream) {
+    RvScratch r;
+    PCU_TRY(rv_prepare(ws, r, v, nv, f, m, fkind, n, stream));
+    unsigned long long bad = 0;
+    PCU_TRY(read_record(r.bad, &bad, stream));
+    if (bad) return bad_corners(bad);
+    double* mom; VorSync seen;
+    PCU_TRY(rv_eval(ws, r, x, r.sync, &mom, passes, &seen, stream));
+    PCU_CUDA(cudaMemcpyAsync(out_moments, mom, (size_t)n * kVorMoments * sizeof(double), cudaMemcpyDeviceToDevice, stream));
+    return PCU_B200_OK;
+}
+
+// sample_mesh_lloyd: the first n samples of sample_mesh_random at `seed` (their fp64 positions) relaxed on the
+// restricted cells, with no domain test for the Newton phase's trial points.  The initial sample reads the face CDF's
+// record (one synchronisation) and fails as sample_mesh_random's caller does on faces out of range or a zero area.
+int sample_mesh_lloyd_device(pcu_b200_workspace* ws, const double* v, long long nv, const void* f, long long m, int fkind,
+                             long long n, unsigned seed, int num_lloyd, int num_newton, double* out, double* energy_host,
+                             int* iters_host, long long* passes, cudaStream_t stream) {
+    RvScratch r;
+    PCU_TRY(rv_prepare(ws, r, v, nv, f, m, fkind, n, stream));
+    return lloyd_run<3>(
+        ws, n, 0, num_lloyd, num_newton, out, energy_host, iters_host, stream,
+        [&](double* x) -> int {
+            MeshCdfScratch ms;
+            PCU_TRY(carve_scratch(ws, kMesh, stream, [&](Carver& cv) { ms.carve(cv, m); }));
+            PCU_TRY(enqueue_mesh_cdf<double>(ws, v, nv, f, fkind, m, ms.cdf, ms.tiles, ms.sc, ms.area, stream));
+            MeshArea area;
+            PCU_TRY(read_record(ms.area, &area, stream));
+            if (area.bad) return bad_corners(area.bad);
+            if (area.total == 0) return fail(PCU_B200_INVALID_ARGUMENT, "Mesh has zero area");
+            const unsigned blocks = (unsigned)std::min<long long>((n + kThreads - 1) / kThreads, (long long)ws->sm_count * 16);
+            PCU_LAUNCH((mesh_sample_kernel<double>), blocks, kThreads, stream, (const unsigned long long*)ms.cdf, m,
+                       (const MeshArea*)ms.area, (unsigned long long)seed, n, (const int*)nullptr, (const long long*)nullptr, v, nv, f,
+                       fkind, (void*)nullptr, 0, (double*)nullptr, x);
+            return PCU_B200_OK;
+        },
+        [&](const double* x, VorSync* sync, double** mom, VorSync* seen) -> int {
+            return rv_eval(ws, r, x, sync, mom, passes, seen, stream);
+        });
 }
 
 // Whether face indices of this kind are 64 bits wide.
@@ -3639,6 +3843,31 @@ int pcu_b200_lloyd(pcu_b200_workspace* ws, int64_t n, int dim, uint32_t seed, in
     int steps = 0;
     const int rs = dim == 3 ? lloyd_device<3>(ws, n, seed, num_lloyd, num_newton, out_points, out_energy, &steps, passes, (cudaStream_t)stream)
                             : lloyd_device<2>(ws, n, seed, num_lloyd, num_newton, out_points, out_energy, &steps, passes, (cudaStream_t)stream);
+    if (out_passes) for (int i = 0; i < 3; ++i) out_passes[i] = passes[i];
+    if (out_newton_steps) *out_newton_steps = steps;
+    return rs;
+}
+
+int pcu_b200_restricted_voronoi_moments(pcu_b200_workspace* ws, const double* seeds, int64_t n, const double* v, int64_t nv,
+                                        const void* f, int64_t nf, int f_kind, double* out_moments, int64_t* out_passes, void* stream) {
+    PCU_TRY(rv_check(ws, v, nv, f, nf, f_kind, n));
+    if (!seeds || !out_moments) return fail(PCU_B200_INVALID_ARGUMENT, "null seeds or output pointer");
+    PCU_ON_DEVICE(ws);
+    long long passes[3] = {0, 0, 0};
+    const int rs = restricted_moments_device(ws, seeds, n, v, nv, f, nf, f_kind, out_moments, passes, (cudaStream_t)stream);
+    if (out_passes) for (int i = 0; i < 3; ++i) out_passes[i] = passes[i];
+    return rs;
+}
+int pcu_b200_sample_mesh_lloyd(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                               int64_t num_samples, uint32_t seed, int num_lloyd, int num_newton, double* out_points,
+                               double* out_energy, int32_t* out_newton_steps, int64_t* out_passes, void* stream) {
+    PCU_TRY(rv_check(ws, v, nv, f, nf, f_kind, num_samples));
+    if (!out_points) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    long long passes[3] = {0, 0, 0};
+    int steps = 0;
+    const int rs = sample_mesh_lloyd_device(ws, v, nv, f, nf, f_kind, num_samples, seed, num_lloyd, num_newton, out_points, out_energy,
+                                            &steps, passes, (cudaStream_t)stream);
     if (out_passes) for (int i = 0; i < 3; ++i) out_passes[i] = passes[i];
     if (out_newton_steps) *out_newton_steps = steps;
     return rs;

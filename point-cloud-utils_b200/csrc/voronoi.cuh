@@ -14,8 +14,11 @@
 //        first unused neighbour (or of the k-th when the list is used up): no seed at least 2R away can cut the cell.
 // Volume, first moment and second moment about the seed are integrated in the same thread with a tetrahedron
 // (triangle) fan from the seed.  Every sum is sequential in one thread: no atomics, results are bit-reproducible.
+// The same passes clip the (face, seed) pairs of cells restricted to a triangle mesh (rvd.cuh), each as a convex
+// polygon (Poly3) with the same certificate, duplicate rule and cut tolerance.
 #pragma once
 #include <cooperative_groups.h>
+#include <type_traits>
 #include "common.cuh"
 #include "compact.cuh"
 
@@ -31,7 +34,8 @@ constexpr int kVorMoments = 5;            // per cell: volume, first moment abou
 constexpr double kVorClipTol = 1e-13;
 
 // One clipping pass over `count` cells.  Entry t of the pass is the cell rows[sub[t]] (a null array is the identity),
-// and its neighbour list is row sub[t] of the lists.
+// and its neighbour list is row sub[t] of the lists.  Restricted cells (rvd.cuh) clip (face, seed) pairs instead: the
+// row is a pair, whose seed and face the pair arrays give, and in the first pass the lists are the seeds' own.
 struct VorPass {
     const double* x;          // (n, D) seeds
     const double* x3;         // (n, 3) seeds (the 2-D seeds with z = 0)
@@ -47,6 +51,10 @@ struct VorPass {
     double* mom;              // (n, kVorMoments)
     unsigned char* uncert;    // (count): 1 = the cell is left to the next pass
     void* cells;              // last resort: one cell record per entry
+    const int* pair_seed;     // restricted cells: the seed of each pair (null: the row is the seed)
+    const int* pair_face;     // the face of each pair
+    const double* tri;        // (faces, 9): every face's corners
+    int list_of_seed;         // the neighbour list of an entry is its seed's row of the lists
 };
 
 // the k-NN search's rounding of d^2, so that "in the list" is decided exactly
@@ -270,6 +278,99 @@ struct Cell2 {
     }
 };
 
+// ---- restricted cells ---------------------------------------------------------------------------------------------
+// One face's share of a restricted cell (DESIGN.md §3, restricted cell): the triangle, relative to the seed, clipped
+// as a convex 3-D polygon (its vertex cycle) by each bisector, over V slots of storage it does not own and V more for
+// the clip's output.  A triangle clipped by k planes has at most 3 + k vertices.
+struct Poly3 {
+    double (*pos)[3];
+    double (*tmp)[3];
+    int V;
+    int nv;
+
+    __host__ __device__ void init(const double* c, const double* t) {   // t: the face's corners a, b, c
+        nv = 3;
+        for (int v = 0; v < 3; ++v)
+            for (int a = 0; a < 3; ++a) pos[v][a] = t[3 * v + a] - c[a];
+    }
+
+    __host__ __device__ double side(const double* p, const double* nrm, double d) const {
+        return p[0] * nrm[0] + p[1] * nrm[1] + p[2] * nrm[2] - d;
+    }
+
+    // Cell2::clip in 3-D: the same tolerance, interpolation from the outside end, and results.
+    __host__ __device__ int clip(const double* nrm, double d) {
+        const double tol = kVorClipTol * d;
+        int nout = 0;
+        for (int v = 0; v < nv; ++v) nout += side(pos[v], nrm, d) > tol;
+        if (nout == 0) return 0;
+        if (nout == nv) { nv = 0; return 3; }
+        int w = 0;
+        for (int v = 0; v < nv; ++v) {
+            const int u = v + 1 == nv ? 0 : v + 1;
+            const double hv = side(pos[v], nrm, d), hu = side(pos[u], nrm, d);
+            if (!(hv > tol)) {
+                if (w >= V) return 2;
+                for (int a = 0; a < 3; ++a) tmp[w][a] = pos[v][a];
+                ++w;
+            }
+            if ((hv > tol) != (hu > tol)) {
+                if (w >= V) return 2;
+                const double* o = hv > tol ? pos[v] : pos[u];
+                const double* i = hv > tol ? pos[u] : pos[v];
+                const double ho = hv > tol ? hv : hu, hi = hv > tol ? hu : hv;
+                const double f = fmin(1.0, ho / (ho - hi));
+                for (int a = 0; a < 3; ++a) tmp[w][a] = o[a] + (i[a] - o[a]) * f;
+                ++w;
+            }
+        }
+        for (int v = 0; v < w; ++v)
+            for (int a = 0; a < 3; ++a) pos[v][a] = tmp[v][a];
+        nv = w;
+        return 1;
+    }
+
+    __host__ __device__ double radius2() const {
+        double r = 0.0;
+        for (int v = 0; v < nv; ++v) r = fmax(r, pos[v][0] * pos[v][0] + pos[v][1] * pos[v][1] + pos[v][2] * pos[v][2]);
+        return r;
+    }
+
+    // Area, first moment and second moment about the seed by a fan from vertex 0: a fan triangle w0 w1 w2 of area A
+    // adds A (w0 + w1 + w2) / 3 and A / 12 (sum |w_a|^2 + |sum w_a|^2).
+    __host__ __device__ void integrate(double* m) const {
+        double ar = 0.0, mx = 0.0, my = 0.0, mz = 0.0, m2 = 0.0;
+        const double* A = pos[0];
+        for (int v = 1; v + 1 < nv; ++v) {
+            const double* B = pos[v];
+            const double* C = pos[v + 1];
+            const double e1[3] = {B[0] - A[0], B[1] - A[1], B[2] - A[2]}, e2[3] = {C[0] - A[0], C[1] - A[1], C[2] - A[2]};
+            const double cx = e1[1] * e2[2] - e1[2] * e2[1], cy = e1[2] * e2[0] - e1[0] * e2[2], cz = e1[0] * e2[1] - e1[1] * e2[0];
+            const double t = 0.5 * sqrt(cx * cx + cy * cy + cz * cz);
+            const double sx = A[0] + B[0] + C[0], sy = A[1] + B[1] + C[1], sz = A[2] + B[2] + C[2];
+            ar += t;
+            mx += t * sx / 3.0;
+            my += t * sy / 3.0;
+            mz += t * sz / 3.0;
+            const double q = A[0] * A[0] + A[1] * A[1] + A[2] * A[2] + B[0] * B[0] + B[1] * B[1] + B[2] * B[2] +
+                             C[0] * C[0] + C[1] * C[1] + C[2] * C[2] + sx * sx + sy * sy + sz * sz;
+            m2 += t * q / 12.0;
+        }
+        m[0] = ar; m[1] = mx; m[2] = my; m[3] = mz; m[4] = m2;
+    }
+};
+
+template <int V>
+struct PolyStack {
+    double pos[V][3];
+    double tmp[V][3];
+    __host__ __device__ Poly3 view() { return Poly3{pos, tmp, V, 0}; }
+};
+__host__ __device__ inline size_t poly_bytes(int V) { return (size_t)V * 48; }
+__host__ __device__ inline Poly3 poly_at(unsigned char* base, int V) {
+    return Poly3{reinterpret_cast<double (*)[3]>(base), reinterpret_cast<double (*)[3]>(base + (size_t)V * 24), V, 0};
+}
+
 // Storage of a cell with a fixed capacity of V vertices (and, in 3-D, P = V / 2 + 8 plane numbers), and its layout in
 // a block of device memory for a capacity chosen at run time.
 template <int D, int V, class I = unsigned char>
@@ -308,16 +409,20 @@ __host__ __device__ inline Cell2 vor_cell_at2(unsigned char* base, int V) {
     return Cell2{reinterpret_cast<double (*)[2]>(base), reinterpret_cast<double (*)[2]>(base + (size_t)V * 16), V, 0};
 }
 
-// Entry t of a pass, in `cell`'s storage.  C: Cell2 or Cell3 at the pass's capacity.
+// Entry t of a pass, in `cell`'s storage.  C: Cell2 or Cell3 at the pass's capacity, or Poly3 for a (face, seed) pair.
 template <int D, class C>
-__host__ __device__ void vor_cell(const VorPass& a, long long t, C& cell) {
+__host__ __device__ __forceinline__ void vor_cell(const VorPass& a, long long t, C& cell) {
     const long long e = a.sub ? (long long)a.sub[t] : t;
-    const long long row = a.rows ? (long long)a.rows[e] : e;
-    const double* c = a.x + row * D;
-    const double* c3 = a.x3 + row * 3;
-    const long long* li = a.nn_idx + e * a.k;
-    const double* ld = a.nn_d2 + e * a.k;
-    cell.init(c);
+    const long long row = a.rows ? (long long)a.rows[e] : e;                    // the output row: a cell or a pair
+    constexpr bool pair = std::is_same<C, Poly3>::value;
+    const long long seed = pair ? (long long)a.pair_seed[row] : row;
+    const long long list = pair && a.list_of_seed ? seed : e;
+    const double* c = a.x + seed * D;
+    const double* c3 = a.x3 + seed * 3;
+    const long long* li = a.nn_idx + list * a.k;
+    const double* ld = a.nn_d2 + list * a.k;
+    if constexpr (pair) cell.init(c, a.tri + 9 * (long long)a.pair_face[row]);
+    else cell.init(c);
     double r2 = cell.radius2();
     bool done = false, empty = false, over = false;
     // a clip by the bisector of seed s; false: stop here (empty or over capacity)
@@ -337,9 +442,9 @@ __host__ __device__ void vor_cell(const VorPass& a, long long t, C& cell) {
         if (s < 0) break;                 // a short list: every seed is in it
         const double d2 = ld[j];
         if (4.0 * r2 * (1.0 + kVorMargin) < d2) { done = true; break; }
-        if (s == row) continue;
+        if (s == seed) continue;
         if (d2 == 0.0) {                  // a duplicate: the lowest index owns the position
-            if (s < row) { empty = true; break; }
+            if (s < seed) { empty = true; break; }
             continue;
         }
         if (!cut(s)) break;
@@ -350,11 +455,11 @@ __host__ __device__ void vor_cell(const VorPass& a, long long t, C& cell) {
         } else if (a.scan_all) {
             const double dk = ld[a.k - 1];
             for (long long s = 0; s < a.n && !empty && !over; ++s) {
-                if (s == row) continue;
+                if (s == seed) continue;
                 const double d2 = vor_d2(c3, a.x3 + s * 3);
                 if (d2 < dk) continue;     // in the list, clipped above
                 if (d2 == 0.0) {
-                    if (s < row) empty = true;
+                    if (s < seed) empty = true;
                     continue;
                 }
                 if (4.0 * r2 * (1.0 + kVorMargin) < d2) continue;
@@ -401,6 +506,25 @@ __global__ void __launch_bounds__(kVorThreads) vor_clip_wide_kernel(VorPass a, i
     }
 }
 
+// The (face, seed) pairs of restricted cells: one thread per entry, its polygon on the stack at V vertices, or for the
+// last resort in device memory (a.cells).
+template <int V>
+__global__ void __launch_bounds__(kVorThreads, 4) rv_clip_kernel(VorPass a) {
+    grid_dependency_wait();
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= a.count) return;
+    PolyStack<V> s;
+    Poly3 cell = s.view();
+    vor_cell<3>(a, t, cell);
+}
+__global__ void __launch_bounds__(kVorThreads) rv_clip_wide_kernel(VorPass a, int V) {
+    grid_dependency_wait();
+    const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= a.count) return;
+    Poly3 cell = poly_at((unsigned char*)a.cells + (size_t)t * poly_bytes(V), V);
+    vor_cell<3>(a, t, cell);
+}
+
 // The next round of the last resort: the entries of this round (sub) whose cells are still flagged, in order.
 __global__ void __launch_bounds__(kThreads) vor_keep_sub_kernel(const unsigned char* __restrict__ keep, long long n,
                                                                 const unsigned* __restrict__ block_offset,
@@ -422,13 +546,14 @@ __global__ void __launch_bounds__(kThreads) vor_lift_kernel(const double* __rest
     x3[i * 3 + 2] = 0.0;
 }
 
-// the (count, 3) seeds of the compacted rows: the queries of the next k-NN search
+// the (count, 3) seeds of the compacted rows (of seed[row] when seed is not null): the queries of the next k-NN search
 __global__ void __launch_bounds__(kThreads) vor_gather_kernel(const double* __restrict__ x3, const int* __restrict__ rows,
-                                                              long long count, double* __restrict__ q) {
+                                                              long long count, double* __restrict__ q,
+                                                              const int* __restrict__ seed) {
     grid_dependency_wait();
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
-    const long long r = rows[i];
+    const long long r = seed ? seed[rows[i]] : rows[i];
     for (int a = 0; a < 3; ++a) q[i * 3 + a] = x3[r * 3 + a];
 }
 
@@ -496,6 +621,7 @@ struct LbArgs {
     VorSync* sync;
     double* energy;    // num_newton + 1: F of the accepted points
     int num_newton;
+    int cube;          // trial points must lie in the unit cube (square); restricted cells have no domain test
 };
 
 // Sum over the grid in a fixed order: the block's tree, then the blocks in index order, redundantly in every block.
@@ -530,7 +656,8 @@ __device__ double lb_grid_sum(double v, double* partial, int& parity) {
 
 // One step of the Newton phase, after the cells of the trial point x_t have been computed (or of the starting point,
 // st->init): the Armijo test of the trial, then either the L-BFGS update and the next direction, or a halved step;
-// and the next trial point x_acc + t p inside the cube (a point outside fails the test without being evaluated).
+// and the next trial point x_acc + t p inside the cube (a point outside fails the test without being evaluated; with
+// a.cube unset, as for restricted cells, every trial point is evaluated).
 // Cooperative: every decision is taken identically by every thread from grid-wide sums.
 __global__ void __launch_bounds__(kThreads) lbfgs_step_kernel(LbArgs a) {
     grid_dependency_wait();
@@ -616,13 +743,16 @@ __global__ void __launch_bounds__(kThreads) lbfgs_step_kernel(LbArgs a) {
             if (!(s.gtp < 0.0)) s.done = 1;          // not a descent direction: the line search cannot succeed
         }
     }
-    while (!s.done) {                                // the trial point, inside the cube
+    while (!s.done) {                                // the trial point, inside the cube when there is one
         double outside = 0.0;
-        for (long long i = gtid; i < N; i += gsize) {
-            const double v = a.x_acc[i] + s.t * a.p[i];
-            outside += (v < 0.0 || v > 1.0) ? 1.0 : 0.0;
+        if (a.cube) {
+            for (long long i = gtid; i < N; i += gsize) {
+                const double v = a.x_acc[i] + s.t * a.p[i];
+                outside += (v < 0.0 || v > 1.0) ? 1.0 : 0.0;
+            }
+            outside = lb_grid_sum(outside, a.partial, parity);
         }
-        if (lb_grid_sum(outside, a.partial, parity) == 0.0) {
+        if (outside == 0.0) {
             for (long long i = gtid; i < N; i += gsize) a.x_t[i] = a.x_acc[i] + s.t * a.p[i];
             break;
         }
