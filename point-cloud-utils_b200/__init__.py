@@ -24,8 +24,6 @@ Everything is computed by hand-written sm_90a kernels behind the C ABI in includ
 There is deliberately NO CPU fallback: importing this package without its compiled extension, or
 calling it without a Hopper (H100) GPU, raises.
 """
-import importlib as _importlib
-
 import numpy as _np
 
 try:
@@ -35,6 +33,8 @@ except ImportError as _e:  # pragma: no cover - exercised only on a broken insta
         "pcu_b200: the compiled extension (_pcu_internal / libpcu_b200.so) is missing or failed to load: %s.\n"
         "Build it in-tree with `python -c 'import __graft_entry__ as g; g.build()'` from the repository root.\n"
         "There is no pure-Python or CPU fallback for this package." % (_e,)) from _e
+from ._call import (_asarrays, _call_args, _check_float, _dev, _form, _is_tensor, _ordinal, _run,  # noqa: E402
+                    _same_device, _torch)
 
 __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_distance", "chamfer_distance",
            "batched_chamfer_distance", "estimate_point_cloud_normals_knn", "estimate_point_cloud_normals_ball",
@@ -70,45 +70,9 @@ def current_device():
     return _pcu_internal._current_device()
 
 
-def _dev(device):
-    """``device=`` keyword -> ordinal for the native layer (-1: let the library choose, see current_device)."""
-    if device is None:
-        return -1
-    if isinstance(device, int):
-        d = device
-    elif isinstance(device, str):
-        name = device.strip().lower()
-        if name == "cuda":
-            return -1
-        if not name.startswith("cuda:") or not name[5:].isdigit():
-            raise ValueError("device must be an int, None, 'cuda' or 'cuda:<i>' (got %r)" % (device,))
-        d = int(name[5:])
-    elif getattr(device, "type", None) == "cuda":           # torch.device
-        d = -1 if device.index is None else int(device.index)
-    else:
-        raise ValueError("device must be an int, None, 'cuda', 'cuda:<i>' or a CUDA torch.device (got %r)" % (device,))
-    if d >= device_count() or d < -1:
-        raise ValueError("device %d out of range: %d usable GPU(s) visible" % (d, device_count()))
-    return d
-
-
 def launch_count():
     """Kernels launched by the native library in this process so far."""
     return _pcu_internal._launch_count()
-
-
-# ---------------------------------------------------------------------------------------------
-# torch plumbing (device residency only; no torch op sits on the hot path)
-def _torch():
-    try:
-        return _importlib.import_module("torch")
-    except ImportError:  # pragma: no cover
-        return None
-
-
-def _is_tensor(x):
-    t = _torch() if type(x).__module__.startswith("torch") else None
-    return t is not None and isinstance(x, t.Tensor)
 
 
 def _check_tensor_pair(a, b, name_a, name_b):
@@ -133,18 +97,6 @@ def _check_tensor_pair(a, b, name_a, name_b):
     return a.detach().contiguous(), b.detach().contiguous()
 
 
-def _same_device(t, device):
-    """CUDA tensors run where they live; a contradicting device= is an argument error."""
-    d = _dev(device)
-    if d >= 0 and d != (t.device.index or 0):
-        raise ValueError("device=%r contradicts the inputs, which live on %s" % (device, t.device))
-
-
-def _stream_of(t):
-    torch = _torch()
-    return torch.cuda.current_stream(t.device).cuda_stream
-
-
 def _stats_from_tensor(buf, which):
     """Decode one pcu_b200_nn_stats from the raw device buffer (synchronises)."""
     host = buf.cpu()
@@ -164,7 +116,7 @@ def _resolved_stats(buf, which, q, d, leaf):
         torch = _torch()
         _pcu_internal._resolve_witness_device(q.dtype == torch.float64, q.data_ptr(), q.shape[0], d.data_ptr(),
                                               d.shape[0], buf.data_ptr() + 8 * _STATS_WORDS * which, int(leaf),
-                                              q.device.index or 0, _stream_of(q))
+                                              *_call_args(q))
         st = _stats_from_tensor(buf, which)
     return st
 
@@ -175,8 +127,7 @@ def _stats_device(a, b, both, leaf):
     buf = torch.empty(2 * _STATS_WORDS, dtype=torch.int64, device=a.device)   # every record is written by the sweep
     val = torch.empty((), dtype=a.dtype, device=a.device)
     _pcu_internal._stats_device(a.dtype == torch.float64, both, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0],
-                                buf.data_ptr(), val.data_ptr() if both else 0, int(leaf), a.device.index or 0,
-                                _stream_of(a))
+                                buf.data_ptr(), val.data_ptr() if both else 0, int(leaf), *_call_args(a))
     return buf, val
 
 
@@ -240,14 +191,13 @@ def prepare_cloud(points, *, k=None, max_points_per_leaf=10, device=None):
             return prepare_cloud(points.detach().numpy(), k=k, max_points_per_leaf=max_points_per_leaf, device=device)
         _same_device(points, device)
         p = points.detach().contiguous()
-        dev = p.device.index or 0
-        h = _pcu_internal._cloud_prepare_device(p.dtype == torch.float64, p.data_ptr(), p.shape[0], dev, _stream_of(p), kk,
+        dev, stream = _call_args(p)
+        h = _pcu_internal._cloud_prepare_device(p.dtype == torch.float64, p.data_ptr(), p.shape[0], dev, stream, kk,
                                                 int(max_points_per_leaf))
         return PreparedCloud(h, p.shape[0], p.dtype == torch.float64, dev, True, **meta)
     pts = _np.asarray(points)
-    d = _dev(device)
-    h = _pcu_internal._cloud_prepare(pts, d, kk, int(max_points_per_leaf))
-    return PreparedCloud(h, pts.shape[0], pts.dtype == _np.float64, _pcu_internal._current_device() if d < 0 else d, False, **meta)
+    h = _pcu_internal._cloud_prepare(pts, _dev(device), kk, int(max_points_per_leaf))
+    return PreparedCloud(h, pts.shape[0], pts.dtype == _np.float64, _ordinal(device), False, **meta)
 
 
 def pinned_empty(n, dtype=_np.float32, cols=3, *, device=None):
@@ -274,7 +224,7 @@ def _prepared_resolved(buf, which, xs, cloud, leaf):
         yp, m = _pcu_internal._cloud_points(cloud._handle), cloud.shape[0]
         q, n, d, k = (xs.data_ptr(), xs.shape[0], yp, m) if which == 0 else (yp, m, xs.data_ptr(), xs.shape[0])
         _pcu_internal._resolve_witness_device(cloud._f64, q, n, d, k, buf.data_ptr() + 8 * _STATS_WORDS * which, int(leaf),
-                                              cloud.device_index, _stream_of(xs))
+                                              *_call_args(xs))
         st = _stats_from_tensor(buf, which)
     return st
 
@@ -293,7 +243,7 @@ def _prepared_stats(x, cloud, both, leaf, device):
         buf = torch.empty(2 * _STATS_WORDS, dtype=torch.int64, device=xs.device)
         val = torch.empty((), dtype=xs.dtype, device=xs.device)
         _pcu_internal._stats_prepared_device(cloud._f64, both, xs.data_ptr(), xs.shape[0], cloud._handle, buf.data_ptr(),
-                                             val.data_ptr() if both else 0, int(leaf), cloud.device_index, _stream_of(xs))
+                                             val.data_ptr() if both else 0, int(leaf), *_call_args(xs))
         return "cuda", xs.dtype, val, (buf, xs)
     if _is_tensor(x):
         x = x.detach().numpy()
@@ -348,7 +298,7 @@ def k_nearest_neighbors(query_points, dataset_points, k, squared_distances=False
         corrs = torch.empty((n, int(k)), dtype=torch.int64, device=q.device)
         _pcu_internal._knn_device(q.dtype == torch.float64, q.data_ptr(), n, d.data_ptr(), d.shape[0], int(k),
                                   bool(squared_distances), dists.data_ptr(), corrs.data_ptr(), 0,
-                                  int(max_points_per_leaf), q.device.index or 0, _stream_of(q))
+                                  int(max_points_per_leaf), *_call_args(q))
         return dists.squeeze(), corrs.squeeze()
     return _pcu_internal.k_nearest_neighbors(_np.asarray(query_points), _np.asarray(dataset_points), int(k),
                                              bool(squared_distances), int(max_points_per_leaf), int(num_threads),
@@ -373,7 +323,7 @@ def _knn_prepared(query_points, cloud, k, squared, leaf, device):
         dists = torch.empty((n, k), dtype=q.dtype, device=q.device)
         corrs = torch.empty((n, k), dtype=torch.int64, device=q.device)
         _pcu_internal._knn_prepared_device(cloud._f64, q.data_ptr(), n, cloud._handle, k, squared, dists.data_ptr(),
-                                           corrs.data_ptr(), 0, leaf, cloud.device_index, _stream_of(q))
+                                           corrs.data_ptr(), 0, leaf, *_call_args(q))
         return dists.squeeze(), corrs.squeeze()
     as_tensor = _is_tensor(query_points)
     qn = query_points.detach().numpy() if as_tensor else _np.asarray(query_points)
@@ -585,54 +535,19 @@ def estimate_point_cloud_normals_knn(points, num_neighbors, view_directions=None
     same plane-fit direction up to rounding (1e-6 in the dot product for well-separated singular values) and, when no
     view directions are given, up to sign -- the reference's sign is whatever Eigen's JacobiSVD returns.
     """
-    if _is_tensor(points):
-        torch = _torch()
-        if points.dtype not in (torch.float32, torch.float64):
-            raise ValueError("Invalid scalar type (%s) for argument 'points'. Expected one of ['float32', 'float64']." % points.dtype)
-        if points.dim() != 2 or points.shape[-1] != 3:
-            raise ValueError("Invalid shape for points, must be (n, 3) but got " + str(tuple(points.shape)))
-        if points.shape[0] == 0:
-            raise ValueError("Invalid point set with zero elements: points must have shape (n, 3)")
-        if int(num_neighbors) <= 0:
-            raise ValueError("Invalid number of neighbors (%d) must be greater than 0." % int(num_neighbors))
-        dirs = None
-        if view_directions is not None:
-            if not _is_tensor(view_directions) or view_directions.dtype != points.dtype or \
-                    view_directions.device != points.device or tuple(view_directions.shape) != tuple(points.shape):
-                raise ValueError("Invalid view directions does not match the number of points. If view directions are passed "
-                                 "in, they must be a tensor with the dtype, device and shape of points.")
-            dirs = view_directions.detach().contiguous()
-        pts = points.detach().contiguous()
-        if not pts.is_cuda:
-            i, nrm = estimate_point_cloud_normals_knn(pts.numpy(), num_neighbors, None if dirs is None else dirs.numpy(),
-                                                      drop_angle_threshold, max_points_per_leaf, num_threads, device=device)
-            return torch.from_numpy(i), torch.from_numpy(nrm)
-        _same_device(pts, device)
-        n = pts.shape[0]
-        idx = torch.empty(n, dtype=torch.int64, device=pts.device)
-        nrm = torch.empty((n, 3), dtype=pts.dtype, device=pts.device)
-        count = torch.empty(1, dtype=torch.int64, device=pts.device)
-        _pcu_internal._normals_knn_device(pts.dtype == torch.float64, pts.data_ptr(), n, 0 if dirs is None else dirs.data_ptr(),
-                                          int(num_neighbors), float(drop_angle_threshold), idx.data_ptr(), nrm.data_ptr(),
-                                          count.data_ptr(), int(max_points_per_leaf), pts.device.index or 0, _stream_of(pts))
-        if dirs is None and n >= int(num_neighbors):
-            return idx, nrm          # every point is kept: no need to wait for the count
-        m = int(count.item())
-        return idx[:m], nrm[:m]
-    if type(points) != _np.ndarray:
-        raise ValueError("Invalid type for points, must be a NumPy array, but got " + str(type(points)) + ".")
-    if view_directions is None:
-        view_directions = _np.zeros([0, 3], dtype=points.dtype)
-    if type(view_directions) != _np.ndarray:
-        raise ValueError("Invalid type for view_directions, must be None or a NumPy array, but got " +
-                         str(type(view_directions)) + ".")
-    if len(points.shape) != 2 or points.shape[-1] != 3:
-        raise ValueError("Invalid shape for points, must be (n, 3) but got " + str(points.shape))
-    if len(view_directions.shape) != 2:
-        raise ValueError("Invalid shape for view_directions, must be (n, 3) but got " + str(view_directions.shape))
-    return _pcu_internal.estimate_point_cloud_normals_knn_internal(points, view_directions, int(num_neighbors),
-                                                                   int(max_points_per_leaf), float(drop_angle_threshold),
-                                                                   int(num_threads), -1, _dev(device))
+    def host(p, dirs):
+        return _pcu_internal.estimate_point_cloud_normals_knn_internal(p, dirs, int(num_neighbors), int(max_points_per_leaf),
+                                                                       float(drop_angle_threshold), int(num_threads), -1,
+                                                                       _dev(device))
+
+    def launch(pts, dirs, idx, nrm, count, dev, stream):
+        _pcu_internal._normals_knn_device(pts.dtype == _torch().float64, pts.data_ptr(), pts.shape[0],
+                                          0 if dirs is None else dirs.data_ptr(), int(num_neighbors),
+                                          float(drop_angle_threshold), idx.data_ptr(), nrm.data_ptr(), count.data_ptr(),
+                                          int(max_points_per_leaf), dev, stream)
+        return dirs is None and pts.shape[0] >= int(num_neighbors)
+
+    return _normals(points, view_directions, device, host, launch, num_neighbors)
 
 
 def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None, drop_angle_threshold=_np.deg2rad(90.0),
@@ -669,7 +584,30 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
     min_pts_per_ball) are the reference's; normals agree up to rounding and, without view directions, up to sign.
     """
     seed = int(_np.random.randint(2 ** 31 - 1))
-    if _is_tensor(points):
+
+    def host(p, dirs):
+        return _pcu_internal.estimate_point_cloud_normals_ball_internal(p, dirs, float(ball_radius), int(min_pts_per_ball),
+                                                                        int(max_pts_per_ball), float(drop_angle_threshold),
+                                                                        int(max_points_per_leaf), int(num_threads),
+                                                                        str(weight_function), seed, _dev(device))
+
+    def launch(pts, dirs, idx, nrm, count, dev, stream):
+        _pcu_internal._normals_ball_device(pts.dtype == _torch().float64, pts.data_ptr(), pts.shape[0],
+                                           0 if dirs is None else dirs.data_ptr(), float(ball_radius), int(min_pts_per_ball),
+                                           int(max_pts_per_ball), float(drop_angle_threshold), str(weight_function), seed,
+                                           idx.data_ptr(), nrm.data_ptr(), count.data_ptr(), dev, stream)
+        return False
+
+    return _normals(points, view_directions, device, host, launch)
+
+
+def _normals(points, view_directions, device, host, launch, num_neighbors=None):
+    """The call path of the two normal estimators.  numpy arrays go to host(points, view_directions), the binding's host
+    entry point; CPU tensors go there as numpy arrays and come back as tensors.  CUDA tensors go to launch(points, view
+    directions or None, idx, normals, count, device index, stream), which returns True when every point is kept, so
+    that the count need not be read.  num_neighbors: the k-NN estimator's, checked with the tensor arguments."""
+    tensor = _is_tensor(points)
+    if tensor:
         torch = _torch()
         if points.dtype not in (torch.float32, torch.float64):
             raise ValueError("Invalid scalar type (%s) for argument 'points'. Expected one of ['float32', 'float64']." % points.dtype)
@@ -677,30 +615,26 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
             raise ValueError("Invalid shape for points, must be (n, 3) but got " + str(tuple(points.shape)))
         if points.shape[0] == 0:
             raise ValueError("Invalid point set with zero elements: points must have shape (n, 3)")
-        dirs = None
-        if view_directions is not None:
-            if not _is_tensor(view_directions) or view_directions.dtype != points.dtype or \
-                    view_directions.device != points.device or tuple(view_directions.shape) != tuple(points.shape):
-                raise ValueError("Invalid view directions does not match the number of points. If view directions are passed "
-                                 "in, they must be a tensor with the dtype, device and shape of points.")
-            dirs = view_directions.detach().contiguous()
-        pts = points.detach().contiguous()
-        if not pts.is_cuda:
-            i, nrm = estimate_point_cloud_normals_ball(pts.numpy(), ball_radius, None if dirs is None else dirs.numpy(),
-                                                       drop_angle_threshold, min_pts_per_ball, max_pts_per_ball, weight_function,
-                                                       max_points_per_leaf, num_threads, device=device)
-            return torch.from_numpy(i), torch.from_numpy(nrm)
-        _same_device(pts, device)
-        n = pts.shape[0]
-        idx = torch.empty(n, dtype=torch.int64, device=pts.device)
-        nrm = torch.empty((n, 3), dtype=pts.dtype, device=pts.device)
-        count = torch.empty(1, dtype=torch.int64, device=pts.device)
-        _pcu_internal._normals_ball_device(pts.dtype == torch.float64, pts.data_ptr(), n, 0 if dirs is None else dirs.data_ptr(),
-                                           float(ball_radius), int(min_pts_per_ball), int(max_pts_per_ball),
-                                           float(drop_angle_threshold), str(weight_function), seed, idx.data_ptr(), nrm.data_ptr(),
-                                           count.data_ptr(), pts.device.index or 0, _stream_of(pts))
-        m = int(count.item())
-        return idx[:m], nrm[:m]
+        if num_neighbors is not None and int(num_neighbors) <= 0:
+            raise ValueError("Invalid number of neighbors (%d) must be greater than 0." % int(num_neighbors))
+        if view_directions is not None and (not _is_tensor(view_directions) or view_directions.dtype != points.dtype or
+                                            view_directions.device != points.device or
+                                            tuple(view_directions.shape) != tuple(points.shape)):
+            raise ValueError("Invalid view directions does not match the number of points. If view directions are passed "
+                             "in, they must be a tensor with the dtype, device and shape of points.")
+        points = points.detach().contiguous()
+        view_directions = None if view_directions is None else view_directions.detach().contiguous()
+        if points.is_cuda:
+            _same_device(points, device)
+            n = points.shape[0]
+            idx = torch.empty(n, dtype=torch.int64, device=points.device)
+            nrm = torch.empty((n, 3), dtype=points.dtype, device=points.device)
+            count = torch.empty(1, dtype=torch.int64, device=points.device)
+            if launch(points, view_directions, idx, nrm, count, *_call_args(points)):
+                return idx, nrm          # every point is kept: no need to wait for the count
+            m = int(count.item())
+            return idx[:m], nrm[:m]
+        points, view_directions = points.numpy(), None if view_directions is None else view_directions.numpy()
     if type(points) != _np.ndarray:
         raise ValueError("Invalid type for points, must be a NumPy array, but got " + str(type(points)) + ".")
     if view_directions is None:
@@ -712,10 +646,8 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
         raise ValueError("Invalid shape for points, must be (n, 3) but got " + str(points.shape))
     if len(view_directions.shape) != 2:
         raise ValueError("Invalid shape for view_directions, must be (n, 3) but got " + str(view_directions.shape))
-    return _pcu_internal.estimate_point_cloud_normals_ball_internal(points, view_directions, float(ball_radius),
-                                                                    int(min_pts_per_ball), int(max_pts_per_ball),
-                                                                    float(drop_angle_threshold), int(max_points_per_leaf),
-                                                                    int(num_threads), str(weight_function), seed, _dev(device))
+    out = host(points, view_directions)
+    return tuple(_torch().from_numpy(o) for o in out) if tensor else out
 
 
 # ---------------------------------------------------------------------------------------------
@@ -805,50 +737,43 @@ from ._mesh_geometry import mesh_face_areas, estimate_mesh_face_normals, estimat
 
 def _voxel_internal(points, attrib, voxel_size, min_bound, max_bound, min_points_per_voxel, device, return_counts=False):
     """downsample_point_cloud_voxel_grid_internal (/root/reference/src/sample_point_cloud.cpp:336-367) on the GPU:
-    (mean points, mean attributes[, points per voxel]); numpy in -> numpy out, CUDA tensors in -> CUDA tensors out."""
+    (mean points, mean attributes[, points per voxel]).  attrib None or empty: no attributes, and an empty (0, 0) array
+    (of attrib's dtype for numpy inputs, of points' for tensors) in their place."""
+    has_att = attrib is not None and int(_np.prod(attrib.shape)) > 0
+    arrays = _asarrays([points, attrib] if has_att else [points])
+    form = _form(arrays, ["points", "attrib"])
+    _check_float(points, "v")
+    if has_att or form == "numpy":
+        _check_float(attrib, "attrib")
+    if len(points.shape) != 2 or points.shape[1] != 3 or points.shape[0] == 0:
+        raise ValueError("points must have shape (n, 3) with n > 0, got " + str(tuple(points.shape)))
+    n = int(points.shape[0])
+    if has_att and attrib.shape[0] != n:                                                          # :184-189
+        raise ValueError("Invalid number of attributes (%d). Must match number of input vertices (%d) or be 0." % (attrib.shape[0], n))
     torch = _torch()
-    is_np = isinstance(points, _np.ndarray)
-    if is_np:
-        if points.dtype not in (_np.float32, _np.float64):
-            raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected one of ['float32', 'float64']." % points.dtype)
-        if attrib.dtype not in (_np.float32, _np.float64):
-            raise ValueError("Invalid scalar type (%s) for argument 'attrib'. Expected one of ['float32', 'float64']." % attrib.dtype)
-        dev = torch.device("cuda", _pcu_internal._current_device() if _dev(device) < 0 else _dev(device))
-        pts = torch.from_numpy(_np.ascontiguousarray(points)).to(dev)
-        att = torch.from_numpy(_np.ascontiguousarray(attrib)).to(dev) if attrib.size else None
-    else:
-        if points.dtype not in (torch.float32, torch.float64) or not points.is_cuda:
-            raise ValueError("points must be a float32 / float64 numpy array or CUDA tensor")
-        pts = points.detach().contiguous()
-        att = attrib.detach().contiguous() if attrib is not None and attrib.numel() else None
-        if att is not None and (att.dtype not in (torch.float32, torch.float64) or att.device != pts.device):
-            raise ValueError("attributes must be float32 / float64 tensors on the device of points")
-    if pts.dim() != 2 or pts.shape[1] != 3 or pts.shape[0] == 0:
-        raise ValueError("points must have shape (n, 3) with n > 0, got " + str(tuple(pts.shape)))
-    n = pts.shape[0]
-    cols = 0
-    if att is not None:
-        if att.shape[0] != n:                                                                   # :184-189
-            raise ValueError("Invalid number of attributes (%d). Must match number of input vertices (%d) or be 0." % (att.shape[0], n))
-        att = att.reshape(n, -1)
-        cols = att.shape[1]
-    out_p = torch.empty((n, 3), dtype=pts.dtype, device=pts.device)
-    out_a = torch.empty((n, cols), dtype=att.dtype, device=pts.device) if cols else None
-    counts = torch.empty(n, dtype=torch.int32, device=pts.device) if return_counts else None
-    rows = torch.empty(1, dtype=torch.int64, device=pts.device)
-    _pcu_internal._voxel_downsample_device(pts.dtype == torch.float64, pts.data_ptr(), n, att.data_ptr() if cols else 0, cols,
-                                           bool(cols and att.dtype == torch.float64), [float(v) for v in voxel_size],
-                                           [float(v) for v in min_bound], [float(v) for v in max_bound], int(min_points_per_voxel),
-                                           out_p.data_ptr(), out_a.data_ptr() if cols else 0, counts.data_ptr() if return_counts else 0,
-                                           rows.data_ptr(), pts.device.index or 0, _stream_of(pts))
-    m = int(rows.item())
-    out_p = out_p[:m]
-    out_a = out_a[:m] if cols else (torch.zeros((0, 0), dtype=pts.dtype, device=pts.device))
-    if is_np:
-        res = (out_p.cpu().numpy(), out_a.cpu().numpy().reshape((m,) + attrib.shape[1:]) if cols else _np.zeros([0, 0], dtype=attrib.dtype))
-        return res + ((counts[:m].cpu().numpy(),) if return_counts else ())
-    res = (out_p, out_a.reshape((m,) + tuple(attrib.shape[1:])) if cols else out_a)
-    return res + ((counts[:m],) if return_counts else ())
+
+    def body(pts, *rest):
+        att, (dev, stream) = (rest[0].reshape(n, -1) if has_att else None), rest[-2:]
+        cols = att.shape[1] if has_att else 0
+        out_p = torch.empty((n, 3), dtype=pts.dtype, device=pts.device)
+        out_a = torch.empty((n, cols), dtype=att.dtype, device=pts.device) if has_att else None
+        counts = torch.empty(n, dtype=torch.int32, device=pts.device) if return_counts else None
+        rows = torch.empty(1, dtype=torch.int64, device=pts.device)
+        _pcu_internal._voxel_downsample_device(pts.dtype == torch.float64, pts.data_ptr(), n, att.data_ptr() if has_att else 0,
+                                               cols, bool(has_att and att.dtype == torch.float64), [float(v) for v in voxel_size],
+                                               [float(v) for v in min_bound], [float(v) for v in max_bound],
+                                               int(min_points_per_voxel), out_p.data_ptr(), out_a.data_ptr() if has_att else 0,
+                                               counts.data_ptr() if return_counts else 0, rows.data_ptr(), dev, stream)
+        m = int(rows.item())
+        out = (out_p[:m],) + ((out_a[:m].reshape((m,) + tuple(attrib.shape[1:])),) if has_att else ())
+        return out + ((counts[:m],) if return_counts else ())
+
+    out = _run(form, arrays, device, body)
+    if has_att:
+        return out
+    if form == "numpy":
+        return (out[0], _np.zeros([0, 0], dtype=attrib.dtype)) + out[1:]
+    return (out[0], torch.zeros((0, 0), dtype=points.dtype, device=points.device)) + out[1:]
 
 
 def downsample_point_cloud_on_voxel_grid(voxel_size, points, *args, min_bound=None, max_bound=None, min_points_per_voxel=1,
@@ -916,7 +841,7 @@ def downsample_point_cloud_on_voxel_grid(voxel_size, points, *args, min_bound=No
     empty = _np.zeros([0, 0]) if is_np else None
     ret_v, ret_a0 = _voxel_internal(points, attribs[0] if attribs else empty, voxel_size, min_bound, max_bound,
                                     min_points_per_voxel, device)
-    ret = [ret_v, ret_a0] if (attribs and ret_a0 is not None) else [ret_v]
+    ret = [ret_v, ret_a0] if attribs else [ret_v]
     for i in range(1, len(attribs)):
         _, ret_ai = _voxel_internal(points, attribs[i], voxel_size, min_bound, max_bound, min_points_per_voxel, device)
         ret.append(ret_ai)

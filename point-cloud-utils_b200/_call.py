@@ -1,9 +1,10 @@
-"""The call path of the mesh-family functions: their input forms, the argument checks they share, the upload of their
-inputs and the round trip from inputs to returned outputs.
+"""The package's call path: from a call's inputs, where it runs and in what form its results come back.
 
-numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA torch tensors in -> CUDA tensors out;
-CPU tensors -> CPU tensors (through numpy).  Arguments are validated, with the reference's messages, before any
-device call."""
+numpy arrays in -> numpy out (each input is uploaded once through torch, to the GPU `device=` names, else
+`current_device()`); CUDA torch tensors in -> CUDA tensors out, on the device they live on (a `device=` that
+contradicts it is an error); CPU tensors -> CPU tensors (through numpy).  Arguments are validated, with the reference's
+messages, before any device call.  The nearest-neighbour family reaches the device through the binding's own entry
+points but takes its device rules (`_dev`, `_same_device`, `_call_args`) from here; its numpy calls never import torch."""
 import numpy as _np
 
 from . import _pcu_internal
@@ -12,12 +13,54 @@ _INDEX_KINDS = {"int32": 0, "int64": 1, "uint32": 2, "uint64": 3}
 
 
 def _torch():
-    import importlib
-    return importlib.import_module("torch")
+    import torch
+    return torch
 
 
 def _is_tensor(x):
-    return type(x).__module__.startswith("torch")
+    """A torch tensor (the type's module is looked at first, so that numpy inputs never import torch)."""
+    return type(x).__module__.startswith("torch") and isinstance(x, _torch().Tensor)
+
+
+def _dev(device):
+    """``device=`` keyword -> ordinal for the native layer (-1: let the library choose, see current_device)."""
+    if device is None:
+        return -1
+    if isinstance(device, int):
+        d = device
+    elif isinstance(device, str):
+        name = device.strip().lower()
+        if name == "cuda":
+            return -1
+        if not name.startswith("cuda:") or not name[5:].isdigit():
+            raise ValueError("device must be an int, None, 'cuda' or 'cuda:<i>' (got %r)" % (device,))
+        d = int(name[5:])
+    elif getattr(device, "type", None) == "cuda":           # torch.device
+        d = -1 if device.index is None else int(device.index)
+    else:
+        raise ValueError("device must be an int, None, 'cuda', 'cuda:<i>' or a CUDA torch.device (got %r)" % (device,))
+    count = _pcu_internal._device_count()
+    if d >= count or d < -1:
+        raise ValueError("device %d out of range: %d usable GPU(s) visible" % (d, count))
+    return d
+
+
+def _ordinal(device):
+    """The GPU a numpy call runs on: the one ``device=`` names, else current_device()."""
+    d = _dev(device)
+    return _pcu_internal._current_device() if d < 0 else d
+
+
+def _same_device(t, device):
+    """CUDA tensors run where they live; a contradicting device= is an argument error."""
+    d = _dev(device)
+    if d >= 0 and d != (t.device.index or 0):
+        raise ValueError("device=%r contradicts the inputs, which live on %s" % (device, t.device))
+
+
+def _call_args(t):
+    """(device index, current stream) of a CUDA tensor: the last two arguments of every device entry point."""
+    return t.device.index or 0, _torch().cuda.current_stream(t.device).cuda_stream
 
 
 def _dtype_name(x):
@@ -40,6 +83,11 @@ def _form(arrays, names):
         if type(a) != _np.ndarray:
             raise ValueError("Invalid type for %s, must be a NumPy array, but got %s." % (name, type(a)))
     return "numpy"
+
+
+def _asarrays(arrays):
+    """Every input that is not a tensor as np.asarray has it (ndarray subclasses such as np.memmap become arrays)."""
+    return [a if _is_tensor(a) else _np.asarray(a) for a in arrays]
 
 
 def _check_float(x, name):
@@ -83,9 +131,8 @@ def _matrix_shape(a):
 def _to_device(arrays, device):
     """numpy arrays -> contiguous CUDA tensors on the device= of the call (one upload each).  Unsigned index arrays
     travel as the signed type of their width (the kernels take the kind separately)."""
-    from . import _dev
     torch = _torch()
-    dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
+    dev = _ordinal(device)
     signed = {"uint32": _np.int32, "uint64": _np.int64}
     return [torch.from_numpy(_np.ascontiguousarray(a).view(signed.get(a.dtype.name, a.dtype))).to(torch.device("cuda", dev))
             for a in arrays]
@@ -93,16 +140,10 @@ def _to_device(arrays, device):
 
 def _upload(form, arrays, device):
     """Contiguous CUDA tensors of the inputs, on the device of the call.  CPU tensors go through numpy."""
-    from . import _same_device
     if form == "cuda":
         _same_device(arrays[0], device)
         return [a.detach().contiguous() for a in arrays]
     return _to_device([a.detach().numpy() if _is_tensor(a) else a for a in arrays], device)
-
-
-def _call_args(t):
-    torch = _torch()
-    return t.device.index or 0, torch.cuda.current_stream(t.device).cuda_stream
 
 
 def _raise_bad(bad):

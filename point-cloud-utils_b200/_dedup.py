@@ -1,50 +1,40 @@
 """deduplicate_point_cloud / deduplicate_mesh_vertices -- the reference's names, arguments and return conventions
 (/root/reference/src/remove_duplicates.cpp:85-176), computed by csrc/dedup.cuh (keys -> radix sort -> run heads).
 
-numpy arrays in -> numpy arrays out (staged on the GPU through torch: device memory and streams only); CUDA torch
-tensors in -> CUDA tensors out.  float32 / float64 points, int32 / int64 faces."""
+Inputs and results take the forms of _call.py.  float32 / float64 points, int32 / int64 faces."""
 import numpy as _np
 
 from . import _pcu_internal
-from ._call import _is_tensor, _torch
+from ._call import _check_float, _check_index, _form, _is_tensor, _run, _same_device, _torch
 
 
-def _run(points, faces, epsilon, device, pname, fname):
+def _dedup(points, faces, epsilon, device, pname):
+    """(points, faces or None, svi, svj) of the deduplicated cloud or mesh."""
+    if not _is_tensor(points):       # lists work, as in the reference
+        points, faces = _np.asarray(points), None if faces is None else _np.asarray(faces)
+    arrays = [points] if faces is None else [points, faces]
+    form = _form(arrays, [pname, "f"])
+    _check_float(points, pname)
+    if len(points.shape) != 2 or points.shape[1] != 3:                    # validate_point_cloud, src/common/common.h:68-73
+        raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). Got points.shape =" + str(tuple(points.shape)) + ".")
+    if faces is not None:
+        _check_index(faces, "f", ("int32", "int64"))
+        if len(faces.shape) != 2:
+            raise ValueError("Invalid shape for faces, must be (m, c) but got " + str(tuple(faces.shape)))
+    n = int(points.shape[0])
     torch = _torch()
-    is_np = not _is_tensor(points)
-    if is_np:
-        points = _np.asarray(points)
-        if points.dtype not in (_np.float32, _np.float64):
-            raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of ['float32', 'float64']." % (points.dtype, pname))
-        if points.ndim != 2 or points.shape[1] != 3:                       # validate_point_cloud, src/common/common.h:68-73
-            raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). Got points.shape =" + str(points.shape) + ".")
-        if faces is not None:
-            faces = _np.asarray(faces)
-            if faces.dtype not in (_np.int32, _np.int64):
-                raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of ['int32', 'int64']." % (faces.dtype, fname))
-            if faces.ndim != 2:
-                raise ValueError("Invalid shape for faces, must be (m, c) but got " + str(faces.shape))
-        dev = torch.device("cuda", _pcu_internal._current_device() if device < 0 else device)
-        pts = torch.from_numpy(_np.ascontiguousarray(points)).to(dev)
-        fcs = torch.from_numpy(_np.ascontiguousarray(faces)).to(dev) if faces is not None else None
-    else:
-        if not points.is_cuda or points.dtype not in (torch.float32, torch.float64):
-            raise ValueError("points must be a float32 / float64 numpy array or CUDA tensor")
-        if points.dim() != 2 or points.shape[1] != 3:
-            raise ValueError("Only 3D inputs are supported: v must have shape (n, 3) (n > 0). Got points.shape =" + str(tuple(points.shape)) + ".")
-        if device >= 0 and points.device.index != device:
-            raise ValueError("device=%d was given but the tensors live on %s" % (device, points.device))
-        pts = points.detach().contiguous()
-        fcs = None
-        if faces is not None:
-            if not _is_tensor(faces) or faces.device != pts.device or faces.dtype not in (torch.int32, torch.int64) or faces.dim() != 2:
-                raise ValueError("faces must be an (m, c) int32 / int64 tensor on the device of the vertices")
-            fcs = faces.detach().contiguous()
-    n = pts.shape[0]
     if n == 0:          # the reference accepts an empty cloud and returns empty arrays
-        empty_i = torch.zeros(0, dtype=torch.int32, device=pts.device)
-        out = (pts.clone(), fcs.clone() if fcs is not None else None, empty_i, empty_i.clone())
-    else:
+        if form == "numpy":
+            empty = _np.zeros(0, dtype=_np.int32)
+            return points.copy(), None if faces is None else faces.copy(), empty, empty.copy()
+        if form == "cuda":
+            _same_device(points, device)
+        empty = torch.zeros(0, dtype=torch.int32, device=points.device)
+        return (points.detach().contiguous().clone(), None if faces is None else faces.detach().contiguous().clone(), empty,
+                empty.clone())
+
+    def body(pts, *rest):
+        fcs, (dev, stream) = (rest[0] if faces is not None else None), rest[-2:]
         nf, cols = (fcs.shape[0], fcs.shape[1]) if fcs is not None else (0, 0)
         out_p = torch.empty((n, 3), dtype=pts.dtype, device=pts.device)
         svi = torch.empty(n, dtype=torch.int32, device=pts.device)
@@ -55,14 +45,14 @@ def _run(points, faces, epsilon, device, pname, fname):
                                           fcs.data_ptr() if (fcs is not None and nf) else 0, nf, cols,
                                           bool(fcs is not None and fcs.dtype == torch.int64), out_p.data_ptr(), svi.data_ptr(),
                                           svj.data_ptr(), out_f.data_ptr() if (out_f is not None and nf) else 0, counts.data_ptr(),
-                                          pts.device.index or 0, torch.cuda.current_stream(pts.device).cuda_stream)
+                                          dev, stream)
         u, kept_f, bad = (int(v) for v in counts.tolist())
         if bad:
             raise ValueError("%d faces refer to vertices outside [0, %d)" % (bad, n))
-        out = (out_p[:u], out_f[:kept_f] if out_f is not None else None, svi[:u], svj)
-    if is_np:
-        return tuple(None if t is None else t.cpu().numpy() for t in out)
-    return out
+        return (out_p[:u], svi[:u], svj) if fcs is None else (out_p[:u], out_f[:kept_f], svi[:u], svj)
+
+    out = _run(form, arrays, device, body)
+    return (out[0], None) + out[1:] if faces is None else out
 
 
 def deduplicate_point_cloud(points, epsilon, return_index=True, *, device=None):
@@ -86,7 +76,7 @@ def deduplicate_point_cloud(points, epsilon, return_index=True, *, device=None):
     lexicographic order.  svi names the FIRST input row of each cluster (libigl's choice among equal rows is unspecified).
     `device` (keyword only): see `k_nearest_neighbors`.
     """
-    x_new, _, svi, svj = _run(points, None, epsilon, -1 if device is None else int(device), "points", "f")
+    x_new, _, svi, svj = _dedup(points, None, epsilon, device, "points")
     if return_index:
         return x_new, svi, svj
     return x_new
@@ -114,7 +104,7 @@ def deduplicate_mesh_vertices(v, f, epsilon, return_index=True, *, device=None):
     """
     if f is None:
         raise ValueError("f must be an (m, 3) array of face indices")
-    v_out, f_out, svi, svj = _run(v, f, epsilon, -1 if device is None else int(device), "v", "f")
+    v_out, f_out, svi, svj = _dedup(v, f, epsilon, device, "v")
     if return_index:
         return v_out, f_out, svi, svj
     return v_out, f_out

@@ -7,7 +7,8 @@ restricted cells, centroid rows, the initial samples, the Lloyd step and the L-B
 import numpy as _np
 
 from . import _pcu_internal
-from ._call import _INDEX_KINDS, _dtype_name, _form, _is_tensor, _run, _torch, _validate_mesh
+from ._call import (_INDEX_KINDS, _call_args, _dtype_name, _form, _ordinal, _run, _same_device, _to_device, _torch,
+                    _validate_mesh)
 
 # Cells (for restricted cells: (face, seed) pairs) handled by each pass (first pass, longer neighbour lists, all seeds)
 # in the last call of this module's functions, in any thread (a plain module global, for tests and tools): the fallback
@@ -16,11 +17,6 @@ last_pass_counts = (0, 0, 0)
 # The CVT energy of the starting point and of every accepted Newton step of the last lloyd_3d / lloyd_2d /
 # sample_mesh_lloyd call.
 last_newton_energies = []
-
-
-def _device_args(t):
-    torch = _torch()
-    return t.device.index or 0, torch.cuda.current_stream(t.device).cuda_stream
 
 
 def voronoi_centroids_unit_cube(centers, *, device=None):
@@ -40,12 +36,7 @@ def voronoi_centroids_unit_cube(centers, *, device=None):
     above 1e-30.  Seeds at one position share one cell, which the lowest index owns; every other row (an empty cell)
     is the seed itself -- the reference leaves such rows uninitialised.
     """
-    global last_pass_counts
-    from . import _dev, _same_device
-    torch = _torch()
-    tensor = _is_tensor(centers)
-    if not tensor and type(centers) != _np.ndarray:
-        raise ValueError("Invalid type for centers, must be a NumPy array, but got " + str(type(centers)) + ".")
+    form = _form([centers], ["centers"])
     if _dtype_name(centers) not in ("float32", "float64"):
         raise ValueError("Invalid scalar type (%s) for argument 'centers'. Expected one of ['float32', 'float64']."
                          % _dtype_name(centers))
@@ -53,27 +44,28 @@ def voronoi_centroids_unit_cube(centers, *, device=None):
     if len(shape) != 2 or shape[1] != 3:
         raise ValueError("Invalid shape for centers, must be (n, 3) but got " + str(shape))
     n = shape[0]
-    if tensor and not centers.is_cuda:
-        return torch.from_numpy(voronoi_centroids_unit_cube(centers.detach().numpy(), device=device))
-    if tensor:
-        _same_device(centers, device)
-        x = centers.detach().to(torch.float64).contiguous()
-        if n == 0:
-            return x.clone()
-        bad = bool(((x < 0) | (x > 1) | torch.isnan(x)).any().item())
-    else:
-        if n == 0:
+    torch = _torch()
+    if n == 0:
+        if form == "numpy":
             return _np.zeros((0, 3), dtype=_np.float64)
-        host = _np.ascontiguousarray(centers, dtype=_np.float64)      # float32 widens exactly
-        bad = bool(((host < 0) | (host > 1) | _np.isnan(host)).any())
-    if bad:
-        raise ValueError("Centers of voronoi diagram must lie in the unit cube [0, 1]^3")
-    if not tensor:
-        dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
-        x = torch.from_numpy(host).to(torch.device("cuda", dev))
-    out = torch.empty_like(x)
-    last_pass_counts = tuple(_pcu_internal._voronoi_centroids_device(x.data_ptr(), n, 3, out.data_ptr(), 0, *_device_args(x)))
-    return out if tensor else out.cpu().numpy()
+        if form == "cuda":
+            _same_device(centers, device)
+        return torch.zeros((0, 3), dtype=torch.float64, device=centers.device)
+    if form != "cuda":
+        host = centers if form == "numpy" else centers.detach().numpy()
+        if ((host < 0) | (host > 1) | _np.isnan(host)).any():
+            raise ValueError("Centers of voronoi diagram must lie in the unit cube [0, 1]^3")
+
+    def body(x, dev, stream):
+        global last_pass_counts
+        x = x.to(torch.float64).contiguous()                            # float32 widens exactly
+        if form == "cuda" and bool(((x < 0) | (x > 1) | torch.isnan(x)).any().item()):
+            raise ValueError("Centers of voronoi diagram must lie in the unit cube [0, 1]^3")
+        out = torch.empty_like(x)
+        last_pass_counts = tuple(_pcu_internal._voronoi_centroids_device(x.data_ptr(), n, 3, out.data_ptr(), 0, dev, stream))
+        return out
+
+    return _run(form, [centers], device, body)
 
 
 def _cell_moments(centers, *, device=None):
@@ -81,31 +73,27 @@ def _cell_moments(centers, *, device=None):
     as numpy arrays; moments (n, 5): volume, first moment about the seed (x, y, z; z = 0 in 2-D) and second moment
     about the seed of every cell.  Not part of the public interface: the cells the relaxations see, for tests."""
     global last_pass_counts
-    from . import _dev
     torch = _torch()
     host = _np.ascontiguousarray(centers, dtype=_np.float64)
     n, dim = host.shape
-    dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
-    x = torch.from_numpy(host).to(torch.device("cuda", dev))
+    x, = _to_device([host], device)
     out = torch.empty_like(x)
     mom = torch.empty((n, 5), dtype=torch.float64, device=x.device)
     last_pass_counts = tuple(_pcu_internal._voronoi_centroids_device(x.data_ptr(), n, dim, out.data_ptr(), mom.data_ptr(),
-                                                                     *_device_args(x)))
+                                                                     *_call_args(x)))
     return out.cpu().numpy(), mom.cpu().numpy()
 
 
 def _lloyd(n, num_lloyd, num_newton, dim, device):
     global last_pass_counts, last_newton_energies
-    from . import _dev
     n = int(n)
     if n <= 0:
         raise ValueError("n must be a positive integer. Got n = %d" % n)
     seed = int(_np.random.randint(2 ** 31 - 1))
     torch = _torch()
-    dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
-    out = torch.empty((n, dim), dtype=torch.float64, device=torch.device("cuda", dev))
+    out = torch.empty((n, dim), dtype=torch.float64, device=torch.device("cuda", _ordinal(device)))
     energies, passes = _pcu_internal._lloyd_device(n, dim, seed, int(num_lloyd), int(num_newton), out.data_ptr(),
-                                                   *_device_args(out))
+                                                   *_call_args(out))
     last_pass_counts = tuple(passes)
     last_newton_energies = list(energies)
     return out.cpu().numpy()

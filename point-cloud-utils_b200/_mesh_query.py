@@ -5,7 +5,7 @@ src/fast_winding_numbers.cpp and src/signed_distance.cpp), computed by csrc/mesh
 Input forms and validation follow _call.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
 from . import _pcu_internal
-from ._call import _INDEX_KINDS, _check_float, _check_index, _check_match, _dtype_name, _form, _raise_bad, _run, _torch, _validate_mesh
+from ._call import _INDEX_KINDS, _check_float, _check_index, _check_match, _dtype_name, _form, _raise_bad, _run, _same_device, _torch, _validate_mesh
 
 
 def _validate_points(p, v, f):
@@ -44,7 +44,6 @@ def closest_points_on_mesh(p, v, f, *, device=None):
     Divergences: libigl's choice among tied faces depends on its tree and is not reproduced; a face corner outside
     [0, #v) raises ValueError (the reference reads out of bounds).
     """
-    from . import _same_device
     form = _form([p, v, f], ["p", "v", "f"])
     _validate_points(p, v, f)
     _validate_mesh(v, f, ("int32", "int64", "uint32", "uint64"))

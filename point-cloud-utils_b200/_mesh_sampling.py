@@ -9,7 +9,7 @@ import math
 import numpy as _np
 
 from . import _pcu_internal
-from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _raise_bad, _run, _torch, _validate_mesh
+from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _raise_bad, _run, _same_device, _torch, _validate_mesh
 
 
 def _seed(random_seed):
@@ -194,7 +194,6 @@ def interpolate_barycentric_coords(f, fi, bc, attribute, *, device=None):
         if form == "numpy":
             return _np.zeros((n, dim), dtype=_np.float64 if out_f64 else _np.float32)
         if form == "cuda":
-            from . import _same_device
             _same_device(f, device)
         return torch.zeros((n, dim), dtype=torch.float64 if out_f64 else torch.float32, device=f.device)
 

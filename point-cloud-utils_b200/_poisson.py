@@ -1,12 +1,12 @@
 """downsample_point_cloud_poisson_disk -- the reference's name, arguments and defaults
 (/root/reference/src/sample_point_cloud.cpp:240-333), computed by csrc/poisson.cuh.
 
-numpy arrays in -> numpy int32 out (the cloud is uploaded once through torch, whatever the number of radii the
-target-count search tries); CUDA torch tensors in -> CUDA int32 tensors out; CPU tensors -> CPU tensors."""
+Inputs and results take the forms of _call.py; the cloud is uploaded once, whatever the number of radii the
+target-count search tries."""
 import numpy as _np
 
 from . import _pcu_internal
-from ._call import _is_tensor, _torch
+from ._call import _dtype_name, _form, _run, _same_device, _torch
 
 
 def target_search(sample, dtype, bbsize, target, tolerance):
@@ -88,66 +88,44 @@ def downsample_point_cloud_poisson_disk(v, radius, target_num_samples=-1, random
     and target_num_samples < len(v), the reference's search never ends (its radius stays 0), while here the one sample
     any positive radius gives -- the row of smallest priority -- is returned.
     """
-    from . import _dev, _same_device
     target = int(target_num_samples)
     if target <= 0 and radius <= 0.0:                                       # :265-267
         raise ValueError("Cannot have both num_samples <= 0 and radius <= 0")
     if float(_np.float32(sample_num_tolerance)) > 1.0 or float(_np.float32(sample_num_tolerance)) <= 0.0:   # :268-270
         raise ValueError("sample_num_tolerance must be in (0, 1]")
-    torch = _torch()
-    if _is_tensor(v):
-        if v.dtype not in (torch.float32, torch.float64):
-            raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected one of ['float32', 'float64']." % v.dtype)
-        if v.dim() != 2 or v.shape[1] != 3:
-            raise ValueError("Invalid shape for v, must be (n, 3) but got " + str(tuple(v.shape)))
-        if not v.is_cuda:
-            return torch.from_numpy(downsample_point_cloud_poisson_disk(v.detach().numpy(), radius, target, random_seed,
-                                                                        sample_num_tolerance, device=device))
-        _same_device(v, device)
-        pts = v.detach().contiguous()
-        dtype = _np.float64 if pts.dtype == torch.float64 else _np.float32
-        host = None
-    else:
-        if type(v) != _np.ndarray:
-            raise ValueError("Invalid type for v, must be a NumPy array, but got " + str(type(v)) + ".")
-        if v.dtype not in (_np.float32, _np.float64):
-            raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected one of ['float32', 'float64']." % v.dtype)
-        if v.ndim != 2 or v.shape[1] != 3:
-            raise ValueError("Invalid shape for v, must be (n, 3) but got " + str(v.shape))
-        dtype = v.dtype.type
-        host = _np.ascontiguousarray(v)
-        pts = None
+    form = _form([v], ["v"])
+    if _dtype_name(v) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s) for argument 'v'. Expected one of ['float32', 'float64']." % v.dtype)
+    if len(v.shape) != 2 or v.shape[1] != 3:
+        raise ValueError("Invalid shape for v, must be (n, 3) but got " + str(tuple(v.shape)))
     n = int(v.shape[0])
-    if n == 0:
-        return _np.zeros(0, dtype=_np.int32) if host is not None else torch.zeros(0, dtype=torch.int32, device=pts.device)
-    if target > 0 and target >= n:                                           # :279-283
-        return _np.arange(n, dtype=_np.int32) if host is not None else torch.arange(n, dtype=torch.int32, device=pts.device)
+    if n == 0 or 0 < n <= target:                                            # :279-283
+        if form == "numpy":
+            return _np.arange(n, dtype=_np.int32)
+        if form == "cuda":
+            _same_device(v, device)
+        torch = _torch()
+        return torch.arange(n, dtype=torch.int32, device=v.device)
     seed = int(random_seed) & 0xFFFFFFFF
     if seed == 0:
         seed = int(_np.random.randint(2 ** 31 - 1))
-    T = _np.dtype(dtype).type
-    if host is not None:
-        if target > 0:
-            lo, hi = host.min(axis=0), host.max(axis=0)
-        dev = _pcu_internal._current_device() if _dev(device) < 0 else _dev(device)
-        pts = torch.from_numpy(host).to(torch.device("cuda", dev))
-    elif target > 0:
-        box = torch.stack((pts.amin(dim=0), pts.amax(dim=0))).cpu().numpy()
-        lo, hi = box[0], box[1]
-    idx = torch.empty(n, dtype=torch.int32, device=pts.device)
-    count = torch.empty(1, dtype=torch.int64, device=pts.device)
-    stream = torch.cuda.current_stream(pts.device).cuda_stream
+    T = _np.float64 if _dtype_name(v) == "float64" else _np.float32
+    torch = _torch()
 
-    def sample(r):
-        _pcu_internal._poisson_disk_device(pts.dtype == torch.float64, pts.data_ptr(), n, float(r), seed, idx.data_ptr(),
-                                           count.data_ptr(), 0, pts.device.index or 0, stream)
-        return int(count.item())
+    def body(pts, dev, stream):
+        idx = torch.empty(n, dtype=torch.int32, device=pts.device)
+        count = torch.empty(1, dtype=torch.int64, device=pts.device)
 
-    if target <= 0:
-        m = sample(radius)         # narrowed to T by the library
-    elif _box_size(lo, hi, T) == 0:
-        m = sample(T(1))           # every row conflicts with every other: one sample
-    else:
-        m = target_search(sample, dtype, _box_size(lo, hi, T), target, sample_num_tolerance)
-    out = idx[:m]
-    return out.cpu().numpy() if host is not None else out
+        def sample(r):
+            _pcu_internal._poisson_disk_device(pts.dtype == torch.float64, pts.data_ptr(), n, float(r), seed, idx.data_ptr(),
+                                               count.data_ptr(), 0, dev, stream)
+            return int(count.item())
+
+        if target <= 0:
+            return idx[:sample(radius)]         # radius narrowed to T by the library
+        lo, hi = torch.stack((pts.amin(dim=0), pts.amax(dim=0))).cpu().numpy()
+        if _box_size(lo, hi, T) == 0:
+            return idx[:sample(T(1))]           # every row conflicts with every other: one sample
+        return idx[:target_search(sample, T, _box_size(lo, hi, T), target, sample_num_tolerance)]
+
+    return _run(form, [v], device, body)

@@ -8,7 +8,7 @@ import numpy as np
 
 from . import _pcu_internal
 from ._call import (_INDEX_KINDS, _call_args, _check_float, _check_index, _check_match, _dtype_name, _form, _matrix_shape,
-                    _raise_bad, _run, _torch, _upload, _validate_mesh)
+                    _raise_bad, _run, _same_device, _torch, _upload, _validate_mesh)
 
 
 def _validate_rays(ray_o, ray_d):
@@ -47,7 +47,6 @@ def _cast(form, scene, ray_o, ray_d, single, n, device, outs, call):
         if form == "numpy":
             return tuple(np.zeros((0,) + tail, dtype=name) for tail, name in outs)
         if form == "cuda":
-            from . import _same_device
             _same_device(ray_d, device)
         return tuple(torch.zeros((0,) + tail, dtype=getattr(torch, name), device=ray_d.device) for tail, name in outs)
 

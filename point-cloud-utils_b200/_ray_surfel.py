@@ -7,7 +7,7 @@ out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's 
 import numpy as np
 
 from . import _pcu_internal
-from ._call import _call_args, _check_float, _check_match, _dtype_name, _form, _is_tensor, _matrix_shape, _run, _torch, _upload
+from ._call import _call_args, _check_float, _check_match, _dtype_name, _form, _is_tensor, _matrix_shape, _run, _same_device, _torch, _upload
 from ._ray_mesh import _Prepared, _bounds, _cast, _validate_rays
 
 _MAX_SUBDIVS = 2 ** 24
@@ -215,7 +215,6 @@ def pointcloud_surfel_geometry(p, n, r=0.1, subdivs=7, *, device=None):
         if form == "numpy":
             return np.zeros((0, 3), dtype=p.dtype), np.zeros((0, 3), dtype=np.int32)
         if form == "cuda":
-            from . import _same_device
             _same_device(p, device)
         return torch.zeros((0, 3), dtype=p.dtype, device=p.device), torch.zeros((0, 3), dtype=torch.int32, device=p.device)
     if m * (subdivs + 1) >= 2 ** 31 - 1:

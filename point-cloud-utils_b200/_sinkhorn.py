@@ -1,14 +1,14 @@
 """pairwise_distances / sinkhorn / earth_movers_distance -- the reference's names, arguments, shape rules and return
 conventions (/root/reference/point_cloud_utils/_sinkhorn.py:4-156), computed by the kernels of csrc/sinkhorn.cuh.
 
-numpy arrays in -> numpy arrays out (the arrays are staged on the GPU through torch, which is plumbing here: device
-memory and streams); CUDA torch tensors in -> CUDA tensors out, nothing synchronises.  float32 / float64."""
+Inputs and results take the forms of _call.py; CUDA tensors in -> CUDA tensors out, nothing synchronises.  float32 /
+float64."""
 import math
 
 import numpy as _np
 
 from . import _pcu_internal
-from ._call import _torch
+from ._call import _asarrays, _dtype_name, _form, _run, _torch
 
 _NORM2, _NORM1, _NORMINF, _NORMNEGINF, _NORM0, _NORMP = range(6)
 
@@ -29,32 +29,13 @@ def _norm_kind(p):
     return _NORMP, float(p)
 
 
-class _Staged:
-    """Inputs as contiguous CUDA tensors of one dtype on one device; remembers how to hand results back."""
-
-    def __init__(self, arrays, device):
-        torch = _torch()
-        self.numpy = not any(type(x).__module__.startswith("torch") for x in arrays)
-        if self.numpy:
-            arrs = [_np.asarray(x) for x in arrays]
-            dt = arrs[0].dtype
-            if dt not in (_np.float32, _np.float64):
-                raise ValueError("Invalid scalar type (%s). Expected one of ['float32', 'float64']." % dt)
-            dev = torch.device("cuda", _pcu_internal._current_device() if device < 0 else device)
-            self.tensors = [torch.from_numpy(_np.ascontiguousarray(x)).to(dev) for x in arrs]
-        else:
-            if not all(isinstance(x, torch.Tensor) and x.is_cuda for x in arrays):
-                raise ValueError("inputs must all be numpy arrays or all be CUDA tensors")
-            if arrays[0].dtype not in (torch.float32, torch.float64):
-                raise ValueError("Invalid scalar type (%s). Expected one of ['float32', 'float64']." % arrays[0].dtype)
-            self.tensors = [x.detach().contiguous() for x in arrays]
-        self.device = self.tensors[0].device
-        self.dtype = self.tensors[0].dtype
-        self.f64 = self.dtype == torch.float64
-        self.stream = torch.cuda.current_stream(self.device).cuda_stream
-
-    def out(self, t):
-        return t.cpu().numpy() if self.numpy else t
+def _float_inputs(arrays, names):
+    """The form of the inputs (numpy arrays, ndarray subclasses included, or tensors) after the check of their dtype."""
+    arrays = _asarrays(arrays)
+    form = _form(arrays, names)
+    if _dtype_name(arrays[0]) not in ("float32", "float64"):
+        raise ValueError("Invalid scalar type (%s). Expected one of ['float32', 'float64']." % arrays[0].dtype)
+    return form, arrays
 
 
 def pairwise_distances(a, b, p=None, *, device=None):
@@ -72,7 +53,6 @@ def pairwise_distances(a, b, p=None, *, device=None):
 
     Mirrors /root/reference/point_cloud_utils/_sinkhorn.py:4-34.
     """
-    from . import _dev
     kind, pv = _norm_kind(p)
     squeezed = False
     if len(a.shape) == 2 and len(b.shape) == 2:
@@ -84,20 +64,21 @@ def pairwise_distances(a, b, p=None, *, device=None):
         raise ValueError("Invalid shape for a. Must be [m, n, d] or [n, d] but got", b.shape)
     if a.shape[0] != b.shape[0] or a.shape[2] != b.shape[2]:
         raise ValueError("operands could not be broadcast together with shapes %s %s" % (tuple(a.shape), tuple(b.shape)))
-    st = _Staged([a, b], _dev(device))
-    ta, tb = st.tensors
-    if tb.dtype != ta.dtype:
+    form, (a, b) = _float_inputs([a, b], ["a", "b"])
+    if b.dtype != a.dtype:
         raise ValueError("a and b must have the same dtype")
     torch = _torch()
-    nb, n, d = ta.shape
-    m = tb.shape[1]
-    out = torch.empty((nb, n, m), dtype=st.dtype, device=st.device)
-    if out.numel():
-        _pcu_internal._pairwise_device(st.f64, ta.data_ptr(), tb.data_ptr(), nb, n, m, d, kind, pv, out.data_ptr(),
-                                       st.device.index or 0, st.stream)
-    if squeezed:
-        out = out.squeeze()          # np.squeeze: every size-1 dimension goes (:31-32)
-    return st.out(out)
+
+    def body(ta, tb, dev, stream):
+        nb, n, d = ta.shape
+        m = tb.shape[1]
+        out = torch.empty((nb, n, m), dtype=ta.dtype, device=ta.device)
+        if out.numel():
+            _pcu_internal._pairwise_device(ta.dtype == torch.float64, ta.data_ptr(), tb.data_ptr(), nb, n, m, d, kind, pv,
+                                           out.data_ptr(), dev, stream)
+        return out
+
+    return _run(form, [a, b], device, body, squeeze=squeezed)     # np.squeeze: every size-1 dimension goes (:31-32)
 
 
 def _squeeze(x):
@@ -122,7 +103,6 @@ def sinkhorn(a, b, M, eps, max_iters=100, stop_thresh=1e-3, *, device=None, _wan
 
     Mirrors /root/reference/point_cloud_utils/_sinkhorn.py:37-126 (shape rules :55-99, iteration :104-118, plan :120-122).
     """
-    from . import _dev
     M, a, b = _squeeze(M), _squeeze(a), _squeeze(b)
     squeezed = False
     if len(M.shape) == 2 and len(a.shape) == 1 and len(b.shape) == 1:
@@ -151,19 +131,20 @@ def sinkhorn(a, b, M, eps, max_iters=100, stop_thresh=1e-3, *, device=None, _wan
         raise ValueError("Got unexpected shape for tensor a (%s). Expected [nb, m] where M has shape [nb, m, n]." % str(tuple(a.shape)))
     if tuple(b.shape) != (nb, n):
         raise ValueError("Got unexpected shape for tensor b (%s). Expected [nb, n] where M has shape [nb, m, n]." % str(tuple(b.shape)))
-    st = _Staged([a, b, M], _dev(device))
-    ta, tb, tM = st.tensors
+    form, (a, b, M) = _float_inputs([a, b, M], ["a", "b", "M"])
     torch = _torch()
-    P = torch.empty((nb, m, n), dtype=st.dtype, device=st.device)
-    cost = torch.empty(nb, dtype=torch.float64, device=st.device) if _want_cost else None
-    _pcu_internal._sinkhorn_device(st.f64, ta.data_ptr(), tb.data_ptr(), tM.data_ptr(), nb, m, n, float(eps), int(max_iters),
-                                   float(stop_thresh), P.data_ptr(), cost.data_ptr() if _want_cost else 0, 0,
-                                   st.device.index or 0, st.stream)
-    if squeezed:
-        P = P.squeeze()
-    if _want_cost:
-        return st.out(P), cost, st
-    return st.out(P)
+
+    def body(ta, tb, tM, dev, stream):
+        P = torch.empty((nb, m, n), dtype=tM.dtype, device=tM.device)
+        cost = torch.empty(nb, dtype=torch.float64, device=tM.device) if _want_cost else None
+        _pcu_internal._sinkhorn_device(tM.dtype == torch.float64, ta.data_ptr(), tb.data_ptr(), tM.data_ptr(), nb, m, n,
+                                       float(eps), int(max_iters), float(stop_thresh), P.data_ptr(),
+                                       cost.data_ptr() if _want_cost else 0, 0, dev, stream)
+        if squeezed:
+            P = P.squeeze()
+        return (P, cost) if _want_cost else P
+
+    return _run(form, [a, b, M], device, body)
 
 
 def earth_movers_distance(p, q, p_norm=2, eps=1e-4, max_iters=100, stop_thresh=1e-3, *, device=None):
@@ -191,15 +172,15 @@ def earth_movers_distance(p, q, p_norm=2, eps=1e-4, max_iters=100, stop_thresh=1
         raise ValueError("Tensors a, b, and M must have the same dtype got: dtype(a) = float64, dtype(b) = float64, dtype(M) = %s"
                          % str(p.dtype))
     M = pairwise_distances(p, q, p_norm, device=device)
-    if isinstance(M, _np.ndarray):
+    form = _form(_asarrays([p, q]), ["p", "q"])
+    if form == "numpy":
         a = _np.ones(p.shape[0]) / p.shape[0]
         b = _np.ones(q.shape[0]) / q.shape[0]
     else:
         torch = _torch()
         a = torch.ones(p.shape[0], dtype=torch.float64, device=M.device) / p.shape[0]
         b = torch.ones(q.shape[0], dtype=torch.float64, device=M.device) / q.shape[0]
-    P, cost, st = sinkhorn(a, b, M, eps, max_iters, stop_thresh, device=device, _want_cost=True)
-    total = cost.sum()
-    if st.numpy:
-        return M.dtype.type(total.item()), P
-    return total.to(M.dtype), P
+    P, cost = sinkhorn(a, b, M, eps, max_iters, stop_thresh, device=device, _want_cost=True)
+    if form == "numpy":
+        return M.dtype.type(cost.sum()), P
+    return cost.sum().to(M.dtype), P

@@ -8,7 +8,7 @@ CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messa
 import numpy as np
 
 from . import _pcu_internal
-from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _is_tensor, _matrix_shape, _run, _torch
+from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _matrix_shape, _run, _torch
 
 _MAX_ROWS = 2 ** 31 - 1
 _MAX_DILATE = (2 ** 31 - 2) // 26         # dilation ranks 26 neighbour flags per voxel in 32 bits
@@ -358,7 +358,8 @@ def erode_sparse_voxel_grid(grid_coordinates, count=1, *, device=None):
 
 def _numpy_dtype(dtype):
     """A numpy dtype, or the numpy dtype of a torch dtype."""
-    return _torch().empty(0, dtype=dtype).numpy().dtype if _is_tensor(dtype) else np.dtype(dtype)
+    torch = _torch()
+    return torch.empty(0, dtype=dtype).numpy().dtype if isinstance(dtype, torch.dtype) else np.dtype(dtype)
 
 
 def sparse_voxel_grid_to_hex_mesh(grid_coordinates, voxel_size=1.0, origin=(0.0, 0.0, 0.0), dtype=np.float64, *, device=None):
