@@ -656,6 +656,27 @@ int pcu_b200_voxelize_destroy(pcu_b200_voxelize* vx);
 int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t seed_x,
                            int64_t seed_y, int64_t seed_z, double fill_value, void* out, void* stream);
 
+/* ---- watertight manifold remeshing ---------------------------------------------------------------------------------
+ * Replaces make_mesh_watertight (the reference's src/manifold.cpp).  Result defined in DESIGN.md §3: the outer
+ * surface of the mesh's voxel occupancy on a cubic grid of 2^d voxels per side (d in [3, 10], the smallest whose
+ * occupied count reaches `resolution`), extracted by marching cubes and projected onto the input in 10 rounds.
+ *   make_mesh_watertight_prepare: v (nv, 3) in the suffix's type, f (nf, 3) of kind f_kind, 1 <= nv, nf < 2^31 - 1.
+ *     Synchronises `stream` once for v's bounds, once or twice per depth tried, once for the surface's counts and once
+ *     per flip pass of each projection round.  *out_counts = {#vw, #fw, d} (host int64).  A non-finite vertex, a
+ *     corner outside [0, nv), a mesh whose vertices all coincide, or more output vertices than f_kind can index fail
+ *     with PCU_B200_INVALID_ARGUMENT.  Dense scratch of 5 bytes per voxel (5 GiB at d = 10) lives for the call only.
+ *     *out_wt (v and f need not outlive prepare) is freed by make_mesh_watertight_destroy, stream-ordered on the
+ *     stream it was prepared on.
+ *   make_mesh_watertight_emit: writes out_v (#vw, 3) in the suffix's type and out_f (#fw, 3) in f's width.
+ * Every array pointer is a DEVICE pointer. */
+typedef struct pcu_b200_watertight pcu_b200_watertight;
+int pcu_b200_make_mesh_watertight_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                              double resolution, pcu_b200_watertight** out_wt, int64_t out_counts[3], void* stream);
+int pcu_b200_make_mesh_watertight_prepare_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                              double resolution, pcu_b200_watertight** out_wt, int64_t out_counts[3], void* stream);
+int pcu_b200_make_mesh_watertight_emit(pcu_b200_workspace* ws, const pcu_b200_watertight* wt, void* out_v, void* out_f, void* stream);
+int pcu_b200_make_mesh_watertight_destroy(pcu_b200_watertight* wt);
+
 /* ---- mesh topology: connected components and vertex removal ----------------------------------------------------------
  * Replace connected_components, remove_mesh_vertices and remove_unreferenced_mesh_vertices (the reference's
  * src/connected_components.cpp, src/remove_mesh_vertices.cpp, src/remove_unreferenced_mesh_vertices.cpp).  Results

@@ -693,6 +693,21 @@ py::tuple voxelize_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_
     return py::make_tuple((uintptr_t)vx, counts[0], counts[1]);
 }
 
+// Watertight remeshing (make_mesh_watertight, _watertight.py): the whole remeshing (synchronises `stream` per phase and
+// per flip pass), returns (handle, #v, #f, depth); _make_mesh_watertight_emit writes v and f; _make_mesh_watertight_destroy.
+py::tuple make_mesh_watertight_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, double resolution,
+                                              int device, uintptr_t stream) {
+    pcu_b200_watertight* wt = nullptr;
+    int64_t counts[3] = {0, 0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_make_mesh_watertight_prepare_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, resolution, &wt,
+                                                                  counts, (void*)stream)
+                      : pcu_b200_make_mesh_watertight_prepare_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, resolution, &wt,
+                                                                  counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)wt, counts[0], counts[1], counts[2]);
+}
+
 // Connected components (connected_components, _mesh_topology.py): validates f and labels (two synchronisations of
 // `stream`), returns (handle, n = max(f) + 1, components); _connected_components_emit writes cv, nv, cf and nf in f's
 // width; _connected_components_destroy.
@@ -1098,6 +1113,9 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_voxelize_prepare_device", &voxelize_prepare_device);
     mod.def("_voxelize_emit_device", forward_to(pcu_b200_voxelize_emit).single());
     mod.def("_voxelize_destroy", destroy(pcu_b200_voxelize_destroy));
+    mod.def("_make_mesh_watertight_prepare_device", &make_mesh_watertight_prepare_device);
+    mod.def("_make_mesh_watertight_emit_device", forward_to(pcu_b200_make_mesh_watertight_emit).single());
+    mod.def("_make_mesh_watertight_destroy", destroy(pcu_b200_make_mesh_watertight_destroy));
     mod.def("_flood_fill_3d_device", forward_to(pcu_b200_flood_fill_3d).single());
     mod.def("_connected_components_prepare_device", &connected_components_prepare_device);
     mod.def("_connected_components_emit_device", forward_to(pcu_b200_connected_components_emit).single());

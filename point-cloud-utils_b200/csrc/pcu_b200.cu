@@ -39,6 +39,7 @@
 #include "raycast.cuh"
 #include "sparse_voxels.cuh"
 #include "voxelize.cuh"
+#include "watertight.cuh"
 #include "mesh_topology.cuh"
 #include "orient.cuh"
 #include "laplacian.cuh"
@@ -313,6 +314,16 @@ struct pcu_b200_voxelize : StreamHandle {
     unsigned char* head = nullptr;
     unsigned* offsets = nullptr;
     ~pcu_b200_voxelize() { release(block); }
+};
+// Watertight remeshing between pcu_b200_make_mesh_watertight_prepare_* and _emit: the result in one block, vertices in
+// fp64 and faces in int32, which emit converts to the input's types.
+struct pcu_b200_watertight : StreamHandle {
+    int t_f64 = 0, fkind = 0, depth = 0;
+    long long nv = 0, nf = 0;
+    unsigned char* block = nullptr;
+    const double* x = nullptr;
+    const int* faces = nullptr;
+    ~pcu_b200_watertight() { release(block); }
 };
 // Connected components between pcu_b200_connected_components_prepare and _emit: int32 labels and counts in one block
 // (cv over n = max(f) + 1 vertices, cf over m faces, nv and nf over the k components, sized n).
@@ -2624,7 +2635,7 @@ int vx_build(pcu_b200_workspace* ws, pcu_b200_voxelize* h, const T* v, long long
     PCU_CUDA(cudaMemsetAsync(sc.counts, 0, sizeof(VxCounts), stream));
     PCU_LAUNCH((vx_bounds_kernel<T>), (unsigned)tiles, kThreads, stream, v, nv, f, fkind, m, g, sc.faces, sc.local, sc.tile, sc.counts);
     PCU_LAUNCH(vx_tiles_kernel, 1, 1024, stream, sc.tile, tiles, sc.counts);
-    PCU_LAUNCH((vx_test_kernel<T, false>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
+    PCU_LAUNCH((vx_test_kernel<T, kVxCount>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
                (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, (McRec*)nullptr);
     VxCounts c;
     PCU_TRY(read_record(sc.counts, &c, stream));
@@ -2648,7 +2659,7 @@ int vx_build(pcu_b200_workspace* ws, pcu_b200_voxelize* h, const T* v, long long
     };
     PCU_TRY(alloc_block(h->block, carve_at(nullptr, carve), stream, "voxelization"));
     carve_at(h->block, carve);
-    PCU_LAUNCH((vx_test_kernel<T, true>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
+    PCU_LAUNCH((vx_test_kernel<T, kVxCodes>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
                (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, hb.sort.a);
     McRec* sorted = nullptr;
     PCU_TRY(radix_sort_records(hb.sort, na, 1, stream, &sorted));
@@ -2746,6 +2757,230 @@ int flood_fill_3d_device(pcu_b200_workspace* ws, const void* grid, int kind, lon
         case PCU_B200_GRID_F64: return ff_device<double>(ws, (const double*)grid, w, h, d, seed, fill, (double*)out, stream);
         default: return fail(PCU_B200_INVALID_ARGUMENT, "unknown grid kind %d", kind);
     }
+}
+
+// ---- watertight manifold remeshing (watertight.cuh) ---------------------------------------------------------------
+// A block of device memory that lives for one call, freed in the order of its stream.
+struct CallBlock {
+    unsigned char* p = nullptr;
+    cudaStream_t stream = nullptr;
+    explicit CallBlock(cudaStream_t s) : stream(s) {}
+    ~CallBlock() { reset(); }
+    void reset() { if (p) cudaFreeAsync(p, stream); p = nullptr; }
+};
+
+// The grid of DESIGN.md §3: c = (lo + hi) / 2, L = 1.4 max_a (hi_a - lo_a), o = c - L / 2, every operation rounded.
+struct WtFrame { double o[3], L; };
+
+// Bounds of v (first synchronisation), then per depth the counting pass (one synchronisation) and, where its pair
+// count reaches the resolution, the grid pass (one more): the depth, the occupancy bytes of its grid in *grid.
+template <typename T>
+int wt_depth_search(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, double resolution,
+                    CallBlock& grid, WtFrame& fr, int& depth, cudaStream_t stream) {
+    const long long tiles = (m + kThreads - 1) / kThreads;
+    struct { VxFace* faces; unsigned long long* local; unsigned long long* tile; VxCounts* counts; WtBounds* bounds; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.faces = cv.take<VxFace>((size_t)m);
+        sc.local = cv.take<unsigned long long>((size_t)m);
+        sc.tile = cv.take<unsigned long long>((size_t)tiles);
+        sc.counts = cv.take<VxCounts>(1);
+        sc.bounds = cv.take<WtBounds>(1);
+    }));
+    WtBounds b;
+    for (int k = 0; k < 3; ++k) { b.lo[k] = LLONG_MAX; b.hi[k] = LLONG_MIN; }
+    b.bad = 0;
+    PCU_CUDA(cudaMemcpyAsync(sc.bounds, &b, sizeof b, cudaMemcpyHostToDevice, stream));
+    PCU_LAUNCH((wt_bounds_kernel<T>), (unsigned)std::min<long long>(blocks_for(nv), (long long)ws->sm_count * 8), kThreads, stream, v, nv,
+               sc.bounds);
+    PCU_TRY(read_record(sc.bounds, &b, stream));
+    if (b.bad) return fail(PCU_B200_INVALID_ARGUMENT, "make_mesh_watertight: v has %llu non-finite coordinates", b.bad);
+    double ext = 0.0, c[3];
+    for (int k = 0; k < 3; ++k) {
+        const auto unord = [](long long x) { x = x >= 0 ? x : x ^ 0x7fffffffffffffffll; double d; std::memcpy(&d, &x, 8); return d; };
+        const double lo = unord(b.lo[k]), hi = unord(b.hi[k]);
+        const volatile double sum = lo + hi, width = hi - lo;
+        c[k] = sum / 2.0;
+        ext = std::max(ext, (double)width);
+    }
+    if (!(ext > 0.0)) return fail(PCU_B200_INVALID_ARGUMENT, "make_mesh_watertight: the mesh has zero extent (every vertex is the same point)");
+    const volatile double L = 1.4 * ext;
+    fr.L = L;
+    if (!std::isfinite(fr.L)) return fail(PCU_B200_INVALID_ARGUMENT, "make_mesh_watertight: the mesh's extent %g overflows fp64", ext);
+    for (int k = 0; k < 3; ++k) { const volatile double h = fr.L / 2.0; fr.o[k] = c[k] - h; }
+    for (depth = kWtMinDepth;; ++depth) {
+        const double s = std::ldexp(fr.L, -depth);
+        VxGeom g;
+        for (int k = 0; k < 3; ++k) { const volatile double hs = s / 2.0, ok = fr.o[k] + hs; g.o[k] = ok; g.s[k] = s; g.h[k] = hs; }
+        PCU_CUDA(cudaMemsetAsync(sc.counts, 0, sizeof(VxCounts), stream));
+        PCU_LAUNCH((vx_bounds_kernel<T>), (unsigned)tiles, kThreads, stream, v, nv, f, fkind, m, g, sc.faces, sc.local, sc.tile, sc.counts);
+        PCU_LAUNCH(vx_tiles_kernel, 1, 1024, stream, sc.tile, tiles, sc.counts);
+        PCU_LAUNCH((vx_test_kernel<T, kVxCount>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
+                   (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, (McRec*)nullptr, (unsigned*)nullptr, 0);
+        VxCounts cnt;
+        PCU_TRY(read_record(sc.counts, &cnt, stream));
+        if (cnt.bad_corner) return bad_corners(cnt.bad_corner);
+        if (cnt.bad_bounds || !(cnt.cand_d < kVxMaxCandidates))   // not reached: the mesh lies inside the grid
+            return fail(PCU_B200_INVALID_ARGUMENT, "make_mesh_watertight: voxel bounds out of range at depth %d", depth);
+        if ((double)cnt.accepted < resolution && depth < kWtMaxDepth) continue;   // occupied <= accepted pairs
+        const size_t bytes = (size_t)1 << (3 * depth);
+        grid.reset();
+        PCU_TRY(alloc_block(grid.p, bytes, stream, "make_mesh_watertight's occupancy grid"));
+        PCU_CUDA(cudaMemsetAsync(grid.p, 0, bytes, stream));
+        PCU_LAUNCH((vx_test_kernel<T, kVxGrid>), vx_test_blocks(ws), kThreads, stream, v, nv, f, fkind, m, g, (const VxFace*)sc.faces,
+                   (const unsigned long long*)sc.local, (const unsigned long long*)sc.tile, sc.counts, (McRec*)nullptr, (unsigned*)grid.p, depth);
+        PCU_TRY(read_record(sc.counts, &cnt, stream));
+        if ((double)cnt.occupied >= resolution || depth == kWtMaxDepth) return PCU_B200_OK;
+    }
+}
+
+// The exterior and the surface of the occupancy grid (two synchronisations: the counts, then nothing until the
+// projection), into the handle's block: x (nv, 3) fp64 pre-projection vertices, faces (nf, 3) int32.
+int wt_surface(pcu_b200_workspace* ws, pcu_b200_watertight* h, unsigned char* grid, int lg, const WtFrame& fr, CallBlock& dense,
+               cudaStream_t stream) {
+    const long long N = 1ll << lg, n = N * N * N;
+    PCU_TRY(alloc_block(dense.p, sizeof(int) * (size_t)n, stream, "make_mesh_watertight's voxel labels"));
+    int* P = (int*)dense.p;
+    FfShape sh;
+    sh.w = sh.h = sh.d = N; sh.n = n; sh.seed = 0;
+    sh.lz = ff_log2_cover(N, 5);
+    sh.ly = ff_log2_cover(N, 8 - sh.lz);
+    sh.lx = ff_log2_cover(N, 10 - sh.lz - sh.ly);
+    sh.tz_n = (unsigned)((N + (1ll << sh.lz) - 1) >> sh.lz);
+    sh.ty_n = (unsigned)((N + (1ll << sh.ly) - 1) >> sh.ly);
+    const long long ftiles = ((N + (1ll << sh.lx) - 1) >> sh.lx) * sh.ty_n * sh.tz_n;
+    PCU_LAUNCH((ff_tile_kernel<unsigned char>), (unsigned)ftiles, kThreads, stream, (const unsigned char*)grid, sh, P);
+    PCU_LAUNCH((ff_cross_kernel<unsigned char>), (unsigned)ftiles, kThreads, stream, (const unsigned char*)grid, sh, P);
+    PCU_LAUNCH(wt_exterior_kernel, blocks_for(n), kThreads, stream, grid, n, P);
+    const unsigned tiles = blocks_for(n);
+    struct { unsigned* sum; unsigned long long* v0; unsigned long long* f0; McCounts* counts; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.sum = cv.take<unsigned>(tiles);
+        sc.v0 = cv.take<unsigned long long>(tiles);
+        sc.f0 = cv.take<unsigned long long>(tiles);
+        sc.counts = cv.take<McCounts>(1);
+    }));
+    PCU_LAUNCH(wt_count_kernel, tiles, kThreads, stream, (const unsigned char*)grid, lg, n, sc.sum);
+    PCU_LAUNCH(mc_tiles_kernel, 1, 1024, stream, (const unsigned*)sc.sum, (long long)tiles, sc.v0, sc.f0, sc.counts);
+    McCounts c;
+    PCU_TRY(read_record(sc.counts, &c, stream));
+    if (c.slots >= 0x7fffffffull || c.faces >= 0x7fffffffull)
+        return fail(PCU_B200_INVALID_ARGUMENT, "make_mesh_watertight: at most 2^31 - 2 vertices and faces are supported, got %llu and %llu",
+                    c.slots, c.faces);
+    h->nv = (long long)c.slots;
+    h->nf = (long long)c.faces;
+    const auto carve = [&](Carver& cv) {
+        h->x = cv.take<double>(3 * (size_t)h->nv);
+        h->faces = cv.take<int>(3 * (size_t)h->nf);
+    };
+    PCU_TRY(alloc_block(h->block, carve_at(nullptr, carve), stream, "make_mesh_watertight"));
+    carve_at(h->block, carve);
+    WtPlace pl;
+    for (int k = 0; k < 3; ++k) pl.o[k] = fr.o[k];
+    pl.s = std::ldexp(fr.L, -lg);
+    PCU_LAUNCH(wt_verts_kernel, tiles, kThreads, stream, (const unsigned char*)grid, lg, n, (const unsigned long long*)sc.v0,
+               (const unsigned long long*)sc.f0, pl, P, const_cast<double*>(h->x));
+    PCU_LAUNCH(wt_faces_kernel, tiles, kThreads, stream, (const unsigned char*)grid, lg, n, (const unsigned long long*)sc.v0,
+               (const unsigned long long*)sc.f0, (const int*)P, const_cast<int*>(h->faces));
+    return PCU_B200_OK;
+}
+
+constexpr int kWtRounds = 10;
+
+// The projection rounds of DESIGN.md §3 on h->x: the input's fp64 tree once, then per round the closest points, the
+// proposals, flip passes until none is flipped (one synchronisation each) and the commit.
+template <typename T>
+int wt_project(pcu_b200_workspace* ws, pcu_b200_watertight* h, const T* v, long long nv, const void* f, long long m, int fkind,
+               cudaStream_t stream) {
+    const long long n = h->nv, nf = h->nf;
+    if (n == 0) return PCU_B200_OK;
+    struct { unsigned char* tree; double* v64; double* x0; double* y; double* alpha; int* rev; double* d; long long* fidx; double* bc;
+             unsigned long long* flipped; } sc;
+    MeshTree<Pt<double>> t;
+    const auto carve = [&](Carver& cv) {
+        sc.tree = cv.take<unsigned char>(carve_at(nullptr, [&](Carver& c2) { carve_mesh_tree<Pt<double>>(c2, m, false, t); }));
+        sc.v64 = sizeof(T) == 8 ? nullptr : cv.take<double>(3 * (size_t)nv);
+        sc.x0 = cv.take<double>(3 * (size_t)n);
+        sc.y = cv.take<double>(3 * (size_t)n);
+        sc.alpha = cv.take<double>((size_t)n);
+        sc.rev = cv.take<int>((size_t)n);
+        sc.d = cv.take<double>((size_t)n);
+        sc.fidx = cv.take<long long>((size_t)n);
+        sc.bc = cv.take<double>(3 * (size_t)n);
+        sc.flipped = cv.take<unsigned long long>(2);
+    };
+    CallBlock blk(stream);
+    PCU_TRY(alloc_block(blk.p, carve_at(nullptr, carve), stream, "make_mesh_watertight's projection"));
+    carve_at(blk.p, carve);
+    const double* v64 = (const double*)v;
+    if (sizeof(T) != 8) {
+        PCU_LAUNCH((wt_widen_kernel<T>), blocks_for(3 * nv), kThreads, stream, v, 3 * nv, sc.v64);
+        v64 = sc.v64;
+    }
+    PCU_TRY(build_mesh_tree<double>(ws, v64, nv, f, m, fkind, false, sc.flipped + 1, stream, t, sc.tree));
+    double* x = const_cast<double*>(h->x);
+    const unsigned vb = blocks_for(n), fb = blocks_for(nf);
+    PCU_LAUNCH(wt_start_kernel, vb, kThreads, stream, (const double*)x, n, sc.x0, sc.alpha);
+    for (int round = 0; round < kWtRounds; ++round) {
+        PCU_LAUNCH((mq_query_kernel<double>), query_blocks(ws, n), kThreads, stream, (const double*)x, n, m, (const MqScratch*)t.sc,
+                   (const MqNode*)t.nodes, (const Pt<double>*)t.leaves, sc.d, (void*)sc.fidx, 1, sc.bc);
+        PCU_LAUNCH(wt_propose_kernel, vb, kThreads, stream, v64, nv, f, fkind, (const long long*)sc.fidx, (const double*)sc.bc,
+                   (const double*)x, (const double*)sc.alpha, n, sc.y);
+        PCU_CUDA(cudaMemsetAsync(sc.rev, 0, sizeof(int) * (size_t)n, stream));
+        for (int pass = 1;; ++pass) {
+            PCU_CUDA(cudaMemsetAsync(sc.flipped, 0, sizeof(unsigned long long), stream));
+            PCU_LAUNCH(wt_flip_kernel, fb, kThreads, stream, h->faces, nf, (const double*)sc.x0, (const double*)x, (const double*)sc.y,
+                       sc.rev, pass, sc.flipped);
+            unsigned long long flipped = 0;
+            PCU_TRY(read_record(sc.flipped, &flipped, stream));
+            if (flipped == 0) break;
+        }
+        PCU_LAUNCH(wt_commit_kernel, vb, kThreads, stream, (const double*)sc.y, (const int*)sc.rev, n, x, sc.alpha);
+    }
+    return PCU_B200_OK;
+}
+
+template <typename T>
+int make_mesh_watertight_prepare_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind,
+                                        double resolution, pcu_b200_watertight** out, long long* out_counts, cudaStream_t stream) {
+    if (!ws || !out || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    if (!v || !f) return fail(PCU_B200_INVALID_ARGUMENT, "null input pointer");
+    if (nv <= 0 || m <= 0) return fail(PCU_B200_INVALID_ARGUMENT, "Invalid input mesh with zero elements");
+    if (nv >= 0x7fffffffLL || m >= 0x7fffffffLL)
+        return fail(PCU_B200_INVALID_ARGUMENT, "make_mesh_watertight: at most 2^31 - 2 vertices and faces are supported");
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_watertight* h) -> int {
+        h->t_f64 = sizeof(T) == 8;
+        h->fkind = fkind;
+        CallBlock grid(stream), dense(stream);
+        WtFrame fr;
+        PCU_TRY(wt_depth_search<T>(ws, v, nv, f, m, fkind, resolution, grid, fr, h->depth, stream));
+        PCU_TRY(wt_surface(ws, h, grid.p, h->depth, fr, dense, stream));
+        grid.reset();
+        dense.reset();
+        const long long most = fkind == kIdxI32 ? (1ll << 31) : fkind == kIdxU32 ? (1ll << 32) : LLONG_MAX;
+        if (h->nv > most) return fail(PCU_B200_INVALID_ARGUMENT, "make_mesh_watertight: %lld vertices cannot be indexed by f's dtype", h->nv);
+        return wt_project<T>(ws, h, v, nv, f, m, fkind, stream);
+    }));
+    out_counts[0] = (*out)->nv;
+    out_counts[1] = (*out)->nf;
+    out_counts[2] = (*out)->depth;
+    return PCU_B200_OK;
+}
+
+int make_mesh_watertight_emit_device(pcu_b200_workspace* ws, const pcu_b200_watertight* h, void* out_v, void* out_f, cudaStream_t stream) {
+    if (!ws || !h) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    PCU_TRY(check_handle_device(ws, h, "watertight"));
+    if (h->nv == 0 && h->nf == 0) return PCU_B200_OK;
+    if (!out_v || !out_f) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    const unsigned blocks = blocks_for(3 * std::max(h->nv, h->nf));
+    if (h->t_f64) PCU_LAUNCH(wt_emit_kernel<double>, blocks, kThreads, stream, h->x, h->nv, h->faces, h->nf, (int)wide_index(h->fkind), (double*)out_v, out_f);
+    else PCU_LAUNCH(wt_emit_kernel<float>, blocks, kThreads, stream, h->x, h->nv, h->faces, h->nf, (int)wide_index(h->fkind), (float*)out_v, out_f);
+    return PCU_B200_OK;
 }
 
 // ---- mesh connected components and vertex removal (mesh_topology.cuh) ----------------------------------------------
@@ -4123,6 +4358,24 @@ int pcu_b200_voxelize_destroy(pcu_b200_voxelize* vx) {
 int pcu_b200_flood_fill_3d(pcu_b200_workspace* ws, const void* grid, int grid_kind, int64_t w, int64_t h, int64_t d, int64_t seed_x,
                            int64_t seed_y, int64_t seed_z, double fill_value, void* out, void* stream) {
     return flood_fill_3d_device(ws, grid, grid_kind, w, h, d, seed_x, seed_y, seed_z, fill_value, out, (cudaStream_t)stream);
+}
+
+int pcu_b200_make_mesh_watertight_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                              double resolution, pcu_b200_watertight** out_wt, int64_t out_counts[3], void* stream) {
+    return make_mesh_watertight_prepare_device<float>(ws, v, nv, f, nf, f_kind, resolution, out_wt, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_make_mesh_watertight_prepare_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                              double resolution, pcu_b200_watertight** out_wt, int64_t out_counts[3], void* stream) {
+    return make_mesh_watertight_prepare_device<double>(ws, v, nv, f, nf, f_kind, resolution, out_wt, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_make_mesh_watertight_emit(pcu_b200_workspace* ws, const pcu_b200_watertight* wt, void* out_v, void* out_f, void* stream) {
+    return make_mesh_watertight_emit_device(ws, wt, out_v, out_f, (cudaStream_t)stream);
+}
+int pcu_b200_make_mesh_watertight_destroy(pcu_b200_watertight* wt) {
+    if (!wt) return PCU_B200_OK;
+    DeviceGuard guard(wt->device);
+    delete wt;
+    return PCU_B200_OK;
 }
 
 int pcu_b200_connected_components_prepare(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_cols, int f_kind,

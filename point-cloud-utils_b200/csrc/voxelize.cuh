@@ -9,8 +9,9 @@
 //   vx_tiles_kernel    one CTA: exclusive scan of the tile sums -> a face's first candidate = tile offset + local prefix
 //   vx_test_kernel     persistent CTAs walk the flat candidate space in slices of kVxSlice candidates; a slice's faces
 //                      come from the prefix sums by binary search, so a face of 10^8 candidates and a million faces of
-//                      ten candidates each spread over the SMs alike.  Run twice: counting (kEmit = false), then, with
-//                      the code buffer sized by that count, writing the kept voxels' Morton codes (kEmit = true).
+//                      ten candidates each spread over the SMs alike.  Run twice: counting (kVxCount), then, with the
+//                      code buffer sized by that count, writing the kept voxels' Morton codes (kVxCodes).  A third mode
+//                      (kVxGrid, make_mesh_watertight) sets the kept voxels' bytes in a dense 2^g-sided grid instead.
 //   then the codes' sort (sort.cuh), their run heads (mc_heads_kernel) and vx_decode_kernel, which compacts the heads
 //   (keep_rank) and decodes them into the (n, 3) int32 result.
 //
@@ -50,7 +51,11 @@ struct VxCounts {
     unsigned long long accepted;     // accepted (face, voxel) pairs
     unsigned long long cursor;       // next free record of the emit pass
     long long unique;                // distinct codes (keep_offsets_kernel)
+    unsigned long long occupied;     // kVxGrid: voxels whose byte this pass set first
 };
+
+// What vx_test_kernel does with an accepted candidate.
+enum VxMode { kVxCount, kVxCodes, kVxGrid };
 
 // ((a - b) x (c - b)) style helpers of triBoxOverlap (src/common/tribox.h), every operation rounded on its own
 __device__ __forceinline__ bool vx_reject(double pa, double pb, double rad) {   // AXISTEST_*: min / max of two, then the test
@@ -193,15 +198,18 @@ __device__ __forceinline__ long long vx_face_of(const unsigned long long* __rest
 
 // Persistent CTAs over the flat candidate space, kVxSlice candidates per step.  The slice's faces (at most kVxSlice)
 // and their first candidates go to shared memory; candidate c of the slice finds its face there by binary search.
-// kEmit = false: adds the accepted count to counts->accepted.  kEmit = true: writes the accepted voxels' codes as
-// sort records, at positions handed out per slice by one atomicAdd on counts->cursor (their order is the sort's
-// business).  Nothing runs when the bounds pass found an error or the total overflows.
-template <typename T, bool kEmit>
+// kVxCount: adds the accepted count to counts->accepted.  kVxCodes: writes the accepted voxels' codes as sort records,
+// at positions handed out per slice by one atomicAdd on counts->cursor (their order is the sort's business).  kVxGrid:
+// sets byte (i 2^g + j) 2^g + k of `grid` (2^(3g) bytes, zero or one each, addressed as 32-bit words) to one for every
+// accepted voxel inside [0, 2^g)^3 -- idempotent, so no order and no sort -- and adds the voxels whose byte it set
+// first to counts->occupied.  Nothing runs when the bounds pass found an error or the total overflows.
+template <typename T, int kMode>
 __global__ void __launch_bounds__(kThreads) vx_test_kernel(const T* __restrict__ v, long long nv, const void* __restrict__ f, int fkind,
                                                            long long m, const __grid_constant__ VxGeom g, const VxFace* __restrict__ faces,
                                                            const unsigned long long* __restrict__ local_start,
                                                            const unsigned long long* __restrict__ tile_off, VxCounts* __restrict__ counts,
-                                                           McRec* __restrict__ recs) {
+                                                           McRec* __restrict__ recs, unsigned* __restrict__ grid = nullptr, int lg = 0) {
+    constexpr bool kEmit = kMode == kVxCodes;
     __shared__ unsigned long long s_start[kVxSlice + 1];
     __shared__ long long s_face[2];
     __shared__ unsigned long long s_base;
@@ -243,6 +251,15 @@ __global__ void __launch_bounds__(kThreads) vx_test_kernel(const T* __restrict__
             for (int k = 0; k < 3; ++k) ctr[k] = __dadd_rn(g.o[k], __dmul_rn((double)idx[k], g.s[k]));
             if (vx_tri_box(ctr, g.h, a, b, cc)) {
                 if constexpr (kEmit) s_code[kept][threadIdx.x] = morton_encode3(idx[0], idx[1], idx[2]);
+                if constexpr (kMode == kVxGrid) {
+                    const unsigned side = 1u << lg;
+                    if ((unsigned)idx[0] < side && (unsigned)idx[1] < side && (unsigned)idx[2] < side) {
+                        const unsigned long long o = ((unsigned long long)idx[0] << (2 * lg)) | ((unsigned long long)idx[1] << lg) | (unsigned)idx[2];
+                        const unsigned bit = 1u << (8 * (unsigned)(o & 3));
+                        if (!(atomicOr(grid + (o >> 2), bit) & bit)) ++kept;
+                    }
+                    continue;
+                }
                 ++kept;
             }
         }
@@ -266,7 +283,7 @@ __global__ void __launch_bounds__(kThreads) vx_test_kernel(const T* __restrict__
     if constexpr (!kEmit) {
         unsigned long long all;
         block_exclusive_scan<kThreads, unsigned long long>(mine, &all);
-        if (threadIdx.x == 0 && all) atomicAdd(&counts->accepted, all);
+        if (threadIdx.x == 0 && all) atomicAdd(kMode == kVxGrid ? &counts->occupied : &counts->accepted, all);
     }
 }
 

@@ -14,6 +14,13 @@ The tables are derived from one rule, not transcribed:
     above (an SDF that is negative inside gives outward faces);
   * the cycles are taken in order of their lowest-numbered edge, each starts at that edge, and each is fan-triangulated
     from it: a cycle of k edges gives k - 2 triangles.
+
+A second table, kMcTrisManifold (make_mesh_watertight), has the same cases, cycles and triangle counts; only the fan's
+apex differs.  It is the first edge in cycle order none of whose chords (its diagonals to the cycle's non-adjacent
+edges) joins two edges on a common cube face.  A segment between two edges of one cube face is shared with the cube
+across that face, so a chord there can give an edge four triangles (case 95's chord 4-6 on its top face meets case
+245's on its bottom face); a chord between edges that share no face lies inside one cube, and on a grid of such cubes
+every surface edge has exactly two triangles.
 """
 import os
 import sys
@@ -86,8 +93,33 @@ def case_cycles(case):
     return cycles
 
 
-def tables():
-    """(edge masks, triangle lists) of the 256 cases."""
+def _edge_faces(e):
+    """The two cube faces (indices into FACES) that edge e lies on."""
+    a, b = EDGES[e]
+    return {i for i, (corners, _) in enumerate(FACES) if a in corners and b in corners}
+
+
+def _shares_face(e, g):
+    return bool(_edge_faces(e) & _edge_faces(g))
+
+
+def manifold_apex(cyc):
+    """Position in `cyc` of the first edge whose chords join no two edges on a common cube face."""
+    k = len(cyc)
+    for j in range(k):
+        if not any(_shares_face(cyc[j], cyc[(j + i) % k]) for i in range(2, k - 1)):
+            return j
+    raise AssertionError(cyc)
+
+
+def _fan(cyc, j):
+    """The fan of cycle `cyc` from position j, in cycle order (orientation kept)."""
+    k = len(cyc)
+    return [(cyc[j], cyc[(j + i) % k], cyc[(j + i + 1) % k]) for i in range(1, k - 1)]
+
+
+def tables(manifold=False):
+    """(edge masks, triangle lists) of the 256 cases; manifold: the triangles of kMcTrisManifold."""
     masks, tris = [], []
     for case in range(256):
         mask = 0
@@ -97,8 +129,34 @@ def tables():
         cyc = case_cycles(case)
         assert sorted(e for c in cyc for e in c) == [e for e in range(12) if mask >> e & 1]
         masks.append(mask)
-        tris.append([(c[0], c[i], c[i + 1]) for c in cyc for i in range(1, len(c) - 1)])
+        tris.append([t for c in cyc for t in _fan(c, manifold_apex(c) if manifold else 0)])
     return masks, tris
+
+
+def check_manifold_table():
+    """The manifold table's asserted properties: the edge masks, cycles and triangle counts of kMcTris, every triangle's
+    edges in one cycle of its case, and no chord between two edges that share a cube face.  Returns the number of
+    cycles whose apex moved."""
+    masks, tris = tables()
+    masks_m, tris_m = tables(manifold=True)
+    assert masks_m == masks and [len(t) for t in tris_m] == [len(t) for t in tris]
+    moved = 0
+    for case in range(256):
+        cycles = case_cycles(case)
+        got = list(tris_m[case])
+        for c in cycles:
+            fan, got = got[:len(c) - 2], got[len(c) - 2:]
+            apex = fan[0][0] if fan else c[0]
+            assert all(t[0] == apex and {t[1], t[2]} <= set(c) for t in fan)
+            assert fan == _fan(c, c.index(apex))
+            for t in fan:                       # chords: the apex's diagonals to non-adjacent cycle edges
+                for e in (t[1], t[2]):
+                    k, p, q = len(c), c.index(apex), c.index(e)
+                    if (q - p) % k not in (1, k - 1):
+                        assert not _shares_face(apex, e), (case, c, apex, e)
+            moved += apex != c[0]
+        assert not got
+    return moved
 
 
 MAX_TRIS = 5      # the most triangles any case has (asserted below); the kernels size per-cube work by it
@@ -106,6 +164,8 @@ MAX_TRIS = 5      # the most triangles any case has (asserted below); the kernel
 
 def render():
     masks, tris = tables()
+    _, tris_m = tables(manifold=True)
+    check_manifold_table()
     most = max(len(t) for t in tris)
     assert most == MAX_TRIS, most
     lines = ["// mc_tables.h -- marching-cubes case tables, written by tools/mc_tables.py (do not edit; DESIGN.md §3).",
@@ -123,6 +183,12 @@ def render():
     lines += ["};", "", "// the triangles' edges, three per triangle, unused entries 255",
               "__device__ const unsigned char kMcTris[256][3 * kMcMaxTris] = {"]
     for case, t in enumerate(tris):
+        flat = [e for tri in t for e in tri] + [255] * (3 * most - 3 * len(t))
+        lines.append("    {%s},   // %d" % (", ".join(str(e) for e in flat), case))
+    lines += ["};", "", "// make_mesh_watertight's triangles: kMcTris with each fan's apex moved to the first edge of its cycle none of",
+              "// whose chords joins two edges on a common cube face (closed 2-manifolds on a grid of cubes); counts as kMcTriCount",
+              "__device__ const unsigned char kMcTrisManifold[256][3 * kMcMaxTris] = {"]
+    for case, t in enumerate(tris_m):
         flat = [e for tri in t for e in tri] + [255] * (3 * most - 3 * len(t))
         lines.append("    {%s},   // %d" % (", ".join(str(e) for e in flat), case))
     lines += ["};", "", "}  // namespace pcu", ""]
