@@ -532,8 +532,10 @@ def estimate_point_cloud_normals_knn(points, num_neighbors, view_directions=None
 
     Mirrors /root/reference/point_cloud_utils/_pointcloud_normals.py:4-54 and
     /root/reference/src/point_cloud_normals.cpp:115-173, :375-411.  Neighbour sets are the reference's; the normal is the
-    same plane-fit direction up to rounding (1e-6 in the dot product for well-separated singular values) and, when no
-    view directions are given, up to sign -- the reference's sign is whatever Eigen's JacobiSVD returns.
+    same plane-fit direction as an SVD of the neighbour offsets, to within sin(angle) <= 64 u s1 / (s2 - s3) of the exact
+    one (u = 2^-53, s1 >= s2 >= s3 the offsets' singular values; plus 2^-23 for float32 outputs) and, when no view
+    directions are given, up to sign -- the reference's sign is whatever Eigen's JacobiSVD returns.  Fewer than three
+    neighbours (num_neighbors < 3) give a zero normal; a neighbourhood of coincident points gives (0, 0, 1).
     """
     def host(p, dirs):
         return _pcu_internal.estimate_point_cloud_normals_knn_internal(p, dirs, int(num_neighbors), int(max_points_per_leaf),
@@ -545,7 +547,6 @@ def estimate_point_cloud_normals_knn(points, num_neighbors, view_directions=None
                                           0 if dirs is None else dirs.data_ptr(), int(num_neighbors),
                                           float(drop_angle_threshold), idx.data_ptr(), nrm.data_ptr(), count.data_ptr(),
                                           int(max_points_per_leaf), dev, stream)
-        return dirs is None and pts.shape[0] >= int(num_neighbors)
 
     return _normals(points, view_directions, device, host, launch, num_neighbors)
 
@@ -581,7 +582,9 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
 
     Mirrors /root/reference/point_cloud_utils/_pointcloud_normals.py:57-123 and
     /root/reference/src/point_cloud_normals.cpp:48-113, :303-370.  Neighbour sets (hence which points are kept by
-    min_pts_per_ball) are the reference's; normals agree up to rounding and, without view directions, up to sign.
+    min_pts_per_ball) are the reference's; normals are within sin(angle) <= 64 u s1 / (s2 - s3) of the exact fit of the
+    (weighted) offsets, as for `estimate_point_cloud_normals_knn`, and, without view directions, agree up to sign.  A
+    ball of coincident points gives (0, 0, 1).
     """
     seed = int(_np.random.randint(2 ** 31 - 1))
 
@@ -596,7 +599,6 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
                                            0 if dirs is None else dirs.data_ptr(), float(ball_radius), int(min_pts_per_ball),
                                            int(max_pts_per_ball), float(drop_angle_threshold), str(weight_function), seed,
                                            idx.data_ptr(), nrm.data_ptr(), count.data_ptr(), dev, stream)
-        return False
 
     return _normals(points, view_directions, device, host, launch)
 
@@ -604,8 +606,9 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
 def _normals(points, view_directions, device, host, launch, num_neighbors=None):
     """The call path of the two normal estimators.  numpy arrays go to host(points, view_directions), the binding's host
     entry point; CPU tensors go there as numpy arrays and come back as tensors.  CUDA tensors go to launch(points, view
-    directions or None, idx, normals, count, device index, stream), which returns True when every point is kept, so
-    that the count need not be read.  num_neighbors: the k-NN estimator's, checked with the tensor arguments."""
+    directions or None, idx, normals, count, device index, stream); the kept count is always read back, since even
+    without view directions a row with a NaN or infinite coordinate is dropped.  num_neighbors: the k-NN estimator's,
+    checked with the tensor arguments."""
     tensor = _is_tensor(points)
     if tensor:
         torch = _torch()
@@ -630,8 +633,7 @@ def _normals(points, view_directions, device, host, launch, num_neighbors=None):
             idx = torch.empty(n, dtype=torch.int64, device=points.device)
             nrm = torch.empty((n, 3), dtype=points.dtype, device=points.device)
             count = torch.empty(1, dtype=torch.int64, device=points.device)
-            if launch(points, view_directions, idx, nrm, count, *_call_args(points)):
-                return idx, nrm          # every point is kept: no need to wait for the count
+            launch(points, view_directions, idx, nrm, count, *_call_args(points))
             m = int(count.item())
             return idx[:m], nrm[:m]
         points, view_directions = points.numpy(), None if view_directions is None else view_directions.numpy()

@@ -9,61 +9,16 @@
 // are the reference's, bit for bit.  The plane fit is where parity is a tolerance: the reference takes the
 // right singular vector of the smallest singular value of the (k, 3) matrix of neighbour offsets from Eigen's
 // JacobiSVD in double precision (Eigen is fetched at build time and is not in the reference tree); here it is
-// the eigenvector of the smallest eigenvalue of the 3 x 3 scatter matrix A^T A, accumulated in fp64 and
-// diagonalised by cyclic Jacobi rotations -- the same subspace, equal up to rounding (and up to sign: without
-// view directions the reference's sign is whatever its SVD happens to return).
+// PlaneFit of plane_fit.h: the offsets scaled by a power of two, the scatter matrix diagonalised by Jacobi
+// rotations and refined on the offsets rotated into its eigenbasis, to the SVD's accuracy u s1 / (s2 - s3) --
+// the same vector up to rounding (and up to sign: without view directions the reference's sign is whatever its SVD
+// happens to return).  Fewer than 3 neighbours give the zero vector, all-zero offsets give (0, 0, 1).
 #pragma once
 #include "common.cuh"
 #include "compact.cuh"
+#include "plane_fit.h"
 
 namespace pcu {
-
-// One Jacobi rotation annihilating a[p][q] of the symmetric 3 x 3 matrix a; v accumulates the rotations.
-template <int P, int Q>
-__device__ __forceinline__ void jacobi_rotate(double (&a)[3][3], double (&v)[3][3]) {
-    const double apq = a[P][Q];
-    if (apq == 0.0) return;
-    const double theta = (a[Q][Q] - a[P][P]) / (2.0 * apq);
-    const double t = (theta >= 0.0 ? 1.0 : -1.0) / (fabs(theta) + sqrt(theta * theta + 1.0));
-    const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
-    constexpr int R = 3 - P - Q;   // the third index
-    const double app = a[P][P], aqq = a[Q][Q], arp = a[R][P], arq = a[R][Q];
-    a[P][P] = app - t * apq;
-    a[Q][Q] = aqq + t * apq;
-    a[P][Q] = a[Q][P] = 0.0;
-    a[R][P] = a[P][R] = c * arp - s * arq;
-    a[R][Q] = a[Q][R] = s * arp + c * arq;
-#pragma unroll
-    for (int i = 0; i < 3; ++i) {
-        const double vip = v[i][P], viq = v[i][Q];
-        v[i][P] = c * vip - s * viq;
-        v[i][Q] = s * vip + c * viq;
-    }
-}
-
-// Unit eigenvector of the smallest eigenvalue of the symmetric positive semi-definite matrix
-// [[xx, xy, xz], [xy, yy, yz], [xz, yz, zz]].
-__device__ __forceinline__ void smallest_eigenvector(double xx, double xy, double xz, double yy, double yz, double zz,
-                                                     double (&n)[3]) {
-    double a[3][3] = {{xx, xy, xz}, {xy, yy, yz}, {xz, yz, zz}};
-    double v[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
-    const double scale = fabs(xx) + fabs(yy) + fabs(zz);
-    for (int sweep = 0; sweep < 16; ++sweep) {
-        const double off = fabs(a[0][1]) + fabs(a[0][2]) + fabs(a[1][2]);
-        if (!(off > 1e-300) || off <= 1e-22 * scale) break;
-        jacobi_rotate<0, 1>(a, v);
-        jacobi_rotate<0, 2>(a, v);
-        jacobi_rotate<1, 2>(a, v);
-    }
-    const double e0 = a[0][0], e1 = a[1][1], e2 = a[2][2];
-    const int which = (e0 <= e1 && e0 <= e2) ? 0 : (e1 <= e2 ? 1 : 2);
-    double nx = which == 0 ? v[0][0] : (which == 1 ? v[0][1] : v[0][2]);
-    double ny = which == 0 ? v[1][0] : (which == 1 ? v[1][1] : v[1][2]);
-    double nz = which == 0 ? v[2][0] : (which == 1 ? v[2][1] : v[2][2]);
-    const double len = sqrt(nx * nx + ny * ny + nz * nz);
-    if (len > 0.0) { nx /= len; ny /= len; nz /= len; }
-    n[0] = nx; n[1] = ny; n[2] = nz;
-}
 
 // Orientation towards / filtering by the view direction (:160-171 and :103-112, the same code in both estimators).
 __device__ __forceinline__ bool orient_by_view(double (&nrm)[3], double vx, double vy, double vz, double drop_angle_threshold) {
@@ -89,16 +44,20 @@ __global__ void __launch_bounds__(kThreads) normals_knn_kernel(const T* __restri
     bool ok = row[k - 1] >= 0;
     double nrm[3] = {0.0, 0.0, 0.0};
     if (ok) {
-        double xx = 0.0, xy = 0.0, xz = 0.0, yy = 0.0, yz = 0.0, zz = 0.0;
-        for (int j = 0; j < k; ++j) {
-            const long long p = row[j];
-            // the reference subtracts in the cloud's precision and widens the difference (:150-154)
-            const double dx = (double)(T)(points[3 * p] - points[3 * i]);
-            const double dy = (double)(T)(points[3 * p + 1] - points[3 * i + 1]);
-            const double dz = (double)(T)(points[3 * p + 2] - points[3 * i + 2]);
-            xx += dx * dx; xy += dx * dy; xz += dx * dz; yy += dy * dy; yz += dy * dz; zz += dz * dz;
-        }
-        smallest_eigenvector(xx, xy, xz, yy, yz, zz, nrm);
+        using R = Real<T>;
+        const T qx = points[3 * i], qy = points[3 * i + 1], qz = points[3 * i + 2];
+        // the reference subtracts in the cloud's precision and widens the difference (:150-154)
+        auto offsets = [&](auto&& f) {
+            for (int j = 0; j < k; ++j) {
+                const long long p = row[j];
+                f((double)R::sub(points[3 * p], qx), (double)R::sub(points[3 * p + 1], qy), (double)R::sub(points[3 * p + 2], qz));
+            }
+        };
+        double big = 0.0;
+        offsets([&](double x, double y, double z) { big = fmax(big, fmax(fabs(x), fmax(fabs(y), fabs(z)))); });
+        PlaneFit fit(pow2_scale(big));
+        do offsets([&](double x, double y, double z) { fit.add(x, y, z); }); while (fit.solve());
+        fit.normal(k, nrm);
         if (view_dirs != nullptr) {
             const double vx = (double)view_dirs[3 * i], vy = (double)view_dirs[3 * i + 1], vz = (double)view_dirs[3 * i + 2];
             ok = orient_by_view(nrm, vx, vy, vz, drop_angle_threshold);   // :160-171
@@ -222,8 +181,23 @@ __global__ void __launch_bounds__(kThreads) cell_order_kernel(Cloud<T> cl) {
     }
 }
 
+// The scale of every ball's fit (PlaneFit): one power of two for the call, bounding every weighted offset a ball holds.
+// A member has d2 < r2, so |offset| <= sqrt(r2) (1 + 2 ulp); Wendland's weight falls from 1 on [0, 1] and rises
+// beyond, so it is at most max(1, w(r_max)).  The bound scales with the cloud (r2 by 4^e for constant weights), and
+// an infinite fp32 r2 admits offsets below 2^129 only.
+template <typename T>
+__device__ __forceinline__ double ball_scale(T r2, const BallParams& bp) {
+    double bound = fmin(sqrt((double)r2), sizeof(T) == 4 ? 0x1p128 : 0x1.fffffffffffffp1023) * (1.0 + 0x1p-20);
+    const double r = bound / bp.radius;
+    if (bp.weight_kind == 1 && r > 1.0) {
+        const double v1 = r - 1.0, v2 = 4 * r + 1.0;
+        bound *= fmax(1.0, v1 * v1 * v1 * v1 * v2 * (1.0 + 0x1p-20));
+    }
+    return pow2_scale(fmin(bound, 0x1.fffffffffffffp1023));
+}
+
 // One thread per point, in CELL order (neighbouring lanes walk overlapping boxes).  normals / keep are indexed by the
-// caller's row.
+// caller's row.  The fit's first pass rides on the walk that counts the ball; each further pass walks it again.
 template <typename T>
 __global__ void __launch_bounds__(kThreads) normals_ball_kernel(Cloud<T> cl, const T* __restrict__ view_dirs, BallParams bp,
                                                                 T* __restrict__ normals, unsigned char* __restrict__ keep) {
@@ -237,36 +211,38 @@ __global__ void __launch_bounds__(kThreads) normals_ball_kernel(Cloud<T> cl, con
     const Pt<T> q = load_pt<T>(cl.sorted + pos);
     const long long row = (long long)q.i;
     const T r2 = (T)bp.radius;                       // radiusSearch takes a DistanceType: the double is narrowed (:74)
-    double xx = 0.0, xy = 0.0, xz = 0.0, yy = 0.0, yz = 0.0, zz = 0.0;
+    auto wendland = [&](double r) { const double v1 = 1.0 - r, v2 = 4 * r + 1.0; return v1 * v1 * v1 * v1 * v2; };
+    PlaneFit fit(ball_scale<T>(r2, bp));
     auto fold = [&](const Pt<T>& p, T d2) {
-        double w = 1.0;
-        if (bp.weight_kind == 1) {                   // wendland_rbf (:334-339), in double like the reference
-            const double r = sqrt((double)d2) / bp.radius;
-            const double v1 = 1.0 - r, v2 = 4 * r + 1.0;
-            w = v1 * v1 * v1 * v1 * v2;
-        }
+        // wendland_rbf (:334-339), in double like the reference
+        const double w = bp.weight_kind == 1 ? wendland(sqrt((double)d2) / bp.radius) : 1.0;
         // (points(nbr, j) - query[j]) * weight: the difference in the cloud's precision, the product in double (:89)
-        const double dx = (double)R::sub(p.x, q.x) * w, dy = (double)R::sub(p.y, q.y) * w, dz = (double)R::sub(p.z, q.z) * w;
-        xx += dx * dx; xy += dx * dy; xz += dx * dz; yy += dy * dy; yz += dy * dz; zz += dz * dz;
+        fit.add((double)R::sub(p.x, q.x) * w, (double)R::sub(p.y, q.y) * w, (double)R::sub(p.z, q.z) * w);
     };
     long long found = 0;
-    walk_ball<T>(cl, g, q, r2, [&](const Pt<T>& p, T d2) { ++found; fold(p, d2); });
+    walk_ball<T>(cl, g, q, r2, [&](const Pt<T>& p, T d2) { ++found; fold(p, d2); });   // also the fit's first pass
     bool ok = found >= (long long)bp.min_pts;        // :75-77 (before the cap)
-    if (ok && bp.max_pts > 0 && found > (long long)bp.max_pts) {
-        xx = xy = xz = yy = yz = zz = 0.0;
+    const bool capped = bp.max_pts > 0 && found > (long long)bp.max_pts;
+    // The capped fit's passes replay one selection sequence: the same subset every time.
+    const unsigned salt = mix32(bp.seed ^ mix32((unsigned)row * 0x9e3779b9u + 0x85ebca6bu));
+    auto fold_subset = [&]() {
         unsigned long long remaining = (unsigned long long)found, needed = (unsigned long long)bp.max_pts;
         unsigned t = 0;
-        const unsigned salt = mix32(bp.seed ^ mix32((unsigned)row * 0x9e3779b9u + 0x85ebca6bu));
         walk_ball<T>(cl, g, q, r2, [&](const Pt<T>& p, T d2) {
             const unsigned long long u = ((unsigned long long)mix32(salt + t * 0x9e3779b9u) * remaining) >> 32;   // uniform in [0, remaining)
             ++t;
             if (u < needed) { fold(p, d2); --needed; }
             --remaining;
         });
-    }
+    };
     double nrm[3] = {0.0, 0.0, 0.0};
     if (ok) {
-        smallest_eigenvector(xx, xy, xz, yy, yz, zz, nrm);
+        if (capped) { fit.reset(); fold_subset(); }
+        while (fit.solve()) {
+            if (capped) fold_subset();
+            else walk_ball<T>(cl, g, q, r2, fold);
+        }
+        fit.normal(capped ? (long long)bp.max_pts : found, nrm);
         if (view_dirs != nullptr)
             ok = orient_by_view(nrm, (double)view_dirs[3 * row], (double)view_dirs[3 * row + 1], (double)view_dirs[3 * row + 2],
                                 bp.drop_angle_threshold);
