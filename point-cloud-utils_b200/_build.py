@@ -1,11 +1,13 @@
 """In-tree build of the native code: libpcu_b200.so (CUDA kernels + C ABI, sm_90a only, i.e. H100) and the
-pybind11 module _pcu_internal that sits on top of it.
+pybind11 module _pcu_internal that sits on top of it.  Every csrc/*.cu compiles to its own object, in parallel, and the
+objects link into the library.
 
     python -m pcu_b200._build          # or:  import __graft_entry__; __graft_entry__.build()
 
 nvcc cross-compiles for sm_90a without a GPU.  The artefacts stay next to the package (they are
 git-ignored), so the package imports from the repository tree.
 """
+import concurrent.futures
 import os
 import subprocess
 import sys
@@ -16,6 +18,7 @@ CSRC = os.path.join(PKG_DIR, "csrc")
 ROOT = os.path.dirname(PKG_DIR)
 LIB = os.path.join(PKG_DIR, "libpcu_b200.so")
 EXT = os.path.join(PKG_DIR, "_pcu_internal" + sysconfig.get_config_var("EXT_SUFFIX"))
+OBJ_DIR = os.path.join(PKG_DIR, "build")
 HOST_CXX = "/usr/bin/g++"  # the image exports CXX=/opt/gcc/bin/g++, a wrapper that lacks parts of the toolchain
 
 NVCC_FLAGS = [
@@ -23,7 +26,6 @@ NVCC_FLAGS = [
     "-lineinfo", "-O3", "-std=c++17",
     "--compiler-bindir", HOST_CXX,
     "-Xcompiler", "-fPIC",
-    "-shared",
 ]
 
 
@@ -59,13 +61,19 @@ def build(force=False, verbose=False):
     """Compile whatever is out of date.  Returns the list of artefacts."""
     import pybind11
 
-    cuda_src = _sources((".cu", ".cuh", ".inl", ".h"))
-    if force or not _newer(LIB, cuda_src):
-        cmd = [nvcc_path()] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
-              ["-o", LIB, os.path.join(CSRC, "pcu_b200.cu")]
-        log = _run(cmd)
-        if verbose:
+    headers = _sources((".cuh", ".h"))
+    units = [f for f in _sources((".cu",)) if os.path.dirname(f) == CSRC]
+    os.makedirs(OBJ_DIR, exist_ok=True)
+    objs = [os.path.join(OBJ_DIR, os.path.basename(u)[:-3] + ".o") for u in units]
+    stale = [(u, o) for u, o in zip(units, objs) if force or not _newer(o, [u] + headers)]
+    ptxas = ["-Xptxas", "-v"] if verbose else []
+    with concurrent.futures.ThreadPoolExecutor(max_workers=max(1, min(len(stale), os.cpu_count() or 1))) as pool:
+        logs = list(pool.map(lambda uo: _run([nvcc_path()] + NVCC_FLAGS + ptxas + ["-c", "-o", uo[1], uo[0]]), stale))
+    if verbose:
+        for log in logs:
             print(log)
+    if force or not _newer(LIB, objs):
+        _run([nvcc_path()] + NVCC_FLAGS + ["-shared", "-o", LIB] + objs)
     bind_src = [os.path.join(CSRC, "binding.cpp"), os.path.join(ROOT, "include", "pcu_b200.h")]
     if force or not _newer(EXT, bind_src + [LIB]):
         cmd = [HOST_CXX, "-O2", "-std=c++17", "-fPIC", "-shared", "-fvisibility=hidden",

@@ -7,24 +7,11 @@
 //   an emit kernel        every thread asks keep_rank for the kept rows before its own and writes its row there
 // so the kept rows leave in ascending order, as a sequential loop that appends them would write them.  n < 2^31 rows:
 // ranks and block counts fit 32 bits.
+// The first two kernels are compiled once, in runtime.cu, and launched through enqueue_keep_offsets (runtime.cuh).
 #pragma once
 #include "common.cuh"
 
 namespace pcu {
-
-__global__ void __launch_bounds__(kThreads) keep_count_kernel(const unsigned char* __restrict__ keep, long long n, unsigned* __restrict__ block_count) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const unsigned mine = i < n ? keep[i] : 0u;
-    const unsigned total = __syncthreads_count((int)mine);
-    if (threadIdx.x == 0) block_count[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024) keep_offsets_kernel(unsigned* __restrict__ block_count, long long nblocks, long long* __restrict__ out_count) {
-    // nblocks = ceil(n / kThreads) with n < 2^31 rows: fits 32 bits
-    const unsigned kept = block_scan_rounds<1024>(
-        (unsigned)nblocks, [&](unsigned b) { return block_count[b]; }, [&](unsigned b, unsigned ex, unsigned) { block_count[b] = ex; });
-    if (threadIdx.x == 0) *out_count = (long long)kept;
-}
 
 // The number of kept rows before this thread's row (kInclusive: up to and including it), over the whole array: the
 // block's offset, the kept rows of the earlier warps of the block, those of the earlier lanes of the warp.  `mine`:

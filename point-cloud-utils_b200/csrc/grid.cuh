@@ -327,7 +327,7 @@ __device__ __forceinline__ bool load_tile_point(const Cloud<T>& c, GridHeader<T>
 }
 
 // How densely the non-empty cells turned out to be filled, left in host-mapped memory for the NEXT call
-// with the same shapes on this workspace (pcu_b200.cu sizes that call's grid from it: surfaces and
+// with the same shapes on this workspace (nearest.cu sizes that call's grid from it: surfaces and
 // other thin sets fill few cells of a box-filling grid, each with many points).  A hint only.
 //   words 0..3: {cell_cap, non-empty cells, n, valid}  (binning kernels)
 //   words 4..6: {queries the 27 cells around them could not settle, queries, valid}  (first slow pass of a search

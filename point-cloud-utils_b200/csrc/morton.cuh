@@ -64,73 +64,4 @@ __host__ __device__ __forceinline__ unsigned long long morton_negate(unsigned lo
     return (xs & kMortonX) | (ys & ym) | (zs & zm);
 }
 
-// pts: (n, 3) int32 or int64 (truncated to int32 like the reference's `int32_t px = pts(i, 0)`, morton.cpp:229)
-template <typename I>
-__global__ void morton_encode_kernel(const I* __restrict__ pts, long long n, unsigned long long* __restrict__ codes) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    codes[i] = morton_encode3((int)pts[3 * i], (int)pts[3 * i + 1], (int)pts[3 * i + 2]);
-}
-__global__ void morton_decode_kernel(const unsigned long long* __restrict__ codes, long long n, int* __restrict__ pts) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    int x, y, z;
-    morton_decode3(codes[i], x, y, z);
-    pts[3 * i] = x; pts[3 * i + 1] = y; pts[3 * i + 2] = z;
-}
-// op 0: a + b; op 1: a - b = a + negate(b)  (morton_code.cpp:160-163)
-__global__ void morton_addsub_kernel(const unsigned long long* __restrict__ a, const unsigned long long* __restrict__ b,
-                                     long long n, int op, unsigned long long* __restrict__ out) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    out[i] = morton_add2(a[i], op ? morton_negate(b[i]) : b[i]);
-}
-
-// morton_knn (morton.cpp:324-414): lower_bound of the query code in the SORTED codes, then the window of k
-// consecutive positions around it (k / 2 above, the rest below, shifted back inside the array at the ends).
-// k has already been clamped to n by the caller (:351).  sort_dist: order the window by squared distance to the
-// query point (ties by position) -- the reference's comparator reads three uninitialised locals there (:381-398),
-// so that ORDER is undefined in the reference; the window itself is exactly the reference's.
-__global__ void morton_knn_kernel(const unsigned long long* __restrict__ codes, long long n,
-                                  const unsigned long long* __restrict__ qcodes, long long m, int k, int sort_dist,
-                                  long long* __restrict__ out_idx) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m) return;
-    const unsigned long long q = qcodes[i];
-    long long lo = 0, hi = n;                 // std::lower_bound
-    while (lo < hi) {
-        const long long mid = lo + (hi - lo) / 2;
-        if (codes[mid] < q) lo = mid + 1; else hi = mid;
-    }
-    const int half_up = k / 2, half_down = k - half_up;
-    long long upper = lo + half_up, lower = lo - half_down;
-    if (upper >= n) { lower -= (upper - n); upper = n; }
-    if (lower < 0) { upper += -lower; lower = 0; }
-    long long* row = out_idx + i * k;
-    const int count = (int)(upper - lower);
-    if (!sort_dist) {
-        for (int j = 0; j < count; ++j) row[j] = lower + j;
-        return;
-    }
-    int qx, qy, qz;
-    morton_decode3(q, qx, qy, qz);
-    for (int j = 0; j < count; ++j) {         // insertion sort by (distance, position)
-        const long long pos = lower + j;
-        int x, y, z;
-        morton_decode3(codes[pos], x, y, z);
-        const double dx = (double)qx - x, dy = (double)qy - y, dz = (double)qz - z;
-        const double d = dx * dx + dy * dy + dz * dz;
-        int s = j;
-        while (s > 0) {
-            int px, py, pz;
-            morton_decode3(codes[row[s - 1]], px, py, pz);
-            const double ex = (double)qx - px, ey = (double)qy - py, ez = (double)qz - pz;
-            if (ex * ex + ey * ey + ez * ez <= d) break;
-            row[s] = row[s - 1];
-            --s;
-        }
-        row[s] = pos;
-    }
-}
-
 }  // namespace pcu

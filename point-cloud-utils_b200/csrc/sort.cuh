@@ -75,31 +75,10 @@ __global__ void __launch_bounds__(kSortThreads) sort_hist_kernel(const Rec* __re
     hist[(size_t)threadIdx.x * ntiles + blockIdx.x] = h[threadIdx.x];
 }
 
-// grid 256: CTA b turns hist[b][0 .. ntiles) into its exclusive prefix sums and writes the row total.  A row counts
-// records, at most n < 2^31, so prefixes and total fit 32 bits.
-__global__ void __launch_bounds__(kSortThreads) sort_scan_rows(unsigned* __restrict__ hist, unsigned ntiles, unsigned long long* __restrict__ total) {
-    unsigned* row = hist + (size_t)blockIdx.x * ntiles;
-    const unsigned all = block_scan_rounds<kSortThreads>(
-        ntiles, [&](unsigned i) { return row[i]; }, [&](unsigned i, unsigned ex, unsigned) { row[i] = ex; });
-    if (threadIdx.x == 0) total[blockIdx.x] = all;
-}
-
-// one CTA of 256 threads: base[bin] = records with a smaller digit; *constant = 1 when one bin holds everything
-__global__ void __launch_bounds__(kSortBins) sort_scan_bins(const unsigned long long* __restrict__ total, long long n,
-                                                            unsigned* __restrict__ base, int* __restrict__ constant) {
-    __shared__ unsigned long long s[kSortBins];
-    __shared__ int any_full;
-    const unsigned long long mine = total[threadIdx.x];
-    s[threadIdx.x] = mine;
-    if (threadIdx.x == 0) any_full = 0;
-    __syncthreads();
-    if (mine == (unsigned long long)n) any_full = 1;
-    unsigned long long before = 0ull;
-    for (int j = 0; j < (int)threadIdx.x; ++j) before += s[j];
-    base[threadIdx.x] = (unsigned)before;
-    __syncthreads();
-    if (threadIdx.x == 0) *constant = any_full;
-}
+// The two scans of a pass are compiled once, in runtime.cu; radix_sort_records (runtime.cuh) launches them.
+__global__ void sort_scan_rows(unsigned* __restrict__ hist, unsigned ntiles, unsigned long long* __restrict__ total);
+__global__ void sort_scan_bins(const unsigned long long* __restrict__ total, long long n, unsigned* __restrict__ base,
+                               int* __restrict__ constant);
 
 template <typename Rec>
 __global__ void __launch_bounds__(kSortThreads) sort_scatter_kernel(const Rec* __restrict__ in, Rec* __restrict__ out, long long n,
