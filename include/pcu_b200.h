@@ -677,6 +677,29 @@ int pcu_b200_make_mesh_watertight_prepare_f64(pcu_b200_workspace* ws, const doub
 int pcu_b200_make_mesh_watertight_emit(pcu_b200_workspace* ws, const pcu_b200_watertight* wt, void* out_v, void* out_f, void* stream);
 int pcu_b200_make_mesh_watertight_destroy(pcu_b200_watertight* wt);
 
+/* ---- shortest-edge decimation -----------------------------------------------------------------------------------------
+ * Replaces decimate_triangle_mesh (the reference's src/mesh_decimate.cpp, libigl's decimate).  Result defined in
+ * DESIGN.md §3: rounds of independent shortest-edge collapses under the link condition, midpoint placement, until at
+ * most max_faces faces remain (max_faces or max_faces - 1 unless the mesh stalls) or no edge can collapse.
+ *   decimate_triangle_mesh_prepare: v (nv, 3) in the suffix's type, f (nf, 3) of kind f_kind, 1 <= nv < 2^31 - 1,
+ *     1 <= nf <= (2^31 - 2) / 6, 1 <= max_faces <= nf.  Synchronises `stream` once for the input check, once for the
+ *     acceptance test, once per round and once for the output counts.  *out_counts = {#v_out, #f_out, rounds} (host
+ *     int64).  A corner outside [0, nv), a non-finite vertex, or a mesh the definition rejects (a repeated corner, an
+ *     edge in three or more faces, a vertex with other than zero or two boundary edges) fail with
+ *     PCU_B200_INVALID_ARGUMENT.  *out_dc (v and f need not outlive prepare) is freed by
+ *     decimate_triangle_mesh_destroy, stream-ordered on the stream it was prepared on.
+ *   decimate_triangle_mesh_emit: writes out_v (#v_out, 3) in the suffix's type, out_f (#f_out, 3), out_v_corr (#v_out)
+ *     and out_f_corr (#f_out) in f's width.
+ * Every array pointer is a DEVICE pointer. */
+typedef struct pcu_b200_decimate pcu_b200_decimate;
+int pcu_b200_decimate_triangle_mesh_prepare_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                                int64_t max_faces, pcu_b200_decimate** out_dc, int64_t out_counts[3], void* stream);
+int pcu_b200_decimate_triangle_mesh_prepare_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind,
+                                                int64_t max_faces, pcu_b200_decimate** out_dc, int64_t out_counts[3], void* stream);
+int pcu_b200_decimate_triangle_mesh_emit(pcu_b200_workspace* ws, const pcu_b200_decimate* dc, void* out_v, void* out_f, void* out_v_corr,
+                                         void* out_f_corr, void* stream);
+int pcu_b200_decimate_triangle_mesh_destroy(pcu_b200_decimate* dc);
+
 /* ---- mesh topology: connected components and vertex removal ----------------------------------------------------------
  * Replace connected_components, remove_mesh_vertices and remove_unreferenced_mesh_vertices (the reference's
  * src/connected_components.cpp, src/remove_mesh_vertices.cpp, src/remove_unreferenced_mesh_vertices.cpp).  Results

@@ -47,7 +47,7 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "marching_cubes_sparse_voxel_grid", "sparse_voxel_grid_boundary",
            "sparse_voxel_grid_from_pointcloud", "dilate_sparse_voxel_grid", "erode_sparse_voxel_grid",
            "sparse_voxel_grid_to_hex_mesh",
-           "voxelize_triangle_mesh", "flood_fill_3d", "voxel_grid_geometry", "make_mesh_watertight",
+           "voxelize_triangle_mesh", "flood_fill_3d", "voxel_grid_geometry", "make_mesh_watertight", "decimate_triangle_mesh",
            "connected_components", "remove_mesh_vertices", "remove_unreferenced_mesh_vertices", "orient_mesh_faces",
            "mesh_face_areas", "estimate_mesh_face_normals", "estimate_mesh_vertex_normals", "laplacian_smooth_mesh",
            "deduplicate_point_cloud", "voronoi_centroids_unit_cube", "lloyd_3d", "lloyd_2d",
@@ -733,6 +733,7 @@ from ._sparse_voxels import (sparse_voxel_grid_from_pointcloud, dilate_sparse_vo
                              sparse_voxel_grid_to_hex_mesh)
 from ._voxels import voxelize_triangle_mesh, flood_fill_3d, voxel_grid_geometry  # noqa: E402
 from ._watertight import make_mesh_watertight  # noqa: E402
+from ._decimate import decimate_triangle_mesh  # noqa: E402
 from ._mesh_topology import (connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices,  # noqa: E402
                              orient_mesh_faces)
 from ._mesh_geometry import mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals, laplacian_smooth_mesh  # noqa: E402

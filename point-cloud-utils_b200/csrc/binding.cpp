@@ -708,6 +708,22 @@ py::tuple make_mesh_watertight_prepare_device(bool is_f64, uintptr_t v, int64_t 
     return py::make_tuple((uintptr_t)wt, counts[0], counts[1], counts[2]);
 }
 
+// Decimation (decimate_triangle_mesh, _decimate.py): the whole decimation (synchronises `stream` before the rounds, per
+// round and for the counts), returns (handle, #v_out, #f_out, rounds); _decimate_triangle_mesh_emit writes v_out, f_out
+// and the correspondences; _decimate_triangle_mesh_destroy.
+py::tuple decimate_triangle_mesh_prepare_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, int64_t max_faces,
+                                                int device, uintptr_t stream) {
+    pcu_b200_decimate* dc = nullptr;
+    int64_t counts[3] = {0, 0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return is_f64 ? pcu_b200_decimate_triangle_mesh_prepare_f64(ws, (const double*)v, nv, (const void*)f, nf, f_kind, max_faces, &dc,
+                                                                    counts, (void*)stream)
+                      : pcu_b200_decimate_triangle_mesh_prepare_f32(ws, (const float*)v, nv, (const void*)f, nf, f_kind, max_faces, &dc,
+                                                                    counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)dc, counts[0], counts[1], counts[2]);
+}
+
 // Connected components (connected_components, _mesh_topology.py): validates f and labels (two synchronisations of
 // `stream`), returns (handle, n = max(f) + 1, components); _connected_components_emit writes cv, nv, cf and nf in f's
 // width; _connected_components_destroy.
@@ -1116,6 +1132,9 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_make_mesh_watertight_prepare_device", &make_mesh_watertight_prepare_device);
     mod.def("_make_mesh_watertight_emit_device", forward_to(pcu_b200_make_mesh_watertight_emit).single());
     mod.def("_make_mesh_watertight_destroy", destroy(pcu_b200_make_mesh_watertight_destroy));
+    mod.def("_decimate_triangle_mesh_prepare_device", &decimate_triangle_mesh_prepare_device);
+    mod.def("_decimate_triangle_mesh_emit_device", forward_to(pcu_b200_decimate_triangle_mesh_emit).single());
+    mod.def("_decimate_triangle_mesh_destroy", destroy(pcu_b200_decimate_triangle_mesh_destroy));
     mod.def("_flood_fill_3d_device", forward_to(pcu_b200_flood_fill_3d).single());
     mod.def("_connected_components_prepare_device", &connected_components_prepare_device);
     mod.def("_connected_components_emit_device", forward_to(pcu_b200_connected_components_emit).single());

@@ -17,6 +17,9 @@ constexpr int kMaxGridDim = 2048;   // cells per axis, upper bound
 constexpr int kThreads = 256;       // default CTA size of the streaming kernels
 constexpr int kMaxLevels = 12;      // 2^11 = kMaxGridDim, plus one
 
+// Index arrays come in four integer types, chosen at run time (pcu_b200_index_kind).
+enum MeshIndexKind { kIdxI32 = 0, kIdxI64 = 1, kIdxU32 = 2, kIdxU64 = 3 };
+
 // Programmatic dependent launch: every kernel of a call's chain is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, so its CTAs may be scheduled while the previous
 // kernel drains; this wait (first statement of every kernel) blocks until that kernel has completed

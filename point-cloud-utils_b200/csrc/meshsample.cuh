@@ -19,9 +19,6 @@ namespace pcu {
 constexpr int kMeshScanThreads = 256;
 constexpr int kMeshScanTile = 4096;     // faces per CTA of the CDF scan (16 per thread)
 
-// Index arrays come in four integer types, chosen at run time (pcu_b200_index_kind).
-enum MeshIndexKind { kIdxI32 = 0, kIdxI64 = 1, kIdxU32 = 2, kIdxU64 = 3 };
-
 // Entry i of an index array of kind `kind`, checked against [0, n): negative entries of a signed array wrap by n when
 // `wrap` is set (numpy's indexing), and -1 stands for anything out of range.
 __device__ __forceinline__ long long load_index(const void* a, long long i, int kind, long long n, bool wrap) {

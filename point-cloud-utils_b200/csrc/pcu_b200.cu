@@ -1567,15 +1567,6 @@ int flood_fill_3d_device(pcu_b200_workspace* ws, const void* grid, int kind, lon
 }
 
 // ---- watertight manifold remeshing (watertight.cuh) ---------------------------------------------------------------
-// A block of device memory that lives for one call, freed in the order of its stream.
-struct CallBlock {
-    unsigned char* p = nullptr;
-    cudaStream_t stream = nullptr;
-    explicit CallBlock(cudaStream_t s) : stream(s) {}
-    ~CallBlock() { reset(); }
-    void reset() { if (p) cudaFreeAsync(p, stream); p = nullptr; }
-};
-
 // The grid of DESIGN.md §3: c = (lo + hi) / 2, L = 1.4 max_a (hi_a - lo_a), o = c - L / 2, every operation rounded.
 struct WtFrame { double o[3], L; };
 

@@ -327,6 +327,15 @@ int prepare_handle(pcu_b200_workspace* ws, cudaStream_t stream, H** out, Build&&
     return PCU_B200_OK;
 }
 
+// A block of device memory that lives for one call, freed in the order of its stream.
+struct CallBlock {
+    unsigned char* p = nullptr;
+    cudaStream_t stream = nullptr;
+    explicit CallBlock(cudaStream_t s) : stream(s) {}
+    ~CallBlock() { reset(); }
+    void reset() { if (p) cudaFreeAsync(p, stream); p = nullptr; }
+};
+
 // An emit runs on the device its handle was prepared on; `what` names the handle.
 inline int check_handle_device(const pcu_b200_workspace* ws, const StreamHandle* h, const char* what) {
     if (h->device != ws->device)
