@@ -1,6 +1,7 @@
 """In-tree build of the native code: libpcu_b200.so (CUDA kernels + C ABI, sm_90a only, i.e. H100) and the
 pybind11 module _pcu_internal that sits on top of it.  Every csrc/*.cu compiles to its own object, in parallel, and the
-objects link into the library.
+objects link into the library.  nvcc writes each object's dependencies (-MD) next to it, and an object is rebuilt only
+when a file it was compiled from has changed since.
 
     python -m pcu_b200._build          # or:  import __graft_entry__; __graft_entry__.build()
 
@@ -36,17 +37,26 @@ def _newer(target, sources):
     return all(os.path.getmtime(s) <= t for s in sources)
 
 
-def _sources(exts):
-    out = []
-    for base in (CSRC, os.path.join(ROOT, "include")):
-        for f in sorted(os.listdir(base)):
-            if f.endswith(exts):
-                out.append(os.path.join(base, f))
-    return out
+def _depends(depfile):
+    """The files a make-style dependency file lists after its target, or None when it is missing.  The units compile
+    from csrc/, so the library's own files are listed relative to it and the tree can move without a rebuild."""
+    try:
+        with open(depfile) as fh:
+            text = fh.read()
+    except FileNotFoundError:
+        return None
+    text = text.replace("\\\n", " ").replace("\\ ", "\0")
+    return [os.path.join(CSRC, w.replace("\0", " ")) for w in text.split(":", 1)[1].split()] if ":" in text else []
 
 
-def _run(cmd):
-    proc = subprocess.run(cmd, capture_output=True, text=True)
+def _stale(obj, depfile):
+    """An object is out of date when it or its dependency file is missing, or when a file it depends on is newer."""
+    deps = _depends(depfile)
+    return deps is None or not all(os.path.exists(d) for d in deps) or not _newer(obj, deps)
+
+
+def _run(cmd, cwd=None):
+    proc = subprocess.run(cmd, capture_output=True, text=True, cwd=cwd)
     if proc.returncode != 0:
         raise RuntimeError("build step failed:\n  %s\n%s%s" % (" ".join(cmd), proc.stdout, proc.stderr))
     return proc.stdout + proc.stderr
@@ -61,14 +71,14 @@ def build(force=False, verbose=False):
     """Compile whatever is out of date.  Returns the list of artefacts."""
     import pybind11
 
-    headers = _sources((".cuh", ".h"))
-    units = [f for f in _sources((".cu",)) if os.path.dirname(f) == CSRC]
+    units = [os.path.join(CSRC, f) for f in sorted(os.listdir(CSRC)) if f.endswith(".cu")]
     os.makedirs(OBJ_DIR, exist_ok=True)
     objs = [os.path.join(OBJ_DIR, os.path.basename(u)[:-3] + ".o") for u in units]
-    stale = [(u, o) for u, o in zip(units, objs) if force or not _newer(o, [u] + headers)]
+    stale = [(u, o, o[:-2] + ".d") for u, o in zip(units, objs) if force or _stale(o, o[:-2] + ".d")]
     ptxas = ["-Xptxas", "-v"] if verbose else []
     with concurrent.futures.ThreadPoolExecutor(max_workers=max(1, min(len(stale), os.cpu_count() or 1))) as pool:
-        logs = list(pool.map(lambda uo: _run([nvcc_path()] + NVCC_FLAGS + ptxas + ["-c", "-o", uo[1], uo[0]]), stale))
+        logs = list(pool.map(lambda uod: _run([nvcc_path()] + NVCC_FLAGS + ptxas + ["-MD", "-MF", uod[2], "-c", "-o", uod[1],
+                                                                                   os.path.basename(uod[0])], cwd=CSRC), stale))
     if verbose:
         for log in logs:
             print(log)

@@ -223,11 +223,6 @@ int pcu_b200_decimate_triangle_mesh_emit(pcu_b200_workspace* ws, const pcu_b200_
                                          void* out_f_corr, void* stream) {
     return decimate_emit_device(ws, dc, out_v, out_f, out_v_corr, out_f_corr, (cudaStream_t)stream);
 }
-int pcu_b200_decimate_triangle_mesh_destroy(pcu_b200_decimate* dc) {
-    if (!dc) return PCU_B200_OK;
-    DeviceGuard guard(dc->device);
-    delete dc;
-    return PCU_B200_OK;
-}
+int pcu_b200_decimate_triangle_mesh_destroy(pcu_b200_decimate* dc) { return destroy_handle(dc); }
 
 }  // extern "C"

@@ -7,7 +7,7 @@
 //   lap_edge_kernel     six directed-edge records per face: the edge opposite corner k joins a = f[k+1] and b = f[k+2];
 //                       records 6t + 2k and 6t + 2k + 1 are (a, b) and (b, a), key (row << bits) | column
 //   radix sort (sort.cuh), stable: each run of equal keys lists its contributions in ascending face order
-//   mc_heads_kernel, keep_count / keep_offsets (compact.cuh): one entry per run, nnz
+//   mc_heads_kernel (runtime.cu), keep_count / keep_offsets (compact.cuh): one entry per run, nnz
 //   lap_entries_kernel  each run head sums its run in order: L_ij = sum of cot / 2, as int32 columns and fp64 values
 //   mg_rows_kernel      row pointers of the entries (rows = vertices)
 //   lap_diag_kernel     L_ii = -sum_j L_ij in ascending column order; `lone` marks the rows without a non-zero weight

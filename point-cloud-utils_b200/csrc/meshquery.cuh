@@ -28,6 +28,8 @@
 //   mq_refit_kernel     faces: bottom-up boxes with per-node arrival counters: the second child to arrive writes both
 //                       children's boxes into the parent (one 64-byte record per visit)
 //   mq_query_kernel     one thread per query: nearer child first, the other pushed; pruning with the margin of §3.
+// mesh_query.cu builds and queries every tree; the passes that are not templates (mq_nodes_kernel, mq_refit_kernel,
+// rv_ball_leaves_kernel, sf_upload_kernel) are defined there, and the other families include this header for its types.
 #pragma once
 #include <type_traits>
 #include "common.cuh"
@@ -109,11 +111,6 @@ struct SfUpload {
 };
 static_assert(sizeof(SfUpload) <= 4096, "within the kernel parameter limit");
 
-__global__ void __launch_bounds__(kThreads) sf_upload_kernel(const SfUpload u) {
-    for (int k = threadIdx.x; k < u.count; k += blockDim.x) u.dst[k] = u.v[k];
-    if (threadIdx.x == 0 && u.dst_src) *u.dst_src = u.src;
-}
-
 template <typename C> __device__ __forceinline__ C sf_div(C a, C b);
 template <> __device__ __forceinline__ float sf_div<float>(float a, float b) { return __fdiv_rn(a, b); }
 template <> __device__ __forceinline__ double sf_div<double>(double a, double b) { return __ddiv_rn(a, b); }
@@ -184,6 +181,18 @@ __device__ __forceinline__ bool sf_box(const T* __restrict__ p, const SfSrc& src
 struct MqScratch {
     int scene[6];                 // ordered-int images of the scene box (min x y z, max x y z)
     unsigned long long bad;       // faces with a corner out of range: left out of the tree, counted for the caller
+};
+
+struct WnNode;   // winding.cuh
+
+// A tree as mesh_query.cu's builder leaves it, in device memory.
+template <typename L>
+struct MeshTree {
+    MqScratch* sc;
+    MqNode* nodes;
+    L* leaves;
+    WnNode* wn;   // far-field data per node (with `moments` only)
+    int* ids;     // surfel leaves: the point id of each leaf
 };
 
 // Leaves in the tree: m less the invalid faces, counted by mq_bounds_kernel (a point tree has none).
@@ -387,23 +396,6 @@ __global__ void __launch_bounds__(kThreads) sf_leaves_kernel(const T* __restrict
     boxes[i] = bx;
 }
 
-// Ball leaf i (i < m - bad): its ball, its face id and its box.
-__global__ void __launch_bounds__(kThreads) rv_ball_leaves_kernel(const double* __restrict__ balls, long long m,
-                                                                  const MqScratch* __restrict__ sc, const MqRec* __restrict__ sorted,
-                                                                  RvBall* __restrict__ leaves, int* __restrict__ ids,
-                                                                  MqBox* __restrict__ boxes) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= m - (long long)sc->bad) return;
-    const long long t = (long long)sorted[i].idx;
-    double a[3], b[3], c[3];
-    mq_leaf_corners<RvBall, double>(balls, 0, nullptr, 0, t, a, b, c);
-    RvBall r;
-    r.c[0] = a[0]; r.c[1] = a[1]; r.c[2] = a[2]; r.r = b[0];
-    leaves[i] = r;
-    ids[i] = (int)t;
-    boxes[i] = mq_leaf_box<RvBall, double>(a, b, c);
-}
-
 // pointcloud_surfel_geometry: surfel i's s + 1 vertices at rows i (s + 1) .. (rim j at + j, the centre at + s), in T
 // (the reference's mixed precision: basis and vertices in T, x0 and y0 in fp32), and its s faces (centre, rim j,
 // rim (j + 1) mod s) at rows i s + j.  One thread per point.
@@ -421,76 +413,6 @@ __global__ void __launch_bounds__(kThreads) sf_geometry_kernel(const T* __restri
     for (int j = 0; j < s; ++j) {
         int* o = out_f + 3 * (i * s + j);
         o[0] = (int)(base + s); o[1] = (int)(base + j); o[2] = (int)(base + (j + 1) % s);
-    }
-}
-
-__device__ __forceinline__ int mq_delta(const MqRec* __restrict__ recs, long long n, long long i, unsigned long long ci, long long j) {
-    if (j < 0 || j >= n) return -1;
-    const unsigned long long cj = recs[j].key[0];
-    return ci == cj ? 64 + __clz((int)(i ^ j)) : __clzll((long long)(ci ^ cj));
-}
-
-// Karras 2012, internal node i of n - 1 (n = valid leaves); node 0 is the root.
-__global__ void __launch_bounds__(kThreads) mq_nodes_kernel(const MqRec* __restrict__ recs, long long m, const MqScratch* __restrict__ sc,
-                                                            MqNode* __restrict__ nodes, int* __restrict__ node_parent,
-                                                            int* __restrict__ leaf_parent) {
-    const long long n = m - (long long)sc->bad;   // < 2^31
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n - 1) return;
-    const unsigned long long ci = recs[i].key[0];
-    const int d = mq_delta(recs, n, i, ci, i + 1) - mq_delta(recs, n, i, ci, i - 1) >= 0 ? 1 : -1;
-    const int dmin = mq_delta(recs, n, i, ci, i - d);
-    long long lmax = 2;
-    while (mq_delta(recs, n, i, ci, i + lmax * d) > dmin) lmax <<= 1;
-    long long l = 0;
-    for (long long t = lmax >> 1; t >= 1; t >>= 1)
-        if (mq_delta(recs, n, i, ci, i + (l + t) * d) > dmin) l += t;
-    const int dnode = mq_delta(recs, n, i, ci, i + l * d);
-    long long s = 0;
-    for (int k = 1; k < 33; ++k) {                 // t = ceil(l / 2^k) down to 1
-        const long long t = (l + (1ll << k) - 1) >> k;
-        if (mq_delta(recs, n, i, ci, i + (s + t) * d) > dnode) s += t;
-        if (t <= 1) break;
-    }
-    const int gamma = (int)(i + s * d) + (d < 0 ? -1 : 0);
-    const int c0 = (d < 0 ? i - l : i) == gamma ? ~gamma : gamma;             // the range's ends are min / max(i, j)
-    const int c1 = (d < 0 ? i : i + l) == gamma + 1 ? ~(gamma + 1) : gamma + 1;
-    nodes[i].c0 = c0;
-    nodes[i].c1 = c1;
-    if (c0 < 0) leaf_parent[~c0] = (int)i; else node_parent[c0] = (int)i;
-    if (c1 < 0) leaf_parent[~c1] = (int)i; else node_parent[c1] = (int)i;
-}
-
-__device__ __forceinline__ MqBox mq_child_box(const MqNode* nodes, const MqBox* boxes, int c) {
-    if (c < 0) return boxes[~c];
-    const float4* p = reinterpret_cast<const float4*>(nodes + c);
-    const float4 q0 = __ldcg(p), q1 = __ldcg(p + 1), q2 = __ldcg(p + 2);   // written by other threads of this launch
-    MqBox b;
-    b.lo[0] = fminf(q0.x, q1.z); b.lo[1] = fminf(q0.y, q1.w); b.lo[2] = fminf(q0.z, q2.x);
-    b.hi[0] = fmaxf(q0.w, q2.y); b.hi[1] = fmaxf(q1.x, q2.z); b.hi[2] = fmaxf(q1.y, q2.w);
-    return b;
-}
-
-// One thread per leaf climbs towards the root; at each node the first arrival stops and the second, which finds both
-// children's boxes complete, writes them into the node.
-__global__ void __launch_bounds__(kThreads) mq_refit_kernel(long long m, const MqScratch* __restrict__ sc, MqNode* nodes,
-                                                            const int* __restrict__ node_parent, const int* __restrict__ leaf_parent,
-                                                            const MqBox* __restrict__ boxes, int* __restrict__ arrivals) {
-    const long long n = m - (long long)sc->bad;
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (n < 2 || i >= n) return;
-    int node = leaf_parent[i];
-    while (true) {
-        __threadfence();
-        if (atomicAdd(&arrivals[node], 1) == 0) return;
-        const int c0 = nodes[node].c0, c1 = nodes[node].c1;
-        const MqBox b0 = mq_child_box(nodes, boxes, c0), b1 = mq_child_box(nodes, boxes, c1);
-        float4* p = reinterpret_cast<float4*>(nodes + node);
-        p[0] = make_float4(b0.lo[0], b0.lo[1], b0.lo[2], b0.hi[0]);
-        p[1] = make_float4(b0.hi[1], b0.hi[2], b1.lo[0], b1.lo[1]);
-        p[2] = make_float4(b1.lo[2], b1.hi[0], b1.hi[1], b1.hi[2]);
-        if (node == 0) return;
-        node = node_parent[node];
     }
 }
 

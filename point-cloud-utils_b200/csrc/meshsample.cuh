@@ -109,47 +109,6 @@ __global__ void __launch_bounds__(kThreads) mesh_area_kernel(const T* __restrict
     }
 }
 
-// The CDF, a multi-CTA inclusive scan of the weights in three launches: each CTA sums its tile of kMeshScanTile faces,
-// one CTA scans those sums, each CTA rescans its tile from its offset.  `cdf` holds the area bits on entry and C on
-// exit (every element is read and rewritten by the same thread).  Integer sums are exact, so the result does not
-// depend on how the scan associates them.
-__global__ void __launch_bounds__(kMeshScanThreads) mesh_cdf_reduce_kernel(const unsigned long long* __restrict__ cdf, long long m,
-                                                                           const MeshScratch* __restrict__ sc,
-                                                                           unsigned long long* __restrict__ tile_sum) {
-    const double s = mesh_weight_scale(sc->max_bits, m);
-    const long long base = (long long)blockIdx.x * kMeshScanTile;
-    const int count = (int)(m - base < kMeshScanTile ? m - base : kMeshScanTile);
-    unsigned long long sum = 0;
-    for (int i = threadIdx.x; i < count; i += kMeshScanThreads) sum += mesh_weight(cdf[base + i], s);
-    unsigned long long total;
-    block_exclusive_scan<kMeshScanThreads, unsigned long long>(sum, &total);
-    if (threadIdx.x == 0) tile_sum[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(1024) mesh_cdf_tiles_kernel(unsigned long long* __restrict__ tile_sum, long long tiles, long long m,
-                                                              const MeshScratch* __restrict__ sc, MeshArea* __restrict__ out) {
-    const unsigned long long W = block_scan_rounds<1024, unsigned long long>(
-        (unsigned)tiles, [&](unsigned b) { return tile_sum[b]; },
-        [&](unsigned b, unsigned long long ex, unsigned long long) { tile_sum[b] = ex; });
-    if (threadIdx.x == 0) {
-        out->total = W;
-        out->scale = mesh_weight_scale(sc->max_bits, m);
-        out->bad = sc->bad;
-    }
-}
-
-__global__ void __launch_bounds__(kMeshScanThreads) mesh_cdf_scan_kernel(unsigned long long* __restrict__ cdf, long long m,
-                                                                         const MeshScratch* __restrict__ sc,
-                                                                         const unsigned long long* __restrict__ tile_offset) {
-    const double s = mesh_weight_scale(sc->max_bits, m);
-    const long long base = (long long)blockIdx.x * kMeshScanTile;
-    const int count = (int)(m - base < kMeshScanTile ? m - base : kMeshScanTile);
-    const unsigned long long off = tile_offset[blockIdx.x];
-    block_scan_rounds<kMeshScanThreads, unsigned long long>(
-        count, [&](int i) { return mesh_weight(cdf[base + i], s); },
-        [&](int i, unsigned long long ex, unsigned long long w) { cdf[base + i] = off + ex + w; });
-}
-
 __device__ __forceinline__ unsigned long long mesh_hash(unsigned long long seed, unsigned long long s, unsigned j) {
     return mix64(mix64(3ull * s + j) ^ seed);
 }

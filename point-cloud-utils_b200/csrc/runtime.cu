@@ -1,5 +1,6 @@
-// runtime.cu -- the shared host runtime (runtime.cuh): error state, launch counting, ordered compaction, the scans of
-// the record sort, and the C entry points of versions, errors, devices, pinned host memory and workspaces.
+// runtime.cu -- the shared host runtime (runtime.cuh): error state, launch counting, ordered compaction, the record sort
+// (sort.cuh) with its kernels, the run heads of sorted one-word records, and the C entry points of versions, errors,
+// devices, pinned host memory and workspaces.
 #include "runtime.cuh"
 #include "compact.cuh"
 
@@ -17,6 +18,86 @@ __global__ void __launch_bounds__(1024) keep_offsets_kernel(unsigned* __restrict
     const unsigned kept = block_scan_rounds<1024>(
         (unsigned)nblocks, [&](unsigned b) { return block_count[b]; }, [&](unsigned b, unsigned ex, unsigned) { block_count[b] = ex; });
     if (threadIdx.x == 0) *out_count = (long long)kept;
+}
+
+template <typename Rec>
+__global__ void __launch_bounds__(kSortThreads) sort_hist_kernel(const Rec* __restrict__ in, long long n, int word, int shift,
+                                                                 unsigned* __restrict__ hist, unsigned ntiles) {
+    __shared__ unsigned h[kSortBins];
+    h[threadIdx.x] = 0u;
+    __syncthreads();
+    const long long base = (long long)blockIdx.x * kSortTile;
+#pragma unroll 4
+    for (int r = 0; r < kSortRounds; ++r) {
+        const long long i = base + r * kSortThreads + threadIdx.x;
+        if (i < n) {
+            const unsigned d = (unsigned)((in[i].key[word] >> shift) & 255u);
+            const unsigned peers = __match_any_sync(__activemask(), d);
+            if ((int)(threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&h[d], (unsigned)__popc(peers));
+        }
+    }
+    __syncthreads();
+    hist[(size_t)threadIdx.x * ntiles + blockIdx.x] = h[threadIdx.x];
+}
+
+template <typename Rec>
+__global__ void __launch_bounds__(kSortThreads) sort_scatter_kernel(const Rec* __restrict__ in, Rec* __restrict__ out, long long n,
+                                                                    int word, int shift, const unsigned* __restrict__ hist,
+                                                                    unsigned ntiles, const unsigned* __restrict__ base,
+                                                                    const int* __restrict__ constant) {
+    const long long tile0 = (long long)blockIdx.x * kSortTile;
+    if (*constant) {                         // the digit is the same everywhere: the pass is the identity
+#pragma unroll 4
+        for (int r = 0; r < kSortRounds; ++r) {
+            const long long i = tile0 + r * kSortThreads + threadIdx.x;
+            if (i < n) store_rec<Rec>(out + i, load_rec<Rec>(in + i));
+        }
+        return;
+    }
+    __shared__ unsigned pos[kSortWarps][kSortBins];
+    for (int j = threadIdx.x; j < kSortWarps * kSortBins; j += kSortThreads) (&pos[0][0])[j] = 0u;
+    __syncthreads();
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const unsigned lt = (1u << lane) - 1u;
+    const long long slice0 = tile0 + (long long)w * (kSortRounds * 32);
+    // 1. this warp's digit counts
+    for (int r = 0; r < kSortRounds; ++r) {
+        const long long i = slice0 + r * 32 + lane;
+        const unsigned d = i < n ? (unsigned)((in[i].key[word] >> shift) & 255u) : 256u + (unsigned)lane;
+        const unsigned peers = __match_any_sync(0xffffffffu, d);
+        if (i < n && (peers & lt) == 0u) pos[w][d] += (unsigned)__popc(peers);
+        __syncwarp();
+    }
+    __syncthreads();
+    // 2. counts -> first global position of each (warp, digit)
+    {
+        const unsigned d = threadIdx.x;
+        unsigned running = base[d] + hist[(size_t)d * ntiles + blockIdx.x];
+#pragma unroll
+        for (int j = 0; j < kSortWarps; ++j) {
+            const unsigned c = pos[j][d];
+            pos[j][d] = running;
+            running += c;
+        }
+    }
+    __syncthreads();
+    // 3. the same walk again, placing the records
+    for (int r = 0; r < kSortRounds; ++r) {
+        const long long i = slice0 + r * 32 + lane;
+        const bool live = i < n;
+        Rec rec;
+        unsigned d = 256u + (unsigned)lane;
+        if (live) { rec = load_rec<Rec>(in + i); d = (unsigned)((rec.key[word] >> shift) & 255u); }
+        const unsigned peers = __match_any_sync(0xffffffffu, d);
+        unsigned dst = 0u;
+        if (live) dst = pos[w][d] + (unsigned)__popc(peers & lt);
+        __syncwarp();
+        if (live) {
+            store_rec<Rec>(out + dst, rec);
+            if ((peers & lt) == 0u) pos[w][d] += (unsigned)__popc(peers);
+        }
+        __syncwarp();
+    }
 }
 
 // grid 256: CTA b turns hist[b][0 .. ntiles) into its exclusive prefix sums and writes the row total.  A row counts
@@ -43,6 +124,12 @@ __global__ void __launch_bounds__(kSortBins) sort_scan_bins(const unsigned long 
     base[threadIdx.x] = (unsigned)before;
     __syncthreads();
     if (threadIdx.x == 0) *constant = any_full;
+}
+
+__global__ void __launch_bounds__(kThreads) mc_heads_kernel(const SortRec<unsigned long long, 1>* __restrict__ recs, long long ns, unsigned char* __restrict__ head) {
+    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= ns) return;
+    head[i] = (i == 0 || recs[i].key[0] != recs[i - 1].key[0]) ? 1 : 0;
 }
 
 }  // namespace pcu
@@ -73,6 +160,36 @@ int enqueue_keep_rows(const unsigned char* keep, long long n, const unsigned* co
     PCU_LAUNCH(keep_rows_kernel<int>, blocks_for(n), kThreads, stream, keep, n, counts, out_idx);
     return PCU_B200_OK;
 }
+
+template <typename Rec>
+int radix_sort_records(const SortScratch<Rec>& s, long long n, int words, cudaStream_t stream, Rec** sorted, int key_bits) {
+    const unsigned ntiles = SortScratch<Rec>::tiles(n);
+    const int bits = key_bits > 0 ? key_bits : (int)sizeof(s.a->key[0]) * 8;
+    Rec *in = s.a, *out = s.b;
+    for (int w = words - 1; w >= 0; --w)          // least significant word first
+        for (int shift = 0; shift < bits; shift += 8) {
+            PCU_LAUNCH((sort_hist_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, n, w, shift, s.hist, ntiles);
+            PCU_LAUNCH(sort_scan_rows, kSortBins, kSortThreads, stream, s.hist, ntiles, s.totals);
+            PCU_LAUNCH(sort_scan_bins, 1, kSortBins, stream, (const unsigned long long*)s.totals, n, s.base, s.constant);
+            PCU_LAUNCH((sort_scatter_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, out, n, w, shift, (const unsigned*)s.hist,
+                       ntiles, (const unsigned*)s.base, (const int*)s.constant);
+            std::swap(in, out);
+        }
+    *sorted = in;
+    return PCU_B200_OK;
+}
+
+// The record types in use: decimation's and orientation's half-edges (unsigned, 2), orientation's with 64-bit faces
+// (unsigned long long, 2), the trees, grids and incidences (unsigned long long, 1), duplicate removal (unsigned and
+// unsigned long long, 3).
+#define PCU_SORT_RECORDS(K, NW) \
+    template int radix_sort_records(const SortScratch<SortRec<K, NW>>&, long long, int, cudaStream_t, SortRec<K, NW>**, int);
+PCU_SORT_RECORDS(unsigned, 2)
+PCU_SORT_RECORDS(unsigned long long, 2)
+PCU_SORT_RECORDS(unsigned long long, 1)
+PCU_SORT_RECORDS(unsigned, 3)
+PCU_SORT_RECORDS(unsigned long long, 3)
+#undef PCU_SORT_RECORDS
 
 }  // namespace pcu_internal
 

@@ -1,7 +1,8 @@
 // runtime.cuh -- the host runtime that every family of the library shares (internal, not installed): error state and
 // launch counting, the launch macros, the workspace and its scratch blocks, the device guard, stream hand-over,
 // ordered compaction, the record sort and host-to-device staging.  Each family's translation unit (nearest.cu,
-// point_ops.cu, pcu_b200.cu) includes it; runtime.cu defines what it declares, and the workspace's C entry points.
+// point_ops.cu, mesh_query.cu, voronoi.cu, voxels.cu, mesh_topology.cu, decimate.cu) includes it; runtime.cu defines
+// what it declares, and the workspace's C entry points.
 //
 // A function that one translation unit calls in another lives in namespace pcu_internal and is declared here;
 // everything else stays in its file's anonymous namespace.  pcu_internal has hidden visibility: the library exports
@@ -33,6 +34,14 @@ namespace pcu {
 
 // Compiled in nearest.cu (kdreplay.cuh); duplicate removal launches it too.
 __global__ void widen_counter_kernel(const unsigned* src, long long* dst);
+
+// Compiled in runtime.cu: head[i] = 1 where sorted one-word record i starts a run of equal keys.  Marching cubes, the
+// sparse voxel grids, voxelization and the Laplacian's assembly launch it.
+__global__ void mc_heads_kernel(const SortRec<unsigned long long, 1>* recs, long long ns, unsigned char* head);
+
+// Defined in meshquery.cuh and mesh_query.cu; the declarations below only refer to them.
+template <typename L> struct MeshTree;
+struct RvBall;
 
 }  // namespace pcu
 
@@ -266,24 +275,10 @@ struct SortScratch {
 
 // Stable LSD radix sort of the `n` records in s.a between the two buffers; returns the buffer holding the sorted records.
 // key_bits > 0: only the low key_bits bits of each key word can be non-zero, and the passes over the bytes above them
-// are skipped.
+// are skipped.  Compiled in runtime.cu, with its kernels, for the record types in use: SortRec<unsigned, 2>,
+// <unsigned long long, 2>, <unsigned long long, 1>, <unsigned, 3> and <unsigned long long, 3>.
 template <typename Rec>
-int radix_sort_records(const SortScratch<Rec>& s, long long n, int words, cudaStream_t stream, Rec** sorted, int key_bits = 0) {
-    const unsigned ntiles = SortScratch<Rec>::tiles(n);
-    const int bits = key_bits > 0 ? key_bits : (int)sizeof(s.a->key[0]) * 8;
-    Rec *in = s.a, *out = s.b;
-    for (int w = words - 1; w >= 0; --w)          // least significant word first
-        for (int shift = 0; shift < bits; shift += 8) {
-            PCU_LAUNCH((sort_hist_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, n, w, shift, s.hist, ntiles);
-            PCU_LAUNCH(sort_scan_rows, kSortBins, kSortThreads, stream, s.hist, ntiles, s.totals);
-            PCU_LAUNCH(sort_scan_bins, 1, kSortBins, stream, (const unsigned long long*)s.totals, n, s.base, s.constant);
-            PCU_LAUNCH((sort_scatter_kernel<Rec>), ntiles, kSortThreads, stream, (const Rec*)in, out, n, w, shift, (const unsigned*)s.hist,
-                       ntiles, (const unsigned*)s.base, (const int*)s.constant);
-            std::swap(in, out);
-        }
-    *sorted = in;
-    return PCU_B200_OK;
-}
+int radix_sort_records(const SortScratch<Rec>& s, long long n, int words, cudaStream_t stream, Rec** sorted, int key_bits = 0);
 
 // ---- what the mesh, voxel and topology families share: count records and stream-ordered handles
 // Copies a count record to the host and waits for it: one synchronisation of `stream`.
@@ -301,6 +296,15 @@ inline int bad_corners(unsigned long long bad) {
 
 // Whether face indices of this kind are 64 bits wide.
 inline bool wide_index(int kind) { return kind & 1; }
+
+// The input check of every call on a mesh (v, f): sampling, queries, rays, restricted Voronoi.
+inline int mesh_check(const void* v, long long nv, const void* f, long long m, int fkind) {
+    if (!v || !f || nv <= 0 || m <= 0)
+        return fail(PCU_B200_INVALID_ARGUMENT, "Invalid input mesh with zero elements: v and f must have shape (n, 3) and (m, 3) (n, m > 0)");
+    if (m > 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "mesh sampling: at most 2^31 - 1 faces, got %lld", m);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    return PCU_B200_OK;
+}
 
 // A handle's block, allocated in the order of `stream`; `what` names the handle's feature when that fails.
 inline int alloc_block(unsigned char*& block, size_t bytes, cudaStream_t stream, const char* what) {
@@ -324,6 +328,15 @@ int prepare_handle(pcu_b200_workspace* ws, cudaStream_t stream, H** out, Build&&
     const int st = build(h);
     if (st != PCU_B200_OK) { delete h; return st; }
     *out = h;
+    return PCU_B200_OK;
+}
+
+// The C destroy of a stream-ordered handle: its blocks are released in the order of its stream, on its device.
+template <class H>
+int destroy_handle(H* h) {
+    if (!h) return PCU_B200_OK;
+    DeviceGuard guard(h->device);
+    delete h;
     return PCU_B200_OK;
 }
 
@@ -367,5 +380,27 @@ int knn_device(pcu_b200_workspace* ws, const T* query, long long n, const T* dat
 template <typename T>
 int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, double radius, unsigned seed, int* out_idx,
                         long long* out_count, int* out_rounds, cudaStream_t stream);
+
+// ---- what mesh_query.cu offers the other families: the fp64 closest-point tree (watertight remeshing's projection), the
+// ball tree (restricted Voronoi cells) and sampled positions (the initial sample of sample_mesh_lloyd)
+// Bytes of the block build_closest_tree builds the tree of m faces into.
+size_t closest_tree_bytes(long long m);
+
+// The closest-point tree of the mesh (v, nv, f, m, fkind), its build's temporaries in the arena and the tree itself in
+// `block`; the count of faces with a corner out of range lands in *out_bad (device memory).
+int build_closest_tree(pcu_b200_workspace* ws, const double* v, long long nv, const void* f, long long m, int fkind,
+                       unsigned long long* out_bad, unsigned char* block, MeshTree<Pt<double>>& tree, cudaStream_t stream);
+
+// The closest points on the tree's m faces of the n points q: distances, int64 face indices and barycentric coordinates.
+int enqueue_closest_points(pcu_b200_workspace* ws, const MeshTree<Pt<double>>& tree, long long m, const double* q, long long n,
+                           double* out_d, long long* out_fidx, double* out_bc, cudaStream_t stream);
+
+// The tree over the (m, 4) balls, built in the arena together with its build's temporaries.
+int build_ball_tree(pcu_b200_workspace* ws, const double* balls, long long m, MeshTree<RvBall>& tree, cudaStream_t stream);
+
+// The fp64 positions of the first n samples of sample_mesh_random at `seed` into x.  The face CDF lives in kMesh; its
+// record is read (one synchronisation), and faces out of range or a zero area fail the call.
+int sample_mesh_positions(pcu_b200_workspace* ws, const double* v, long long nv, const void* f, long long m, int fkind, long long n,
+                          unsigned seed, double* x, cudaStream_t stream);
 
 }  // namespace pcu_internal

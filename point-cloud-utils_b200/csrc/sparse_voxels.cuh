@@ -6,7 +6,7 @@
 //   mc_classify_kernel   case byte of every cube, bad-index count, slots and triangles per CTA tile
 //   mc_tiles_kernel      one CTA: exclusive scans of the tile totals -> first slot and first face of every tile
 //   mc_slots_kernel      per slot the record {key = (min corner << b) | max corner, slot}, sorted by sort.cuh
-//   mc_heads_kernel      run heads of the sorted keys (keep_count / keep_offsets number them: one run per vertex)
+//   mc_heads_kernel      (runtime.cu) run heads of the sorted keys (keep_count / keep_offsets number them: one run per vertex)
 //   mc_runs_kernel       per slot its run; the run head (the run's smallest slot: the sort is stable) owns the run
 //   mc_owner_kernel      the owners, counted in slot order (keep_count / keep_offsets), give each run its vertex id
 //   mc_emit_kernel       owners write their vertex, cubes their faces
@@ -157,12 +157,6 @@ __global__ void __launch_bounds__(kThreads) mc_slots_kernel(const void* __restri
             ++s;
         }
     }
-}
-
-__global__ void __launch_bounds__(kThreads) mc_heads_kernel(const McRec* __restrict__ recs, long long ns, unsigned char* __restrict__ head) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= ns) return;
-    head[i] = (i == 0 || recs[i].key[0] != recs[i - 1].key[0]) ? 1 : 0;
 }
 
 // After keep_count / keep_offsets over `head`: run of every sorted record = heads at or before it, minus one.
