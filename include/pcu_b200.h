@@ -530,6 +530,12 @@ int pcu_b200_ray_mesh_intersection_prepared_f64(pcu_b200_workspace* ws, const pc
  *   pointcloud_surfel_geometry: the fans as a mesh: out_v ((s + 1) np rows, rim j of point i at i (s + 1) + j, the
  *     centre at i (s + 1) + s) in p's precision, and out_f (s np rows (centre, rim j, rim (j + 1) mod s)) int32;
  *     (s + 1) np must be below 2^31 - 1.
+ *   pointcloud_sphere_geometry ("sphere" geometry, make_sphere_geometry): a UV sphere of radius r[i] around p[i] with
+ *     num_stacks >= 1 latitudinal and num_slices >= 1 longitudinal divisions.  V = (stacks + 1)(slices + 1) vertices per
+ *     point in p's precision, vertex (a, b) at row i V + a (slices + 1) + b, and F = 2 (stacks - 1) slices int32 faces per
+ *     point at rows i F .., in the reference's loop order; poles and seam duplicated.  Coordinates are computed in fp64
+ *     without contraction from cos and sin of the reference's angles (C library, on the host) and rounded once to p's
+ *     type (DESIGN.md §3).  V np must be below 2^31 - 1; np = 0 does nothing.
  * Every array pointer is a DEVICE pointer and the calls are stream-ordered. */
 int pcu_b200_ray_surfel_intersection_f32(pcu_b200_workspace* ws, const float* p, const float* n, const float* r, int64_t np, int subdivs,
                                          const float* o, int o_stride, const float* d, int64_t nr, float near, float far, int32_t* out_pid,
@@ -551,6 +557,10 @@ int pcu_b200_pointcloud_surfel_geometry_f32(pcu_b200_workspace* ws, const float*
                                             float* out_v, int32_t* out_f, void* stream);
 int pcu_b200_pointcloud_surfel_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np,
                                             int subdivs, double* out_v, int32_t* out_f, void* stream);
+int pcu_b200_pointcloud_sphere_geometry_f32(pcu_b200_workspace* ws, const float* p, const float* r, int64_t np, int num_stacks,
+                                            int num_slices, float* out_v, int32_t* out_f, void* stream);
+int pcu_b200_pointcloud_sphere_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* r, int64_t np, int num_stacks,
+                                            int num_slices, double* out_v, int32_t* out_f, void* stream);
 
 /* ---- marching cubes on a sparse voxel grid and the grid's boundary ---------------------------------------------------
  * Replace marching_cubes_sparse_voxel_grid (src/marching_cubes.cpp:35-85) and sparse_voxel_grid_boundary
@@ -728,6 +738,15 @@ int pcu_b200_decimate_triangle_mesh_destroy(pcu_b200_decimate* dc);
  *     rows, consistently oriented within each patch (faces joined by edges that no third face has), and
  *     out_components (nf) each face's patch, patch j being the j-th in ascending order of its smallest face; both in
  *     f's width.  Never synchronises `stream`.
+ *   adjacency_list_prepare (the reference's src/adjacency_list.cpp, libigl's adjacency_list): f (nf, 3) of any index
+ *     kind, 1 <= nf <= 357913941 (6 nf directed edges fit int32 ranks).  List i of the n = max(f) + 1 lists holds, in
+ *     ascending order and once each, every vertex that shares a face with i, and i itself when some face names i at
+ *     two or more corners; an index no face names has an empty list.  Synchronises `stream` twice: once to read max(f),
+ *     once to read the entry count nnz.  *out_counts = {n, nnz} (host int64).  An entry of f that is negative or above
+ *     2^31 - 2 fails with PCU_B200_INVALID_ARGUMENT.  *out_adj (f need not outlive prepare) is freed by
+ *     adjacency_list_destroy, stream-ordered on the stream it was prepared on.
+ *   adjacency_list_emit: writes out_offsets (n + 1) and out_neighbors (nnz) in f's width: list i is
+ *     out_neighbors[out_offsets[i] .. out_offsets[i + 1]).
  * Every array pointer is a DEVICE pointer. */
 typedef struct pcu_b200_components pcu_b200_components;
 int pcu_b200_connected_components_prepare(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_cols, int f_kind,
@@ -747,6 +766,11 @@ int pcu_b200_remove_unreferenced_mesh_vertices_f64(pcu_b200_workspace* ws, const
                                                    void* stream);
 int pcu_b200_orient_mesh_faces(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, void* out_f, void* out_components,
                                void* stream);
+typedef struct pcu_b200_adjacency pcu_b200_adjacency;
+int pcu_b200_adjacency_list_prepare(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, pcu_b200_adjacency** out_adj,
+                                    int64_t out_counts[2], void* stream);
+int pcu_b200_adjacency_list_emit(pcu_b200_workspace* ws, const pcu_b200_adjacency* adj, void* out_offsets, void* out_neighbors, void* stream);
+int pcu_b200_adjacency_list_destroy(pcu_b200_adjacency* adj);
 
 /* ---- mesh normals, face areas and Laplacian smoothing ------------------------------------------------------------
  * Replace mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals and laplacian_smooth_mesh (the

@@ -43,12 +43,13 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "sample_mesh_random", "sample_mesh_poisson_disk", "interpolate_barycentric_coords", "closest_points_on_mesh",
            "triangle_soup_fast_winding_number", "point_cloud_fast_winding_number", "signed_distance_to_mesh",
            "ray_mesh_intersection", "RayMeshIntersector",
-           "ray_surfel_intersection", "RaySurfelIntersector", "pointcloud_surfel_geometry",
+           "ray_surfel_intersection", "RaySurfelIntersector", "pointcloud_surfel_geometry", "pointcloud_sphere_geometry",
            "marching_cubes_sparse_voxel_grid", "sparse_voxel_grid_boundary",
            "sparse_voxel_grid_from_pointcloud", "dilate_sparse_voxel_grid", "erode_sparse_voxel_grid",
            "sparse_voxel_grid_to_hex_mesh",
            "voxelize_triangle_mesh", "flood_fill_3d", "voxel_grid_geometry", "make_mesh_watertight", "decimate_triangle_mesh",
            "connected_components", "remove_mesh_vertices", "remove_unreferenced_mesh_vertices", "orient_mesh_faces",
+           "adjacency_list",
            "mesh_face_areas", "estimate_mesh_face_normals", "estimate_mesh_vertex_normals", "laplacian_smooth_mesh",
            "deduplicate_point_cloud", "voronoi_centroids_unit_cube", "lloyd_3d", "lloyd_2d",
            "sample_mesh_lloyd",
@@ -727,7 +728,8 @@ from ._mesh_sampling import sample_mesh_random, sample_mesh_poisson_disk, interp
 from ._mesh_query import (closest_points_on_mesh, triangle_soup_fast_winding_number,  # noqa: E402
                           point_cloud_fast_winding_number, signed_distance_to_mesh)
 from ._ray_mesh import ray_mesh_intersection, RayMeshIntersector  # noqa: E402
-from ._ray_surfel import ray_surfel_intersection, RaySurfelIntersector, pointcloud_surfel_geometry  # noqa: E402
+from ._ray_surfel import (ray_surfel_intersection, RaySurfelIntersector, pointcloud_surfel_geometry,  # noqa: E402
+                          pointcloud_sphere_geometry)
 from ._sparse_voxels import marching_cubes_sparse_voxel_grid, sparse_voxel_grid_boundary  # noqa: E402
 from ._sparse_voxels import (sparse_voxel_grid_from_pointcloud, dilate_sparse_voxel_grid, erode_sparse_voxel_grid,  # noqa: E402
                              sparse_voxel_grid_to_hex_mesh)
@@ -735,7 +737,7 @@ from ._voxels import voxelize_triangle_mesh, flood_fill_3d, voxel_grid_geometry 
 from ._watertight import make_mesh_watertight  # noqa: E402
 from ._decimate import decimate_triangle_mesh  # noqa: E402
 from ._mesh_topology import (connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices,  # noqa: E402
-                             orient_mesh_faces)
+                             orient_mesh_faces, adjacency_list)
 from ._mesh_geometry import mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals, laplacian_smooth_mesh  # noqa: E402
 
 

@@ -128,6 +128,18 @@ def _matrix_shape(a):
     return (s[0], 1) if len(s) == 1 else (s if len(s) == 2 else (int(_np.prod(s)), 1))
 
 
+def _validate_mesh_faces(f):
+    """validate_mesh_faces (src/common/common.h:112-127) on the matrix the binding sees; returns its row count."""
+    rows, cols = _matrix_shape(f)
+    if rows == 0:
+        raise ValueError("Invalid input faces with zero elements: f must have shape (n, 3) where n > 0. Got f.shape =(%d, %d)."
+                         % (rows, cols))
+    if cols != 3:
+        raise ValueError("Only triangle inputs are supported: f must have shape (n, 3) where n > 0. Got f.shape =(%d, %d)."
+                         % (rows, cols))
+    return rows
+
+
 def _to_device(arrays, device):
     """numpy arrays -> contiguous CUDA tensors on the device= of the call (one upload each).  Unsigned index arrays
     travel as the signed type of their width (the kernels take the kind separately)."""

@@ -1,14 +1,15 @@
-"""connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices and orient_mesh_faces -- the
-reference's names, arguments and outputs (the reference's src/connected_components.cpp, src/remove_mesh_vertices.cpp,
-src/remove_unreferenced_mesh_vertices.cpp and src/orient_mesh_faces.cpp), computed by csrc/mesh_topology.cuh and
-csrc/orient.cuh.
+"""connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices, orient_mesh_faces and adjacency_list
+-- the reference's names, arguments and outputs (the reference's src/connected_components.cpp,
+src/remove_mesh_vertices.cpp, src/remove_unreferenced_mesh_vertices.cpp, src/orient_mesh_faces.cpp and
+src/adjacency_list.cpp), computed by csrc/mesh_topology.cuh, csrc/orient.cuh and csrc/laplacian.cuh.
 
 numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA torch tensors in -> CUDA tensors out;
 CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages and in its order, before any
 device call.  Shapes are the reference's through npe::move, which squeezes them as numpy does: an (m, 1) result is
 (m,), a single entry is a 0-d array and a single (1, 3) row is (3,)."""
 from . import _pcu_internal
-from ._call import _INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _matrix_shape, _run, _torch, _validate_mesh
+from ._call import (_INDEX_KINDS, _check_float, _check_index, _dtype_name, _form, _matrix_shape, _run, _torch, _validate_mesh,
+                    _validate_mesh_faces)
 
 _MAX_ROWS = 2 ** 31 - 1
 
@@ -190,13 +191,7 @@ def orient_mesh_faces(f, weighting_type="uniform", *, device=None):
     _check_index(f, "f", _INDEX_KINDS)
     if len(f.shape) not in (1, 2):
         raise ValueError("orient_mesh_faces: f must be a 1-D or 2-D array, got shape %s" % (tuple(f.shape),))
-    rows, cols = _matrix_shape(f)
-    if rows == 0:
-        raise ValueError("Invalid input faces with zero elements: f must have shape (n, 3) where n > 0. Got f.shape =(%d, %d)."
-                         % (rows, cols))
-    if cols != 3:
-        raise ValueError("Only triangle inputs are supported: f must have shape (n, 3) where n > 0. Got f.shape =(%d, %d)."
-                         % (rows, cols))
+    rows = _validate_mesh_faces(f)
     if rows > _MAX_ORIENT_FACES:
         raise ValueError("orient_mesh_faces: at most 2^30 - 1 faces are supported, got %d" % rows)
     torch = _torch()
@@ -209,3 +204,55 @@ def orient_mesh_faces(f, weighting_type="uniform", *, device=None):
         return out_f, out_c
 
     return _run(form, [f], device, body, index=(f, [0, 1]), squeeze=True)
+
+
+_MAX_ADJACENCY_FACES = (2 ** 31 - 1) // 6
+
+
+def adjacency_list(f, *, return_csr=False, device=None):
+    """
+    Compute the adjacency list given a set of mesh faces.
+
+    Args:
+        f : \\#f by 3 Matrix of face (triangle) indices
+        return_csr : (keyword only, not in the reference) return the lists as two flat arrays instead of Python lists
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        adj_list : a list of lists such that adj_list[i] contains the indexes of vertices adjacent to vertex i
+        or, with return_csr=True, (offsets, neighbors): arrays in f's dtype and form of shape (n + 1,) and
+            (offsets[-1],), list i being neighbors[offsets[i]:offsets[i + 1]]; a CUDA input gives CUDA tensors on its
+            device, ready for torch's or scipy's sparse constructors
+
+    Dtypes: f int32 / int64.  Defined in DESIGN.md §3 as libigl's adjacency_list(F, A, sorted=false) computes it: there
+    are n = max(f) + 1 lists (not #v: there is no v); every face (a, b, c) adds a<->b, b<->c and c<->a in both
+    directions, and each list is then sorted ascending without duplicates.  So list i holds every vertex that shares a
+    face with i, i itself when some face names i at two or more corners, and an index no face names gets an empty
+    list.  The default result holds Python ints whatever f's form; both results come from one device computation.
+    Divergences: a negative index or an index above 2^31 - 2 raises ValueError (in the reference the outcome depends on
+    the other indices), and so do more than 357913941 faces.
+    """
+    form = _form([f], ["f"])
+    _check_index(f, "f", {"int32": 0, "int64": 1})
+    if len(f.shape) not in (1, 2):
+        raise ValueError("adjacency_list: f must be a 1-D or 2-D array, got shape %s" % (tuple(f.shape),))
+    rows = _validate_mesh_faces(f)
+    if rows > _MAX_ADJACENCY_FACES:
+        raise ValueError("adjacency_list: at most %d faces are supported, got %d" % (_MAX_ADJACENCY_FACES, rows))
+    torch = _torch()
+
+    def body(ft, dev, stream):
+        handle, n, nnz = _pcu_internal._adjacency_list_prepare_device(ft.data_ptr(), rows, _INDEX_KINDS[_dtype_name(f)], dev, stream)
+        try:
+            offsets = torch.empty(n + 1, dtype=ft.dtype, device=ft.device)
+            neighbors = torch.empty(nnz, dtype=ft.dtype, device=ft.device)
+            _pcu_internal._adjacency_list_emit_device(handle, offsets.data_ptr(), neighbors.data_ptr(), dev, stream)
+        finally:
+            _pcu_internal._adjacency_list_destroy(handle)
+        return offsets, neighbors
+
+    offsets, neighbors = _run(form, [f], device, body, index=(f, [0, 1]))
+    if return_csr:
+        return offsets, neighbors
+    o, nb = offsets.tolist(), neighbors.tolist()
+    return [nb[o[i]:o[i + 1]] for i in range(len(o) - 1)]

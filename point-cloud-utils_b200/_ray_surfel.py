@@ -1,6 +1,7 @@
-"""ray_surfel_intersection, RaySurfelIntersector and pointcloud_surfel_geometry -- the reference's names, arguments and
-outputs (the reference's src/ray_point_cloud_intersection.cpp, point_cloud_utils/_ray_point_cloud_intersector.py and
-_point_cloud_geometry.py), computed by csrc/raycast.cuh on the surfel tree of csrc/meshquery.cuh.
+"""ray_surfel_intersection, RaySurfelIntersector, pointcloud_surfel_geometry and pointcloud_sphere_geometry -- the
+reference's names, arguments and outputs (the reference's src/ray_point_cloud_intersection.cpp,
+point_cloud_utils/_ray_point_cloud_intersector.py and _point_cloud_geometry.py), computed by csrc/raycast.cuh on the
+surfel tree of csrc/meshquery.cuh, and by the geometry kernels of csrc/meshquery.cuh.
 
 Input forms and validation follow _call.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
@@ -229,3 +230,60 @@ def pointcloud_surfel_geometry(p, n, r=0.1, subdivs=7, *, device=None):
         return v, f
 
     return _run(form, [p, n, _radius_like(r, p, form)], device, body)
+
+
+def pointcloud_sphere_geometry(p, r, num_stacks, num_slices, *, device=None):
+    """
+    Generate sphere geometry for a point cloud (i.e. one sphere per point)
+
+    Args:
+        p : \\#p by 3 array of vertex positions (each row is a vertex) (float32 / float64)
+        r : Array or Scalar describing the radius along each axis (Either one radius per vertex, or a global size for
+            the whole point cloud); cast to p's dtype
+        num_stacks : Number of latitudal subdivisions (at least 1)
+        num_slices : Number of longitudal subdivisions (at least 1)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        verts : an array of shape (#p * V, 3) (p's dtype), V = (num_stacks + 1)(num_slices + 1): point i's vertex
+                (a, b) at row i V + a (num_slices + 1) + b
+        faces : an int32 array of shape (#p * F, 3) indexing into verts, F = 2 (num_stacks - 1) num_slices
+
+    The reference's generate_splat_geometry ("sphere", make_sphere_geometry) for each point, defined in DESIGN.md §3:
+    stack a at angle pi / 2 - a (pi / num_stacks) and sector b at angle b (2 pi / num_slices), both in fp64, with the
+    C library's cos and sin; xy = r cos(stack), z = r sin(stack), x = xy cos(sector), y = xy sin(sector), and each
+    coordinate (p's type)(p_k + x_k) with the sum in fp64 (so float32 p rounds twice).  Faces per sector, stack by
+    stack: (k1 + 1, k2, k2 + 1) on the first stack, (k1, k2, k1 + 1) on the last, both in that order in between.  The
+    poles and the seam are duplicated, as in the reference.  Zero points give empty (0, 3) arrays.
+    Divergences: num_stacks or num_slices below 1 raise ValueError (the reference sizes its faces negatively or writes
+    NaN vertices), and so does a p that is not (n, 3); more than 2^31 - 2 vertices in all raise ValueError, where the
+    reference's int indices would overflow.
+    """
+    r = _validate_radius(p, r)
+    form = _form([p], ["p"])
+    _check_float(p, "v")
+    if len(p.shape) != 2 or p.shape[1] != 3:
+        raise ValueError("Only 3D inputs are supported: p must have shape (n, 3). Got p.shape = %s." % (tuple(p.shape),))
+    stacks, slices = int(num_stacks), int(num_slices)
+    if stacks < 1 or slices < 1:
+        raise ValueError("pointcloud_sphere_geometry: num_stacks and num_slices must be at least 1, got %d and %d" % (stacks, slices))
+    torch = _torch()
+    m = int(p.shape[0])
+    if m == 0:
+        if form == "numpy":
+            return np.zeros((0, 3), dtype=p.dtype), np.zeros((0, 3), dtype=np.int32)
+        if form == "cuda":
+            _same_device(p, device)
+        return torch.zeros((0, 3), dtype=p.dtype, device=p.device), torch.zeros((0, 3), dtype=torch.int32, device=p.device)
+    nvp, nfp = (stacks + 1) * (slices + 1), 2 * (stacks - 1) * slices
+    if m * nvp >= 2 ** 31 - 1:
+        raise ValueError("pointcloud_sphere_geometry: int32 faces index at most 2^31 - 2 vertices, got %d points of %d" % (m, nvp))
+
+    def body(pt, rt, dev, stream):
+        v = torch.empty((m * nvp, 3), dtype=pt.dtype, device=pt.device)
+        f = torch.empty((m * nfp, 3), dtype=torch.int32, device=pt.device)
+        _pcu_internal._sphere_geometry_device(pt.dtype == torch.float64, pt.data_ptr(), rt.data_ptr(), m, stacks, slices, v.data_ptr(),
+                                              f.data_ptr(), dev, stream)
+        return v, f
+
+    return _run(form, [p, _radius_like(r, p, form)], device, body)

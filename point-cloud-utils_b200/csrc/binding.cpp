@@ -735,6 +735,17 @@ py::tuple connected_components_prepare_device(uintptr_t f, int64_t nf, int f_col
     });
     return py::make_tuple((uintptr_t)cc, counts[0], counts[1]);
 }
+// Adjacency lists (adjacency_list, _mesh_topology.py): validates f and builds the CSR (two synchronisations of `stream`),
+// returns (handle, n = max(f) + 1, nnz); _adjacency_list_emit writes the offsets and neighbours in f's width;
+// _adjacency_list_destroy.
+py::tuple adjacency_list_prepare_device(uintptr_t f, int64_t nf, int f_kind, int device, uintptr_t stream) {
+    pcu_b200_adjacency* adj = nullptr;
+    int64_t counts[2] = {0, 0};
+    on_workspace(device, stream, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
+        return pcu_b200_adjacency_list_prepare(ws, (const void*)f, nf, f_kind, &adj, counts, (void*)stream);
+    });
+    return py::make_tuple((uintptr_t)adj, counts[0], counts[1]);
+}
 // remove_mesh_vertices: out_v (capacity nv rows), out_f (capacity nf rows, f's width); one synchronisation; returns
 // (kept vertices, kept faces).
 py::tuple remove_mesh_vertices_device(bool is_f64, uintptr_t v, int64_t nv, uintptr_t f, int64_t nf, int f_kind, uintptr_t mask,
@@ -1114,6 +1125,7 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_ray_surfel_prepared_device",
             forward_to(pcu_b200_ray_surfel_intersection_prepared_f32, pcu_b200_ray_surfel_intersection_prepared_f64).pair());
     mod.def("_surfel_geometry_device", forward_to(pcu_b200_pointcloud_surfel_geometry_f32, pcu_b200_pointcloud_surfel_geometry_f64).pair());
+    mod.def("_sphere_geometry_device", forward_to(pcu_b200_pointcloud_sphere_geometry_f32, pcu_b200_pointcloud_sphere_geometry_f64).pair());
     mod.def("_interpolate_barycentric_device", &interpolate_barycentric_device);
     mod.def("_marching_cubes_prepare_device", &marching_cubes_prepare_device);
     mod.def("_marching_cubes_emit_device", forward_to(pcu_b200_marching_cubes_emit).single());
@@ -1142,6 +1154,9 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_remove_mesh_vertices_device", &remove_mesh_vertices_device);
     mod.def("_remove_unreferenced_device", &remove_unreferenced_device);
     mod.def("_orient_mesh_faces_device", forward_to(pcu_b200_orient_mesh_faces).single());
+    mod.def("_adjacency_list_prepare_device", &adjacency_list_prepare_device);
+    mod.def("_adjacency_list_emit_device", forward_to(pcu_b200_adjacency_list_emit).single());
+    mod.def("_adjacency_list_destroy", destroy(pcu_b200_adjacency_list_destroy));
     mod.def("_mesh_face_device", &mesh_face_device);
     mod.def("_mesh_vertex_normals_device", forward_to(pcu_b200_mesh_vertex_normals_f32, pcu_b200_mesh_vertex_normals_f64).pair());
     mod.def("_laplacian_smooth_device", &laplacian_smooth_device);

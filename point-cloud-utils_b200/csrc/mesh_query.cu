@@ -1,6 +1,6 @@
 // mesh_query.cu -- mesh sampling and barycentric interpolation, closest points, winding numbers of meshes and oriented
-// point clouds, signed distances, and rays against meshes and surfels (meshsample.cuh, meshquery.cuh, winding.cuh,
-// raycast.cuh): launch sequencing and C entry points.  It owns the tree builder and offers the other mesh families
+// point clouds, signed distances, rays against meshes and surfels, and the surfel and sphere geometry of point clouds
+// (meshsample.cuh, meshquery.cuh, winding.cuh, raycast.cuh): launch sequencing and C entry points.  It owns the tree builder and offers the other mesh families
 // (runtime.cuh) the fp64 closest-point tree, the ball tree of restricted Voronoi cells and the sampling CDF's positions.
 #include "runtime.cuh"
 #include "meshsample.cuh"
@@ -692,6 +692,50 @@ int surfel_geometry_device(pcu_b200_workspace* ws, const T* p, const T* nrm, con
     return PCU_B200_OK;
 }
 
+// The sphere table of DESIGN.md §3, as the reference computes its angles in fp64: t[a] = cos(pi / 2 - a (pi / stacks))
+// and t[stacks + 1 + a] = sin of it for a = 0 .. stacks, then cos and sin of b (2 pi / slices) for b = 0 .. slices, from
+// the C library.
+void sphere_table(int stacks, int slices, double* t) {
+    const double stack_step = M_PI / stacks, sector_step = 2 * M_PI / slices;
+    for (int a = 0; a <= stacks; ++a) {
+        const double angle = M_PI / 2 - a * stack_step;
+        t[a] = std::cos(angle);
+        t[stacks + 1 + a] = std::sin(angle);
+    }
+    double* u = t + 2 * ((size_t)stacks + 1);
+    for (int b = 0; b <= slices; ++b) {
+        const double angle = b * sector_step;
+        u[b] = std::cos(angle);
+        u[slices + 1 + b] = std::sin(angle);
+    }
+}
+
+// pointcloud_sphere_geometry: (stacks + 1)(slices + 1) m vertices in T and 2 (stacks - 1) slices m int32 faces.
+template <typename T>
+int sphere_geometry_device(pcu_b200_workspace* ws, const T* p, const T* r, long long m, int stacks, int slices, T* out_v, int* out_f,
+                           cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (m < 0) return fail(PCU_B200_INVALID_ARGUMENT, "sphere geometry: negative point count %lld", m);
+    if (stacks < 1 || slices < 1)
+        return fail(PCU_B200_INVALID_ARGUMENT, "sphere geometry: num_stacks and num_slices must be at least 1, got %d and %d", stacks, slices);
+    const long long V = ((long long)stacks + 1) * ((long long)slices + 1), F = 2 * ((long long)stacks - 1) * slices;
+    if (m > 0 && (m >= INT_MAX || V >= INT_MAX || m * V >= INT_MAX))
+        return fail(PCU_B200_INVALID_ARGUMENT, "sphere geometry: int32 faces index at most 2^31 - 2 vertices, got %lld points of %lld", m, V);
+    if (m > 0 && (!p || !r || !out_v || (F > 0 && !out_f))) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    PCU_ON_DEVICE(ws);
+    if (m == 0) return PCU_B200_OK;
+    const size_t entries = 2 * ((size_t)stacks + 1) + 2 * ((size_t)slices + 1);
+    double* tab = nullptr;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) { tab = cv.take<double>(entries); }));
+    std::vector<double> host(entries);
+    sphere_table(stacks, slices, host.data());
+    PCU_TRY(h2d(ws, tab, host.data(), sizeof(double) * entries, stream));
+    const long long nv = m * V, nf = m * F;
+    PCU_LAUNCH(sp_geometry_kernel<T>, blocks_for(nv + nf), kThreads, stream, p, r, (const double*)tab, (unsigned)stacks, (unsigned)slices,
+               (unsigned)nv, (unsigned)nf, out_v, out_f);
+    return PCU_B200_OK;
+}
+
 }  // namespace
 
 namespace __attribute__((visibility("hidden"))) pcu_internal {
@@ -900,6 +944,14 @@ int pcu_b200_pointcloud_surfel_geometry_f32(pcu_b200_workspace* ws, const float*
 int pcu_b200_pointcloud_surfel_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* r, int64_t np,
                                             int subdivs, double* out_v, int32_t* out_f, void* stream) {
     return surfel_geometry_device<double>(ws, p, n, r, np, subdivs, out_v, out_f, (cudaStream_t)stream);
+}
+int pcu_b200_pointcloud_sphere_geometry_f32(pcu_b200_workspace* ws, const float* p, const float* r, int64_t np, int num_stacks,
+                                            int num_slices, float* out_v, int32_t* out_f, void* stream) {
+    return sphere_geometry_device<float>(ws, p, r, np, num_stacks, num_slices, out_v, out_f, (cudaStream_t)stream);
+}
+int pcu_b200_pointcloud_sphere_geometry_f64(pcu_b200_workspace* ws, const double* p, const double* r, int64_t np, int num_stacks,
+                                            int num_slices, double* out_v, int32_t* out_f, void* stream) {
+    return sphere_geometry_device<double>(ws, p, r, np, num_stacks, num_slices, out_v, out_f, (cudaStream_t)stream);
 }
 
 }  // extern "C"

@@ -1,6 +1,6 @@
-// mesh_topology.cu -- connected components and vertex removal, consistent face orientation, face areas and normals,
-// vertex normals and Laplacian smoothing (mesh_topology.cuh, orient.cuh, mesh_geometry.cuh, laplacian.cuh): launch
-// sequencing and C entry points.
+// mesh_topology.cu -- connected components and vertex removal, adjacency lists, consistent face orientation, face areas
+// and normals, vertex normals and Laplacian smoothing (mesh_topology.cuh, orient.cuh, mesh_geometry.cuh, laplacian.cuh):
+// launch sequencing and C entry points.
 #include "runtime.cuh"
 #include "mesh_topology.cuh"
 #include "orient.cuh"
@@ -20,6 +20,17 @@ struct pcu_b200_components : StreamHandle {
     const int* nv = nullptr;
     const int* nf = nullptr;
     ~pcu_b200_components() { release(block); }
+};
+
+// Adjacency lists between pcu_b200_adjacency_list_prepare and _emit: the int32 CSR in one block (rowptr over the n + 1
+// row boundaries, col over the nnz entries).
+struct pcu_b200_adjacency : StreamHandle {
+    int fkind = 0;
+    long long n = 0, nnz = 0;
+    unsigned char* block = nullptr;
+    const int* rowptr = nullptr;
+    const int* col = nullptr;
+    ~pcu_b200_adjacency() { release(block); }
 };
 
 namespace {
@@ -468,6 +479,86 @@ int laplacian_smooth_device(pcu_b200_workspace* ws, const T* v, long long nv, co
     return PCU_B200_OK;
 }
 
+// ---- adjacency lists (mesh_topology.cuh, on the Laplacian's assembly) -----------------------------------------------
+// Validate f and read max(f) (first synchronisation); the Laplacian's sorted directed-edge records over the rows [0, n)
+// and their run heads, and read the entry count (second synchronisation); then the CSR in the handle's block.  The sort's
+// second buffer, free once the sort is done, holds the entries' row records.
+int adj_build(pcu_b200_workspace* ws, pcu_b200_adjacency* h, const void* f, long long m, int fkind, cudaStream_t stream) {
+    const long long e = 6 * m;
+    struct { AdjCounts* rec; SortScratch<MgRec> sort; unsigned char* head; unsigned* counts; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.rec = cv.take<AdjCounts>(1);
+        sc.sort.carve(cv, e);
+        sc.head = cv.take<unsigned char>((size_t)e);
+        sc.counts = cv.take<unsigned>(keep_count_words(e));
+    }));
+    PCU_CUDA(cudaMemsetAsync(sc.rec, 0, sizeof(AdjCounts), stream));
+    PCU_LAUNCH(cc_validate_kernel, cc_validate_blocks(ws, 3 * m), kThreads, stream, f, fkind, 3 * m, &sc.rec->valid);
+    AdjCounts hc;
+    PCU_TRY(read_record(sc.rec, &hc, stream));
+    if (hc.valid.bad)
+        return fail(PCU_B200_INVALID_ARGUMENT, "adjacency_list: %llu face indices are negative or above 2^31 - 2", hc.valid.bad);
+    const long long n = (long long)hc.valid.max_index + 1;
+    const int bits = mg_index_bits(n);
+    PCU_LAUNCH(lap_edge_kernel, blocks_for(m), kThreads, stream, f, fkind, m, n, bits, sc.sort.a);
+    MgRec* sorted = nullptr;
+    PCU_TRY(radix_sort_records(sc.sort, e, 1, stream, &sorted, 2 * bits));
+    PCU_LAUNCH(mc_heads_kernel, blocks_for(e), kThreads, stream, (const MgRec*)sorted, e, sc.head);
+    PCU_TRY(enqueue_keep_offsets(sc.head, e, sc.counts, &sc.rec->nnz, stream));
+    PCU_TRY(read_record(sc.rec, &hc, stream));
+    const long long nnz = hc.nnz;
+    struct { int *rowptr, *col; } b;
+    const auto carve = [&](Carver& cv) {
+        b.rowptr = cv.take<int>((size_t)n + 1);
+        b.col = cv.take<int>((size_t)nnz);
+    };
+    PCU_TRY(alloc_block(h->block, carve_at(nullptr, carve), stream, "adjacency lists"));
+    carve_at(h->block, carve);
+    MgRec* rows = sorted == sc.sort.a ? sc.sort.b : sc.sort.a;
+    PCU_LAUNCH(adj_entries_kernel, blocks_for(e), kThreads, stream, (const MgRec*)sorted, e, (const unsigned char*)sc.head,
+               (const unsigned*)sc.counts, bits, rows, b.col);
+    PCU_LAUNCH(mg_rows_kernel, blocks_for(nnz + 1), kThreads, stream, (const MgRec*)rows, nnz, n, b.rowptr, (int*)nullptr, 0);
+    h->n = n;
+    h->nnz = nnz;
+    h->rowptr = b.rowptr;
+    h->col = b.col;
+    return PCU_B200_OK;
+}
+
+int adjacency_list_prepare_device(pcu_b200_workspace* ws, const void* f, long long m, int fkind, pcu_b200_adjacency** out,
+                                  long long* out_counts, cudaStream_t stream) {
+    if (!ws || !out || !out_counts) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    *out = nullptr;
+    if (!f) return fail(PCU_B200_INVALID_ARGUMENT, "null input pointer");
+    if (m <= 0 || m > 0x7fffffffLL / 6)
+        return fail(PCU_B200_INVALID_ARGUMENT, "adjacency_list: between 1 and 357913941 faces are supported, got %lld", m);
+    if (fkind < kIdxI32 || fkind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown face index kind %d", fkind);
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    PCU_TRY(prepare_handle(ws, stream, out, [&](pcu_b200_adjacency* h) {
+        h->fkind = fkind;
+        return adj_build(ws, h, f, m, fkind, stream);
+    }));
+    out_counts[0] = (*out)->n;
+    out_counts[1] = (*out)->nnz;
+    return PCU_B200_OK;
+}
+
+int adjacency_list_emit_device(pcu_b200_workspace* ws, const pcu_b200_adjacency* h, void* out_offsets, void* out_neighbors,
+                               cudaStream_t stream) {
+    if (!ws || !h || !out_offsets || !out_neighbors) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    PCU_TRY(check_handle_device(ws, h, "adjacency"));
+    PCU_ON_DEVICE(ws);
+    PCU_TRY(adopt_stream(ws, stream));
+    const unsigned blocks = blocks_for(std::max(h->n + 1, h->nnz));
+    if (wide_index(h->fkind))
+        PCU_LAUNCH(adj_emit_kernel<long long>, blocks, kThreads, stream, h->rowptr, h->n, h->col, h->nnz, (long long*)out_offsets,
+                   (long long*)out_neighbors);
+    else
+        PCU_LAUNCH(adj_emit_kernel<int>, blocks, kThreads, stream, h->rowptr, h->n, h->col, h->nnz, (int*)out_offsets, (int*)out_neighbors);
+    return PCU_B200_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -481,6 +572,14 @@ int pcu_b200_connected_components_emit(pcu_b200_workspace* ws, const pcu_b200_co
     return connected_components_emit_device(ws, cc, out_cv, out_nv, out_cf, out_nf, (cudaStream_t)stream);
 }
 int pcu_b200_connected_components_destroy(pcu_b200_components* cc) { return destroy_handle(cc); }
+int pcu_b200_adjacency_list_prepare(pcu_b200_workspace* ws, const void* f, int64_t nf, int f_kind, pcu_b200_adjacency** out_adj,
+                                    int64_t out_counts[2], void* stream) {
+    return adjacency_list_prepare_device(ws, f, nf, f_kind, out_adj, (long long*)out_counts, (cudaStream_t)stream);
+}
+int pcu_b200_adjacency_list_emit(pcu_b200_workspace* ws, const pcu_b200_adjacency* adj, void* out_offsets, void* out_neighbors, void* stream) {
+    return adjacency_list_emit_device(ws, adj, out_offsets, out_neighbors, (cudaStream_t)stream);
+}
+int pcu_b200_adjacency_list_destroy(pcu_b200_adjacency* adj) { return destroy_handle(adj); }
 int pcu_b200_remove_mesh_vertices_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind,
                                       const uint8_t* mask, float* out_v, void* out_f, int64_t out_counts[2], void* stream) {
     return remove_mesh_vertices_device<float>(ws, v, nv, f, nf, f_kind, mask, out_v, out_f, (long long*)out_counts, (cudaStream_t)stream);

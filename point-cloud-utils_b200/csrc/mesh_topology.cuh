@@ -21,10 +21,22 @@
 //
 // remove_mesh_vertices / remove_unreferenced_mesh_vertices: order-preserving compactions (compact.cuh) of the kept
 // vertices and, for the mask, of the kept faces; one synchronisation each, to read MtCounts.
+//
+// adjacency_list (the reference's src/adjacency_list.cpp, libigl's adjacency_list): the Laplacian's sparsity pattern
+// (laplacian.cuh) over the rows [0, n), n = max(f) + 1, in CSR form:
+//   cc_validate_kernel  max(f) and the entries outside [0, 2^31 - 2] (the host reads them: first synchronisation)
+//   lap_edge_kernel     six directed-edge records per face, key (row << bits) | column, with nv = n
+//   radix sort (sort.cuh), mc_heads_kernel (runtime.cu), keep_count / keep_offsets (compact.cuh): one entry per
+//                       distinct (row, column) pair, ascending; the host reads their count nnz (second synchronisation)
+//   adj_entries_kernel  entry e of every run: its column into the handle, its row as the key of mg_rows_kernel
+//   mg_rows_kernel      (mesh_geometry.cuh) the row pointers: row i holds entries [rowptr[i], rowptr[i + 1])
+//   adj_emit_kernel     both arrays in f's width.
+// A face with a repeated corner gives the pair (a, a) and so a self-loop, as in libigl.
 #pragma once
 #include "common.cuh"
 #include "compact.cuh"
 #include "meshsample.cuh"
+#include "mesh_geometry.cuh"
 #include "union_find.cuh"
 
 namespace pcu {
@@ -37,6 +49,12 @@ struct CcCounts {
     unsigned max_index;       // max(f) over the other entries
     unsigned pad;
     long long ncomp;          // components (keep_offsets_kernel)
+};
+
+// What the host reads from adjacency_list (zeroed per call).
+struct AdjCounts {
+    CcCounts valid;           // cc_validate_kernel's bad entries and max(f)
+    long long nnz;            // distinct (row, column) pairs (keep_offsets_kernel)
 };
 
 // What the host reads from a vertex removal (zeroed per call).
@@ -132,6 +150,33 @@ __global__ void __launch_bounds__(kThreads) cc_emit_kernel(const int* __restrict
     if (i < n) out_cv[i] = (I)cv[i];
     if (i < m) out_cf[i] = (I)cf[i];
     if (i < k) { out_nv[i] = (I)nv[i]; out_nf[i] = (I)nf[i]; }
+}
+
+// ---- adjacency_list -----------------------------------------------------------------------------------------------
+// After keep_count / keep_offsets over the run heads of the sorted directed-edge records: entry e of every run, its row
+// (for mg_rows_kernel's key) and its column.
+__global__ void __launch_bounds__(kThreads) adj_entries_kernel(const MgRec* __restrict__ sorted, long long n, const unsigned char* __restrict__ head,
+                                                               const unsigned* __restrict__ block_offset, int bits, MgRec* __restrict__ rows,
+                                                               int* __restrict__ col) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    const bool mine = i < n && head[i];
+    const unsigned e = keep_rank(mine, block_offset);
+    if (!mine) return;
+    const unsigned long long key = sorted[i].key[0];
+    MgRec r;
+    r.key[0] = key >> bits;
+    r.idx = e;
+    store_rec(rows + e, r);
+    col[e] = (int)(key & ((1ull << bits) - 1ull));
+}
+
+// The n + 1 row pointers and the nnz columns in f's width I.
+template <typename I>
+__global__ void __launch_bounds__(kThreads) adj_emit_kernel(const int* __restrict__ rowptr, long long n, const int* __restrict__ col,
+                                                            long long nnz, I* __restrict__ out_offsets, I* __restrict__ out_neighbors) {
+    const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
+    if (i <= n) out_offsets[i] = (I)rowptr[i];
+    if (i < nnz) out_neighbors[i] = (I)col[i];
 }
 
 // ---- remove_mesh_vertices -----------------------------------------------------------------------------------------

@@ -416,6 +416,52 @@ __global__ void __launch_bounds__(kThreads) sf_geometry_kernel(const T* __restri
     }
 }
 
+// pointcloud_sphere_geometry: the reference's make_sphere_geometry for every point (DESIGN.md §3).  Point i has
+// V = (stacks + 1)(slices + 1) vertices and F = 2 (stacks - 1) slices faces.  Threads [0, nv) write vertex rows,
+// threads [nv, nv + nf) write faces, so a point's rows are written by consecutive threads (nv = m V < 2^31 - 1 and
+// nf = m F < 2 nv: both fit 32 bits).  tab holds cos and sin of the stack angles a = 0 .. stacks, then cos and sin of
+// the sector angles b = 0 .. slices, from the host's C library.  Vertex (a, b): xy = r_i cos_a, z = r_i sin_a,
+// x = xy cos_b, y = xy sin_b, each product rounded on its own, and row k = (T)(p_ik + (x, y, z)_k) with the sum in fp64.
+// Faces of stack a, sector j, k1 = a (slices + 1) + j, k2 = k1 + slices + 1: (k1, k2, k1 + 1) unless a = 0, then
+// (k1 + 1, k2, k2 + 1) unless a = stacks - 1, offset by i V.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) sp_geometry_kernel(const T* __restrict__ p, const T* __restrict__ r, const double* __restrict__ tab,
+                                                               unsigned stacks, unsigned slices, unsigned nv, unsigned nf,
+                                                               T* __restrict__ out_v, int* __restrict__ out_f) {
+    const long long g = (long long)blockIdx.x * kThreads + threadIdx.x;
+    const unsigned cols = slices + 1, V = (stacks + 1) * cols;
+    if (g < nv) {
+        const unsigned k = (unsigned)g, i = k / V, q = k - i * V, a = q / cols, b = q - a * cols;
+        const double ri = (double)r[i];
+        const double xy = __dmul_rn(ri, __ldg(tab + a)), z = __dmul_rn(ri, __ldg(tab + stacks + 1 + a));
+        const double* sector = tab + 2 * (stacks + 1);
+        const double x = __dmul_rn(xy, __ldg(sector + b)), y = __dmul_rn(xy, __ldg(sector + cols + b));
+        T* o = out_v + 3 * (size_t)k;
+        o[0] = (T)__dadd_rn((double)p[3 * (size_t)i], x);
+        o[1] = (T)__dadd_rn((double)p[3 * (size_t)i + 1], y);
+        o[2] = (T)__dadd_rn((double)p[3 * (size_t)i + 2], z);
+        return;
+    }
+    if (g >= (long long)nv + nf) return;
+    const unsigned e = (unsigned)(g - nv), F = 2 * (stacks - 1) * slices, i = e / F;
+    unsigned q = e - i * F, a, j;
+    bool upper;   // the (k1, k2, k1 + 1) triangle, else the (k1 + 1, k2, k2 + 1) one
+    if (q < slices) {
+        a = 0; j = q; upper = false;
+    } else {
+        q -= slices;
+        a = 1 + q / (2 * slices);
+        const unsigned rem = q - (a - 1) * (2 * slices);
+        if (a < stacks - 1) { j = rem >> 1; upper = (rem & 1) == 0; }
+        else { j = rem; upper = true; }
+    }
+    const int k1 = (int)(i * V + a * cols + j), k2 = k1 + (int)cols;
+    int* o = out_f + 3 * (size_t)e;
+    o[0] = upper ? k1 : k1 + 1;
+    o[1] = k2;
+    o[2] = upper ? k1 + 1 : k2 + 1;
+}
+
 // ---- the per-(query, face) definition (DESIGN.md §3) ---------------------------------------------------------------
 template <typename T>
 struct MqHit { T d2, b0, b1, b2; };
