@@ -33,8 +33,8 @@ except ImportError as _e:  # pragma: no cover - exercised only on a broken insta
         "pcu_b200: the compiled extension (_pcu_internal / libpcu_b200.so) is missing or failed to load: %s.\n"
         "Build it in-tree with `python -c 'import __graft_entry__ as g; g.build()'` from the repository root.\n"
         "There is no pure-Python or CPU fallback for this package." % (_e,)) from _e
-from ._call import (_asarrays, _call_args, _check_float, _dev, _form, _is_tensor, _ordinal, _run,  # noqa: E402
-                    _same_device, _torch)
+from ._call import (_as_form, _asarrays, _call_args, _check_clouds, _check_float, _check_match, _dev,  # noqa: E402
+                    _dtype_name, _form, _is_tensor, _numpy, _ordinal, _run, _same_device, _shape, _torch)
 
 __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_distance", "chamfer_distance",
            "batched_chamfer_distance", "estimate_point_cloud_normals_knn", "estimate_point_cloud_normals_ball",
@@ -56,7 +56,8 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "deduplicate_mesh_vertices", "prepare_cloud", "pinned_empty", "PreparedCloud", "device_count",
            "current_device", "launch_count"]
 
-_STATS_WORDS = 10  # sizeof(pcu_b200_nn_stats) / 8
+_STATS = _pcu_internal._stats_dtype()   # pcu_b200_nn_stats as a numpy record type: host records come as it, device ones are read as it
+_STATS_WORDS = _STATS.itemsize // 8
 
 
 def device_count():
@@ -76,64 +77,20 @@ def launch_count():
     return _pcu_internal._launch_count()
 
 
-def _check_tensor_pair(a, b, name_a, name_b):
-    torch = _torch()
-    if not _is_tensor(b):
-        raise ValueError("%s and %s must both be torch tensors or both be numpy arrays" % (name_a, name_b))
-    if a.dtype not in (torch.float32, torch.float64):
-        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected one of ['float32', 'float64']."
-                         % (a.dtype, name_a))
-    if b.dtype != a.dtype:
-        raise ValueError("Invalid scalar type (%s) for argument '%s'. Expected it to match argument '%s' which is "
-                         "of type %s." % (b.dtype, name_b, name_a, a.dtype))
-    if a.device != b.device:
-        raise ValueError("%s and %s must live on the same device" % (name_a, name_b))
-    shapes = "Got %s.shape = %s, %s.shape = %s." % (name_a, tuple(a.shape), name_b, tuple(b.shape))
-    if a.dim() != 2 or b.dim() != 2 or a.shape[1] != 3 or b.shape[1] != 3:
-        raise ValueError("Only 3D inputs are supported: %s and %s must have shape (n, 3) and (m, 3). %s"
-                         % (name_a, name_b, shapes))
-    if a.shape[0] == 0 or b.shape[0] == 0:
-        raise ValueError("Invalid input set with zero elements: %s and %s must have shape (n, 3) and (m, 3). %s"
-                         % (name_a, name_b, shapes))
-    return a.detach().contiguous(), b.detach().contiguous()
+def _stats_from_tensor(buf, which=slice(None)):
+    """Record `which` (default: every record) of a device buffer of pcu_b200_nn_stats, read back (synchronises)."""
+    return buf.cpu().numpy().view(_STATS)[which]
 
 
-def _stats_from_tensor(buf, which):
-    """Decode one pcu_b200_nn_stats from the raw device buffer (synchronises)."""
-    host = buf.cpu()
-    f = host.view(_torch().float64)
-    i = host.view(_torch().int64)
-    o = _STATS_WORDS * which
-    return {"sum_dist": float(f[o]), "sum_sq_dist": float(f[o + 1]), "max_sq_dist": float(f[o + 2]),
-            "argmax_query": int(i[o + 3]), "argmax_data": int(i[o + 4]), "n_queries": int(i[o + 5]),
-            "n_tied": int(i[o + 6]), "n_far": int(i[o + 7]), "witness_tied": int(i[o + 8]),
-            "pair_value": float(f[o + 9])}
+def _pair_value(words):
+    """The fp64 Chamfer value a two-way sweep leaves in record 0 (pair_value), as a 1-element view of its words."""
+    at = _STATS.fields["pair_value"][1] // 8
+    return words.view(_torch().float64)[at:at + 1]
 
 
-def _resolved_stats(buf, which, q, d, leaf):
-    """Stats record `which` of `buf`; when its Hausdorff witness hinges on tie order, have the device replay it."""
-    st = _stats_from_tensor(buf, which)
-    if st["witness_tied"]:
-        torch = _torch()
-        _pcu_internal._resolve_witness_device(q.dtype == torch.float64, q.data_ptr(), q.shape[0], d.data_ptr(),
-                                              d.shape[0], buf.data_ptr() + 8 * _STATS_WORDS * which, int(leaf),
-                                              *_call_args(q))
-        st = _stats_from_tensor(buf, which)
-    return st
-
-
-def _stats_device(a, b, both, leaf):
-    torch = _torch()
-    assert _pcu_internal._stats_nbytes() == 8 * _STATS_WORDS
-    buf = torch.empty(2 * _STATS_WORDS, dtype=torch.int64, device=a.device)   # every record is written by the sweep
-    val = torch.empty((), dtype=a.dtype, device=a.device)
-    _pcu_internal._stats_device(a.dtype == torch.float64, both, a.data_ptr(), a.shape[0], b.data_ptr(), b.shape[0],
-                                buf.data_ptr(), val.data_ptr() if both else 0, int(leaf), *_call_args(a))
-    return buf, val
-
-
-def _metric_value(max_sq, squared, dtype):
-    d2 = dtype(max_sq)
+def _metric_value(max_sq, squared, x):
+    """A Hausdorff distance from a record's max_sq_dist, rounded in the precision of the points x."""
+    d2 = _np.dtype(_dtype_name(x)).type(max_sq)
     if d2 == -1:   # no query found a neighbour: the reference's padded distance, not its root
         return -1.0
     return float(d2 if squared else _np.sqrt(d2))
@@ -184,21 +141,14 @@ def prepare_cloud(points, *, k=None, max_points_per_leaf=10, device=None):
     if int(max_points_per_leaf) <= 0:
         raise ValueError("max_points_per_leaf must be greater than 0.")
     meta = dict(knn_k=(kk or None), max_points_per_leaf=(int(max_points_per_leaf) if kk else None))
-    if _is_tensor(points):
-        torch = _torch()
-        if points.dtype not in (torch.float32, torch.float64) or points.dim() != 2 or points.shape[1] != 3 or points.shape[0] == 0:
-            raise ValueError("points must be a float32 / float64 tensor of shape (n, 3) with n > 0")
-        if not points.is_cuda:
-            return prepare_cloud(points.detach().numpy(), k=k, max_points_per_leaf=max_points_per_leaf, device=device)
-        _same_device(points, device)
-        p = points.detach().contiguous()
+    form, (p,) = _nn_args([points], ["points"], device)
+    f64 = _dtype_name(p) == "float64"
+    if form == "cuda":
         dev, stream = _call_args(p)
-        h = _pcu_internal._cloud_prepare_device(p.dtype == torch.float64, p.data_ptr(), p.shape[0], dev, stream, kk,
-                                                int(max_points_per_leaf))
-        return PreparedCloud(h, p.shape[0], p.dtype == torch.float64, dev, True, **meta)
-    pts = _np.asarray(points)
-    h = _pcu_internal._cloud_prepare(pts, _dev(device), kk, int(max_points_per_leaf))
-    return PreparedCloud(h, pts.shape[0], pts.dtype == _np.float64, _ordinal(device), False, **meta)
+        h = _pcu_internal._cloud_prepare_device(f64, p.data_ptr(), p.shape[0], dev, stream, kk, int(max_points_per_leaf))
+        return PreparedCloud(h, p.shape[0], f64, dev, True, **meta)
+    h = _pcu_internal._cloud_prepare_host(p, _dev(device), kk, int(max_points_per_leaf))
+    return PreparedCloud(h, p.shape[0], f64, _ordinal(device), False, **meta)
 
 
 def pinned_empty(n, dtype=_np.float32, cols=3, *, device=None):
@@ -218,41 +168,88 @@ def pinned_empty(n, dtype=_np.float32, cols=3, *, device=None):
     return _pcu_internal._pinned_empty(int(n), int(cols), dt == _np.dtype(_np.float64))
 
 
-def _prepared_resolved(buf, which, xs, cloud, leaf):
-    """Record `which` of a prepared-cloud call on device tensors, its Hausdorff witness replayed when tie order decided it."""
-    st = _stats_from_tensor(buf, which)
-    if st["witness_tied"]:
-        yp, m = _pcu_internal._cloud_points(cloud._handle), cloud.shape[0]
-        q, n, d, k = (xs.data_ptr(), xs.shape[0], yp, m) if which == 0 else (yp, m, xs.data_ptr(), xs.shape[0])
-        _pcu_internal._resolve_witness_device(cloud._f64, q, n, d, k, buf.data_ptr() + 8 * _STATS_WORDS * which, int(leaf),
-                                              *_call_args(xs))
-        st = _stats_from_tensor(buf, which)
-    return st
+def _nn_args(clouds, names, device):
+    """(form, inputs) of a nearest-neighbour call, checked before any device call: the point sets as the reference checks
+    them (_check_clouds) and, when the last one is a PreparedCloud, that it is open and lives on the device of the call.
+    CUDA tensors come back detached and contiguous; numpy arrays and CPU tensors as the numpy arrays the binding's host
+    entry points take.  A PreparedCloud comes back as it is."""
+    cloud = clouds[-1] if isinstance(clouds[-1], PreparedCloud) else None
+    arrays = _asarrays(clouds[:-1] if cloud is not None else clouds)
+    form = _form(arrays, names)
+    _check_clouds(arrays + ([cloud] if cloud is not None else []), names)
+    if cloud is not None:
+        if not cloud._handle:
+            raise ValueError("the PreparedCloud has been closed")
+        if form == "cuda" and (arrays[0].device.index or 0) != cloud.device_index:
+            raise ValueError("%s lives on %s, the prepared cloud on cuda:%d" % (names[0], arrays[0].device, cloud.device_index))
+        d = _dev(device)
+        if d >= 0 and d != cloud.device_index:
+            raise ValueError("device=%r contradicts the prepared cloud, which lives on cuda:%d" % (device, cloud.device_index))
+    elif form == "cuda":
+        _same_device(arrays[0], device)
+    arrays = [a.detach().contiguous() for a in arrays] if form == "cuda" else _numpy(arrays)
+    return form, arrays + ([cloud] if cloud is not None else [])
+
+
+def _stats_device(a, b, both, leaf):
+    """The fused statistics sweep(s) of the CUDA tensor a against b (a tensor or a PreparedCloud on a's device), with
+    checked arguments: (the raw records, 2 * _STATS_WORDS int64 on the device; the Chamfer value, a 0-d tensor, or None
+    one way).  Each record the sweep computes is written whole; nothing synchronises."""
+    torch = _torch()
+    words = torch.empty(2 * _STATS_WORDS, dtype=torch.int64, device=a.device)
+    value = torch.empty((), dtype=a.dtype, device=a.device) if both else None
+    prepared = isinstance(b, PreparedCloud)
+    target = (b._handle,) if prepared else (b.data_ptr(), b.shape[0])
+    out = (words.data_ptr(), value.data_ptr()) if both else (words.data_ptr(),)
+    if prepared:
+        sweep = _pcu_internal._chamfer_prepared_device if both else _pcu_internal._nn_stats_prepared_device
+    else:
+        sweep = _pcu_internal._chamfer_device if both else _pcu_internal._nn_stats_device
+    sweep(a.dtype == torch.float64, a.data_ptr(), a.shape[0], *target, *out, int(leaf), *_call_args(a))
+    return words, value
+
+
+def _sweep(x, y, both, leaf, device, names=("x", "y")):
+    """The fused statistics sweep of x against y (an array or a PreparedCloud): one way (both False: the record of
+    x -> y) or both ways in one launch sequence (the records of x -> y and y -> x, and the Chamfer value).  Returns
+    (form, value, records, x, y): value is None one way, else a numpy scalar for host calls and an unsynchronised 0-d
+    tensor for CUDA tensors; records are the host's two records, or the device's raw words (_stats_device), which
+    _records reads; x and y as the call took them."""
+    form, (x, y) = _nn_args([x, y], list(names), device)
+    if form == "cuda":
+        records, value = _stats_device(x, y, both, leaf)
+    elif isinstance(y, PreparedCloud):
+        value, *records = _pcu_internal._stats_prepared_host(x, y._handle, y._f64, both, int(leaf), y.device_index)
+    else:
+        value, *records = _pcu_internal._chamfer_stats(x, y, int(leaf), _dev(device), both)
+    return form, value, records, x, y
 
 
 def _prepared_stats(x, cloud, both, leaf, device):
-    """(where, dtype, value, payload) like _both_stats, for a PreparedCloud second argument."""
-    if not cloud._handle:
-        raise ValueError("the PreparedCloud has been closed")
-    if _is_tensor(x) and x.is_cuda:
-        torch = _torch()
-        if x.dtype != (torch.float64 if cloud._f64 else torch.float32) or x.dim() != 2 or x.shape[1] != 3 or x.shape[0] == 0:
-            raise ValueError("the first argument must be an (n, 3) tensor of the prepared cloud's dtype (%s)" % cloud.dtype)
-        if (x.device.index or 0) != cloud.device_index:
-            raise ValueError("the points live on %s, the prepared cloud on cuda:%d" % (x.device, cloud.device_index))
-        xs = x.detach().contiguous()
-        buf = torch.empty(2 * _STATS_WORDS, dtype=torch.int64, device=xs.device)
-        val = torch.empty((), dtype=xs.dtype, device=xs.device)
-        _pcu_internal._stats_prepared_device(cloud._f64, both, xs.data_ptr(), xs.shape[0], cloud._handle, buf.data_ptr(),
-                                             val.data_ptr() if both else 0, int(leaf), *_call_args(xs))
-        return "cuda", xs.dtype, val, (buf, xs)
-    if _is_tensor(x):
-        x = x.detach().numpy()
-    d = _dev(device)
-    if d >= 0 and d != cloud.device_index:
-        raise ValueError("device=%r contradicts the prepared cloud, which lives on cuda:%d" % (device, cloud.device_index))
-    res = _pcu_internal._stats_prepared(_np.asarray(x), cloud._handle, cloud._f64, both, int(leaf), cloud.device_index)
-    return "host", cloud.dtype.type, res[0], res[1:]
+    """_sweep against a PreparedCloud as (where, dtype, value, records); on the device the records are (raw words, x)."""
+    form, value, records, xs, _ = _sweep(x, cloud, both, leaf, device)
+    if form == "cuda":
+        return "cuda", xs.dtype, value, (records, xs)
+    return "host", xs.dtype.type, value, tuple(records[:1 if value is None else 2])
+
+
+def _records(sweep, leaf):
+    """The records of a _sweep (one or two).  On the device, a record whose Hausdorff witness the order of exactly tied
+    neighbours decided (witness_tied) is replayed first in the reference's tie order; the host sweeps replay their own."""
+    form, value, records, x, y = sweep
+    count = 1 if value is None else 2
+    if form != "cuda":
+        return records[:count]
+    host = _stats_from_tensor(records)
+    tied = [i for i in range(count) if host[i]["witness_tied"]]
+    if tied:
+        data = (_pcu_internal._cloud_points(y._handle) if isinstance(y, PreparedCloud) else y.data_ptr(), y.shape[0])
+        for i in tied:
+            q, d = ((x.data_ptr(), x.shape[0]), data) if i == 0 else (data, (x.data_ptr(), x.shape[0]))
+            _pcu_internal._resolve_witness_device(x.dtype == _torch().float64, *q, *d, records.data_ptr() + 8 * _STATS_WORDS * i,
+                                                  int(leaf), *_call_args(x))
+        host = _stats_from_tensor(records)
+    return list(host[:count])
 
 
 # ---------------------------------------------------------------------------------------------
@@ -280,62 +277,26 @@ def k_nearest_neighbors(query_points, dataset_points, k, squared_distances=False
 
     Mirrors /root/reference/src/point_cloud_distance.cpp:123-164.
     """
-    if isinstance(dataset_points, PreparedCloud):
-        return _knn_prepared(query_points, dataset_points, int(k), bool(squared_distances), int(max_points_per_leaf), device)
-    if _is_tensor(query_points) or _is_tensor(dataset_points):
-        torch = _torch()
-        if not _is_tensor(query_points):
-            raise ValueError("query_points and dataset_points must both be torch tensors or both be numpy arrays")
-        if int(k) <= 0:
-            raise ValueError("Invalid value for k (%d) must be greater than 0." % int(k))
-        q, d = _check_tensor_pair(query_points, dataset_points, "query_points", "dataset_points")
-        if not q.is_cuda:
-            dn, cn = _pcu_internal.k_nearest_neighbors(q.numpy(), d.numpy(), int(k), bool(squared_distances),
-                                                       int(max_points_per_leaf), int(num_threads), _dev(device))
-            return torch.from_numpy(_np.asarray(dn)), torch.from_numpy(_np.asarray(cn))
-        _same_device(q, device)
-        n = q.shape[0]
-        dists = torch.empty((n, int(k)), dtype=q.dtype, device=q.device)
-        corrs = torch.empty((n, int(k)), dtype=torch.int64, device=q.device)
-        _pcu_internal._knn_device(q.dtype == torch.float64, q.data_ptr(), n, d.data_ptr(), d.shape[0], int(k),
-                                  bool(squared_distances), dists.data_ptr(), corrs.data_ptr(), 0,
-                                  int(max_points_per_leaf), *_call_args(q))
-        return dists.squeeze(), corrs.squeeze()
-    return _pcu_internal.k_nearest_neighbors(_np.asarray(query_points), _np.asarray(dataset_points), int(k),
-                                             bool(squared_distances), int(max_points_per_leaf), int(num_threads),
-                                             _dev(device))
-
-
-def _knn_prepared(query_points, cloud, k, squared, leaf, device):
-    """k_nearest_neighbors against a PreparedCloud: numpy in -> numpy out, CUDA tensor in -> CUDA tensors out."""
-    if not cloud._handle:
-        raise ValueError("the prepared cloud has been closed")
+    k, squared, leaf = int(k), bool(squared_distances), int(max_points_per_leaf)
     if k <= 0:
         raise ValueError("Invalid value for k (%d) must be greater than 0." % k)
-    if _is_tensor(query_points) and query_points.is_cuda:
-        torch = _torch()
-        q = query_points.detach().contiguous()
-        if q.dtype != (torch.float64 if cloud._f64 else torch.float32) or q.dim() != 2 or q.shape[1] != 3 or q.shape[0] == 0:
-            raise ValueError("query_points must be a non-empty (n, 3) tensor of the prepared cloud's precision (%s)" % cloud.dtype)
-        if (q.device.index or 0) != cloud.device_index:
-            raise ValueError("query_points live on %s, the prepared cloud on device %d" % (q.device, cloud.device_index))
-        _same_device(q, device)
-        n = q.shape[0]
-        dists = torch.empty((n, k), dtype=q.dtype, device=q.device)
-        corrs = torch.empty((n, k), dtype=torch.int64, device=q.device)
-        _pcu_internal._knn_prepared_device(cloud._f64, q.data_ptr(), n, cloud._handle, k, squared, dists.data_ptr(),
+    form, (q, d) = _nn_args([query_points, dataset_points], ["query_points", "dataset_points"], device)
+    prepared = isinstance(d, PreparedCloud)
+    if form != "cuda":
+        if prepared:
+            return _as_form(form, _pcu_internal._knn_prepared_host(q, d._handle, d._f64, k, squared, leaf, d.device_index))
+        return _as_form(form, _pcu_internal._knn_host(q, d, k, squared, leaf, _dev(device)))
+    torch = _torch()
+    n = q.shape[0]
+    dists = torch.empty((n, k), dtype=q.dtype, device=q.device)
+    corrs = torch.empty((n, k), dtype=torch.int64, device=q.device)
+    if prepared:
+        _pcu_internal._knn_prepared_device(q.dtype == torch.float64, q.data_ptr(), n, d._handle, k, squared, dists.data_ptr(),
                                            corrs.data_ptr(), 0, leaf, *_call_args(q))
-        return dists.squeeze(), corrs.squeeze()
-    as_tensor = _is_tensor(query_points)
-    qn = query_points.detach().numpy() if as_tensor else _np.asarray(query_points)
-    d = _dev(device)
-    if d >= 0 and d != cloud.device_index:
-        raise ValueError("device=%d was given but the prepared cloud lives on device %d" % (d, cloud.device_index))
-    dn, cn = _pcu_internal._knn_prepared(qn, cloud._handle, cloud._f64, k, squared, leaf, cloud.device_index)
-    if as_tensor:
-        torch = _torch()
-        return torch.from_numpy(_np.asarray(dn)), torch.from_numpy(_np.asarray(cn))
-    return dn, cn
+    else:
+        _pcu_internal._knn_device(q.dtype == torch.float64, q.data_ptr(), n, d.data_ptr(), d.shape[0], k, squared,
+                                  dists.data_ptr(), corrs.data_ptr(), 0, leaf, *_call_args(q))
+    return dists.squeeze(), corrs.squeeze()
 
 
 def one_sided_hausdorff_distance(source, target, return_index=True, squared_distances=False, max_points_per_leaf=10,
@@ -360,53 +321,10 @@ def one_sided_hausdorff_distance(source, target, return_index=True, squared_dist
     Mirrors /root/reference/src/point_cloud_distance.cpp:186-234.  One fused sweep: no per-point distance array
     is written; the maximum, its first row and that row's neighbour are reduced inside the search kernel.
     """
-    if isinstance(target, PreparedCloud):
-        where, dtype, _, payload = _prepared_stats(source, target, False, max_points_per_leaf, device)
-        if where == "cuda":
-            st = _prepared_resolved(payload[0], 0, payload[1], target, max_points_per_leaf)
-            np_t = _np.float32 if dtype == _torch().float32 else _np.float64
-        else:
-            st, np_t = payload[0], dtype
-        value = _metric_value(st["max_sq_dist"], squared_distances, np_t)
-        return (value, st["argmax_query"], st["argmax_data"]) if return_index else value
-    if _is_tensor(source) or _is_tensor(target):
-        if not _is_tensor(source):
-            raise ValueError("source and target must both be torch tensors or both be numpy arrays")
-        s, t = _check_tensor_pair(source, target, "source", "target")
-        if not s.is_cuda:
-            return _pcu_internal.one_sided_hausdorff_distance(s.numpy(), t.numpy(), bool(return_index),
-                                                              bool(squared_distances), int(max_points_per_leaf),
-                                                              _dev(device))
-        _same_device(s, device)
-        buf, _ = _stats_device(s, t, False, max_points_per_leaf)
-        st = _resolved_stats(buf, 0, s, t, max_points_per_leaf)
-        value = _metric_value(st["max_sq_dist"], squared_distances,
-                              _np.float32 if s.dtype == _torch().float32 else _np.float64)
-        if return_index:
-            return value, st["argmax_query"], st["argmax_data"]
-        return value
-    return _pcu_internal.one_sided_hausdorff_distance(_np.asarray(source), _np.asarray(target), bool(return_index),
-                                                      bool(squared_distances), int(max_points_per_leaf), _dev(device))
-
-
-def _both_stats(x, y, max_points_per_leaf, device=None):
-    """(dtype, chamfer value, stats x->y, stats y->x) from ONE fused bidirectional launch sequence."""
-    if isinstance(y, PreparedCloud):
-        where, dtype, val, payload = _prepared_stats(x, y, True, max_points_per_leaf, device)
-        if where == "cuda":
-            return ("cuda-prepared", dtype, val, payload + (y,))
-        return ("host", dtype, val, payload)
-    if _is_tensor(x) or _is_tensor(y):
-        if not _is_tensor(x):
-            raise ValueError("x and y must both be torch tensors or both be numpy arrays")
-        xs, ys = _check_tensor_pair(x, y, "x", "y")
-        if xs.is_cuda:
-            _same_device(xs, device)
-            buf, val = _stats_device(xs, ys, True, max_points_per_leaf)
-            return ("cuda", xs.dtype, val, (buf, xs, ys))
-        x, y = xs.numpy(), ys.numpy()
-    val, sxy, syx = _pcu_internal._chamfer_stats(_np.asarray(x), _np.asarray(y), int(max_points_per_leaf), _dev(device))
-    return ("host", _np.asarray(x).dtype.type, val, (sxy, syx))
+    sweep = _sweep(source, target, False, max_points_per_leaf, device, ("source", "target"))
+    st = _records(sweep, max_points_per_leaf)[0]
+    value = _metric_value(st["max_sq_dist"], squared_distances, sweep[3])
+    return (value, int(st["argmax_query"]), int(st["argmax_data"])) if return_index else value
 
 
 def hausdorff_distance(x, y, return_index=False, squared_distances=False, max_points_per_leaf=10, *, device=None):
@@ -430,27 +348,15 @@ def hausdorff_distance(x, y, return_index=False, squared_distances=False, max_po
     Mirrors /root/reference/point_cloud_utils/__init__.py:52-81 (two one-sided passes, `>` / `<=` branch rule);
     both directions come from one fused launch sequence over the two binned clouds.
     """
-    where, dtype, _, st = _both_stats(x, y, max_points_per_leaf, device)
-    if where == "cuda-prepared":
-        buf, xs, cloud = st
-        sxy = _prepared_resolved(buf, 0, xs, cloud, max_points_per_leaf)
-        syx = _prepared_resolved(buf, 1, xs, cloud, max_points_per_leaf)
-        np_t = _np.float32 if dtype == _torch().float32 else _np.float64
-    elif where == "cuda":
-        buf, xs, ys = st
-        sxy = _resolved_stats(buf, 0, xs, ys, max_points_per_leaf)
-        syx = _resolved_stats(buf, 1, ys, xs, max_points_per_leaf)
-        np_t = _np.float32 if dtype == _torch().float32 else _np.float64
-    else:
-        sxy, syx = st
-        np_t = dtype
-    h_xy = _metric_value(sxy["max_sq_dist"], squared_distances, np_t)
-    h_yx = _metric_value(syx["max_sq_dist"], squared_distances, np_t)
+    sweep = _sweep(x, y, True, max_points_per_leaf, device)
+    sxy, syx = _records(sweep, max_points_per_leaf)
+    h_xy = _metric_value(sxy["max_sq_dist"], squared_distances, sweep[3])
+    h_yx = _metric_value(syx["max_sq_dist"], squared_distances, sweep[3])
     hausdorff = max(h_xy, h_yx)
     if return_index and h_xy > h_yx:
-        return hausdorff, sxy["argmax_query"], sxy["argmax_data"]
+        return hausdorff, int(sxy["argmax_query"]), int(sxy["argmax_data"])
     elif return_index and h_xy <= h_yx:
-        return hausdorff, syx["argmax_data"], syx["argmax_query"]
+        return hausdorff, int(syx["argmax_data"]), int(syx["argmax_query"])
     return hausdorff
 
 
@@ -476,8 +382,7 @@ def chamfer_distance(x, y, return_index=False, p_norm=2, max_points_per_leaf=10,
     whole computation is one fused bidirectional sweep (no index or distance array is materialised).
     """
     if p_norm == 2 and not return_index:
-        where, _, val, _ = _both_stats(x, y, max_points_per_leaf, device)
-        return val
+        return _sweep(x, y, True, max_points_per_leaf, device)[1]
     if isinstance(y, PreparedCloud):
         raise ValueError("a PreparedCloud serves the fused metrics (p_norm = 2, return_index = False); pass the array for the others")
     dists_x_to_y, corrs_x_to_y = k_nearest_neighbors(x, y, k=1, squared_distances=False,
@@ -539,9 +444,8 @@ def estimate_point_cloud_normals_knn(points, num_neighbors, view_directions=None
     neighbours (num_neighbors < 3) give a zero normal; a neighbourhood of coincident points gives (0, 0, 1).
     """
     def host(p, dirs):
-        return _pcu_internal.estimate_point_cloud_normals_knn_internal(p, dirs, int(num_neighbors), int(max_points_per_leaf),
-                                                                       float(drop_angle_threshold), int(num_threads), -1,
-                                                                       _dev(device))
+        return _pcu_internal._normals_knn_host(p, dirs, int(num_neighbors), float(drop_angle_threshold), int(max_points_per_leaf),
+                                               _dev(device))
 
     def launch(pts, dirs, idx, nrm, count, dev, stream):
         _pcu_internal._normals_knn_device(pts.dtype == _torch().float64, pts.data_ptr(), pts.shape[0],
@@ -590,10 +494,8 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
     seed = int(_np.random.randint(2 ** 31 - 1))
 
     def host(p, dirs):
-        return _pcu_internal.estimate_point_cloud_normals_ball_internal(p, dirs, float(ball_radius), int(min_pts_per_ball),
-                                                                        int(max_pts_per_ball), float(drop_angle_threshold),
-                                                                        int(max_points_per_leaf), int(num_threads),
-                                                                        str(weight_function), seed, _dev(device))
+        return _pcu_internal._normals_ball_host(p, dirs, float(ball_radius), int(min_pts_per_ball), int(max_pts_per_ball),
+                                                float(drop_angle_threshold), str(weight_function), seed, _dev(device))
 
     def launch(pts, dirs, idx, nrm, count, dev, stream):
         _pcu_internal._normals_ball_device(pts.dtype == _torch().float64, pts.data_ptr(), pts.shape[0],
@@ -605,52 +507,46 @@ def estimate_point_cloud_normals_ball(points, ball_radius, view_directions=None,
 
 
 def _normals(points, view_directions, device, host, launch, num_neighbors=None):
-    """The call path of the two normal estimators.  numpy arrays go to host(points, view_directions), the binding's host
-    entry point; CPU tensors go there as numpy arrays and come back as tensors.  CUDA tensors go to launch(points, view
-    directions or None, idx, normals, count, device index, stream); the kept count is always read back, since even
-    without view directions a row with a NaN or infinite coordinate is dropped.  num_neighbors: the k-NN estimator's,
-    checked with the tensor arguments."""
-    tensor = _is_tensor(points)
-    if tensor:
-        torch = _torch()
-        if points.dtype not in (torch.float32, torch.float64):
-            raise ValueError("Invalid scalar type (%s) for argument 'points'. Expected one of ['float32', 'float64']." % points.dtype)
-        if points.dim() != 2 or points.shape[-1] != 3:
-            raise ValueError("Invalid shape for points, must be (n, 3) but got " + str(tuple(points.shape)))
-        if points.shape[0] == 0:
-            raise ValueError("Invalid point set with zero elements: points must have shape (n, 3)")
-        if num_neighbors is not None and int(num_neighbors) <= 0:
-            raise ValueError("Invalid number of neighbors (%d) must be greater than 0." % int(num_neighbors))
-        if view_directions is not None and (not _is_tensor(view_directions) or view_directions.dtype != points.dtype or
-                                            view_directions.device != points.device or
-                                            tuple(view_directions.shape) != tuple(points.shape)):
-            raise ValueError("Invalid view directions does not match the number of points. If view directions are passed "
-                             "in, they must be a tensor with the dtype, device and shape of points.")
-        points = points.detach().contiguous()
-        view_directions = None if view_directions is None else view_directions.detach().contiguous()
-        if points.is_cuda:
-            _same_device(points, device)
-            n = points.shape[0]
-            idx = torch.empty(n, dtype=torch.int64, device=points.device)
-            nrm = torch.empty((n, 3), dtype=points.dtype, device=points.device)
-            count = torch.empty(1, dtype=torch.int64, device=points.device)
-            launch(points, view_directions, idx, nrm, count, *_call_args(points))
-            m = int(count.item())
-            return idx[:m], nrm[:m]
-        points, view_directions = points.numpy(), None if view_directions is None else view_directions.numpy()
-    if type(points) != _np.ndarray:
-        raise ValueError("Invalid type for points, must be a NumPy array, but got " + str(type(points)) + ".")
-    if view_directions is None:
-        view_directions = _np.zeros([0, 3], dtype=points.dtype)
-    if type(view_directions) != _np.ndarray:
-        raise ValueError("Invalid type for view_directions, must be None or a NumPy array, but got " +
-                         str(type(view_directions)) + ".")
-    if len(points.shape) != 2 or points.shape[-1] != 3:
-        raise ValueError("Invalid shape for points, must be (n, 3) but got " + str(points.shape))
-    if len(view_directions.shape) != 2:
-        raise ValueError("Invalid shape for view_directions, must be (n, 3) but got " + str(view_directions.shape))
-    out = host(points, view_directions)
-    return tuple(_torch().from_numpy(o) for o in out) if tensor else out
+    """The call path of the two normal estimators.  numpy arrays and CPU tensors go to host(points, view directions) as
+    numpy arrays, the binding's host entry point, with a (0, 3) array for no view directions, as in the reference's
+    wrapper.  CUDA tensors go to launch(points, view directions or None, idx, normals, count, device index, stream); the
+    kept count is always read back, since even without view directions a row with a NaN or infinite coordinate is
+    dropped.  num_neighbors: the k-NN estimator's, checked with the points."""
+    arrays = [points] if view_directions is None else [points, view_directions]
+    form = _form(arrays, ["points", "view_directions"])
+    _check_float(points, "points")
+    if len(points.shape) != 2 or points.shape[1] != 3:
+        raise ValueError("Invalid shape for points, must be (n, 3) but got " + _shape(points))
+    if points.shape[0] == 0:                                            # validate_input, src/point_cloud_normals.cpp:25-33
+        raise ValueError("Invalid point set with zero elements: points must have shape (n, 3), but got points.shape = %s."
+                         % _shape(points))
+    if num_neighbors is not None and int(num_neighbors) <= 0:
+        raise ValueError("Invalid number of neighbors (%d) must be greater than 0." % int(num_neighbors))
+    if view_directions is not None:
+        _check_match(view_directions, "view_dirs", points, "points")
+        if len(view_directions.shape) != 2:
+            raise ValueError("Invalid shape for view_directions, must be (n, 3) but got " + _shape(view_directions))
+        # :34-42; an empty numpy array stands for no view directions there, as in the reference's binding
+        if tuple(view_directions.shape) != tuple(points.shape) and not (form == "numpy" and view_directions.shape[0] == 0):
+            raise ValueError("Invalid view directions does not match the number of points. If view directions are passed in, "
+                             "they must have the same shape as points. Got points.shape = %s, and view_dirs.shape = %s."
+                             % (_shape(points), _shape(view_directions)))
+    if form != "cuda":
+        points, dirs = (_numpy(arrays) + [None])[:2]
+        if dirs is None or dirs.shape[0] == 0:
+            dirs = _np.zeros([0, 3], dtype=points.dtype)
+        return _as_form(form, host(points, dirs))
+    torch = _torch()
+    _same_device(points, device)
+    points = points.detach().contiguous()
+    view_directions = None if view_directions is None else view_directions.detach().contiguous()
+    n = points.shape[0]
+    idx = torch.empty(n, dtype=torch.int64, device=points.device)
+    nrm = torch.empty((n, 3), dtype=points.dtype, device=points.device)
+    count = torch.empty(1, dtype=torch.int64, device=points.device)
+    launch(points, view_directions, idx, nrm, count, *_call_args(points))
+    m = int(count.item())
+    return idx[:m], nrm[:m]
 
 
 # ---------------------------------------------------------------------------------------------

@@ -8,39 +8,32 @@ all-gather of the per-pair values when the caller wants them all.
 import numpy as _np
 
 from . import _pcu_internal
-from ._call import _torch
+from ._call import _as_form, _asarrays, _call_args, _dtype_name, _form, _numpy, _torch
 
 
 def batched_chamfer(x, y, max_points_per_leaf=10, return_sum=False, device=-1):
     """x: (B, n, 3), y: (B, m, 3) float32, numpy or CUDA tensors -> (B,) Chamfer distances
     (and, with return_sum, their fp64 sum as computed on the device)."""
-    if type(x).__module__.startswith("torch"):
-        torch = _torch()
-        if not isinstance(y, torch.Tensor) or x.dtype != torch.float32 or y.dtype != torch.float32:
-            raise ValueError("batched_chamfer_distance: x and y must both be float32 tensors")
-        if x.dim() != 3 or y.dim() != 3 or x.shape[2] != 3 or y.shape[2] != 3 or x.shape[0] != y.shape[0]:
-            raise ValueError("batched_chamfer_distance: x and y must have shape (B, n, 3) and (B, m, 3)")
-        if x.shape[0] == 0 or x.shape[1] == 0 or y.shape[1] == 0:
-            raise ValueError("Invalid input set with zero elements: x and y must have shape (B, n, 3) and (B, m, 3)")
-        if not x.is_cuda:
-            out, total = _pcu_internal._batched_chamfer(x.numpy(), y.numpy(), int(max_points_per_leaf), int(device))
-            out = torch.from_numpy(_np.asarray(out))
-            return (out, total) if return_sum else out
-        if x.device != y.device:
-            raise ValueError("x and y must live on the same device")
-        xs, ys = x.detach().contiguous(), y.detach().contiguous()
-        B = xs.shape[0]
-        out = torch.empty(B, dtype=torch.float32, device=xs.device)
-        total = torch.empty((), dtype=torch.float64, device=xs.device)   # written by the last kernel of the call
-        want_sum = return_sum
-        _pcu_internal._batched_chamfer_device(xs.data_ptr(), ys.data_ptr(), B, xs.shape[1], ys.shape[1],
-                                              out.data_ptr(), total.data_ptr() if want_sum else 0,
-                                              int(max_points_per_leaf), xs.device.index or 0,
-                                              torch.cuda.current_stream(xs.device).cuda_stream)
-        if return_sum:
-            return out, total
-        return out
-    out, total = _pcu_internal._batched_chamfer(_np.asarray(x), _np.asarray(y), int(max_points_per_leaf), int(device))
+    arrays = _asarrays([x, y])
+    form = _form(arrays, ["x", "y"])
+    x, y = arrays
+    if _dtype_name(x) != "float32" or _dtype_name(y) != "float32":
+        raise ValueError("batched_chamfer_distance: x and y must both be float32")
+    if len(x.shape) != 3 or len(y.shape) != 3 or x.shape[2] != 3 or y.shape[2] != 3 or x.shape[0] != y.shape[0]:
+        raise ValueError("batched_chamfer_distance: x and y must have shape (B, n, 3) and (B, m, 3)")
+    if x.shape[0] == 0 or x.shape[1] == 0 or y.shape[1] == 0:
+        raise ValueError("Invalid input set with zero elements: x and y must have shape (B, n, 3) and (B, m, 3)")
+    if form != "cuda":
+        out, total = _pcu_internal._batched_chamfer_host(*_numpy([x, y]), int(max_points_per_leaf), int(device))
+        out = _as_form(form, out)
+        return (out, total) if return_sum else out
+    torch = _torch()
+    xs, ys = x.detach().contiguous(), y.detach().contiguous()
+    B = xs.shape[0]
+    out = torch.empty(B, dtype=torch.float32, device=xs.device)
+    total = torch.empty((), dtype=torch.float64, device=xs.device)   # written by the last kernel of the call
+    _pcu_internal._batched_chamfer_device(xs.data_ptr(), ys.data_ptr(), B, xs.shape[1], ys.shape[1], out.data_ptr(),
+                                          total.data_ptr() if return_sum else 0, int(max_points_per_leaf), *_call_args(xs))
     return (out, total) if return_sum else out
 
 
@@ -108,13 +101,11 @@ def distributed_chamfer_sum(x, y, exchange, max_points_per_leaf=10):
     the sum over ranks of that one fp64 on `exchange`'s side stream.  Returns the 1-element fp64 tensor that
     holds the all-rank sum once `exchange.wait()` has been called; no torch kernel and no host synchronisation
     sit between the sweep and the collective."""
-    from . import _both_stats, _STATS_WORDS
-    where, _, _, st = _both_stats(x, y, max_points_per_leaf)
-    if where != "cuda":
+    from . import _pair_value, _sweep
+    form, _, words, _, _ = _sweep(x, y, True, max_points_per_leaf, None)
+    if form != "cuda":
         raise ValueError("distributed_chamfer_sum wants CUDA tensors")
-    buf = st[0]
-    value64 = buf.view(_torch().float64)[_STATS_WORDS - 1:_STATS_WORDS]   # record 0's pair_value
-    return exchange.submit(value64)
+    return exchange.submit(_pair_value(words))
 
 
 def gather_values(vals, batch, group=None):

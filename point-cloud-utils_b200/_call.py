@@ -3,8 +3,9 @@
 numpy arrays in -> numpy out (each input is uploaded once through torch, to the GPU `device=` names, else
 `current_device()`); CUDA torch tensors in -> CUDA tensors out, on the device they live on (a `device=` that
 contradicts it is an error); CPU tensors -> CPU tensors (through numpy).  Arguments are validated, with the reference's
-messages, before any device call.  The nearest-neighbour family reaches the device through the binding's own entry
-points but takes its device rules (`_dev`, `_same_device`, `_call_args`) from here; its numpy calls never import torch."""
+messages, before any device call.  The nearest-neighbour family takes its forms, checks and device rules from here too,
+but its numpy arrays and CPU tensors go to the binding's host entry points, which stage them through the library's
+page-locked ring (`_numpy` in, `_as_form` out); its numpy calls never import torch."""
 import numpy as _np
 
 from . import _pcu_internal
@@ -106,6 +107,27 @@ def _check_match(x, name, ref, ref_name):
                          % (_dtype_name(x), name, ref_name, _dtype_name(ref)))
 
 
+def _shape(x):
+    """A shape as the reference's bindings print one: (n, 3)."""
+    return "(%s)" % ", ".join(str(int(s)) for s in x.shape)
+
+
+def _check_clouds(clouds, names):
+    """The reference's checks of one or two point sets, in its order: the first one's dtype, the second's against it,
+    then (n, 3) shapes with n > 0 (src/point_cloud_distance.cpp:133-149).  Anything with a dtype and a shape will do."""
+    _check_float(clouds[0], names[0])
+    for c, name in zip(clouds[1:], names[1:]):
+        _check_match(c, name, clouds[0], names[0])
+    shapes = [tuple(c.shape) for c in clouds]
+    if all(len(s) == 2 and s[0] > 0 and s[1] == 3 for s in shapes):
+        return
+    got = "%s must have shape %s. Got %s." % (" and ".join(names), " and ".join(("(n, 3)", "(m, 3)")[:len(names)]),
+                                             ", ".join("%s.shape = %s" % (n, _shape(c)) for c, n in zip(clouds, names)))
+    if any(len(s) != 2 for s in shapes) or all(s[0] > 0 for s in shapes):
+        raise ValueError("Only 3D inputs are supported: " + got)
+    raise ValueError("Invalid input set with zero elements: " + got)
+
+
 def _validate_mesh(v, f, face_dtypes):
     """The binding's dtype checks, then validate_mesh (src/common/common.h:131-148)."""
     _check_float(v, "v")
@@ -150,12 +172,28 @@ def _to_device(arrays, device):
             for a in arrays]
 
 
+def _numpy(arrays):
+    """The inputs as numpy arrays: CPU tensors as the arrays that share their memory."""
+    return [a.detach().numpy() if _is_tensor(a) else a for a in arrays]
+
+
+def _as_form(form, out):
+    """Host outputs (one or a tuple) in the form of the call's inputs: for CPU tensors every array becomes a tensor,
+    scalars stay as they are."""
+    if form != "cpu":
+        return out
+    torch = _torch()
+    if isinstance(out, tuple):
+        return tuple(torch.from_numpy(o) if isinstance(o, _np.ndarray) else o for o in out)
+    return torch.from_numpy(out) if isinstance(out, _np.ndarray) else out
+
+
 def _upload(form, arrays, device):
     """Contiguous CUDA tensors of the inputs, on the device of the call.  CPU tensors go through numpy."""
     if form == "cuda":
         _same_device(arrays[0], device)
         return [a.detach().contiguous() for a in arrays]
-    return _to_device([a.detach().numpy() if _is_tensor(a) else a for a in arrays], device)
+    return _to_device(_numpy(arrays), device)
 
 
 def _raise_bad(bad):

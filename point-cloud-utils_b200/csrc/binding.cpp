@@ -1,10 +1,12 @@
 // binding.cpp -- pybind11 module `_pcu_internal`, the layer between the Python package and the C ABI of
 // libpcu_b200.so (include/pcu_b200.h).  All computation goes through that ABI; there is no CPU implementation
-// behind these functions.  The module has three kinds of functions:
-//   - numpy entry points, which run the library's host entry points.  Those named after the reference's numpyeigen
-//     bindings (k_nearest_neighbors, one_sided_hausdorff_distance, the normal estimators, the Morton-code functions)
-//     keep its argument names, defaults, dtype and shape rules, error type (ValueError), int64 indices and squeezed
-//     outputs; the underscored ones (_chamfer_stats, _cloud_prepare, ...) serve the Python package;
+// behind these functions.  The drop-in boundary is the Python package: it checks every argument, with the reference's
+// rules and messages, before it calls in here.  The module has three kinds of functions:
+//   - numpy entry points, which run the library's host entry points.  The nearest-neighbour family's (`_*_host` and
+//     `_chamfer_stats`) take arrays the package has checked and keep only a guard against arrays their C entry point
+//     would read out of bounds; they return the library's int64 indices, squeezed k-NN outputs and statistics records
+//     as numpy records of pcu_b200_nn_stats.  The
+//     Morton-code functions are still named after the reference's bindings and keep its checks;
 //   - device entry points (`_*_device`), which the Python package uses for CUDA torch tensors: the caller passes
 //     data_ptr()s, a device and a stream handle; nothing is copied and nothing synchronises unless the C entry point
 //     says so.  Those that only forward to the C ABI are generated from the C signatures (Forward below); the rest
@@ -20,7 +22,6 @@
 #include <map>
 #include <memory>
 #include <mutex>
-#include <sstream>
 #include <stdexcept>
 #include <string>
 #include <tuple>
@@ -282,210 +283,108 @@ template <class H> auto destroy(int (*f)(H*)) {
     };
 }
 
-enum class Dt { f32, f64 };
-
-Dt common_dtype(const py::array& a, const py::array& b, const char* na, const char* nb) {
-    // numpyeigen: dense_float / dense_double only, second argument npe_matches(first)
-    // (point_cloud_distance.cpp:124-125, :187-188)
-    const bool a32 = a.dtype().is(py::dtype::of<float>()), a64 = a.dtype().is(py::dtype::of<double>());
-    if (!a32 && !a64) {
-        std::ostringstream ss;
-        ss << "Invalid scalar type (" << std::string(py::str(a.dtype())) << ") for argument '" << na
-           << "'. Expected one of ['float32', 'float64'].";
-        throw py::value_error(ss.str());
-    }
-    if (!b.dtype().is(a.dtype())) {
-        std::ostringstream ss;
-        ss << "Invalid scalar type (" << std::string(py::str(b.dtype())) << ") for argument '" << nb
-           << "'. Expected it to match argument '" << na << "' which is of type " << std::string(py::str(a.dtype())) << ".";
-        throw py::value_error(ss.str());
-    }
-    return a32 ? Dt::f32 : Dt::f64;
-}
-
-void check_shapes(const py::array& a, const py::array& b, const char* na, const char* nb) {
-    auto shape_str = [](const py::array& x) {
-        std::ostringstream ss;
-        ss << "(";
-        for (py::ssize_t i = 0; i < x.ndim(); ++i) ss << (i ? ", " : "") << x.shape(i);
-        ss << ")";
-        return ss.str();
-    };
-    if (a.ndim() != 2 || b.ndim() != 2) {
-        std::ostringstream ss;
-        ss << "Only 3D inputs are supported: " << na << " and " << nb << " must have shape (n, 3) and (m, 3). Got "
-           << na << ".shape = " << shape_str(a) << ", " << nb << ".shape = " << shape_str(b) << ".";
-        throw py::value_error(ss.str());
-    }
-    if (a.shape(0) == 0 || b.shape(0) == 0) {
-        std::ostringstream ss;
-        ss << "Invalid input set with zero elements: " << na << " and " << nb
-           << " must have shape (n, 3) and (m, 3). Got " << na << ".shape = " << shape_str(a) << ", " << nb
-           << ".shape = " << shape_str(b) << ".";
-        throw py::value_error(ss.str());
-    }
-    if (a.shape(1) != 3 || b.shape(1) != 3) {
-        std::ostringstream ss;
-        ss << "Only 3D inputs are supported: " << na << " and " << nb << " must have shape (n, 3) and (m, 3). Got "
-           << na << ".shape = " << shape_str(a) << ", " << nb << ".shape = " << shape_str(b) << ".";
-        throw py::value_error(ss.str());
-    }
-}
-
 template <typename T>
 py::array_t<T, py::array::c_style> dense(const py::array& a) {
     return py::array_t<T, py::array::c_style | py::array::forcecast>::ensure(a);
 }
 
+// The host entry points take arrays the Python package has checked against the reference's rules.  This guard only
+// keeps an array of another dtype or shape from reaching a C entry point, which would read out of bounds: a C-contiguous
+// (rows, 3) array of T (rows < 0: any number of rows), copied into one when it is laid out otherwise.
+template <typename T>
+py::array_t<T, py::array::c_style> points_of(const py::array& a, int64_t rows = -1) {
+    if (!a.dtype().is(py::dtype::of<T>()) || a.ndim() != 2 || a.shape(1) != 3 || (rows >= 0 && a.shape(0) != rows))
+        throw py::value_error("pcu_b200: expected an (n, 3) array of the points' dtype");
+    return dense<T>(a);
+}
+bool is_f64(const py::array& a) { return a.dtype().is(py::dtype::of<double>()); }
+
 // device < 0: the caller named none (the reference's interface has no such argument) -> the library's rule
 // (PCU_B200_DEVICE, the CUDA runtime's current device, LOCAL_RANK, 0; see pcu_b200_current_device)
 int current_device_or_default(int device) { return device < 0 ? pcu_b200_current_device() : device; }
 
-template <typename T>
-py::tuple knn_numpy(const py::array& q_in, const py::array& d_in, int k, bool squared, int leaf, int device) {
-    auto q = dense<T>(q_in);
-    auto d = dense<T>(d_in);
-    const int64_t n = q.shape(0), m = d.shape(0);
+// k nearest neighbours of numpy queries: (dists, corrs), squeezed as npe::move squeezes them (pinned for (n, 1) -> (n,)
+// by tests/test_examples.py:363-368).  knn(ws, queries, n, dists, corrs) runs the host entry point against the dataset.
+template <typename T, class F>
+py::tuple knn_host(const py::array& q_in, int k, int leaf, int device, F&& knn) {
+    auto q = points_of<T>(q_in);
+    const int64_t n = q.shape(0);
     py::array_t<T> dists = result_array<T>((py::ssize_t)n, (py::ssize_t)k);
     py::array_t<int64_t> corrs = result_array<int64_t>((py::ssize_t)n, (py::ssize_t)k);
-    int64_t tied = 0;
-    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        return pick<T>(pcu_b200_knn_host_f32, pcu_b200_knn_host_f64)(ws, q.data(), n, d.data(), m, k, squared, dists.mutable_data(),
-                                                                      corrs.mutable_data(), &tied);
-    });
-    // npe::move hands the matrix to numpy and squeezes every size-1 dimension
-    // (pinned for (n, 1) -> (n,) by tests/test_examples.py:363-368)
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) { return knn(ws, q.data(), n, dists.mutable_data(), corrs.mutable_data()); });
     return py::make_tuple(dists.attr("squeeze")(), corrs.attr("squeeze")());
 }
 
-py::tuple k_nearest_neighbors(const py::array& query_points, const py::array& dataset_points, int k,
-                              bool squared_distances, int max_points_per_leaf, int num_threads, int device) {
-    (void)num_threads;  // CPU thread count of the reference; results never depended on it
-    if (k <= 0) throw py::value_error("Invalid value for k (" + std::to_string(k) + ") must be greater than 0.");
-    const Dt dt = common_dtype(query_points, dataset_points, "query_points", "dataset_points");
-    check_shapes(query_points, dataset_points, "query_points", "dataset_points");
-    const int dev = current_device_or_default(device);
-    return dt == Dt::f32 ? knn_numpy<float>(query_points, dataset_points, k, squared_distances, max_points_per_leaf, dev)
-                         : knn_numpy<double>(query_points, dataset_points, k, squared_distances, max_points_per_leaf, dev);
-}
-
-py::dict stats_to_dict(const pcu_b200_nn_stats& s) {
-    py::dict d;
-    d["sum_dist"] = s.sum_dist;
-    d["sum_sq_dist"] = s.sum_sq_dist;
-    d["max_sq_dist"] = s.max_sq_dist;
-    d["argmax_query"] = s.argmax_query;
-    d["argmax_data"] = s.argmax_data;
-    d["n_queries"] = s.n_queries;
-    d["n_tied"] = s.n_tied;
-    d["n_far"] = s.n_far;
-    d["witness_tied"] = s.witness_tied;
-    d["pair_value"] = s.pair_value;
-    return d;
-}
-
 template <typename T>
-pcu_b200_nn_stats one_sided_numpy(const py::array& s_in, const py::array& t_in, int leaf, int device) {
-    auto s = dense<T>(s_in);
-    auto t = dense<T>(t_in);
-    pcu_b200_nn_stats st{};
-    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        return pick<T>(pcu_b200_nn_stats_host_f32, pcu_b200_nn_stats_host_f64)(ws, s.data(), s.shape(0), t.data(), t.shape(0), &st);
+py::tuple knn_numpy_t(const py::array& q, const py::array& d_in, int k, bool squared, int leaf, int device) {
+    auto d = points_of<T>(d_in);
+    return knn_host<T>(q, k, leaf, device, [&](pcu_b200_workspace* ws, const T* qp, int64_t n, T* dists, int64_t* corrs) {
+        int64_t tied = 0;
+        return pick<T>(pcu_b200_knn_host_f32, pcu_b200_knn_host_f64)(ws, qp, n, d.data(), d.shape(0), k, squared, dists, corrs, &tied);
     });
-    return st;
 }
-
-template <typename T>
-T metric_value(double max_sq, bool squared) {
-    const T d2 = (T)max_sq;  // exact: max_sq is the input-precision value widened
-    if (d2 == (T)-1) return d2;  // no query found a neighbour: the reference's padded distance, not its root
-    return squared ? d2 : (T)std::sqrt(d2);  // correctly rounded sqrt in the input precision (:84-88)
-}
-
-py::object one_sided_hausdorff_distance(const py::array& source, const py::array& target, bool return_index,
-                                        bool squared_distances, int max_points_per_leaf, int device) {
-    const Dt dt = common_dtype(source, target, "source", "target");
-    check_shapes(source, target, "source", "target");
+py::tuple knn_numpy(const py::array& q, const py::array& d, int k, bool squared, int leaf, int device) {
     const int dev = current_device_or_default(device);
-    const pcu_b200_nn_stats st = dt == Dt::f32 ? one_sided_numpy<float>(source, target, max_points_per_leaf, dev)
-                                               : one_sided_numpy<double>(source, target, max_points_per_leaf, dev);
-    const double value = dt == Dt::f32 ? (double)metric_value<float>(st.max_sq_dist, squared_distances)
-                                       : metric_value<double>(st.max_sq_dist, squared_distances);
-    if (return_index) return py::make_tuple(value, st.argmax_query, st.argmax_data);
-    return py::float_(value);
+    return is_f64(q) ? knn_numpy_t<double>(q, d, k, squared, leaf, dev) : knn_numpy_t<float>(q, d, k, squared, leaf, dev);
 }
 
-template <typename T>
-py::tuple chamfer_numpy(const py::array& x_in, const py::array& y_in, int leaf, int device) {
-    auto x = dense<T>(x_in);
-    auto y = dense<T>(y_in);
-    pcu_b200_nn_stats st[2] = {};
+// The fused statistics sweep(s) of numpy points x, one way or both: (the Chamfer value in the input precision, or None
+// one way; the record x -> y; the record y -> x, zero one way).  The records are numpy records of the struct itself
+// (PYBIND11_NUMPY_DTYPE below), the type the Python package reads device records as.
+// sweep(ws, x, n, records, value or nullptr) runs the host entry point against the second cloud.
+template <typename T, class F>
+py::tuple stats_host(const py::array& x_in, bool both, int leaf, int device, F&& sweep) {
+    auto x = points_of<T>(x_in);
+    py::array_t<pcu_b200_nn_stats> recs(2);
+    std::fill_n(recs.mutable_data(), 2, pcu_b200_nn_stats{});
     T v = 0;
-    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        return pick<T>(pcu_b200_chamfer_host_f32, pcu_b200_chamfer_host_f64)(ws, x.data(), x.shape(0), y.data(), y.shape(0), st, &v);
-    });
-    return py::make_tuple(py::dtype::of<T>().attr("type")(v), stats_to_dict(st[0]), stats_to_dict(st[1]));
+    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) { return sweep(ws, x.data(), x.shape(0), recs.mutable_data(), both ? &v : nullptr); });
+    return py::make_tuple(both ? py::object(py::dtype::of<T>().attr("type")(v)) : py::object(py::none()), recs[py::int_(0)], recs[py::int_(1)]);
 }
 
-// Fused bidirectional sweep on numpy inputs: (chamfer value in input precision, stats x->y, stats y->x)
-py::tuple chamfer_stats(const py::array& x_in, const py::array& y_in, int max_points_per_leaf, int device) {
-    const Dt dt = common_dtype(x_in, y_in, "x", "y");
-    check_shapes(x_in, y_in, "x", "y");
-    const int dev = current_device_or_default(device);
-    return dt == Dt::f32 ? chamfer_numpy<float>(x_in, y_in, max_points_per_leaf, dev)
-                         : chamfer_numpy<double>(x_in, y_in, max_points_per_leaf, dev);
-}
-
-// validate_input of the reference (src/point_cloud_normals.cpp:25-42) plus the npe dtype rule
-Dt validate_normals_input(const py::array& points, const py::array& view_dirs) {
-    const Dt dt = common_dtype(points, view_dirs, "points", "view_dirs");
-    auto shape_of = [](const py::array& a) {
-        std::ostringstream ss;
-        ss << "(";
-        for (py::ssize_t i = 0; i < a.ndim(); ++i) ss << (i ? ", " : "") << a.shape(i);
-        ss << ")";
-        return ss.str();
-    };
-    if (points.ndim() != 2 || points.shape(0) == 0 || points.shape(1) != 3)      // validate_input, :25-33
-        throw py::value_error("Invalid point set with zero elements: points must have shape (n, 3), but got points.shape = " +
-                              shape_of(points) + ".");
-    if (view_dirs.ndim() != 2 || (view_dirs.shape(0) != 0 && (view_dirs.shape(0) != points.shape(0) || view_dirs.shape(1) != 3)))
-        throw py::value_error("Invalid view directions does not match the number of points. If view directions are passed in, "
-                              "they must have the same shape as points. Got points.shape = " + shape_of(points) +
-                              ", and view_dirs.shape = " + shape_of(view_dirs) + ".");   // :34-42
-    return dt;
-}
-
-// estimate_point_cloud_normals_knn_internal (src/point_cloud_normals.cpp:375-411): (indices of the kept points,
-// their unit normals).  view_dirs is a (0, 3) array when no view directions are given, as in the reference's wrapper.
 template <typename T>
-py::tuple normals_knn_numpy(const py::array& p_in, const py::array& v_in, int k, int leaf, double drop_angle, int device) {
-    auto pts = dense<T>(p_in);
-    auto dirs = dense<T>(v_in);
+py::tuple stats_numpy_t(const py::array& x, const py::array& y_in, bool both, int leaf, int device) {
+    auto y = points_of<T>(y_in);
+    return stats_host<T>(x, both, leaf, device, [&](pcu_b200_workspace* ws, const T* xp, int64_t n, pcu_b200_nn_stats* st, T* v) {
+        return v ? pick<T>(pcu_b200_chamfer_host_f32, pcu_b200_chamfer_host_f64)(ws, xp, n, y.data(), y.shape(0), st, v)
+                 : pick<T>(pcu_b200_nn_stats_host_f32, pcu_b200_nn_stats_host_f64)(ws, xp, n, y.data(), y.shape(0), st);
+    });
+}
+py::tuple stats_numpy(const py::array& x, const py::array& y, int leaf, int device, bool both) {
+    const int dev = current_device_or_default(device);
+    return is_f64(x) ? stats_numpy_t<double>(x, y, both, leaf, dev) : stats_numpy_t<float>(x, y, both, leaf, dev);
+}
+
+// The normal estimators on numpy points (src/point_cloud_normals.cpp:303-411): (indices of the kept points, their unit
+// normals).  view_dirs is a (0, 3) array when no view directions are given, as in the reference's wrapper.
+// estimate(ws, points, n, view_dirs or nullptr, idx, normals, &kept) runs the host entry point.
+template <typename T, class F>
+py::tuple normals_host(const py::array& p_in, const py::array& v_in, int leaf, int device, F&& estimate) {
+    auto pts = points_of<T>(p_in);
     const int64_t n = pts.shape(0);
+    auto dirs = points_of<T>(v_in, v_in.ndim() == 2 && v_in.shape(0) == 0 ? 0 : n);
     const bool has_dirs = dirs.shape(0) != 0;
     py::array_t<int64_t> idx({(py::ssize_t)n});
     py::array_t<T> normals({(py::ssize_t)n, (py::ssize_t)3});
     int64_t kept = 0;
     on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        return pick<T>(pcu_b200_normals_knn_host_f32, pcu_b200_normals_knn_host_f64)(
-            ws, pts.data(), n, has_dirs ? dirs.data() : nullptr, k, drop_angle, idx.mutable_data(), normals.mutable_data(), &kept);
+        return estimate(ws, pts.data(), n, has_dirs ? dirs.data() : nullptr, idx.mutable_data(), normals.mutable_data(), &kept);
     });
     idx.resize({(py::ssize_t)kept});
     normals.resize({(py::ssize_t)kept, (py::ssize_t)3});
     return py::make_tuple(idx, normals);
 }
 
-py::tuple estimate_point_cloud_normals_knn_internal(const py::array& points, const py::array& view_dirs, int num_neighbors,
-                                                    int max_points_per_leaf, double drop_angle_threshold, int num_threads,
-                                                    int random_seed, int device) {
-    (void)num_threads; (void)random_seed;   // CPU threading / rand() seeding of the reference: no effect on the k-NN variant
-    if (num_neighbors <= 0)
-        throw py::value_error("Invalid number of neighbors (" + std::to_string(num_neighbors) + ") must be greater than 0.");
-    const Dt dt = validate_normals_input(points, view_dirs);
+template <typename T>
+py::tuple normals_knn_t(const py::array& p, const py::array& v, int k, double drop_angle, int leaf, int device) {
+    return normals_host<T>(p, v, leaf, device, [&](pcu_b200_workspace* ws, const T* pts, int64_t n, const T* dirs, int64_t* idx,
+                                                   T* normals, int64_t* kept) {
+        return pick<T>(pcu_b200_normals_knn_host_f32, pcu_b200_normals_knn_host_f64)(ws, pts, n, dirs, k, drop_angle, idx, normals, kept);
+    });
+}
+py::tuple normals_knn_numpy(const py::array& p, const py::array& v, int k, double drop_angle, int leaf, int device) {
     const int dev = current_device_or_default(device);
-    return dt == Dt::f32 ? normals_knn_numpy<float>(points, view_dirs, num_neighbors, max_points_per_leaf, drop_angle_threshold, dev)
-                         : normals_knn_numpy<double>(points, view_dirs, num_neighbors, max_points_per_leaf, drop_angle_threshold, dev);
+    return is_f64(p) ? normals_knn_t<double>(p, v, k, drop_angle, leaf, dev) : normals_knn_t<float>(p, v, k, drop_angle, leaf, dev);
 }
 
 // estimate_point_cloud_normals_ball_internal (src/point_cloud_normals.cpp:303-370), argument order of the reference
@@ -505,32 +404,17 @@ pcu_b200_ball_options ball_options(double radius, int min_pts, int max_pts, doub
 }
 
 template <typename T>
-py::tuple normals_ball_numpy(const py::array& p_in, const py::array& v_in, const pcu_b200_ball_options& o, int device) {
-    auto pts = dense<T>(p_in);
-    auto dirs = dense<T>(v_in);
-    const int64_t n = pts.shape(0);
-    const bool has_dirs = dirs.shape(0) != 0;
-    py::array_t<int64_t> idx({(py::ssize_t)n});
-    py::array_t<T> normals({(py::ssize_t)n, (py::ssize_t)3});
-    int64_t kept = 0;
-    on_workspace(device, kHostKey, kDefaultLeaf, [&](pcu_b200_workspace* ws) {
-        return pick<T>(pcu_b200_normals_ball_host_f32, pcu_b200_normals_ball_host_f64)(
-            ws, pts.data(), n, has_dirs ? dirs.data() : nullptr, &o, idx.mutable_data(), normals.mutable_data(), &kept);
+py::tuple normals_ball_t(const py::array& p, const py::array& v, const pcu_b200_ball_options& o, int device) {
+    return normals_host<T>(p, v, kDefaultLeaf, device, [&](pcu_b200_workspace* ws, const T* pts, int64_t n, const T* dirs,
+                                                            int64_t* idx, T* normals, int64_t* kept) {
+        return pick<T>(pcu_b200_normals_ball_host_f32, pcu_b200_normals_ball_host_f64)(ws, pts, n, dirs, &o, idx, normals, kept);
     });
-    idx.resize({(py::ssize_t)kept});
-    normals.resize({(py::ssize_t)kept, (py::ssize_t)3});
-    return py::make_tuple(idx, normals);
 }
-
-py::tuple estimate_point_cloud_normals_ball_internal(const py::array& points, const py::array& view_dirs, double radius,
-                                                     int min_pts_per_ball, int max_pts_per_ball, double drop_angle_threshold,
-                                                     int max_points_per_leaf, int num_threads, const std::string& weight_function,
-                                                     int random_seed, int device) {
-    (void)max_points_per_leaf; (void)num_threads;   // kd-tree leaf size / CPU threads of the reference: no effect on the result
+py::tuple normals_ball_numpy(const py::array& p, const py::array& v, double radius, int min_pts_per_ball, int max_pts_per_ball,
+                             double drop_angle_threshold, const std::string& weight_function, int random_seed, int device) {
     const pcu_b200_ball_options o = ball_options(radius, min_pts_per_ball, max_pts_per_ball, drop_angle_threshold, weight_function, random_seed);
-    const Dt dt = validate_normals_input(points, view_dirs);
     const int dev = current_device_or_default(device);
-    return dt == Dt::f32 ? normals_ball_numpy<float>(points, view_dirs, o, dev) : normals_ball_numpy<double>(points, view_dirs, o, dev);
+    return is_f64(p) ? normals_ball_t<double>(p, v, o, dev) : normals_ball_t<float>(p, v, o, dev);
 }
 
 void normals_ball_device(bool is_f64, uintptr_t points, int64_t n, uintptr_t view_dirs, double radius, int min_pts, int max_pts,
@@ -903,7 +787,7 @@ py::array morton_knn(const py::array& codes_in, const py::array& qcodes_in, int 
 // ---- prepared clouds (handles travel as integers; point-cloud-utils_b200/__init__.py wraps them in PreparedCloud) ----
 template <typename T>
 pcu_b200_cloud* cloud_prepare_numpy_t(const py::array& pts_in, int knn_k, int leaf, int device) {
-    auto p = dense<T>(pts_in);
+    auto p = points_of<T>(pts_in);
     pcu_b200_cloud* cloud = nullptr;
     on_workspace(device, kHostKey, leaf > 0 ? leaf : kDefaultLeaf, [&](pcu_b200_workspace* ws) {   // leaf 0: the library's default
         if (knn_k > 0)
@@ -913,15 +797,9 @@ pcu_b200_cloud* cloud_prepare_numpy_t(const py::array& pts_in, int knn_k, int le
     });
     return cloud;
 }
-uintptr_t cloud_prepare_numpy(const py::array& pts_in, int device, int knn_k, int leaf) {
-    const bool f32 = pts_in.dtype().is(py::dtype::of<float>()), f64 = pts_in.dtype().is(py::dtype::of<double>());
-    if (!f32 && !f64)
-        throw py::value_error("Invalid scalar type (" + std::string(py::str(pts_in.dtype())) + ") for argument 'points'. Expected one of ['float32', 'float64'].");
-    if (pts_in.ndim() != 2 || pts_in.shape(1) != 3 || pts_in.shape(0) == 0)
-        throw py::value_error("Only 3D inputs are supported: points must have shape (n, 3) with n > 0.");
+uintptr_t cloud_prepare_numpy(const py::array& pts, int device, int knn_k, int leaf) {
     const int dev = current_device_or_default(device);
-    return (uintptr_t)(f32 ? cloud_prepare_numpy_t<float>(pts_in, knn_k, leaf, dev)
-                           : cloud_prepare_numpy_t<double>(pts_in, knn_k, leaf, dev));
+    return (uintptr_t)(is_f64(pts) ? cloud_prepare_numpy_t<double>(pts, knn_k, leaf, dev) : cloud_prepare_numpy_t<float>(pts, knn_k, leaf, dev));
 }
 uintptr_t cloud_prepare_device(bool is_f64, uintptr_t pts, int64_t n, int device, uintptr_t stream, int knn_k, int leaf) {
     pcu_b200_cloud* cloud = nullptr;
@@ -934,71 +812,29 @@ uintptr_t cloud_prepare_device(bool is_f64, uintptr_t pts, int64_t n, int device
     });
     return (uintptr_t)cloud;
 }
-// k nearest neighbours of numpy points in a prepared cloud: (dists, corrs) like k_nearest_neighbors
+// k_nearest_neighbors and the statistics sweeps of numpy points against a prepared cloud of the precision cloud_is_f64
 template <typename T>
-py::tuple knn_prepared_numpy_t(const py::array& q_in, pcu_b200_cloud* cloud, int k, bool squared, int leaf, int device) {
-    auto q = dense<T>(q_in);
-    const int64_t n = q.shape(0);
-    py::array_t<T> dists = result_array<T>((py::ssize_t)n, (py::ssize_t)k);
-    py::array_t<int64_t> corrs = result_array<int64_t>((py::ssize_t)n, (py::ssize_t)k);
-    int64_t tied = 0;
-    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        return pick<T>(pcu_b200_knn_prepared_host_f32, pcu_b200_knn_prepared_host_f64)(ws, q.data(), n, cloud, k, squared,
-                                                                                        dists.mutable_data(), corrs.mutable_data(), &tied);
+py::tuple knn_prepared_numpy_t(const py::array& q, pcu_b200_cloud* cloud, int k, bool squared, int leaf, int device) {
+    return knn_host<T>(q, k, leaf, device, [&](pcu_b200_workspace* ws, const T* qp, int64_t n, T* dists, int64_t* corrs) {
+        int64_t tied = 0;
+        return pick<T>(pcu_b200_knn_prepared_host_f32, pcu_b200_knn_prepared_host_f64)(ws, qp, n, cloud, k, squared, dists, corrs, &tied);
     });
-    return py::make_tuple(dists.attr("squeeze")(), corrs.attr("squeeze")());
 }
-py::tuple knn_prepared_numpy(const py::array& q_in, uintptr_t cloud, bool cloud_is_f64, int k, bool squared, int max_points_per_leaf, int device) {
-    if (k <= 0) throw py::value_error("Invalid value for k (" + std::to_string(k) + ") must be greater than 0.");
-    const bool f32 = q_in.dtype().is(py::dtype::of<float>()), f64 = q_in.dtype().is(py::dtype::of<double>());
-    if ((!f32 && !f64) || f64 != cloud_is_f64)
-        throw py::value_error("Invalid scalar type (" + std::string(py::str(q_in.dtype())) + "): expected the prepared cloud's " +
-                              (cloud_is_f64 ? "float64" : "float32") + ".");
-    if (q_in.ndim() != 2 || q_in.shape(1) != 3)
-        throw py::value_error("Only 3D inputs are supported: points must have shape (n, 3).");
-    if (q_in.shape(0) == 0) throw py::value_error("Invalid input set with zero elements: points must have shape (n, 3) with n > 0.");
-    const int dev = current_device_or_default(device);
-    return f32 ? knn_prepared_numpy_t<float>(q_in, (pcu_b200_cloud*)cloud, k, squared, max_points_per_leaf, dev)
-               : knn_prepared_numpy_t<double>(q_in, (pcu_b200_cloud*)cloud, k, squared, max_points_per_leaf, dev);
+py::tuple knn_prepared_numpy(const py::array& q, uintptr_t cloud, bool cloud_is_f64, int k, bool squared, int leaf, int device) {
+    auto* y = (pcu_b200_cloud*)cloud;
+    return cloud_is_f64 ? knn_prepared_numpy_t<double>(q, y, k, squared, leaf, device) : knn_prepared_numpy_t<float>(q, y, k, squared, leaf, device);
 }
 
 template <typename T>
-py::tuple stats_prepared_numpy_t(const py::array& x_in, const pcu_b200_cloud* y, bool both, int leaf, int device) {
-    auto x = dense<T>(x_in);
-    pcu_b200_nn_stats st[2] = {};
-    T v = 0;
-    on_workspace(device, kHostKey, leaf, [&](pcu_b200_workspace* ws) {
-        return both ? pick<T>(pcu_b200_chamfer_prepared_host_f32, pcu_b200_chamfer_prepared_host_f64)(ws, x.data(), x.shape(0), y, st, &v)
-                    : pick<T>(pcu_b200_nn_stats_prepared_host_f32, pcu_b200_nn_stats_prepared_host_f64)(ws, x.data(), x.shape(0), y, st);
+py::tuple stats_prepared_numpy_t(const py::array& x, const pcu_b200_cloud* y, bool both, int leaf, int device) {
+    return stats_host<T>(x, both, leaf, device, [&](pcu_b200_workspace* ws, const T* xp, int64_t n, pcu_b200_nn_stats* st, T* v) {
+        return v ? pick<T>(pcu_b200_chamfer_prepared_host_f32, pcu_b200_chamfer_prepared_host_f64)(ws, xp, n, y, st, v)
+                 : pick<T>(pcu_b200_nn_stats_prepared_host_f32, pcu_b200_nn_stats_prepared_host_f64)(ws, xp, n, y, st);
     });
-    if (both) return py::make_tuple(py::dtype::of<T>().attr("type")(v), stats_to_dict(st[0]), stats_to_dict(st[1]));
-    return py::make_tuple(py::none(), stats_to_dict(st[0]));
 }
-// fused sweep(s) of numpy points against a prepared cloud: (value or None, stats[, stats])
-py::tuple stats_prepared_numpy(const py::array& x_in, uintptr_t cloud, bool cloud_is_f64, bool both, int max_points_per_leaf, int device) {
-    const bool f32 = x_in.dtype().is(py::dtype::of<float>()), f64 = x_in.dtype().is(py::dtype::of<double>());
-    if ((!f32 && !f64) || f64 != cloud_is_f64)
-        throw py::value_error("Invalid scalar type (" + std::string(py::str(x_in.dtype())) + "): expected the prepared cloud's " +
-                              (cloud_is_f64 ? "float64" : "float32") + ".");
-    if (x_in.ndim() != 2 || x_in.shape(1) != 3)
-        throw py::value_error("Only 3D inputs are supported: points must have shape (n, 3).");
-    if (x_in.shape(0) == 0) throw py::value_error("Invalid input set with zero elements: points must have shape (n, 3) with n > 0.");
-    const int dev = current_device_or_default(device);
+py::tuple stats_prepared_numpy(const py::array& x, uintptr_t cloud, bool cloud_is_f64, bool both, int leaf, int device) {
     auto* y = (const pcu_b200_cloud*)cloud;
-    return f32 ? stats_prepared_numpy_t<float>(x_in, y, both, max_points_per_leaf, dev)
-               : stats_prepared_numpy_t<double>(x_in, y, both, max_points_per_leaf, dev);
-}
-void stats_prepared_device(bool is_f64, bool both, uintptr_t a, int64_t n, uintptr_t cloud, uintptr_t out_stats, uintptr_t out_value,
-                           int max_points_per_leaf, int device, uintptr_t stream) {
-    auto* st = (pcu_b200_nn_stats*)out_stats;
-    auto* y = (const pcu_b200_cloud*)cloud;
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        if (both)
-            return is_f64 ? pcu_b200_chamfer_prepared_f64(ws, (const double*)a, n, y, st, (double*)out_value, (void*)stream)
-                          : pcu_b200_chamfer_prepared_f32(ws, (const float*)a, n, y, st, (float*)out_value, (void*)stream);
-        return is_f64 ? pcu_b200_nn_stats_prepared_f64(ws, (const double*)a, n, y, st, (void*)stream)
-                      : pcu_b200_nn_stats_prepared_f32(ws, (const float*)a, n, y, st, (void*)stream);
-    });
+    return cloud_is_f64 ? stats_prepared_numpy_t<double>(x, y, both, leaf, device) : stats_prepared_numpy_t<float>(x, y, both, leaf, device);
 }
 
 // ---- voxel-grid down-sampling on device pointers (the Python layer owns the arrays) ----
@@ -1015,26 +851,12 @@ void voxel_downsample_device(bool is_f64, uintptr_t pts, int64_t n, uintptr_t at
     });
 }
 
-void stats_device(bool is_f64, bool both, uintptr_t a, int64_t n, uintptr_t b, int64_t m, uintptr_t out_stats,
-                  uintptr_t out_value, int max_points_per_leaf, int device, uintptr_t stream) {
-    auto* st = (pcu_b200_nn_stats*)out_stats;
-    on_workspace(device, stream, max_points_per_leaf, [&](pcu_b200_workspace* ws) {
-        if (both)
-            return is_f64 ? pcu_b200_chamfer_f64(ws, (const double*)a, n, (const double*)b, m, st, (double*)out_value, (void*)stream)
-                          : pcu_b200_chamfer_f32(ws, (const float*)a, n, (const float*)b, m, st, (float*)out_value, (void*)stream);
-        return is_f64 ? pcu_b200_nn_stats_f64(ws, (const double*)a, n, (const double*)b, m, st, (void*)stream)
-                      : pcu_b200_nn_stats_f32(ws, (const float*)a, n, (const float*)b, m, st, (void*)stream);
-    });
-}
-
 // Batched Chamfer on numpy inputs: x (B, n, 3), y (B, m, 3) float32 -> ((B,) float32, fp64 sum)
 py::tuple batched_chamfer_numpy(const py::array& x_in, const py::array& y_in, int max_points_per_leaf, int device) {
-    if (!x_in.dtype().is(py::dtype::of<float>()) || !y_in.dtype().is(py::dtype::of<float>()))
-        throw py::value_error("batched_chamfer_distance: x and y must both be float32");
-    if (x_in.ndim() != 3 || y_in.ndim() != 3 || x_in.shape(2) != 3 || y_in.shape(2) != 3 || x_in.shape(0) != y_in.shape(0))
-        throw py::value_error("batched_chamfer_distance: x and y must have shape (B, n, 3) and (B, m, 3)");
-    if (x_in.shape(0) == 0 || x_in.shape(1) == 0 || y_in.shape(1) == 0)
-        throw py::value_error("Invalid input set with zero elements: x and y must have shape (B, n, 3) and (B, m, 3)");
+    // the guard of points_of for batches: float32, (B, n, 3) and (B, m, 3)
+    for (const py::array* a : {&x_in, &y_in})
+        if (!a->dtype().is(py::dtype::of<float>()) || a->ndim() != 3 || a->shape(2) != 3 || a->shape(0) != x_in.shape(0))
+            throw py::value_error("pcu_b200: expected (B, n, 3) float32 arrays");
     auto x = dense<float>(x_in);
     auto y = dense<float>(y_in);
     const int64_t B = x.shape(0), n = x.shape(1), m = y.shape(1);
@@ -1077,27 +899,21 @@ py::dict debug_kd_tree(const py::array& pts, int leaf, int device) {
 }  // namespace
 
 PYBIND11_MODULE(_pcu_internal, mod) {
-    mod.doc() = "H100-native nearest-neighbour bindings (drop-in for point_cloud_utils._pcu_internal on this path)";
-    mod.def("k_nearest_neighbors", &k_nearest_neighbors, py::arg("query_points"), py::arg("dataset_points"),
-            py::arg("k"), py::arg("squared_distances") = false, py::arg("max_points_per_leaf") = 10,
-            py::arg("num_threads") = -1, py::arg("device") = -1,
-            "Compute the k nearest neighbors (L2 distance) from each point in the query point cloud to the dataset "
-            "point cloud.  Returns (dists, corrs): (n, k) arrays, squeezed to (n,) when k == 1; corrs is int64.");
-    mod.def("one_sided_hausdorff_distance", &one_sided_hausdorff_distance, py::arg("source"), py::arg("target"),
-            py::arg("return_index") = true, py::arg("squared_distances") = false, py::arg("max_points_per_leaf") = 10,
-            py::arg("device") = -1,
-            "Compute the one sided Hausdorff distance from source to target.  Returns d or (d, i, j).");
-    mod.def("estimate_point_cloud_normals_knn_internal", &estimate_point_cloud_normals_knn_internal, py::arg("points"),
-            py::arg("view_dirs"), py::arg("num_neighbors"), py::arg("max_points_per_leaf") = 10,
-            py::arg("drop_angle_threshold") = 1.5707963267948966, py::arg("num_threads") = 0, py::arg("random_seed") = -1,
-            py::arg("device") = -1,
-            "Indices of the kept points and their unit normals (plane fit to the k nearest neighbours of each point).");
+    mod.doc() = "pcu_b200's native layer: host and device entry points of libpcu_b200.so for the Python package, which "
+                "checks every argument (the drop-in boundary is the package, not this module)";
+    mod.def("_knn_host", &knn_numpy);
+    mod.def("_knn_device", forward_to(pcu_b200_knn_f32, pcu_b200_knn_f64).pair_with_leaf());
+    PYBIND11_NUMPY_DTYPE(pcu_b200_nn_stats, sum_dist, sum_sq_dist, max_sq_dist, argmax_query, argmax_data, n_queries, n_tied, n_far,
+                         witness_tied, pair_value);
+    mod.def("_stats_dtype", []() { return py::dtype::of<pcu_b200_nn_stats>(); });
+    mod.def("_chamfer_stats", &stats_numpy, py::arg("x"), py::arg("y"), py::arg("max_points_per_leaf") = 10, py::arg("device") = -1,
+            py::arg("both") = true);
+    mod.def("_nn_stats_device", forward_to(pcu_b200_nn_stats_f32, pcu_b200_nn_stats_f64).pair_with_leaf());
+    mod.def("_chamfer_device", forward_to(pcu_b200_chamfer_f32, pcu_b200_chamfer_f64).pair_with_leaf());
+    mod.def("_resolve_witness_device", forward_to(pcu_b200_resolve_witness_f32, pcu_b200_resolve_witness_f64).pair_with_leaf());
+    mod.def("_normals_knn_host", &normals_knn_numpy);
     mod.def("_normals_knn_device", forward_to(pcu_b200_normals_knn_f32, pcu_b200_normals_knn_f64).pair_with_leaf());
-    mod.def("estimate_point_cloud_normals_ball_internal", &estimate_point_cloud_normals_ball_internal, py::arg("points"),
-            py::arg("view_dirs"), py::arg("radius"), py::arg("min_pts_per_ball"), py::arg("max_pts_per_ball") = -1,
-            py::arg("drop_angle_threshold") = 1.5707963267948966, py::arg("max_points_per_leaf") = 10, py::arg("num_threads") = 0,
-            py::arg("weight_function") = "constant", py::arg("random_seed") = -1, py::arg("device") = -1,
-            "Indices of the kept points and their unit normals (plane fit to the points in a ball around each point).");
+    mod.def("_normals_ball_host", &normals_ball_numpy);
     mod.def("_normals_ball_device", &normals_ball_device);
     mod.def("_poisson_disk_device", forward_to(pcu_b200_poisson_disk_f32, pcu_b200_poisson_disk_f64).pair());
     mod.def("_voronoi_centroids_device", &voronoi_centroids_device);
@@ -1160,16 +976,16 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_mesh_face_device", &mesh_face_device);
     mod.def("_mesh_vertex_normals_device", forward_to(pcu_b200_mesh_vertex_normals_f32, pcu_b200_mesh_vertex_normals_f64).pair());
     mod.def("_laplacian_smooth_device", &laplacian_smooth_device);
-    mod.def("_cloud_prepare", &cloud_prepare_numpy, py::arg("points"), py::arg("device") = -1, py::arg("knn_k") = 0,
-            py::arg("max_points_per_leaf") = 10);
+    mod.def("_cloud_prepare_host", &cloud_prepare_numpy);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),
             py::arg("stream"), py::arg("knn_k") = 0, py::arg("max_points_per_leaf") = 10);
-    mod.def("_knn_prepared", &knn_prepared_numpy);
+    mod.def("_knn_prepared_host", &knn_prepared_numpy);
     mod.def("_knn_prepared_device", forward_to(pcu_b200_knn_prepared_f32, pcu_b200_knn_prepared_f64).pair_with_leaf());
     mod.def("_cloud_destroy", destroy(pcu_b200_cloud_destroy));
     mod.def("_cloud_points", [](uintptr_t cloud) { return (uintptr_t)pcu_b200_cloud_points((const pcu_b200_cloud*)cloud); });
-    mod.def("_stats_prepared", &stats_prepared_numpy);
-    mod.def("_stats_prepared_device", &stats_prepared_device);
+    mod.def("_stats_prepared_host", &stats_prepared_numpy);
+    mod.def("_nn_stats_prepared_device", forward_to(pcu_b200_nn_stats_prepared_f32, pcu_b200_nn_stats_prepared_f64).pair_with_leaf());
+    mod.def("_chamfer_prepared_device", forward_to(pcu_b200_chamfer_prepared_f32, pcu_b200_chamfer_prepared_f64).pair_with_leaf());
     mod.def("_voxel_downsample_device", &voxel_downsample_device);
     mod.def("_deduplicate_device", forward_to(pcu_b200_deduplicate_f32, pcu_b200_deduplicate_f64).pair());
     mod.def("_pairwise_device", forward_to(pcu_b200_pairwise_distances_f32, pcu_b200_pairwise_distances_f64).pair());
@@ -1187,15 +1003,9 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("morton_knn", &morton_knn, py::arg("codes"), py::arg("qcodes"), py::arg("k"), py::arg("sort_dist") = true,
             py::arg("device") = -1,
             "Queries a sorted array of morton encoded points to find the (approximate) k nearest neighbors: (m, min(k, n)) int64.");
-    mod.def("_chamfer_stats", &chamfer_stats, py::arg("x"), py::arg("y"), py::arg("max_points_per_leaf") = 10,
-            py::arg("device") = -1);
-    mod.def("_batched_chamfer", &batched_chamfer_numpy, py::arg("x"), py::arg("y"), py::arg("max_points_per_leaf") = 10,
-            py::arg("device") = -1);
+    mod.def("_batched_chamfer_host", &batched_chamfer_numpy);
     mod.def("_batched_chamfer_device", forward_to(pcu_b200_batched_chamfer_f32).single_with_leaf());
     mod.def("_batched_chamfer_stats_device", forward_to(pcu_b200_debug_batched_chamfer_stats_f32).single_with_leaf());
-    mod.def("_knn_device", forward_to(pcu_b200_knn_f32, pcu_b200_knn_f64).pair_with_leaf());
-    mod.def("_stats_device", &stats_device);
-    mod.def("_resolve_witness_device", forward_to(pcu_b200_resolve_witness_f32, pcu_b200_resolve_witness_f64).pair_with_leaf());
     // diagnostics address a workspace by (device, stream); stream None = the numpy path's own workspace,
     // device < 0 = the device a call that names none would use
     auto key_of = [](const py::object& stream) { return stream.is_none() ? kHostKey : stream.cast<uintptr_t>(); };

@@ -1,6 +1,11 @@
-"""The point-cloud functions outside the nearest-neighbour sweep take their input forms and their device from one call
-path: numpy in -> numpy out, CUDA tensors in -> CUDA tensors out on their device, CPU tensors in -> CPU tensors out.
-On the CPU: every argument error comes before any device call, and device= is read the one way the package reads it.
+"""The point-cloud functions take their input forms and their device from one call path: numpy in -> numpy out, CUDA
+tensors in -> CUDA tensors out on their device, CPU tensors in -> CPU tensors out.  The nearest-neighbour family (k-NN,
+the Hausdorff distances, Chamfer, prepared clouds, batched Chamfer and the normal estimators) checks its arguments on
+that path too, with plain and prepared second arguments alike, before its numpy arrays and CPU tensors go to the
+binding's host entry points.
+On the CPU: every argument error comes before any device call, numpy arrays and CPU tensors raise the same message for
+the same mistake, and device= is read the one way the package reads it.  On the GPU, CUDA tensors raise those messages
+too, before any device call.
 On the GPU: numpy, CUDA-tensor and CPU-tensor calls of every function give results of the right form, dtype and
 device that are bit-identical (voxel means and the EMD value, fp64 sums in the order the device's atomics take: to
 rounding), and CUDA tensors with a contradicting device= raise."""
@@ -15,7 +20,7 @@ def _boom(*args, **kwargs):
 @pytest.fixture
 def no_device(monkeypatch):
     """The package with every way to the device replaced by an assertion: uploads (once device= has been checked), and
-    the binding's entry points."""
+    the binding's host and device entry points."""
     import pcu_b200 as pcu
     from pcu_b200 import _call
 
@@ -25,7 +30,7 @@ def no_device(monkeypatch):
 
     monkeypatch.setattr(_call, "_ordinal", upload)
     for name in dir(pcu._pcu_internal):
-        if name.endswith("_device") or name.endswith("_internal"):
+        if name.endswith(("_device", "_internal", "_host")) or name == "_chamfer_stats":
             monkeypatch.setattr(pcu._pcu_internal, name, _boom)
     return pcu
 
@@ -87,14 +92,20 @@ def _cases(pcu, torch):
         # normals
         (pcu.estimate_point_cloud_normals_knn, (p[:, :2], 5), {}, "Invalid shape for points"),
         (pcu.estimate_point_cloud_normals_knn, (p.tolist(), 5), {}, "Invalid type for points"),
-        (pcu.estimate_point_cloud_normals_knn, (t.half(), 5), {}, "Invalid scalar type (torch.float16) for argument 'points'"),
+        (pcu.estimate_point_cloud_normals_knn, (t.half(), 5), {}, "Invalid scalar type (float16) for argument 'points'"),
         (pcu.estimate_point_cloud_normals_knn, (t[:, :2], 5), {}, "Invalid shape for points"),
         (pcu.estimate_point_cloud_normals_knn, (t[:0], 5), {}, "Invalid point set with zero elements"),
         (pcu.estimate_point_cloud_normals_knn, (t, 0), {}, "Invalid number of neighbors (0)"),
         (pcu.estimate_point_cloud_normals_knn, (t, 5), {"view_directions": t[:10]}, "Invalid view directions"),
         (pcu.estimate_point_cloud_normals_ball, (p[:, :2], 0.1), {}, "Invalid shape for points"),
-        (pcu.estimate_point_cloud_normals_ball, (t.half(), 0.1), {}, "Invalid scalar type (torch.float16) for argument 'points'"),
-        (pcu.estimate_point_cloud_normals_ball, (t, 0.1), {"view_directions": p}, "Invalid view directions"),
+        (pcu.estimate_point_cloud_normals_ball, (t.half(), 0.1), {}, "Invalid scalar type (float16) for argument 'points'"),
+        (pcu.estimate_point_cloud_normals_ball, (t, 0.1), {"view_directions": p}, "Invalid type for points, must be a NumPy array"),
+        (pcu.estimate_point_cloud_normals_ball, (p, 0.1), {"view_directions": p.tolist()}, "Invalid type for view_directions"),
+        # nearest neighbours: numpy arrays and tensors do not mix (the rest is in _nn_cases)
+        (pcu.k_nearest_neighbors, (p, t, 1), {}, "Invalid type for dataset_points, must be a NumPy array"),
+        (pcu.chamfer_distance, (t, p), {}, "Invalid type for x, must be a NumPy array"),
+        (pcu.one_sided_hausdorff_distance, (t, p), {}, "Invalid type for source, must be a NumPy array"),
+        (pcu.batched_chamfer_distance, (torch.zeros((2, 5, 3)), np.zeros((2, 5, 3), np.float32)), {}, "Invalid type for x"),
         # Voronoi centroids
         (pcu.voronoi_centroids_unit_cube, (p.astype(np.int32),), {}, "Invalid scalar type (int32) for argument 'centers'"),
         (pcu.voronoi_centroids_unit_cube, (p[:, :2],), {}, "Invalid shape for centers"),
@@ -102,6 +113,99 @@ def _cases(pcu, torch):
         (pcu.voronoi_centroids_unit_cube, (p + 1.0,), {}, "Centers of voronoi diagram must lie in the unit cube [0, 1]^3"),
         (pcu.voronoi_centroids_unit_cube, (t + 1.0,), {}, "Centers of voronoi diagram must lie in the unit cube [0, 1]^3"),
     ]
+
+
+def _fake_cloud(pcu, handle, device_index=0):
+    """A PreparedCloud of 40 float64 points on cuda:device_index that holds no device memory (handle 0: closed)."""
+    class Fake(pcu.PreparedCloud):
+        def close(self):
+            self._handle = 0
+    return Fake(handle, 40, True, device_index, False)
+
+
+def _nn_cases(pcu, make):
+    """Argument errors of the nearest-neighbour family, with the arrays made by `make` from numpy arrays, and the message
+    each raises: the reference's checks in its order (k, dtypes, shapes), then a prepared cloud's."""
+    rng = np.random.default_rng(1)
+    a, b = rng.random((50, 3)), rng.random((40, 3))
+    cloud, closed = _fake_cloud(pcu, 1), _fake_cloud(pcu, 0)
+    ab = "query_points and dataset_points must have shape (n, 3) and (m, 3). Got query_points.shape = "
+    f32 = "Invalid scalar type (float64) for argument 'dataset_points'. Expected it to match argument 'query_points' which is of type float32."
+    batch = rng.random((2, 5, 3)).astype(np.float32)
+    cases = [
+        (pcu.k_nearest_neighbors, (a, b, 0), {}, "Invalid value for k (0) must be greater than 0."),
+        (pcu.k_nearest_neighbors, (a, cloud, -1), {}, "Invalid value for k (-1) must be greater than 0."),
+        (pcu.k_nearest_neighbors, (a.astype(np.int64), b, 1), {},
+         "Invalid scalar type (int64) for argument 'query_points'. Expected one of ['float32', 'float64']."),
+        (pcu.k_nearest_neighbors, (a.astype(np.float32), b, 1), {}, f32),
+        (pcu.k_nearest_neighbors, (a.astype(np.float32), cloud, 1), {}, f32),
+        (pcu.k_nearest_neighbors, (a[:, :2], b, 1), {}, "Only 3D inputs are supported: " + ab + "(50, 2), dataset_points.shape = (40, 3)."),
+        (pcu.k_nearest_neighbors, (a[:, :2], cloud, 1), {}, "Only 3D inputs are supported: " + ab + "(50, 2), dataset_points.shape = (40, 3)."),
+        (pcu.k_nearest_neighbors, (a[0], b, 1), {}, "Only 3D inputs are supported: " + ab + "(3), dataset_points.shape = (40, 3)."),
+        (pcu.k_nearest_neighbors, (a, b[:0], 1), {}, "Invalid input set with zero elements: " + ab + "(50, 3), dataset_points.shape = (0, 3)."),
+        (pcu.k_nearest_neighbors, (a[:0, :2], cloud, 1), {}, "Invalid input set with zero elements: " + ab + "(0, 2), dataset_points.shape = (40, 3)."),
+        (pcu.k_nearest_neighbors, (a, closed, 1), {}, "the PreparedCloud has been closed"),
+        (pcu.k_nearest_neighbors, (a, cloud, 1), {"device": 1}, "device=1 contradicts the prepared cloud, which lives on cuda:0"),
+        (pcu.k_nearest_neighbors, (a, b, 1), {"device": "cuda:99"}, "out of range"),
+        (pcu.one_sided_hausdorff_distance, (a, b[:, :1]), {}, "Only 3D inputs are supported: source and target must have shape"),
+        (pcu.one_sided_hausdorff_distance, (a[:0], cloud), {}, "Invalid input set with zero elements: source and target must"),
+        (pcu.one_sided_hausdorff_distance, (a, closed), {}, "the PreparedCloud has been closed"),
+        (pcu.one_sided_hausdorff_distance, (a, cloud), {"device": "cuda:1"}, "device='cuda:1' contradicts the prepared cloud"),
+        (pcu.hausdorff_distance, (a, b.astype(np.float32)), {}, "Invalid scalar type (float32) for argument 'y'. Expected it to match"),
+        (pcu.hausdorff_distance, (a.astype(np.float32), cloud), {}, "Invalid scalar type (float64) for argument 'y'. Expected it to match"),
+        (pcu.chamfer_distance, (a.astype(np.float16), b), {}, "Invalid scalar type (float16) for argument 'x'"),
+        (pcu.chamfer_distance, (a, closed), {}, "the PreparedCloud has been closed"),
+        (pcu.chamfer_distance, (a, cloud), {"device": 1}, "device=1 contradicts the prepared cloud"),
+        (pcu.chamfer_distance, (a, b[:, :2]), {"p_norm": 1}, "Only 3D inputs are supported: query_points and dataset_points"),
+        (pcu.chamfer_distance, (a, cloud), {"return_index": True}, "a PreparedCloud serves the fused metrics"),
+        (pcu.prepare_cloud, (a.astype(np.int32),), {}, "Invalid scalar type (int32) for argument 'points'"),
+        (pcu.prepare_cloud, (a[:0],), {}, "Invalid input set with zero elements: points must have shape (n, 3). Got points.shape = (0, 3)."),
+        (pcu.prepare_cloud, (a[:, :2],), {}, "Only 3D inputs are supported: points must have shape (n, 3). Got points.shape = (50, 2)."),
+        (pcu.prepare_cloud, (a,), {"k": 0}, "Invalid value for k (0) must be greater than 0."),
+        (pcu.batched_chamfer_distance, (batch, batch.astype(np.float64)), {}, "batched_chamfer_distance: x and y must both be float32"),
+        (pcu.batched_chamfer_distance, (batch, batch[:1]), {}, "must have shape (B, n, 3) and (B, m, 3)"),
+        (pcu.batched_chamfer_distance, (batch, batch[:, :0]), {}, "Invalid input set with zero elements"),
+        (pcu.estimate_point_cloud_normals_knn, (a.astype(np.int64), 5), {}, "Invalid scalar type (int64) for argument 'points'"),
+        (pcu.estimate_point_cloud_normals_knn, (a[:0], 5), {},
+         "Invalid point set with zero elements: points must have shape (n, 3), but got points.shape = (0, 3)."),
+        (pcu.estimate_point_cloud_normals_knn, (a, 5), {"view_directions": a.astype(np.float32)},
+         "Invalid scalar type (float32) for argument 'view_dirs'. Expected it to match argument 'points' which is of type float64."),
+        (pcu.estimate_point_cloud_normals_knn, (a, 5), {"view_directions": a[:10]},
+         "Invalid view directions does not match the number of points. If view directions are passed in, they must have the "
+         "same shape as points. Got points.shape = (50, 3), and view_dirs.shape = (10, 3)."),
+        (pcu.estimate_point_cloud_normals_ball, (a, 0.1), {"view_directions": a[:, 0]}, "Invalid shape for view_directions"),
+    ]
+    return [(fn, tuple(make(x) if isinstance(x, np.ndarray) else x for x in args),
+             {k: make(v) if isinstance(v, np.ndarray) else v for k, v in kwargs.items()}, msg) for fn, args, kwargs, msg in cases]
+
+
+def _raises(fn, args, kwargs, msg):
+    with pytest.raises(ValueError) as e:
+        fn(*args, **kwargs)
+    assert msg in str(e.value), (fn.__name__, msg, str(e.value))
+    return str(e.value)
+
+
+def test_nearest_neighbour_errors_come_before_any_device_call(no_device, monkeypatch):
+    """numpy arrays and CPU tensors: every argument error before any device call, and one message for one mistake."""
+    import torch
+    monkeypatch.setattr(no_device._pcu_internal, "_device_count", lambda: 2)   # device=1 names a device, not a range error
+    numpy = [_raises(*case) for case in _nn_cases(no_device, lambda a: a)]
+    cpu = [_raises(*case) for case in _nn_cases(no_device, torch.from_numpy)]
+    assert cpu == numpy
+
+
+@pytest.mark.gpu
+def test_nearest_neighbour_errors_on_cuda_tensors(no_device, monkeypatch):
+    """CUDA tensors: the same messages, before any device call; and a prepared cloud on another device."""
+    import torch
+    monkeypatch.setattr(no_device._pcu_internal, "_device_count", lambda: 2)
+    numpy = [_raises(*case) for case in _nn_cases(no_device, lambda a: a)]
+    cuda = [_raises(*case) for case in _nn_cases(no_device, lambda a: torch.from_numpy(a).cuda())]
+    assert cuda == numpy
+    x = torch.zeros((5, 3), dtype=torch.float64, device="cuda")
+    _raises(no_device.chamfer_distance, (x, _fake_cloud(no_device, 1, device_index=1)), {},
+            "x lives on cuda:0, the prepared cloud on cuda:1")
 
 
 def test_argument_errors_come_before_any_device_call(no_device):
