@@ -10,6 +10,8 @@ import os
 import numpy as np
 import pytest
 
+from meshes import icosphere, to_form, to_numpy
+
 IDX = [np.int32, np.int64]
 FORMS = ["numpy", "cuda", "cpu"]
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -113,43 +115,12 @@ def test_argument_errors(pcu):
         pcu.adjacency_list(f, True)                          # return_csr is keyword only
 
 
-# ---- meshes ---------------------------------------------------------------------------------------------------------
-def icosphere(level):
-    t = (1 + 5 ** 0.5) / 2
-    v = np.array([(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t),
-                  (t, 0, -1), (t, 0, 1), (-t, 0, -1), (-t, 0, 1)], np.float64)
-    f = np.array([(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2),
-                  (10, 7, 6), (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11),
-                  (6, 2, 10), (8, 6, 7), (9, 8, 1)], np.int64)
-    for _ in range(level):
-        e = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), 1)
-        uniq, inv = np.unique(e[:, 0] * len(v) + e[:, 1], return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, (v[uniq // len(v)] + v[uniq % len(v)]) / 2])
-        a, b, c = mid[:, 0], mid[:, 1], mid[:, 2]
-        f = np.concatenate([np.stack([f[:, 0], a, c], 1), np.stack([f[:, 1], b, a], 1), np.stack([f[:, 2], c, b], 1),
-                            np.stack([a, b, c], 1)])
-    return v, f
-
-
 # ---- GPU ------------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _np(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 def check(pcu, f, form="numpy"):
     """Both return forms of adjacency_list(f) against the restatement; returns the CSR."""
     import torch
     want = restate(f)
-    ft = _to(form, f)
+    ft = to_form(form, f)
     got = pcu.adjacency_list(ft, return_csr=True)
     assert isinstance(got, tuple) and len(got) == 2
     for g, w in zip(got, want):
@@ -157,7 +128,7 @@ def check(pcu, f, form="numpy"):
             assert isinstance(g, np.ndarray)
         else:
             assert isinstance(g, torch.Tensor) and g.is_cuda == (form == "cuda")
-        g = _np(g)
+        g = to_numpy(g)
         assert g.dtype == w.dtype and g.shape == w.shape and np.array_equal(g, w)
     lists = pcu.adjacency_list(ft)
     assert isinstance(lists, list) and lists == as_lists(*want)
@@ -174,7 +145,7 @@ def test_forms_and_dtypes(pcu, form, idt):
         f = random_faces(rng, m, hi, idt)
         check(pcu, f, form)
         if m <= 300:
-            assert pcu.adjacency_list(_to(form, f)) == literal(f)
+            assert pcu.adjacency_list(to_form(form, f)) == literal(f)
 
 
 @pytest.mark.gpu

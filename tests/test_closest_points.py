@@ -5,7 +5,8 @@ import inspect
 import numpy as np
 import pytest
 
-from test_mesh_sampling import MESHES, degenerate_mesh, flat_grid, icosphere, spanning_mesh  # noqa: F401
+from meshes import icosphere
+from test_mesh_sampling import MESHES, degenerate_mesh, flat_grid, spanning_mesh  # noqa: F401
 
 FDTYPES = [np.int32, np.int64, np.uint32, np.uint64]
 

@@ -11,6 +11,8 @@ import pytest
 import scipy.sparse
 import scipy.sparse.csgraph
 
+from meshes import icosphere, to_form, to_numpy
+
 IDX = [np.int32, np.int64, np.uint32, np.uint64]
 
 
@@ -141,25 +143,6 @@ def test_argument_errors():
 
 
 # ---- meshes ---------------------------------------------------------------------------------------------------------
-def icosphere(sub):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(sub):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        key = np.minimum(e[:, 0], e[:, 1]) * (1 << 32) + np.maximum(e[:, 0], e[:, 1])
-        uk, inv = np.unique(key, return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uk >> 32] + v[uk & 0xFFFFFFFF])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
-
-
 def lattice(k, lo=-1.0, hi=1.0):
     """(coordinates (k^3, 3), cubes ((k-1)^3, 8) int64) of a k^3 lattice, x fastest."""
     ax = np.linspace(lo, hi, k)
@@ -188,23 +171,11 @@ def two_spheres(pcu, k=64):
 
 
 # ---- the GPU --------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _np(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 def check(got, f):
     want = restate(f)
     assert len(got) == 4
     for g, w in zip(got, want):
-        g = _np(g)
+        g = to_numpy(g)
         assert same(g, w), (g.dtype, g.shape, w.dtype, w.shape)
 
 
@@ -226,7 +197,7 @@ def test_forms(pcu, form, idt):
     import torch
     v, f = icosphere(2)
     f = np.concatenate([f, f + len(v) + 5]).astype(idt)
-    got = pcu.connected_components(_to(form, v), _to(form, f))
+    got = pcu.connected_components(to_form(form, v), to_form(form, f))
     kinds = {"numpy": np.ndarray, "cuda": torch.Tensor, "cpu": torch.Tensor}
     for g in got:
         assert isinstance(g, kinds[form])
@@ -240,7 +211,7 @@ def test_vertex_range_and_shapes(pcu):
     v = np.random.default_rng(0).random((20, 3))
     f = np.array([[0, 1, 2], [3, 4, 5]], np.int64)           # max(f) + 1 = 6 < #v
     check(pcu.connected_components(v, f), f)
-    assert _np(pcu.connected_components(v, f)[0]).shape == (6,)
+    assert to_numpy(pcu.connected_components(v, f)[0]).shape == (6,)
     f = np.array([[0, 1, 2], [30, 4, 25]], np.int32)          # max(f) + 1 = 31 > #v
     check(pcu.connected_components(v, f), f)
     cv, nv, cf, nf = pcu.connected_components(v, np.array([[2, 0, 1]], np.int32))   # one face, one component

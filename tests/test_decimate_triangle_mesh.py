@@ -9,6 +9,8 @@ import pytest
 import scipy.sparse as sp
 from scipy.sparse.csgraph import connected_components
 
+from meshes import icosphere, noisy_icosphere
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 REJECTED = "produced an empty mesh"
 
@@ -138,27 +140,6 @@ def output(x, F, alive, vdtype, fdtype):
 
 
 # ---- meshes --------------------------------------------------------------------------------------------------------
-def icosphere(level):
-    t = (1 + 5 ** 0.5) / 2
-    v = [(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t),
-         (t, 0, -1), (t, 0, 1), (-t, 0, -1), (-t, 0, 1)]
-    f = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2), (10, 7, 6),
-         (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11), (6, 2, 10), (8, 6, 7),
-         (9, 8, 1)]
-    v = np.array(v, np.float64)
-    f = np.array(f, np.int64)
-    for _ in range(level):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        key = np.sort(e, 1)
-        uniq, inv = np.unique(key[:, 0] * len(v) + key[:, 1], return_inverse=True)
-        a, b = uniq // len(v), uniq % len(v)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, (v[a] + v[b]) / 2])
-        f = np.concatenate([np.stack([f[:, 0], mid[:, 0], mid[:, 2]], 1), np.stack([f[:, 1], mid[:, 1], mid[:, 0]], 1),
-                            np.stack([f[:, 2], mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
-
-
 def grid_faces(nu, nv, wrap_u, wrap_v):
     """Two triangles per cell of an nu x nv vertex grid, wrapped along u and / or v."""
     cu, cv = (nu if wrap_u else nu - 1), (nv if wrap_v else nv - 1)
@@ -198,12 +179,6 @@ def many_components():
         fs.append(f + off)
         off += len(v)
     return np.concatenate(vs), np.concatenate(fs)
-
-
-def noisy_icosphere(level=4, seed=1):
-    v, f = icosphere(level)
-    rng = np.random.default_rng(seed)
-    return v * (1 + 0.02 * rng.standard_normal((len(v), 1))), f
 
 
 def bunny():
@@ -445,7 +420,7 @@ def quality(v, f, res):
 # mean edge 0.9993 and Hausdorff 1.000; noisy icosphere at f // 10, 0.9993 and 1.000.  The bounds leave a margin.
 @pytest.mark.parametrize("name,frac", [("bunny", 4), ("noisy_icosphere", 10)])
 def test_quality_against_sequential_greedy(name, frac):
-    v, f = bunny() if name == "bunny" else noisy_icosphere()
+    v, f = bunny() if name == "bunny" else noisy_icosphere(4, 1, 0.02)
     target = len(f) // frac
     ours, ref = quality(v, f, decimate(v, f, target)), quality(v, f, greedy(v, f, target))
     assert ours[0] <= 1.02 * ref[0], (ours, ref)

@@ -9,6 +9,8 @@ import pytest
 import scipy.sparse
 import scipy.sparse.csgraph
 
+from meshes import to_form, to_numpy
+
 DTYPES = [np.int32, np.int64, np.float32, np.float64]
 
 
@@ -176,18 +178,6 @@ def test_argument_errors():
 
 
 # ---- the GPU ----------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _back(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("dtype", DTYPES)
 @pytest.mark.parametrize("form", ["numpy", "cuda", "cpu"])
@@ -197,10 +187,10 @@ def test_equals_restatement(pcu, dtype, form):
     for shape in [(37, 29, 41), (1, 1, 50), (70, 3, 1), (64, 64, 64), (5, 300, 7)]:
         g = random_grid(rng, shape, dtype, levels=2)
         seed = tuple(int(rng.integers(0, s)) for s in shape)
-        got = pcu.flood_fill_3d(_to(form, g), seed, -2.5)
+        got = pcu.flood_fill_3d(to_form(form, g), seed, -2.5)
         if form == "cuda":
             assert isinstance(got, torch.Tensor) and got.is_cuda
-        assert same(_back(got), restate(g, seed, -2.5)), shape
+        assert same(to_numpy(got), restate(g, seed, -2.5)), shape
 
 
 @pytest.mark.gpu

@@ -26,6 +26,8 @@ from contextlib import closing
 import numpy as np
 import pytest
 
+from meshes import to_numpy
+
 F32, F64 = np.float32, np.float64
 DTYPES = [F32, F64]
 KS_MAX = [1, 3, 8, 20, 40]     # thread lists of capacity 4 / 8 / 16 / 32, the warp pass and the k > 32 descent
@@ -230,10 +232,6 @@ def test_oracle_back_ends_agree(name, dtype, oracle):
 
 
 # ------------------------------------------------------------------------------------------------ GPU
-def _np(a):
-    return a.cpu().numpy() if hasattr(a, "cpu") else np.asarray(a)
-
-
 def _forms(pcu, q, d, k):
     """(label, query argument, dataset argument, closer) for every entry point of k_nearest_neighbors."""
     import torch
@@ -257,7 +255,7 @@ def test_knn_matches_oracle(name, dtype, k, pcu, oracle):
         rd, ri = oracle.k_nearest_neighbors(q, d, k, sq)
         for label, qa, da in _forms(pcu, q, d, k):
             gd, gi = pcu.k_nearest_neighbors(qa, da, k, sq)
-            gd, gi = _np(gd), _np(gi)
+            gd, gi = to_numpy(gd), to_numpy(gi)
             bad = np.flatnonzero((gi.reshape(len(q), -1) != ri.reshape(len(q), -1)).any(axis=1) |
                                  (gd.reshape(len(q), -1).view(np.uint8).reshape(len(q), -1) !=
                                   rd.reshape(len(q), -1).view(np.uint8).reshape(len(q), -1)).any(axis=1))
@@ -303,8 +301,8 @@ def test_metrics_match_oracle(name, dtype, pcu, oracle):
         xb, yb = np.stack([q[:n], q[:n]]), np.stack([d[:n], d[:n]])
         unfound_b = _unfound_rows(q[:n], d[:n]) + _unfound_rows(d[:n], q[:n])
         ref_b = float(oracle.chamfer_distance(q[:n], d[:n]))
-        for got in list(_np(pcu.batched_chamfer_distance(xb, yb))) + \
-                list(_np(pcu.batched_chamfer_distance(torch.from_numpy(xb).cuda(), torch.from_numpy(yb).cuda()))):
+        for got in list(to_numpy(pcu.batched_chamfer_distance(xb, yb))) + \
+                list(to_numpy(pcu.batched_chamfer_distance(torch.from_numpy(xb).cuda(), torch.from_numpy(yb).cuda()))):
             if unfound_b:
                 assert np.isinf(got) and got > 0
             else:
@@ -319,8 +317,8 @@ def test_metrics_match_oracle(name, dtype, pcu, oracle):
     rcham, rxy, ryx = oracle.chamfer_distance(q, d, return_index=True)
     for xa, ya in ((q, d), (qt, dt), (qt.cpu(), dt.cpu())):
         cham, cxy, cyx = pcu.chamfer_distance(xa, ya, return_index=True)
-        np.testing.assert_array_equal(_np(cxy), rxy)
-        np.testing.assert_array_equal(_np(cyx), ryx)
+        np.testing.assert_array_equal(to_numpy(cxy), rxy)
+        np.testing.assert_array_equal(to_numpy(cyx), ryx)
         cham = float(cham)
         assert cham == pytest.approx(float(rcham), rel=1e-5, abs=0), (type(xa), cham, rcham)
 
@@ -351,4 +349,4 @@ def test_spread_families_reach_the_slow_passes(dtype, fill, pcu, oracle):
         assert pcu.one_sided_hausdorff_distance(qt, lt, True, sq) == ref
     for k in KS_MAX:
         gd, gi = pcu.k_nearest_neighbors(qt, lt, k)
-        assert (_np(gi) == -1).all() and (_np(gd) == -1).all()
+        assert (to_numpy(gi) == -1).all() and (to_numpy(gd) == -1).all()

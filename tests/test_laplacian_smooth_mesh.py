@@ -8,7 +8,8 @@ icosphere, repeatability, the input forms and the RuntimeWarning of a capped sol
 import numpy as np
 import pytest
 
-from test_mesh_geometry import corner_dot, face_area, icosphere
+from meshes import noisy_icosphere, to_form, to_numpy
+from test_mesh_geometry import corner_dot, face_area
 
 DBL_EPS = np.finfo(np.float64).eps
 
@@ -134,12 +135,6 @@ def literal_smooth(v, f, num_iters, step_size=0.1, use_cotan_weights=False):
 
 
 # ---- meshes ---------------------------------------------------------------------------------------------------------
-def noisy_icosphere(sub, seed=0, amp=0.05):
-    v, f = icosphere(sub)
-    rng = np.random.default_rng(seed)
-    return v * (1.0 + amp * rng.standard_normal((len(v), 1))), f
-
-
 def twisted_cube(sub):
     """A unit cube's 12 triangles, loop-free midpoint subdivision `sub` times, twisted about z."""
     v = np.array([[x, y, z] for z in (0, 1) for y in (0, 1) for x in (0, 1)], np.float64) - 0.5
@@ -241,20 +236,8 @@ def test_argument_errors(pcu):
 
 
 # ---- the GPU --------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _np(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 def check_close(got, want, v):
-    got = _np(got)
+    got = to_numpy(got)
     assert got.dtype == want.dtype and got.shape == want.shape
     tol = 1e-9 * np.linalg.norm(v.astype(np.float64).max(0) - v.astype(np.float64).min(0))
     diff = np.abs(got.astype(np.float64) - want.astype(np.float64))
@@ -304,13 +287,13 @@ def test_forms_and_repeatability(pcu, form):
     v = v.astype(np.float32)
     kind = np.ndarray if form == "numpy" else torch.Tensor
     for cotan in (False, True):
-        a = pcu.laplacian_smooth_mesh(_to(form, v), _to(form, f), 3, 0.1, cotan)
-        b = pcu.laplacian_smooth_mesh(_to(form, v), _to(form, f), 3, 0.1, cotan)
+        a = pcu.laplacian_smooth_mesh(to_form(form, v), to_form(form, f), 3, 0.1, cotan)
+        b = pcu.laplacian_smooth_mesh(to_form(form, v), to_form(form, f), 3, 0.1, cotan)
         assert isinstance(a, kind) and (form == "numpy" or a.is_cuda == (form == "cuda"))
-        assert np.array_equal(_np(a).view(np.uint8), _np(b).view(np.uint8))
+        assert np.array_equal(to_numpy(a).view(np.uint8), to_numpy(b).view(np.uint8))
         check_close(a, restate_smooth(v, f, 3, 0.1, cotan), v)
-    z = pcu.laplacian_smooth_mesh(_to(form, v), _to(form, f), 0, use_cotan_weights=True)
-    assert isinstance(z, kind) and np.array_equal(_np(z), v)
+    z = pcu.laplacian_smooth_mesh(to_form(form, v), to_form(form, f), 0, use_cotan_weights=True)
+    assert isinstance(z, kind) and np.array_equal(to_numpy(z), v)
 
 
 @pytest.mark.gpu

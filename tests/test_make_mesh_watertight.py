@@ -7,6 +7,8 @@ import sys
 import numpy as np
 import pytest
 
+from meshes import icosphere, torus
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import mc_tables  # noqa: E402
@@ -262,39 +264,6 @@ def test_signature():
 
 
 # ---- meshes --------------------------------------------------------------------------------------------------------
-def icosphere(level):
-    t = (1 + 5 ** 0.5) / 2
-    v = [(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t),
-         (t, 0, -1), (t, 0, 1), (-t, 0, -1), (-t, 0, 1)]
-    f = [(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2), (10, 7, 6),
-         (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11), (6, 2, 10), (8, 6, 7),
-         (9, 8, 1)]
-    v = np.array(v, np.float64)
-    f = np.array(f, np.int64)
-    for _ in range(level):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        key = np.sort(e, 1)
-        uniq, inv = np.unique(key[:, 0] * len(v) + key[:, 1], return_inverse=True)
-        a, b = uniq // len(v), uniq % len(v)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, (v[a] + v[b]) / 2])
-        m01, m12, m20 = mid[:, 0], mid[:, 1], mid[:, 2]
-        f = np.concatenate([np.stack([f[:, 0], m01, m20], 1), np.stack([f[:, 1], m12, m01], 1),
-                            np.stack([f[:, 2], m20, m12], 1), np.stack([m01, m12, m20], 1)])
-    v /= np.linalg.norm(v, axis=1, keepdims=True)
-    return v, f
-
-
-def torus(R=1.0, r=0.35, nu=96, nv=48):
-    u, w = np.meshgrid(np.arange(nu) * 2 * np.pi / nu, np.arange(nv) * 2 * np.pi / nv, indexing="ij")
-    v = np.stack([(R + r * np.cos(w)) * np.cos(u), (R + r * np.cos(w)) * np.sin(u), r * np.sin(w)], -1).reshape(-1, 3)
-    i, j = np.meshgrid(np.arange(nu), np.arange(nv), indexing="ij")
-    a, b = i * nv + j, ((i + 1) % nu) * nv + j
-    c, d = ((i + 1) % nu) * nv + (j + 1) % nv, i * nv + (j + 1) % nv
-    f = np.concatenate([np.stack([a, b, c], -1).reshape(-1, 3), np.stack([a, c, d], -1).reshape(-1, 3)])
-    return v, f
-
-
 def cube(offset=(0.0, 0.0, 0.0)):
     v = CORNERS[[0, 1, 2, 3, 4, 5, 6, 7]].astype(np.float64) + np.asarray(offset)
     f = np.array([[0, 3, 2], [0, 2, 1], [4, 5, 6], [4, 6, 7], [0, 1, 5], [0, 5, 4], [3, 7, 6], [3, 6, 2], [0, 4, 7],

@@ -8,6 +8,8 @@ import sys
 import numpy as np
 import pytest
 
+from meshes import icosphere, to_form, to_numpy
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(ROOT, "tools"))
 import mc_tables  # noqa: E402
@@ -195,18 +197,6 @@ def assert_same(got, want):
     assert np.array_equal(gf.astype(np.int64), wf)
 
 
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _back(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("cdt", [np.float32, np.float64])
 @pytest.mark.parametrize("sdt", [np.float32, np.float64])
@@ -228,10 +218,10 @@ def test_forms(form):
     gc, ci = lattice(20, np.float32)
     s = (np.linalg.norm(gc, axis=1) - 0.55).astype(np.float32)[:, None]    # (n, 1) scalars
     for idt in (np.int32, np.uint64):
-        v, f = pcu.marching_cubes_sparse_voxel_grid(_to(form, s), _to(form, gc), _to(form, ci.astype(idt)), 0.0)
+        v, f = pcu.marching_cubes_sparse_voxel_grid(to_form(form, s), to_form(form, gc), to_form(form, ci.astype(idt)), 0.0)
         if form != "numpy":
             assert isinstance(v, torch.Tensor) and v.is_cuda == (form == "cuda") and f.is_cuda == (form == "cuda")
-        assert_same((_back(v), _back(f)), restate(s, gc, ci, 0.0))
+        assert_same((to_numpy(v), to_numpy(f)), restate(s, gc, ci, 0.0))
 
 
 @pytest.mark.gpu
@@ -300,12 +290,12 @@ def test_bad_indices_and_no_level_set():
         with pytest.raises(ValueError, match="outside"):
             pcu.marching_cubes_sparse_voxel_grid(s, gc, bad, 0.0)
         with pytest.raises(ValueError, match="outside"):
-            pcu.marching_cubes_sparse_voxel_grid(_to("cuda", s), _to("cuda", gc), _to("cuda", bad), 0.0)
+            pcu.marching_cubes_sparse_voxel_grid(to_form("cuda", s), to_form("cuda", gc), to_form("cuda", bad), 0.0)
     with pytest.raises(ValueError) as e:
         pcu.marching_cubes_sparse_voxel_grid(s, gc, ci, 5.25)
     assert str(e.value) == "No level set found for isovalue 5.250000"
     with pytest.raises(ValueError, match="No level set found for isovalue -7.000000"):
-        pcu.marching_cubes_sparse_voxel_grid(_to("cuda", s), _to("cuda", gc), _to("cuda", ci), -7)
+        pcu.marching_cubes_sparse_voxel_grid(to_form("cuda", s), to_form("cuda", gc), to_form("cuda", ci), -7)
     v, f = pcu.marching_cubes_sparse_voxel_grid(s, gc, ci, 0.0)    # the calls above left nothing behind
     assert_same((v, f), restate(s, gc, ci, 0.0))
 
@@ -363,24 +353,6 @@ def test_full_size_dense_against_torch_restatement():
     assert torch.equal(v.view(torch.int32), wv.view(torch.int32))
     assert torch.equal(f.long(), wf)
     assert f.dtype == torch.int32 and len(v) > 10 ** 5
-
-
-def icosphere(sub):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(sub):
-        edges = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), axis=1)
-        uniq, inv = np.unique(edges, axis=0, return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uniq[:, 0]] + v[uniq[:, 1]])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
 
 
 @pytest.mark.gpu

@@ -8,6 +8,8 @@ to 1e-10) and a 1.3 * 10^6-face icosphere."""
 import numpy as np
 import pytest
 
+from meshes import icosphere, to_form, to_numpy
+
 IDX = [np.int32, np.int64, np.uint32, np.uint64]
 DBL_MAX = np.finfo(np.float64).max
 
@@ -110,24 +112,6 @@ def random_mesh(rng, nv, m, vdt, idt):
     return v, f
 
 
-def icosphere(sub):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(sub):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        uk, inv = np.unique(np.minimum(e[:, 0], e[:, 1]) * (1 << 32) + np.maximum(e[:, 0], e[:, 1]), return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uk >> 32] + v[uk & 0xFFFFFFFF])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
-
-
 def fan(n):
     """n faces around vertex 0 (a pole), each with two rim vertices of its own ring."""
     ang = np.linspace(0.0, 2 * np.pi, n, endpoint=False)
@@ -205,27 +189,15 @@ def test_argument_errors(pcu):
 
 
 # ---- the GPU --------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _np(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 def same(got, want):
-    got = _np(got)
+    got = to_numpy(got)
     return got.dtype == want.dtype and got.shape == want.shape and np.array_equal(got.view(np.uint8), want.view(np.uint8))
 
 
 def close_angle(got, want, tol=1e-13):
     """Within tol per component in float64; in float32 within 1 ulp of the restatement, or within tol where a
     component is so close to 0 that its ulp is finer than tol."""
-    got = _np(got)
+    got = to_numpy(got)
     if got.dtype != want.dtype or got.shape != want.shape:
         return False
     diff = np.abs(got.astype(np.float64) - want.astype(np.float64))
@@ -263,8 +235,8 @@ def test_forms(pcu, form):
     rng = np.random.default_rng(3)
     v, f = random_mesh(rng, 400, 600, np.float32, np.int64)
     kind = np.ndarray if form == "numpy" else torch.Tensor
-    outs = [pcu.mesh_face_areas(_to(form, v), _to(form, f)), pcu.estimate_mesh_face_normals(_to(form, v), _to(form, f)),
-            pcu.estimate_mesh_vertex_normals(_to(form, v), _to(form, f), "area")]
+    outs = [pcu.mesh_face_areas(to_form(form, v), to_form(form, f)), pcu.estimate_mesh_face_normals(to_form(form, v), to_form(form, f)),
+            pcu.estimate_mesh_vertex_normals(to_form(form, v), to_form(form, f), "area")]
     assert all(isinstance(o, kind) and (form == "numpy" or o.is_cuda == (form == "cuda")) for o in outs)
     assert same(outs[0], restate_areas(v, f))
     assert same(outs[1], restate_face_normals(v, f))
@@ -294,7 +266,7 @@ def test_fan_around_one_vertex(pcu):
     for vdt in (np.float64, np.float32):
         v = v.astype(vdt)
         check_all(pcu, v, f, angle=False)
-        got, want = _np(pcu.estimate_mesh_vertex_normals(v, f, "angle")), restate_vertex_normals(v, f, "angle")
+        got, want = to_numpy(pcu.estimate_mesh_vertex_normals(v, f, "angle")), restate_vertex_normals(v, f, "angle")
         assert close_angle(got[1:], want[1:])
         # the pole sums 10^5 angles, each within an ulp or so of numpy's arctan2: the tolerance grows with the count
         assert close_angle(got[:1], want[:1], 1e5 * 1e-15)
@@ -307,7 +279,7 @@ def test_large_icosphere(pcu):
     for vdt in (np.float64, np.float32):
         check_all(pcu, v.astype(vdt), f)
     again = pcu.estimate_mesh_vertex_normals(v, f, "angle")
-    assert same(again, _np(pcu.estimate_mesh_vertex_normals(v, f, "angle")))
+    assert same(again, to_numpy(pcu.estimate_mesh_vertex_normals(v, f, "angle")))
 
 
 @pytest.mark.gpu

@@ -11,6 +11,7 @@ import numpy as np
 import pytest
 from scipy.stats import chi2
 
+from meshes import icosphere
 from test_poisson_disk import poisson_disk_indices
 
 M32 = np.uint64(0xFFFFFFFF)
@@ -107,28 +108,6 @@ def mesh_poisson(v, f, num_samples, radius, seed, oversampling_factor=40.0):
 
 
 # ---- meshes, generated from seeds ---------------------------------------------------------------------------------
-def icosphere(subdivisions, jitter=0.0, seed=0, dtype=np.float64):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(subdivisions):
-        edges = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), axis=1)
-        uniq, inv = np.unique(edges, axis=0, return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uniq[:, 0]] + v[uniq[:, 1]])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        ab, bc_, ca = mid[:, 0], mid[:, 1], mid[:, 2]
-        f = np.concatenate([np.stack([a, ab, ca], 1), np.stack([b, bc_, ab], 1), np.stack([c, ca, bc_], 1),
-                            np.stack([ab, bc_, ca], 1)])
-    v = v / np.linalg.norm(v, axis=1, keepdims=True)
-    if jitter:
-        v = v + jitter * np.random.default_rng(seed).standard_normal(v.shape)
-    return v.astype(dtype), f
-
-
 def flat_grid(n, dtype=np.float64):
     g = np.stack(np.meshgrid(np.arange(n + 1), np.arange(n + 1), indexing="ij"), -1).reshape(-1, 2)
     v = np.concatenate([g / n, np.zeros((len(g), 1))], axis=1)

@@ -14,6 +14,8 @@ import pytest
 import scipy.sparse
 import scipy.sparse.csgraph
 
+from meshes import icosphere, to_form, to_numpy
+
 IDX = [np.int32, np.int64, np.uint32, np.uint64]
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -24,11 +26,7 @@ def same(a, b):
 
 
 def same_pair(got, want):
-    return len(got) == 2 and all(same(_np(g), w) for g, w in zip(got, want))
-
-
-def _np(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
+    return len(got) == 2 and all(same(to_numpy(g), w) for g, w in zip(got, want))
 
 
 # ---- the literal transcription of libigl ----------------------------------------------------------------------------
@@ -345,37 +343,10 @@ def test_argument_errors():
 
 
 # ---- the GPU --------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
 def check(pcu, f):
     got = pcu.orient_mesh_faces(f)
     assert same_pair(got, restate(f))
     return got
-
-
-def icosphere(sub):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(sub):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        key = np.minimum(e[:, 0], e[:, 1]) * (1 << 32) + np.maximum(e[:, 0], e[:, 1])
-        uk, inv = np.unique(key, return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uk >> 32] + v[uk & 0xFFFFFFFF])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
 
 
 def welded_sphere(sub):
@@ -424,13 +395,13 @@ def test_forms_and_shapes(pcu, form, idt):
     f = np.concatenate([f, reverse_some(klein(5, 5), rng) + 500]).astype(idt)
     kinds = {"numpy": np.ndarray, "cuda": torch.Tensor, "cpu": torch.Tensor}
     for x in (f, f[:1], f[1:2], f[:2]):
-        got = pcu.orient_mesh_faces(_to(form, x))
+        got = pcu.orient_mesh_faces(to_form(form, x))
         for g in got:
             assert isinstance(g, kinds[form])
             if form != "numpy":
                 assert g.is_cuda == (form == "cuda")
         assert same_pair(got, restate(x))
-    ff, c = pcu.orient_mesh_faces(_to(form, f[:1]), "area")        # weighting_type is ignored
+    ff, c = pcu.orient_mesh_faces(to_form(form, f[:1]), "area")        # weighting_type is ignored
     assert tuple(ff.shape) == (3,) and tuple(c.shape) == () and int(c) == 0
 
 

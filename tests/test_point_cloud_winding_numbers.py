@@ -7,8 +7,8 @@ import math
 import numpy as np
 import pytest
 
+from meshes import icosphere
 from test_closest_points import assert_bits, queries
-from test_mesh_sampling import icosphere
 from test_winding_numbers import CLOSED
 
 # Twice the largest |w(beta = 2) - w(exact)| over every query set below and the full-size rows: 0.0568 (nested shells

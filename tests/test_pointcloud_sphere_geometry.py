@@ -10,6 +10,8 @@ import math
 import numpy as np
 import pytest
 
+from meshes import to_form, to_numpy
+
 STACKS = [1, 2, 3, 16]
 SLICES = [1, 2, 3, 32]
 
@@ -162,18 +164,6 @@ def test_zero_points_without_a_device(pcu):
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _np(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 def r_form(r, k):
     """Scalar, (N,), (N, 1), list; k = 0 takes r[0] for every point."""
     return [float(r[0]), r, r[:, None], list(r)][k % 4]
@@ -202,12 +192,12 @@ def test_forms(pcu, form):
     import torch
     for dtype in (np.float32, np.float64):
         p, r = cloud(5, 19, dtype)
-        for rk, rr in enumerate([0.25, r, r[:, None], list(r), _to(form, r) if form != "numpy" else r]):
-            v, f = pcu.pointcloud_sphere_geometry(_to(form, p), rr, 3, 5)
+        for rk, rr in enumerate([0.25, r, r[:, None], list(r), to_form(form, r) if form != "numpy" else r]):
+            v, f = pcu.pointcloud_sphere_geometry(to_form(form, p), rr, 3, 5)
             if form != "numpy":
                 assert isinstance(v, torch.Tensor) and v.is_cuda == (form == "cuda") and f.dtype == torch.int32
             wv, wf = restate(p, (np.full(19, 0.25) if rk == 0 else r).astype(dtype), 3, 5)
-            assert bits_equal(_np(v), wv) and bits_equal(_np(f), wf)
+            assert bits_equal(to_numpy(v), wv) and bits_equal(to_numpy(f), wf)
 
 
 @pytest.mark.gpu

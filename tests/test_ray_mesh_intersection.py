@@ -6,8 +6,8 @@ import inspect
 import numpy as np
 import pytest
 
+from meshes import icosphere
 from test_closest_points import FDTYPES, assert_bits
-from test_mesh_sampling import icosphere
 from test_winding_numbers import ALL_MESHES
 
 F32 = np.float32

@@ -8,6 +8,7 @@ import math
 import numpy as np
 import pytest
 
+from meshes import to_numpy
 from test_closest_points import assert_bits
 from test_ray_mesh_intersection import _as, ray_sets, restate
 
@@ -224,10 +225,6 @@ def _forms(pcu, form, *xs):
     return [t.cuda() for t in ts] if form == "cuda" else ts
 
 
-def _np(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 def _r_form(r, k):
     return [float(r[0]), r, r[:, None], list(r)][k % 4]
 
@@ -257,8 +254,8 @@ def test_geometry_matches_the_restatement(pcu, dtype, s):
         ev, ef = fan(p, n, _r_value(r, k, dtype), s, dtype)
         ev = ev.reshape(-1, 3)[np.concatenate([np.arange(len(p))[:, None] * (s + 1) + np.arange(s + 1)]).ravel()]
         assert type(v) is type(pf) or form != "numpy"
-        _assert_same(_np(v), ev.astype(dtype), "%s %s v" % (form, k))
-        assert _np(f).dtype == np.int32 and np.array_equal(_np(f), ef), form
+        _assert_same(to_numpy(v), ev.astype(dtype), "%s %s v" % (form, k))
+        assert to_numpy(f).dtype == np.int32 and np.array_equal(to_numpy(f), ef), form
 
 
 @pytest.mark.gpu
@@ -276,7 +273,7 @@ def test_casts_match_the_restatement(pcu, dtype, s):
             form = ("numpy", "cuda", "cpu")[k % 3]
             args = _forms(pcu, form, p, n, o, d)
             pid, t = pcu.ray_surfel_intersection(*args, _r_form(r, k) if k % 4 != 0 else r, s, near, far)
-            pid, t = _np(pid), _np(t)
+            pid, t = to_numpy(pid), to_numpy(t)
             what = "%s %s %s" % (name, form, (near, far))
             assert pid.dtype == np.int32 and np.array_equal(pid, epid), what
             assert_bits(t, et.astype(dtype), what + " t")

@@ -7,6 +7,8 @@ dtype and input form, the squeezed shapes, all-false and all-true masks, the uns
 import numpy as np
 import pytest
 
+from meshes import icosphere, to_form
+
 IDX = [np.int32, np.int64, np.uint32, np.uint64]
 
 
@@ -174,33 +176,6 @@ def test_argument_errors():
 
 
 # ---- the GPU --------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def icosphere8():
-    """The subdivision-8 icosphere (1 310 720 faces)."""
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(8):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        uk, inv = np.unique(np.minimum(e[:, 0], e[:, 1]) * (1 << 32) + np.maximum(e[:, 0], e[:, 1]), return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uk >> 32] + v[uk & 0xFFFFFFFF])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("vdt", [np.float32, np.float64])
 @pytest.mark.parametrize("idt", [np.int32, np.int64])
@@ -233,13 +208,13 @@ def test_forms(pcu, form):
     rng = np.random.default_rng(23)
     v, f = random_mesh(rng, 400, 600, np.float32, np.int64)
     mask = rng.random(400) < 0.8
-    got = pcu.remove_mesh_vertices(_to(form, v), _to(form, f), _to(form, mask))
+    got = pcu.remove_mesh_vertices(to_form(form, v), to_form(form, f), to_form(form, mask))
     kinds = {"numpy": np.ndarray, "cuda": torch.Tensor, "cpu": torch.Tensor}
     assert all(isinstance(g, kinds[form]) and (form == "numpy" or g.is_cuda == (form == "cuda")) for g in got)
     assert all_same(got, restate_mask(v, f, mask))
     for idt in (np.int32, np.uint32, np.uint64):
         fu = f.astype(idt)
-        got = pcu.remove_unreferenced_mesh_vertices(_to(form, v), _to(form, fu))
+        got = pcu.remove_unreferenced_mesh_vertices(to_form(form, v), to_form(form, fu))
         assert all(isinstance(g, kinds[form]) for g in got)
         assert all_same(got, restate_unref(v, fu))
 
@@ -278,7 +253,7 @@ def test_corner_errors(pcu):
 
 @pytest.mark.gpu
 def test_large_icosphere(pcu):
-    v, f = icosphere8()
+    v, f = icosphere(8)
     rng = np.random.default_rng(24)
     mask = v[:, 2] > -0.3
     assert all_same(pcu.remove_mesh_vertices(v, f, mask), restate_mask(v, f, mask))

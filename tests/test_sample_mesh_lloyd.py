@@ -9,7 +9,8 @@ import inspect
 import numpy as np
 import pytest
 
-from test_mesh_sampling import degenerate_mesh, dense_samples, flat_grid, icosphere, spanning_mesh
+from meshes import icosphere
+from test_mesh_sampling import degenerate_mesh, dense_samples, flat_grid, spanning_mesh
 from test_voronoi_lloyd import cell_moments
 
 

@@ -9,6 +9,7 @@ import bisect
 import numpy as np
 import pytest
 
+from meshes import to_form, to_numpy
 from oracle import oracle as O
 
 OVERFLOW = "Invalid vertex leads to an overflow integer. Perhaps grid_size is too small."
@@ -379,22 +380,6 @@ def test_signatures():
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _back(x, form):
-    if form == "numpy":
-        assert isinstance(x, np.ndarray)
-        return x
-    assert x.is_cuda == (form == "cuda")
-    return x.cpu().numpy()
-
-
 def _same(got, want):
     assert got.dtype == want.dtype, (got.dtype, want.dtype)
     assert got.shape == want.shape, (got.shape, want.shape)
@@ -411,13 +396,13 @@ def test_from_points_equals_restatement(form):
         for dt in (np.float32, np.float64):
             for size, origin in ((0.1, (0.0, 0.0, 0.0)), ((0.05, 0.2, 0.3), (0.5, -0.25, 1.0))):
                 pp = p.astype(dt)
-                g, idx = pcu.sparse_voxel_grid_from_pointcloud(_to(form, pp), size, origin)
+                g, idx = pcu.sparse_voxel_grid_from_pointcloud(to_form(form, pp), size, origin)
                 wg, widx = from_points(pp, np.broadcast_to(size, 3), origin)
-                _same(_back(g, form), wg.squeeze())
-                _same(_back(idx, form), widx.squeeze())
+                _same(to_numpy(g, form), wg.squeeze())
+                _same(to_numpy(idx, form), widx.squeeze())
     for bad in (np.inf, -np.inf, 1e10):
         with pytest.raises(ValueError) as e:
-            pcu.sparse_voxel_grid_from_pointcloud(_to(form, np.array([[0.0, 0.0, 0.0], [0.0, bad, 0.0]])), 1.0)
+            pcu.sparse_voxel_grid_from_pointcloud(to_form(form, np.array([[0.0, 0.0, 0.0], [0.0, bad, 0.0]])), 1.0)
         assert str(e.value) == OVERFLOW
 
 
@@ -433,29 +418,29 @@ def test_dilate_erode_hex_equal_restatement(form):
                 want = gg
                 for _ in range(count):
                     want = dilate_once(want)
-                _same(_back(pcu.dilate_sparse_voxel_grid(_to(form, gg), count), form), want if count == 0 else want.squeeze())
+                _same(to_numpy(pcu.dilate_sparse_voxel_grid(to_form(form, gg), count), form), want if count == 0 else want.squeeze())
             e = erode_once(gg)
-            _same(_back(pcu.erode_sparse_voxel_grid(_to(form, gg)), form), e.squeeze() if len(e) else e)
+            _same(to_numpy(pcu.erode_sparse_voxel_grid(to_form(form, gg)), form), e.squeeze() if len(e) else e)
             for hdt in (np.float32, np.float64, np.float16):
-                v, c = pcu.sparse_voxel_grid_to_hex_mesh(_to(form, gg), (0.3, 0.25, 0.5), (1.0, -2.0, 0.125), hdt)
+                v, c = pcu.sparse_voxel_grid_to_hex_mesh(to_form(form, gg), (0.3, 0.25, 0.5), (1.0, -2.0, 0.125), hdt)
                 wv, wc = hex_mesh(gg, (0.3, 0.25, 0.5), (1.0, -2.0, 0.125))
-                _same(_back(v, form), wv.astype(hdt))
-                _same(_back(c, form), wc.squeeze())
+                _same(to_numpy(v, form), wv.astype(hdt))
+                _same(to_numpy(c, form), wc.squeeze())
     b = block(9)
     want = b
     for _ in range(3):
         want = erode_once(want)
-    got = pcu.erode_sparse_voxel_grid(_to(form, b), 3)                 # 9^3 -> 7^3 -> 5^3 -> 3^3
-    _same(_back(got, form), want)
+    got = pcu.erode_sparse_voxel_grid(to_form(form, b), 3)                 # 9^3 -> 7^3 -> 5^3 -> 3^3
+    _same(to_numpy(got, form), want)
     assert len(want) == 27
-    one = pcu.erode_sparse_voxel_grid(_to(form, b), 4)                  # -> the single centre voxel, squeezed
-    _same(_back(one, form), np.array([4, 4, 4], np.int32))
-    empty = pcu.erode_sparse_voxel_grid(_to(form, block(2)))
-    assert _back(empty, form).shape == (0, 3)
+    one = pcu.erode_sparse_voxel_grid(to_form(form, b), 4)                  # -> the single centre voxel, squeezed
+    _same(to_numpy(one, form), np.array([4, 4, 4], np.int32))
+    empty = pcu.erode_sparse_voxel_grid(to_form(form, block(2)))
+    assert to_numpy(empty, form).shape == (0, 3)
     with pytest.raises(ValueError, match="Invalid grid_coordinates has zero rows!"):
-        pcu.erode_sparse_voxel_grid(_to(form, block(2)), 2)            # a round on the empty result, as in the reference
+        pcu.erode_sparse_voxel_grid(to_form(form, block(2)), 2)            # a round on the empty result, as in the reference
     with pytest.raises(ValueError, match=r"but got \(3, 1\)"):
-        pcu.erode_sparse_voxel_grid(_to(form, b), 5)                   # the squeezed one-row result, as in the reference
+        pcu.erode_sparse_voxel_grid(to_form(form, b), 5)                   # the squeezed one-row result, as in the reference
 
 
 @pytest.mark.gpu
@@ -466,7 +451,7 @@ def test_range_check():
         for fn in (pcu.dilate_sparse_voxel_grid, pcu.erode_sparse_voxel_grid, pcu.sparse_voxel_grid_to_hex_mesh):
             for form in ("numpy", "cuda"):
                 with pytest.raises(ValueError) as e:
-                    fn(_to(form, g))
+                    fn(to_form(form, g))
                 assert str(e.value) == OVERFLOW
 
 

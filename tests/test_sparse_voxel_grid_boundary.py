@@ -4,6 +4,7 @@ against a set-based neighbour test; argument errors; on the GPU, the function ag
 import numpy as np
 import pytest
 
+from meshes import to_form, to_numpy
 from oracle import oracle as O
 
 X = np.uint64(0x1249249249249249)
@@ -115,18 +116,6 @@ def test_argument_errors():
 
 
 # ---- GPU -----------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _back(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("form", ["numpy", "cuda", "cpu"])
 def test_equals_restatement(form):
@@ -138,11 +127,11 @@ def test_equals_restatement(form):
     for name, g in sets.items():
         for dt in (np.int32, np.int64):
             gg = g.astype(dt)
-            got = pcu.sparse_voxel_grid_boundary(_to(form, gg))
+            got = pcu.sparse_voxel_grid_boundary(to_form(form, gg))
             if form != "numpy":
                 assert got.is_cuda == (form == "cuda")
-            assert _back(got).dtype == np.int64
-            assert np.array_equal(_back(got), restate(gg)), (name, dt)
+            assert to_numpy(got).dtype == np.int64
+            assert np.array_equal(to_numpy(got), restate(gg)), (name, dt)
 
 
 @pytest.mark.gpu
@@ -152,7 +141,7 @@ def test_range_check_and_shapes():
         g = np.concatenate([block(3, dtype=np.int64), np.array([bad], np.int64)])
         for form in ("numpy", "cuda"):
             with pytest.raises(ValueError) as e:
-                pcu.sparse_voxel_grid_boundary(_to(form, g))
+                pcu.sparse_voxel_grid_boundary(to_form(form, g))
             assert str(e.value) == OVERFLOW
         if bad[2] != 2 ** 33:
             with pytest.raises(ValueError, match="overflow"):

@@ -5,6 +5,8 @@ that the reference's own documented pairing produces."""
 import numpy as np
 import pytest
 
+from meshes import to_form, to_numpy
+
 # the reference's tables (src/mesh_for_voxels.cpp)
 FACES = np.array([2, 7, 6, 2, 3, 7, 0, 4, 5, 0, 5, 1, 0, 2, 6, 0, 6, 4, 1, 7, 3, 1, 5, 7, 0, 3, 2, 0, 1, 3, 4, 6, 7, 4, 7, 5],
                  np.int32).reshape(12, 3)
@@ -78,22 +80,6 @@ def test_argument_errors():
 
 
 # ---- GPU ------------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _back(x, form):
-    if form == "numpy":
-        assert isinstance(x, np.ndarray)
-        return x
-    assert x.is_cuda == (form == "cuda")
-    return x.cpu().numpy()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("form", ["numpy", "cuda", "cpu"])
 def test_equals_restatement(form):
@@ -101,15 +87,15 @@ def test_equals_restatement(form):
     rng = np.random.default_rng(1)
     all_cases = list(cases()) + [(rng.integers(-300, 300, (10 ** 6, 3)).astype(np.int32), (0.01, 0.02, 0.03), (1.0, 2.0, 3.0), 0.05)]
     for ijk, size, origin, gap in all_cases:
-        v, f = pcu.voxel_grid_geometry(_to(form, ijk), size, origin, gap)
+        v, f = pcu.voxel_grid_geometry(to_form(form, ijk), size, origin, gap)
         wv, wf = restate(ijk, size, origin, gap)
-        v, f = _back(v, form), _back(f, form)
+        v, f = to_numpy(v, form), to_numpy(f, form)
         assert v.dtype == np.float32 and f.dtype == np.int32
         assert np.array_equal(v, wv) and np.array_equal(f, wf)
-    v, f = pcu.voxel_grid_geometry(_to(form, np.array([[1, 2, 3]], np.int64)), 2.0)
-    assert _back(v, form).shape == (8, 3) and _back(f, form).shape == (12, 3)
-    v, _ = pcu.voxel_grid_geometry(_to(form, np.array([[0, 0, 0]], np.int32)), float("nan"))   # NaN passes, as there
-    assert np.isnan(_back(v, form)).all()
+    v, f = pcu.voxel_grid_geometry(to_form(form, np.array([[1, 2, 3]], np.int64)), 2.0)
+    assert to_numpy(v, form).shape == (8, 3) and to_numpy(f, form).shape == (12, 3)
+    v, _ = pcu.voxel_grid_geometry(to_form(form, np.array([[0, 0, 0]], np.int32)), float("nan"))   # NaN passes, as there
+    assert np.isnan(to_numpy(v, form)).all()
 
 
 @pytest.mark.gpu

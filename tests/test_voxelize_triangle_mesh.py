@@ -7,6 +7,8 @@ import math
 import numpy as np
 import pytest
 
+from meshes import to_form, to_numpy
+
 INDEX_DTYPES = [np.int32, np.int64, np.uint32, np.uint64]
 
 
@@ -246,18 +248,6 @@ def test_argument_errors():
 
 
 # ---- the GPU ----------------------------------------------------------------------------------------------------------
-def _to(form, a):
-    import torch
-    if form == "numpy":
-        return a
-    t = torch.from_numpy(np.ascontiguousarray(a))
-    return t.cuda() if form == "cuda" else t
-
-
-def _back(x):
-    return x if isinstance(x, np.ndarray) else x.cpu().numpy()
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("vdt", [np.float32, np.float64])
 @pytest.mark.parametrize("idt", INDEX_DTYPES)
@@ -277,12 +267,12 @@ def test_forms(pcu, oracle, form):
     import torch
     rng = np.random.default_rng(4)
     v, f = random_mesh(rng, nv=200, nf=500, scale=2.0, dtype=np.float32)
-    got = pcu.voxelize_triangle_mesh(_to(form, v), _to(form, f), (0.4, 0.6, 0.5), (0.1, 0.2, 0.3))
+    got = pcu.voxelize_triangle_mesh(to_form(form, v), to_form(form, f), (0.4, 0.6, 0.5), (0.1, 0.2, 0.3))
     if form == "cuda":
         assert isinstance(got, torch.Tensor) and got.is_cuda and got.dtype == torch.int32
     elif form == "cpu":
         assert isinstance(got, torch.Tensor) and not got.is_cuda
-    assert np.array_equal(_back(got), restate(v, f, (0.4, 0.6, 0.5), (0.1, 0.2, 0.3), oracle))
+    assert np.array_equal(to_numpy(got), restate(v, f, (0.4, 0.6, 0.5), (0.1, 0.2, 0.3), oracle))
 
 
 @pytest.mark.gpu

@@ -8,8 +8,9 @@ import math
 import numpy as np
 import pytest
 
+from meshes import icosphere, torus
 from test_closest_points import FDTYPES, assert_bits, queries
-from test_mesh_sampling import MESHES, icosphere
+from test_mesh_sampling import MESHES
 
 # Twice the largest |w(beta = 2) - w(exact)| over every query set below and the full-size rows: 0.00976, measured on
 # an H100 80GB HBM3, the same for fp32 and fp64 inputs.
@@ -70,18 +71,6 @@ def exact_w(q, v, f, chunk=64, bound=False):
 
 
 # ---- meshes ---------------------------------------------------------------------------------------------------------
-def torus(nu=40, nv=20, R=1.0, r=0.4, dtype=np.float64):
-    u = 2 * np.pi * np.arange(nu) / nu
-    t = 2 * np.pi * np.arange(nv) / nv
-    uu, tt = np.meshgrid(u, t, indexing="ij")
-    v = np.stack([(R + r * np.cos(tt)) * np.cos(uu), (R + r * np.cos(tt)) * np.sin(uu), r * np.sin(tt)], -1).reshape(-1, 3)
-    i, j = np.meshgrid(np.arange(nu), np.arange(nv), indexing="ij")
-    a, b = i * nv + j, ((i + 1) % nu) * nv + j
-    c, d = ((i + 1) % nu) * nv + (j + 1) % nv, i * nv + (j + 1) % nv
-    f = np.concatenate([np.stack([a, b, c], -1).reshape(-1, 3), np.stack([a, c, d], -1).reshape(-1, 3)])
-    return v.astype(dtype), f.astype(np.int64)
-
-
 def nested(opposite, dtype=np.float64):
     v, f = icosphere(3, 0.0, 0, dtype)
     inner = f[:, ::-1] if opposite else f
@@ -100,7 +89,7 @@ def doubled(dtype=np.float64):
 
 ALL_MESHES = dict(MESHES)
 ALL_MESHES.update({
-    "torus": lambda dt: torus(dtype=dt),
+    "torus": lambda dt: torus(40, 20, 0.4, dt),
     "nested": lambda dt: nested(False, dt),
     "nested-opposite": lambda dt: nested(True, dt),
     "reversed": reversed_sphere,
@@ -110,7 +99,7 @@ ALL_MESHES.update({
 # For the closed meshes: (query, winding number) pairs well away from the surface.
 CLOSED = {
     "icosphere": lambda dt: (icosphere(3, 0.01, 1, dt), [((0, 0, 0), 1), ((0.3, -0.2, 0.5), 1), ((1.5, 0, 0), 0), ((0, 3, 1), 0)]),
-    "torus": lambda dt: (torus(dtype=dt), [((1, 0, 0), 1), ((0, -1.1, 0.1), 1), ((0, 0, 0), 0), ((0, 0, 1), 0), ((2, 2, 0), 0)]),
+    "torus": lambda dt: (torus(40, 20, 0.4, dt), [((1, 0, 0), 1), ((0, -1.1, 0.1), 1), ((0, 0, 0), 0), ((0, 0, 1), 0), ((2, 2, 0), 0)]),
     "nested": lambda dt: (nested(False, dt), [((0, 0, 0), 2), ((0, 0.75, 0), 1), ((0, 0, 2), 0)]),
     "nested-opposite": lambda dt: (nested(True, dt), [((0, 0, 0), 0), ((0, 0.75, 0), 1), ((0, 0, 2), 0)]),
     "reversed": lambda dt: (reversed_sphere(dt), [((0, 0, 0), -1), ((0.2, 0.1, 0), -1), ((0, 0, 1.5), 0)]),
@@ -302,7 +291,7 @@ def test_scale_does_not_matter(pcu, vdtype, scale):
 @pytest.mark.gpu
 @pytest.mark.parametrize("vdtype", [np.float32, np.float64])
 def test_determinism(pcu, vdtype):
-    v, f = torus(dtype=vdtype)
+    v, f = torus(40, 20, 0.4, vdtype)
     p = queries(v, f, 3000, 11)
     w = pcu.triangle_soup_fast_winding_number(v, f, p)
     assert_bits(pcu.triangle_soup_fast_winding_number(v, f, p), w, "second call")

@@ -16,36 +16,20 @@ bandwidth.
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+from meshes import icosphere  # noqa: E402
+from timing import card, timeit  # noqa: E402
 import pcu_b200 as pcu  # noqa: E402
 
 PEAK_BYTES = 3.35e12
 PHASES = [("validate", ("cc_validate",)), ("edges", ("lap_edge",)), ("sort", ("sort_",)),
           ("runs", ("mc_heads", "keep_count", "keep_offsets")), ("csr", ("adj_entries", "mg_rows")), ("emit", ("adj_emit",))]
-
-
-def icosphere(level):
-    t = (1 + 5 ** 0.5) / 2
-    v = np.array([(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t),
-                  (t, 0, -1), (t, 0, 1), (-t, 0, -1), (-t, 0, 1)], np.float64)
-    f = np.array([(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2),
-                  (10, 7, 6), (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11),
-                  (6, 2, 10), (8, 6, 7), (9, 8, 1)], np.int64)
-    for _ in range(level):
-        e = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), 1)
-        uniq, inv = np.unique(e[:, 0] * len(v) + e[:, 1], return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, (v[uniq // len(v)] + v[uniq % len(v)]) / 2])
-        a, b, c = mid[:, 0], mid[:, 1], mid[:, 2]
-        f = np.concatenate([np.stack([f[:, 0], a, c], 1), np.stack([f[:, 1], b, a], 1), np.stack([f[:, 2], c, b], 1),
-                            np.stack([a, b, c], 1)])
-    return v, f
 
 
 def host_csr(f):
@@ -119,22 +103,13 @@ def sphere_rows():
             p = torch.from_numpy(rng.standard_normal((n, 3))).to(device="cuda", dtype=dt)
             r = torch.from_numpy(0.01 + 0.01 * rng.random(n)).to(device="cuda", dtype=dt)
             call = lambda: pcu.pointcloud_sphere_geometry(p, r, stacks, slices)   # noqa: E731
-            call()
-            torch.cuda.synchronize()
-            times = []
-            for _ in range(10):
-                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                a.record()
-                call()
-                b.record()
-                b.synchronize()
-                times.append(a.elapsed_time(b))
+            call_ms, call_ms_min = timeit(call, warm=1, flush=False)
             kern = kernel_ms(call, lambda name: "kernel" if "sp_geometry" in name else None).get("kernel", float("nan"))
             V, F, size = (stacks + 1) * (slices + 1), 2 * (stacks - 1) * slices, p.element_size()
             moved = n * (V * 3 * size + F * 12 + 4 * size)
             row = {"what": "pointcloud_sphere_geometry", "points": n, "stacks": stacks, "slices": slices,
                    "dtype": str(dt).replace("torch.", ""), "vertices": n * V, "faces": n * F, "bytes": moved,
-                   "call_ms": round(statistics.median(times), 4), "call_ms_min": round(min(times), 4), "kernel_ms": kern,
+                   "call_ms": round(call_ms, 4), "call_ms_min": round(call_ms_min, 4), "kernel_ms": kern,
                    "kernel_TBps": round(moved / (kern * 1e-3) / 1e12, 3), "share_of_3.35TBps": round(moved / (kern * 1e-3) / PEAK_BYTES, 3)}
             print(json.dumps(row), flush=True)
             rows.append(row)
@@ -144,8 +119,7 @@ def sphere_rows():
 
 
 def main():
-    print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip(), flush=True)
+    print(card(), flush=True)
     rows = [adjacency_rows()] + sphere_rows()
     if len(sys.argv) > 1:
         with open(sys.argv[1], "w") as fh:

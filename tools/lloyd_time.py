@@ -10,10 +10,10 @@ The cells each pass handled are printed beside every time.  The reference's time
 part of it as checked out.  `python tools/lloyd_time.py [repeats [cluster repeats]]`; the card's name and power limit are printed first."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import subprocess
 import time
 import numpy as np
 import torch
+from timing import card
 import pcu_b200 as pcu
 
 flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
@@ -34,8 +34,7 @@ def timed(fn, reps):
     return np.median(ts) * 1e3, min(ts) * 1e3
 
 
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip())
+print(card())
 rng = np.random.default_rng(0)
 
 

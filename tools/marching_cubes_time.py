@@ -13,10 +13,10 @@ cube_indices plus the outputs; "at 3.35 TB/s" is the time those bytes alone woul
 bandwidth.  `python tools/marching_cubes_time.py`; the card's name and power limit are printed first."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import subprocess
 import time
 import numpy as np
 import torch
+from timing import card
 import pcu_b200 as pcu
 
 flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
@@ -93,8 +93,7 @@ def phases(fn):
     return {k: v / 1e3 for k, v in out.items()}
 
 
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip(), flush=True)
+print(card(), flush=True)
 runs = [("sphere 256^3 int32/fp32", lambda: sphere(256, torch.float32, torch.int32)),
         ("sphere 256^3 int64/fp64", lambda: sphere(256, torch.float64, torch.int64)),
         ("torus band 1024^3 int32/fp32", lambda: torus_band(1024))]

@@ -12,45 +12,15 @@ CG iterations of every step.  "bytes": the inputs read plus the outputs written,
 the H100's HBM3 data-sheet bandwidth.  scipy's host solve (spsolve of the same system, one step) is printed for
 context.  `python tools/mesh_geometry_time.py`; the card's name and power limit are printed first."""
 import sys, os
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import subprocess
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import time
 import numpy as np
 import torch
+from meshes import noisy_icosphere
+from timing import card, timeit
 import pcu_b200 as pcu
 from pcu_b200 import _mesh_geometry
-
-flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
-
-
-def icosphere(sub):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(sub):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        uk, inv = np.unique(np.minimum(e[:, 0], e[:, 1]) * (1 << 32) + np.maximum(e[:, 0], e[:, 1]), return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uk >> 32] + v[uk & 0xFFFFFFFF])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
-
-
-def timeit(fn, warm=2, it=7):
-    for _ in range(warm): fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(it):
-        flush_buf.add_(1)
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(); fn(); b.record(); torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts)), float(np.min(ts))
 
 
 NORMAL_PHASES = [("face", ("mg_face",)), ("incidence", ("mg_corner", "sort_", "mg_rows")), ("vertex", ("mg_vertex_normal",))]
@@ -80,19 +50,9 @@ def phases(fn, table):
     return "  ".join("%s %.3f" % (k, v) for k, v in tot.items()) + ("  other %.3f" % other if other else "")
 
 
-def card():
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
-                             text=True).stdout.strip()
-    except OSError:
-        out = torch.cuda.get_device_name()
-    print("card:", out)
-
-
 def main():
-    card()
-    v64, f = icosphere(8)
-    v64 = v64 * (1.0 + 0.01 * np.random.default_rng(0).standard_normal((len(v64), 1)))
+    print("card:", card())
+    v64, f = noisy_icosphere(8, 0, 0.01)
     nv, m = len(v64), len(f)
     print("icosphere: %d vertices, %d faces" % (nv, m))
     ft = torch.from_numpy(f).cuda()
@@ -105,7 +65,7 @@ def main():
         for w in ("uniform", "area", "angle"):
             rows.append(("vertex normals %s" % w, lambda w=w: pcu.estimate_mesh_vertex_normals(vt, ft, w), inp + 3 * nv * es, NORMAL_PHASES))
         for name, fn, nbytes, table in rows:
-            med, mn = timeit(fn)
+            med, mn = timeit(fn, warm=2, it=7)
             print("%-8s %-24s median %8.3f ms  min %8.3f ms  bytes %6.1f MB (%.3f ms at 3.35 TB/s)  phases: %s"
                   % (str(dt).replace("torch.", ""), name, med, mn, nbytes / 1e6, nbytes / 3.35e9, phases(fn, table)))
         csr = 6 * m * (4 + 8) + (nv + 1) * 4 + nv * 8   # upper bound: 6 entries per face before the runs are merged
@@ -120,7 +80,6 @@ def main():
     try:
         import scipy.sparse as sp
         import scipy.sparse.linalg as spl
-        sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
         from test_laplacian_smooth_mesh import cot_laplacian
         t0 = time.perf_counter()
         off, diag = cot_laplacian(v64, f)

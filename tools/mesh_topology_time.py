@@ -16,34 +16,16 @@ the outputs written; "at 3.35 TB/s" is the time those bytes alone would take at 
 scipy.sparse.csgraph.connected_components on the host is printed for context.  `python tools/mesh_topology_time.py`;
 the card's name and power limit are printed first."""
 import sys, os
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import subprocess
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import time
 import numpy as np
 import scipy.sparse
 import scipy.sparse.csgraph
 import torch
+from meshes import icosphere
+from timing import card, timeit
 import pcu_b200 as pcu
-
-flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
-
-
-def icosphere(sub):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(sub):
-        e = np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]])
-        uk, inv = np.unique(np.minimum(e[:, 0], e[:, 1]) * (1 << 32) + np.maximum(e[:, 0], e[:, 1]), return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uk >> 32] + v[uk & 0xFFFFFFFF])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
 
 
 def noisy_mc(k=160, seed=5):
@@ -56,18 +38,6 @@ def noisy_mc(k=160, seed=5):
     idx = torch.arange(k ** 3).reshape(k, k, k)[:-1, :-1, :-1].ravel()
     off = torch.tensor([0, 1, 1 + k, k, k * k, 1 + k * k, 1 + k + k * k, k + k * k])
     return pcu.marching_cubes_sparse_voxel_grid((g.ravel() - 0.4).cuda(), gc.cuda(), (idx[:, None] + off).cuda(), 0.0)
-
-
-def timeit(fn, warm=3, it=10):
-    for _ in range(warm): fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(it):
-        flush_buf.add_(1)
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        a.record(); fn(); b.record(); torch.cuda.synchronize()
-        ts.append(a.elapsed_time(b))
-    return float(np.median(ts)), float(np.min(ts))
 
 
 CC_PHASES = [("validate", ("cc_validate",)), ("hook", ("cc_init", "cc_hook")), ("flatten", ("cc_flatten",)),
@@ -100,8 +70,7 @@ def scipy_ms(f):
     return 1e3 * (time.perf_counter() - t0), k
 
 
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip(), flush=True)
+print(card(), flush=True)
 v, f = icosphere(8)
 perm = np.random.default_rng(2).permutation(len(v))
 inv = np.empty_like(perm)

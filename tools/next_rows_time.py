@@ -4,6 +4,7 @@ import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
 import torch
+from timing import timeit
 import pcu_b200 as pcu
 
 n = int(sys.argv[1]) if len(sys.argv) > 1 else 1000000
@@ -11,13 +12,7 @@ g = torch.Generator(device="cuda").manual_seed(0)
 
 
 def timed(label, fn, reps=5):
-    fn(); torch.cuda.synchronize()
-    a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    best = 1e30
-    for _ in range(reps):
-        a.record(); fn(); b.record(); torch.cuda.synchronize()
-        best = min(best, a.elapsed_time(b))
-    print("%-58s %9.3f ms" % (label, best), flush=True)
+    print("%-58s %9.3f ms" % (label, timeit(fn, warm=1, it=reps, flush=False)[1]), flush=True)
 
 
 x = torch.rand((n, 3), generator=g, device="cuda")

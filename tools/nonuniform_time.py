@@ -2,15 +2,8 @@
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch
+from timing import timeit
 import pcu_b200 as pcu
-
-def timeit(fn, warm=3, it=10):
-    for _ in range(warm): fn()
-    torch.cuda.synchronize(); ts = []
-    for _ in range(it):
-        a = torch.cuda.Event(enable_timing=True); b = torch.cuda.Event(enable_timing=True)
-        a.record(); fn(); b.record(); torch.cuda.synchronize(); ts.append(a.elapsed_time(b))
-    return float(np.median(ts))
 
 n = 1000000
 g = torch.Generator(device="cuda").manual_seed(0)
@@ -25,5 +18,5 @@ for name, mk in (("uniform", lambda: torch.rand((n, 3), generator=g, device="cud
         a = torch.cuda.Event(enable_timing=True); b = torch.cuda.Event(enable_timing=True)
         a.record(); pcu.chamfer_distance(x, y); b.record(); torch.cuda.synchronize()
         seq.append("%.3f" % a.elapsed_time(b))
-    ms = timeit(lambda: pcu.chamfer_distance(x, y))
+    ms = timeit(lambda: pcu.chamfer_distance(x, y), flush=False)[0]
     print("%-8s calls %s  steady %.3f ms -> %.3e qpts/s  refinement %s" % (name, " ".join(seq), ms, 2 * n / ms * 1e3, pcu._pcu_internal._grid_refinement()), flush=True)

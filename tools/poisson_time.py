@@ -3,28 +3,16 @@ and selection rounds per call, for uniform and sphere-surface fp32 clouds at rad
 the points, a tight cluster, and a target-count call.  `python tools/poisson_time.py [n ...]` (default 10^6 10^7)."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import subprocess
 import torch, numpy as np
+from timing import card, timeit
 import pcu_b200 as pcu
 
 I = pcu._pcu_internal
-flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
 
 
 def one_call(x, radius, rounds, count, idx):
     I._poisson_disk_device(x.dtype == torch.float64, x.data_ptr(), x.shape[0], float(radius), 12345, idx.data_ptr(),
                            count.data_ptr(), rounds.data_ptr(), x.device.index or 0, torch.cuda.current_stream().cuda_stream)
-
-
-def timeit(fn, warm=2, it=7):
-    for _ in range(warm): fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(it):
-        flush_buf.add_(1)
-        a = torch.cuda.Event(enable_timing=True); b = torch.cuda.Event(enable_timing=True)
-        a.record(); fn(); b.record(); torch.cuda.synchronize(); ts.append(a.elapsed_time(b))
-    return float(np.median(ts)), float(np.min(ts))
 
 
 def radius_for(x, keep, idx, count, rounds):
@@ -39,8 +27,7 @@ def radius_for(x, keep, idx, count, rounds):
     return mid
 
 
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip(), flush=True)
+print(card(), flush=True)
 sizes = [int(float(a)) for a in sys.argv[1:]] or [1000000, 10000000]
 g = torch.Generator(device="cuda").manual_seed(0)
 for n in sizes:
@@ -53,7 +40,7 @@ for n in sizes:
     for name, x in clouds.items():
         for keep in (0.01, 0.10):
             r = radius_for(x, keep, idx, count, rounds)
-            med, mn = timeit(lambda: one_call(x, r, rounds, count, idx))
+            med, mn = timeit(lambda: one_call(x, r, rounds, count, idx), warm=2, it=7)
             print("%-7s n=%8d r=%.5f kept %5.2f %%: median %8.3f ms  min %8.3f ms  rounds %d"
                   % (name, n, r, 100.0 * int(count.item()) / n, med, mn, int(rounds.item())), flush=True)
     del clouds, s

@@ -13,46 +13,16 @@ device-resident inputs, warm-up, L2 flushed before every timed call) and device 
 
 `python tools/ray_surfel_time.py [subdivisions]` (default 8).  The card's name and power limit are printed first."""
 import sys, os
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import subprocess
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np
 import torch
+from meshes import icosphere
+from timing import card, timeit
 import pcu_b200 as pcu
 
 I = pcu._pcu_internal
-flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
 SUBDIVS = 7
-
-
-def icosphere(subdivisions, jitter, seed):
-    t = (1.0 + 5.0 ** 0.5) / 2.0
-    v = np.array([[-1, t, 0], [1, t, 0], [-1, -t, 0], [1, -t, 0], [0, -1, t], [0, 1, t], [0, -1, -t], [0, 1, -t],
-                  [t, 0, -1], [t, 0, 1], [-t, 0, -1], [-t, 0, 1]], dtype=np.float64)
-    f = np.array([[0, 11, 5], [0, 5, 1], [0, 1, 7], [0, 7, 10], [0, 10, 11], [1, 5, 9], [5, 11, 4], [11, 10, 2],
-                  [10, 7, 6], [7, 1, 8], [3, 9, 4], [3, 4, 2], [3, 2, 6], [3, 6, 8], [3, 8, 9], [4, 9, 5], [2, 4, 11],
-                  [6, 2, 10], [8, 6, 7], [9, 8, 1]], dtype=np.int64)
-    for _ in range(subdivisions):
-        edges = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), axis=1)
-        uniq, inv = np.unique(edges, axis=0, return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, 0.5 * (v[uniq[:, 0]] + v[uniq[:, 1]])])
-        a, b, c = f[:, 0], f[:, 1], f[:, 2]
-        f = np.concatenate([np.stack([a, mid[:, 0], mid[:, 2]], 1), np.stack([b, mid[:, 1], mid[:, 0]], 1),
-                            np.stack([c, mid[:, 2], mid[:, 1]], 1), mid])
-    v = v / np.linalg.norm(v, axis=1, keepdims=True)
-    v = v + jitter * np.random.default_rng(seed).standard_normal(v.shape) * 2.0 ** -subdivisions
-    return v, f.astype(np.int32)
-
-
-def timeit(fn, warm=3, it=10):
-    for _ in range(warm): fn()
-    torch.cuda.synchronize()
-    ts = []
-    for _ in range(it):
-        flush_buf.add_(1)
-        a = torch.cuda.Event(enable_timing=True); b = torch.cuda.Event(enable_timing=True)
-        a.record(); fn(); b.record(); torch.cuda.synchronize(); ts.append(a.elapsed_time(b))
-    return float(np.median(ts)), float(np.min(ts))
 
 
 def held(make):
@@ -64,10 +34,10 @@ def held(make):
     return obj, before - torch.cuda.mem_get_info()[0]
 
 
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip(), flush=True)
+print(card(), flush=True)
 sub = int(sys.argv[1]) if len(sys.argv) > 1 else 8
-v64, f = icosphere(sub, 0.2, 1)
+v64, f = icosphere(sub, 0.2 * 2.0 ** -sub, 1)
+f = f.astype(np.int32)
 m = 10 ** 6
 fid, bc = pcu.sample_mesh_random(v64, f, m, 7)
 p64 = pcu.interpolate_barycentric_coords(f, fid, bc, v64)

@@ -16,10 +16,10 @@ come from a torch.profiler pass of their own, summed kernel times by kernel-name
 tools/sparse_voxel_time.py`; the card's name and power limit are printed first."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import subprocess
 import time
 import numpy as np
 import torch
+from timing import card
 import pcu_b200 as pcu
 
 flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
@@ -71,8 +71,7 @@ def sphere(n, seed):
     return d / d.norm(dim=1, keepdim=True)
 
 
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip(), flush=True)
+print(card(), flush=True)
 
 s = 1.0 / 512
 pts = sphere(10 ** 7, 0).float()

@@ -11,7 +11,6 @@ Prints, after the card's name and power limit:
 temporary directory, so that nothing is written into the repository)."""
 import json
 import os
-import subprocess
 import sys
 import tempfile
 
@@ -19,13 +18,13 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 import numpy as np
 import torch
+from timing import card
 import pcu_b200 as pcu
 
 out_dir = sys.argv[1] if len(sys.argv) > 1 else tempfile.mkdtemp(prefix="pcu_tail_")
 steps = int(sys.argv[2]) if len(sys.argv) > 2 else 200
 os.makedirs(out_dir, exist_ok=True)
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip(), flush=True)
+print(card(), flush=True)
 
 rng = np.random.default_rng(1000)   # bench.py's C3 clouds (rank 0)
 x = torch.from_numpy(rng.random((1000000, 3), dtype=np.float32)).cuda()

@@ -19,10 +19,10 @@ card's name and power limit are printed first."""
 import sys, os
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import math
-import subprocess
 import time
 import numpy as np
 import torch
+from timing import card
 import pcu_b200 as pcu
 
 flush_buf = torch.empty(64 << 20, dtype=torch.int32, device="cuda")   # 256 MB, several times the 50 MB L2
@@ -119,8 +119,7 @@ def accepted_pairs(v, f, size):
     return n, acc
 
 
-print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm,clocks.sm", "--format=csv,noheader"],
-                     capture_output=True, text=True).stdout.strip(), flush=True)
+print(card(), flush=True)
 v64, f = sphere_mesh(708, 708)
 cube_v, cube_f = tilted_cube(512)
 vx_runs = [("sphere 1.0e6 faces 256^3 fp32", v64.float(), f, 2.0 / 256), ("sphere 1.0e6 faces 256^3 fp64", v64, f, 2.0 / 256),

@@ -10,13 +10,15 @@ the profile.  `python tools/watertight_time.py [out.json]`; the card's name and 
 import json
 import os
 import statistics
-import subprocess
 import sys
 import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path[:0] = [ROOT, os.path.join(ROOT, "tests")]
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
+from meshes import icosphere  # noqa: E402
+from timing import card  # noqa: E402
 import pcu_b200 as pcu  # noqa: E402
 
 PHASES = [("depth search", ("wt_bounds", "vx_bounds", "vx_tiles", "vx_test_kernel<double, 0>")),
@@ -27,24 +29,6 @@ PHASES = [("depth search", ("wt_bounds", "vx_bounds", "vx_tiles", "vx_test_kerne
           ("tree", ("mq_", "radix", "sort", "digit", "scan"))]
 
 
-def icosphere(level):
-    t = (1 + 5 ** 0.5) / 2
-    v = np.array([(-1, t, 0), (1, t, 0), (-1, -t, 0), (1, -t, 0), (0, -1, t), (0, 1, t), (0, -1, -t), (0, 1, -t),
-                  (t, 0, -1), (t, 0, 1), (-t, 0, -1), (-t, 0, 1)], np.float64)
-    f = np.array([(0, 11, 5), (0, 5, 1), (0, 1, 7), (0, 7, 10), (0, 10, 11), (1, 5, 9), (5, 11, 4), (11, 10, 2),
-                  (10, 7, 6), (7, 1, 8), (3, 9, 4), (3, 4, 2), (3, 2, 6), (3, 6, 8), (3, 8, 9), (4, 9, 5), (2, 4, 11),
-                  (6, 2, 10), (8, 6, 7), (9, 8, 1)], np.int64)
-    for _ in range(level):
-        e = np.sort(np.concatenate([f[:, [0, 1]], f[:, [1, 2]], f[:, [2, 0]]]), 1)
-        uniq, inv = np.unique(e[:, 0] * len(v) + e[:, 1], return_inverse=True)
-        mid = len(v) + inv.reshape(3, -1).T
-        v = np.concatenate([v, (v[uniq // len(v)] + v[uniq % len(v)]) / 2])
-        a, b, c = mid[:, 0], mid[:, 1], mid[:, 2]
-        f = np.concatenate([np.stack([f[:, 0], a, c], 1), np.stack([f[:, 1], b, a], 1), np.stack([f[:, 2], c, b], 1),
-                            np.stack([a, b, c], 1)])
-    return v / np.linalg.norm(v, axis=1, keepdims=True), f
-
-
 def phase_of(name):
     for phase, keys in PHASES:
         if any(k in name for k in keys):
@@ -53,8 +37,7 @@ def phase_of(name):
 
 
 def main():
-    print(subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip())
+    print(card())
     v, f = icosphere(8)
     vt, ft = torch.from_numpy(v).cuda(), torch.from_numpy(f).cuda()
     rows = []
