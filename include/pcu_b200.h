@@ -772,14 +772,17 @@ int pcu_b200_adjacency_list_prepare(pcu_b200_workspace* ws, const void* f, int64
 int pcu_b200_adjacency_list_emit(pcu_b200_workspace* ws, const pcu_b200_adjacency* adj, void* out_offsets, void* out_neighbors, void* stream);
 int pcu_b200_adjacency_list_destroy(pcu_b200_adjacency* adj);
 
-/* ---- mesh normals, face areas and Laplacian smoothing ------------------------------------------------------------
- * Replace mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals and laplacian_smooth_mesh (the
- * reference's src/face_areas.cpp, src/mesh_normals.cpp, src/smooth.cpp).  Results defined in DESIGN.md §3.  v (nv, 3)
- * in the suffix's type, f (nf, 3) of kind f_kind (pcu_b200_index_kind); 1 <= nv <= 2^31 - 2, 1 <= nf <= 357913941.
+/* ---- mesh normals, face areas, curvatures and Laplacian smoothing ------------------------------------------------
+ * Replace mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals, mesh_principal_curvatures and
+ * laplacian_smooth_mesh (the reference's src/face_areas.cpp, src/mesh_normals.cpp, src/curvature.cpp, src/smooth.cpp).
+ * Results defined in DESIGN.md §3.  v (nv, 3) in the suffix's type, f (nf, 3) of kind f_kind (pcu_b200_index_kind); 1 <= nv <= 2^31 - 2, 1 <= nf <= 357913941.
  * A face with a corner outside [0, nv) fails with PCU_B200_INVALID_ARGUMENT (the outputs are written nonetheless).
  *   mesh_face_areas: out_areas (nf), the reference's formula in v's precision.  Synchronises `stream` once.
  *   mesh_face_normals: out_n (nf, 3), unit normals from fp64, 0 for a face of zero area.  Synchronises once.
  *   mesh_vertex_normals: out_n (nv, 3); weighting 0 uniform, 1 area, 2 angle.  Synchronises once.
+ *   mesh_principal_curvatures: out_k1, out_k2 (nv) and out_d1, out_d2 (nv, 3), k1 >= k2, NaN curvatures and zero
+ *     directions where undetermined.  r <= 0: the one-ring tensor estimate; r > 0: a quadric fit over the ball of
+ *     radius r around each vertex.  A non-finite r fails with PCU_B200_INVALID_ARGUMENT.  Synchronises once.
  *   laplacian_smooth_mesh: out_v (nv, 3); num_iters >= 0 (0 copies v and does not synchronise).  out_cg_iters and
  *     out_residual (host, num_iters entries) receive every step's conjugate-gradient iterations and its largest
  *     |r| / |b| at exit (<= 1e-12 when it converged; a step stops after max_cg_iters iterations).  Synchronises once
@@ -798,6 +801,10 @@ int pcu_b200_mesh_vertex_normals_f32(pcu_b200_workspace* ws, const float* v, int
                                      float* out_n, void* stream);
 int pcu_b200_mesh_vertex_normals_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, int weighting,
                                      double* out_n, void* stream);
+int pcu_b200_mesh_principal_curvatures_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, double r,
+                                           float* out_k1, float* out_k2, float* out_d1, float* out_d2, void* stream);
+int pcu_b200_mesh_principal_curvatures_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, double r,
+                                           double* out_k1, double* out_k2, double* out_d1, double* out_d2, void* stream);
 int pcu_b200_laplacian_smooth_mesh_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, int num_iters,
                                        double step_size, int use_cotan_weights, int max_cg_iters, float* out_v, int32_t* out_cg_iters,
                                        double* out_residual, void* stream);

@@ -51,6 +51,7 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "connected_components", "remove_mesh_vertices", "remove_unreferenced_mesh_vertices", "orient_mesh_faces",
            "adjacency_list",
            "mesh_face_areas", "estimate_mesh_face_normals", "estimate_mesh_vertex_normals", "laplacian_smooth_mesh",
+           "mesh_principal_curvatures", "mesh_mean_and_gaussian_curvatures",
            "deduplicate_point_cloud", "voronoi_centroids_unit_cube", "lloyd_3d", "lloyd_2d",
            "sample_mesh_lloyd",
            "deduplicate_mesh_vertices", "prepare_cloud", "pinned_empty", "PreparedCloud", "device_count",
@@ -635,6 +636,7 @@ from ._decimate import decimate_triangle_mesh  # noqa: E402
 from ._mesh_topology import (connected_components, remove_mesh_vertices, remove_unreferenced_mesh_vertices,  # noqa: E402
                              orient_mesh_faces, adjacency_list)
 from ._mesh_geometry import mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals, laplacian_smooth_mesh  # noqa: E402
+from ._mesh_geometry import mesh_principal_curvatures, mesh_mean_and_gaussian_curvatures  # noqa: E402
 
 
 def _voxel_internal(points, attrib, voxel_size, min_bound, max_bound, min_points_per_voxel, device, return_counts=False):

@@ -1,11 +1,13 @@
-"""mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals and laplacian_smooth_mesh -- the
-reference's names, arguments and outputs (the reference's src/face_areas.cpp, src/mesh_normals.cpp and src/smooth.cpp),
-computed by csrc/mesh_geometry.cuh and csrc/laplacian.cuh.
+"""mesh_face_areas, estimate_mesh_face_normals, estimate_mesh_vertex_normals, mesh_principal_curvatures,
+mesh_mean_and_gaussian_curvatures and laplacian_smooth_mesh -- the reference's names, arguments and outputs (the
+reference's src/face_areas.cpp, src/mesh_normals.cpp, src/curvature.cpp and src/smooth.cpp), computed by
+csrc/mesh_geometry.cuh, csrc/curvature.cuh and csrc/laplacian.cuh.
 
 numpy arrays in -> numpy out (each input is uploaded once through torch); CUDA torch tensors in -> CUDA tensors out;
 CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages and in its order, before any
 device call.  Shapes are the reference's through npe::move, which squeezes them as numpy does: a single face gives a
 0-d area and a (3,) normal, a single vertex a (3,) result."""
+import math
 import warnings
 
 from . import _pcu_internal
@@ -121,6 +123,73 @@ def estimate_mesh_vertex_normals(v, f, weighting_type="uniform", *, device=None)
         return out
 
     return _run(form, [v, f], device, body, squeeze=True)
+
+
+def mesh_principal_curvatures(v, f, r=-1.0, *, device=None):
+    """
+    Compute the principal curvatures and principal directions at every vertex of a triangle mesh
+
+    Args:
+        v : (#v, 3)-shaped array of mesh vertex 3D positions
+        f : (#f, 3)-shaped array of face (triangle) indices
+        r : the radius of the ball each vertex's quadric is fitted over; r <= 0 (default) uses the one-ring estimate
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        k1 : (#v,)-shaped array of the larger principal curvature at each vertex
+        k2 : (#v,)-shaped array of the smaller principal curvature at each vertex
+        d1 : (#v, 3)-shaped array of the unit principal direction of k1 at each vertex
+        d2 : (#v, 3)-shaped array of the unit principal direction of k2 at each vertex
+
+    Dtypes: v float32 / float64, f int32 / int64 / uint32 / uint64; every output has v's dtype.  Defined in DESIGN.md
+    §3, computed in fp64 and rounded once.  On a sphere of radius R whose faces wind counter-clockwise seen from
+    outside, k1 = k2 = 1 / R; reversed faces flip the sign.  k1 >= k2.  d1's component of largest magnitude is positive
+    and d2 = n x d1.  A vertex whose curvature is undetermined (no face of nonzero area, fewer than 5 neighbours in the
+    ball, ...) gets k1 = k2 = NaN and zero directions.
+      r <= 0: Rusinkiewicz's (2004) one-ring tensor estimate, with Max's vertex normals and mixed Voronoi areas.
+      r > 0: a quadric z = a x^2 + b x y + c y^2 + d x + e y fitted, in the frame of the vertex normal, to every other
+             vertex j with |v_j - v_i|^2 < r^2; more robust on noisy meshes.  A ball that reaches another sheet of the
+             surface (thin parts) mixes both sheets.
+    The reference declares this function but ships no implementation.
+    Divergences: a non-finite r and a face corner outside [0, #v) raise ValueError.
+    """
+    form = _form([v, f], ["v", "f"])
+    _validate_mesh(v, f, _INDEX_KINDS)
+    r = float(r)
+    if not math.isfinite(r):
+        raise ValueError("mesh_principal_curvatures: r must be finite, got %r" % (r,))
+    nvert, nface = _check_size("mesh_principal_curvatures", v, f)
+    torch = _torch()
+
+    def body(vt, ft, dev, stream):
+        k1, k2 = (torch.empty((nvert,), dtype=vt.dtype, device=vt.device) for _ in range(2))
+        d1, d2 = (torch.empty((nvert, 3), dtype=vt.dtype, device=vt.device) for _ in range(2))
+        _pcu_internal._mesh_curvatures_device(vt.dtype == torch.float64, vt.data_ptr(), nvert, ft.data_ptr(), nface,
+                                              _INDEX_KINDS[_dtype_name(f)], r, k1.data_ptr(), k2.data_ptr(), d1.data_ptr(),
+                                              d2.data_ptr(), dev, stream)
+        return k1, k2, d1, d2
+
+    return _run(form, [v, f], device, body, squeeze=True)
+
+
+def mesh_mean_and_gaussian_curvatures(v, f, r=-1.0, *, device=None):
+    """
+    Compute the mean and Gaussian curvatures at every vertex of a triangle mesh
+
+    Args:
+        v : (#v, 3)-shaped array of mesh vertex 3D positions
+        f : (#f, 3)-shaped array of face (triangle) indices
+        r : see `mesh_principal_curvatures`
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        kh : (#v,)-shaped array of mean curvatures, 0.5 * (k1 + k2)
+        kg : (#v,)-shaped array of Gaussian curvatures, k1 * k2
+
+    Computed from `mesh_principal_curvatures`' k1 and k2 in their dtype and form; NaN where they are.
+    """
+    k1, k2, _, _ = mesh_principal_curvatures(v, f, r, device=device)
+    return 0.5 * (k1 + k2), k1 * k2
 
 
 def _smooth(v, f, num_iters, step_size, use_cotan_weights, device):

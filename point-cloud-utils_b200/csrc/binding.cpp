@@ -975,6 +975,8 @@ PYBIND11_MODULE(_pcu_internal, mod) {
     mod.def("_adjacency_list_destroy", destroy(pcu_b200_adjacency_list_destroy));
     mod.def("_mesh_face_device", &mesh_face_device);
     mod.def("_mesh_vertex_normals_device", forward_to(pcu_b200_mesh_vertex_normals_f32, pcu_b200_mesh_vertex_normals_f64).pair());
+    mod.def("_mesh_curvatures_device",
+            forward_to(pcu_b200_mesh_principal_curvatures_f32, pcu_b200_mesh_principal_curvatures_f64).pair());
     mod.def("_laplacian_smooth_device", &laplacian_smooth_device);
     mod.def("_cloud_prepare_host", &cloud_prepare_numpy);
     mod.def("_cloud_prepare_device", &cloud_prepare_device, py::arg("is_f64"), py::arg("points"), py::arg("n"), py::arg("device"),

@@ -106,6 +106,12 @@ __device__ __forceinline__ double corner_dot(const double a[3], const double b[3
     return s;
 }
 
+// Max's (1999) corner weight |e1 x e2| / (|e1|^2 |e2|^2), e1 = b - a, e2 = c - a; 0 where |e1 x e2| = 0.
+__device__ __forceinline__ double max_weight(const double a[3], const double b[3], const double c[3]) {
+    const double A = face_area(a, b, c);
+    return A == 0.0 ? 0.0 : __ddiv_rn(A, __dmul_rn(corner_dot(a, b, b), corner_dot(a, c, c)));
+}
+
 // The reference's face area (src/face_areas.cpp), operation for operation in T: edge lengths a = |v1 - v0|,
 // b = |v2 - v1|, c = |v0 - v2| as sqrt((x x + y y) + z z), p = (a + b + c) 0.5, sqrt(((p max(p - a, 0)) max(p - b, 0))
 // max(p - c, 0)), with max(x, 0) = x < 0 ? 0 : x as std::max returns it.
@@ -135,7 +141,8 @@ struct FaceOut {
     T* area;            // (m) the reference's face area, in T
     T* normal;          // (m, 3) unit normal, fp64 rounded once to T
     double* unit;       // (m, 3) unit normal in fp64
-    double* weight;     // (m, 3) corner weights of the vertex normals: |e1 x e2| (weighting 1) or the angle (weighting 2)
+    double* weight;     // (m, 3) corner weights of the vertex normals: |e1 x e2| (weighting 1), the angle (weighting 2) or
+                        // |e1 x e2| / (|e1|^2 |e2|^2), 0 where |e1 x e2| = 0 (weighting 3: Max's weights, curvature.cuh)
     int weighting;
     double* dbla;       // (m) face_area
     double* halfcot;    // (m, 3) cot / 2 of every corner's angle, 0 where dblA = 0
@@ -179,7 +186,9 @@ __global__ void __launch_bounds__(kThreads) mg_face_kernel(const T* __restrict__
                 const double* a = p[k];
                 const double* b = p[(k + 1) % 3];
                 const double* e = p[(k + 2) % 3];
-                out.weight[3 * t + k] = out.weighting == 1 ? face_area(p[0], p[1], p[2]) : atan2(face_area(a, b, e), corner_dot(a, b, e));
+                out.weight[3 * t + k] = out.weighting == 1   ? face_area(p[0], p[1], p[2])
+                                        : out.weighting == 2 ? atan2(face_area(a, b, e), corner_dot(a, b, e))
+                                                             : max_weight(a, b, e);
             }
         if (out.dbla || out.halfcot || out.partial) {
             const double A = bad ? 0.0 : face_area(p[0], p[1], p[2]);

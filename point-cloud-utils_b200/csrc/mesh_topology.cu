@@ -1,10 +1,11 @@
 // mesh_topology.cu -- connected components and vertex removal, adjacency lists, consistent face orientation, face areas
-// and normals, vertex normals and Laplacian smoothing (mesh_topology.cuh, orient.cuh, mesh_geometry.cuh, laplacian.cuh):
-// launch sequencing and C entry points.
+// and normals, vertex normals, principal curvatures and Laplacian smoothing (mesh_topology.cuh, orient.cuh,
+// mesh_geometry.cuh, curvature.cuh, laplacian.cuh): launch sequencing and C entry points.
 #include "runtime.cuh"
 #include "mesh_topology.cuh"
 #include "orient.cuh"
 #include "laplacian.cuh"
+#include "curvature.cuh"
 
 using namespace pcu;
 using namespace pcu_internal;
@@ -337,6 +338,61 @@ int vertex_normals_device(pcu_b200_workspace* ws, const T* v, long long nv, cons
     return host.bad ? bad_corners(host.bad) : PCU_B200_OK;
 }
 
+// mesh_principal_curvatures (curvature.cuh): face pass (unit normals, Max's weights and, for the one-ring mode, dblA
+// and half-cotangents), corner CSR, fp64 vertex normals; then the one-ring kernels (r <= 0) or the ball pass of
+// nearest.cu (r > 0).  The normals and the record live in kMesh, which the ball pass's binning does not re-carve.  One
+// synchronisation.
+template <typename T>
+int mesh_curvatures_device(pcu_b200_workspace* ws, const T* v, long long nv, const void* f, long long m, int fkind, double r, T* out_k1,
+                           T* out_k2, T* out_d1, T* out_d2, cudaStream_t stream) {
+    PCU_TRY(mg_check(ws, v, nv, f, m, fkind, out_k1));
+    if (!out_k2 || !out_d1 || !out_d2) return fail(PCU_B200_INVALID_ARGUMENT, "null argument");
+    if (!std::isfinite(r)) return fail(PCU_B200_INVALID_ARGUMENT, "mesh_principal_curvatures: r must be finite, got %g", r);
+    PCU_ON_DEVICE(ws);
+    const bool ring = !(r > 0.0);
+    struct { MgRecord* rec; double* normal; } keep;
+    PCU_TRY(carve_scratch(ws, kMesh, stream, [&](Carver& cv) {
+        keep.rec = cv.take<MgRecord>(1);
+        keep.normal = cv.take<double>(3 * (size_t)nv);
+    }));
+    struct { double *unit, *weight, *dbla, *halfcot, *frame_u, *efg; SortScratch<MgRec> sort; int *first, *corner; } sc;
+    PCU_TRY(carve_scratch(ws, kArena, stream, [&](Carver& cv) {
+        sc.unit = cv.take<double>(3 * (size_t)m);
+        sc.weight = cv.take<double>(3 * (size_t)m);
+        sc.dbla = ring ? cv.take<double>((size_t)m) : nullptr;
+        sc.halfcot = ring ? cv.take<double>(3 * (size_t)m) : nullptr;
+        sc.frame_u = ring ? cv.take<double>(3 * (size_t)m) : nullptr;
+        sc.efg = ring ? cv.take<double>(3 * (size_t)m) : nullptr;
+        sc.sort.carve(cv, 3 * m);
+        sc.first = cv.take<int>((size_t)nv + 1);
+        sc.corner = cv.take<int>(3 * (size_t)m);
+    }));
+    PCU_CUDA(cudaMemsetAsync(keep.rec, 0, sizeof(MgRecord), stream));
+    FaceOut<T> o = {};
+    o.unit = sc.unit;
+    o.weight = sc.weight;
+    o.weighting = 3;
+    o.dbla = sc.dbla;
+    o.halfcot = sc.halfcot;
+    PCU_TRY(mg_face_pass<T>(v, nv, f, fkind, m, o, keep.rec, stream));
+    PCU_TRY(enqueue_incidence(sc.sort, f, fkind, m, nv, sc.first, sc.corner, stream));
+    PCU_LAUNCH(mg_vertex_normal_kernel<double>, blocks_for(nv), kThreads, stream, (const int*)sc.first, (const int*)sc.corner, nv,
+               (const double*)sc.unit, (const double*)sc.weight, keep.normal);
+    if (ring) {
+        // the corner areas overwrite Max's weights, which the vertex normals no longer need
+        PCU_LAUNCH(curv_face_kernel<T>, blocks_for(m), kThreads, stream, v, nv, f, fkind, m, (const double*)keep.normal,
+                   (const double*)sc.unit, (const double*)sc.dbla, (const double*)sc.halfcot, sc.frame_u, sc.efg, sc.weight);
+        PCU_LAUNCH(curv_vertex_kernel<T>, blocks_for(nv), kThreads, stream, (const int*)sc.first, (const int*)sc.corner, nv,
+                   (const double*)keep.normal, (const double*)sc.unit, (const double*)sc.frame_u, (const double*)sc.efg,
+                   (const double*)sc.weight, out_k1, out_k2, out_d1, out_d2);
+    } else {
+        PCU_TRY(curvature_ball_device<T>(ws, v, nv, keep.normal, r, out_k1, out_k2, out_d1, out_d2, stream));
+    }
+    MgRecord host;
+    PCU_TRY(read_record(keep.rec, &host, stream));
+    return host.bad ? bad_corners(host.bad) : PCU_B200_OK;
+}
+
 constexpr int kCgWindow = 16;   // CG iterations enqueued between two reads of the solver's record
 
 // The buffers of one smoothing call.
@@ -628,6 +684,14 @@ int pcu_b200_mesh_vertex_normals_f32(pcu_b200_workspace* ws, const float* v, int
 int pcu_b200_mesh_vertex_normals_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, int weighting,
                                      double* out_n, void* stream) {
     return vertex_normals_device<double>(ws, v, nv, f, nf, f_kind, weighting, out_n, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_principal_curvatures_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, double r,
+                                           float* out_k1, float* out_k2, float* out_d1, float* out_d2, void* stream) {
+    return mesh_curvatures_device<float>(ws, v, nv, f, nf, f_kind, r, out_k1, out_k2, out_d1, out_d2, (cudaStream_t)stream);
+}
+int pcu_b200_mesh_principal_curvatures_f64(pcu_b200_workspace* ws, const double* v, int64_t nv, const void* f, int64_t nf, int f_kind, double r,
+                                           double* out_k1, double* out_k2, double* out_d1, double* out_d2, void* stream) {
+    return mesh_curvatures_device<double>(ws, v, nv, f, nf, f_kind, r, out_k1, out_k2, out_d1, out_d2, (cudaStream_t)stream);
 }
 int pcu_b200_laplacian_smooth_mesh_f32(pcu_b200_workspace* ws, const float* v, int64_t nv, const void* f, int64_t nf, int f_kind, int num_iters,
                                        double step_size, int use_cotan_weights, int max_cg_iters, float* out_v, int32_t* out_cg_iters,

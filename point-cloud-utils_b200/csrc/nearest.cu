@@ -1146,6 +1146,25 @@ int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, do
     return PCU_B200_OK;
 }
 
+// ---- principal curvatures from a quadric fit over a ball (mesh_principal_curvatures, r > 0) --------------------------
+// The vertices are binned once (cells no finer than r / 2) and put in row order within every cell, then one thread per
+// vertex walks its ball (curv_ball_kernel).
+template <typename T>
+int curvature_ball_device(pcu_b200_workspace* ws, const T* v, long long nv, const double* normal, double r, T* out_k1, T* out_k2,
+                          T* out_d1, T* out_d2, cudaStream_t stream) {
+    PCU_TRY(check_cloud_args<T>(v, nv, v, 1));
+    Plan<T> plan;
+    PCU_TRY(single_cloud_plan<T>(ws, v, nv, 0.5 * r, plan, stream));
+    PCU_TRY(enqueue_binning(ws, plan, stream, nullptr, true));
+    PCU_LAUNCH((cell_order_kernel<T>), (unsigned)std::min<long long>(((long long)plan.cv.v[0].cell_cap + kThreads - 1) / kThreads, (long long)ws->sm_count * 64), kThreads, stream, plan.cv.v[0]);
+    PCU_LAUNCH((curv_ball_kernel<T>), blocks_for(nv), kThreads, stream, plan.cv.v[0], normal, r, out_k1, out_k2, out_d1, out_d2);
+    return PCU_B200_OK;
+}
+
+template int curvature_ball_device<float>(pcu_b200_workspace*, const float*, long long, const double*, double, float*, float*, float*,
+                                          float*, cudaStream_t);
+template int curvature_ball_device<double>(pcu_b200_workspace*, const double*, long long, const double*, double, double*, double*,
+                                           double*, double*, cudaStream_t);
 template int knn_device<float>(pcu_b200_workspace*, const float*, long long, const float*, long long, int, int, float*, long long*,
                                long long*, cudaStream_t, pcu_b200_cloud*, bool);
 template int knn_device<double>(pcu_b200_workspace*, const double*, long long, const double*, long long, int, int, double*, long long*,

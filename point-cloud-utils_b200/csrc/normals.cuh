@@ -13,10 +13,14 @@
 // rotations and refined on the offsets rotated into its eigenbasis, to the SVD's accuracy u s1 / (s2 - s3) --
 // the same vector up to rounding (and up to sign: without view directions the reference's sign is whatever its SVD
 // happens to return).  Fewer than 3 neighbours give the zero vector, all-zero offsets give (0, 0, 1).
+//
+// The ball walk below also serves the ball mode of mesh_principal_curvatures (curv_ball_kernel, with the rules of
+// curvature.cuh).
 #pragma once
 #include "common.cuh"
 #include "compact.cuh"
 #include "plane_fit.h"
+#include "curvature.cuh"
 
 namespace pcu {
 
@@ -249,6 +253,87 @@ __global__ void __launch_bounds__(kThreads) normals_ball_kernel(Cloud<T> cl, con
     }
     normals[3 * row] = (T)nrm[0]; normals[3 * row + 1] = (T)nrm[1]; normals[3 * row + 2] = (T)nrm[2];
     keep[row] = ok ? 1 : 0;
+}
+
+// ---- principal curvatures from a quadric fit over a ball (mesh_principal_curvatures with r > 0, curvature.cuh) -----
+// One thread per vertex, in CELL order, over the binned vertices.  The ball is { j != i : d2(p_i, p_j) < (T)(r r) }.
+// With n = the vertex's fp64 normal and (t1, t2) its frame, each neighbour's offset o = p_j - p_i (fp64) gives
+// (x, y, z) = (o . t1, o . t2, o . n) / r, and z = a x^2 + b x y + c y^2 + d x + e y is fitted by least squares: the
+// 5 x 5 normal equations, folded in cell order, solved by Cholesky.  Undetermined: fewer than 5 neighbours, a zero
+// normal, or a pivot <= 1e-12 times the largest diagonal entry of the system.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) curv_ball_kernel(Cloud<T> cl, const double* __restrict__ normal, double r, T* __restrict__ out_k1,
+                                                             T* __restrict__ out_k2, T* __restrict__ out_d1, T* __restrict__ out_d2) {
+    grid_dependency_wait();
+    __shared__ GridHeader<T> g;
+    if (threadIdx.x == 0) g = *cl.grid;
+    __syncthreads();
+    const long long pos = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (pos >= cl.n) return;
+    const Pt<T> q = load_pt<T>(cl.sorted + pos);
+    const long long row = (long long)q.i;
+    double n[3], t1[3], t2[3];
+#pragma unroll
+    for (int a = 0; a < 3; ++a) n[a] = normal[3 * row + a];
+    const bool has_normal = n[0] != 0.0 || n[1] != 0.0 || n[2] != 0.0;
+    curv_frame(n, t1, t2);
+    double M[15], y[5];   // M: the lower triangle by rows, M[i (i + 1) / 2 + j] for j <= i
+#pragma unroll
+    for (int k = 0; k < 15; ++k) M[k] = 0.0;
+#pragma unroll
+    for (int k = 0; k < 5; ++k) y[k] = 0.0;
+    long long found = 0;
+    if (has_normal)
+        walk_ball<T>(cl, g, q, (T)(r * r), [&](const Pt<T>& p, T) {
+            if (p.i == q.i) return;
+            ++found;
+            const double o[3] = {(double)p.x - (double)q.x, (double)p.y - (double)q.y, (double)p.z - (double)q.z};
+            const double x = curv_dot(o, t1) / r, yy = curv_dot(o, t2) / r, z = curv_dot(o, n) / r;
+            const double phi[5] = {x * x, x * yy, yy * yy, x, yy};
+#pragma unroll
+            for (int i = 0; i < 5; ++i) {
+#pragma unroll
+                for (int j = 0; j <= i; ++j) M[i * (i + 1) / 2 + j] += phi[i] * phi[j];
+                y[i] += phi[i] * z;
+            }
+        });
+    bool ok = has_normal && found >= 5;
+    double big = 0.0;
+#pragma unroll
+    for (int i = 0; i < 5; ++i) big = fmax(big, M[i * (i + 1) / 2 + i]);
+    // M = L L^T in place: pivot_k = M_kk - sum_{j<k} L_kj^2 must exceed 1e-12 big; L_ik = (M_ik - sum_{j<k} L_ij L_kj) / L_kk
+#pragma unroll
+    for (int k = 0; k < 5; ++k) {
+        double piv = M[k * (k + 1) / 2 + k];
+#pragma unroll
+        for (int j = 0; j < k; ++j) piv -= M[k * (k + 1) / 2 + j] * M[k * (k + 1) / 2 + j];
+        ok = ok && piv > 1e-12 * big;
+        const double lkk = sqrt(fmax(piv, 0.0));
+        M[k * (k + 1) / 2 + k] = lkk;
+#pragma unroll
+        for (int i = k + 1; i < 5; ++i) {
+            double s = M[i * (i + 1) / 2 + k];
+#pragma unroll
+            for (int j = 0; j < k; ++j) s -= M[i * (i + 1) / 2 + j] * M[k * (k + 1) / 2 + j];
+            M[i * (i + 1) / 2 + k] = s / lkk;
+        }
+    }
+    // L z = y, then L^T x = z
+#pragma unroll
+    for (int i = 0; i < 5; ++i) {
+#pragma unroll
+        for (int j = 0; j < i; ++j) y[i] -= M[i * (i + 1) / 2 + j] * y[j];
+        y[i] /= M[i * (i + 1) / 2 + i];
+    }
+#pragma unroll
+    for (int i = 4; i >= 0; --i) {
+#pragma unroll
+        for (int j = i + 1; j < 5; ++j) y[i] -= M[j * (j + 1) / 2 + i] * y[j];
+        y[i] /= M[i * (i + 1) / 2 + i];
+    }
+    double k1 = 0.0, k2 = 0.0, d1[3] = {t1[0], t1[1], t1[2]}, d2[3] = {0.0, 0.0, 0.0};
+    if (ok) curv_monge(y, r, n, t1, t2, k1, k2, d1, d2);
+    curv_store<T>(row, ok, k1, k2, d1, d2, out_k1, out_k2, out_d1, out_d2);
 }
 
 // The kept points and their normals in index order (the reference's single-thread loop appends in that order,

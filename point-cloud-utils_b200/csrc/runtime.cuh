@@ -106,7 +106,8 @@ enum Scratch {
     kIo,      // device copies of a host entry point's inputs and outputs: outlive the device call they are passed to
     kAux,     // intermediate results (normals, Poisson disk) that outlive a nested call's re-carving of the arena
     kMesh,    // the face CDF and dense samples of mesh Poisson-disk sampling, which outlive the point-cloud Poisson-disk
-              // call it makes (that one re-carves the arena and aux)
+              // call it makes (that one re-carves the arena and aux), and the fp64 vertex normals of mesh curvatures,
+              // which outlive the ball pass's binning
     kVorList, // the Voronoi cells' fallback passes (rows, queries, longer neighbour lists), sized once the first pass is done
     kLloyd,   // the points, L-BFGS history and sync record of a Lloyd relaxation, which outlive every cell evaluation
     kRvd,     // the faces and the per-seed buffers of restricted Voronoi cells, which outlive every cell evaluation of a call
@@ -380,6 +381,12 @@ int knn_device(pcu_b200_workspace* ws, const T* query, long long n, const T* dat
 template <typename T>
 int poisson_disk_device(pcu_b200_workspace* ws, const T* points, long long n, double radius, unsigned seed, int* out_idx,
                         long long* out_count, int* out_rounds, cudaStream_t stream);
+
+// The ball mode of mesh_principal_curvatures (curv_ball_kernel of normals.cuh): the nv vertices binned in the arena,
+// `normal` their fp64 unit normals (device memory that the arena does not hold), r > 0 the ball's radius.
+template <typename T>
+int curvature_ball_device(pcu_b200_workspace* ws, const T* v, long long nv, const double* normal, double r, T* out_k1, T* out_k2,
+                          T* out_d1, T* out_d2, cudaStream_t stream);
 
 // ---- what mesh_query.cu offers the other families: the fp64 closest-point tree (watertight remeshing's projection), the
 // ball tree (restricted Voronoi cells) and sampled positions (the initial sample of sample_mesh_lloyd)
