@@ -470,6 +470,17 @@ int pcu_b200_point_cloud_fast_winding_number_f32(pcu_b200_workspace* ws, const f
                                                  const float* q, int64_t nq, double accuracy_scale, float* out_w, void* stream);
 int pcu_b200_point_cloud_fast_winding_number_f64(pcu_b200_workspace* ws, const double* p, const double* n, const double* a, int64_t np,
                                                  const double* q, int64_t nq, double accuracy_scale, double* out_w, void* stream);
+/* Replaces estimate_point_cloud_areas (src/point_areas.cpp, libigl's igl::copyleft::cgal::point_areas): out_areas[r]
+ * (n rows) is the area of point idx[r, 0] from the neighbour row idx[r, 0:k], defined in DESIGN.md §3 -- the neighbours
+ * whose normals have a positive dot product with the centre's, projected onto their PCA plane, and the centre's mixed
+ * Voronoi area over its star in the 2-D Delaunay triangulation; fp64 throughout, rounded once to the suffix's type.
+ * points and normals (n, 3), idx (n, k) of kind idx_kind (pcu_b200_index_kind), 0 <= k <= 256, 0 <= n < 2^31 - 1.
+ * Entries of idx outside [0, n) are left out of their row and counted in *out_bad (device uint64); when it is not zero
+ * the outputs are unspecified.  Every pointer is a DEVICE pointer and the call is stream-ordered. */
+int pcu_b200_estimate_point_cloud_areas_f32(pcu_b200_workspace* ws, const float* points, int64_t n, const float* normals, const void* idx,
+                                            int k, int idx_kind, float* out_areas, uint64_t* out_bad, void* stream);
+int pcu_b200_estimate_point_cloud_areas_f64(pcu_b200_workspace* ws, const double* points, int64_t n, const double* normals,
+                                            const void* idx, int k, int idx_kind, double* out_areas, uint64_t* out_bad, void* stream);
 int pcu_b200_signed_distance_to_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
                                          int64_t nf, int f_kind, float lower_bound, float upper_bound, float* out_s, int32_t* out_fidx,
                                          float* out_bc, uint64_t* out_bad, void* stream);

@@ -196,11 +196,12 @@ def _upload(form, arrays, device):
     return _to_device(_numpy(arrays), device)
 
 
-def _raise_bad(bad):
-    """Raises for a count (a device tensor or a host scalar) of faces with a corner out of range."""
+def _raise_bad(bad, message="Invalid face indices: %d faces have a corner outside [0, #v)"):
+    """Raises for a count (a device tensor or a host scalar) of faces with a corner out of range, or of whatever else
+    `message` names."""
     nbad = int(bad.item())
     if nbad:
-        raise ValueError("Invalid face indices: %d faces have a corner outside [0, #v)" % nbad)
+        raise ValueError(message % nbad)
 
 
 def _run(form, arrays, device, body, index=None, squeeze=False):

@@ -1,11 +1,13 @@
-"""closest_points_on_mesh, triangle_soup_fast_winding_number, point_cloud_fast_winding_number and signed_distance_to_mesh
--- the reference's names, arguments and outputs (the reference's src/closest_point_on_mesh.cpp,
-src/fast_winding_numbers.cpp and src/signed_distance.cpp), computed by csrc/meshquery.cuh and csrc/winding.cuh.
+"""closest_points_on_mesh, triangle_soup_fast_winding_number, point_cloud_fast_winding_number,
+estimate_point_cloud_areas and signed_distance_to_mesh -- the reference's names, arguments and outputs (the reference's
+src/closest_point_on_mesh.cpp, src/fast_winding_numbers.cpp, src/point_areas.cpp and src/signed_distance.cpp), computed
+by csrc/meshquery.cuh, csrc/winding.cuh and csrc/point_areas.cuh.
 
 Input forms and validation follow _call.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
 from . import _pcu_internal
-from ._call import _INDEX_KINDS, _check_float, _check_index, _check_match, _dtype_name, _form, _raise_bad, _run, _same_device, _torch, _validate_mesh
+from ._call import (_INDEX_KINDS, _check_float, _check_index, _check_match, _dtype_name, _form, _matrix_shape, _raise_bad, _run,
+                    _same_device, _torch, _validate_mesh)
 
 
 def _validate_points(p, v, f):
@@ -161,6 +163,7 @@ def point_cloud_fast_winding_number(p, n, a, q, *, device=None):
     fp64 in a fixed order, so the result depends only on (p, n, a, q_i) (DESIGN.md §3).
     Divergences: a of any shape with exactly #p elements is accepted and any other size raises ValueError (the reference
     reads a short vector out of bounds); #p = 0 gives w = 0 for every query.
+    For a scanned cloud, `estimate_point_cloud_areas(p, k_nearest_neighbors(p, p, k)[1], n)` gives the areas a.
     """
     form = _form([p, n, a, q], ["p", "n", "a", "q"])
     _check_float(p, "p")
@@ -184,6 +187,68 @@ def point_cloud_fast_winding_number(p, n, a, q, *, device=None):
         return w
 
     return _run(form, [p, n, a, q], device, body)
+
+
+_AREAS_MAX_K = 256   # kAreaMaxK of csrc/point_areas.cuh
+
+
+def estimate_point_cloud_areas(p, i, n, *, device=None):
+    """
+    Estimate the area of the surface around each point of an oriented point cloud
+
+    Args:
+        p : (#p, 3)-shaped array of 3D points (float32 / float64)
+        i : (#p, k)-shaped array of indices where i[a, b] is the index of the b^th nearest neighbor to point p[a]
+            (int32 / int64 / uint32 / uint64), with the point itself in column 0 -- what k_nearest_neighbors(p, p, k)[1]
+            returns; a (#p,)-shaped array counts as k = 1.  k <= 256.
+        n : (#p, 3)-shaped array of point normals (p's dtype)
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        a : a (#p,)-shaped array of areas (p's dtype): a[r] is the area of point i[r, 0] from the neighbours in row r, for
+            the areas `point_cloud_fast_winding_number` takes
+
+    Mirrors the reference's src/point_areas.cpp (libigl's igl::copyleft::cgal::point_areas, which is not in the
+    reference's tree).  The result is a pure function of (p, n, i[r]), defined in DESIGN.md §3: the neighbours whose
+    normals have a positive dot product with the centre's are projected onto their PCA plane; the centre's star in the
+    2-D Delaunay triangulation of the projected points is walked from its nearest neighbour, with fixed rules for ties;
+    the area is Meyer et al.'s mixed Voronoi area of the centre over that star, or 0 when fewer than three neighbours
+    are kept or the star is empty.  Everything is computed in fp64 and rounded once to p's dtype.
+    Divergence: an entry of i outside [0, #p), such as the -1 that k_nearest_neighbors writes when k > #p, raises
+    ValueError (the reference reads out of bounds).
+    """
+    form = _form([p, i, n], ["p", "i", "n"])
+    _check_float(p, "p")
+    _check_index(i, "i", _INDEX_KINDS)
+    _check_match(n, "n", p, "p")
+    _validate_point_cloud_normals(p, n)
+    m = int(p.shape[0])
+    rows, k = (int(i.shape[0]), 1 if len(i.shape) == 1 else int(i.shape[1])) if len(i.shape) in (1, 2) else (-1, 0)
+    if rows != m:
+        shape = _matrix_shape(i)
+        raise ValueError("Invalid shape for i (knn indices), must be (#p, k) where #p is the number of input points (%d). "
+                         "Got (%d, %d)" % (m, shape[0], shape[1]))
+    if k > _AREAS_MAX_K:
+        raise ValueError("Invalid shape for i (knn indices): at most %d neighbours per point are supported, got k = %d"
+                         % (_AREAS_MAX_K, k))
+    torch = _torch()
+    if m == 0:
+        if form == "numpy":
+            import numpy as np
+            return np.zeros(0, dtype=p.dtype)
+        if form == "cuda":
+            _same_device(p, device)
+        return torch.zeros(0, dtype=p.dtype, device=p.device)
+
+    def body(pt, it, nt, dev, stream):
+        a = torch.empty(m, dtype=pt.dtype, device=pt.device)
+        bad = torch.empty(1, dtype=torch.int64, device=pt.device)
+        _pcu_internal._estimate_point_cloud_areas_device(pt.dtype == torch.float64, pt.data_ptr(), m, nt.data_ptr(), it.data_ptr(), k,
+                                                         _INDEX_KINDS[_dtype_name(i)], a.data_ptr(), bad.data_ptr(), dev, stream)
+        _raise_bad(bad, "Invalid knn indices: %d entries of i are outside [0, #p)")
+        return a
+
+    return _run(form, [p, i, n], device, body, squeeze=True)
 
 
 def signed_distance_to_mesh(p, v, f, lower_bound=-float("inf"), upper_bound=float("inf"), *, device=None):

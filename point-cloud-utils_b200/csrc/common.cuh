@@ -20,6 +20,23 @@ constexpr int kMaxLevels = 12;      // 2^11 = kMaxGridDim, plus one
 // Index arrays come in four integer types, chosen at run time (pcu_b200_index_kind).
 enum MeshIndexKind { kIdxI32 = 0, kIdxI64 = 1, kIdxU32 = 2, kIdxU64 = 3 };
 
+// Entry i of an index array of kind `kind`, checked against [0, n): negative entries of a signed array wrap by n when
+// `wrap` is set (numpy's indexing), and -1 stands for anything out of range.
+__device__ __forceinline__ long long load_index(const void* a, long long i, int kind, long long n, bool wrap) {
+    long long x;
+    switch (kind) {
+        case kIdxI32: x = ((const int*)a)[i]; break;
+        case kIdxI64: x = ((const long long*)a)[i]; break;
+        case kIdxU32: x = (long long)((const unsigned*)a)[i]; break;
+        default: {
+            const unsigned long long u = ((const unsigned long long*)a)[i];
+            x = u >= (unsigned long long)n ? -1 - n : (long long)u;   // never wraps
+        }
+    }
+    if (x < 0 && wrap) x += n;
+    return x >= 0 && x < n ? x : -1;
+}
+
 // Programmatic dependent launch: every kernel of a call's chain is launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, so its CTAs may be scheduled while the previous
 // kernel drains; this wait (first statement of every kernel) blocks until that kernel has completed

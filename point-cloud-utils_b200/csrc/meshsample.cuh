@@ -19,23 +19,6 @@ namespace pcu {
 constexpr int kMeshScanThreads = 256;
 constexpr int kMeshScanTile = 4096;     // faces per CTA of the CDF scan (16 per thread)
 
-// Entry i of an index array of kind `kind`, checked against [0, n): negative entries of a signed array wrap by n when
-// `wrap` is set (numpy's indexing), and -1 stands for anything out of range.
-__device__ __forceinline__ long long load_index(const void* a, long long i, int kind, long long n, bool wrap) {
-    long long x;
-    switch (kind) {
-        case kIdxI32: x = ((const int*)a)[i]; break;
-        case kIdxI64: x = ((const long long*)a)[i]; break;
-        case kIdxU32: x = (long long)((const unsigned*)a)[i]; break;
-        default: {
-            const unsigned long long u = ((const unsigned long long*)a)[i];
-            x = u >= (unsigned long long)n ? -1 - n : (long long)u;   // never wraps
-        }
-    }
-    if (x < 0 && wrap) x += n;
-    return x >= 0 && x < n ? x : -1;
-}
-
 // {W, S, faces with a corner out of range}: what the host reads to size and validate a call (pcu_b200_mesh_area).
 struct MeshArea {
     unsigned long long total;

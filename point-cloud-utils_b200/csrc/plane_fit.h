@@ -115,12 +115,18 @@ struct PlaneFit {
         return pass == 1 || (turn > 0x1p-26 && pass < kMaxPasses);
     }
 
+    // The column of the basis v that is the normal when the fit is defined: the first smallest diagonal entry.  The other
+    // two columns span the fitted plane.
+    PCU_HD int normal_axis() const {
+        const double e0 = a[0][0], e1 = a[1][1], e2 = a[2][2];
+        return (e0 <= e1 && e0 <= e2) ? 0 : (e1 <= e2 ? 1 : 2);
+    }
+
     // The unit normal of m offsets (see the rules above).
     PCU_HD void normal(long long m, double (&n)[3]) const {
         if (m < 3) { n[0] = n[1] = n[2] = 0.0; return; }
         if (zero) { n[0] = 0.0; n[1] = 0.0; n[2] = 1.0; return; }
-        const double e0 = a[0][0], e1 = a[1][1], e2 = a[2][2];
-        const int c = (e0 <= e1 && e0 <= e2) ? 0 : (e1 <= e2 ? 1 : 2);
+        const int c = normal_axis();
         const double nx = v[0][c], ny = v[1][c], nz = v[2][c];
         const double len = sqrt(nx * nx + ny * ny + nz * nz);
         n[0] = nx / len; n[1] = ny / len; n[2] = nz / len;

@@ -1,8 +1,10 @@
 // point_ops.cu -- point-cloud operations that share nothing with the nearest-neighbour sweep: duplicate removal, Morton
-// codes, voxel-grid downsampling, dense pairwise distances and Sinkhorn, and their device and host C entry points.
+// codes, voxel-grid downsampling, dense pairwise distances and Sinkhorn, point areas from given neighbour rows, and
+// their device and host C entry points.
 #include "runtime.cuh"
 #include "dedup.cuh"
 #include "morton.cuh"
+#include "point_areas.cuh"
 #include "sinkhorn.cuh"
 #include "voxel.cuh"
 
@@ -297,6 +299,25 @@ int sinkhorn_device(pcu_b200_workspace* ws, const T* a, const T* b, const T* M, 
     return PCU_B200_OK;
 }
 
+// ---- point areas (estimate_point_cloud_areas, src/point_areas.cpp) -------------------------------------------
+template <typename T>
+int point_areas_device(pcu_b200_workspace* ws, const T* points, long long n, const T* normals, const void* idx, int k, int kind,
+                       T* out_areas, unsigned long long* out_bad, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (n < 0 || (n > 0 && (!points || !normals || (k > 0 && !idx) || !out_areas)) || !out_bad)
+        return fail(PCU_B200_INVALID_ARGUMENT, "points, normals, idx and the outputs must be non-null");
+    if (n >= 0x7fffffffLL) return fail(PCU_B200_INVALID_ARGUMENT, "point cloud too large (%lld rows)", n);
+    if (k < 0 || k > kAreaMaxK)
+        return fail(PCU_B200_INVALID_ARGUMENT, "estimate_point_cloud_areas: i may have at most %d columns, got %d", kAreaMaxK, k);
+    if (kind < kIdxI32 || kind > kIdxU64) return fail(PCU_B200_INVALID_ARGUMENT, "unknown index kind %d", kind);
+    PCU_ON_DEVICE(ws);
+    PCU_CUDA(cudaMemsetAsync(out_bad, 0, sizeof(unsigned long long), stream));
+    if (n == 0) return PCU_B200_OK;
+    const int cap = std::max(32, (k + 31) / 32 * 32);
+    return launch_pdl(point_areas_kernel<T>, dim3((unsigned)((n + kAreaWarps - 1) / kAreaWarps)), dim3(kAreaWarps * 32),
+                      point_area_smem<T>(cap), stream, points, normals, n, idx, k, kind, cap, out_areas, out_bad);
+}
+
 // voxel-grid down-sampling on HOST arrays: stage, run, fetch the row count, then exactly the rows that exist
 template <typename T>
 int voxel_downsample_host(pcu_b200_workspace* ws, const T* points, long long n, const void* attrib, int attrib_cols, int attrib_is_f64,
@@ -435,6 +456,16 @@ int pcu_b200_sinkhorn_f32(pcu_b200_workspace* ws, const float* a, const float* b
 int pcu_b200_sinkhorn_f64(pcu_b200_workspace* ws, const double* a, const double* b, const double* M, int64_t nb, int64_t n, int64_t m,
                           double eps, int max_iters, double stop_thresh, double* out_P, double* out_cost, int32_t* out_iters, void* stream) {
     return sinkhorn_device<double>(ws, a, b, M, nb, n, m, eps, max_iters, stop_thresh, out_P, out_cost, out_iters, (cudaStream_t)stream);
+}
+
+int pcu_b200_estimate_point_cloud_areas_f32(pcu_b200_workspace* ws, const float* points, int64_t n, const float* normals, const void* idx,
+                                            int k, int idx_kind, float* out_areas, uint64_t* out_bad, void* stream) {
+    return point_areas_device<float>(ws, points, n, normals, idx, k, idx_kind, out_areas, (unsigned long long*)out_bad, (cudaStream_t)stream);
+}
+int pcu_b200_estimate_point_cloud_areas_f64(pcu_b200_workspace* ws, const double* points, int64_t n, const double* normals,
+                                            const void* idx, int k, int idx_kind, double* out_areas, uint64_t* out_bad, void* stream) {
+    return point_areas_device<double>(ws, points, n, normals, idx, k, idx_kind, out_areas, (unsigned long long*)out_bad,
+                                      (cudaStream_t)stream);
 }
 
 int pcu_b200_morton_encode_i32(pcu_b200_workspace* ws, const int32_t* pts, int64_t n, uint64_t* out_codes, void* stream) {
