@@ -481,6 +481,20 @@ int pcu_b200_estimate_point_cloud_areas_f32(pcu_b200_workspace* ws, const float*
                                             int k, int idx_kind, float* out_areas, uint64_t* out_bad, void* stream);
 int pcu_b200_estimate_point_cloud_areas_f64(pcu_b200_workspace* ws, const double* points, int64_t n, const double* normals,
                                             const void* idx, int k, int idx_kind, double* out_areas, uint64_t* out_bad, void* stream);
+/* pointcloud_apss_curvature and project_points_onto_apss: the algebraic point set surface (Guennebaud & Gross 2007,
+ * the spherical fit with beta = 1) of the oriented cloud (p, n) with ball radius r, a true distance, finite and > 0
+ * (DESIGN.md §3).  Each query is iterated onto the surface (at most 20 steps, until a step of at most 1e-10 r):
+ * out_x (nq, 3) its projection, out_n (nq, 3) the unit normal and out_kh (nq) the signed mean curvature of the last
+ * fitted sphere, +1/R on a sphere with outward normals.  Normals are normalised in fp64; a zero normal leaves its
+ * point out of every fit.  A query whose ball holds fewer than 4 points with a normal, or whose fit has no step, is
+ * undetermined: x = NaN, n = 0, kh = NaN; np = 0 makes every query undetermined.  fp64 throughout, rounded once.
+ * q == NULL: the queries are the points themselves (nq = np), run in cell order, each result in its point's row.
+ * out_x and out_n may be NULL.  0 <= np < 2^31 - 1.  Every pointer is a DEVICE pointer and the call is stream-ordered:
+ * it does not synchronise. */
+int pcu_b200_apss_project_f32(pcu_b200_workspace* ws, const float* p, const float* n, int64_t np, const float* q, int64_t nq, double r,
+                              float* out_x, float* out_n, float* out_kh, void* stream);
+int pcu_b200_apss_project_f64(pcu_b200_workspace* ws, const double* p, const double* n, int64_t np, const double* q, int64_t nq, double r,
+                              double* out_x, double* out_n, double* out_kh, void* stream);
 int pcu_b200_signed_distance_to_mesh_f32(pcu_b200_workspace* ws, const float* p, int64_t np, const float* v, int64_t nv, const void* f,
                                          int64_t nf, int f_kind, float lower_bound, float upper_bound, float* out_s, int32_t* out_fidx,
                                          float* out_bc, uint64_t* out_bad, void* stream);

@@ -42,7 +42,7 @@ __all__ = ["k_nearest_neighbors", "one_sided_hausdorff_distance", "hausdorff_dis
            "earth_movers_distance", "downsample_point_cloud_on_voxel_grid", "downsample_point_cloud_poisson_disk",
            "sample_mesh_random", "sample_mesh_poisson_disk", "interpolate_barycentric_coords", "closest_points_on_mesh",
            "triangle_soup_fast_winding_number", "point_cloud_fast_winding_number", "estimate_point_cloud_areas",
-           "signed_distance_to_mesh",
+           "pointcloud_apss_curvature", "project_points_onto_apss", "signed_distance_to_mesh",
            "ray_mesh_intersection", "RayMeshIntersector",
            "ray_surfel_intersection", "RaySurfelIntersector", "pointcloud_surfel_geometry", "pointcloud_sphere_geometry",
            "marching_cubes_sparse_voxel_grid", "sparse_voxel_grid_boundary",
@@ -624,7 +624,8 @@ from ._poisson import downsample_point_cloud_poisson_disk  # noqa: E402  (Poisso
 from ._lloyd import voronoi_centroids_unit_cube, lloyd_3d, lloyd_2d, sample_mesh_lloyd  # noqa: E402  (Voronoi, Lloyd)
 from ._mesh_sampling import sample_mesh_random, sample_mesh_poisson_disk, interpolate_barycentric_coords  # noqa: E402
 from ._mesh_query import (closest_points_on_mesh, triangle_soup_fast_winding_number,  # noqa: E402
-                          point_cloud_fast_winding_number, estimate_point_cloud_areas, signed_distance_to_mesh)
+                          point_cloud_fast_winding_number, estimate_point_cloud_areas, pointcloud_apss_curvature,
+                          project_points_onto_apss, signed_distance_to_mesh)
 from ._ray_mesh import ray_mesh_intersection, RayMeshIntersector  # noqa: E402
 from ._ray_surfel import (ray_surfel_intersection, RaySurfelIntersector, pointcloud_surfel_geometry,  # noqa: E402
                           pointcloud_sphere_geometry)

@@ -1,7 +1,8 @@
 """closest_points_on_mesh, triangle_soup_fast_winding_number, point_cloud_fast_winding_number,
-estimate_point_cloud_areas and signed_distance_to_mesh -- the reference's names, arguments and outputs (the reference's
-src/closest_point_on_mesh.cpp, src/fast_winding_numbers.cpp, src/point_areas.cpp and src/signed_distance.cpp), computed
-by csrc/meshquery.cuh, csrc/winding.cuh and csrc/point_areas.cuh.
+estimate_point_cloud_areas, signed_distance_to_mesh, pointcloud_apss_curvature and project_points_onto_apss -- the
+reference's names, arguments and outputs (the reference's src/closest_point_on_mesh.cpp, src/fast_winding_numbers.cpp,
+src/point_areas.cpp, src/signed_distance.cpp and src/curvature.cpp), computed by csrc/meshquery.cuh, csrc/winding.cuh,
+csrc/point_areas.cuh and csrc/apss.cuh.
 
 Input forms and validation follow _call.py: numpy arrays in -> numpy out; CUDA torch tensors in -> CUDA tensors
 out; CPU tensors -> CPU tensors.  Arguments are validated, with the reference's messages, before any device call."""
@@ -300,3 +301,110 @@ def signed_distance_to_mesh(p, v, f, lower_bound=-float("inf"), upper_bound=floa
         return s, fidx, bc
 
     return _run(form, [p, v, f], device, body)
+
+
+def _apss_radius(r):
+    """The ball radius of the APSS functions: a finite number > 0."""
+    import math
+    try:
+        r = float(r)
+    except (TypeError, ValueError):
+        raise ValueError("Invalid radius r (%r): must be a finite number greater than 0." % (r,)) from None
+    if not (math.isfinite(r) and r > 0.0):
+        raise ValueError("Invalid radius r (%r): must be a finite number greater than 0." % (r,))
+    return r
+
+
+def _apss_device(pt, nt, qt, nq, r, out_x, out_n, kh, dev, stream):
+    """One native call: qt None runs the queries at the points themselves; out_x / out_n None are not written."""
+    torch = _torch()
+    _pcu_internal._apss_device(pt.dtype == torch.float64, pt.data_ptr(), nt.data_ptr(), int(pt.shape[0]),
+                               0 if qt is None else qt.data_ptr(), nq, r, 0 if out_x is None else out_x.data_ptr(),
+                               0 if out_n is None else out_n.data_ptr(), kh.data_ptr(), dev, stream)
+
+
+def pointcloud_apss_curvature(p, n, r, *, device=None):
+    """
+    Estimate the mean curvature of the surface an oriented point cloud samples, with an algebraic point set surface
+
+    Args:
+        p : (#p, 3)-shaped array of points (float32 / float64)
+        n : (#p, 3)-shaped array of point normals (p's dtype), normalised in fp64 before use; a zero normal leaves its
+            point out of every fit
+        r : the radius of the ball each fit uses, a true distance (not squared), finite and > 0
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        kh : a (#p,)-shaped array (p's dtype): the mean curvature of the surface at the projection of each point, +1/R
+             on a sphere of radius R with outward normals; NaN where it is undetermined
+
+    The reference declares pointcloud_apss_curvature(v, f) in src/curvature.cpp with its body commented out; APSS needs
+    oriented points and no faces, so this takes (p, n, r).  kh[i] is exactly project_points_onto_apss(p, n, p, r)[2][i]:
+    see that function for the surface and DESIGN.md §3 for the rules.
+    """
+    form = _form([p, n], ["p", "n"])
+    _check_float(p, "p")
+    _check_match(n, "n", p, "p")
+    _validate_point_cloud_normals(p, n)
+    r = _apss_radius(r)
+    m = int(p.shape[0])
+    torch = _torch()
+    if m == 0:
+        if form == "numpy":
+            import numpy as np
+            return np.zeros(0, dtype=p.dtype)
+        if form == "cuda":
+            _same_device(p, device)
+        return torch.zeros(0, dtype=p.dtype, device=p.device)
+
+    def body(pt, nt, dev, stream):
+        kh = torch.empty(m, dtype=pt.dtype, device=pt.device)
+        _apss_device(pt, nt, None, m, r, None, None, kh, dev, stream)
+        return kh
+
+    return _run(form, [p, n], device, body)
+
+
+def project_points_onto_apss(p, n, q, r, *, device=None):
+    """
+    Project query points onto the algebraic point set surface of an oriented point cloud
+
+    Args:
+        p : (#p, 3)-shaped array of points (float32 / float64)
+        n : (#p, 3)-shaped array of point normals (p's dtype), normalised in fp64 before use; a zero normal leaves its
+            point out of every fit
+        q : (#q, 3)-shaped array of query points (p's dtype, #q > 0)
+        r : the radius of the ball each fit uses, a true distance (not squared), finite and > 0
+        device: see `k_nearest_neighbors` (keyword only).
+
+    Returns:
+        x : a (#q, 3)-shaped array of the projected points (p's dtype)
+        nx : a (#q, 3)-shaped array of unit surface normals at x (p's dtype), oriented like n
+        kh : a (#q,)-shaped array of mean curvatures at x (p's dtype), +1/R on a sphere of radius R with outward normals
+
+    The surface is Guennebaud and Gross's APSS (SIGGRAPH 2007) with the spherical parameter 1: around an iterate x,
+    every point within distance r whose normal is not zero is weighted by (1 - |p_j - x|^2 / r^2)^4, an algebraic
+    sphere is fitted to those points and normals in closed form, and x moves to the closest point of that sphere.
+    The iteration starts at q and stops after a step of at most 1e-10 r, or after 20 steps.  nx and kh come from the
+    last fitted sphere.  A query whose ball holds fewer than 4 points with a normal, or whose sphere gives no step, is
+    undetermined: x = NaN, nx = 0, kh = NaN; so is every query when #p = 0.  Everything is computed in fp64 and rounded
+    once to p's dtype (DESIGN.md §3).
+    """
+    form = _form([p, n, q], ["p", "n", "q"])
+    _check_float(p, "p")
+    _check_match(n, "n", p, "p")
+    _check_match(q, "q", p, "p")
+    _validate_point_cloud_normals(p, n)
+    _validate_nonempty_points(q)
+    r = _apss_radius(r)
+    torch = _torch()
+
+    def body(pt, nt, qt, dev, stream):
+        nq = int(qt.shape[0])
+        x = torch.empty((nq, 3), dtype=pt.dtype, device=pt.device)
+        nx = torch.empty((nq, 3), dtype=pt.dtype, device=pt.device)
+        kh = torch.empty(nq, dtype=pt.dtype, device=pt.device)
+        _apss_device(pt, nt, qt, nq, r, x, nx, kh, dev, stream)
+        return x, nx, kh
+
+    return _run(form, [p, n, q], device, body)

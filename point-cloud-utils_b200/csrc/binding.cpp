@@ -928,6 +928,7 @@ PYBIND11_MODULE(_pcu_internal, mod) {
             forward_to(pcu_b200_point_cloud_fast_winding_number_f32, pcu_b200_point_cloud_fast_winding_number_f64).pair());
     mod.def("_estimate_point_cloud_areas_device",
             forward_to(pcu_b200_estimate_point_cloud_areas_f32, pcu_b200_estimate_point_cloud_areas_f64).pair());
+    mod.def("_apss_device", forward_to(pcu_b200_apss_project_f32, pcu_b200_apss_project_f64).pair());
     mod.def("_signed_distance_to_mesh_device",
             forward_to(pcu_b200_signed_distance_to_mesh_f32, pcu_b200_signed_distance_to_mesh_f64).pair());
     mod.def("_sample_mesh_poisson_disk_device",

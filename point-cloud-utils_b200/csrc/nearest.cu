@@ -1,6 +1,6 @@
 // nearest.cu -- the nearest-neighbour family: the grid build and its plan, k nearest neighbours, the fused k = 1
 // statistics (Chamfer, Hausdorff) and their witness replay, prepared clouds, batched Chamfer, normals, Poisson-disk
-// downsampling, and their device and host C entry points.
+// downsampling, algebraic point set surfaces, and their device and host C entry points.
 //
 // It owns no algorithmic decisions that depend on the data: grid shapes, far-query lists and tie lists are produced
 // and consumed on the device, so a device-pointer call enqueues a fixed sequence of launches and returns without
@@ -13,6 +13,7 @@
 #include "pyramid.cuh"
 #include "kdreplay.cuh"
 #include "normals.cuh"
+#include "apss.cuh"
 #include "poisson.cuh"
 
 using namespace pcu;
@@ -673,6 +674,37 @@ int normals_ball_device(pcu_b200_workspace* ws, const T* points, long long n, co
     return PCU_B200_OK;
 }
 
+// ---- algebraic point set surfaces (pointcloud_apss_curvature, project_points_onto_apss) -----------------------------
+// The points are binned as for the ball curvatures (cells no finer than r / 2, then row order within every cell), their
+// unit fp64 normals are written in cell order into aux scratch, then one thread per query iterates its projection
+// (apss.cuh).  Stream-ordered: no synchronisation.
+template <typename T>
+int apss_device(pcu_b200_workspace* ws, const T* p, const T* n, long long np, const T* q, long long nq, double r, T* out_x, T* out_n,
+                T* out_kh, cudaStream_t stream) {
+    if (!ws) return fail(PCU_B200_INVALID_ARGUMENT, "null workspace");
+    if (!(r > 0.0) || !std::isfinite(r)) return fail(PCU_B200_INVALID_ARGUMENT, "apss: r must be finite and > 0, got %g", r);
+    if (np < 0 || nq < 0) return fail(PCU_B200_INVALID_ARGUMENT, "apss: negative size (np = %lld, nq = %lld)", np, nq);
+    if (!q && nq != np) return fail(PCU_B200_INVALID_ARGUMENT, "apss: without q the queries are the %lld points, got nq = %lld", np, nq);
+    if (np > 0 && (!p || !n)) return fail(PCU_B200_INVALID_ARGUMENT, "null point or normal pointer");
+    if (nq > 0 && !out_kh) return fail(PCU_B200_INVALID_ARGUMENT, "null output pointer");
+    PCU_ON_DEVICE(ws);
+    if (nq == 0) return PCU_B200_OK;
+    if (np == 0) {
+        PCU_LAUNCH((apss_undetermined_kernel<T>), blocks_for(nq), kThreads, stream, nq, out_x, out_n, out_kh);
+        return PCU_B200_OK;
+    }
+    PCU_TRY(check_cloud_args<T>(p, np, p, 1));
+    Plan<T> plan;
+    PCU_TRY(single_cloud_plan<T>(ws, p, np, 0.5 * r, plan, stream));
+    double* nrm;
+    PCU_TRY(carve_scratch(ws, kAux, stream, [&](Carver& cv) { nrm = cv.take<double>(3 * (size_t)np); }));
+    PCU_TRY(enqueue_binning(ws, plan, stream, nullptr, true));
+    PCU_LAUNCH((cell_order_kernel<T>), (unsigned)std::min<long long>(((long long)plan.cv.v[0].cell_cap + kThreads - 1) / kThreads, (long long)ws->sm_count * 64), kThreads, stream, plan.cv.v[0]);
+    PCU_LAUNCH((apss_normals_kernel<T>), blocks_for(np), kThreads, stream, plan.cv.v[0], n, nrm);
+    PCU_LAUNCH((apss_kernel<T>), blocks_for(nq), kThreads, stream, plan.cv.v[0], (const double*)nrm, q, nq, r, out_x, out_n, out_kh);
+    return PCU_B200_OK;
+}
+
 // ---- Poisson-disk downsampling (downsample_point_cloud_poisson_disk) --------------------------------------------
 // The cloud is binned once (cells no finer than half the radius, as for the ball normals), then ONE cooperative launch
 // runs every selection round of poisson.cuh with grid barriers between them -- the number of rounds depends on the
@@ -1298,6 +1330,15 @@ int pcu_b200_poisson_disk_f32(pcu_b200_workspace* ws, const float* points, int64
 int pcu_b200_poisson_disk_f64(pcu_b200_workspace* ws, const double* points, int64_t n, double radius, uint32_t seed,
                               int32_t* out_idx, int64_t* out_count, int32_t* out_rounds, void* stream) {
     return poisson_disk_device<double>(ws, points, n, radius, seed, out_idx, (long long*)out_count, out_rounds, (cudaStream_t)stream);
+}
+
+int pcu_b200_apss_project_f32(pcu_b200_workspace* ws, const float* p, const float* n, int64_t np, const float* q, int64_t nq, double r,
+                              float* out_x, float* out_n, float* out_kh, void* stream) {
+    return apss_device<float>(ws, p, n, np, q, nq, r, out_x, out_n, out_kh, (cudaStream_t)stream);
+}
+int pcu_b200_apss_project_f64(pcu_b200_workspace* ws, const double* p, const double* n, int64_t np, const double* q, int64_t nq, double r,
+                              double* out_x, double* out_n, double* out_kh, void* stream) {
+    return apss_device<double>(ws, p, n, np, q, nq, r, out_x, out_n, out_kh, (cudaStream_t)stream);
 }
 
 int pcu_b200_debug_kd_times(pcu_b200_workspace* ws, uint64_t* out40) {
